@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py - TensorProto encode+decode throughput on B200 (BASELINE.json metric), one JSON line.
+"""bench.py - TensorProto encode+decode throughput on H100 (BASELINE.json metric), one JSON line.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2|c3|c4|c5] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2|c3|c4|c5] [--impl reference] [--dump-outputs DIR]
 
 A *step* is one pass of the hot path over one batch of synthetic requests: ONE ``b200tfs_encode_requests`` call
 over the batch's PredictRequests (device tensors -> wire arena) and ONE decode call over the batch's
@@ -16,7 +16,7 @@ PredictResponses (wire -> device tensors).  Workloads (BASELINE.json ``configs``
 timed, max over ranks; ``e2e`` = the same through the host-buffer C-ABI entry points on pinned host memory with the
 H2D / D2H copies inside the timed region; ``roofline`` = algorithmic bytes (SURVEY 8d: 2P+H per direction) of the
 two launches of a step / their measured durations / the measured HBM copy peak; ``cpu_baseline`` = the unmodified
-reference (baseline/ref_loader.py) on one host core over a bounded sample.  Every batch is larger than the 126 MB
+reference (baseline/ref_loader.py) on one host core over a bounded sample.  Every batch is larger than the 50 MB
 L2 (or rotates through a ring that is), and every run ends with a bit-exact comparison of the device's wire bytes
 and decoded tensors against the oracle - AFTER the timed region, on the buffers the timed steps wrote.
 
@@ -40,7 +40,7 @@ import numpy as np
 REPO = os.path.dirname(os.path.abspath(__file__))
 sys.path[:0] = [os.path.join(REPO, "min-tfs-client_b200"), REPO]
 
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024     # H100 SXM
 METRIC = "TensorProto encode+decode GB/s"
 
 
@@ -624,6 +624,53 @@ class DeviceBatch:
                 "against": "oracle/wire_oracle.c (pinned to the reference's goldens)",
                 "when": "after the timed region, on the buffers the timed steps wrote", "snan_probe": "planted in every float32 tensor"}
 
+    def dump(self, out_dir, s, max_elems=4 << 20, head=64, chunk=256):
+        """Write slot s's outputs for comparing builds: request_wire.npy (wire bytes, one float32 each), request_wire_lengths.npy,
+        response_<key>.npy (decoded values, float32) and, for float32 outputs, response_<key>_probe.npy (the planted sNaN
+        probe's bits as float64: the values are NaNs).  Arrays above max_elems are a fixed, seeded sample; the wire sample keeps
+        every record's first `head` bytes.  Varint workloads re-run slot s's encode (same inputs, same buffers) to learn offsets."""
+        wl, n = self.wl, self.n
+        st = self.sets[s % self.slots]
+        self.encode_results(s)
+        lens = np.array([int(st["rec_len"][j]) for j in range(n)], dtype=np.int64)
+        offs = np.array([int(st["rec_off"][j]) for j in range(n)], dtype=np.int64)
+        out_np = np.float32 if wl.out_dtype is None else wl.np_dtype      # float32, or fp16 / bf16 after the decode-side cast
+        per = self.dst_bytes // np.dtype(out_np).itemsize                  # elements per decoded tensor
+        probe = min(len(SNAN_PROBE), per) if wl.out_dtype is None else 0    # every float32 response tensor starts with the probe
+        m = per - probe
+
+        def sample(total, seed, keep=None):
+            if total <= max_elems:
+                return np.arange(total, dtype=np.int64)
+            keep = np.zeros(0, np.int64) if keep is None else keep
+            rand = np.random.default_rng(seed).integers(0, total, max(0, max_elems - keep.size), dtype=np.int64)
+            return np.unique(np.concatenate([keep, rand]))
+
+        start = np.concatenate([[0], np.cumsum(lens)])
+        heads = np.concatenate([start[j] + np.arange(min(head, lens[j])) for j in range(n)]) if n else np.zeros(0, np.int64)
+        wpos, ypos = sample(int(start[-1]), 1, heads), sample(n * m, 2)
+        wire, y, pbits = np.empty(wpos.size, np.float32), np.empty(ypos.size, np.float32), np.empty((n, probe), np.float64)
+        for j0 in range(0, n, chunk):
+            j1 = min(n, j0 + chunk)
+            lo = int(offs[j0])
+            arena = self.download(st["arena"] + lo, int(offs[j1 - 1] + lens[j1 - 1]) - lo)
+            sel = (wpos >= start[j0]) & (wpos < start[j1])
+            req = np.searchsorted(start, wpos[sel], side="right") - 1
+            wire[sel] = arena[offs[req] - lo + wpos[sel] - start[req]]
+            dst = self.download(st["dst"] + j0 * self.dst_stride, (j1 - j0) * self.dst_stride).reshape(j1 - j0, self.dst_stride)
+            vals = dst[:, :self.dst_bytes].copy()
+            pbits[j0:j1] = vals[:, :4 * probe].view(np.uint32)
+            vals = vals.view(out_np)
+            sel = (ypos >= j0 * m) & (ypos < j1 * m)
+            y[sel] = vals[ypos[sel] // m - j0, probe + ypos[sel] % m].astype(np.float32)
+        key = self.host_resp[wl.seed_of(self.lo)][0]
+        os.makedirs(out_dir, exist_ok=True)
+        np.save(os.path.join(out_dir, "request_wire.npy"), wire)
+        np.save(os.path.join(out_dir, "request_wire_lengths.npy"), lens.astype(np.float64))
+        np.save(os.path.join(out_dir, f"response_{key}.npy"), y)
+        if probe:
+            np.save(os.path.join(out_dir, f"response_{key}_probe.npy"), pbits.reshape(-1))
+
     def close(self):
         self.lib.b200tfs_destroy(self.ctx)
 
@@ -648,7 +695,7 @@ class HostLeg:
             for name in ("enc", "dec"):
                 ctx = C.c_void_p()
                 N.check(lib.b200tfs_create(db.device, C.byref(ctx)))
-                if depth > 1:      # the leg overlaps the copy directions ACROSS calls; slicing inside each call on top of that costs 3 %
+                if depth > 1:      # the leg overlaps the copy directions ACROSS calls; slicing inside each call on top of that is switched off
                     N.check(lib.b200tfs_set_pipeline(ctx, 0, 0))
                 if name == "dec" and wl.out_dtype is not None:
                     N.check(lib.b200tfs_set_decode_cast(ctx, wl.out_dtype))
@@ -749,45 +796,13 @@ def peaks():
     if os.path.exists(path):
         with open(path) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(workload, n_on_rank=None):
-    """dram read+write bytes per launch of the step's dominant kernel(s) (every captured kernel within 2x of the largest: the
-    C2 / C5 step has two, encode and decode; the C3 step one), averaged, from the newest committed ncu --set full summary that has
-    entries for this workload (profiles/rNN_ncu_summary.json, written by tools/ncu_summary.py).  C5 was captured on the per-GPU
-    share at N=8 (1024 requests); another share is scaled by its request count and says so."""
-    import glob
-
-    unit = {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    tag, scale, note = workload, 1.0, None
-    if workload == "c5":
-        tag = "c5share"
-        if n_on_rank and n_on_rank != 1024:
-            scale, note = n_on_rank / 1024.0, f"captured on 1024 requests, scaled to this rank's {n_on_rank}"
-    for path in sorted(glob.glob(os.path.join(REPO, "profiles", "r*_ncu_summary.json")), reverse=True):
-        with open(path) as fh:
-            caps = [c for c in json.load(fh).get("full_capture", []) if c.get("workload", "c2_single") == tag]
-        per = {}
-        for c in caps:
-            r, w = c.get("dram__bytes_read.sum"), c.get("dram__bytes_write.sum")
-            if r and w:
-                per.setdefault(c["kernel"], []).append(float(r["value"]) * unit.get(r["unit"], 1) + float(w["value"]) * unit.get(w["unit"], 1))
-        if per:
-            avg = {k: sum(v) / len(v) for k, v in per.items()}
-            top = max(avg.values())
-            dom = {k: v * scale for k, v in avg.items() if v * 2 >= top}
-            src = {"source": os.path.relpath(path, REPO), "per_kernel_bytes": dom}
-            if note:
-                src["note"] = note
-            return sum(dom.values()) / len(dom), src
-    return None, None
+    return 3350.0, "nominal (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 # ------------------------------------------------------------------------------------------------
 # one workload on this rank -> the pieces of the bench line
 # ------------------------------------------------------------------------------------------------
-def run_workload(wl: Workload, world: World, steps, warmup, e2e_steps, full_verify, sampler=None, e2e=True):
+def run_workload(wl: Workload, world: World, steps, warmup, e2e_steps, full_verify, sampler=None, e2e=True, dump_dir=None):
     peak, peak_src = peaks()
     db = DeviceBatch(wl, world.local_rank, world.size, world.rank)
     assert db.footprint > L2_BYTES or db.n == 0, "the batch ring must exceed L2"
@@ -827,6 +842,8 @@ def run_workload(wl: Workload, world: World, steps, warmup, e2e_steps, full_veri
     world.barrier()
     launches = (db.launches() - l0) if mode == "eager" else per_replay * (steps // db.slots) + (db.graphs["step_rem"][1] if steps % db.slots else 0)
     clocks = sampler.stop(t0, t1) if sampler else None
+    if dump_dir and world.rank == 0 and db.n:
+        db.dump(dump_dir, (steps - 1) % db.slots)         # the slot the last timed step wrote
     ms_max = world.max(ms)
     payload = world.sum(float(db.payload_bytes() * steps))
     value = payload / (ms_max * 1e-3) / 1e9
@@ -842,20 +859,19 @@ def run_workload(wl: Workload, world: World, steps, warmup, e2e_steps, full_veri
         db.timer.run(lambda k: db.replay("dec"), 1)
         t_dec = db.timer.run(lambda k: db.replay("dec"), reps_k) / (reps_k * db.slots)
     enc_kernel = "move_kernel" + (" (+ venc_len, frame_requests_kernel, venc_emit for the int64 labels: deferred framing, no host round trip)" if db.varint else "")
-    dec_kernel = ("decode_fused_staged_kernel" if db.resp_len * db.n > 148 * 8 * 32768 else "decode_fused_kernel") + \
+    dec_kernel = ("decode_fused_staged_kernel" if db.resp_len * db.n > 132 * 8 * 32768 else "decode_fused_kernel") + \
         ("" if wl.out_dtype is None else " (DT_FLOAT outputs narrowed to fp16 / bf16 in the same launch: b200tfs_set_decode_cast)")
     step_alg = enc_alg + dec_alg
     achieved = step_alg / ((t_enc + t_dec) * 1e-3) / 1e9 if db.n else 0.0
-    traffic, traffic_src = ncu_traffic(wl.name, db.n)
     roofline = {
         "bound": "hbm", "kernel": f"{enc_kernel} (encode) / {dec_kernel} (decode)", "achieved": achieved, "peak": peak, "unit": "GB/s",
-        "frac": achieved / peak, "frac_of_nominal_8000": achieved / 8000.0, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+        "frac": achieved / peak, "frac_of_nominal_3350": achieved / 3350.0, "peak_source": peak_src,
         "algorithmic_bytes_per_launch": step_alg / 2, "avg_launch_us": (t_enc + t_dec) / 2 * 1e3,
         "encode": {"launch_us": t_enc * 1e3, "algorithmic_bytes": enc_alg, "frac": enc_alg / (t_enc * 1e-3) / 1e9 / peak if db.n else 0.0},
         "decode": {"launch_us": t_dec * 1e3, "algorithmic_bytes": dec_alg, "frac": dec_alg / (t_dec * 1e-3) / 1e9 / peak if db.n else 0.0},
         "step_vs_launches": {"ms_per_step_this_rank": ms / steps, "encode_plus_decode_ms": t_enc + t_dec},
-        "peak_note": "peak is the driver's torch copy_ measurement over 2 GiB; a fraction above 1 means these kernels move bytes faster than that copy kernel "
-                     "does (nominal HBM3e: 8 TB/s, see frac_of_nominal_8000)",
+        "peak_note": "peak is MEASURED_PEAKS.json's hbm_gbs (a measured copy rate) when that file is present, else the H100 SXM data sheet's "
+                     "3.35 TB/s; a fraction above 1 of a measured peak means these kernels move bytes faster than that copy did",
         "how": f"this rank's share ({db.n} requests + {db.n} responses per step); each of the step's two calls timed alone over the same ring "
                f"({mode}), CUDA events on the context's stream; frac = algorithmic bytes of both / their summed durations / peak",
     }
@@ -863,7 +879,7 @@ def run_workload(wl: Workload, world: World, steps, warmup, e2e_steps, full_veri
     e2e_line = None
     if e2e and db.n:
         sub_mb = int(os.environ.get("B200TFS_E2E_SUB_MB", "128"))
-        sub = max(1, min(db.n, (sub_mb << 20) // max(db.src_bytes + db.resp_len, 1)))   # ~128 MB of H2D per sub-batch (64: 40.2 GB/s, 128: 41.6 on C2)
+        sub = max(1, min(db.n, (sub_mb << 20) // max(db.src_bytes + db.resp_len, 1)))   # ~128 MB of H2D per sub-batch
         depth = int(os.environ.get("B200TFS_E2E_DEPTH", "4"))
         leg = HostLeg(db, sub, depth)
         leg.verify()
@@ -915,7 +931,7 @@ def run_workload(wl: Workload, world: World, steps, warmup, e2e_steps, full_veri
            "parity": parity, "clocks": clocks,
            "config": {"workload": wl.title, "requests_per_step": wl.batch, "requests_on_this_rank": db.n,
                       "payload_bytes_per_step": int(world.sum(float(db.payload_bytes()))), "ring_slots": db.slots, "ring_bytes": db.footprint,
-                      "l2": f"each rank's buffers ({db.footprint >> 20} MiB over {db.slots} slot(s)) exceed the 126 MiB L2; steps rotate through the slots",
+                      "l2": f"each rank's buffers ({db.footprint >> 20} MiB over {db.slots} slot(s)) exceed the 50 MiB L2; steps rotate through the slots",
                       "timed_region": mode, "wire_mode": "typed fields (float_val / int64_val), sNaN quieting on: bit-exact vs the reference",
                       "sharding": ("one batch cut by request index across the ranks (r // ceil(n/G)), no collective" if wl.sharded
                                    else "every rank runs the whole batch on its own GPU (independent requests), no collective"),
@@ -1198,6 +1214,9 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-extra", action="store_true", help="default c2 run only: skip the short c3 / c4 / c5 passes reported under `workloads`")
     ap.add_argument("--verify", default="full", choices=["full", "sample"], help="parity check after the timed region")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the wire bytes and decoded tensors of the last step "
+                                                            "(rank 0's share) to DIR/<name>.npy, float32 / float64 (the planted NaN probe as bit patterns), "
+                                                            "a seeded sample of large arrays")
     args = ap.parse_args()
     if args.impl == "reference":   # CPU only: rank 0 works alone, nobody needs a process group
         run_reference(args)
@@ -1209,7 +1228,8 @@ def main():
     warmup = max(args.warmup, 3)
     wl = WORKLOADS[args.workload](args.batch or None)
     sampler = ClockSampler(world.local_rank)
-    res = run_workload(wl, world, args.steps, warmup, args.e2e_steps, full_verify=(args.verify == "full"), sampler=sampler)
+    res = run_workload(wl, world, args.steps, warmup, args.e2e_steps, full_verify=(args.verify == "full"), sampler=sampler,
+                       dump_dir=args.dump_outputs)
     extras = {}
     if args.workload == "c2":
         if not args.no_extra:

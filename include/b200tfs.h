@@ -1,5 +1,5 @@
 /* b200tfs.h - C ABI of libb200tfs.so: the TensorProto / PredictRequest / PredictResponse wire codec
- * of zendesk/min-tfs-client's Predict hot path, run as hand-written sm_100a CUDA kernels.
+ * of zendesk/min-tfs-client's Predict hot path, run as hand-written sm_90a (H100) CUDA kernels.
  *
  * The reference has no FFI: its hot path is Python calling the protobuf runtime.  The seams this
  * library replaces are (paths relative to the reference checkout):
@@ -410,15 +410,13 @@ int b200tfs_pipelined_calls(b200tfs_ctx* ctx, uint64_t* count);
 /* Output straight into the caller's buffer: when wire_host (encode) / dst_host (decode) is page-locked memory the device can
  * address (b200tfs_host_alloc, cudaHostAlloc, cudaHostRegister), is 256-byte aligned and - encode - has room for the arena
  * layout (b200tfs_request_arena_size bytes: records start 256-byte aligned, so record 0 need not start at offset 0; read
- * rec_off), the kernels write it themselves with posted PCIe writes and no device-to-host copy is queued at all (one 4 MiB call:
- * 177 -> 156 us with four slices).  Pageable or unaligned buffers take the staged route as before.  B200TFS_DIRECT_OUT=0 or
+ * rec_off), the kernels write it themselves with posted PCIe writes and no device-to-host copy is queued at all.  Pageable or unaligned buffers take the staged route as before.  B200TFS_DIRECT_OUT=0 or
  * b200tfs_set_pipeline(ctx, 0, 0) switches it off; this counts the calls that took it.                                                            */
 int b200tfs_direct_calls(b200tfs_ctx* ctx, uint64_t* count);
 /* Tune it per context: calls moving fewer than min_bytes of fixed-width payload stay monolithic (0 = never slice), at most
- * max_slices slices (2..8; default 4 - every slice costs about seven driver calls, ~7 us of host time).  A caller that keeps
- * several contexts busy at once already overlaps the two copy directions ACROSS calls and should switch slicing off: measured
- * on C2 with 8 contexts in flight, 40.2 GB/s monolithic vs 38.9 sliced; one call at a time: 177 -> 161 us (4 MiB), 2454 -> 1692 us
- * (64 MiB) (profiles/r02_pipeline.md).                                                              */
+ * max_slices slices (2..8; default 4 - every slice costs about seven driver calls of host time).  A caller that keeps
+ * several contexts busy at once already overlaps the two copy directions ACROSS calls and should switch slicing off: there the
+ * slices only add driver calls, while a lone call gains from overlapping its own copies with its kernels.                    */
 int b200tfs_set_pipeline(b200tfs_ctx* ctx, uint64_t min_bytes, int32_t max_slices);
 int b200tfs_encode_tensor_protos_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_tensor* tensors,
                                       void* wire_host, uint64_t wire_cap, uint64_t* rec_off,

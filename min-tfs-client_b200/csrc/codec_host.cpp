@@ -78,7 +78,7 @@ struct MeasuredTensor {     // what b200tfs_measure learnt about one varint tens
 
 struct b200tfs_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;   // H100 SXM; replaced by the device's own count when the context is created
   cudaStream_t stream = nullptr;       // the stream every call is ordered on: the context's own, or the caller's (b200tfs_set_stream)
   cudaStream_t own_stream = nullptr;
   cudaStream_t aux_stream = nullptr;   // uploads done at capture time, outside the graph being recorded; the pipelined host path's H2D copies
@@ -197,7 +197,7 @@ static int claim_slot(b200tfs_ctx* c, uint64_t bytes, Slot** out) {
 // Bring a slot's pinned image to its device image.  While a graph is being captured the slot is private to that graph and its
 // image never changes (plans, tables and framing programs are functions of the call's arguments, which a graph freezes
 // anyway): it is copied NOW, on a side stream, instead of being recorded as a copy node that every replay would repeat
-// (2-3 us of stream time per node; a captured C3 encode had three of them).
+// (each such node costs stream time on every replay; a captured C3 encode had three of them).
 static int upload_slot(b200tfs_ctx* c, Slot* slot, uint64_t bytes) {
   if (c->capturing) {
     CU(cudaMemcpyAsync(slot->dev.p, slot->host.p, bytes, cudaMemcpyHostToDevice, c->aux_stream));
@@ -1270,12 +1270,12 @@ static void adopt_pinned_template(b200tfs_ctx* c) {
 }
 
 // tile size of a decode launch over `wire_total` bytes: every CTA of the fused kernel first verifies the record's framing, so
-// big batches get fatter tiles than the plain move: measured 0.745 / 0.775 / 0.80 of peak at 64 / 128 / 256 KB
+// big batches get fatter tiles than the plain move (up to 256 KB): fewer CTAs repeat that verification
 static uint32_t decode_vpt(const b200tfs_ctx* c, int32_t n, const uint64_t* rec_len) {
   uint64_t wire_total = 0;
   for (int i = 0; i < n; ++i) wire_total += rec_len[i];
   // a narrowing launch (b200tfs_set_decode_cast) moves its tiles through the general tile routine, whose rounds of 8 KB run one
-  // after the other inside a CTA: small tiles, many CTAs (256 KB tiles: 270 us for the C4 batch; 64 KB: see profiles/r02_c4.md)
+  // after the other inside a CTA: small tiles, many CTAs (64 KB rather than 256 KB)
   return pick_vec_per_tile(c, c->decode_cast ? wire_total / 2 : wire_total, c->decode_cast ? 65536 : 262144);
 }
 
@@ -1407,7 +1407,7 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
     return B200TFS_OK;
   };
   // The narrowing decode of a batch whose template the host knows, as three launches: the narrowing tile move runs twice as
-  // long inside the fused kernel as in the generic move engine (profiles/r02_c4.md), so (1) two CTAs per record verify the
+  // long inside the fused kernel as in the generic move engine (it shares the walker's register cap there), so (1) two CTAs per record verify the
   // framing against the host's template - handed over in the parameters, the very one the plan below is built from - leave the
   // verdict in guard[r] and publish the table, (2) move_guarded_kernel moves every record's chunks from a host-built plan
   // and stores only where guard[r] says so, (3) the whole decode runs for the records still unguarded (none, normally: its
@@ -1578,8 +1578,8 @@ uint64_t tensor_src_bytes(const b200tfs_tensor& t) {
 struct StagePiece { const uint8_t* dev; const uint8_t* host; uint64_t nb; };
 
 // Host-to-device copies of a batch, merged where consecutive ones continue each other on BOTH sides (a batch whose tensors lie
-// back to back in one pinned buffer - bench.py's lanes, a caller's arena - becomes one copy instead of one per tensor: ~2 us of
-// driver time each, 15-20 % of a 602 KB tensor's time on the link).
+// back to back in one pinned buffer - bench.py's lanes, a caller's arena - becomes one copy instead of one per tensor: each copy
+// costs driver time, a sizeable share of a 602 KB tensor's time on the link).
 struct CopyMerger {
   cudaStream_t stream;
   uint8_t* d = nullptr; const uint8_t* h = nullptr; uint64_t n = 0;
@@ -1658,9 +1658,8 @@ bool host_measurable_varint(const b200tfs_tensor& t) {
 }
 
 // Is this host pointer page-locked memory the device can address (cudaHostAlloc / cudaHostRegister under unified addressing)?
-// Then a kernel may write its output there itself - posted PCIe writes at the link rate (4 MiB: 96 us from launch to synchronise
-// against 178 for H2D + kernel + D2H, profiles/r02_pipeline.md) - and the device-to-host copy disappears.  (The other direction
-// does not pay: SM-issued reads of host memory run at ~34 GB/s, the copy engine's at 55.)
+// Then a kernel may write its output there itself - posted PCIe writes at the link rate - and the device-to-host copy
+// disappears.  (The other direction does not pay: SM-issued reads of host memory are slower than the copy engine's.)
 uint8_t* device_view_of_host(const void* p) {
   cudaPointerAttributes a;
   if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return nullptr; }
@@ -1807,7 +1806,7 @@ int b200tfs_encode_requests_host_async(b200tfs_ctx* c, int32_t n, const b200tfs_
   }
   // Packed-varint inputs of up to 4096 elements that lie in HOST memory (labels, ids, one sequence of token ids) are measured
   // right here - a few microseconds of host arithmetic instead of a counting kernel, a device-to-host copy and a stream
-  // synchronise (b200tfs_measure: 30-40 us before anything else of the call can be queued).
+  // synchronise (b200tfs_measure: the call can queue nothing else until that round trip is over).
   bool device_measure = false;
   for (auto& t : ts) {
     if (!host_measurable_varint(t)) { device_measure = device_measure || needs_measure_one(t); continue; }

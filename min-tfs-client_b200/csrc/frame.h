@@ -4,7 +4,7 @@
 // A request's program is looked at through a FrameView: its segments, values and terms (request-local indices), the value of
 // every FT_TOTAL term already fetched, its slice of the blob.  On the device a warp stages all of that in shared memory with
 // three rounds of parallel loads and one lane then runs frame_request_run out of shared memory - a lone lane chasing the
-// tables through global memory paid ~60 dependent L2 round trips per request (30+ us for a batch; 102 us C3 encode).
+// tables through global memory paid ~60 dependent L2 round trips per request.
 #pragma once
 #include "plan.h"
 #include "wire.h"

@@ -1,5 +1,5 @@
-// kernels.cu - sm_100a kernels of the TensorProto wire codec (pure HBM-bound byte packing: no
-// tensor cores, no tcgen05 - see DESIGN.md "Roofline").
+// kernels.cu - sm_90a (H100) kernels of the TensorProto wire codec (pure HBM-bound byte packing: no
+// tensor cores - see DESIGN.md "Roofline").
 //
 //   move_kernel{,_inline}  the pack/unpack engine: moves every payload between tensor memory and the
 //                      wire arena (128-bit coalesced loads/stores, destination-aligned, a whole 32 KB
@@ -216,7 +216,7 @@ __device__ __forceinline__ bool body_aligned(const uint8_t* __restrict__ src, ui
 // S = source body rounded down to 16 bytes; output vector v = bytes [k, k+16) of blocks v, v+1.
 // Each source block is loaded ONCE: lane L takes block v+1 from lane L+1 by shuffle (lane 31, and
 // the last lane of a ragged tile, load it themselves: +1/32 traffic).  ncu showed why: two loads
-// of the same block in flight together are not merged - both go to DRAM (profiles/r01_*).
+// of the same block in flight together are not merged - both go to DRAM.
 __device__ __forceinline__ uint4 shfl_down1(const uint4& v) {
   uint4 r;
   r.x = __shfl_down_sync(0xFFFFFFFFu, v.x, 1); r.y = __shfl_down_sync(0xFFFFFFFFu, v.y, 1);
@@ -292,7 +292,7 @@ __device__ __forceinline__ bool body_same_width(const uint8_t* src, uint8_t* dst
 }
 
 // f16 / bf16 -> f32 (encode-side cast).  Both sides 16-byte aligned; unit u = 16 source bytes -> 32 out.  Eight loads per thread
-// are in flight before the first store, like the same-width bodies (two were: 0.74 of peak on the C4 batch).
+// are in flight before the first store, like the same-width bodies (two were too few to cover DRAM latency).
 template <bool BF>
 __device__ __forceinline__ void body_widen(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, uint32_t units) {
   constexpr uint32_t kU = 8;
@@ -333,7 +333,7 @@ __device__ __forceinline__ uint32_t narrow2(uint32_t a, uint32_t b) {
 // Output vector u (8 halfs) <- source blocks 2u, 2u+1 (+ 2u+2 when the source is shifted).  Every warp owns a contiguous run of
 // 32 * kU output vectors per round, so that block 2u+2 is the neighbour lane's block 2(u+1) - by shuffle - and only the run's
 // last vector needs a load of its own; all 2 * kU (+1) loads of a thread are issued before its first store (with two vectors per
-// thread the C4 batch decode ran at 0.48 of peak: 24 warps per SM x 64 B in flight each).
+// thread too few bytes are in flight per SM to cover DRAM latency).
 // `mid` runs once, between the first round's loads and its stores (the fused decode's framing verdict: nothing may be stored
 // before it, but the tile's bytes can already be on their way).
 template <bool BF, int Q, class Mid>
@@ -759,8 +759,8 @@ __device__ __forceinline__ void staged_finish(const StagedTile& t, const uint8_t
 // Each CTA checks, one byte per thread, that this record's framing bytes equal the template's (and
 // that packed-varint chunks still end on a terminator); identical framing bytes of an identical
 // length parse identically, so the CTA takes its tile straight from the template.  Cost: one DRAM
-// round trip for the two framing lines instead of a serial tag walk (a lone GPU lane needs ~15 us
-// for the ~100 header bytes).
+// round trip for the two framing lines instead of a serial tag walk (a lone GPU lane walks ~100 header
+// bytes through many dependent loads).
 //
 // Slow path - thread 0 walks the tags through the line cache (walker.h), lays the outputs out in the
 // record's destination slot and finds which value chunk tile j falls in; CTA (record 0, tile 0) also
@@ -856,14 +856,14 @@ __device__ __noinline__ void fused_slow_path(const FusedParams& fp, uint32_t r, 
 // loads at once and checks, one byte per thread, that this record's framing bytes equal the template's while those loads are
 // in flight (packed-varint chunks must still end on a terminator) - one DRAM round trip in all.  Otherwise the template the
 // previous launch left in device memory is used (one more dependent load).  A record that misses the template is walked:
-// thread 0 goes through the tags with the line cache (a lone GPU lane needs ~15 us for ~100 header bytes), lays the outputs out
+// thread 0 goes through the tags with the line cache (a lone GPU lane walks ~100 header bytes through dependent loads), lays the outputs out
 // and finds which value chunk tile j falls in; CTA (record 0, tile 0) also leaves the template for the next launch.
 //
 // STAGED: tiles of more than one 32 KB chunk (big batches) take the TMA-staged path above; the other instantiation - a single
 // response, small batches - carries none of that code and instead runs the verdict as the `mid` hook of the tile move (the
 // registers that holds across the barrier cost the big-batch kernel a CTA per SM, so only this one does it).
 // CAST: the instantiations behind b200tfs_set_decode_cast carry the narrowing tile move as well; the plain ones are exactly the
-// round-1/2 kernels (the extra branch and registers cost the single-response launch 0.25 us when it lived in the same kernel).
+// round-1/2 kernels (the extra branch and registers slowed the single-response launch when it lived in the same kernel).
 template <bool STAGED, bool CAST>
 __device__ __forceinline__ void decode_fused_body(const FusedParams& fp) {
   pdl_launch_dependents();
@@ -1031,9 +1031,11 @@ __device__ __forceinline__ void decode_fused_body(const FusedParams& fp) {
 // two CTAs per SM: the tile (8 x 128-bit per thread) stays in registers across the verdict's barrier without spilling; this instantiation serves
 // single responses and small batches, where a third resident CTA has nothing to hide
 __global__ void __launch_bounds__(kMoveThreads, 2) decode_fused_kernel(const __grid_constant__ FusedParams fp) { decode_fused_body<false, false>(fp); }
-__global__ void __launch_bounds__(kMoveThreads, 3) decode_fused_staged_kernel(const __grid_constant__ FusedParams fp) { decode_fused_body<true, false>(fp); }
+// the staged (batch) instantiations too: on sm_90a a third CTA per SM caps them at 80 registers and spills the walker's state
+// (132 B of stores); at two the batch decode measured 3-4 % faster on an H100 (C2 773 -> 750 us, C5 share 3569 -> 3426 us)
+__global__ void __launch_bounds__(kMoveThreads, 2) decode_fused_staged_kernel(const __grid_constant__ FusedParams fp) { decode_fused_body<true, false>(fp); }
 __global__ void __launch_bounds__(kMoveThreads, 2) decode_fused_cast_kernel(const __grid_constant__ FusedParams fp) { decode_fused_body<false, true>(fp); }
-__global__ void __launch_bounds__(kMoveThreads, 3) decode_fused_staged_cast_kernel(const __grid_constant__ FusedParams fp) { decode_fused_body<true, true>(fp); }
+__global__ void __launch_bounds__(kMoveThreads, 2) decode_fused_staged_cast_kernel(const __grid_constant__ FusedParams fp) { decode_fused_body<true, true>(fp); }
 
 // ------------------------------------------------------------------------------------------------
 // packed varints: venc_len / venc_emit / vdec_count / vdec_emit
@@ -1120,8 +1122,8 @@ __global__ void __launch_bounds__(256) fill_edge_kernel(uint8_t* __restrict__ ds
 // launchers (the only symbols codec_host.cpp sees)
 // ------------------------------------------------------------------------------------------------
 // launch, optionally with programmatic stream serialization (see pdl_* above).  Measured on the C2 bench:
-// with it, 8 overlapping lanes gain 4 % (0.89 -> 0.93 of HBM peak) but a single stream of back-to-back
-// launches loses 0.6 us per launch (3.5 -> 4.1 us), so it is opt-in: B200TFS_PDL=1.
+// with it, overlapping lanes gained a little bandwidth but a single stream of back-to-back launches
+// got slower per launch, so it is opt-in: B200TFS_PDL=1.
 template <class... KArgs, class... Args>
 static cudaError_t launch_pdl(void (*kernel)(KArgs...), uint32_t grid, uint32_t block, uint32_t dyn_smem, cudaStream_t stream, Args&&... args) {
   static const bool env_off = [] { const char* e = getenv("B200TFS_PDL"); return !(e && e[0] == '1'); }();
@@ -1178,7 +1180,7 @@ uint32_t tiles_for_host(uint64_t n_out, uint32_t vpt) { return tiles_for(n_out, 
 cudaError_t launch_fill_edge(uint8_t* dst, uint32_t elem_size, uint64_t have, const unsigned long long* have_dev, uint64_t n_elems,
                              cudaStream_t stream) {
   if (!n_elems) return cudaSuccess;
-  const uint64_t blocks = std::min<uint64_t>((n_elems + 255) / 256, 148 * 8);
+  const uint64_t blocks = std::min<uint64_t>((n_elems + 255) / 256, 132 * 8);   // 8 CTAs on each of the H100's 132 SMs
   fill_edge_kernel<<<(uint32_t)blocks, 256, 0, stream>>>(dst, elem_size, have, have_dev, n_elems);
   return cudaGetLastError();
 }
@@ -1197,9 +1199,9 @@ cudaError_t launch_decode_fused(const FusedParams& fp, uint32_t grid, cudaStream
       opted[dev] = true;
     }
   }
-  // Tiles of more than one 32 KB chunk (big batches: up to 256 KB per CTA) go through the TMA-staged path: measured
-  // 0.87 -> 0.90 of peak on 1024 x 602 KB.  One-chunk tiles (a single 4 MiB response) keep the register path and no
-  // staging buffers: there the staged path gained 0.15 us on one stream but cost 13 % when 16 lanes overlap.
+  // Tiles of more than one 32 KB chunk (big batches: up to 256 KB per CTA) go through the TMA-staged path, which moved
+  // big batches faster.  One-chunk tiles (a single 4 MiB response) keep the register path and no staging buffers: there
+  // the staged path gained little on one stream and lost bandwidth when many lanes overlap.
   if (fp.cast) {
     if (fp.vpt > kStageVecs && fp.mode != 1) return launch_pdl(decode_fused_staged_cast_kernel, grid, kMoveThreads, kFusedDynSmem, stream, fp);
     return launch_pdl(decode_fused_cast_kernel, grid, kMoveThreads, 0, stream, fp);

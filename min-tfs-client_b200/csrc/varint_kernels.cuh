@@ -17,11 +17,10 @@
 //                              12-byte window (7-bit groups compressed with masks and shifts)
 //
 // There is no separate scan kernel: a tile's prefix is one coalesced read of <= 256 + n_tiles/256
-// counters.  Two single-pass decoders were measured and dropped (16M int64, B200): a decoupled look-back over
-// per-tile states (emit 113 -> 135 us: ~100 tiles start per microsecond, a 32-wide look-back cannot keep up
-// and seven warps idle at the barrier behind it) and a ticketed "wait until every predecessor has published,
-// then one parallel read" (205 us: the wait is the slowest of 255 neighbours).  The counting pass costs 27 us
-// and leaves the wire in L2 for the decoder.  History and numbers: profiles/r01_varint.md.
+// counters.  Two single-pass decoders were tried and dropped: a decoupled look-back over per-tile states
+// (tiles start faster than a 32-wide look-back can keep up, and seven warps idle at the barrier behind it) and
+// a ticketed "wait until every predecessor has published, then one parallel read" (the wait is the slowest of
+// 255 neighbours).  The counting pass is cheap and leaves the wire in L2 for the decoder.
 //
 // What the reference does here: tensors.py:22 (`.item()` per element into RepeatedScalarContainer,
 // the runtime then writes one varint at a time) and tensors.py:46 (list of Python ints -> np.array).
@@ -355,13 +354,13 @@ __global__ void __launch_bounds__(kVarThreads, 5) venc_emit_kernel(const __grid_
 // E3: ONE pass - count, place and emit in a single kernel (the deferred encode's anchored jobs: a packed-varint payload whose
 // first byte the host could fix in advance).  venc_emit recomputes every length anyway; what it lacks is where its tile's
 // bytes go, i.e. the byte count of all tiles before it.  That prefix comes from a two-level look-back instead of a counting
-// kernel (which read the whole tensor once more - 25 of 95 us on 16M int64):
+// kernel (which reads the whole tensor once more):
 //   * tiles take their number from a ticket (started tiles only ever wait for tiles that started earlier);
 //   * a tile publishes its byte count as soon as its lengths are scanned; groups of kVarFuseGroup consecutive tiles: the tile
 //     whose publication completes a group sums the group and resolves the group's exclusive prefix by a decoupled look-back
 //     over GROUP descriptors (a few per microsecond - a 32-wide window always reaches a resolved group; at TILE level ~100
 //     tiles start per microsecond and round 1's tile-level look-back could not keep up), before it builds its own image;
-//   * every tile builds its image first (the expensive part, ~3 us) and only then reads what it needs - the previous group's
+//   * every tile builds its image first (the expensive part) and only then reads what it needs - the previous group's
 //     inclusive prefix and the counts of the tiles before it inside its group, all long since published - so the look-back
 //     costs nothing on the critical path.  The image is built at phase 0 and realigned on the way out (two 128-bit shared
 //     loads and a funnel shift per 128-bit store), since the destination's phase is not known while building.
@@ -385,8 +384,7 @@ struct FuseJob {
 
 // Run by ONE warp of the CTA (all 32 lanes), the tile's bookkeeper, while the other warps do the tile's heavy work.  Lane 0
 // publishes the tile's count - one store, flag and count in the same word, so no fence and no atomic is needed anywhere in
-// this protocol (a __threadfence here waited for the PREVIOUS tile's streaming stores of the persistent CTA: 192 us instead of
-// 123).  The group's LAST tile (by ticket) resolves the group: it collects the 32 counts (all from earlier tickets, i.e. from
+// this protocol (a __threadfence here would wait for the PREVIOUS tile's streaming stores of the persistent CTA).  The group's LAST tile (by ticket) resolves the group: it collects the 32 counts (all from earlier tickets, i.e. from
 // tiles that have started and publish before they wait for anything), publishes the AGG descriptor, looks back over earlier
 // groups and publishes the INC descriptor.  Returns the job's total in every lane when this warp resolved the job's LAST
 // group, else ~0ull.
@@ -448,7 +446,7 @@ __device__ __forceinline__ unsigned long long fuse_prefix_complete(const FuseJob
 // Persistent CTAs: each takes tiles by ticket until none are left (the next ticket is fetched while the current tile is being
 // worked on).  The LAST warp is the tile's bookkeeper: while the other seven build their part of the image it publishes the
 // count, resolves the group if need be and fetches the tile's prefix - three dependent L2 round trips that, done by the whole
-// CTA behind barriers (first version: 123 us on 16M int64, 40 % issue-active, barrier stalls 11 per issue), cost more than the
+// CTA behind barriers (the first version: low issue activity, many barrier stalls), cost more than the
 // counting kernel they replace - and then builds its own 256 elements.
 __global__ void __launch_bounds__(kVarThreads, 5) venc_fused_kernel(const __grid_constant__ VarTables tb, const __grid_constant__ VarFuse fz) {
   __shared__ __align__(16) uint8_t smem[kVarImageBytes + 16];

@@ -190,7 +190,7 @@ class Codec:
         ctx = C.c_void_p()
         rc = self._lib.b200tfs_create(device, C.byref(ctx))
         if rc != N.OK:
-            raise RuntimeError(f"cannot create a B200 codec context on device {device}: {N.last_error()}")
+            raise RuntimeError(f"cannot create a GPU codec context on device {device}: {N.last_error()}")
         self._ctx = ctx
         self.device = device
         self._pinned = D.PinnedArrays()

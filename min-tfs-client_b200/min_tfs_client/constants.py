@@ -41,7 +41,7 @@ ENUM_TO_TF_MAPPING = {v: NP_TO_TF_MAPPING[k].TFDType for k, v in NP_TO_ENUM_MAPP
 
 NUMERICAL_TYPES = {np_type for np_type, _, _ in _ROWS if np_type is not np.str_}
 
-# --- additions for the B200 codec -------------------------------------------------------------
+# --- additions for the GPU codec --------------------------------------------------------------
 try:  # optional: bfloat16 host arrays
     import ml_dtypes as _ml_dtypes
 

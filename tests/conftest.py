@@ -11,7 +11,7 @@ for p in (PKG_ROOT, REPO, os.path.dirname(os.path.abspath(__file__))):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def _have_gpu():

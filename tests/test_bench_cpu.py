@@ -65,23 +65,6 @@ def test_cpu_baseline_leg_runs_the_unmodified_reference():
     assert bench.cpu_c_oracle(1)["value"] > r["value"]          # plain C beats per-element Python
 
 
-def test_staged_reference_archive_matches_the_checkout():
-    """baseline/_ref/min_tfs_client_reference.zip holds the three reference modules byte for byte (when both are present)."""
-    import hashlib
-    import zipfile
-
-    from baseline import ref_loader, stage_reference
-
-    if not (os.path.isdir(ref_loader.REF_DIR) and os.path.exists(ref_loader.ZIP)):
-        pytest.skip("needs the reference checkout and the staged archive")
-    with zipfile.ZipFile(ref_loader.ZIP) as z:
-        manifest = json.loads(z.read("MANIFEST.json"))
-        for f in stage_reference.FILES:
-            with open(os.path.join(ref_loader.REF_DIR, f), "rb") as fh:
-                blob = fh.read()
-            assert z.read("min_tfs_client/" + f) == blob and manifest[f] == hashlib.sha256(blob).hexdigest()
-
-
 def test_host_cores_is_sane():
     h = bench.host_cores()
     assert 1 <= h["used"] <= h["affinity"]
@@ -108,3 +91,49 @@ def test_reference_arm_prints_one_contract_line():
     out1 = subprocess.run([sys.executable, os.path.join(REPO, "bench.py"), "--impl", "reference", "--steps", "1"], capture_output=True, text=True,
                           env=dict(os.environ, RANK="1"), timeout=60)
     assert out1.returncode == 0 and out1.stdout.strip() == ""
+
+
+class _FakeBatch:
+    """DeviceBatch.dump over host memory: ragged records with gaps, decoded float32 tensors led by the sNaN probe."""
+    dump = bench.DeviceBatch.dump
+
+    def __init__(self, wl, n=60, per=200, stride=1024):
+        rng = np.random.default_rng(5)
+        self.wl, self.n, self.slots, self.lo, self.dst_stride = wl, n, 1, 0, stride
+        self.lens = rng.integers(100, 400, n)
+        self.offs = np.concatenate([[0], np.cumsum(self.lens + 7)])[:n]
+        self.arena = rng.integers(0, 256, int(self.offs[-1] + self.lens[-1])).astype(np.uint8)
+        self.vals = rng.standard_normal((n, per)).astype(np.float32 if wl.out_dtype is None else wl.np_dtype)
+        if wl.out_dtype is None:
+            self.vals[:, :4] = bench.SNAN_PROBE
+        self.dst_bytes = self.vals[0].nbytes
+        self.dst = np.zeros((n, stride), np.uint8)
+        self.dst[:, :self.dst_bytes] = self.vals.view(np.uint8).reshape(n, -1)
+        self.sets = [{"rec_len": list(self.lens), "rec_off": list(self.offs), "arena": 0, "dst": 1 << 40}]
+        self.host_resp = {0: ("y", None)}
+
+    def encode_results(self, s):
+        pass
+
+    def download(self, ptr, nbytes):
+        mem = self.dst.reshape(-1) if ptr >= 1 << 40 else self.arena
+        return mem[ptr % (1 << 40):][:nbytes].copy()
+
+
+@pytest.mark.parametrize("wl", [bench.C2(), bench.C4()], ids=["f32_with_probe", "f16"])
+def test_dump_outputs_maps_samples_to_the_right_bytes(wl, tmp_path):
+    fb, probe = _FakeBatch(wl), 4 if wl.out_dtype is None else 0
+    start = np.concatenate([[0], np.cumsum(fb.lens)])
+    wire = np.concatenate([fb.arena[o: o + k] for o, k in zip(fb.offs, fb.lens)])
+    vals = fb.vals[:, probe:].astype(np.float32).reshape(-1)
+    heads = np.concatenate([start[j] + np.arange(64) for j in range(fb.n)])          # every record's framing is in the sample
+    for cap, wpos, ypos in ((1 << 30, np.arange(wire.size), np.arange(vals.size)),
+                            (5000, np.unique(np.concatenate([heads, np.random.default_rng(1).integers(0, wire.size, 5000 - heads.size)])),
+                             np.unique(np.random.default_rng(2).integers(0, vals.size, 5000)))):
+        fb.dump(str(tmp_path / str(cap)), 0, max_elems=cap, chunk=16)
+        got = {f.stem: np.load(f) for f in (tmp_path / str(cap)).iterdir()}
+        assert all(np.isfinite(a).all() for a in got.values()) and np.array_equal(got["request_wire_lengths"], fb.lens)
+        assert np.array_equal(got["request_wire"], wire[wpos]) and np.array_equal(got["response_y"], vals[ypos])
+        assert ("response_y_probe" in got) == bool(probe)
+        if probe:
+            assert np.array_equal(got["response_y_probe"], np.tile(bench.SNAN_PROBE.view(np.uint32), fb.n))

@@ -40,7 +40,7 @@ def main():
     dev = Dev(0)
     lib = dev.lib
     out = {}
-    peak = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(REPO, "MEASURED_PEAKS.json")) else 6650.0
+    peak = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists(os.path.join(REPO, "MEASURED_PEAKS.json")) else 3350.0
     # ---- C5 share: 1024 x fp32[3,224,224] ------------------------------------------------------
     n, P = 1024, 3 * 224 * 224 * 4
     src = dev.malloc(n * P)

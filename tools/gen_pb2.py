@@ -23,8 +23,8 @@ and, for the client's other RPCs (reference requests.py:67-110), host-side messa
   tensorflow_serving/apis/get_model_status.proto, tensorflow_serving/util/status.proto,
   tensorflow/core/{lib/core,protobuf}/error_codes.proto
 
-``tests/test_schema.py`` re-reads the reference ``.proto`` files (when ``/root/reference`` exists)
-with a tiny tokenizer and checks every field name / number / type / label against these tables.
+``tests/test_schema.py`` checks every field name / number / type / label of the generated modules against a
+snapshot of these tables stored in ``tests/golden/schema.json`` (recorded from the generated modules).
 
 Usage:  python tools/gen_pb2.py            (rewrites the modules in place; idempotent)
 """

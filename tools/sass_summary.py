@@ -3,7 +3,7 @@
 bytes move - 128-bit global loads / stores, TMA bulk copies and their mbarrier traffic, shuffles, local-memory (stack) accesses,
 tensor-core ops (none: this path has no FLOPs).  Needs no GPU.
 
-    python tools/sass_summary.py > profiles/r02_sass.md
+    python tools/sass_summary.py > sass.md
 """
 import collections
 import os
@@ -48,7 +48,7 @@ def sass():
 
 
 def ptxas():
-    flags = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-c",
+    flags = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-Xptxas", "-v", "-c",
              os.path.join(CSRC, "kernels.cu"), "-o", "/tmp/_sass_summary.o"]
     err = subprocess.run(["nvcc"] + flags, capture_output=True, text=True).stderr
     info, cur = {}, None
@@ -77,7 +77,7 @@ def demangle(n):
 
 def main():
     ks, info = sass(), ptxas()
-    print("# SASS of the shipped library (`min-tfs-client_b200/lib/libb200tfs.so`, sm_100a) - `python tools/sass_summary.py`\n")
+    print("# SASS of the shipped library (`min-tfs-client_b200/lib/libb200tfs.so`, sm_90a) - `python tools/sass_summary.py`\n")
     print("Per kernel: instructions (x 16 B = code size), registers / stack / spill bytes / static shared memory as ptxas reports them, and how "
           "many instructions of each kind the cubin holds (static counts, not executed counts).\n")
     print("| kernel | SASS instr | code KB | regs | stack B | spill st/ld B | smem B |")
