@@ -323,7 +323,7 @@ int b200tfs_parse_tensor_protos(b200tfs_ctx* ctx, const void* arena_dev, int32_t
 /* Unpack m tabulated outputs into device buffers: out_rec_off[j] is the arena offset of the record
  * outs[j] came from (NULL: all zero); dst[j] receives outs[j].dst_bytes bytes (or
  * n_elems * sizeof(dst_dtype[j]) when dst_dtype[j] != outs[j].dtype and the cast is supported:
- * FLOAT -> HALF / BFLOAT16 round-to-nearest-even).  status[j] (host, filled after an internal sync
+ * FLOAT -> HALF / BFLOAT16 round-to-nearest-even; NaNs as b200tfs_set_decode_cast describes).  status[j] (host, filled after an internal sync
  * only if `status` is non-NULL) reports per-output errors found while unpacking (element count
  * mismatch, integer out of range).  Async when status is NULL.                                    */
 int b200tfs_unpack_outputs(b200tfs_ctx* ctx, const void* arena_dev, int32_t m, const b200tfs_output* outs,
@@ -347,7 +347,9 @@ int b200tfs_decode_responses(b200tfs_ctx* ctx, const void* arena_dev, int32_t n,
 /* Narrow on the way out (what a caller of the reference writes as tensor_proto_to_ndarray(...).astype(np.float16), tensors.py:42-46
  * followed by a host-side cast): after b200tfs_set_decode_cast(ctx, DT_HALF or DT_BFLOAT16) every DT_FLOAT output of
  * b200tfs_decode_responses / b200tfs_decode_responses_host_async on this context is written as fp16 / bf16 (IEEE round to nearest
- * even, the rounding of numpy's astype; b200tfs_output.dst_bytes = 2 * n_elems, .dtype stays DT_FLOAT, the wire's).  Outputs of
+ * even, the rounding of numpy's astype; b200tfs_output.dst_bytes = 2 * n_elems, .dtype stays DT_FLOAT, the wire's).  A NaN is
+ * quieted first, as the reference's decode does, then becomes sign | 0x7E00 | ((w >> 13) & 0x3FF) in fp16 (numpy's astype) and
+ * sign | 0x7FC0 in bf16 (ml_dtypes' astype).  Outputs of
  * other dtypes are unaffected.  DT_FLOAT (or 0) switches it off.  This is the decode half of BASELINE config C4 (a fp16 / bf16
  * tensor travels as DT_FLOAT); the encode half is b200tfs_tensor.src_dtype != wire_dtype.  No host involvement between the
  * launches and graph-capturable, like the uncast decode (the two-phase route - b200tfs_parse_responses +

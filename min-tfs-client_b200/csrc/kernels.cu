@@ -122,10 +122,15 @@ __device__ __forceinline__ uint32_t widen_f16(uint32_t h) {
   return f16_bits_to_f32_bits(h);
 }
 __device__ __forceinline__ uint32_t widen_bf16(uint32_t h) { return quiet_f32(h << 16); }
+// narrowing casts give what numpy's astype(float16) / ml_dtypes' astype(bfloat16) give for the float32 the reference
+// decodes, whose NaNs are quiet: float16 keeps the sign and the top ten payload bits of the quieted NaN, bfloat16 writes
+// the quiet NaN with the sign kept.  cvt.rn.{f16,bf16}.f32 alone would turn every NaN into 0x7FFF.
 __device__ __forceinline__ uint32_t f32_bits_to_f16_bits(uint32_t w) {
+  if ((w & 0x7FFFFFFFu) > 0x7F800000u) return ((w >> 16) & 0x8000u) | 0x7E00u | ((w >> 13) & 0x3FFu);
   return (uint32_t)__half_as_ushort(__float2half_rn(__uint_as_float(w)));
 }
 __device__ __forceinline__ uint32_t f32_bits_to_bf16_bits(uint32_t w) {
+  if ((w & 0x7FFFFFFFu) > 0x7F800000u) return ((w >> 16) & 0x8000u) | 0x7FC0u;
   return (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(__uint_as_float(w)));
 }
 

@@ -734,6 +734,55 @@ int32_t orc_write_output(const orc_parsed* P, int i, int half_mode, void* dst) {
   }
 }
 
+/* ------------------------------------------------------------------ 16-bit float conversions --- */
+/* float32 bits -> float16 (to_bf16 = 0) or bfloat16 (1) bits as `tensor_proto_to_ndarray(...).astype(...)` gives them:
+ * the float32 was read back through a C double, so a NaN is quiet before it is narrowed (numpy keeps the top ten payload
+ * bits for float16, ml_dtypes writes the canonical quiet NaN for bfloat16, sign kept by both).  Everything else rounds
+ * to nearest even: integer arithmetic only, so the reference does not share the rounding hardware it checks. */
+static uint16_t narrow_bits(uint32_t w, int to_bf16) {
+  const int mb = to_bf16 ? 7 : 10, bias = to_bf16 ? 127 : 15; /* kept mantissa bits, exponent bias */
+  const uint32_t inf = to_bf16 ? 0x7F80u : 0x7C00u;
+  const uint32_t sign = (w >> 16) & 0x8000u;
+  int e = (int)((w >> 23) & 0xFF);
+  uint32_t sig = w & 0x7FFFFFu;
+  if (e == 0xFF) {
+    if (!sig) return (uint16_t)(sign | inf);
+    w |= 0x400000u;
+    return (uint16_t)(to_bf16 ? sign | 0x7FC0u : sign | 0x7E00u | ((w >> 13) & 0x3FFu));
+  }
+  if (!e && !sig) return (uint16_t)sign;
+  /* value = sig * 2^(k - 23) with 2^23 <= sig < 2^24 */
+  int k = e - 127;
+  if (e) sig |= 0x800000u;
+  else { k = -126; while (!(sig & 0x800000u)) { sig <<= 1; --k; } }
+  /* quantum of the result: 2^(t - mb), t = k clamped to the smallest normal exponent (subnormal results) */
+  int t = k < 1 - bias ? 1 - bias : k;
+  int sh = 23 + t - k - mb; /* >= 23 - mb > 0 */
+  if (sh > 25) sh = 25;     /* sig < 2^24 <= half: rounds to zero either way */
+  uint32_t q = sig >> sh, rem = sig & ((1u << sh) - 1), half = 1u << (sh - 1);
+  if (rem > half || (rem == half && (q & 1))) ++q;
+  /* biased exponent t + bias over q's implicit bit: a carry out of the mantissa moves into the exponent, a subnormal q
+   * that rounds up to 2^mb becomes the smallest normal */
+  uint32_t mag = ((uint32_t)(t + bias - 1) << mb) + q;
+  if (mag >= inf) mag = inf;
+  return (uint16_t)(sign | mag);
+}
+
+void orc_narrow_f32(const uint32_t* src, uint16_t* dst, int64_t n, int to_bf16) {
+  for (int64_t i = 0; i < n; ++i) dst[i] = narrow_bits(src[i], to_bf16);
+}
+
+/* float16 / bfloat16 bits -> float32 bits as the reference puts them on the wire for wire_dtype DT_FLOAT (put_values) */
+void orc_widen_16(const uint16_t* src, uint32_t* dst, int64_t n, int from_bf16) {
+  for (int64_t i = 0; i < n; ++i)
+    dst[i] = through_double(from_bf16 ? (uint32_t)src[i] << 16 : half_to_float_bits(src[i]));
+}
+
+/* DT_HALF half_val integers read as values (the reference's quirk, orc_write_output with half_mode 1) */
+void orc_int_to_half(const int32_t* src, uint16_t* dst, int64_t n) {
+  for (int64_t i = 0; i < n; ++i) dst[i] = int_to_half(src[i]);
+}
+
 /* typed values present for output i (complex: pairs), whatever the shape says; -1 if the dtype has no typed field */
 int64_t orc_value_count(const orc_parsed* P, int i) { return element_count(&P->outs[i]); }
 int64_t orc_content_len(const orc_parsed* P, int i) { return (int64_t)P->outs[i].content_len; }

@@ -75,6 +75,11 @@ def lib():
         L.orc_value_count.argtypes = [C.c_void_p, C.c_int]
         L.orc_content_off.restype = C.c_int64
         L.orc_content_off.argtypes = [C.c_void_p, C.c_int]
+        for fn in (L.orc_narrow_f32, L.orc_widen_16):
+            fn.restype = None
+            fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int]
+        L.orc_int_to_half.restype = None
+        L.orc_int_to_half.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
         _lib = L
     return _lib
 
@@ -202,6 +207,38 @@ def _materialise(handle, i, d: _Desc, wire: bytes, half_mode: int, tolerant: boo
     if rc != OK:
         raise _EXC.get(rc, ValueError)(f"oracle status {rc}")
     return out
+
+
+def _is_bf16(np_dtype) -> bool:
+    name = np.dtype(np_dtype).name
+    if name not in ("float16", "bfloat16"):
+        raise ValueError(f"not a 16-bit float dtype: {name}")
+    return name == "bfloat16"
+
+
+def narrow_f32(x, np_dtype) -> np.ndarray:
+    """float32 -> float16 / bfloat16 the way ``tensor_proto_to_ndarray(...).astype(np_dtype)`` narrows a decoded
+    float32: NaNs quieted first (the reference's double trip), then round to nearest even, computed with integers."""
+    bits = np.ascontiguousarray(np.asarray(x).view(np.uint32))
+    out = np.empty(bits.shape, dtype=np.uint16)
+    lib().orc_narrow_f32(bits.ctypes.data, out.ctypes.data, bits.size, int(_is_bf16(np_dtype)))
+    return out.view(_np_dtype(_DT["bfloat16"]) if _is_bf16(np_dtype) else np.float16)
+
+
+def widen_16(x) -> np.ndarray:
+    """float16 / bfloat16 -> the float32 the reference puts on the wire for ``wire_dtype=DT_FLOAT`` (exact; NaNs quiet)."""
+    x = np.ascontiguousarray(x)
+    out = np.empty(x.shape, dtype=np.uint32)
+    lib().orc_widen_16(x.view(np.uint16).ctypes.data, out.ctypes.data, x.size, int(_is_bf16(x.dtype)))
+    return out.view(np.float32)
+
+
+def int_to_half(v) -> np.ndarray:
+    """int32 ``half_val`` values -> float16 values, round to nearest even (the reference's DT_HALF quirk)."""
+    v = np.ascontiguousarray(v, dtype=np.int32)
+    out = np.empty(v.shape, dtype=np.uint16)
+    lib().orc_int_to_half(v.ctypes.data, out.ctypes.data, v.size)
+    return out.view(np.float16)
 
 
 def _np_dtype(enum):
