@@ -340,7 +340,9 @@ int b200tfs_unpack_outputs(b200tfs_ctx* ctx, const void* arena_dev, int32_t m, c
  * framing skip the tag walk.  One corner is reported rather than decoded: a record that has exactly
  * that record's LENGTH but other framing, and whose values are spread over more 32 KB..256 KB tiles
  * than that record's, gets B200TFS_E_NONCANONICAL; decode it with the next launch (which starts
- * without a remembered framing) or with b200tfs_parse_responses + b200tfs_unpack_outputs.          */
+ * without a remembered framing) or with b200tfs_parse_responses + b200tfs_unpack_outputs.
+ * The launch stores only into [dst_off, dst_off + dst_bytes) of the B200TFS_OK fixed-width outputs of B200TFS_OK records:
+ * every other byte of every slot - all of it for a record that did not decode - keeps what the caller left there.   */
 #define B200TFS_FUSED_MAX_OUTPUTS 8
 int b200tfs_decode_responses(b200tfs_ctx* ctx, const void* arena_dev, int32_t n, const uint64_t* rec_off,
                              const uint64_t* rec_len, void* dst_dev, uint64_t dst_stride);

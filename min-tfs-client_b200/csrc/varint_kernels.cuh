@@ -635,10 +635,11 @@ __global__ void __launch_bounds__(kVarThreads) vdec_emit_kernel(const __grid_con
   VarSeg sg;
   VarJobDev jb;
   fetch_tile(tb, t, sg, jb);
-  if ((jb.flags & kVarFlagPadEdge) ? *jb.total > jb.n_elems : *jb.total != jb.n_elems) {  // element count != prod(shape): reshape() would raise
-    if (threadIdx.x == 0) *jb.status = B200TFS_E_SHAPE;
-    return;
-  }
+  // element count != prod(shape): reshape() would raise.  The tile still looks for malformed varints (nothing is stored): the
+  // runtime refuses such a message before any reshape, so B200TFS_E_PARSE must win over B200TFS_E_SHAPE (atomicMin does)
+  const bool count_ok = (jb.flags & kVarFlagPadEdge) ? *jb.total <= jb.n_elems : *jb.total == jb.n_elems;
+  if (!count_ok && threadIdx.x == 0) atomicMin(jb.status, B200TFS_E_SHAPE);
+  const uint64_t n_store = count_ok ? jb.n_elems : 0;
   const uint64_t share = prefix_share(jb, t - jb.first_tile);
   const uint8_t* lo = sg.src;
   const uint8_t* hi = sg.src + sg.n;
@@ -703,16 +704,16 @@ __global__ void __launch_bounds__(kVarThreads) vdec_emit_kernel(const __grid_con
   if (threadIdx.x == 0 && hi > G && hi <= G + kVarTileBytes && (hi[-1] & 0x80)) atomicMin(jb.status, B200TFS_E_PARSE);   // the chunk's last varint never ends
   int32_t st_local;
   switch (jb.dtype) {
-    case DT_INT64: case DT_UINT64: st_local = decode_elems<VS_U64>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-    case DT_INT32: case DT_UINT32: st_local = decode_elems<VS_U32>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-    case DT_INT16: st_local = decode_elems<VS_I16>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-    case DT_INT8: st_local = decode_elems<VS_I8>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-    case DT_UINT16: st_local = decode_elems<VS_U16>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-    case DT_UINT8: st_local = decode_elems<VS_U8>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-    case DT_BOOL: st_local = decode_elems<VS_BOOL>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
+    case DT_INT64: case DT_UINT64: st_local = decode_elems<VS_U64>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
+    case DT_INT32: case DT_UINT32: st_local = decode_elems<VS_U32>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
+    case DT_INT16: st_local = decode_elems<VS_I16>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
+    case DT_INT8: st_local = decode_elems<VS_I8>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
+    case DT_UINT16: st_local = decode_elems<VS_U16>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
+    case DT_UINT8: st_local = decode_elems<VS_U8>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
+    case DT_BOOL: st_local = decode_elems<VS_BOOL>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
     case DT_HALF: case DT_BFLOAT16:
-      st_local = (jb.flags & kVarFlagHalfAsValue) ? decode_elems<VS_HALF_VALUE>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems)
-                                                  : decode_elems<VS_HALF_BITS>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems);
+      st_local = (jb.flags & kVarFlagHalfAsValue) ? decode_elems<VS_HALF_VALUE>(smraw, start_at, n_here, jb.dst, idx0, n_store)
+                                                  : decode_elems<VS_HALF_BITS>(smraw, start_at, n_here, jb.dst, idx0, n_store);
       break;
     default: st_local = B200TFS_OK; break;
   }

@@ -425,10 +425,42 @@ B2_HD SpillEntry* spill_find(SpillArea& sp, uint32_t kind, uint32_t seq, uint32_
   return nullptr;
 }
 
+// Every varint of `count` pieces of `len` bytes, `stride` apart, ends within ten bytes (the walk has checked that each piece
+// ends on a terminator).
+B2_HD bool varint_pieces_ok(Cursor& c, const b200tfs_run& r) {
+#pragma unroll 1
+  for (uint32_t q = 0; q < r.count; ++q) {
+    uint32_t run = 0;
+#pragma unroll 1
+    for (uint32_t i = 0; i < r.len; ++i) {
+      run = (rd8(c, (uint32_t)r.off + q * r.stride + i) & 0x80) ? run + 1 : 0;
+      if (run >= 10) return false;
+    }
+  }
+  return true;
+}
+
+// Packed varints of a field the dtype does not select are dropped from the table, so no varint decode kernel ever reads them;
+// the runtime parses them all the same and refuses the whole message when one is malformed.  Check those here (they are
+// absent from the responses a server writes, so this costs nothing there).
+B2_HD bool foreign_varints_ok(Cursor& c, const b200tfs_output& o, const SpillArea& sp, const WalkAux& a, uint32_t field) {
+  const int inl = o.n_runs < B200TFS_MAX_RUNS ? o.n_runs : B200TFS_MAX_RUNS;
+  for (int i = 0; i < inl; ++i)
+    if (o.runs[i].field != field && !fixed_wire_width(o.runs[i].field) && !varint_pieces_ok(c, o.runs[i])) return false;
+  const uint32_t n = sp.used < sp.cap ? sp.used : sp.cap;
+  for (uint32_t i = 0; i < n && o.n_runs > B200TFS_MAX_RUNS; ++i) {
+    const SpillEntry& e = sp.e[i];
+    if (e.kind == SPILL_RUN && e.seq == a.seq && e.run.field != field && !fixed_wire_width(e.run.field) && !varint_pieces_ok(c, e.run))
+      return false;
+  }
+  return true;
+}
+
 // Settle dtype -> field, keep that field's runs, element counts.  Mirrors what
 // tensor_proto_to_ndarray (tensors.py:42-46) would conclude from the parsed message.
-B2_HD void finalize_output(b200tfs_output& o, SpillArea& sp, const WalkAux& a) {
+B2_HD void finalize_output(Cursor& c, b200tfs_output& o, SpillArea& sp, const WalkAux& a) {
   o.spill_seq = a.seq;
+  if (!foreign_varints_ok(c, o, sp, a, dtype_info(o.dtype).field)) { c.err = B200TFS_E_PARSE; return; }
   if (a.too_deep) { o.status = B200TFS_E_NONCANONICAL; o.n_runs = 0; o.n_inline = 0; return; }
   const DtypeInfo di = dtype_info(o.dtype);
   if (di.field == 0) { o.status = B200TFS_E_KEY; o.n_runs = 0; o.n_inline = 0; return; }  // types.py:40 KeyError
@@ -595,7 +627,8 @@ B2_HD int walk_response(Cursor& c, int max_outputs, b200tfs_output* outs, int* n
       // (incl. key/value with a mismatched wire type) stays an unknown field of the response and never
       // reaches the outputs map (pinned: tests/golden/decode.json "entry_with_foreign_field").
       if (foreign) continue;
-      finalize_output(o, sp, aux);
+      finalize_output(c, o, sp, aux);
+      if (c.err) break;
       // duplicate key: the later entry replaces the earlier one
       int slot = -1;
       for (int i = 0; i < n; ++i) if (keys_equal(c, outs[i], o)) { slot = i; break; }
@@ -628,8 +661,8 @@ B2_HD int walk_tensor_proto(Cursor& c, b200tfs_output* out, SpillArea& sp) {
   walk_tensor(c, *out, sp, aux);
   if (c.err) return c.err;
   if (sp.used > sp.cap) return B200TFS_E_SPILL;
-  finalize_output(*out, sp, aux);
-  return B200TFS_OK;
+  finalize_output(c, *out, sp, aux);
+  return c.err ? c.err : B200TFS_OK;
 }
 
 }  // namespace b200tfs

@@ -411,6 +411,9 @@ class Codec:
             raise KeyError(enum)
         np_type = numpy_for_enum(enum)
         shape = self._shape(o)
+        if (o.flags & N.OF_RANK0) and strict:
+            # reshape() with no dims raises whatever the values are, so this comes before any element-count error
+            raise TypeError("reshape() takes exactly 1 argument (0 given)")
         if strict and enum in (DT_COMPLEX64, DT_COMPLEX128) and o.n_elems:
             raise ValueError("cannot reshape array: the reference reads complex values as separate floats")
         content_only = o.n_runs == 0 and o.content_len and o.n_strings == 0
@@ -427,8 +430,6 @@ class Codec:
             raise NotImplementedError("wire layout not tabulated by the device parser")
         elif o.status != N.OK:
             N.check(o.status)
-        if (o.flags & N.OF_RANK0) and strict:
-            raise TypeError("reshape() takes exactly 1 argument (0 given)")
         dst_code = enum
         if out_dtype is not None:
             dst_code = _as_enum(out_dtype)
@@ -496,7 +497,7 @@ class Codec:
             for key, o in pr.outputs.items():
                 od = out_dtypes.get(key) if out_dtypes else None
                 if int(o.dtype) == DT_STRING and o.status == N.OK:
-                    results[i][0][key] = self._decode_strings(pr.wire, pr.offset, o)
+                    results[i][0][key] = self._decode_strings(pr.wire, pr.offset, o, pr.length, key)
                     continue
                 np_type, dst_code, shape = self._resolve_output(o, strict, od)
                 jobs.append((i, key, o, np_type, dst_code, shape))
@@ -580,7 +581,7 @@ class Codec:
                 o = outs[i * K + j]
                 key = self._text(buf, base + o.key_off, o.key_len)
                 if int(o.dtype) == DT_STRING and o.status == N.OK:
-                    arrays[key] = self._decode_strings(buf, base, o)
+                    arrays[key] = self._decode_strings(buf, base, o, len(wires[i]), key)
                     continue
                 if cast_code and ((int(o.dtype) == 1) != (key in cast_keys)):
                     return None      # the launch narrowed every float32 output: only right when exactly those were asked for
@@ -608,10 +609,16 @@ class Codec:
         return results
 
     @staticmethod
-    def _decode_strings(buf: np.ndarray, base: int, o: N.Output) -> np.ndarray:
+    def _decode_strings(buf: np.ndarray, base: int, o: N.Output, rec_len: int = 0, key: str = "") -> np.ndarray:
         from tensorflow.core.framework.tensor_pb2 import TensorProto
 
         proto = TensorProto.FromString(buf[base + o.msg_off: base + o.msg_off + o.msg_len].tobytes())
+        if rec_len and (len(proto.string_val) != o.n_strings or len(proto.tensor_shape.dim) != o.rank):
+            # the map entry carried its TensorProto in several `value` occurrences, which the runtime merges (the table counts
+            # all of them; msg_off is the last one): parse the whole response the way the runtime does
+            from tensorflow_serving.apis.predict_pb2 import PredictResponse
+
+            proto = PredictResponse.FromString(buf[base: base + rec_len].tobytes()).outputs[key]
         shape = tuple(int(d.size) for d in proto.tensor_shape.dim)     # the host message is at hand: any rank
         return np.array([e for e in proto.string_val], dtype=np.str_).reshape(*shape)
 

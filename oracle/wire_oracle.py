@@ -185,6 +185,10 @@ def _materialise(handle, i, d: _Desc, wire: bytes, half_mode: int, tolerant: boo
         if lib().orc_content_len(handle, i) == nb and nb:
             off = lib().orc_content_off(handle, i)
             return np.frombuffer(wire[off: off + nb], dtype=_np_dtype(d.dtype)).reshape(shape).copy()
+    if tolerant and status == E_SHAPE and d.dtype in _NP and lib().orc_content_len(handle, i):
+        # MakeNdarray takes tensor_content whenever it is there (tensor_util.py:565-642 in the reference's vendored tree): bytes of
+        # the wrong length do not reshape, and the typed values are never looked at (ref_port.make_ndarray_tf)
+        raise ValueError("tensor_content does not match the shape")
     if tolerant and status == E_SHAPE and d.dtype in _NP:
         # TensorFlow's MakeNdarray (tensor_util.py:631-640 in the reference's vendored tree): no values -> zeros, fewer values
         # than the shape holds -> the last one repeats ("edge" padding); more values stays an error
