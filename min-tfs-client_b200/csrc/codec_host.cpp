@@ -112,9 +112,6 @@ struct b200tfs_ctx {
   cudaEvent_t tpl_event = nullptr;   // recorded behind every eager decode launch: once it has completed, tpl_pinned is current
   bool tpl_event_pending = false;
   bool opt_no_inline = false;        // B200TFS_NO_INLINE_TEMPLATE=1: never hand the template over in the kernel parameters (experiments)
-  bool opt_flat_budget = false;      // B200TFS_FLAT_BUDGET=1: every record gets ceil(len / tile) + 8 CTAs whatever the host knows (experiments)
-  bool opt_table_dev = false;        // B200TFS_TABLE_DEV=1: the decode table goes to device memory and is fetched by b200tfs_decode_results
-  Growable fused_dev;
   uint64_t stage_shift = 0;          // *_host decode: the wire sits at stage_dev + stage_shift (placed so that the payload is 16-byte aligned)
   int32_t fused_n = 0;      // records of the last b200tfs_decode_responses
   std::vector<int32_t> pending_status;   // varint decode: which output each status word in scratch_host belongs to
@@ -248,10 +245,6 @@ int b200tfs_create(int device, b200tfs_ctx** out) {
   if (tb) c->tile_bytes_override = (uint32_t)strtoul(tb, nullptr, 10);
   const char* oi = getenv("B200TFS_NO_INLINE_TEMPLATE");
   c->opt_no_inline = oi && oi[0] == '1';
-  const char* ofb = getenv("B200TFS_FLAT_BUDGET");
-  c->opt_flat_budget = ofb && ofb[0] == '1';
-  const char* od = getenv("B200TFS_TABLE_DEV");
-  c->opt_table_dev = od && od[0] == '1';
   e = cudaEventCreateWithFlags(&c->tpl_event, cudaEventDisableTiming);
   if (e != cudaSuccess) { delete c; return fail(B200TFS_E_CUDA, "cudaEventCreate: %s", cudaGetErrorString(e)); }
   e = cudaStreamCreateWithFlags(&c->d2h_stream, cudaStreamNonBlocking);
@@ -281,7 +274,6 @@ int b200tfs_destroy(b200tfs_ctx* c) {
   if (c->tpl_dev) cudaFree(c->tpl_dev);
   if (c->tpl_pinned) cudaFreeHost(c->tpl_pinned);
   if (c->tpl_event) cudaEventDestroy(c->tpl_event);
-  if (c->fused_dev.p) cudaFree(c->fused_dev.p);
   for (Slot* g : c->graph_slots) { cudaFreeHost(g->host.p); cudaFree(g->dev.p); delete g; }
   if (c->scratch_dev.p) cudaFree(c->scratch_dev.p);
   if (c->spill_dev.p) cudaFree(c->spill_dev.p);
@@ -1357,7 +1349,7 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
   // the flat slack, 8 of the 9 CTAs of a 4 KB response and 137 of the 265 of a narrowed 16 MiB one had no tile.  Should a record
   // of that length carry OTHER framing that needs more tiles, its status says so (B200TFS_E_NONCANONICAL, b200tfs.h).
   const TplHead& kh = (host_tpl && host_tpl->in.head.valid) ? host_tpl->in.head : c->tpl_known.head;
-  const bool budget_known = kh.valid && kh.vpt == vpt && kh.cast == fp.cast && kh.dst_need <= dst_stride && !c->opt_flat_budget;
+  const bool budget_known = kh.valid && kh.vpt == vpt && kh.cast == fp.cast && kh.dst_need <= dst_stride;
   auto ctas_for = [&](uint64_t len) -> uint64_t {
     if (budget_known && len == kh.rec_len) return (uint64_t)kh.total_tiles + 2;
     return (len + tile_bytes - 1) / tile_bytes + kFusedSlackTiles;
@@ -1365,10 +1357,6 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
   // the table is written by the kernel straight into pinned host memory (unified addressing): ~1 KB
   // of posted PCIe writes per record instead of a device table plus a copy node behind every launch
   uint8_t* d = (uint8_t*)c->fused_host.p;
-  if (c->opt_table_dev) {
-    if ((rc = grow_dev(c, c->fused_dev, L.total))) return rc;
-    d = (uint8_t*)c->fused_dev.p;
-  }
   fp.outs = (b200tfs_output*)(d + L.outs); fp.n_outs = (int32_t*)(d + L.nouts);
   fp.specs = (b200tfs_model_spec*)(d + L.specs); fp.status = (int32_t*)(d + L.status);
   // lay the CTAs of a launch out: record r owns `per(len)` consecutive CTAs; small batches in the parameters, else one uploaded table
@@ -1413,7 +1401,7 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
   // and stores only where guard[r] says so, (3) the whole decode runs for the records still unguarded (none, normally: its
   // CTAs leave after one load).
   const TplInline* kt = (host_tpl && host_tpl->in.head.valid) ? &host_tpl->in : &c->tpl_known;
-  bool split = fp.cast && !sl && budget_known && kh.total_tiles > 0 && (uint64_t)n * kh.rec_len >= (4ull << 20) && !c->opt_no_inline && !c->opt_flat_budget;
+  bool split = fp.cast && !sl && budget_known && kh.total_tiles > 0 && (uint64_t)n * kh.rec_len >= (4ull << 20) && !c->opt_no_inline;
   for (int i = 0; i < n && split; ++i) split = rec_len[i] == kh.rec_len;
   if (split) {
     if ((rc = grow_dev(c, c->guard_dev, 4ull * n))) return rc;
@@ -1490,7 +1478,6 @@ int b200tfs_decode_results(b200tfs_ctx* c, int32_t n, b200tfs_output* outs, int3
   if (c->capturing) return fail(B200TFS_E_ARG, "cannot collect results during graph capture");
   if (n > c->fused_n) return fail(B200TFS_E_ARG, "only %d records were decoded", c->fused_n);
   FusedLayout L = fused_layout(c->fused_n);
-  if (c->opt_table_dev && c->fused_dev.p) CU(cudaMemcpyAsync(c->fused_host.p, c->fused_dev.p, L.total, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   const uint8_t* h = (const uint8_t*)c->fused_host.p;
   if (outs) memcpy(outs, h + L.outs, sizeof(b200tfs_output) * (uint64_t)n * kFusedMaxOutputs);

@@ -40,7 +40,7 @@ B2_HD uint64_t frame_seg_len(const FrameSeg& sg, const uint64_t* val) {
     case FS_VARINT: return varint_len(val[sg.a]);
     case FS_BE32: return 4;
     case FS_ITEM: case FS_SMALL: return sg.b;      // the host wrote the payload's length next to its index
-    default: return val[sg.b];                     // FS_VARJOB / FS_TINYVAR / FS_ANCHOR: b = the value that is its packed length
+    default: return val[sg.b];                     // FS_VARJOB / FS_TINYVAR: b = the value that is its packed length
   }
 }
 
@@ -52,7 +52,7 @@ B2_HD void frame_request_run(const FrameTables& ft, const FrameReq& rq, const Fr
     for (uint32_t k = 0; k < fv.n_terms; ++k) {
       const uint32_t ti = fv.first_term - rq.first_term + k;
       const FrameTerm t = V.terms[ti];
-      if (t.kind == FT_TOTAL || t.kind == FT_TINY || t.kind == FT_TOTALF) x += V.term_total[ti];
+      if (t.kind == FT_TOTAL || t.kind == FT_TINY) x += V.term_total[ti];
       else if (t.kind == FT_VAL) x += val[t.idx];
       else x += varint_len(val[t.idx]);
     }
@@ -66,7 +66,7 @@ B2_HD void frame_request_run(const FrameTables& ft, const FrameReq& rq, const Fr
   }
   const uint64_t total = val[rq.total_val];
   uint64_t start = rq.slot_off + pad;
-  if (rq.anchor_seg != ~0u) {     // the payload is in place already: the record starts as far in front of it as its prefix is long
+  if (rq.anchor_seg != ~0u) {     // the host fixed where the payload goes: the record starts as far in front of it as its prefix is long
     uint64_t before = 0;
     for (uint32_t k = 0; k < rq.anchor_seg; ++k) before += frame_seg_len(V.segs[k], val);
     start = rq.anchor_off - before;     // >= slot_off: the host put the anchor behind the longest prefix possible
@@ -93,7 +93,6 @@ B2_HD void frame_request_run(const FrameTables& ft, const FrameReq& rq, const Fr
       case FS_BE32: { const uint64_t m = val[sg.a]; w[0] = (uint8_t)(m >> 24); w[1] = (uint8_t)(m >> 16); w[2] = (uint8_t)(m >> 8); w[3] = (uint8_t)m; w += 4; break; }
       case FS_ITEM: ft.items[sg.a].dst = w; w += sg.b; break;
       case FS_SMALL: ft.smalls[sg.a].dst = w; w += sg.b; break;
-      case FS_ANCHOR: w += val[sg.b]; break;      // written by venc_fused_kernel
       case FS_TINYVAR: { const TinyVar t = ft.tiny[sg.a]; for (uint32_t e = 0; e < t.n; ++e) w += put_varint(w, tiny_elem(t, e)); break; }
       default: { const uint64_t L = val[sg.b]; ft.jobs[sg.a].dst = w; ft.jobs[sg.a].cap = L; w += L; break; }
     }
@@ -107,8 +106,7 @@ B2_HD void frame_request(const FrameTables& ft, uint32_t r) {
   uint64_t* tt = ft.scratch_terms + rq.first_term;
   for (uint32_t t = 0; t < rq.n_term; ++t) {
     const FrameTerm ft_t = ft.terms[rq.first_term + t];
-    tt[t] = ft_t.kind == FT_TOTAL ? (uint64_t)ft.totals[ft_t.idx] : ft_t.kind == FT_TOTALF ? (uint64_t)ft.totals_fused[ft_t.idx]
-            : ft_t.kind == FT_TINY ? tiny_total(ft.tiny[ft_t.idx]) : 0;
+    tt[t] = ft_t.kind == FT_TOTAL ? (uint64_t)ft.totals[ft_t.idx] : ft_t.kind == FT_TINY ? tiny_total(ft.tiny[ft_t.idx]) : 0;
   }
   FrameView V{ft.segs + rq.first_seg, ft.vals + rq.first_val, ft.terms + rq.first_term, tt, ft.blob + rq.first_blob, ft.scratch_vals + rq.first_val};
   frame_request_run(ft, rq, V, r);

@@ -485,16 +485,6 @@ __device__ __forceinline__ bool move_tile(const uint8_t* __restrict__ src, uint8
 }
 
 // ------------------------------------------------------------------------------------------------
-// a source alignment known only at run time (warp-uniform): which of the 8 words of two neighbouring blocks an output word starts in
-__device__ __forceinline__ uint4 shift_pair_dyn(const uint4& lo, const uint4& hi, uint32_t q, uint32_t s) {
-  switch (q) {
-    case 0: return shift_pair<0>(lo, hi, s);
-    case 1: return shift_pair<1>(lo, hi, s);
-    case 2: return shift_pair<2>(lo, hi, s);
-    default: return shift_pair<3>(lo, hi, s);
-  }
-}
-
 // one out-of-line copy of the decode-side tile move for the paths where speed is not the point (a walked record, a staged
 // tile whose geometry does not qualify): called, not inlined, so that the hot paths stay compact
 __device__ __noinline__ void move_tile_cold(const uint8_t* src, uint8_t* dst, uint64_t n_out, uint32_t op, uint32_t n_tiles, uint32_t tile,
@@ -1086,7 +1076,6 @@ __global__ void __launch_bounds__(32 * kFrameWarps) frame_requests_kernel(const 
   __syncwarp();
   for (uint32_t k = lane; k < rq.n_term; k += 32)                                            // round 3: the job totals
     if (S.terms[k].kind == FT_TOTAL) S.term_total[k] = (uint64_t)ft.totals[S.terms[k].idx];
-    else if (S.terms[k].kind == FT_TOTALF) S.term_total[k] = (uint64_t)ft.totals_fused[S.terms[k].idx];
   for (uint32_t k = 0; k < rq.n_term; ++k)                                                   // ... and the tiny inputs: one element per lane
     if (S.terms[k].kind == FT_TINY) {                                                        // (warp-uniform branch)
       const TinyVar t = ft.tiny[S.terms[k].idx];
@@ -1215,22 +1204,6 @@ cudaError_t launch_decode_fused(const FusedParams& fp, uint32_t grid, cudaStream
   return launch_pdl(decode_fused_kernel, grid, kMoveThreads, 0, stream, fp);
 }
 
-// CTAs that are resident at once on the current device (persistent kernels take their tiles by ticket); per device, computed once
-template <int Tag, typename K>     // Tag: one cache per kernel (the two users have the same function type)
-static uint32_t persistent_grid(K kernel) {
-  static uint32_t cached[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) dev = 0;
-  if (!cached[dev]) {
-    int per_sm = 0, sms = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kVarThreads, 0);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cached[dev] = (uint32_t)max(1, per_sm) * (uint32_t)max(1, sms);
-  }
-  return cached[dev];
-}
-
 cudaError_t launch_move_guarded(const uint8_t* plan_dev, uint32_t n_tiles, cudaStream_t stream) {
   if (!n_tiles) return cudaSuccess;
   return launch_pdl(move_guarded_kernel, n_tiles, kMoveThreads, 0, stream, plan_dev);
@@ -1241,19 +1214,9 @@ cudaError_t launch_venc_len(const VarTables& tb, cudaStream_t stream) {
   venc_len_kernel<<<tb.n_tiles, kVarThreads, 0, stream>>>(tb);
   return cudaGetLastError();
 }
-cudaError_t launch_venc_fused(const VarTables& tb, const VarFuse& fz, cudaStream_t stream) {
-  if (!tb.n_tiles) return cudaSuccess;
-  venc_fused_kernel<<<min(tb.n_tiles, persistent_grid<0>(venc_fused_kernel)), kVarThreads, 0, stream>>>(tb, fz);
-  return cudaGetLastError();
-}
 cudaError_t launch_venc_emit(const VarTables& tb, cudaStream_t stream) {
   if (!tb.n_tiles) return cudaSuccess;
   venc_emit_kernel<<<tb.n_tiles, kVarThreads, 0, stream>>>(tb);
-  return cudaGetLastError();
-}
-cudaError_t launch_vdec_fused(const VarTables& tb, const VarFuse& fz, cudaStream_t stream) {
-  if (!tb.n_tiles) return cudaSuccess;
-  vdec_fused_kernel<<<min(tb.n_tiles, persistent_grid<1>(vdec_fused_kernel)), kVarThreads, 0, stream>>>(tb, fz);
   return cudaGetLastError();
 }
 cudaError_t launch_vdec_count(const VarTables& tb, cudaStream_t stream) {

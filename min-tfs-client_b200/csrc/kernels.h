@@ -36,8 +36,6 @@ cudaError_t launch_fill_edge(uint8_t* dst, uint32_t elem_size, uint64_t have, co
 cudaError_t launch_frame_requests(const FrameTables& ft, cudaStream_t stream);
 cudaError_t launch_venc_len(const VarTables& tb, cudaStream_t stream);
 cudaError_t launch_venc_emit(const VarTables& tb, cudaStream_t stream);
-cudaError_t launch_vdec_fused(const VarTables& tb, const VarFuse& fz, cudaStream_t stream);   // single-pass decode: counters zeroed beforehand
-cudaError_t launch_venc_fused(const VarTables& tb, const VarFuse& fz, cudaStream_t stream);   // single-pass: counters zeroed beforehand
 cudaError_t launch_vdec_count(const VarTables& tb, cudaStream_t stream);
 cudaError_t launch_vdec_emit(const VarTables& tb, cudaStream_t stream);
 

@@ -156,8 +156,7 @@ struct VarJobDev {
   int32_t flags;
   uint32_t first_tile;
   uint32_t n_tiles;
-  uint32_t fuse_group0;  // single-pass kernels: the job's first group descriptor (VarFuse)
-  uint32_t pad;
+  uint32_t pad[2];
 };
 
 // what every varint kernel receives (by value, in the parameter space).  A single job with a single segment - one
@@ -187,8 +186,6 @@ enum FrameSegKind : uint32_t {
   FS_ITEM = 3,    // a = MoveItem index, b = its byte count: the payload lands here (dst patched)
   FS_SMALL = 4,   // a = SmallItem index, b = its byte count: likewise
   FS_VARJOB = 5,  // a = varint job index, b = value id of its packed length: the varints land here (dst and cap patched)
-  FS_ANCHOR = 7,  // a = fused varint job index, b = value id of its packed length: the payload is ALREADY in place at the record's
-                  // anchor (venc_fused_kernel wrote it before the framing kernel ran); everything before it is laid out backwards
   FS_TINYVAR = 6  // a = index into FrameTables::tiny, b = value id of its packed length: a packed-varint input of at most
                   // kTinyVarElems elements (a label, an id, a few flags) is counted AND written by the framing kernel itself -
                   // no counting kernel, no emit kernel, no counters to zero for it
@@ -196,14 +193,14 @@ enum FrameSegKind : uint32_t {
 constexpr uint32_t kTinyVarElems = 32;
 struct TinyVar { const uint8_t* src; uint32_t n, elem_size, is_signed, pad; };
 struct FrameSeg { uint32_t kind, a, b, pad; };
-enum FrameTermKind : uint32_t { FT_TOTAL = 0, FT_VAL = 1, FT_VLEN = 2, FT_TINY = 3, FT_TOTALF = 4 };   // FT_TOTALF: + totals_fused[job]   // + total[job], + value[i], + varint_len(value[i]), + packed length of tiny[idx]
+enum FrameTermKind : uint32_t { FT_TOTAL = 0, FT_VAL = 1, FT_VLEN = 2, FT_TINY = 3 };   // + total[job], + value[i], + varint_len(value[i]), + packed length of tiny[idx]
 struct FrameTerm { uint32_t kind, idx; };
 struct FrameVal { int64_t c; uint32_t first_term, n_terms; };               // evaluated in order: terms refer to earlier values only
 struct FrameReq {
   uint32_t first_seg, n_seg, first_val, n_val;
   uint32_t first_term, n_term, first_blob, n_blob;
   uint32_t align_seg;       // the payload segment that should start 128-byte aligned (index relative to first_seg), ~0u: none
-  uint32_t anchor_seg;      // ~0u, or the FS_ANCHOR segment: its first byte lies at anchor_off and the record is laid out around it
+  uint32_t anchor_seg;      // ~0u, or an FS_ITEM segment whose first byte the host fixed at anchor_off: the record is laid out around it
   uint32_t pad0;
   uint64_t anchor_off;
   uint32_t total_val;       // value id of the record's byte length (incl. a gRPC prefix)
@@ -213,21 +210,12 @@ struct FrameTables {
   const FrameReq* reqs; const FrameSeg* segs; const FrameVal* vals; const FrameTerm* terms; const uint8_t* blob;
   const unsigned long long* totals;   // packed length of every varint job (the counting kernel's result), by job index
   const TinyVar* tiny;                // FS_TINYVAR / FT_TINY
-  const unsigned long long* totals_fused;   // packed length of every single-pass job (FT_TOTALF)
   uint64_t* scratch_vals;   // one evaluated value per FrameVal
   uint64_t* scratch_terms;  // one fetched total per FrameTerm (used by the table-walking path)
   uint8_t* arena;
   MoveItem* items; SmallItem* smalls; VarJobDev* jobs;    // patched
   uint64_t* rec_off; uint64_t* rec_len; int32_t* status;  // pinned host memory: read by b200tfs_encode_results
   uint32_t n;
-};
-
-// single-pass varint encode (venc_fused_kernel): the look-back state behind VarTables.  VarJobDev::tile_val holds the per-tile
-// state (flag | count), VarJobDev::fuse_group0 the job's first group descriptor; everything is zeroed before the launch.
-struct VarFuse {
-  uint32_t* ticket;                    // tiles take their number from here
-  unsigned long long* group_state;     // per group of 32 tiles: 2-bit flag (1 = sum known, 2 = inclusive prefix known) | bytes
-  uint32_t* group_arrivals;            // tiles of the group that have published their count
 };
 
 // decode tiles of a chunk [src, src + n): aligned windows of kVarTileBytes starting at src rounded down to 16

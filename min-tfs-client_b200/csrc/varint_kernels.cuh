@@ -17,10 +17,9 @@
 //                              12-byte window (7-bit groups compressed with masks and shifts)
 //
 // There is no separate scan kernel: a tile's prefix is one coalesced read of <= 256 + n_tiles/256
-// counters.  Two single-pass decoders were tried and dropped: a decoupled look-back over per-tile states
-// (tiles start faster than a 32-wide look-back can keep up, and seven warps idle at the barrier behind it) and
-// a ticketed "wait until every predecessor has published, then one parallel read" (the wait is the slowest of
-// 255 neighbours).  The counting pass is cheap and leaves the wire in L2 for the decoder.
+// counters.  Single-pass encoders and decoders (ticketed tiles with a decoupled look-back over tile or group
+// states, or a wait for every predecessor to publish) were tried, measured slower than count + emit, and removed.
+// The counting pass is cheap and leaves the wire in L2 for the decoder.
 //
 // What the reference does here: tensors.py:22 (`.item()` per element into RepeatedScalarContainer,
 // the runtime then writes one varint at a time) and tensors.py:46 (list of Python ints -> np.array).
@@ -350,173 +349,6 @@ __global__ void __launch_bounds__(kVarThreads, 5) venc_emit_kernel(const __grid_
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// E3: ONE pass - count, place and emit in a single kernel (the deferred encode's anchored jobs: a packed-varint payload whose
-// first byte the host could fix in advance).  venc_emit recomputes every length anyway; what it lacks is where its tile's
-// bytes go, i.e. the byte count of all tiles before it.  That prefix comes from a two-level look-back instead of a counting
-// kernel (which reads the whole tensor once more):
-//   * tiles take their number from a ticket (started tiles only ever wait for tiles that started earlier);
-//   * a tile publishes its byte count as soon as its lengths are scanned; groups of kVarFuseGroup consecutive tiles: the tile
-//     whose publication completes a group sums the group and resolves the group's exclusive prefix by a decoupled look-back
-//     over GROUP descriptors (a few per microsecond - a 32-wide window always reaches a resolved group; at TILE level ~100
-//     tiles start per microsecond and round 1's tile-level look-back could not keep up), before it builds its own image;
-//   * every tile builds its image first (the expensive part) and only then reads what it needs - the previous group's
-//     inclusive prefix and the counts of the tiles before it inside its group, all long since published - so the look-back
-//     costs nothing on the critical path.  The image is built at phase 0 and realigned on the way out (two 128-bit shared
-//     loads and a funnel shift per 128-bit store), since the destination's phase is not known while building.
-// ------------------------------------------------------------------------------------------------
-constexpr uint32_t kVarFuseGroup = 32;
-constexpr uint32_t kFuseFlag = 0x80000000u;
-constexpr unsigned long long kFuseAgg = 1ull << 62, kFuseInc = 2ull << 62, kFuseMask = (1ull << 62) - 1;
-
-__device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) { uint32_t v; asm volatile("ld.volatile.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
-__device__ __forceinline__ unsigned long long ld_volatile_u64(const unsigned long long* p) {
-  unsigned long long v; asm volatile("ld.volatile.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory"); return v;
-}
-
-// --- the two-level look-back, shared by the single-pass encoder (counts = bytes) and decoder (counts = elements) -------------
-struct FuseJob {
-  uint32_t* tile_state;            // [n_tiles] flag | count
-  unsigned long long* gs;          // [n_groups] group descriptors
-  uint32_t* arrivals;              // [n_groups]
-  uint32_t n_tiles;
-};
-
-// Run by ONE warp of the CTA (all 32 lanes), the tile's bookkeeper, while the other warps do the tile's heavy work.  Lane 0
-// publishes the tile's count - one store, flag and count in the same word, so no fence and no atomic is needed anywhere in
-// this protocol (a __threadfence here would wait for the PREVIOUS tile's streaming stores of the persistent CTA).  The group's LAST tile (by ticket) resolves the group: it collects the 32 counts (all from earlier tickets, i.e. from
-// tiles that have started and publish before they wait for anything), publishes the AGG descriptor, looks back over earlier
-// groups and publishes the INC descriptor.  Returns the job's total in every lane when this warp resolved the job's LAST
-// group, else ~0ull.
-__device__ __forceinline__ unsigned long long fuse_publish_warp(const FuseJob& J, uint32_t t_rel, uint32_t count) {
-  const uint32_t lane = threadIdx.x & 31;
-  const uint32_t g_rel = t_rel / kVarFuseGroup, k_in = t_rel % kVarFuseGroup;
-  const uint32_t n_groups = (J.n_tiles + kVarFuseGroup - 1) / kVarFuseGroup;
-  const uint32_t in_group = min(kVarFuseGroup, J.n_tiles - g_rel * kVarFuseGroup);
-  if (lane == 0) asm volatile("st.volatile.global.u32 [%0], %1;" :: "l"(J.tile_state + t_rel), "r"(kFuseFlag | count) : "memory");
-  if (k_in + 1 != in_group) return ~0ull;
-  uint32_t c = 0;
-  if (lane < k_in) { uint32_t v; do { v = ld_volatile_u32(J.tile_state + g_rel * kVarFuseGroup + lane); } while (!(v & kFuseFlag)); c = v & ~kFuseFlag; }
-  if (lane == k_in) c = count;
-#pragma unroll
-  for (int d = 16; d; d >>= 1) c += __shfl_xor_sync(0xFFFFFFFFu, c, d);
-  if (lane == 0 && g_rel + 1 < n_groups)
-    asm volatile("st.volatile.global.u64 [%0], %1;" :: "l"(J.gs + g_rel), "l"(kFuseAgg | (unsigned long long)c) : "memory");
-  unsigned long long prefix = 0;
-  int32_t look = (int32_t)g_rel - 1;
-  while (look >= 0) {
-    const int32_t idx = look - (int32_t)lane;
-    unsigned long long d = kFuseInc;   // lanes before the first group contribute a resolved zero
-    if (idx >= 0) { do { d = ld_volatile_u64(J.gs + idx); } while ((d >> 62) == 0); }
-    const uint32_t inc_mask = __ballot_sync(0xFFFFFFFFu, (d >> 62) == 2);
-    const uint32_t first_inc = inc_mask ? (uint32_t)__ffs(inc_mask) - 1u : 32u;    // nearest resolved group in this window
-    unsigned long long part = (lane <= first_inc) ? (d & kFuseMask) : 0ull;
-#pragma unroll
-    for (int s = 16; s; s >>= 1) part += __shfl_xor_sync(0xFFFFFFFFu, part, s);
-    prefix += part;
-    if (inc_mask) break;
-    look -= 32;
-  }
-  if (lane == 0) asm volatile("st.volatile.global.u64 [%0], %1;" :: "l"(J.gs + g_rel), "l"(kFuseInc | (prefix + c)) : "memory");
-  return (g_rel + 1 == n_groups) ? prefix + c : ~0ull;
-}
-
-// The counts of all tiles before t_rel = the previous group's inclusive prefix + the tiles before it inside its group, in two
-// steps so that the loads' round trip is spent under the tile's own work: fuse_prefix_issue right after the publication,
-// fuse_prefix_complete when the prefix is needed (it re-reads only what was not there yet).  Bookkeeper warp, all lanes.
-struct FusePending { unsigned long long d; uint32_t v; };
-__device__ __forceinline__ FusePending fuse_prefix_issue(const FuseJob& J, uint32_t t_rel) {
-  const uint32_t lane = threadIdx.x & 31, g_rel = t_rel / kVarFuseGroup, k_in = t_rel % kVarFuseGroup;
-  FusePending p{kFuseInc, kFuseFlag};
-  if (g_rel > 0 && lane == 0) p.d = ld_volatile_u64(J.gs + g_rel - 1);
-  if (lane < k_in) p.v = ld_volatile_u32(J.tile_state + g_rel * kVarFuseGroup + lane);
-  return p;
-}
-__device__ __forceinline__ unsigned long long fuse_prefix_complete(const FuseJob& J, uint32_t t_rel, FusePending p) {
-  const uint32_t lane = threadIdx.x & 31, g_rel = t_rel / kVarFuseGroup;
-  while ((p.d >> 62) != 2) p.d = ld_volatile_u64(J.gs + g_rel - 1);                               // lane 0 only can fail this
-  while (!(p.v & kFuseFlag)) p.v = ld_volatile_u32(J.tile_state + g_rel * kVarFuseGroup + lane);   // lanes < k_in only
-  uint32_t c = p.v & ~kFuseFlag;
-#pragma unroll
-  for (int d = 16; d; d >>= 1) c += __shfl_xor_sync(0xFFFFFFFFu, c, d);
-  const unsigned long long before = __shfl_sync(0xFFFFFFFFu, p.d & kFuseMask, 0);
-  return before + c;
-}
-
-// Persistent CTAs: each takes tiles by ticket until none are left (the next ticket is fetched while the current tile is being
-// worked on).  The LAST warp is the tile's bookkeeper: while the other seven build their part of the image it publishes the
-// count, resolves the group if need be and fetches the tile's prefix - three dependent L2 round trips that, done by the whole
-// CTA behind barriers (the first version: low issue activity, many barrier stalls), cost more than the
-// counting kernel they replace - and then builds its own 256 elements.
-__global__ void __launch_bounds__(kVarThreads, 5) venc_fused_kernel(const __grid_constant__ VarTables tb, const __grid_constant__ VarFuse fz) {
-  __shared__ __align__(16) uint8_t smem[kVarImageBytes + 16];
-  __shared__ VarShared sh;
-  __shared__ uint32_t s_ticket, s_next;
-  __shared__ unsigned long long s_base;
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr uint32_t kKeeper = kVarThreads / 32 - 1;
-  if (threadIdx.x == 0) s_ticket = atomicAdd(fz.ticket, 1u);
-  __syncthreads();
-  for (;;) {
-    const uint32_t t = s_ticket;
-    if (t >= tb.n_tiles) break;
-    VarSeg sg;
-    VarJobDev jb;
-    fetch_tile(tb, t, sg, jb);
-    const uint32_t t_rel = t - jb.first_tile;
-    const uint64_t e0 = (uint64_t)(t - sg.first_tile) * kVarTileElems;
-    const uint32_t cnt = (uint32_t)min((uint64_t)kVarTileElems, sg.n - e0);
-    const FuseJob J{jb.tile_val, fz.group_state + jb.fuse_group0, fz.group_arrivals + jb.fuse_group0, jb.n_tiles};
-    uint64_t mine[kVarPerThread];
-    uint32_t lens;
-    const uint32_t sum = venc_load_tile(smem, sg, jb, e0, cnt, mine, lens);
-    uint32_t total;
-    uint64_t unused;
-    const uint32_t off = block_scan_sum(sum, &total, 0ull, &unused, sh);
-    FusePending pend{};
-    uint32_t nxt = 0;
-    if (warp == kKeeper) {
-      if (lane == 0) nxt = atomicAdd(fz.ticket, 1u);                      // the next tile's ticket: in flight while we work
-      const unsigned long long job_total = fuse_publish_warp(J, t_rel, total);
-      if (lane == 0 && job_total != ~0ull) *jb.total = job_total;         // the packed length: read by the framing kernel behind us
-      pend = fuse_prefix_issue(J, t_rel);
-    }
-    venc_build_image(smem + 16, mine, lens, off);      // image at smem[16 ..): block -1 stays free for the realigning copy below
-    if (warp == kKeeper) {
-      const unsigned long long b = fuse_prefix_complete(J, t_rel, pend);
-      if (lane == 0) { s_base = b; s_next = nxt; }
-    }
-    __syncthreads();
-    const uint64_t base = s_base;
-    if (base < jb.cap) {
-      const uint32_t n_out = (uint32_t)min((uint64_t)total, jb.cap - base);
-      // image bytes [0, n_out) at smem + 16  ->  g[0, n_out), g = jb.dst + base of any alignment
-      uint8_t* g = jb.dst + base;
-      const uint32_t ph = (uint32_t)((uintptr_t)g & 15);
-      uint8_t* gbase = g - ph;                          // 16-byte aligned; destination vector v covers image bytes [16v - ph, 16v - ph + 16)
-      const uint32_t lo = ph, hi = ph + n_out;
-      const uint32_t v_lo = (lo + 15) >> 4, v_hi = hi >> 4;
-      const uint8_t* img = smem + 16;
-      if (v_lo < v_hi) {
-        const uint32_t k = (16 - ph) & 15;              // image offset of vector v inside its 16-byte block
-        for (uint32_t v = v_lo + threadIdx.x; v < v_hi; v += kVarThreads) {
-          const uint4* blk = reinterpret_cast<const uint4*>(img + 16 * v - ph - k);    // block holding the vector's first byte (16-aligned)
-          uint4 o = blk[0];
-          if (k) o = shift_pair_dyn(blk[0], blk[1], k >> 2, (k & 3) * 8);
-          st_stream(gbase + 16 * v, o);
-        }
-        for (uint32_t i = lo + threadIdx.x; i < v_lo * 16; i += kVarThreads) gbase[i] = img[i - ph];
-        for (uint32_t i = v_hi * 16 + threadIdx.x; i < hi; i += kVarThreads) gbase[i] = img[i - ph];
-      } else {
-        for (uint32_t i = lo + threadIdx.x; i < hi; i += kVarThreads) gbase[i] = img[i - ph];
-      }
-    }
-    __syncthreads();                                   // the image and s_base are free again
-    if (threadIdx.x == 0) s_ticket = s_next;
-    __syncthreads();
-  }
-}
-
 // D1: varint terminators (bytes with the top bit clear) per decode tile.  One WARP per tile: sixteen
 // aligned 128-bit loads per lane in two batches of eight, a warp reduction, no block barrier.
 __global__ void __launch_bounds__(kVarThreads, 5) vdec_count_kernel(const __grid_constant__ VarTables tb) {
@@ -718,125 +550,4 @@ __global__ void __launch_bounds__(kVarThreads) vdec_emit_kernel(const __grid_con
     default: st_local = B200TFS_OK; break;
   }
   if (st_local != B200TFS_OK) atomicMin(jb.status, st_local);
-}
-
-// D3: ONE pass decode - the terminator counts that place a tile's elements in the tensor come from the same two-level look-back
-// as the encoder's byte counts (fuse_publish_warp / fuse_prefix_warp) instead of a counting kernel that read the wire once more.
-// Persistent CTAs take tiles by ticket; the last warp keeps the books (publish, resolve, prefix) while the others compact the
-// tile's varint starts.  The element-count check (reshape() would raise) moves to the end: the tile that resolves the job's last
-// group knows the total; elements beyond the tensor are never written either way (n_store).
-__global__ void __launch_bounds__(kVarThreads) vdec_fused_kernel(const __grid_constant__ VarTables tb, const __grid_constant__ VarFuse fz) {
-  constexpr uint32_t kBlocks = kVarTileBytes / 16;             // 512: two per thread
-  constexpr uint32_t kKeeper = kVarThreads / 32 - 1;
-  __shared__ __align__(16) uint8_t smraw[16 + kVarTileBytes + 16];
-  __shared__ uint16_t start_at[kVarTileBytes];
-  __shared__ VarShared sh;
-  __shared__ uint32_t s_ticket, s_next;
-  __shared__ unsigned long long s_base;
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) s_ticket = atomicAdd(fz.ticket, 1u);
-  __syncthreads();
-  for (;;) {
-    const uint32_t t = s_ticket;
-    if (t >= tb.n_tiles) break;
-    VarSeg sg;
-    VarJobDev jb;
-    fetch_tile(tb, t, sg, jb);
-    const uint32_t t_rel = t - jb.first_tile;
-    const FuseJob J{jb.tile_val, fz.group_state + jb.fuse_group0, fz.group_arrivals + jb.fuse_group0, jb.n_tiles};
-    const uint8_t* lo = sg.src;
-    const uint8_t* hi = sg.src + sg.n;
-    const uint8_t* G = reinterpret_cast<const uint8_t*>((uintptr_t)sg.src & ~(uintptr_t)15) + (uint64_t)(t - sg.first_tile) * kVarTileBytes;
-    auto stage = [&](int32_t k) {
-      const uint8_t* p = G + 16 * (int64_t)k;
-      uint8_t* s = smraw + 16 * (k + 1);
-      if (p >= lo && p + 16 <= hi) *reinterpret_cast<uint4*>(s) = ld_stream(p);
-      else {
-        uint4 z = make_uint4(0u, 0u, 0u, 0u);
-        *reinterpret_cast<uint4*>(s) = z;
-        if (p + 16 > lo && p < hi)
-          for (int i = 0; i < 16; ++i) if (p + i >= lo && p + i < hi) s[i] = p[i];
-      }
-    };
-    stage((int32_t)threadIdx.x);
-    stage((int32_t)(threadIdx.x + kVarThreads));
-    if (threadIdx.x < 2) stage(threadIdx.x == 0 ? -1 : (int32_t)kBlocks);
-    __syncthreads();
-    // Phase 1 - starts and terminators of this thread's two blocks (bit tricks on one 128-bit shared load each)
-    uint32_t startm[2], terms = 0;
-#pragma unroll
-    for (uint32_t r = 0; r < 2; ++r) {
-      const uint32_t k = threadIdx.x + r * kVarThreads;
-      const uint8_t* s = smraw + 16 * (k + 1);
-      const uint4 w = *reinterpret_cast<const uint4*>(s);
-      auto msb4 = [](uint32_t x) { return (((x >> 7) & 0x01010101u) * 0x01020408u) >> 24; };   // 4 top bits -> nibble
-      const uint32_t cont = msb4(w.x) | (msb4(w.y) << 4) | (msb4(w.z) << 8) | (msb4(w.w) << 12);
-      const uint32_t prev_term = (s[-1] & 0x80) ? 0u : 1u;
-      uint32_t st = (((~cont) << 1) | prev_term) & 0xFFFFu;
-      uint32_t inside = 0xFFFFu;
-      const uint8_t* p = G + 16 * k;
-      if (!(p >= lo && p + 16 <= hi)) {              // block straddles an end of the chunk: positions inside it only
-        const int64_t first = max((int64_t)0, min((int64_t)16, (int64_t)(lo - p))), last = max((int64_t)0, min((int64_t)16, (int64_t)(hi - p)));
-        inside = ((1u << last) - 1u) & ~((1u << first) - 1u);
-      }
-      startm[r] = st & inside;
-      terms += __popc(~cont & inside);
-    }
-    // Phase 2 - rank the starts in position order (second-round blocks lie after every first-round block); the same scan adds
-    // up the tile's terminators
-    const uint32_t packed = __popc(startm[0]) | (__popc(startm[1]) << 16);
-    uint32_t packed_total;
-    uint64_t tile_terms;
-    const uint32_t rank = block_scan_sum(packed, &packed_total, (uint64_t)terms, &tile_terms, sh);
-    const uint32_t first_total = packed_total & 0xFFFFu, n_here = first_total + (packed_total >> 16);
-    FusePending pend{};
-    uint32_t nxt = 0;
-    if (warp == kKeeper) {
-      if (lane == 0) nxt = atomicAdd(fz.ticket, 1u);
-      const unsigned long long job_total = fuse_publish_warp(J, t_rel, (uint32_t)tile_terms);
-      if (lane == 0 && job_total != ~0ull) {
-        *jb.total = job_total;
-        if ((jb.flags & kVarFlagPadEdge) ? job_total > jb.n_elems : job_total != jb.n_elems) atomicMin(jb.status, B200TFS_E_SHAPE);   // reshape() would raise
-      }
-      pend = fuse_prefix_issue(J, t_rel);
-    }
-#pragma unroll
-    for (uint32_t r = 0; r < 2; ++r) {
-      uint32_t starts = startm[r], at = (r == 0) ? (rank & 0xFFFFu) : first_total + (rank >> 16);
-      const uint32_t at0 = 16 * (threadIdx.x + r * kVarThreads + 1);
-      while (starts) {
-        const uint32_t i = __ffs(starts) - 1;
-        starts &= starts - 1;
-        start_at[at++] = (uint16_t)(at0 + i);
-      }
-    }
-    if (warp == kKeeper) {
-      const unsigned long long b = fuse_prefix_complete(J, t_rel, pend);
-      if (lane == 0) { s_base = b; s_next = nxt; }
-    }
-    __syncthreads();
-    // Phase 3 - the index of an element in the tensor is the number of terminators before it (+1 when a varint straddles in
-    // from the previous tile: it precedes ours but its terminator is here)
-    const uint64_t idx0 = s_base + (smraw[15] >> 7);
-    if (threadIdx.x == 0 && hi > G && hi <= G + kVarTileBytes && (hi[-1] & 0x80)) atomicMin(jb.status, B200TFS_E_PARSE);   // the chunk's last varint never ends
-    int32_t st_local;
-    switch (jb.dtype) {
-      case DT_INT64: case DT_UINT64: st_local = decode_elems<VS_U64>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-      case DT_INT32: case DT_UINT32: st_local = decode_elems<VS_U32>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-      case DT_INT16: st_local = decode_elems<VS_I16>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-      case DT_INT8: st_local = decode_elems<VS_I8>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-      case DT_UINT16: st_local = decode_elems<VS_U16>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-      case DT_UINT8: st_local = decode_elems<VS_U8>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-      case DT_BOOL: st_local = decode_elems<VS_BOOL>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems); break;
-      case DT_HALF: case DT_BFLOAT16:
-        st_local = (jb.flags & kVarFlagHalfAsValue) ? decode_elems<VS_HALF_VALUE>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems)
-                                                    : decode_elems<VS_HALF_BITS>(smraw, start_at, n_here, jb.dst, idx0, jb.n_elems);
-        break;
-      default: st_local = B200TFS_OK; break;
-    }
-    if (st_local != B200TFS_OK) atomicMin(jb.status, st_local);
-    __syncthreads();                                   // the tile's shared memory and s_base are free again
-    if (threadIdx.x == 0) s_ticket = s_next;
-    __syncthreads();
-  }
 }

@@ -93,9 +93,10 @@ def test_deferred_frame_matches_golden(name):
         assert any(poff[i] % 128 == 0 for i in fixed if plen[i] == top)
 
 
-def test_deferred_frame_varint_lengths_cross_the_varint_boundaries():
+def test_deferred_frame_lengths_and_layout_across_varint_boundaries():
     """The dependent varints (payload length, TensorProto length, entry length, gRPC length) each change size as the packed length
-    crosses 127 / 128, 16383 / 16384, ...: every side of those edges, against the oracle."""
+    crosses 127 / 128, 16383 / 16384, ...: every side of those edges, against the oracle, with the payloads placed as the encoder
+    places them."""
     for n in (1, 100, 127, 128, 129, 5000, 16380, 16383, 16384, 16390, 70000):
         ids = (np.arange(n, dtype=np.int64) % 100)              # one byte each: packed length == n
         x = np.arange(6, dtype=np.float32).reshape(2, 3)
@@ -105,16 +106,18 @@ def test_deferred_frame_varint_lengths_cross_the_varint_boundaries():
         assert wire == want, n
         wire5, *_ = deferred_wire("m", 7, inputs, grpc=True)
         assert wire5 == b"\x00" + len(want).to_bytes(4, "big") + want
-        # the varint input LAST on the wire and the only large one: the single-pass (anchored) layout - its payload sits at a position
-        # the host fixed in advance (128-byte aligned) and the record is laid out backwards from there
+        # the varint input LAST on the wire: the fixed-width payload in front of it starts 128-byte aligned, the varint payload
+        # ends the record
         last = [("img", x), ("z_ids", ids)]
         want = wire_oracle.encode_predict_request("m", 7, last)
         wire, off, poff, plen = deferred_wire("m", 7, last)
         assert wire == want, n
-        if n > 32:
-            assert poff[1] % 128 == 0 and off + len(want) == poff[1] + plen[1]
+        assert poff[0] % 128 == 0 and off + len(want) == poff[1] + plen[1], (n, off, poff)
         assert deferred_wire("m", 7, last, grpc=True)[0] == b"\x00" + len(want).to_bytes(4, "big") + want
-        assert deferred_wire("", None, [("only", ids)])[0] == wire_oracle.encode_predict_request("", None, [("only", ids)])
+        # a varint input alone: with no fixed-width payload, its own payload starts 128-byte aligned
+        want = wire_oracle.encode_predict_request("", None, [("only", ids)])
+        wire, off, poff, plen = deferred_wire("", None, [("only", ids)])
+        assert wire == want and poff[0] % 128 == 0 and off + len(want) == poff[0] + plen[0], (n, off, poff)
     # a request whose only inputs are empty or zero-element tensors, and one with no inputs at all
     assert deferred_wire("m", None, [("e", np.zeros((0, 3), np.int64))])[0] == wire_oracle.encode_predict_request("m", None, [("e", np.zeros((0, 3), np.int64))])
     assert deferred_wire("", 0, [])[0] == wire_oracle.encode_predict_request("", 0, [])

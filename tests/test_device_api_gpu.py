@@ -759,26 +759,30 @@ def _requests_on_device(dev, batch, grpc=False):
     return (N.Request * len(reqs))(*reqs), keep, ptrs
 
 
+def _deferred_batch(rng, scale):
+    """requests with fixed-width, tiny and large packed-varint inputs, zero-element tensors, and one request without inputs;
+    `scale` changes the values (and with them the varint lengths) but not the shapes"""
+    out = []
+    for i in range(9):
+        img = rng.standard_normal((3, 16, 16)).astype(np.float32)
+        img.reshape(-1)[:2] = np.array([0x7F800001, 0xFF800001], dtype=np.uint32).view(np.float32)
+        label = np.array([[(i * 37) % 1000 * scale]], dtype=np.int64)
+        toks = (rng.integers(0, 50000, size=(2, 40 + i)) * scale - (i % 3)).astype(np.int32)      # some negatives: ten-byte varints
+        out.append(("default", 1 if i % 2 else None, [("image", img), ("label", label), ("tokens", toks), ("mask", toks > 100),
+                                                       ("empty", np.zeros((0, 4), np.int64))]))
+    out.append(("m", 3, [("big", (rng.integers(0, 2 ** 62, size=70000, dtype=np.int64) >> rng.integers(0, 62, size=70000)))]))
+    out.append(("two", 2, [("a_ids", (rng.integers(0, 50000, size=5000) * scale).astype(np.int64)),                                 # two large varint inputs
+                           ("b_ids", (rng.integers(-9, 300, size=4097) * scale).astype(np.int16)), ("x", rng.standard_normal(9).astype(np.float32))]))
+    out.append(("", None, []))
+    return out
+
+
 def test_deferred_encode_no_host_round_trip(dev):
     """b200tfs_encode_requests_async: packed-varint inputs are measured, framed and emitted by kernels alone (count -> frame ->
     move + emit), bit-exact against the oracle; the whole call is captured in a CUDA graph and the replay re-measures: new label
     values of other varint lengths give other record lengths, again bit-exact."""
     rng = np.random.default_rng(31)
-    def batch_for(scale):
-        out = []
-        for i in range(9):
-            img = rng.standard_normal((3, 16, 16)).astype(np.float32)
-            img.reshape(-1)[:2] = np.array([0x7F800001, 0xFF800001], dtype=np.uint32).view(np.float32)
-            label = np.array([[(i * 37) % 1000 * scale]], dtype=np.int64)
-            toks = (rng.integers(0, 50000, size=(2, 40 + i)) * scale - (i % 3)).astype(np.int32)      # some negatives: ten-byte varints
-            out.append(("default", 1 if i % 2 else None, [("image", img), ("label", label), ("tokens", toks), ("mask", toks > 100),
-                                                           ("empty", np.zeros((0, 4), np.int64))]))
-        out.append(("m", 3, [("big", (rng.integers(0, 2 ** 62, size=70000, dtype=np.int64) >> rng.integers(0, 62, size=70000)))]))   # single pass
-        out.append(("two", 2, [("a_ids", (rng.integers(0, 50000, size=5000) * scale).astype(np.int64)),                                 # two large varint
-                               ("b_ids", (rng.integers(-9, 300, size=4097) * scale).astype(np.int16)), ("x", rng.standard_normal(9).astype(np.float32))]))  # inputs: two-pass
-        out.append(("", None, []))
-        return out
-    batch = batch_for(1)
+    batch = _deferred_batch(rng, 1)
     for grpc in (False, True):
         rq, keep, ptrs = _requests_on_device(dev, batch, grpc)
         n = len(batch)
@@ -807,7 +811,7 @@ def test_deferred_encode_no_host_round_trip(dev):
     N.check(dev.lib.b200tfs_encode_requests_async(dev.ctx, n, rq, arena, need.value))
     g = C.c_void_p()
     N.check(dev.lib.b200tfs_capture_end(dev.ctx, C.byref(g)))
-    batch2 = batch_for(977)
+    batch2 = _deferred_batch(rng, 977)
     k = 0
     for model, version, inputs in batch2:
         for key, a in inputs:
@@ -827,6 +831,38 @@ def test_deferred_encode_no_host_round_trip(dev):
         assert whole[off[i]: off[i] + ln[i]].tobytes() == want, i
     assert [int(x) for x in ln] != lens1            # the replay really produced other lengths
     dev.lib.b200tfs_graph_destroy(g)
+
+
+def test_deferred_frame_on_the_host_lays_records_out_like_the_device(dev):
+    """b200tfs_request_frame_deferred runs the framing code on the host, with packed lengths the caller supplies (here: numpy's).
+    For a request encoded alone by b200tfs_encode_requests_async it must give the device's rec_off / rec_len, and every
+    payload_off must point at the bytes the device wrote for that input."""
+    from test_deferred_frame_cpu import deferred_wire, payload_bytes
+    rng = np.random.default_rng(53)
+    x = np.arange(6, dtype=np.float32).reshape(2, 3)
+    batch = []
+    for n in (100, 5000, 70000):
+        ids = rng.integers(0, 2 ** 40, size=n, dtype=np.int64) >> rng.integers(0, 40, size=n)
+        batch += [("m", 7, [("img", x), ("z_ids", ids)]), ("m", 7, [("z_ids", ids)])]
+    batch.append(("two", 2, [("a_ids", rng.integers(0, 50000, size=5000).astype(np.int64)),
+                             ("b_ids", rng.integers(-9, 300, size=4097).astype(np.int16))]))
+    batch += _deferred_batch(rng, 1)
+    for model, version, inputs in batch:
+        rq, keep, ptrs = _requests_on_device(dev, [(model, version, inputs)])
+        need = C.c_uint64()
+        N.check(dev.lib.b200tfs_request_arena_size(1, rq, C.byref(need)))
+        arena = dev.malloc(need.value)
+        N.check(dev.lib.b200tfs_memset(dev.ctx, arena, 0xCD, need.value))
+        N.check(dev.lib.b200tfs_encode_requests_async(dev.ctx, 1, rq, arena, need.value))
+        off, ln = C.c_uint64(), C.c_uint64()
+        N.check(dev.lib.b200tfs_encode_results(dev.ctx, 1, C.byref(off), C.byref(ln)))
+        whole = dev.download(arena, need.value)
+        what = (model, [(k, a.dtype.name, a.shape) for k, a in inputs])
+        wire, host_off, poff, plen = deferred_wire(model, version, inputs)
+        assert (off.value, ln.value) == (host_off, len(wire)), what
+        assert whole[off.value: off.value + ln.value].tobytes() == wire, what
+        for (key, a), p, length in zip(inputs, poff, plen):
+            assert whole[p: p + length].tobytes() == payload_bytes(a), (what, key)
 
 
 def _decode_cast(dev, wires, dst_stride, cast):

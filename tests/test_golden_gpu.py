@@ -4,7 +4,6 @@ Every comparison is bit-exact: encoded wire bytes == the reference's SerializeTo
 decoded arrays == the reference's tensor_proto_to_ndarray output (or the same exception type).
 """
 import hashlib
-import os
 
 import numpy as np
 import pytest
@@ -392,17 +391,3 @@ def test_randomised_requests_and_responses_against_oracle(codec):
         assert set(got) == set(ref), it
         for key in ref:
             assert got[key].dtype == ref[key].dtype and got[key].shape == ref[key].shape and got[key].tobytes() == ref[key].tobytes(), (it, key, ref[key].dtype)
-
-
-@pytest.mark.gpu
-def test_single_pass_varint_kernels_agree(codec):
-    """The experimental single-pass kernels (B200TFS_FUSED_VARINT=1: ticketed tiles + two-level look-back instead of a counting
-    kernel) are not the default path - they measured slower - but must stay bit-exact: the varint tests again, in a process with
-    the switch on."""
-    import subprocess
-    import sys
-    env = dict(os.environ, B200TFS_FUSED_VARINT="1")
-    here = os.path.dirname(os.path.abspath(__file__))
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(here, "test_golden_gpu.py"), os.path.join(here, "test_device_api_gpu.py"),
-                        "-m", "gpu", "-q", "-x", "-k", "(varint or deferred) and not single_pass"], env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]

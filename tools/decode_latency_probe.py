@@ -23,8 +23,6 @@ print(json.dumps({k: (round(v["launch_us"], 3) if isinstance(v, dict) and "launc
 VARIANTS = [
     ("default", {}),
     ("no inline template", {"B200TFS_NO_INLINE_TEMPLATE": "1"}),
-    ("table in device memory", {"B200TFS_TABLE_DEV": "1"}),
-    ("table in device memory, no inline", {"B200TFS_TABLE_DEV": "1", "B200TFS_NO_INLINE_TEMPLATE": "1"}),
     ("16 KB tiles (272 CTAs)", {"B200TFS_TILE_BYTES": "16384"}),
     ("8 KB tiles (544 CTAs)", {"B200TFS_TILE_BYTES": "8192"}),
     ("64 KB tiles (72 CTAs)", {"B200TFS_TILE_BYTES": "65536"}),

@@ -66,7 +66,7 @@ def main():
         t_m, _ = timed(dev, lambda: N.check(lib.b200tfs_measure(dev.ctx, 1, vt)), args.reps)
         t_e, _ = timed(dev, lambda: N.check(lib.b200tfs_encode_tensor_protos(dev.ctx, 1, vt, arena, need.value, o, ln)), args.reps)
         # the deferred encode: the same tensor as the only input of a PredictRequest, packed_len unset - no host round trip; the
-        # count -> frame -> emit; B200TFS_FUSED_VARINT=1 switches to the single-pass kernel (count + place + emit)
+        # count -> frame -> emit
         vt2 = (N.Tensor * 1)(N.Tensor(data=v, src_dtype=dt, wire_dtype=dt, rank=1, flags=0, dims=vd, key=b"ids", key_len=3, packed_len=0))
         rq = (N.Request * 1)(N.Request(model_name=b"m", model_name_len=1, has_version=0, order=N.ORDER_UPB, version=0, n_inputs=1, flags=0, inputs=vt2))
         need2 = C.c_uint64()
