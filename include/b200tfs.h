@@ -90,6 +90,8 @@ extern "C" {
 #define B200TFS_OF_UNPACKED 0x80u      /* some values arrived as unpacked scalar elements (wire type 0 / 1 / 5)   */
 #define B200TFS_OF_SPILLED 0x100u      /* more dims than B200TFS_MAX_RANK and / or more value runs than B200TFS_MAX_RUNS: the rest
                                           is held by the context (b200tfs_output_dims / b200tfs_output_runs)               */
+#define B200TFS_OF_DEVICE_VARINT 0x200u /* set by b200tfs_decode_results (b200tfs_set_decode_varints): the single-launch decode
+                                           decoded this packed-varint output into its range itself; `status` is that decode's */
 #define B200TFS_OF_DIM_INFERRED 0x4u   /* one dim was -1 and was inferred from the element count                 */
 #define B200TFS_OF_HAS_UNKNOWN 0x8u    /* unknown fields were skipped inside this entry                           */
 #define B200TFS_OF_RANK0 0x10u         /* no dims: the reference raises TypeError here (reshape() with no args)   */
@@ -333,7 +335,8 @@ int b200tfs_unpack_outputs(b200tfs_ctx* ctx, const void* arena_dev, int32_t m, c
 /* Single-launch decode for the steady-state path: one kernel walks the tags AND moves the values,
  * with no host round trip.  Record i's fixed-width outputs (float_val / double_val / complex) are
  * written to dst_dev + i*dst_stride, each output 256-byte aligned in table order (b200tfs_output.dst_off);
- * outputs with varint or string values are tabulated only - finish those with b200tfs_unpack_outputs.
+ * outputs with varint or string values are tabulated only - finish those with b200tfs_unpack_outputs (or, for the
+ * varint ones, switch on b200tfs_set_decode_varints).
  * At most B200TFS_FUSED_MAX_OUTPUTS outputs per record.  Asynchronous and CUDA-graph capturable;
  * collect the table afterwards with b200tfs_decode_results (which synchronises).
  * Each launch remembers the framing of its record 0; records of the next launch that carry the same
@@ -342,7 +345,10 @@ int b200tfs_unpack_outputs(b200tfs_ctx* ctx, const void* arena_dev, int32_t m, c
  * than that record's, gets B200TFS_E_NONCANONICAL; decode it with the next launch (which starts
  * without a remembered framing) or with b200tfs_parse_responses + b200tfs_unpack_outputs.
  * The launch stores only into [dst_off, dst_off + dst_bytes) of the B200TFS_OK fixed-width outputs of B200TFS_OK records:
- * every other byte of every slot - all of it for a record that did not decode - keeps what the caller left there.   */
+ * every other byte of every slot - all of it for a record that did not decode - keeps what the caller left there.
+ * With b200tfs_set_decode_varints(ctx, 1) the packed-varint outputs get ranges of their own as well (see there); a
+ * varint output stores only inside its own range, and when its status is not B200TFS_OK that range's contents are
+ * unspecified.                                                                                                       */
 #define B200TFS_FUSED_MAX_OUTPUTS 8
 int b200tfs_decode_responses(b200tfs_ctx* ctx, const void* arena_dev, int32_t n, const uint64_t* rec_off,
                              const uint64_t* rec_len, void* dst_dev, uint64_t dst_stride);
@@ -359,6 +365,29 @@ int b200tfs_decode_responses(b200tfs_ctx* ctx, const void* arena_dev, int32_t n,
  * context has seen before runs as three launches (verify, guarded move, fallback: b200tfs_kernel_launches counts them); the
  * results and the table are the same.                                                               */
 int b200tfs_set_decode_cast(b200tfs_ctx* ctx, int32_t float_as);
+/* Decode packed-varint outputs too (int_val, int64_val, uint32_val, uint64_val, bool_val, half_val): after
+ * b200tfs_set_decode_varints(ctx, 1) every later b200tfs_decode_responses / b200tfs_decode_responses_host_async of this
+ * context also decodes them, still without the host between its launches and still graph-capturable (0 switches it off;
+ * allowed before a capture, not during one).  Layout: every B200TFS_OK varint output with n_elems > 0 gets a 256-byte aligned
+ * range [dst_off, dst_off + dst_bytes) of the record's slot, in table order together with the fixed-width outputs
+ * (dst_bytes = n_elems * element size in memory; a range that does not fit dst_stride: B200TFS_E_SIZE).  Values: what
+ * b200tfs_unpack_outputs writes with dst_dtype NULL (int_val truncated to int32, bool normalised, half_val as TF bit
+ * patterns).  b200tfs_decode_results then reports, for every output decoded this way, B200TFS_OF_DEVICE_VARINT in `flags`
+ * and in `status`: B200TFS_OK; B200TFS_E_SHAPE (value count != n_elems); B200TFS_E_PARSE (a malformed varint; wins over
+ * E_SHAPE); B200TFS_E_RANGE (a value that does not fit the dtype); B200TFS_E_NONCANONICAL (values in rows of unpacked
+ * elements: finish that output with b200tfs_unpack_outputs).  The launch appends three kernels (plan, count, emit - the
+ * two-phase route's own decoders over tables built on the device) and one status copy; b200tfs_kernel_launches counts them.
+ * b200tfs_decode_results folds those statuses in when the most recent b200tfs_decode_responses* CALL on the context ran with the
+ * switch on - like the record count it answers for, that is the last call, not the last graph replayed: replay a graph captured
+ * with the switch on after an eager call with it off, and its varint outputs read as tabulated only (their ranges are written). */
+int b200tfs_set_decode_varints(b200tfs_ctx* ctx, int32_t on);
+/* What dst_stride the single-launch decode needs for n records in HOST memory (needs no device): the records are walked and laid out
+ * as the launch lays them out (varints != 0: with b200tfs_set_decode_varints on), with no cast; *slot_bytes receives the most bytes
+ * any record's slot uses (round up to 256 for dst_stride), *n_varint_outputs (may be NULL) how many varint ranges the batch has -
+ * 0: the switch would decode nothing more.  Records that do not walk (malformed, more than B200TFS_FUSED_MAX_OUTPUTS outputs)
+ * count 0 bytes: the launch does not decode them either.                                                                   */
+int b200tfs_decode_slot_bytes(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t varints,
+                              uint64_t* slot_bytes, int32_t* n_varint_outputs);
 /* How the records of every b200tfs_decode_responses launch of this context were served so far (cumulative; synchronises):
  * by the framing template handed over in the kernel parameters (the host walked record 0 of a host-resident wire itself,
  * or adopted the previous launch's template from pinned memory while the stream was idle), by the template the previous

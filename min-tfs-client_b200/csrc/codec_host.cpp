@@ -92,6 +92,9 @@ struct b200tfs_ctx {
   bool opt_direct_out = true;          // B200TFS_DIRECT_OUT=0: always stage the output on the device and copy it back
   Growable guard_dev;                  // the narrowing batch decode's per-record verdicts (FusedParams::guard)
   uint32_t decode_cast = 0;            // b200tfs_set_decode_cast: DT_FLOAT outputs of the single-launch decode leave as DT_HALF / DT_BFLOAT16
+  uint32_t decode_varints = 0;         // b200tfs_set_decode_varints: the single-launch decode decodes packed-varint outputs too
+  bool fused_varints = false;          // ... and the last one did: b200tfs_decode_results folds the statuses vdec_plan_kernel's jobs left
+  Growable vdec_dev;                   // its device-built tables and counters (VarPlan)
   Slot slots[kSlots];
   int next_slot = 0;
   Growable scratch_dev;   // parse tables / varint tile tables
@@ -279,6 +282,7 @@ int b200tfs_destroy(b200tfs_ctx* c) {
   if (c->spill_dev.p) cudaFree(c->spill_dev.p);
   if (c->gather_dev.p) cudaFree(c->gather_dev.p);
   if (c->guard_dev.p) cudaFree(c->guard_dev.p);
+  if (c->vdec_dev.p) cudaFree(c->vdec_dev.p);
   if (c->enc_host.p) cudaFreeHost(c->enc_host.p);
   if (c->measured_dev.p) cudaFree(c->measured_dev.p);
   if (c->scratch_host.p) cudaFreeHost(c->scratch_host.p);
@@ -1239,15 +1243,33 @@ extern "C" int b200tfs_unpack_outputs(b200tfs_ctx* c, const void* arena_dev, int
 // fused single-launch decode + CUDA graph capture
 // ------------------------------------------------------------------------------------------------
 namespace {
-struct FusedLayout { uint64_t outs, nouts, specs, status, total; };
+struct FusedLayout { uint64_t outs, nouts, specs, status, vstatus, total; };
 FusedLayout fused_layout(int32_t n) {
   FusedLayout L;
   L.outs = 0;
   L.nouts = L.outs + sizeof(b200tfs_output) * (uint64_t)n * kFusedMaxOutputs;
   L.specs = (L.nouts + 4ull * n + 15) & ~15ull;
   L.status = L.specs + sizeof(b200tfs_model_spec) * (uint64_t)n;
-  L.total = (L.status + 4ull * n + 15) & ~15ull;
+  L.vstatus = (L.status + 4ull * n + 15) & ~15ull;     // b200tfs_set_decode_varints: one status word per (record, output) slot
+  L.total = (L.vstatus + 4ull * n * kFusedMaxOutputs + 15) & ~15ull;
   return L;
+}
+
+// Layout of the device tables of the varint outputs of a single-launch decode (VarPlan), for n records and tile_cap tiles
+struct VarPlanLayout { uint64_t jobs, segs, tile_seg, tile_val, group_sum, total, status, n_tiles, bytes; };
+VarPlanLayout var_plan_layout(uint64_t n, uint64_t tile_cap) {
+  const uint64_t slots = n * kFusedMaxOutputs;
+  VarPlanLayout V;
+  V.jobs = 0;
+  V.segs = V.jobs + slots * sizeof(VarJobDev);
+  V.tile_seg = (V.segs + slots * B200TFS_MAX_RUNS * sizeof(VarSeg) + 15) & ~15ull;
+  V.tile_val = (V.tile_seg + 4 * tile_cap + 15) & ~15ull;
+  V.group_sum = (V.tile_val + 4 * tile_cap + 15) & ~15ull;
+  V.total = (V.group_sum + 4 * (tile_cap / kVarGroupTiles + slots + 2) + 15) & ~15ull;
+  V.status = V.total + 8 * slots;
+  V.n_tiles = (V.status + 4 * slots + 15) & ~15ull;
+  V.bytes = V.n_tiles + 16;
+  return V;
 }
 }  // namespace
 
@@ -1273,7 +1295,8 @@ static uint32_t decode_vpt(const b200tfs_ctx* c, int32_t n, const uint64_t* rec_
 
 // Walk record 0 on the host (its bytes are in host memory) and build its template: the launch that follows then takes the
 // template path from its first CTA on.  Returns false when the record does not qualify (the kernel will walk it).
-static bool host_template(const uint8_t* rec0, uint64_t len, uint32_t vpt, uint64_t dst_stride, uint32_t serial, uint32_t cast, Template* T) {
+static bool host_template(const uint8_t* rec0, uint64_t len, uint32_t vpt, uint64_t dst_stride, uint32_t serial, uint32_t cast, uint32_t varints,
+                          Template* T) {
   T->in.head.valid = 0;
   if (!rec0 || len == 0 || len > 0x7FFFFFFFull) return false;
   b200tfs_output outs[kFusedMaxOutputs + 1];
@@ -1284,11 +1307,37 @@ static bool host_template(const uint8_t* rec0, uint64_t len, uint32_t vpt, uint6
   SpillArea sp{nullptr, 0u, 0u};
   const int st = walk_response(cur, kFusedMaxOutputs, outs, &cnt, &spec, sp);
   if (st != B200TFS_OK) return false;
-  const uint64_t used = tpl_layout_outputs(outs, cnt, dst_stride, cast);
+  const uint64_t used = tpl_layout_outputs(outs, cnt, dst_stride, cast, varints);
   for (int k = 0; k < cnt; ++k) if (outs[k].status == B200TFS_E_SIZE) return false;
   // the kernel's own check: the chunks' tiles must fit the budget the launch gives the record
-  tpl_learn(T, cur, (uint32_t)len, outs, cnt, spec, st, vpt, (used + 255) & ~255ull, serial, cast);
+  tpl_learn(T, cur, (uint32_t)len, outs, cnt, spec, st, vpt, (used + 255) & ~255ull, serial, cast, varints);
   return T->in.head.valid != 0;
+}
+
+// Slot bytes the single-launch decode lays out for host-resident records (the same walk and layout rule, with no stride limit and
+// no cast, which can only shrink a range): the most any record uses, and how many varint ranges the batch has
+int b200tfs_decode_slot_bytes(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t varints,
+                              uint64_t* slot_bytes, int32_t* n_varint_outputs) {
+  if (n < 0 || (n && (!wire_host || !rec_off || !rec_len)) || !slot_bytes) return fail(B200TFS_E_ARG, "bad arguments");
+  uint64_t most = 0;
+  int32_t nv = 0;
+  for (int i = 0; i < n; ++i) {
+    if (rec_len[i] > 0x7FFFFFFFull) continue;     // the launch rejects such a record: it gets no slot bytes
+    b200tfs_output outs[kFusedMaxOutputs + 1];
+    b200tfs_model_spec spec;
+    int cnt = 0;
+    Cursor cur;
+    cur_open_host(cur, (const uint8_t*)wire_host + rec_off[i], (uint32_t)rec_len[i]);
+    SpillArea sp{nullptr, 0u, 0u};
+    if (walk_response(cur, kFusedMaxOutputs, outs, &cnt, &spec, sp) != B200TFS_OK) continue;
+    most = std::max(most, tpl_layout_outputs(outs, cnt, ~0ull, 0u, varints ? 1u : 0u));
+    for (int k = 0; k < cnt && varints; ++k)
+      if (outs[k].status == B200TFS_OK && outs[k].n_elems && dtype_info(outs[k].dtype).kind != VK_FIXED && tpl_gets_range(1u, outs[k].dtype))
+        ++nv;
+  }
+  *slot_bytes = most;
+  if (n_varint_outputs) *n_varint_outputs = nv;
+  return B200TFS_OK;
 }
 
 // the pipelined host decode of ONE record: launch k covers tiles [tile_lo[k], tile_lo[k+1]) of the full grid (the last one also the
@@ -1307,6 +1356,13 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
   FusedLayout L = fused_layout(n);
   int rc;
   if ((rc = grow_host(c, c->fused_host, L.total))) return rc;
+  // varint outputs (b200tfs_set_decode_varints): tables sized from a bound the host knows, before anything is queued
+  uint64_t var_tile_cap = 0;
+  if (c->decode_varints) {
+    for (int i = 0; i < n; ++i) var_tile_cap += var_record_tile_bound(rec_len[i]);
+    if (var_tile_cap > 0x7FFFFFFFull) return fail(B200TFS_E_TOOBIG, "batch needs more than 2^31 varint tiles");
+    if ((rc = grow_dev(c, c->vdec_dev, var_plan_layout((uint64_t)n, var_tile_cap).bytes))) return rc;
+  }
   if (!c->tpl_dev) {
     if (c->capturing) return fail(B200TFS_E_ARG, "run b200tfs_decode_responses once before capturing it");
     CU(cudaMalloc(&c->tpl_dev, 2 * sizeof(Template) + 64));   // + the three path counters (b200tfs_decode_stats)
@@ -1324,6 +1380,7 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
   if (++c->serial == 0) c->serial = 1;
   fp.serial = c->serial;
   fp.cast = c->decode_cast;
+  fp.varints = c->decode_varints;
   fp.tpli.head.valid = 0;
   if (host_tpl && host_tpl->in.head.valid) {
     if (vpt <= kStageVecsHost) {   // the single-response / small-batch kernel takes its template from the parameters when the host has one
@@ -1341,7 +1398,8 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
     // well be busy again: the caller's own copy of the next response usually precedes this call)
     if (!c->capturing && (!c->tpl_event_pending || cudaEventQuery(c->tpl_event) == cudaSuccess)) { c->tpl_event_pending = false; adopt_pinned_template(c); }
     const TplHead& h = c->tpl_known.head;
-    if (vpt <= kStageVecsHost && !c->opt_no_inline && h.valid && h.rec_len == rec_len[0] && h.vpt == vpt && h.cast == fp.cast && h.dst_need <= dst_stride)
+    if (vpt <= kStageVecsHost && !c->opt_no_inline && h.valid && h.rec_len == rec_len[0] && h.vpt == vpt && h.cast == fp.cast &&
+        h.varints == fp.varints && h.dst_need <= dst_stride)
       fp.tpli = c->tpl_known;
   }
   // CTAs per record: a record of the length the host knows a template for gets that template's tiles + the publishing CTA + one
@@ -1349,7 +1407,7 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
   // the flat slack, 8 of the 9 CTAs of a 4 KB response and 137 of the 265 of a narrowed 16 MiB one had no tile.  Should a record
   // of that length carry OTHER framing that needs more tiles, its status says so (B200TFS_E_NONCANONICAL, b200tfs.h).
   const TplHead& kh = (host_tpl && host_tpl->in.head.valid) ? host_tpl->in.head : c->tpl_known.head;
-  const bool budget_known = kh.valid && kh.vpt == vpt && kh.cast == fp.cast && kh.dst_need <= dst_stride;
+  const bool budget_known = kh.valid && kh.vpt == vpt && kh.cast == fp.cast && kh.varints == fp.varints && kh.dst_need <= dst_stride;
   auto ctas_for = [&](uint64_t len) -> uint64_t {
     if (budget_known && len == kh.rec_len) return (uint64_t)kh.total_tiles + 2;
     return (len + tile_bytes - 1) / tile_bytes + kFusedSlackTiles;
@@ -1449,6 +1507,26 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
     CU(launch_decode_fused(fp, (uint32_t)grid, c->stream));
     c->launches += 1;
   }
+  c->fused_varints = fp.varints != 0;
+  if (fp.varints) {
+    // plan -> count -> emit over the table the launch(es) above published, then the per-output statuses to pinned memory
+    const VarPlanLayout V = var_plan_layout((uint64_t)n, var_tile_cap);
+    uint8_t* vd = (uint8_t*)c->vdec_dev.p;
+    VarPlan vp{};
+    vp.outs = fp.outs; vp.n_outs = fp.n_outs; vp.rec_status = fp.status;
+    vp.w = fp.w; vp.rec_off = fp.rec_off;
+    if (n <= kFusedInlineRecs) for (int i = 0; i < n; ++i) vp.off_inl[i] = rec_off[i];
+    vp.dst = fp.dst; vp.dst_stride = dst_stride; vp.n = (uint32_t)n; vp.tile_cap = (uint32_t)var_tile_cap;
+    vp.jobs = (VarJobDev*)(vd + V.jobs); vp.segs = (VarSeg*)(vd + V.segs); vp.tile_seg = (uint32_t*)(vd + V.tile_seg);
+    vp.tile_val = (uint32_t*)(vd + V.tile_val); vp.group_sum = (uint32_t*)(vd + V.group_sum);
+    vp.total = (unsigned long long*)(vd + V.total); vp.status = (int32_t*)(vd + V.status); vp.n_tiles = (uint32_t*)(vd + V.n_tiles);
+    CU(launch_vdec_plan(vp, c->stream));
+    VarTables tb{};
+    tb.segs = vp.segs; tb.tile_seg = vp.tile_seg; tb.jobs = vp.jobs; tb.n_tiles = vp.tile_cap; tb.n_tiles_dev = vp.n_tiles;
+    CU(launch_vdec_dev(tb, (uint32_t)c->sm_count * 4, c->stream));
+    CU(cudaMemcpyAsync((uint8_t*)c->fused_host.p + L.vstatus, vp.status, 4ull * n * kFusedMaxOutputs, cudaMemcpyDeviceToHost, c->stream));
+    c->launches += 3;
+  }
   c->fused_n = n;
   if (!c->capturing) { CU(cudaEventRecord(c->tpl_event, c->stream)); c->tpl_event_pending = true; }
   return B200TFS_OK;
@@ -1472,6 +1550,13 @@ int b200tfs_set_decode_cast(b200tfs_ctx* c, int32_t float_as) {
   return B200TFS_OK;
 }
 
+int b200tfs_set_decode_varints(b200tfs_ctx* c, int32_t on) {
+  if (!c) return fail(B200TFS_E_ARG, "ctx is NULL");
+  if (c->capturing) return fail(B200TFS_E_ARG, "cannot switch the varint decode during graph capture");
+  c->decode_varints = on ? 1u : 0u;
+  return B200TFS_OK;
+}
+
 int b200tfs_decode_results(b200tfs_ctx* c, int32_t n, b200tfs_output* outs, int32_t* n_outs, b200tfs_model_spec* specs,
                            int32_t* rec_status) {
   if (!c || n < 0) return fail(B200TFS_E_ARG, "bad arguments");
@@ -1481,6 +1566,19 @@ int b200tfs_decode_results(b200tfs_ctx* c, int32_t n, b200tfs_output* outs, int3
   CU(cudaStreamSynchronize(c->stream));
   const uint8_t* h = (const uint8_t*)c->fused_host.p;
   if (outs) memcpy(outs, h + L.outs, sizeof(b200tfs_output) * (uint64_t)n * kFusedMaxOutputs);
+  if (outs && c->fused_varints) {   // what the varint decode found, for exactly the outputs vdec_plan_kernel took
+    const int32_t* rs = (const int32_t*)(h + L.status);
+    const int32_t* no = (const int32_t*)(h + L.nouts);
+    const int32_t* vs = (const int32_t*)(h + L.vstatus);
+    for (int r = 0; r < n; ++r)
+      for (int k = 0; k < no[r] && rs[r] == B200TFS_OK && k < kFusedMaxOutputs; ++k) {
+        b200tfs_output& o = outs[(size_t)r * kFusedMaxOutputs + k];
+        const int32_t s = vs[(size_t)r * kFusedMaxOutputs + k];
+        if (s == kVarSlotIdle) continue;
+        o.status = s;
+        o.flags |= B200TFS_OF_DEVICE_VARINT;
+      }
+  }
   if (n_outs) memcpy(n_outs, h + L.nouts, 4ull * n);
   if (specs) memcpy(specs, h + L.specs, sizeof(b200tfs_model_spec) * (uint64_t)n);
   if (rec_status) memcpy(rec_status, h + L.status, 4ull * n);
@@ -1922,7 +2020,8 @@ int b200tfs_decode_responses_host_async(b200tfs_ctx* c, const void* wire_host, i
   Template T;
   uint64_t shift = 0;
   const bool have = vpt <= kStageVecsHost && !c->capturing &&
-                    host_template((const uint8_t*)wire_host + rec_off[0], rec_len[0], vpt, dst_stride, c->serial + 1 ? c->serial + 1 : 1, c->decode_cast, &T);
+                    host_template((const uint8_t*)wire_host + rec_off[0], rec_len[0], vpt, dst_stride, c->serial + 1 ? c->serial + 1 : 1, c->decode_cast,
+                                  c->decode_varints, &T);
   if (have) {
     uint32_t big = 0;
     for (uint32_t q = 1; q < T.in.head.n_chunks; ++q) if (T.in.chunk[q].len > T.in.chunk[big].len) big = q;

@@ -21,7 +21,8 @@
 //   frame_requests_kernel  deferred framing (frame.h): one warp per request evaluates the request's framing program from the
 //                      device-side totals, writes every header byte, patches the destinations of the movers behind it.
 //   venc_* / vdec_*    packed-varint encode and decode (int_val / int64_val / uint32_val / uint64_val /
-//                      half_val / bool_val): varint_kernels.cuh.
+//                      half_val / bool_val): varint_kernels.cuh.  vdec_plan_kernel + vdec_{count,emit}_dev_kernel decode the
+//                      varint outputs of a single-launch decode from tables built on the device (b200tfs_set_decode_varints).
 //
 // What the reference does at these points: tensors.py:22 (per-element .item() loop feeding
 // RepeatedScalarContainer.extend), prediction_service_pb2_grpc.py:52-53 (SerializeToString /
@@ -787,7 +788,7 @@ __device__ __noinline__ void fused_slow_path(const FusedParams& fp, uint32_t r, 
     uint64_t cursor = 0;   // bytes used in this record's destination slot
     uint32_t t_base = 0;   // tiles consumed by earlier chunks
     if (st == B200TFS_OK) {
-      cursor = tpl_layout_outputs(outs_s, cnt, fp.dst_stride, fp.cast);
+      cursor = tpl_layout_outputs(outs_s, cnt, fp.dst_stride, fp.cast, fp.varints);
       // tiles are handed out by ascending wire offset of the chunk (same order the template uses)
       uint32_t done_mask[kFusedMaxOutputs] = {0};
       for (;;) {
@@ -823,7 +824,8 @@ __device__ __noinline__ void fused_slow_path(const FusedParams& fp, uint32_t r, 
       fp.specs[r] = spec_s;
       for (int k = 0; k < cnt && st == B200TFS_OK; ++k) fp.outs[(size_t)r * kFusedMaxOutputs + k] = outs_s[k];
       if (r == 0) {   // leave the template for the next launch, and its inline part in pinned memory for the host
-        if (len <= 0x7FFFFFFFull) tpl_learn(fp.tpl_write, c, (uint32_t)len, outs_s, cnt, spec_s, st, fp.vpt, (cursor + 255) & ~255ull, fp.serial, fp.cast);
+        if (len <= 0x7FFFFFFFull) tpl_learn(fp.tpl_write, c, (uint32_t)len, outs_s, cnt, spec_s, st, fp.vpt, (cursor + 255) & ~255ull, fp.serial, fp.cast,
+                                            fp.varints);
         else fp.tpl_write->in.head.valid = 0;
         if (fp.tpl_pinned) {   // valid or not, stamped with this launch's serial: the host drops what it knew before either way
           fp.tpl_pinned->head.valid = 0;
@@ -912,7 +914,7 @@ __device__ __forceinline__ void decode_fused_body(const FusedParams& fp) {
     }
     __syncthreads();
     const uint32_t nch = th_s.n_chunks;
-    if (th_s.valid && th_s.rec_len == len && th_s.vpt == fp.vpt && th_s.cast == fp.cast && th_s.dst_need <= fp.dst_stride &&
+    if (th_s.valid && th_s.rec_len == len && th_s.vpt == fp.vpt && th_s.cast == fp.cast && th_s.varints == fp.varints && th_s.dst_need <= fp.dst_stride &&
         (th_s.total_tiles < budget || (CAST && fp.mode == 1))) {
       // The verdict: do this record's framing bytes equal the template's (and do packed-varint chunks still end on a terminator)?
       // It needs the record's framing bytes - a DRAM round trip.  The batch kernel decides per CTA (one byte per thread, one
@@ -1228,6 +1230,18 @@ cudaError_t launch_vdec_count(const VarTables& tb, cudaStream_t stream) {
 cudaError_t launch_vdec_emit(const VarTables& tb, cudaStream_t stream) {
   if (!tb.n_tiles) return cudaSuccess;
   vdec_emit_kernel<<<tb.n_tiles, kVarThreads, 0, stream>>>(tb);
+  return cudaGetLastError();
+}
+cudaError_t launch_vdec_plan(const VarPlan& vp, cudaStream_t stream) {
+  vdec_plan_kernel<<<1, kVarPlanThreads, 0, stream>>>(vp);
+  return cudaGetLastError();
+}
+cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t stream) {
+  const uint32_t per = kVarThreads / 32;
+  vdec_count_dev_kernel<<<std::max(1u, std::min((tb.n_tiles + per - 1) / per, max_ctas)), kVarThreads, 0, stream>>>(tb);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  vdec_emit_dev_kernel<<<std::max(1u, std::min(tb.n_tiles, max_ctas)), kVarThreads, 0, stream>>>(tb);
   return cudaGetLastError();
 }
 

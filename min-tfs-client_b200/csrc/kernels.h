@@ -38,5 +38,9 @@ cudaError_t launch_venc_len(const VarTables& tb, cudaStream_t stream);
 cudaError_t launch_venc_emit(const VarTables& tb, cudaStream_t stream);
 cudaError_t launch_vdec_count(const VarTables& tb, cudaStream_t stream);
 cudaError_t launch_vdec_emit(const VarTables& tb, cudaStream_t stream);
+// packed-varint outputs of the single-launch decode: the plan kernel, then count + emit over the tables it built (tb.n_tiles is
+// the host's bound, tb.n_tiles_dev the real count; each kernel runs at most max_ctas CTAs and strides over the tiles)
+cudaError_t launch_vdec_plan(const VarPlan& vp, cudaStream_t stream);
+cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t stream);
 
 }  // namespace b200tfs

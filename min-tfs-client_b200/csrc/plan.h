@@ -79,6 +79,7 @@ struct TplHead {
   uint32_t vpt, total_tiles;
   uint32_t serial, cast;       // serial: which learning produced it (the table entries below belong to exactly this serial);
                                // cast: the float narrowing it was laid out for (0 / DT_HALF / DT_BFLOAT16: FusedParams::cast)
+  uint32_t varints, pad;       // varints: laid out with ranges for the packed-varint outputs (FusedParams::varints)
 };
 // the part of a template every CTA needs before it can start on its tile: small enough to ride in the kernel parameters
 // (no load at all ahead of the tile's loads) when the host knows it - because it walked record 0 itself (host-buffer entry
@@ -121,6 +122,8 @@ struct FusedParams {
   uint32_t tile_bias;        // a SLICE of a one-record launch (the pipelined host path): CTA b works as CTA b + tile_bias of the full grid
   uint32_t trusted;          // != 0: the host built the inline template from THIS record's own bytes: no verdict (a slice's launch runs
                              // before the record's tail - and with it part of the framing - has arrived on the device)
+  uint32_t varints;          // != 0: packed-varint outputs get ranges of the slot too (b200tfs_set_decode_varints; vdec_plan_kernel fills them)
+  uint32_t pad;
   FusedInline inl;
   TplInline tpli;            // head.valid != 0: the template as the host knows it (tier 1; tpl_read is tier 2, the walk tier 3)
 };
@@ -169,7 +172,37 @@ struct VarTables {
   uint32_t single;      // 1: seg0 / job0 below describe every tile
   VarSeg seg0;
   VarJobDev job0;
+  const uint32_t* n_tiles_dev;   // vdec_*_dev_kernel: the tile count vdec_plan_kernel left in device memory (n_tiles is then a bound)
 };
+
+// ---- packed-varint outputs of the single-launch decode (b200tfs_set_decode_varints) ----------------------------------
+// vdec_plan_kernel reads the table the fused launch published and builds the decode tables on the device: output k of
+// record r is job r * kFusedMaxOutputs + k and owns segments [job * B200TFS_MAX_RUNS, + n_runs) - fixed slots, so the
+// plan needs no atomics and the host needs no copy of the table.  Every tile table is sized by the host from a bound it knows.
+constexpr uint32_t kVarPlanThreads = 1024;
+constexpr int32_t kVarSlotIdle = 1;       // status word of a slot the plan did not take (not a packed-varint output to decode)
+struct VarPlan {
+  const b200tfs_output* outs;      // the fused launch's table (pinned host memory, written by that launch)
+  const int32_t* n_outs;
+  const int32_t* rec_status;
+  const uint8_t* w;                // wire arena
+  const uint64_t* rec_off;         // n > kFusedInlineRecs: device copy; else off_inl
+  uint64_t off_inl[kFusedInlineRecs];
+  uint8_t* dst;
+  uint64_t dst_stride;
+  uint32_t n, tile_cap;
+  VarJobDev* jobs;                 // [n * kFusedMaxOutputs]
+  VarSeg* segs;                    // [n * kFusedMaxOutputs * B200TFS_MAX_RUNS]
+  uint32_t* tile_seg;              // [tile_cap]
+  uint32_t* tile_val;              // [tile_cap]
+  uint32_t* group_sum;             // [tile_cap / kVarGroupTiles + n * kFusedMaxOutputs]
+  unsigned long long* total;       // [n * kFusedMaxOutputs]
+  int32_t* status;                 // [n * kFusedMaxOutputs]
+  uint32_t* n_tiles;               // [1]
+};
+// tiles a record of `len` bytes can need: each of its <= kFusedMaxOutputs * B200TFS_MAX_RUNS chunks of L bytes spans at most
+// ceil((L + 15) / kVarTileBytes) windows, and the chunks lie inside the record
+constexpr uint64_t var_record_tile_bound(uint64_t len) { return len / kVarTileBytes + 2 + 2ull * kFusedMaxOutputs * B200TFS_MAX_RUNS; }
 
 // ---- deferred framing: the length prefixes of packed-varint inputs computed ON THE DEVICE -----------------------------
 // Every length on the wire precedes its content, and a packed-varint payload's length is only known once the counting

@@ -20,19 +20,24 @@ B2_HD uint32_t tpl_tiles_for(uint64_t n_out, uint32_t vpt) {
 }
 
 // Destination layout of a walked record: every fixed-width output that decoded cleanly gets a 256-byte aligned range of
-// the record's slot, in table order.  Returns the bytes of the slot in use.  (Varint / string outputs are tabulated only.)
+// the record's slot, in table order.  Returns the bytes of the slot in use.  (String outputs are tabulated only; so are
+// varint outputs unless `varints` != 0 - b200tfs_set_decode_varints - which gives them ranges in the same order.)
 // `cast` != 0: DT_FLOAT outputs leave as DT_HALF / DT_BFLOAT16 (two bytes per element; dst_bytes says so, dtype stays the wire's).
 B2_HD bool tpl_narrows(uint32_t cast, int32_t dtype) { return cast != 0 && dtype == DT_FLOAT; }
 B2_HD uint32_t tpl_move_op(uint32_t cast, int32_t dtype) {
   if (dtype != DT_FLOAT) return OP_COPY;
   return cast == (uint32_t)DT_HALF ? OP_F2H : cast == (uint32_t)DT_BFLOAT16 ? OP_F2B : OP_QUIET_DST;
 }
-B2_HD uint64_t tpl_layout_outputs(b200tfs_output* outs, int cnt, uint64_t dst_stride, uint32_t cast = 0) {
+B2_HD bool tpl_gets_range(uint32_t varints, int32_t dtype) {
+  const uint32_t kind = dtype_info(dtype).kind;
+  return kind == VK_FIXED || (varints && (kind == VK_VARINT || kind == VK_BOOL));
+}
+B2_HD uint64_t tpl_layout_outputs(b200tfs_output* outs, int cnt, uint64_t dst_stride, uint32_t cast = 0, uint32_t varints = 0) {
   uint64_t cursor = 0;
   for (int k = 0; k < cnt; ++k) {
     b200tfs_output& o = outs[k];
     if (o.status != B200TFS_OK || !o.n_elems) continue;
-    if (dtype_info(o.dtype).kind != VK_FIXED) continue;
+    if (!tpl_gets_range(varints, o.dtype)) continue;
     if (tpl_narrows(cast, o.dtype)) o.dst_bytes = o.n_elems * 2;
     cursor = (cursor + 255) & ~255ull;
     if (cursor + o.dst_bytes > dst_stride) { o.status = B200TFS_E_SIZE; continue; }
@@ -45,7 +50,7 @@ B2_HD uint64_t tpl_layout_outputs(b200tfs_output* outs, int cnt, uint64_t dst_st
 // Build the template of a walked record (chunks sorted by wire offset, framing bytes).  T->in.head.valid stays 0 when the
 // record does not qualify.  `c` is the cursor the record was walked with (its bytes are read through rd8).
 B2_HD void tpl_learn(Template* T, Cursor& c, uint32_t len, const b200tfs_output* outs, int cnt, const b200tfs_model_spec& spec,
-                     int st, uint32_t vpt, uint64_t dst_need, uint32_t serial, uint32_t cast = 0) {
+                     int st, uint32_t vpt, uint64_t dst_need, uint32_t serial, uint32_t cast = 0, uint32_t varints = 0) {
   T->in.head.valid = 0;
   if (st != B200TFS_OK || cnt > kFusedMaxOutputs) return;
   TplChunk ch[kTplChunks];
@@ -107,7 +112,7 @@ B2_HD void tpl_learn(Template* T, Cursor& c, uint32_t len, const b200tfs_output*
   }
   TplHead& h = T->in.head;
   h.n_chunks = n; h.n_outs = (uint32_t)cnt; h.framing_len = framing; h.rec_len = len; h.vpt = vpt; h.total_tiles = tiles;
-  h.dst_need = dst_need; h.serial = serial; h.cast = cast;
+  h.dst_need = dst_need; h.serial = serial; h.cast = cast; h.varints = varints; h.pad = 0;
   T->spec = spec;
   for (int k = 0; k < cnt; ++k) T->outs[k] = outs[k];
   h.valid = 1;   // device callers fence before publishing the structure to other CTAs / launches

@@ -351,9 +351,7 @@ __global__ void __launch_bounds__(kVarThreads, 5) venc_emit_kernel(const __grid_
 
 // D1: varint terminators (bytes with the top bit clear) per decode tile.  One WARP per tile: sixteen
 // aligned 128-bit loads per lane in two batches of eight, a warp reduction, no block barrier.
-__global__ void __launch_bounds__(kVarThreads, 5) vdec_count_kernel(const __grid_constant__ VarTables tb) {
-  const uint32_t t = blockIdx.x * (kVarThreads / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (t >= tb.n_tiles) return;
+__device__ __forceinline__ void vdec_count_tile(const VarTables& tb, uint32_t t, uint32_t lane) {
   VarSeg sg;
   VarJobDev jb;
   fetch_tile(tb, t, sg, jb);
@@ -386,6 +384,16 @@ __global__ void __launch_bounds__(kVarThreads, 5) vdec_count_kernel(const __grid
 #pragma unroll
   for (int d = 16; d; d >>= 1) cnt += __shfl_xor_sync(0xFFFFFFFFu, cnt, d);
   if (lane == 0) publish_tile(jb, t - jb.first_tile, cnt);
+}
+__global__ void __launch_bounds__(kVarThreads, 5) vdec_count_kernel(const __grid_constant__ VarTables tb) {
+  const uint32_t t = blockIdx.x * (kVarThreads / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (t >= tb.n_tiles) return;
+  vdec_count_tile(tb, t, lane);
+}
+// the same over tables vdec_plan_kernel built: the tile count is in device memory, the grid a fixed bound (warp-stride loop)
+__global__ void __launch_bounds__(kVarThreads, 5) vdec_count_dev_kernel(const __grid_constant__ VarTables tb) {
+  const uint32_t nt = *tb.n_tiles_dev, lane = threadIdx.x & 31;
+  for (uint32_t t = blockIdx.x * (kVarThreads / 32) + (threadIdx.x >> 5); t < nt; t += gridDim.x * (kVarThreads / 32)) vdec_count_tile(tb, t, lane);
 }
 
 // how a decoded value is stored
@@ -458,12 +466,11 @@ __device__ __forceinline__ int32_t decode_elems(const uint8_t* smraw, const uint
 // finds the varints that START there (previous byte is a terminator - the zero before the chunk's first byte
 // is one); a block scan ranks them; they are compacted into a list so that the decode step hands out
 // ELEMENTS, not byte blocks, to threads: balanced work and coalesced stores.
-__global__ void __launch_bounds__(kVarThreads) vdec_emit_kernel(const __grid_constant__ VarTables tb) {
+__device__ __forceinline__ void vdec_emit_tile(const VarTables& tb, uint32_t t) {
   constexpr uint32_t kBlocks = kVarTileBytes / 16;             // 512: two per thread
   __shared__ __align__(16) uint8_t smraw[16 + kVarTileBytes + 16];
   __shared__ uint16_t start_at[kVarTileBytes];
   __shared__ VarShared sh;
-  const uint32_t t = blockIdx.x;
   VarSeg sg;
   VarJobDev jb;
   fetch_tile(tb, t, sg, jb);
@@ -550,4 +557,99 @@ __global__ void __launch_bounds__(kVarThreads) vdec_emit_kernel(const __grid_con
     default: st_local = B200TFS_OK; break;
   }
   if (st_local != B200TFS_OK) atomicMin(jb.status, st_local);
+}
+__global__ void __launch_bounds__(kVarThreads) vdec_emit_kernel(const __grid_constant__ VarTables tb) { vdec_emit_tile(tb, blockIdx.x); }
+// the same over tables vdec_plan_kernel built (grid-stride loop; the barrier keeps the next tile's staging behind this one's reads)
+__global__ void __launch_bounds__(kVarThreads) vdec_emit_dev_kernel(const __grid_constant__ VarTables tb) {
+  const uint32_t nt = *tb.n_tiles_dev;
+  for (uint32_t t = blockIdx.x; t < nt; t += gridDim.x) {
+    vdec_emit_tile(tb, t);
+    __syncthreads();
+  }
+}
+
+// Plan of the packed-varint outputs of a single-launch decode (b200tfs_set_decode_varints), on the device: one CTA reads the
+// table the fused launch just published, gives output k of record r the fixed job r * kFusedMaxOutputs + k and its runs the
+// fixed segments behind it, scans the tile counts (one block scan per kVarPlanThreads slots, the carry in a register), writes
+// the tile -> segment map, zeroes the counters and leaves the tile count for the count / emit kernels.  Nothing waits on
+// another CTA; a captured graph replays it as it is.
+__global__ void __launch_bounds__(kVarPlanThreads) vdec_plan_kernel(const __grid_constant__ VarPlan vp) {
+  __shared__ unsigned long long warp_sum[kVarPlanThreads / 32];
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const uint32_t slots = vp.n * (uint32_t)kFusedMaxOutputs;
+  unsigned long long carry = 0;     // tiles (low 32 bits) and counter groups (high 32 bits) of the slots before this round
+  for (uint32_t s0 = 0; s0 < slots; s0 += kVarPlanThreads) {
+    const uint32_t s = s0 + threadIdx.x, r = s / kFusedMaxOutputs, k = s % kFusedMaxOutputs;
+    int32_t st = kVarSlotIdle;
+    uint32_t tiles = 0, n_runs = 0;
+    const b200tfs_output* o = vp.outs + s;
+    const uint8_t* rec = nullptr;
+    if (s < slots && vp.rec_status[r] == B200TFS_OK && (int32_t)k < vp.n_outs[r] && o->status == B200TFS_OK && o->n_elems &&
+        (dtype_info(o->dtype).kind == VK_VARINT || dtype_info(o->dtype).kind == VK_BOOL)) {
+      rec = vp.w + (vp.n <= (uint32_t)kFusedInlineRecs ? vp.off_inl[r] : vp.rec_off[r]);
+      n_runs = (uint32_t)o->n_runs;
+      st = B200TFS_OK;
+      // rows of unpacked elements (and more runs than the table holds) are left to b200tfs_unpack_outputs, which gathers them
+      if ((o->flags & (B200TFS_OF_UNPACKED | B200TFS_OF_SPILLED)) || o->n_inline != n_runs || n_runs > B200TFS_MAX_RUNS) st = B200TFS_E_NONCANONICAL;
+      for (uint32_t q = 0; q < n_runs && st == B200TFS_OK; ++q) {
+        if (o->runs[q].count != 1) st = B200TFS_E_NONCANONICAL;
+        else tiles += (uint32_t)var_decode_tiles(rec + o->runs[q].off, o->runs[q].len);
+      }
+      if (st != B200TFS_OK) { tiles = 0; n_runs = 0; }
+    }
+    const uint32_t groups = (tiles + kVarGroupTiles - 1) / kVarGroupTiles;
+    // block-wide exclusive scan of (tiles, groups) packed in 64 bits
+    const unsigned long long v = (unsigned long long)tiles | ((unsigned long long)groups << 32);
+    unsigned long long inc = v;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const unsigned long long x = __shfl_up_sync(0xFFFFFFFFu, inc, d);
+      if (lane >= (uint32_t)d) inc += x;
+    }
+    if (lane == 31) warp_sum[wid] = inc;
+    __syncthreads();
+    unsigned long long before = carry, round = 0;
+    for (uint32_t w = 0; w < kVarPlanThreads / 32; ++w) {
+      const unsigned long long x = warp_sum[w];
+      if (w < wid) before += x;
+      round += x;
+    }
+    __syncthreads();
+    before += inc - v;
+    carry += round;
+    const uint32_t first_tile = (uint32_t)before, first_group = (uint32_t)(before >> 32);
+    // beyond the host's bound (never: var_record_tile_bound) - the tiles inside it still run, but can never match the count
+    const bool over = st == B200TFS_OK && first_tile + tiles > vp.tile_cap;
+    if (s < slots) {
+      vp.status[s] = over ? B200TFS_E_NONCANONICAL : st;
+      vp.total[s] = 0;
+      VarJobDev jb{};
+      if (st == B200TFS_OK) {
+        jb.dst = vp.dst + (uint64_t)r * vp.dst_stride + o->dst_off;
+        jb.n_elems = over ? ~0ull : o->n_elems;
+        jb.dtype = o->dtype;
+        jb.elem_size = dtype_info(o->dtype).elem_size;
+        jb.is_signed = dtype_info(o->dtype).is_signed;
+        jb.first_tile = first_tile;
+        jb.n_tiles = tiles;
+        jb.tile_val = vp.tile_val + first_tile;
+        jb.group_sum = vp.group_sum + first_group;
+        jb.total = vp.total + s;
+        jb.status = vp.status + s;
+        const uint32_t run_tiles = over ? vp.tile_cap - min(first_tile, vp.tile_cap) : tiles;   // the tiles that will run
+        for (uint32_t g = 0; g < (run_tiles + kVarGroupTiles - 1) / kVarGroupTiles; ++g) jb.group_sum[g] = 0;
+        uint32_t t = first_tile;
+        for (uint32_t q = 0; q < n_runs; ++q) {
+          const uint8_t* src = rec + o->runs[q].off;
+          const uint32_t len = o->runs[q].len, nt = (uint32_t)var_decode_tiles(src, len);
+          const uint32_t seg = s * B200TFS_MAX_RUNS + q;
+          vp.segs[seg] = VarSeg{src, len, s, t};
+          for (uint32_t i = 0; i < nt && t + i < vp.tile_cap; ++i) vp.tile_seg[t + i] = seg;
+          t += nt;
+        }
+      }
+      vp.jobs[s] = jb;
+    }
+  }
+  if (threadIdx.x == 0) *vp.n_tiles = (uint32_t)min((unsigned long long)vp.tile_cap, carry & 0xFFFFFFFFull);
 }

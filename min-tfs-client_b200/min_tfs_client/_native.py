@@ -25,7 +25,7 @@ F_PRESERIALIZED = 0x4
 F_DEVICE_DATA = 0x8
 RF_GRPC_FRAME = 0x1
 OF_TENSOR_CONTENT, OF_MULTI_CHUNK, OF_DIM_INFERRED, OF_HAS_UNKNOWN, OF_RANK0, OF_VARINT, OF_PAD_EDGE = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20, 0x40
-OF_UNPACKED, OF_SPILLED = 0x80, 0x100
+OF_UNPACKED, OF_SPILLED, OF_DEVICE_VARINT = 0x80, 0x100, 0x200
 ORDER_GIVEN, ORDER_UPB, ORDER_BYTES = 0, 1, 2
 MAX_RANK, MAX_RUNS, FUSED_MAX_OUTPUTS = 16, 8, 8
 DT_HALF_REFQUIRK = -19
@@ -142,6 +142,8 @@ SIGNATURES = {
     "b200tfs_direct_calls": (C.c_int, [_vp, _u64p]),
     "b200tfs_set_pipeline": (C.c_int, [_vp, C.c_uint64, C.c_int32]),
     "b200tfs_set_decode_cast": (C.c_int, [_vp, C.c_int32]),
+    "b200tfs_set_decode_varints": (C.c_int, [_vp, C.c_int32]),
+    "b200tfs_decode_slot_bytes": (C.c_int, [_vp, C.c_int32, _u64p, _u64p, C.c_int32, _u64p, _i32p]),
     "b200tfs_decode_responses_host_async": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64]),
     "b200tfs_encode_tensor_protos_host": (C.c_int, [_vp, C.c_int32, C.POINTER(Tensor), _vp, C.c_uint64, _u64p, _u64p]),
     "b200tfs_parse_responses_host": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(Output), _i32p,

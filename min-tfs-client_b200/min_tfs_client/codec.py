@@ -145,6 +145,23 @@ class DecodedSpec:
 
 
 _FUSED_MOVES = frozenset((1, 2, 8, 18))   # DT_FLOAT, DT_DOUBLE, DT_COMPLEX64, DT_COMPLEX128: what decode_fused_kernel moves itself
+# the dtypes whose values are packed varints (int_val, int64_val, uint32_val, uint64_val, bool_val, half_val): what the same launch
+# decodes as well once b200tfs_set_decode_varints is on
+_VARINT_DTYPES = frozenset((3, 4, 5, 6, 9, 10, 14, 17, 19, 22, 23))
+
+
+def _device_varint(o: N.Output) -> bool:
+    """A varint output the single-launch decode decoded into its range.  One it decoded with an error, or could not lay out
+    (E_SIZE), reads afterwards as the table reads with the switch off - status OK, tabulated only - so that the unpack route
+    finishes it and raises exactly what it raises today."""
+    if o.flags & N.OF_DEVICE_VARINT:
+        if o.status == N.OK:
+            return True
+        o.flags &= ~N.OF_DEVICE_VARINT
+        o.status = N.OK
+    elif o.status == N.E_SIZE and int(o.dtype) in _VARINT_DTYPES:
+        o.status = N.OK     # not laid out: never viewed, the unpack route (or the caller) decodes it
+    return False
 
 
 class OpenResponse:
@@ -162,9 +179,12 @@ class OpenResponse:
         """The decoded output, or None when the launch did not move it (varint-packed, string, tensor_content only): the
         caller then decodes ``wire_of(key)`` on its own.  Raises what the reference raises for this output."""
         o = self.table[key]
-        if int(o.dtype) not in _FUSED_MOVES or o.status != N.OK or not o.n_runs or not o.n_elems:
+        dev_varint = _device_varint(o)
+        if not dev_varint and (int(o.dtype) not in _FUSED_MOVES or o.status != N.OK or not o.n_runs or not o.n_elems):
             return None
         np_type, dst_code, shape = self._codec._resolve_output(o, strict, None)
+        if dev_varint and dst_code != int(o.dtype):
+            return None      # strict DT_HALF: the reference reads half_val as values, the launch wrote TF's bit patterns
         at = int(o.dst_off)
         arr = self._dst[at: at + int(o.dst_bytes)].view(np_type).reshape(shape)
         if key in self._handed:      # tensor_proto_to_ndarray returns a fresh array per call (tensors.py:46): never alias two results
@@ -195,6 +215,10 @@ class Codec:
         self.device = device
         self._pinned = D.PinnedArrays()
         self._wire_pinned = None      # page-locked landing buffer of encode(..., out="pinned")
+        # whether a response decoded so far carried packed-varint outputs.  Until then the single-launch decode leaves them to the
+        # unpack route and float-only traffic pays nothing; from then on every call sizes its slots from its own records
+        # (_slot_stride) and the launch decodes varint outputs too when they have some (b200tfs_set_decode_varints)
+        self._seen_varints = False
 
     def close(self):
         if getattr(self, "_ctx", None):
@@ -523,15 +547,19 @@ class Codec:
         n = len(wires)
         buf, off, ln = self._pack_wires(wires)
         K = N.FUSED_MAX_OUTPUTS
-        stride = (max(int(ln[i]) for i in range(n)) + 256 * (K + 1) + 255) & ~255   # every fixed output fits, each 256-aligned
+        stride, varints = self._slot_stride(buf, off, ln)
         dst = np.empty(n * stride, dtype=np.uint8)
         if cast_code:
             N.check(self._lib.b200tfs_set_decode_cast(self._ctx, cast_code))
+        if varints:
+            N.check(self._lib.b200tfs_set_decode_varints(self._ctx, 1))
         try:
             N.check(self._lib.b200tfs_decode_responses_host_async(self._ctx, buf.ctypes.data, n, off, ln, dst.ctypes.data, stride))
         finally:
             if cast_code:
                 N.check(self._lib.b200tfs_set_decode_cast(self._ctx, 0))
+            if varints:
+                N.check(self._lib.b200tfs_set_decode_varints(self._ctx, 0))
         outs = (N.Output * (n * K))()
         n_outs = (C.c_int32 * n)()
         specs = (N.ModelSpec * n)()
@@ -554,12 +582,31 @@ class Codec:
         for j in range(n_outs[0]):
             o = outs[j]
             table[self._text(buf, int(off[0]) + o.key_off, o.key_len)] = o
+            if o.n_elems and int(o.dtype) in _VARINT_DTYPES:
+                self._seen_varints = True
         return OpenResponse(self, buf, int(off[0]), dst, table)
+
+    def _slot_stride(self, buf, off, ln) -> Tuple[int, bool]:
+        """(dst_stride, decode varints) for the records of ONE call.  Every fixed-width output fits the parent layout's stride
+        (longest record + one 256-byte alignment per output).  Once this codec has seen varint outputs, the host walks the
+        call's records (b200tfs_decode_slot_bytes) and, when they carry varint outputs, the stride is what their layout with
+        varint ranges needs - so a float-only call keeps the plain stride, and a denser response never pushes an output out."""
+        n = len(ln)
+        stride = (max(int(ln[i]) for i in range(n)) + 256 * (N.FUSED_MAX_OUTPUTS + 1) + 255) & ~255
+        if not self._seen_varints:
+            return stride, False
+        need, nv = C.c_uint64(), C.c_int32()
+        N.check(self._lib.b200tfs_decode_slot_bytes(buf.ctypes.data, n, off, ln, 1, C.byref(need), C.byref(nv)))
+        if not nv.value:
+            return stride, False
+        return max(stride, (need.value + 255) & ~255), True
 
     def _decode_fused(self, wires: Sequence[bytes], strict: bool, cast=None):
         """One launch, one synchronise: tag walk (or framing-template check), destination layout and the move of every
-        fixed-width output in ``decode_fused_kernel``; the outputs come back as views of one host buffer.  Varint-packed
-        and tensor_content-only outputs are tabulated by the same launch and unpacked by a second one.  Returns None when
+        fixed-width output in ``decode_fused_kernel``; the outputs come back as views of one host buffer.  Once this codec has
+        seen varint-packed outputs, the same launch decodes those too (b200tfs_set_decode_varints) and they come back as views
+        as well; the ones it cannot finish (TF's padding, strict DT_HALF, rows of unpacked elements, errors) and
+        tensor_content-only outputs are unpacked by a second one.  Returns None when
         a record needs the two-phase path (more than eight outputs, a malformed record: that path raises what the
         reference raises)."""
         cast_code, cast_keys = cast if cast else (0, {})
@@ -585,9 +632,17 @@ class Codec:
                     continue
                 if cast_code and ((int(o.dtype) == 1) != (key in cast_keys)):
                     return None      # the launch narrowed every float32 output: only right when exactly those were asked for
+                unplaced = o.status == N.E_SIZE   # no room in the slot (_slot_stride sizes it so that this does not happen)
+                if unplaced:
+                    o.status = N.OK               # ... as the walk tabulated it: the unpack route decodes it
+                dev_varint = False
+                if int(o.dtype) in _VARINT_DTYPES and o.n_elems:
+                    self._seen_varints = True
+                    dev_varint = _device_varint(o)
                 np_type, dst_code, shape = self._resolve_output(o, strict, cast_keys.get(key))
-                if o.status == N.OK and int(o.dtype) in _FUSED_MOVES and o.n_runs and o.n_elems and \
-                        (dst_code == int(o.dtype) or (cast_code and int(o.dtype) == 1 and dst_code == cast_code)):
+                if not unplaced and ((dev_varint and dst_code == int(o.dtype)) or
+                                     o.status == N.OK and int(o.dtype) in _FUSED_MOVES and o.n_runs and o.n_elems and
+                                     (dst_code == int(o.dtype) or (cast_code and int(o.dtype) == 1 and dst_code == cast_code))):
                     at = i * stride + int(o.dst_off)
                     arrays[key] = dst[at: at + int(o.dst_bytes)].view(np_type).reshape(shape)
                 else:
