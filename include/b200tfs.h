@@ -397,6 +397,66 @@ int b200tfs_decode_stats(b200tfs_ctx* ctx, uint64_t* param_template, uint64_t* d
 int b200tfs_decode_results(b200tfs_ctx* ctx, int32_t n, b200tfs_output* outs, int32_t* n_outs,
                            b200tfs_model_spec* specs, int32_t* rec_status);
 
+/* ---- batch decode into one tensor per output, concatenated along axis 0 ---------------------------
+ * What a client that split a batch into n requests wants back: for each requested key, the outputs of every record
+ * concatenated along their first dimension - np.concatenate([decode(w)[key] for w in wires], axis=0) - written straight into
+ * one device buffer per key, every payload byte read once and written once.  Record r's rows start where the rows of
+ * records 0..r-1 end; since those counts are only known once the records are parsed, the destinations are planned on the
+ * device (a replayed CUDA graph adapts to new row counts).  Only the requested outputs are decoded.                       */
+#define B200TFS_CONCAT_MAX_KEYS 8
+typedef struct b200tfs_concat_key {
+  const char* key;        /* in: map key bytes (not NUL terminated); the keys of one call must be distinct            */
+  int64_t key_len;
+  void* dst;              /* in: b200tfs_decode_concat*: device destination of the concatenated tensor               */
+  uint64_t dst_cap;       /* in: its capacity in bytes - nothing is ever stored at or past dst + dst_cap              */
+  int32_t dtype;          /* out (b200tfs_concat_layout): DT_* of the first record that has the key                   */
+  int32_t rank;           /* out: rank of the concatenated tensor                                                     */
+  int64_t dims[B200TFS_MAX_RANK]; /* out: dims[0] = rows of all records together, the rest those of every record      */
+  uint64_t bytes;         /* out: bytes of the concatenated tensor in memory (2 per float32 element with a cast)      */
+  int32_t status;         /* out: B200TFS_OK (also for a DT_STRING key: bytes 0, decoded on the host) or the first
+                             problem in record order: the record's error (E_PARSE, ...,
+                             E_NONCANONICAL for a record the device route cannot tabulate: more than
+                             B200TFS_FUSED_MAX_OUTPUTS outputs, rank > B200TFS_MAX_RANK, more than B200TFS_MAX_RUNS runs),
+                             the output's tabulated error (E_SHAPE, E_KEY, ...), E_KEY when the record lacks the key,
+                             E_SHAPE for rank 0 / another rank / other trailing dims, E_DTYPE for another dtype            */
+  int32_t bad_rec;        /* out: the record `status` is about (-1 when OK)                                          */
+} b200tfs_concat_key;
+/* Host only (needs no device): walks the n records in host memory and fills the out fields of keys[0..n_keys), which is what
+ * a caller needs to allocate exact-size destinations.  cast: 0, or DT_HALF / DT_BFLOAT16 as b200tfs_set_decode_cast sets it. */
+int b200tfs_concat_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
+                          b200tfs_concat_key* keys, int32_t cast);
+/* The keys of one record in host memory, in table order (the order of their first map entry): key_off[i] (from the start of
+ * the record) and key_len[i] for i < *count; at most `cap` are written.  A record that does not walk: its error.            */
+int b200tfs_response_keys(const void* rec_host, uint64_t rec_len, int32_t cap, uint64_t* key_off, uint32_t* key_len,
+                          int32_t* count);
+/* Decode n PredictResponses of the device arena into keys[k].dst for every k < n_keys (<= B200TFS_CONCAT_MAX_KEYS; only the
+ * in fields are read).  Asynchronous and CUDA-graph capturable: the host is not involved between the launches (parse,
+ * one-CTA plan, move engine, packed-varint plan / count / emit - b200tfs_kernel_launches counts six).  The scratch it needs
+ * is sized from n, n_keys and rec_len alone, so a graph captured once serves any records of those lengths.  Float32 outputs
+ * are narrowed per b200tfs_set_decode_cast.  Values: what b200tfs_unpack_outputs writes with dst_dtype NULL (half_val as TF
+ * bit patterns).  Stores: only into [dst_off, dst_off + dst_bytes) of the (record, key) pairs b200tfs_concat_results reports
+ * B200TFS_OK, or reports with B200TFS_OF_DEVICE_VARINT (a packed-varint output whose place was reserved; when its decode
+ * failed the contents are unspecified), never at or past dst_cap.  Every other byte keeps what the caller left there.      */
+int b200tfs_decode_concat(b200tfs_ctx* ctx, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                          int32_t n_keys, const b200tfs_concat_key* keys);
+/* The same for records in host memory: the wire is copied to the device inside (asynchronous; wire_host should be pinned). */
+int b200tfs_decode_concat_host_async(b200tfs_ctx* ctx, const void* wire_host, int32_t n, const uint64_t* rec_off,
+                                     const uint64_t* rec_len, int32_t n_keys, const b200tfs_concat_key* keys);
+/* Results of the context's most recent b200tfs_decode_concat* call (synchronises).  outs[r * n_keys + k]: record r's table entry
+ * for key k, with dst_off = where its rows start inside keys[k].dst and `status`: B200TFS_OK (decoded); the record's or the
+ * output's error; B200TFS_E_KEY (no such key); B200TFS_E_DTYPE / B200TFS_E_SHAPE (dtype / rank / trailing dims differ from the
+ * first record that decoded the key; rank 0); B200TFS_E_SIZE (its rows end past dst_cap); B200TFS_E_NONCANONICAL, which is
+ * either a packed-varint output in rows of unpacked elements (its place [dst_off, dst_off + dst_bytes) is reserved; finish it
+ * with b200tfs_unpack_outputs there), a string output (nothing reserved: strings are decoded on the host), or a record the
+ * device parse cannot tabulate (more than B200TFS_FUSED_MAX_OUTPUTS outputs, rank > B200TFS_MAX_RANK, more than
+ * B200TFS_MAX_RUNS runs; nothing reserved).  Outputs the tolerant decode would accept although their table entry is an error -
+ * tensor_content only, fewer fixed-width values than the shape holds (TF's padding) - keep that error (B200TFS_E_SHAPE) and
+ * get no place: whether to accept them is the caller's policy, and the row count of such a batch is only known once it is
+ * chosen.  Packed-varint outputs carry B200TFS_OF_DEVICE_VARINT and that decode's status.  specs[r] and rec_status[r] as
+ * b200tfs_parse_responses gives them; any pointer may be NULL.                                                           */
+int b200tfs_concat_results(b200tfs_ctx* ctx, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs,
+                           int32_t* rec_status);
+
 /* ---- CUDA graphs: record a fixed sequence of encode / decode calls once, replay it per request ---
  * Between capture_begin and capture_end the asynchronous entry points (b200tfs_encode_requests,
  * b200tfs_encode_tensor_protos, b200tfs_decode_responses, b200tfs_memcpy_*) only record work; calls

@@ -132,6 +132,10 @@ struct b200tfs_ctx {
   Growable enc_host;                    // b200tfs_encode_requests_async: rec_off | rec_len | status, written by frame_requests_kernel (pinned)
   int32_t enc_n = 0;
   bool has_graphs = false;              // a CUDA graph captured on this context refers to the scratch buffers: they may not move any more
+  Growable concat_dev;                  // b200tfs_decode_concat: parse table, plan image, varint tables (ConcatLayout)
+  int32_t concat_n = 0, concat_k = 0;   // ... of its most recent call, what b200tfs_concat_results answers for
+  uint8_t* concat_dst[B200TFS_CONCAT_MAX_KEYS] = {};
+  uint64_t concat_vouts_off = 0, concat_vstat_off = 0;
 };
 
 // `baked`: the buffer's address ends up inside captured graphs (every context-owned scratch buffer except the plan-upload
@@ -283,6 +287,7 @@ int b200tfs_destroy(b200tfs_ctx* c) {
   if (c->gather_dev.p) cudaFree(c->gather_dev.p);
   if (c->guard_dev.p) cudaFree(c->guard_dev.p);
   if (c->vdec_dev.p) cudaFree(c->vdec_dev.p);
+  if (c->concat_dev.p) cudaFree(c->concat_dev.p);
   if (c->enc_host.p) cudaFreeHost(c->enc_host.p);
   if (c->measured_dev.p) cudaFree(c->measured_dev.p);
   if (c->scratch_host.p) cudaFreeHost(c->scratch_host.p);
@@ -2116,6 +2121,239 @@ int b200tfs_unpack_outputs_host(b200tfs_ctx* c, int32_t m, const b200tfs_output*
     }
   CU(cudaStreamSynchronize(c->stream));
   collect_varint_status(c, status);
+  return B200TFS_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// decode into one tensor per key, concatenated along axis 0
+// ------------------------------------------------------------------------------------------------
+static int concat_check_keys(int32_t n_keys, const b200tfs_concat_key* keys) {
+  if (n_keys <= 0 || n_keys > B200TFS_CONCAT_MAX_KEYS || !keys) return fail(B200TFS_E_ARG, "n_keys must be 1..%d", B200TFS_CONCAT_MAX_KEYS);
+  for (int k = 0; k < n_keys; ++k) {
+    if (keys[k].key_len < 0 || keys[k].key_len > 0xFFFFFFFFll || (keys[k].key_len && !keys[k].key)) return fail(B200TFS_E_ARG, "key %d: bad key", k);
+    for (int j = 0; j < k; ++j)
+      if (keys[j].key_len == keys[k].key_len && !memcmp(keys[j].key, keys[k].key, (size_t)keys[k].key_len))
+        return fail(B200TFS_E_ARG, "key %d repeats key %d", k, j);
+  }
+  return B200TFS_OK;
+}
+
+int b200tfs_response_keys(const void* rec_host, uint64_t rec_len, int32_t cap, uint64_t* key_off, uint32_t* key_len, int32_t* count) {
+  if (!count || cap < 0 || (cap && (!key_off || !key_len)) || (rec_len && !rec_host)) return fail(B200TFS_E_ARG, "bad arguments");
+  *count = 0;
+  if (rec_len > 0x7FFFFFFFull) return B200TFS_E_PARSE;
+  std::vector<b200tfs_output> outs;
+  for (int max = 16;; max *= 2) {   // PredictResponse.FromString has no limit on the map size
+    outs.assign((size_t)max + 1, b200tfs_output{});
+    b200tfs_model_spec spec;
+    int cnt = 0;
+    Cursor cur;
+    cur_open_host(cur, (const uint8_t*)rec_host, (uint32_t)rec_len);
+    std::vector<SpillEntry> spill(4096);
+    SpillArea sp{spill.data(), (uint32_t)spill.size(), 0u};
+    const int st = walk_response(cur, max, outs.data(), &cnt, &spec, sp);
+    if (st == B200TFS_E_SIZE && max < (1 << 20)) continue;
+    if (st != B200TFS_OK && st != B200TFS_E_SPILL) return st;   // a spill only concerns dims / runs: the keys are all there
+    *count = cnt;
+    for (int i = 0; i < cnt && i < cap; ++i) { key_off[i] = outs[i].key_off; key_len[i] = outs[i].key_len; }
+    return B200TFS_OK;
+  }
+}
+
+int b200tfs_concat_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
+                          b200tfs_concat_key* keys, int32_t cast) {
+  if (n <= 0 || !wire_host || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
+  int rc = concat_check_keys(n_keys, keys);
+  if (rc) return rc;
+  if (cast != 0 && cast != DT_FLOAT && cast != DT_HALF && cast != DT_BFLOAT16) return fail(B200TFS_E_DTYPE, "cast to dtype %d", cast);
+  const uint32_t cst = (cast == DT_HALF || cast == DT_BFLOAT16) ? (uint32_t)cast : 0u;
+  for (int k = 0; k < n_keys; ++k) {
+    b200tfs_concat_key& K = keys[k];
+    K.dtype = 0; K.rank = 0; K.bytes = 0; K.status = B200TFS_E_KEY; K.bad_rec = -1;
+    for (int d = 0; d < B200TFS_MAX_RANK; ++d) K.dims[d] = 0;
+  }
+  std::vector<uint8_t> have(n_keys, 0);   // a reference record for the key was found
+  std::vector<int> done(n_keys, 0);       // the key's status is final
+  for (int r = 0; r < n; ++r) {
+    b200tfs_output outs[kFusedMaxOutputs + 1];
+    b200tfs_model_spec spec;
+    int cnt = 0, st = B200TFS_E_PARSE;
+    const uint8_t* rec = (const uint8_t*)wire_host + rec_off[r];
+    if (rec_len[r] <= 0x7FFFFFFFull) {
+      Cursor cur;
+      cur_open_host(cur, rec, (uint32_t)rec_len[r]);
+      SpillArea sp{nullptr, 0u, 0u};
+      st = walk_response(cur, kFusedMaxOutputs, outs, &cnt, &spec, sp);
+      if (st == B200TFS_E_SPILL || st == B200TFS_E_SIZE) st = B200TFS_E_NONCANONICAL;
+    }
+    for (int k = 0; k < n_keys; ++k) {
+      if (done[k]) continue;
+      b200tfs_concat_key& K = keys[k];
+      int32_t s = st;
+      const b200tfs_output* o = nullptr;
+      if (s == B200TFS_OK) {
+        for (int j = 0; j < cnt && !o; ++j)
+          if ((int64_t)outs[j].key_len == K.key_len && !memcmp(rec + outs[j].key_off, K.key, (size_t)K.key_len)) o = &outs[j];
+        if (!o) s = B200TFS_E_KEY;
+        else if ((s = o->status) == B200TFS_OK) {
+          if (o->rank == 0) s = B200TFS_E_SHAPE;
+          else if (o->rank > B200TFS_MAX_RANK) s = B200TFS_E_NONCANONICAL;
+          else if (have[k] && o->dtype != K.dtype) s = B200TFS_E_DTYPE;
+          else if (have[k] && o->rank != K.rank) s = B200TFS_E_SHAPE;
+          else for (int d = 1; have[k] && d < o->rank; ++d) if (o->dims[d] != K.dims[d]) s = B200TFS_E_SHAPE;
+        }
+      }
+      if (s != B200TFS_OK) { K.status = s; K.bad_rec = r; done[k] = 1; continue; }
+      if (!have[k]) {
+        have[k] = 1;
+        K.dtype = o->dtype; K.rank = o->rank;
+        for (int d = 0; d < o->rank; ++d) K.dims[d] = o->dims[d];
+        K.dims[0] = 0;
+      }
+      K.dims[0] += o->dims[0];
+      K.bytes += tpl_narrows(cst, o->dtype) ? o->n_elems * 2 : o->dst_bytes;
+    }
+  }
+  for (int k = 0; k < n_keys; ++k) if (!done[k]) keys[k].status = B200TFS_OK;
+  return B200TFS_OK;
+}
+
+namespace {
+// device scratch of b200tfs_decode_concat for n records, n_keys keys, tile_cap move tiles and var_tile_cap varint tiles
+struct ConcatLayout { uint64_t outs, nouts, specs, status, spill, kst, match, plan, plan_tiles, vouts, vnouts, vstatus, var, bytes; };
+ConcatLayout concat_layout(uint64_t n, uint64_t n_keys, uint64_t tile_cap, uint64_t var_tile_cap) {
+  auto up = [](uint64_t x) { return (x + 255) & ~255ull; };
+  ConcatLayout L;
+  L.outs = 0;
+  L.nouts = up(L.outs + sizeof(b200tfs_output) * n * (kFusedMaxOutputs + 1));
+  L.specs = up(L.nouts + 4 * n);
+  L.status = up(L.specs + sizeof(b200tfs_model_spec) * n);
+  L.spill = up(L.status + 4 * n);
+  L.kst = up(L.spill + 4 * n);
+  L.match = up(L.kst + 4 * n * n_keys);
+  L.plan = up(L.match + 4 * n * n_keys);
+  L.plan_tiles = ((((sizeof(PlanHeader) + 15) & ~15ull) + n * n_keys * B200TFS_MAX_RUNS * sizeof(MoveItem) + 15) & ~15ull);
+  L.vouts = up(L.plan + L.plan_tiles + tile_cap * sizeof(TileRef));
+  L.vnouts = up(L.vouts + sizeof(b200tfs_output) * n * kFusedMaxOutputs);
+  L.vstatus = up(L.vnouts + 4 * n);
+  L.var = up(L.vstatus + 4 * n);
+  L.bytes = L.var + var_plan_layout(n, var_tile_cap).bytes;
+  return L;
+}
+}  // namespace
+
+int b200tfs_decode_concat(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                          int32_t n_keys, const b200tfs_concat_key* keys) {
+  if (!c || n <= 0 || !arena_dev || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
+  int rc = concat_check_keys(n_keys, keys);
+  if (rc) return rc;
+  for (int k = 0; k < n_keys; ++k) if (keys[k].dst_cap && !keys[k].dst) return fail(B200TFS_E_ARG, "key %d: dst is NULL", k);
+  if (!c->capturing) CU(cudaSetDevice(c->device));
+  uint64_t wire_total = 0, tile_cap = 0, var_tile_cap = 0;
+  for (int i = 0; i < n; ++i) wire_total += rec_len[i];
+  const uint32_t vpt = pick_vec_per_tile(c, c->decode_cast ? wire_total / 2 : wire_total);
+  for (int i = 0; i < n; ++i) {
+    tile_cap += concat_record_tile_bound(rec_len[i], 16ull * vpt, (uint32_t)n_keys);
+    var_tile_cap += var_record_tile_bound(rec_len[i]);
+  }
+  if (tile_cap > 0x7FFFFFFFull || var_tile_cap > 0x7FFFFFFFull) return fail(B200TFS_E_TOOBIG, "batch needs more than 2^31 tiles");
+  const ConcatLayout L = concat_layout((uint64_t)n, (uint64_t)n_keys, tile_cap, var_tile_cap);
+  if (L.plan_tiles > 0xFFFFFFFFull) return fail(B200TFS_E_TOOBIG, "plan image larger than 4 GiB");
+  if ((rc = grow_dev(c, c->concat_dev, L.bytes))) return rc;
+  // rec_off | rec_len | keys | key bytes: one upload (a captured call keeps a private copy)
+  uint64_t key_bytes = 0;
+  for (int k = 0; k < n_keys; ++k) key_bytes += (uint64_t)keys[k].key_len;
+  const uint64_t o_len = 8ull * n, o_keys = (o_len + 8ull * n + 15) & ~15ull, o_kb = o_keys + sizeof(ConcatKeyDev) * n_keys;
+  Slot* slot;
+  if ((rc = claim_slot(c, o_kb + key_bytes + 16, &slot))) return rc;
+  uint8_t* h = (uint8_t*)slot->host.p;
+  uint8_t* sd = (uint8_t*)slot->dev.p;
+  memcpy(h, rec_off, 8ull * n);
+  memcpy(h + o_len, rec_len, 8ull * n);
+  uint64_t at = o_kb;
+  for (int k = 0; k < n_keys; ++k) {
+    ConcatKeyDev kd{sd + at, (uint8_t*)keys[k].dst, keys[k].dst_cap, (uint32_t)keys[k].key_len, 0u};
+    memcpy(h + o_keys + sizeof(ConcatKeyDev) * k, &kd, sizeof kd);
+    if (keys[k].key_len) memcpy(h + at, keys[k].key, (size_t)keys[k].key_len);
+    at += (uint64_t)keys[k].key_len;
+    c->concat_dst[k] = (uint8_t*)keys[k].dst;
+  }
+  if ((rc = upload_slot(c, slot, at))) return rc;
+  uint8_t* d = (uint8_t*)c->concat_dev.p;
+  const uint64_t* off_dev = (const uint64_t*)sd;
+  CU(launch_parse_responses((const uint8_t*)arena_dev, off_dev, (const uint64_t*)(sd + o_len), n, kFusedMaxOutputs, (b200tfs_output*)(d + L.outs),
+                            (int32_t*)(d + L.nouts), (b200tfs_model_spec*)(d + L.specs), (int32_t*)(d + L.status), nullptr, 0u,
+                            (uint32_t*)(d + L.spill), c->stream));
+  ConcatPlan cp{};
+  cp.w = (const uint8_t*)arena_dev; cp.rec_off = off_dev; cp.outs = (const b200tfs_output*)(d + L.outs);
+  cp.n_outs = (const int32_t*)(d + L.nouts); cp.rec_status = (const int32_t*)(d + L.status);
+  cp.keys = (const ConcatKeyDev*)(sd + o_keys);
+  cp.n = (uint32_t)n; cp.n_keys = (uint32_t)n_keys; cp.out_stride = kFusedMaxOutputs + 1; cp.cast = c->decode_cast;
+  cp.vpt = vpt; cp.tile_cap = (uint32_t)tile_cap;
+  cp.kst = (int32_t*)(d + L.kst); cp.match = (int32_t*)(d + L.match); cp.plan = d + L.plan;
+  cp.vouts = (b200tfs_output*)(d + L.vouts); cp.vn_outs = (int32_t*)(d + L.vnouts); cp.vrec_status = (int32_t*)(d + L.vstatus);
+  CU(launch_concat_plan(cp, (uint32_t)tile_cap, c->stream));
+  // packed-varint outputs: the single-launch decode's plan / count / emit over the table the plan kernel wrote (its dst_off is
+  // the absolute address: dst 0, stride 0)
+  const VarPlanLayout V = var_plan_layout((uint64_t)n, var_tile_cap);
+  uint8_t* vd = d + L.var;
+  VarPlan vp{};
+  vp.outs = cp.vouts; vp.n_outs = cp.vn_outs; vp.rec_status = cp.vrec_status;
+  vp.w = cp.w; vp.rec_off = off_dev;
+  if (n <= kFusedInlineRecs) for (int i = 0; i < n; ++i) vp.off_inl[i] = rec_off[i];
+  vp.dst = nullptr; vp.dst_stride = 0; vp.n = (uint32_t)n; vp.tile_cap = (uint32_t)var_tile_cap;
+  vp.jobs = (VarJobDev*)(vd + V.jobs); vp.segs = (VarSeg*)(vd + V.segs); vp.tile_seg = (uint32_t*)(vd + V.tile_seg);
+  vp.tile_val = (uint32_t*)(vd + V.tile_val); vp.group_sum = (uint32_t*)(vd + V.group_sum);
+  vp.total = (unsigned long long*)(vd + V.total); vp.status = (int32_t*)(vd + V.status); vp.n_tiles = (uint32_t*)(vd + V.n_tiles);
+  CU(launch_vdec_plan(vp, c->stream));
+  VarTables tb{};
+  tb.segs = vp.segs; tb.tile_seg = vp.tile_seg; tb.jobs = vp.jobs; tb.n_tiles = vp.tile_cap; tb.n_tiles_dev = vp.n_tiles;
+  CU(launch_vdec_dev(tb, (uint32_t)c->sm_count * 4, c->stream));
+  if (slot->done && !c->capturing) { CU(cudaEventRecord(slot->done, c->stream)); slot->pending = true; }   // the kernels read the upload
+  c->launches += 6;
+  c->concat_n = n; c->concat_k = n_keys; c->concat_vouts_off = L.vouts; c->concat_vstat_off = L.var + V.status;
+  return B200TFS_OK;
+}
+
+int b200tfs_decode_concat_host_async(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                                     int32_t n_keys, const b200tfs_concat_key* keys) {
+  if (!c || n <= 0 || !wire_host || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
+  if (c->capturing) return fail(B200TFS_E_ARG, "capture b200tfs_decode_concat over a device arena instead");
+  CU(cudaSetDevice(c->device));
+  uint64_t span;
+  int rc = stage_wire(c, wire_host, n, rec_off, rec_len, &span);
+  if (rc) return rc;
+  return b200tfs_decode_concat(c, c->stage_dev.p, n, rec_off, rec_len, n_keys, keys);
+}
+
+int b200tfs_concat_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs, int32_t* rec_status) {
+  if (!c || n < 0 || n_keys < 0) return fail(B200TFS_E_ARG, "bad arguments");
+  if (c->capturing) return fail(B200TFS_E_ARG, "cannot collect results during graph capture");
+  if (n != c->concat_n || n_keys != c->concat_k) return fail(B200TFS_E_ARG, "the last b200tfs_decode_concat had %d records and %d keys", c->concat_n, c->concat_k);
+  if (n == 0) return B200TFS_OK;
+  CU(cudaSetDevice(c->device));
+  CU(cudaStreamSynchronize(c->stream));
+  const ConcatLayout L = concat_layout((uint64_t)n, (uint64_t)n_keys, 0, 0);   // specs and status do not depend on the tile bounds
+  const uint8_t* d = (const uint8_t*)c->concat_dev.p;
+  if (outs) {
+    std::vector<b200tfs_output> v((size_t)n * kFusedMaxOutputs);
+    std::vector<int32_t> vs((size_t)n * kFusedMaxOutputs);
+    CU(cudaMemcpy(v.data(), d + c->concat_vouts_off, sizeof(b200tfs_output) * v.size(), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(vs.data(), d + c->concat_vstat_off, 4 * vs.size(), cudaMemcpyDeviceToHost));
+    for (int r = 0; r < n; ++r)
+      for (int k = 0; k < n_keys; ++k) {
+        b200tfs_output o = v[(size_t)r * kFusedMaxOutputs + k];
+        const int32_t s = vs[(size_t)r * kFusedMaxOutputs + k];
+        if (s != kVarSlotIdle) { o.status = s; o.flags |= B200TFS_OF_DEVICE_VARINT; }
+        o.dst_off -= (uint64_t)(uintptr_t)c->concat_dst[k];
+        outs[(size_t)r * n_keys + k] = o;
+      }
+  }
+  if (specs) CU(cudaMemcpy(specs, d + L.specs, sizeof(b200tfs_model_spec) * (uint64_t)n, cudaMemcpyDeviceToHost));
+  if (rec_status) {
+    CU(cudaMemcpy(rec_status, d + L.status, 4ull * n, cudaMemcpyDeviceToHost));
+    for (int r = 0; r < n; ++r) if (rec_status[r] == B200TFS_E_SPILL || rec_status[r] == B200TFS_E_SIZE) rec_status[r] = B200TFS_E_NONCANONICAL;
+  }
   return B200TFS_OK;
 }
 

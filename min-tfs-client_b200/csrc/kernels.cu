@@ -1040,6 +1040,141 @@ __global__ void __launch_bounds__(kMoveThreads, 2) decode_fused_staged_cast_kern
 #include "varint_kernels.cuh"
 
 // ------------------------------------------------------------------------------------------------
+// concat_plan_kernel (plan.h ConcatPlan): one CTA plans b200tfs_decode_concat.  Per requested key, pass A matches the key in
+// every record's table and finds the first record that decoded it (the reference for dtype, rank and trailing dims); pass B
+// checks every record against it, scans the bytes of the records into offsets inside the key's destination and the move
+// tiles into the tile table, and writes the move items and the varint table.  Block scans with the carry in a register:
+// nothing waits on another CTA, and a replayed graph re-plans from whatever row counts the new records carry.
+// ------------------------------------------------------------------------------------------------
+// exclusive scan of one value per thread across the CTA; `carry` (uniform) advances by the round's total
+__device__ __forceinline__ uint64_t concat_scan(uint64_t v, uint64_t& carry, unsigned long long* warp_sum) {
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  uint64_t inc = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint64_t x = __shfl_up_sync(0xFFFFFFFFu, inc, d);
+    if (lane >= (uint32_t)d) inc += x;
+  }
+  if (lane == 31) warp_sum[wid] = inc;
+  __syncthreads();
+  uint64_t before = carry, round = 0;
+  for (uint32_t w = 0; w < kConcatPlanThreads / 32; ++w) {
+    const uint64_t x = warp_sum[w];
+    if (w < wid) before += x;
+    round += x;
+  }
+  __syncthreads();
+  carry += round;
+  return before + inc - v;
+}
+
+__global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const __grid_constant__ ConcatPlan cp) {
+  __shared__ unsigned long long warp_sum[kConcatPlanThreads / 32];
+  __shared__ uint32_t ref_rec;
+  const uint32_t n = cp.n, nk = cp.n_keys;
+  MoveItem* items = reinterpret_cast<MoveItem*>(cp.plan + ((sizeof(PlanHeader) + 15) & ~15ull));
+  const uint64_t n_items = (uint64_t)n * nk * B200TFS_MAX_RUNS;
+  const uint64_t off_tiles = (((sizeof(PlanHeader) + 15) & ~15ull) + n_items * sizeof(MoveItem) + 15) & ~15ull;
+  TileRef* tref = reinterpret_cast<TileRef*>(cp.plan + off_tiles);
+  uint64_t tile_carry = 0;
+  for (uint32_t k = 0; k < nk; ++k) {
+    const ConcatKeyDev key = cp.keys[k];
+    if (threadIdx.x == 0) ref_rec = n;
+    __syncthreads();
+    // pass A: the key in each record's table, and the record's own verdict on it
+    for (uint32_t r = threadIdx.x; r < n; r += kConcatPlanThreads) {
+      int32_t st = cp.rec_status[r], m = -1;
+      if (st == B200TFS_E_SPILL || st == B200TFS_E_SIZE) st = B200TFS_E_NONCANONICAL;   // more than the table holds: another route
+      if (st == B200TFS_OK) {
+        const b200tfs_output* t = cp.outs + (size_t)r * cp.out_stride;
+        const uint8_t* rec = cp.w + cp.rec_off[r];
+        for (int32_t j = 0; j < cp.n_outs[r] && m < 0; ++j) {
+          if (t[j].key_len != key.key_len) continue;
+          bool same = true;
+          for (uint32_t i = 0; i < key.key_len && same; ++i) same = rec[t[j].key_off + i] == key.key[i];
+          if (same) m = j;
+        }
+        if (m < 0) st = B200TFS_E_KEY;
+        else {
+          const b200tfs_output& o = t[m];
+          st = o.status;
+          if (st == B200TFS_OK && o.rank == 0) st = B200TFS_E_SHAPE;
+          if (st == B200TFS_OK && o.rank > B200TFS_MAX_RANK) st = B200TFS_E_NONCANONICAL;
+        }
+      }
+      cp.kst[(size_t)r * nk + k] = st;
+      cp.match[(size_t)r * nk + k] = m;
+      if (st == B200TFS_OK) atomicMin(&ref_rec, r);
+    }
+    __syncthreads();
+    const uint32_t rr = ref_rec;
+    const b200tfs_output* ro = rr < n ? cp.outs + (size_t)rr * cp.out_stride + cp.match[(size_t)rr * nk + k] : nullptr;
+    // pass B: consistency, offsets, tiles, items
+    uint64_t byte_carry = 0;
+    for (uint32_t r0 = 0; r0 < n; r0 += kConcatPlanThreads) {      // uniform trip count: the scans have barriers inside
+      const uint32_t r = r0 + threadIdx.x;
+      int32_t st = B200TFS_E_ARG;
+      const b200tfs_output* o = nullptr;
+      uint64_t bytes = 0;
+      if (r < n) {
+        st = cp.kst[(size_t)r * nk + k];
+        const int32_t m = cp.match[(size_t)r * nk + k];
+        if (m >= 0) o = cp.outs + (size_t)r * cp.out_stride + m;
+        if (st == B200TFS_OK) {
+          if (o->dtype != ro->dtype) st = B200TFS_E_DTYPE;
+          else if (o->rank != ro->rank) st = B200TFS_E_SHAPE;
+          else for (int32_t d = 1; d < o->rank; ++d) if (o->dims[d] != ro->dims[d]) st = B200TFS_E_SHAPE;
+        }
+        if (st == B200TFS_OK && dtype_info(o->dtype).kind == VK_STRING) st = B200TFS_E_NONCANONICAL;   // strings are decoded on the host
+        if (st == B200TFS_OK) bytes = tpl_narrows(cp.cast, o->dtype) ? o->n_elems * 2 : o->dst_bytes;
+      }
+      const uint64_t off = concat_scan(bytes, byte_carry, warp_sum);
+      if (st == B200TFS_OK && off + bytes > key.cap) st = B200TFS_E_SIZE;
+      uint32_t tiles = 0;
+      const bool narrow = st == B200TFS_OK && tpl_narrows(cp.cast, o->dtype);
+      if (st == B200TFS_OK && bytes && dtype_info(o->dtype).kind == VK_FIXED)   // OK fixed-width outputs with elements have value runs
+        for (int32_t q = 0; q < o->n_runs; ++q) tiles += tiles_for(((uint64_t)o->runs[q].len * o->runs[q].count) >> (narrow ? 1 : 0), cp.vpt);
+      const uint64_t first = concat_scan(tiles, tile_carry, warp_sum);
+      if (r < n) {
+        if (tiles && first + tiles > cp.tile_cap) st = B200TFS_E_NONCANONICAL;   // past the host's bound (never: concat_record_tile_bound)
+        if (st == B200TFS_OK && tiles) {
+          const uint8_t* rec = cp.w + cp.rec_off[r];
+          const uint32_t op = tpl_move_op(cp.cast, o->dtype);
+          uint64_t t = first, run = 0;
+          for (int32_t q = 0; q < o->n_runs; ++q) {
+            const b200tfs_run& rn = o->runs[q];
+            const uint64_t nb = ((uint64_t)rn.len * rn.count) >> (narrow ? 1 : 0);
+            const uint32_t nt = tiles_for(nb, cp.vpt), item = (uint32_t)(((uint64_t)r * nk + k) * B200TFS_MAX_RUNS + q);
+            items[item] = MoveItem{rec + rn.off, key.dst + off + run, nb, op, nt, rn.count > 1 ? rn.len : 0u, rn.count > 1 ? rn.stride : 0u};
+            for (uint32_t i = 0; i < nt && t + i < cp.tile_cap; ++i) tref[t + i] = TileRef{item, i};
+            t += nt;
+            run += nb;
+          }
+        }
+        b200tfs_output v{};
+        if (o) v = *o;
+        v.status = st;
+        v.dst_off = (uint64_t)(uintptr_t)(key.dst + off);
+        v.dst_bytes = bytes;
+        cp.vouts[(size_t)r * kFusedMaxOutputs + k] = v;
+        if (k == 0) { cp.vn_outs[r] = (int32_t)nk; cp.vrec_status[r] = B200TFS_OK; }
+      }
+    }
+  }
+  if (threadIdx.x == 0) {
+    PlanHeader ph{};
+    ph.n_items = (uint32_t)n_items;
+    ph.n_tiles = (uint32_t)min(tile_carry, (uint64_t)cp.tile_cap);
+    ph.vec_per_tile = cp.vpt;
+    ph.off_items = (uint32_t)((sizeof(PlanHeader) + 15) & ~15ull);
+    ph.off_tiles = (uint32_t)off_tiles;
+    ph.off_small = (uint32_t)off_tiles;
+    ph.guard_div = 1;
+    *reinterpret_cast<PlanHeader*>(cp.plan) = ph;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // frame_requests_kernel (plan.h "deferred framing"): one thread per request evaluates the request's values from the job
 // totals the counting kernel just produced, places the record in its slot (largest payload 128-byte aligned, like the host
 // planner's place_record), writes every framing byte and patches the destinations of the payload movers behind it.
@@ -1204,6 +1339,16 @@ cudaError_t launch_decode_fused(const FusedParams& fp, uint32_t grid, cudaStream
   }
   if (fp.vpt > kStageVecs) return launch_pdl(decode_fused_staged_kernel, grid, kMoveThreads, kFusedDynSmem, stream, fp);
   return launch_pdl(decode_fused_kernel, grid, kMoveThreads, 0, stream, fp);
+}
+
+cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStream_t stream) {
+  concat_plan_kernel<<<1, kConcatPlanThreads, 0, stream>>>(cp);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess || !move_grid) return e;
+  // a plain launch: move_kernel reads PlanHeader::independent before it waits on the kernel in front of it, and here that kernel
+  // writes the header
+  move_kernel<<<move_grid, kMoveThreads, 0, stream>>>((const uint8_t*)cp.plan);
+  return cudaGetLastError();
 }
 
 cudaError_t launch_move_guarded(const uint8_t* plan_dev, uint32_t n_tiles, cudaStream_t stream) {

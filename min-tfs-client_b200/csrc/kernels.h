@@ -42,5 +42,8 @@ cudaError_t launch_vdec_emit(const VarTables& tb, cudaStream_t stream);
 // the host's bound, tb.n_tiles_dev the real count; each kernel runs at most max_ctas CTAs and strides over the tiles)
 cudaError_t launch_vdec_plan(const VarPlan& vp, cudaStream_t stream);
 cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t stream);
+// b200tfs_decode_concat: concat_plan_kernel, then move_kernel over the plan image it wrote, with move_grid CTAs (the host's bound
+// on the tiles; the CTAs past the plan's own count leave at once)
+cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStream_t stream);
 
 }  // namespace b200tfs

@@ -204,6 +204,36 @@ struct VarPlan {
 // ceil((L + 15) / kVarTileBytes) windows, and the chunks lie inside the record
 constexpr uint64_t var_record_tile_bound(uint64_t len) { return len / kVarTileBytes + 2 + 2ull * kFusedMaxOutputs * B200TFS_MAX_RUNS; }
 
+// ---- decode into one tensor per key, concatenated along axis 0 (b200tfs_decode_concat) -----------------------------
+// concat_plan_kernel (one CTA) reads the parse kernel's table, matches the requested keys, scans every record's bytes into
+// its offset inside the key's destination and writes (a) a move plan image - PlanHeader | MoveItem[n * n_keys *
+// B200TFS_MAX_RUNS] (fixed slots) | TileRef[tile_cap] - that move_kernel runs over with a grid of tile_cap CTAs (the ones
+// past PlanHeader::n_tiles leave at once), and (b) a table in the single-launch decode's layout (kFusedMaxOutputs slots per
+// record, dst_off = the absolute destination address, dst_stride 0) that vdec_plan_kernel turns into packed-varint jobs.
+constexpr uint32_t kConcatPlanThreads = 1024;
+struct ConcatKeyDev { const uint8_t* key; uint8_t* dst; uint64_t cap; uint32_t key_len, pad; };
+struct ConcatPlan {
+  const uint8_t* w;                // wire arena
+  const uint64_t* rec_off;         // [n], device
+  const b200tfs_output* outs;      // parse table: record r at outs[r * out_stride]
+  const int32_t* n_outs;
+  const int32_t* rec_status;
+  const ConcatKeyDev* keys;        // [n_keys]
+  uint32_t n, n_keys, out_stride, cast;
+  uint32_t vpt, tile_cap;
+  int32_t* kst;                    // [n * n_keys] scratch: (record, key) status before the consistency checks
+  int32_t* match;                  // [n * n_keys] scratch: table index of the key in the record, -1 if absent
+  uint8_t* plan;                   // move plan image
+  b200tfs_output* vouts;           // [n * kFusedMaxOutputs]
+  int32_t* vn_outs;                // [n]
+  int32_t* vrec_status;            // [n]
+};
+// move tiles a record of `len` bytes can need for n_keys distinct outputs: every run of n_out <= its wire bytes takes at
+// most n_out / tile + 1 tiles, and a record holds at most B200TFS_MAX_RUNS runs per output
+constexpr uint64_t concat_record_tile_bound(uint64_t len, uint64_t tile_bytes, uint32_t n_keys) {
+  return len / tile_bytes + 1ull + (uint64_t)n_keys * B200TFS_MAX_RUNS;
+}
+
 // ---- deferred framing: the length prefixes of packed-varint inputs computed ON THE DEVICE -----------------------------
 // Every length on the wire precedes its content, and a packed-varint payload's length is only known once the counting
 // kernel has run.  Instead of bringing it to the host (b200tfs_measure: a stream synchronise in the middle of an encode),

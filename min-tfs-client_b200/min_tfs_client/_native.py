@@ -27,7 +27,7 @@ RF_GRPC_FRAME = 0x1
 OF_TENSOR_CONTENT, OF_MULTI_CHUNK, OF_DIM_INFERRED, OF_HAS_UNKNOWN, OF_RANK0, OF_VARINT, OF_PAD_EDGE = 0x1, 0x2, 0x4, 0x8, 0x10, 0x20, 0x40
 OF_UNPACKED, OF_SPILLED, OF_DEVICE_VARINT = 0x80, 0x100, 0x200
 ORDER_GIVEN, ORDER_UPB, ORDER_BYTES = 0, 1, 2
-MAX_RANK, MAX_RUNS, FUSED_MAX_OUTPUTS = 16, 8, 8
+MAX_RANK, MAX_RUNS, FUSED_MAX_OUTPUTS, CONCAT_MAX_KEYS = 16, 8, 8, 8
 DT_HALF_REFQUIRK = -19
 
 
@@ -74,6 +74,14 @@ class ModelSpec(C.Structure):
     _fields_ = [
         ("name_off", C.c_uint64), ("name_len", C.c_uint32), ("signature_len", C.c_uint32), ("signature_off", C.c_uint64),
         ("label_off", C.c_uint64), ("label_len", C.c_uint32), ("has_version", C.c_int32), ("version", C.c_int64),
+    ]
+
+
+class ConcatKey(C.Structure):
+    """b200tfs_concat_key: one requested output of b200tfs_decode_concat (in: key, dst, dst_cap; out: the layout)."""
+    _fields_ = [
+        ("key", C.c_char_p), ("key_len", C.c_int64), ("dst", C.c_void_p), ("dst_cap", C.c_uint64), ("dtype", C.c_int32),
+        ("rank", C.c_int32), ("dims", C.c_int64 * MAX_RANK), ("bytes", C.c_uint64), ("status", C.c_int32), ("bad_rec", C.c_int32),
     ]
 
 
@@ -131,6 +139,11 @@ SIGNATURES = {
     "b200tfs_decode_responses": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64]),
     "b200tfs_decode_results": (C.c_int, [_vp, C.c_int32, C.POINTER(Output), _i32p, C.POINTER(ModelSpec), _i32p]),
     "b200tfs_decode_stats": (C.c_int, [_vp, _u64p, _u64p, _u64p]),
+    "b200tfs_concat_layout": (C.c_int, [_vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(ConcatKey), C.c_int32]),
+    "b200tfs_response_keys": (C.c_int, [_vp, C.c_uint64, C.c_int32, _u64p, C.POINTER(C.c_uint32), _i32p]),
+    "b200tfs_decode_concat": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(ConcatKey)]),
+    "b200tfs_decode_concat_host_async": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(ConcatKey)]),
+    "b200tfs_concat_results": (C.c_int, [_vp, C.c_int32, C.c_int32, C.POINTER(Output), C.POINTER(ModelSpec), _i32p]),
     "b200tfs_capture_begin": (C.c_int, [_vp]),
     "b200tfs_capture_end": (C.c_int, [_vp, _vpp]),
     "b200tfs_graph_launch": (C.c_int, [_vp, _vp]),

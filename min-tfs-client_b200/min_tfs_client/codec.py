@@ -219,6 +219,8 @@ class Codec:
         # unpack route and float-only traffic pays nothing; from then on every call sizes its slots from its own records
         # (_slot_stride) and the launch decodes varint outputs too when they have some (b200tfs_set_decode_varints)
         self._seen_varints = False
+        # decode_predict_responses_concat calls the device route finished (the others were decoded response by response)
+        self.concat_device_calls = 0
 
     def close(self):
         if getattr(self, "_ctx", None):
@@ -511,6 +513,11 @@ class Codec:
                 fused = self._decode_fused(wires, strict, cast=(next(iter(wanted)), dict(out_dtypes)))
                 if fused is not None:
                     return fused
+        return self._decode_two_phase(wires, strict, out_dtypes, max_outputs)
+
+    def _decode_two_phase(self, wires, strict, out_dtypes, max_outputs, keys=None):
+        """The parse kernel, then the unpack of every output - of the outputs named in `keys` only, when given (the others are
+        neither converted nor checked)."""
         parsed = self.parse_predict_responses(wires, max_outputs=max_outputs)
         if not parsed:
             return []
@@ -519,6 +526,8 @@ class Codec:
         for i, pr in enumerate(parsed):
             results.append(({}, pr.model_spec))
             for key, o in pr.outputs.items():
+                if keys is not None and key not in keys:
+                    continue
                 od = out_dtypes.get(key) if out_dtypes else None
                 if int(o.dtype) == DT_STRING and o.status == N.OK:
                     results[i][0][key] = self._decode_strings(pr.wire, pr.offset, o, pr.length, key)
@@ -662,6 +671,205 @@ class Codec:
                 N.check(st[k])
                 results[i][0][key] = made[k]
         return results
+
+    # ---- batch decode into one tensor per key ------------------------------------------------------
+    def decode_predict_responses_concat(self, wires: Sequence[bytes], keys: Optional[Sequence[str]] = None, *, strict: bool = False,
+                                        out_dtypes: Optional[Mapping] = None, device: bool = False,
+                                        out: Optional[Mapping] = None) -> Tuple[Dict[str, object], List[DecodedSpec]]:
+        """Decode a batch of PredictResponses into ONE tensor per output: for every key, the outputs of all responses
+        concatenated along axis 0 - ``np.concatenate([decode_predict_responses([w], ...)[0][0][key] for w in wires], axis=0)``,
+        bit for bit and with the same exceptions, except that outputs of different dtypes raise ValueError instead of being
+        promoted, and that outputs which are not requested are not decoded (an error confined to them does not raise).
+
+        ``keys=None``: every key of the first response.  ``device=True`` returns ``DeviceArray``s (``__cuda_array_interface__``:
+        ``torch.as_tensor(a, device="cuda")`` takes them without a copy); otherwise numpy arrays, one device-to-host copy per
+        key.  ``out={key: array}`` writes in place: a C-contiguous device array (CUDA array interface / DLPack) or a numpy /
+        ``pinned_empty`` array of exactly the result's dtype and shape.  Returns ``({key: tensor}, [DecodedSpec per response])``.
+        """
+        n = len(wires)
+        if n == 0:
+            raise ValueError("need at least one response to concatenate")
+        out = dict(out or {})
+        buf, off, ln = self._pack_wires(wires)
+        if keys is None:
+            keys = self._response_keys(buf, int(off[0]), int(ln[0]))
+            if keys is None:      # the first response does not parse: the parse raises what the reference raises
+                self.parse_predict_responses(wires[:1])
+                from google.protobuf.message import DecodeError
+
+                raise DecodeError("Error parsing message (response 0)")
+        keys = list(dict.fromkeys(keys))
+        for k in out:
+            if k not in keys:
+                raise KeyError(k)
+        if out_dtypes:        # only the requested outputs are decoded: entries for other keys play no part
+            out_dtypes = {k: v for k, v in out_dtypes.items() if k in keys} or None
+        fast = self._concat_device(wires, buf, off, ln, keys, strict, out_dtypes, device, out) if len(keys) <= N.CONCAT_MAX_KEYS else None
+        if fast is not None:
+            return fast
+        return self._concat_per_record(wires, keys, strict, out_dtypes, device, out)
+
+    def _response_keys(self, buf, base: int, length: int) -> Optional[List[str]]:
+        cap = 64
+        while True:
+            ko, kl, cnt = (C.c_uint64 * cap)(), (C.c_uint32 * cap)(), C.c_int32()
+            rc = self._lib.b200tfs_response_keys(buf.ctypes.data + base, length, cap, ko, kl, C.byref(cnt))
+            if rc != N.OK:
+                return None
+            if cnt.value <= cap:
+                return [self._text(buf, base + int(ko[i]), int(kl[i])) for i in range(cnt.value)]
+            cap = cnt.value
+
+    def _concat_per_record(self, wires, keys, strict, out_dtypes, device, out):
+        """The definition itself, response by response, for the requested outputs: what the device route hands over when a batch
+        holds a case it does not take (a malformed record, more than FUSED_MAX_OUTPUTS outputs or MAX_RANK dims, TF padding,
+        tensor_content only, strings, mismatches).  Like the device route it converts and checks the requested outputs only."""
+        wanted = set(keys)
+        per = [self._decode_two_phase([w], strict, out_dtypes, 16, wanted)[0] for w in wires]
+        result = {}
+        for k in dict.fromkeys(keys):
+            parts = [p[0][k] for p in per]
+            if any(a.ndim == 0 for a in parts):
+                raise ValueError("zero-dimensional arrays cannot be concatenated")
+            if len({a.dtype for a in parts}) > 1:
+                raise ValueError(f"output {k!r}: responses disagree on the dtype ({', '.join(sorted({str(a.dtype) for a in parts}))})")
+            cat = np.concatenate(parts, axis=0)
+            if device and cat.dtype.kind in "US":
+                raise TypeError(f"output {k!r}: string tensors are decoded on the host")
+            result[k] = self._concat_deliver(k, cat, device, out)
+        return result, [p[1] for p in per]
+
+    def _concat_deliver(self, key, arr: np.ndarray, device: bool, out):
+        dst = out.get(key)
+        if dst is None:
+            return self.device_array(arr) if device else arr
+        if D.is_device_object(dst):
+            ptr, shape, dtype, _keep = D.device_view(dst)
+            if dtype != arr.dtype or tuple(shape) != arr.shape:
+                raise ValueError(f"out[{key!r}]: {dtype}{tuple(shape)} does not match the decoded {arr.dtype}{arr.shape}")
+            if arr.nbytes:
+                a = np.ascontiguousarray(arr)
+                N.check(self._lib.b200tfs_memcpy_h2d(self._ctx, ptr, a.ctypes.data, a.nbytes))
+                self.sync()
+            return dst
+        if not isinstance(dst, np.ndarray) or dst.dtype != arr.dtype or dst.shape != arr.shape:
+            raise ValueError(f"out[{key!r}] does not match the decoded {arr.dtype}{arr.shape}")
+        np.copyto(dst, arr)
+        return dst
+
+    def _concat_device(self, wires, buf, off, ln, keys, strict, out_dtypes, device, out):
+        """The device route (b200tfs_decode_concat): parse, one-CTA plan, move, varint decode - or None when the batch holds
+        a case it leaves to the per-response route."""
+        n, nk = len(wires), len(keys)
+        kb = [k.encode("utf-8") for k in keys]
+        cast_code = 0
+        if out_dtypes:
+            if strict:
+                return None
+            try:
+                wanted = {int(enum_for_numpy(np.dtype(v).type)) for v in out_dtypes.values()}
+            except (KeyError, ValueError, TypeError):
+                return None
+            if len(wanted) != 1 or next(iter(wanted)) not in (int(DT_HALF), int(DT_BFLOAT16)):
+                return None
+            cast_code = next(iter(wanted))
+        ck = (N.ConcatKey * nk)()
+        for i, k in enumerate(kb):
+            ck[i].key, ck[i].key_len = k, len(k)
+        N.check(self._lib.b200tfs_concat_layout(buf.ctypes.data, n, off, ln, nk, ck, cast_code))
+        shapes, np_types = [], []
+        for i in range(nk):
+            c = ck[i]
+            if c.status != N.OK or c.dtype == DT_STRING:
+                return None
+            if strict and (c.dtype == DT_BFLOAT16 or c.dtype in (DT_COMPLEX64, DT_COMPLEX128)):
+                return None
+            if cast_code and ((c.dtype == DT_FLOAT) != (keys[i] in out_dtypes)):
+                return None       # the narrowing applies to every float32 output: only right when exactly those asked for it
+            shapes.append(tuple(int(c.dims[d]) for d in range(c.rank)))
+            np_types.append(np.dtype(numpy_for_enum(cast_code if cast_code and c.dtype == DT_FLOAT else int(c.dtype))))
+        # destinations: the caller's device arrays, else device arrays of our own (returned, or copied into the host result)
+        dev, ptrs, holds = [], [], []
+        for i, k in enumerate(keys):
+            dst = out.get(k)
+            if dst is not None and D.is_device_object(dst):
+                ptr, shape, dtype, keep = D.device_view(dst)
+                if dtype != np_types[i] or tuple(shape) != shapes[i]:
+                    raise ValueError(f"out[{k!r}]: {dtype}{tuple(shape)} does not match the decoded {np_types[i]}{shapes[i]}")
+                dev.append(dst)
+                ptrs.append(ptr)
+                holds.append(keep)
+            else:
+                if dst is not None and (not isinstance(dst, np.ndarray) or dst.dtype != np_types[i] or dst.shape != shapes[i] or
+                                        not dst.flags.c_contiguous):
+                    raise ValueError(f"out[{k!r}] does not match the decoded {np_types[i]}{shapes[i]}")
+                a = D.DeviceArray(self, shapes[i], np_types[i])
+                dev.append(a)
+                ptrs.append(a.ptr)
+            ck[i].dst, ck[i].dst_cap = ptrs[i], int(ck[i].bytes)
+        wire = D.DeviceArray(self, (len(buf),), np.uint8).copy_from_host(buf)
+        if cast_code:
+            N.check(self._lib.b200tfs_set_decode_cast(self._ctx, cast_code))
+        try:
+            N.check(self._lib.b200tfs_decode_concat(self._ctx, wire.ptr, n, off, ln, nk, ck))
+        finally:
+            if cast_code:
+                N.check(self._lib.b200tfs_set_decode_cast(self._ctx, 0))
+        outs, specs, rec_status = (N.Output * (n * nk))(), (N.ModelSpec * n)(), (C.c_int32 * n)()
+        N.check(self._lib.b200tfs_concat_results(self._ctx, n, nk, outs, specs, rec_status))   # synchronises
+        raw = np.frombuffer(outs, dtype=np.uint8).reshape(n * nk, C.sizeof(N.Output))
+        status = raw[:, N.Output.status.offset: N.Output.status.offset + 4].copy().view(np.int32).ravel()
+        redo = set(np.flatnonzero(status != N.OK).tolist())
+        if strict:     # the reference reads half_val as VALUES; the device wrote TF's bit patterns
+            for i in range(nk):
+                if ck[i].dtype == DT_HALF:
+                    redo.update(r * nk + i for r in range(n))
+        jobs = []
+        for j in sorted(redo):
+            r, i = divmod(j, nk)
+            o = outs[j]
+            if rec_status[r] != N.OK:
+                return None
+            if o.flags & N.OF_DEVICE_VARINT:
+                o.flags &= ~N.OF_DEVICE_VARINT    # finished below by the unpack route, which raises what it raises today
+                o.status = N.OK
+            elif o.status == N.E_NONCANONICAL:
+                o.status = N.OK
+            elif o.status != N.OK:
+                return None
+            _, dst_code, _ = self._resolve_output(o, strict, out_dtypes.get(keys[i]) if out_dtypes else None)
+            if o.n_elems:
+                jobs.append((j, r, ptrs[i] + int(o.dst_off), dst_code))
+        if jobs:
+            m = len(jobs)
+            o_arr = (N.Output * m)(*[outs[j[0]] for j in jobs])
+            rec = (C.c_uint64 * m)(*[int(off[j[1]]) for j in jobs])
+            dd = (C.c_void_p * m)(*[j[2] for j in jobs])
+            codes = (C.c_int32 * m)(*[j[3] for j in jobs])
+            st = (C.c_int32 * m)()
+            N.check(self._lib.b200tfs_unpack_outputs(self._ctx, wire.ptr, m, o_arr, rec, dd, codes, st))
+            if any(st[q] != N.OK for q in range(m)):
+                return None
+        result = {}
+        for i, k in enumerate(keys):
+            dst = out.get(k)
+            if dst is not None and D.is_device_object(dst):
+                result[k] = dst
+            elif dst is not None or not device:
+                host = dst if dst is not None else np.empty(shapes[i], dtype=np_types[i])
+                if host.nbytes:
+                    N.check(self._lib.b200tfs_memcpy_d2h(self._ctx, host.ctypes.data, ptrs[i], host.nbytes))
+                result[k] = host
+            else:
+                result[k] = dev[i]
+        self.sync()
+        self.concat_device_calls += 1
+        spec_list = []
+        for r in range(n):
+            base, s = int(off[r]), specs[r]
+            spec_list.append(DecodedSpec(self._text(buf, base + s.name_off, s.name_len), int(s.version), bool(s.has_version),
+                                         self._text(buf, base + s.label_off, s.label_len), self._text(buf, base + s.signature_off, s.signature_len)))
+        return result, spec_list
 
     @staticmethod
     def _decode_strings(buf: np.ndarray, base: int, o: N.Output, rec_len: int = 0, key: str = "") -> np.ndarray:
