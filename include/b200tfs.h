@@ -528,6 +528,60 @@ int b200tfs_unpack_outputs_host(b200tfs_ctx* ctx, int32_t m, const b200tfs_outpu
                                 const uint64_t* out_rec_off, void* const* dst_host,
                                 const int32_t* dst_dtype, int32_t* status);
 
+/* ---- Classify / Regress requests: a batch of tf.Examples from columnar arrays -----------------------
+ * What requests.py examples_from_input_dict + TensorServingClient._make_example_request build, serialised with
+ * SerializeToString(deterministic=True).  ClassificationRequest and RegressionRequest share their field numbers (model_spec = 1,
+ * input = 2), so one set of bytes serves both RPCs.  Row i of every column is example i, flattened in C order; the feature map of
+ * every example lists the columns in `order` (B200TFS_ORDER_UPB: what deterministic serialisation gives).  Floating columns
+ * (DT_FLOAT, DT_DOUBLE, DT_HALF) become float_list the way astype(float32) and a Python float make them: float32 signalling NaNs
+ * quieted; float64 rounded to nearest even, NaN -> sign | 0x7FC00000 | (mantissa >> 29); float16 widened exactly, NaNs quieted.
+ * Integer and bool columns become int64_list: sign-extended, uint64 wraps (2**64-1 is written as -1), a bool byte != 0 is 1.
+ * A row of 0 elements still writes its empty list.  Strings (bytes_list) are not taken: such requests are assembled on the host. */
+#define B200TFS_F_BROADCAST 0x10u     /* b200tfs_feature.flags: a 0-d column, whose one row is repeated in every example            */
+typedef struct b200tfs_feature {
+  const void* data;     /* n_examples rows of row_elems elements (one row with B200TFS_F_BROADCAST), C-contiguous, native order,
+                           aligned to the element size; a DEVICE pointer for the _async entry point                              */
+  int32_t src_dtype;    /* DT_FLOAT / DT_DOUBLE / DT_HALF / DT_INT8..64 / DT_UINT8..64 / DT_BOOL; others: B200TFS_E_DTYPE         */
+  uint32_t flags;       /* B200TFS_F_DEVICE_DATA (the _host entry point: `data` is in HBM already), B200TFS_F_BROADCAST           */
+  int64_t row_elems;    /* elements per example                                                                                 */
+  const char* key;      /* feature name bytes (UTF-8, not NUL terminated)                                                       */
+  int64_t key_len;
+} b200tfs_feature;
+
+typedef struct b200tfs_example_request {
+  const char* model_name;
+  int64_t model_name_len;
+  int32_t has_version;  /* model_version is not None                                                                            */
+  int32_t order;        /* B200TFS_ORDER_*: order of the features inside every example                                          */
+  int64_t version;
+  int64_t n_examples;   /* >= 0; an example has at least one feature                                                            */
+  int32_t n_features;
+  int32_t flags;        /* B200TFS_RF_GRPC_FRAME                                                                                */
+  const b200tfs_feature* features;
+} b200tfs_example_request;
+
+/* Exact wire length (host, closed form) of a request without integer columns - replaces building the request with
+ * requests.py examples_from_input_dict / _make_example_request and asking the message for ByteSize().  A request with an
+ * integer column: B200TFS_E_ARG (its length depends on the values).  Over 2 GiB: B200TFS_E_TOOBIG.                       */
+int b200tfs_example_request_size(const b200tfs_example_request* r, uint64_t* total_len);
+/* Arena bytes b200tfs_encode_example_requests_async needs: one 256-byte aligned slot per request, sized for its worst case
+ * (10 bytes per integer element).  A request that cannot stay under 2 GiB whatever its values: B200TFS_E_TOOBIG.       */
+int b200tfs_example_arena_size(int32_t n, const b200tfs_example_request* reqs, uint64_t* bytes);
+/* Encode n requests from DEVICE columns into the device arena (256-byte aligned; b200tfs_example_arena_size bytes) - what
+ * requests.py examples_from_input_dict + _make_example_request + SerializeToString(deterministic=True) produce.  Kernels only:
+ * count (requests with an integer column: packed lengths and example sizes), scan (example offsets), emit (framing and values,
+ * one contiguous range of examples and of wire per CTA), frame (the request prefix, written in front of the examples once
+ * their total is known).  Never synchronises and is graph-capturable; a replay adapts to new integer values.  Collect rec_off /
+ * rec_len with b200tfs_encode_results (a request over 2 GiB: B200TFS_E_TOOBIG).                                          */
+int b200tfs_encode_example_requests_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, void* arena_dev,
+                                          uint64_t arena_cap);
+/* The same from HOST columns (pinned or pageable; B200TFS_F_DEVICE_DATA columns are read in place): the columns are copied to
+ * the device, encoded, and the records copied back into wire_host (capacity wire_cap: b200tfs_example_arena_size bytes are
+ * always enough); rec_off / rec_len count from wire_host.  Synchronous.  Replaces requests.py examples_from_input_dict +
+ * _make_example_request + SerializeToString.                                                                              */
+int b200tfs_encode_example_requests_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, void* wire_host,
+                                         uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
+
 #ifdef __cplusplus
 }
 #endif

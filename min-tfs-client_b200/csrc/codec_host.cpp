@@ -2363,3 +2363,4 @@ int b200tfs_concat_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_ou
 // varint dtypes (phase 2: kernels in kernels.cu; wired here)
 // ------------------------------------------------------------------------------------------------
 #include "varint_host.inc"
+#include "example_host.inc"

@@ -1,0 +1,278 @@
+// example_kernels.cuh - Classify / Regress requests: a batch of tf.Examples from columnar arrays (plan.h ExTables; planned by
+// example_host.inc).  Included by kernels.cu inside namespace b200tfs, after concat_scan.
+//
+//   ex_count_kernel  requests with an integer column: one warp per example finds the packed length of every integer row, then
+//                    the example's byte length through its nested lengths (list <- Feature <- map entry <- Features <- Example);
+//                    one CTA per kExTile examples leaves their sum in tile_sum
+//   ex_scan_kernel   the same tiles: the tile's offset is the sum of the tiles before it in its request (read, never waited
+//                    for: the count kernel has finished), then a block scan of the example sizes gives every example's offset
+//   ex_emit_kernel   one CTA per contiguous range of examples, i.e. of wire: warps write whole examples (framing, converted float
+//                    rows, int64 varints) into a shared-memory image of the wire, which the CTA stores with aligned 128-bit
+//                    vectors; an example larger than the image is written in place by one warp
+//   ex_frame_kernel  one warp per request: the examples' total, the request prefix in front of the anchor, rec_off / rec_len /
+//                    status to pinned memory
+//
+// What the reference does here: requests.py examples_from_input_dict (a Python loop per example and per feature) and the
+// protobuf runtime serialising the ClassificationRequest / RegressionRequest it filled.
+
+// float32 bits of element j of a float row: what astype(float32) and the trip through a Python float give
+__device__ __forceinline__ uint32_t ex_f64_to_f32_bits(uint64_t d) {
+  if ((d & 0x7FFFFFFFFFFFFFFFull) > 0x7FF0000000000000ull)      // NaN: quieted, the top 22 payload bits kept (x86 cvtsd2ss)
+    return ((uint32_t)(d >> 32) & 0x80000000u) | 0x7FC00000u | (uint32_t)((d & 0x000FFFFFFFFFFFFFull) >> 29);
+  return __float_as_uint(__double2float_rn(__longlong_as_double((long long)d)));
+}
+__device__ __forceinline__ uint32_t ex_float_bits(const ExFeat& f, const uint8_t* row, uint64_t j) {
+  if (f.op == EXO_F32) return quiet_f32(*reinterpret_cast<const uint32_t*>(row + 4 * j));
+  if (f.op == EXO_F64) return ex_f64_to_f32_bits(*reinterpret_cast<const unsigned long long*>(row + 8 * j));
+  return widen_f16(*reinterpret_cast<const uint16_t*>(row + 2 * j));
+}
+// element of an integer row as astype(int64) gives it (bool: any nonzero byte is 1)
+__device__ __forceinline__ uint64_t ex_int(const ExFeat& f, const uint8_t* p) {
+  switch (f.esz) {
+    case 1: { const uint8_t t = *p; return f.op == EXO_BOOL ? (uint64_t)(t != 0) : f.sgn ? (uint64_t)(int64_t)(int8_t)t : t; }
+    case 2: { const uint16_t t = *reinterpret_cast<const uint16_t*>(p); return f.sgn ? (uint64_t)(int64_t)(int16_t)t : t; }
+    case 4: { const uint32_t t = *reinterpret_cast<const uint32_t*>(p); return f.sgn ? (uint64_t)(int64_t)(int32_t)t : t; }
+    default: return *reinterpret_cast<const unsigned long long*>(p);
+  }
+}
+__device__ __forceinline__ uint64_t ex_payload(const ExTables& T, const ExReq& q, const ExFeat& f, uint64_t i) {
+  return f.op < EXO_INT ? 4 * f.row_elems : T.L[q.L0 + i * q.n_int + f.lcol];
+}
+__device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
+#pragma unroll
+  for (int d = 16; d; d >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, d);
+  return v;
+}
+
+// Example i of request q, written by the calling warp at w (shared or global memory).
+__device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, uint8_t* w) {
+  const uint32_t lane = threadIdx.x & 31;
+  uint64_t F = 0, hl;
+  for (uint32_t c = 0; c < q.n_feat; c += 32) {     // map entries, one feature per lane
+    uint64_t e = 0;
+    if (c + lane < q.n_feat) {
+      const ExFeat& f = T.feats[q.first_feat + c + lane];
+      e = ex_entry_len(ex_payload(T, q, f, i), f.key_len, &hl);
+    }
+    F += warp_sum64(e);
+  }
+  const uint64_t X = 1 + varint_len(F) + F;
+  uint64_t pos = 2 + varint_len(X) + varint_len(F);
+  if (lane == 0) {
+    w[0] = 0x0A;
+    const uint32_t p = 1 + put_varint(w + 1, X);
+    w[p] = 0x0A;
+    put_varint(w + p + 1, F);
+  }
+  for (uint32_t c = 0; c < q.n_feat; c += 32) {
+    const uint32_t k = c + lane;
+    uint64_t e = 0, P = 0;
+    hl = 0;
+    if (k < q.n_feat) {
+      const ExFeat f = T.feats[q.first_feat + k];
+      P = ex_payload(T, q, f, i);
+      e = ex_entry_len(P, f.key_len, &hl);
+    }
+    uint64_t inc = e;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint64_t x = __shfl_up_sync(0xFFFFFFFFu, inc, d);
+      if (lane >= (uint32_t)d) inc += x;
+    }
+    const uint64_t at = pos + inc - e;
+    if (k < q.n_feat) {       // 0A vi(entry) 0A vi(klen) key 12 vi(Feature) {12|1A} vi(list) [0A vi(P)]
+      const ExFeat& f = T.feats[q.first_feat + k];
+      const uint64_t list = P ? 1 + varint_len(P) + P : 0, feature = 1 + varint_len(list) + list;
+      uint8_t* h = w + at;
+      const uint64_t entry = 1 + varint_len(f.key_len) + f.key_len + 1 + varint_len(feature) + feature;
+      *h++ = 0x0A; h += put_varint(h, entry);
+      *h++ = 0x0A; h += put_varint(h, f.key_len);
+      for (uint32_t b = 0; b < f.key_len; ++b) *h++ = T.blob[f.key_off + b];
+      *h++ = 0x12; h += put_varint(h, feature);
+      *h++ = f.op < EXO_INT ? 0x12 : 0x1A; h += put_varint(h, list);
+      if (P) { *h++ = 0x0A; put_varint(h, P); }
+    }
+    const uint32_t nk = min(32u, q.n_feat - c);
+    for (uint32_t s = 0; s < nk; ++s) {             // the rows, one after the other, by the whole warp
+      const uint64_t Ps = __shfl_sync(0xFFFFFFFFu, P, s);
+      const uint64_t ps = __shfl_sync(0xFFFFFFFFu, at + hl, s);
+      if (!Ps) continue;
+      const ExFeat f = T.feats[q.first_feat + c + s];
+      const uint8_t* row = f.data + i * f.row_stride;
+      uint8_t* d = w + ps;
+      if (f.op < EXO_INT) {
+        for (uint64_t j = lane; j < f.row_elems; j += 32) {
+          const uint32_t b = ex_float_bits(f, row, j);
+          d[4 * j] = (uint8_t)b; d[4 * j + 1] = (uint8_t)(b >> 8); d[4 * j + 2] = (uint8_t)(b >> 16); d[4 * j + 3] = (uint8_t)(b >> 24);
+        }
+      } else {
+        uint64_t base = 0;
+        for (uint64_t j0 = 0; j0 < f.row_elems; j0 += 32) {
+          const uint64_t j = j0 + lane;
+          uint64_t v = 0;
+          uint32_t len = 0;
+          if (j < f.row_elems) { v = ex_int(f, row + j * f.esz); len = vlen64(v); }
+          uint32_t incl = len;
+#pragma unroll
+          for (int dd = 1; dd < 32; dd <<= 1) {
+            const uint32_t x = __shfl_up_sync(0xFFFFFFFFu, incl, dd);
+            if (lane >= (uint32_t)dd) incl += x;
+          }
+          if (len) put_varint(d + base + incl - len, v);
+          base += __shfl_sync(0xFFFFFFFFu, incl, 31);
+        }
+      }
+    }
+    pos += __shfl_sync(0xFFFFFFFFu, inc, 31);
+  }
+}
+
+__global__ void __launch_bounds__(kExTile) ex_count_kernel(const __grid_constant__ ExTables T) {
+  __shared__ unsigned long long warp_sum[kExTile / 32];
+  const ExSpan sp = T.tiles[blockIdx.x];
+  const ExReq q = T.reqs[sp.req];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint64_t mine = 0;
+  for (uint64_t i = sp.e0 + warp; i < sp.e1; i += kExTile / 32) {
+    uint64_t F = 0, hl;
+    for (uint32_t k = 0; k < q.n_feat; ++k) {
+      const ExFeat f = T.feats[q.first_feat + k];
+      uint64_t P = 4 * f.row_elems;
+      if (f.op >= EXO_INT) {
+        const uint8_t* row = f.data + i * f.row_stride;
+        uint64_t s = 0;
+        for (uint64_t j = lane; j < f.row_elems; j += 32) s += vlen64(ex_int(f, row + j * f.esz));
+        P = warp_sum64(s);
+        if (lane == 0) T.L[q.L0 + i * q.n_int + f.lcol] = P;
+      }
+      F += ex_entry_len(P, f.key_len, &hl);
+    }
+    const uint64_t S = ex_example_len(F);
+    if (lane == 0) { T.S[q.ex0 + i] = S; mine += S; }
+  }
+  uint64_t total = 0;
+  concat_scan(mine, total, warp_sum);
+  if (threadIdx.x == 0) T.tile_sum[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(kExTile) ex_scan_kernel(const __grid_constant__ ExTables T) {
+  __shared__ unsigned long long warp_sum[kExTile / 32];
+  const uint32_t t = blockIdx.x;
+  const ExSpan sp = T.tiles[t];
+  const ExReq q = T.reqs[sp.req];
+  uint64_t carry = 0;
+  for (uint32_t k0 = q.first_tile; k0 < t; k0 += kExTile) {     // the tiles in front of this one (uniform trip count)
+    const uint32_t k = k0 + threadIdx.x;
+    concat_scan(k < t ? (uint64_t)T.tile_sum[k] : 0ull, carry, warp_sum);
+  }
+  const uint64_t i = sp.e0 + threadIdx.x;
+  const uint64_t o = concat_scan(i < sp.e1 ? T.S[q.ex0 + i] : 0ull, carry, warp_sum);
+  if (i < sp.e1) T.off[q.ex0 + i] = o;
+}
+
+// where example i of request q starts / ends, from the anchor
+__device__ __forceinline__ uint64_t ex_start(const ExTables& T, const ExReq& q, uint64_t i) {
+  return q.n_int ? T.off[q.ex0 + i] : i * q.fixed_size;
+}
+__device__ __forceinline__ uint64_t ex_end(const ExTables& T, const ExReq& q, uint64_t i) {
+  return q.n_int ? T.off[q.ex0 + i] + T.S[q.ex0 + i] : (i + 1) * q.fixed_size;
+}
+
+// Store arena bytes [lo, hi) from the image img of the wire that starts at arena offset ws (16-byte aligned): the whole aligned
+// vectors with 128-bit stores, the bytes of a partial vector at either end (which the neighbouring range shares) one by one.
+__device__ __forceinline__ void ex_flush(uint8_t* arena, const uint8_t* img, uint64_t ws, uint64_t lo, uint64_t hi) {
+  if (hi <= lo) return;
+  const uint64_t a = min((uint64_t)((lo + 15) & ~15ull), hi), b = max((uint64_t)(hi & ~15ull), a);
+  for (uint64_t x = lo + threadIdx.x; x < a; x += blockDim.x) arena[x] = img[x - ws];
+  for (uint64_t x = a + 16ull * threadIdx.x; x < b; x += 16ull * blockDim.x)
+    st_stream(arena + x, *reinterpret_cast<const uint4*>(img + (x - ws)));
+  for (uint64_t x = b + threadIdx.x; x < hi; x += blockDim.x) arena[x] = img[x - ws];
+}
+
+__global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_constant__ ExTables T) {
+  __shared__ __align__(16) uint8_t img[kExStage + 16];
+  __shared__ uint64_t next;
+  constexpr uint32_t kWarps = kExEmitThreads / 32;
+  const ExSpan sp = T.spans[blockIdx.x];
+  const ExReq q = T.reqs[sp.req];
+  const uint32_t warp = threadIdx.x >> 5;
+  const uint64_t A = q.anchor;
+  uint64_t lo = A + ex_start(T, q, sp.e0);   // first byte not stored yet
+  uint64_t ws = lo & ~15ull;                 // arena offset of img[0]
+  uint64_t i = sp.e0;
+  while (i < sp.e1) {
+    if (threadIdx.x == 0) {                  // the longest run of examples from i whose bytes fit the image
+      uint64_t g = i, h = sp.e1;
+      while (g < h) {
+        const uint64_t m = (g + h + 1) / 2;
+        if (A + ex_end(T, q, m - 1) - ws <= kExStage) g = m; else h = m - 1;
+      }
+      next = g;
+    }
+    __syncthreads();
+    const uint64_t j = next;
+    if (j > i) {
+      for (uint64_t e = i + warp; e < j; e += kWarps) ex_write_example(T, q, e, img + (A + ex_start(T, q, e) - ws));
+      __syncthreads();
+      const uint64_t be = A + ex_end(T, q, j - 1), cut = be & ~15ull;
+      if (cut > ws) {                        // store every whole vector; the partial one moves to the front of the image
+        ex_flush(T.arena, img, ws, lo, cut);
+        const uint8_t t = threadIdx.x < be - cut ? img[cut - ws + threadIdx.x] : 0;
+        __syncthreads();
+        if (threadIdx.x < be - cut) img[threadIdx.x] = t;
+        ws = lo = cut;
+      }
+      i = j;
+    } else {                                 // example i alone is larger than the image: one warp writes it in place
+      ex_flush(T.arena, img, ws, lo, A + ex_start(T, q, i));
+      if (warp == 0) ex_write_example(T, q, i, T.arena + A + ex_start(T, q, i));
+      lo = A + ex_end(T, q, i);
+      ws = lo & ~15ull;
+      ++i;
+    }
+    __syncthreads();
+  }
+  ex_flush(T.arena, img, ws, lo, A + ex_end(T, q, sp.e1 - 1));
+}
+
+constexpr uint32_t kExFrameWarps = 4;
+__global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __grid_constant__ ExTables T) {
+  const uint32_t r = blockIdx.x * kExFrameWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= T.n_req) return;
+  const ExReq q = T.reqs[r];
+  uint64_t el = 0;
+  if (q.n_int) {
+    for (uint32_t k = lane; k < q.n_tiles; k += 32) el += T.tile_sum[q.first_tile + k];
+    el = warp_sum64(el);
+  } else {
+    el = q.n_ex * q.fixed_size;
+  }
+  if (lane) return;
+  // [00 be32(msg)] model_spec 12 vi(input) 0A vi(example_list) | examples...
+  const uint64_t input = 1 + varint_len(el) + el, msg = q.spec_len + 1 + varint_len(input) + input;
+  const uint64_t pre = (q.grpc ? 5 : 0) + q.spec_len + 1 + varint_len(input) + 1 + varint_len(el);
+  int32_t st = B200TFS_OK;
+  if (msg > 0x7FFFFFFFull) st = B200TFS_E_TOOBIG;
+  else if (q.anchor + el > q.slot_end) st = B200TFS_E_SIZE;
+  T.status[r] = st;
+  T.rec_off[r] = st ? 0 : q.anchor - pre;
+  T.rec_len[r] = st ? 0 : pre + el;
+  if (st) return;
+  uint8_t* w = T.arena + q.anchor - pre;
+  if (q.grpc) { *w++ = 0; *w++ = (uint8_t)(msg >> 24); *w++ = (uint8_t)(msg >> 16); *w++ = (uint8_t)(msg >> 8); *w++ = (uint8_t)msg; }
+  for (uint32_t b = 0; b < q.spec_len; ++b) *w++ = T.blob[q.spec_off + b];
+  *w++ = 0x12; w += put_varint(w, input);
+  *w++ = 0x0A; put_varint(w, el);
+}
+
+cudaError_t launch_example_requests(const ExTables& T, cudaStream_t stream, uint32_t* launched) {
+  *launched = 0;
+  if (T.n_tiles) {
+    ex_count_kernel<<<T.n_tiles, kExTile, 0, stream>>>(T);
+    ex_scan_kernel<<<T.n_tiles, kExTile, 0, stream>>>(T);
+    *launched += 2;
+  }
+  if (T.n_spans) { ex_emit_kernel<<<T.n_spans, kExEmitThreads, 0, stream>>>(T); *launched += 1; }
+  if (T.n_req) { ex_frame_kernel<<<(T.n_req + kExFrameWarps - 1) / kExFrameWarps, 32 * kExFrameWarps, 0, stream>>>(T); *launched += 1; }
+  return cudaGetLastError();
+}

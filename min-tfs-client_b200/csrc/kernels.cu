@@ -20,6 +20,8 @@
 //                      tabulates dtype, dims and where the values lie.
 //   frame_requests_kernel  deferred framing (frame.h): one warp per request evaluates the request's framing program from the
 //                      device-side totals, writes every header byte, patches the destinations of the movers behind it.
+//   ex_count / ex_scan / ex_emit / ex_frame_kernel   Classify / Regress requests: a batch of tf.Examples from columnar
+//                      arrays (example_kernels.cuh).
 //   venc_* / vdec_*    packed-varint encode and decode (int_val / int64_val / uint32_val / uint64_val /
 //                      half_val / bool_val): varint_kernels.cuh.  vdec_plan_kernel + vdec_{count,emit}_dev_kernel decode the
 //                      varint outputs of a single-launch decode from tables built on the device (b200tfs_set_decode_varints).
@@ -1173,6 +1175,11 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
     *reinterpret_cast<PlanHeader*>(cp.plan) = ph;
   }
 }
+
+// ------------------------------------------------------------------------------------------------
+// tf.Example requests (Classify / Regress): ex_count / ex_scan / ex_emit / ex_frame
+// ------------------------------------------------------------------------------------------------
+#include "example_kernels.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // frame_requests_kernel (plan.h "deferred framing"): one thread per request evaluates the request's values from the job

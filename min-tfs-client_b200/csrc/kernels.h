@@ -45,5 +45,7 @@ cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t
 // b200tfs_decode_concat: concat_plan_kernel, then move_kernel over the plan image it wrote, with move_grid CTAs (the host's bound
 // on the tiles; the CTAs past the plan's own count leave at once)
 cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStream_t stream);
+// tf.Example requests (example_kernels.cuh): count + scan (when T.n_tiles), emit, frame; *launched receives how many kernels
+cudaError_t launch_example_requests(const ExTables& T, cudaStream_t stream, uint32_t* launched);
 
 }  // namespace b200tfs

@@ -9,6 +9,7 @@
 #include <stdint.h>
 
 #include "../../include/b200tfs.h"
+#include "wire.h"
 
 namespace b200tfs {
 
@@ -289,6 +290,59 @@ struct FrameTables {
 #endif
 B2_PLAN_HD uint64_t var_decode_tiles(const void* src, uint64_t n) {
   return n ? (((uint64_t)((uintptr_t)src & 15) + n + kVarTileBytes - 1) / kVarTileBytes) : 0;
+}
+
+// ---- tf.Example requests (example_host.inc plans, example_kernels.cuh runs) ----------------------------------------------
+// One request's examples start at a host-fixed anchor inside its slot; the request prefix is written in front of them once
+// their total is known.  Requests with an integer column get their example sizes from the count kernel and their offsets
+// from the scan kernel (tiles of kExTile examples); float-only requests have one closed-form example size.
+enum ExOp : uint32_t { EXO_F32 = 0, EXO_F64 = 1, EXO_F16 = 2, EXO_INT = 3, EXO_BOOL = 4 };
+constexpr uint32_t kExTile = kConcatPlanThreads;   // examples per count / scan CTA (one thread each in the scan)
+constexpr uint32_t kExEmitThreads = 256;
+constexpr uint32_t kExStage = 16384;               // shared-memory image of the wire one emit batch writes
+struct ExFeat {             // one column of one request, in wire order
+  const uint8_t* data;
+  uint64_t row_stride;      // bytes between the rows of consecutive examples (0: a broadcast column)
+  uint64_t row_elems;
+  uint32_t op, esz, sgn;    // ExOp, element size in memory, sign-extend (EXO_INT)
+  uint32_t key_off, key_len;   // key bytes in ExTables::blob
+  uint32_t lcol;            // integer columns: column of the request's length table
+};
+struct ExReq {
+  uint32_t first_feat, n_feat, n_int;   // n_int == 0: float-only, every example is fixed_size bytes
+  uint32_t spec_off, spec_len;          // the model_spec field (tag included) in ExTables::blob
+  uint32_t grpc;                        // gRPC's five-byte length-prefixed-message header in front
+  uint32_t first_tile, n_tiles;         // count / scan tiles (integer requests)
+  uint64_t n_ex, ex0;                   // examples, and the first one's index in the per-example tables of the call
+  uint64_t L0;                          // first entry of the request in ExTables::L (n_ex * n_int entries)
+  uint64_t fixed_size;                  // float-only: bytes of one example in the example_list (its tag included)
+  uint64_t anchor, slot_end;            // arena offsets: where example 0 starts, where the slot ends
+};
+struct ExSpan { uint32_t req, pad; uint64_t e0, e1; };   // a CTA's examples [e0, e1) of request `req`
+struct ExTables {
+  const ExReq* reqs; const ExFeat* feats; const uint8_t* blob;
+  const ExSpan* tiles;                  // count / scan CTAs
+  const ExSpan* spans;                  // emit CTAs
+  uint64_t* L;                          // packed length of every (example, integer column)
+  uint64_t* S;                          // bytes of every example of an integer request
+  uint64_t* off;                        // its offset from the anchor
+  unsigned long long* tile_sum;         // bytes of every tile's examples
+  uint8_t* arena;
+  uint64_t* rec_off; uint64_t* rec_len; int32_t* status;   // pinned host memory: read by b200tfs_encode_results
+  uint32_t n_req, n_tiles, n_spans;
+};
+// Bytes of one feature map entry (its tag included) whose list payload is P bytes; *hl receives those in front of the payload:
+//   0A vi(entry) 0A vi(klen) key 12 vi(Feature) {12 float_list | 1A int64_list} vi(list) [0A vi(P) payload]
+B2_PLAN_HD uint64_t ex_entry_len(uint64_t P, uint64_t klen, uint64_t* hl) {
+  const uint64_t list = P ? 1 + varint_len(P) + P : 0, feature = 1 + varint_len(list) + list;
+  const uint64_t entry = 1 + varint_len(klen) + klen + 1 + varint_len(feature) + feature;
+  *hl = 1 + varint_len(entry) + entry - P;
+  return 1 + varint_len(entry) + entry;
+}
+// bytes of one example in the example_list (its tag included) whose map entries add up to F bytes: 0A vi(X) 0A vi(F) entries
+B2_PLAN_HD uint64_t ex_example_len(uint64_t F) {
+  const uint64_t x = 1 + varint_len(F) + F;
+  return 1 + varint_len(x) + x;
 }
 
 }  // namespace b200tfs

@@ -85,6 +85,26 @@ class ConcatKey(C.Structure):
     ]
 
 
+F_BROADCAST = 0x10
+
+
+class Feature(C.Structure):
+    """b200tfs_feature: one column of a tf.Example request (row i is example i; F_BROADCAST: one row for every example)."""
+    _fields_ = [
+        ("data", C.c_void_p), ("src_dtype", C.c_int32), ("flags", C.c_uint32), ("row_elems", C.c_int64), ("key", C.c_char_p),
+        ("key_len", C.c_int64),
+    ]
+
+
+class ExampleRequest(C.Structure):
+    """b200tfs_example_request: one ClassificationRequest / RegressionRequest built from columns."""
+    _fields_ = [
+        ("model_name", C.c_char_p), ("model_name_len", C.c_int64), ("has_version", C.c_int32), ("order", C.c_int32),
+        ("version", C.c_int64), ("n_examples", C.c_int64), ("n_features", C.c_int32), ("flags", C.c_int32),
+        ("features", C.POINTER(Feature)),
+    ]
+
+
 _u64p = C.POINTER(C.c_uint64)
 _i32p = C.POINTER(C.c_int32)
 _vp = C.c_void_p
@@ -163,6 +183,10 @@ SIGNATURES = {
                                                C.POINTER(ModelSpec), _i32p]),
     "b200tfs_parse_tensor_protos_host": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.POINTER(Output), _i32p]),
     "b200tfs_unpack_outputs_host": (C.c_int, [_vp, C.c_int32, C.POINTER(Output), _u64p, _vpp, _i32p, _i32p]),
+    "b200tfs_example_request_size": (C.c_int, [C.POINTER(ExampleRequest), _u64p]),
+    "b200tfs_example_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), _u64p]),
+    "b200tfs_encode_example_requests_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), _vp, C.c_uint64]),
+    "b200tfs_encode_example_requests_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), _vp, C.c_uint64, _u64p, _u64p]),
 }
 
 _lib = None

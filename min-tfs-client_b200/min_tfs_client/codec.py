@@ -130,6 +130,60 @@ def _wire_bound(p: "_Prepared", tensor_content: bool) -> int:
     return n * per[p.itemsize] + frame
 
 
+_EXAMPLE_DTYPES = {np.dtype(t): _validated_enum(np.empty(0, t)) for t in (
+    np.float16, np.float32, np.float64, np.int8, np.int16, np.int32, np.int64, np.uint8, np.uint16, np.uint32, np.uint64, np.bool_)}
+
+
+def _example_columns(input_dict: Mapping):
+    """(n_examples, [(Feature, keep-alive), ...]) for the device route, or None for a request ``examples_from_input_dict``
+    assembles on the host (str / bytes columns, dtypes without a device conversion - which it rejects or converts itself).
+    Raises the ValueError ``examples_from_input_dict`` raises for disagreeing example counts, and for device arrays of a dtype
+    the device route does not take."""
+    cols = []
+    for k, v in input_dict.items():
+        key = k.encode("utf-8") if isinstance(k, str) else bytes(k)
+        if D.is_device_object(v):
+            ptr, shape, dtype, hold = D.device_view(v)
+            if dtype not in _EXAMPLE_DTYPES:
+                raise ValueError(f"input {k!r}: device arrays of dtype {dtype} have no tf.Example feature kind on the device")
+            cols.append((key, ptr, shape, dtype, hold, True))
+        else:
+            a = np.asarray(v)
+            dtype = a.dtype.newbyteorder("=")
+            if dtype not in _EXAMPLE_DTYPES:
+                return None
+            cols.append((key, None, a.shape, dtype, a, False))
+    rows = {shape[0] for _, _, shape, _, _, _ in cols if len(shape)}
+    if len(rows) > 1:
+        raise ValueError(f"inputs disagree on the number of examples: {sorted(rows)}")
+    n = rows.pop() if rows else (1 if cols else 0)
+    preps = []
+    for key, ptr, shape, dtype, hold, on_device in cols:
+        row_elems = int(np.prod(shape[1:], dtype=np.int64)) if len(shape) else 1
+        flags = 0 if len(shape) else N.F_BROADCAST
+        if on_device:
+            flags |= N.F_DEVICE_DATA
+        else:
+            hold = np.require(hold.astype(dtype, copy=False), requirements="CA")
+            ptr = hold.ctypes.data
+        size = int(np.prod(shape, dtype=np.int64))
+        f = N.Feature(data=ptr if size else None, src_dtype=_EXAMPLE_DTYPES[dtype], flags=flags, row_elems=row_elems,
+                      key=key, key_len=len(key))
+        preps.append((f, hold, key))
+    return n, preps
+
+
+def _host_example_request(model_name, model_version, input_dict, grpc_frame: bool) -> bytes:
+    """A request with a column the device route does not take, as ``examples_from_input_dict`` and protobuf make it."""
+    from tensorflow_serving.apis.classification_pb2 import ClassificationRequest
+
+    from .requests import TensorServingClient
+
+    wire = TensorServingClient._make_example_request(None, ClassificationRequest, model_name, input_dict, model_version) \
+        .SerializeToString(deterministic=True)
+    return (b"\x00" + len(wire).to_bytes(4, "big") + wire) if grpc_frame else wire
+
+
 class DecodedSpec:
     """model_spec of a parsed response (model.proto:9-33)."""
 
@@ -363,6 +417,48 @@ class Codec:
 
     def encode_predict_request(self, model_name: str, input_dict: Mapping, model_version: Optional[int] = None, **kw) -> bytes:
         return self.encode_predict_requests([(model_name, model_version, input_dict)], **kw)[0]
+
+    def encode_example_requests(self, requests: Iterable[Tuple[str, Optional[int], Mapping]], *, order="deterministic",
+                                grpc_frame: bool = False) -> List[bytes]:
+        """Each item is ``(model_name, model_version, input_dict)``; returns one ClassificationRequest / RegressionRequest wire
+        per item (the two messages share their field numbers, so the bytes serve both RPCs).
+
+        The bytes equal ``_make_example_request(...).SerializeToString(deterministic=True)`` of the request
+        ``examples_from_input_dict`` builds - one tf.Example per row, 0-d arrays repeated in every example - with
+        ``order="deterministic"``, or list every example's features in insertion order with ``order="given"``.  Values may be
+        numpy arrays (pageable or ``pinned_empty``) or device arrays (``__cuda_array_interface__`` / DLPack).  A request with a
+        str / bytes column (or a dtype the device route does not take) is assembled on the host by ``examples_from_input_dict``,
+        in deterministic order; device arrays of such dtypes raise ValueError.
+        """
+        order_code = _ORDER[order] if isinstance(order, str) else int(order)
+        items = list(requests)
+        out: List[Optional[bytes]] = [None] * len(items)
+        keep, structs, dev_idx = [], [], []
+        for i, (model_name, model_version, input_dict) in enumerate(items):
+            cols = _example_columns(input_dict)
+            if cols is None:
+                out[i] = _host_example_request(model_name, model_version, input_dict, grpc_frame)
+                continue
+            n, preps = cols
+            feats = (N.Feature * max(len(preps), 1))(*[p[0] for p in preps])
+            name = model_name.encode("utf-8") if isinstance(model_name, str) else bytes(model_name)
+            structs.append(N.ExampleRequest(model_name=name, model_name_len=len(name), has_version=int(model_version is not None),
+                                            order=order_code, version=int(model_version) if model_version is not None else 0,
+                                            n_examples=n, n_features=len(preps), flags=N.RF_GRPC_FRAME if grpc_frame else 0,
+                                            features=feats))
+            keep.append((preps, feats, name))
+            dev_idx.append(i)
+        if dev_idx:
+            m = len(dev_idx)
+            reqs = (N.ExampleRequest * m)(*structs)
+            cap = C.c_uint64()
+            N.check(self._lib.b200tfs_example_arena_size(m, reqs, C.byref(cap)))
+            wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
+            off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
+            N.check(self._lib.b200tfs_encode_example_requests_host(self._ctx, m, reqs, wire.ctypes.data, cap.value, off, ln))
+            for j, i in enumerate(dev_idx):
+                out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
+        return out  # type: ignore[return-value]
 
     # ---- decode --------------------------------------------------------------------------------
     def _pack_wires(self, wires: Sequence[bytes]):

@@ -106,6 +106,12 @@ def gpu_request_serializer(request) -> bytes:
     return get_codec().encode_predict_request(model_name, input_dict, model_version)
 
 
+def gpu_example_request_serializer(request) -> bytes:
+    """``request_serializer`` for ``channel.unary_unary(CLASSIFY_METHOD | REGRESS_METHOD, ...)``: (model_name, model_version,
+    input_dict) -> the ClassificationRequest / RegressionRequest bytes ``_make_example_request`` would serialise, packed on the GPU."""
+    return get_codec().encode_example_requests([request])[0]
+
+
 def gpu_response_deserializer(wire: bytes) -> PredictResponseView:
     """``response_deserializer`` for ``channel.unary_unary``: bytes -> lazy response view."""
     return PredictResponseView(wire)
