@@ -135,7 +135,7 @@ struct b200tfs_ctx {
   Growable concat_dev;                  // b200tfs_decode_concat: parse table, plan image, varint tables (ConcatLayout)
   int32_t concat_n = 0, concat_k = 0;   // ... of its most recent call, what b200tfs_concat_results answers for
   uint8_t* concat_dst[B200TFS_CONCAT_MAX_KEYS] = {};
-  uint64_t concat_vouts_off = 0, concat_vstat_off = 0;
+  uint64_t concat_vouts_off = 0, concat_vstat_off = 0, concat_specs_off = 0, concat_status_off = 0;   // its ConcatLayout
 };
 
 // `baked`: the buffer's address ends up inside captured graphs (every context-owned scratch buffer except the plan-upload
@@ -210,6 +210,38 @@ static int upload_slot(b200tfs_ctx* c, Slot* slot, uint64_t bytes) {
   }
   CU(cudaMemcpyAsync(slot->dev.p, slot->host.p, bytes, cudaMemcpyHostToDevice, c->stream));
   if (slot->done) { CU(cudaEventRecord(slot->done, c->stream)); slot->pending = true; }
+  return B200TFS_OK;
+}
+
+// The regions of a scratch buffer or an upload image, laid out one behind the other: take() hands out a region's offset,
+// `end` is where the last one ends.  Each layout is one function that the code sizing the buffer and the code using it both call.
+struct Layout {
+  uint64_t end = 0;
+  uint64_t take(uint64_t bytes, uint64_t align = 16) {
+    const uint64_t at = (end + align - 1) & ~(align - 1);
+    end = at + bytes;
+    return at;
+  }
+};
+
+// One host array of an upload image, and where it goes
+struct ImagePart { uint64_t off; const void* src; uint64_t bytes; };
+struct NoFill { void operator()(uint8_t*, uint8_t*) const {} };
+
+// Claim an upload slot for an image of `bytes`, copy every part to its offset, let `fill(host, dev)` write what depends on the
+// device address, and bring the first `sent` bytes (all of them by default) to the device.  *dev receives the device base.
+template <class Fill = NoFill>
+static int upload_image(b200tfs_ctx* c, uint64_t bytes, std::initializer_list<ImagePart> parts, uint8_t** dev, Slot** out = nullptr,
+                        Fill&& fill = Fill(), uint64_t sent = ~0ull) {
+  Slot* slot;
+  int rc = claim_slot(c, bytes, &slot);
+  if (rc) return rc;
+  uint8_t* h = (uint8_t*)slot->host.p;
+  for (const ImagePart& p : parts) if (p.bytes) memcpy(h + p.off, p.src, p.bytes);
+  fill(h, (uint8_t*)slot->dev.p);
+  if ((rc = upload_slot(c, slot, std::min(sent, bytes)))) return rc;
+  *dev = (uint8_t*)slot->dev.p;
+  if (out) *out = slot;
   return B200TFS_OK;
 }
 
@@ -602,14 +634,11 @@ int build_plan(b200tfs_ctx* c, PlanBuilder& pb, bool force_dev, BuiltPlan* bp) {
   ph.vec_per_tile = vpt;
   ph.guard = pb.guard; ph.guard_div = pb.guard_div ? pb.guard_div : 1u;
   ph.independent = pb.independent ? 1u : 0u;
-  uint64_t off = (sizeof(PlanHeader) + 15) & ~15ull;
-  ph.off_items = (uint32_t)off; off += pb.items.size() * sizeof(MoveItem);
-  ph.off_tiles = (uint32_t)off; if (!uniform) off += n_tiles * sizeof(TileRef);
-  off = (off + 15) & ~15ull;
-  ph.off_small = (uint32_t)off; off += pb.smalls.size() * sizeof(SmallItem);
-  const uint64_t off_blob = off;
-  off += pb.blob.size();
-  const uint64_t image = (off + 15) & ~15ull;
+  const PlanGeometry g = plan_geometry(pb.items.size(), uniform ? 0 : n_tiles, pb.smalls.size());
+  ph.off_items = (uint32_t)g.off_items; ph.off_tiles = (uint32_t)g.off_tiles; ph.off_small = (uint32_t)g.off_small;
+  Layout P{g.end};
+  const uint64_t off_blob = P.take(pb.blob.size(), 1);
+  const uint64_t image = P.take(0);
   if (image > 0xFFFFFFFFull) return fail(B200TFS_E_TOOBIG, "plan image larger than 4 GiB");
   bp->image = image;
   uint8_t* img;
@@ -973,12 +1002,11 @@ static int parse_common(b200tfs_ctx* c, const void* arena_dev, int32_t n, const 
   CU(cudaSetDevice(c->device));
   if (bare) max_outputs = 1;
   const uint64_t stride = bare ? 1 : (uint64_t)max_outputs + 1;  // responses: one scratch slot per record
-  const uint64_t b_off = 0, b_len = b_off + 8ull * n, b_outs = (b_len + 8ull * n + 15) & ~15ull;
-  const uint64_t b_nouts = b_outs + sizeof(b200tfs_output) * (uint64_t)n * stride;
-  const uint64_t b_specs = (b_nouts + 4ull * n + 15) & ~15ull;
-  const uint64_t b_status = b_specs + sizeof(b200tfs_model_spec) * (uint64_t)n;
-  const uint64_t b_spill = (b_status + 4ull * n + 15) & ~15ull;      // uint32 spill_used[n]
-  const uint64_t total = (b_spill + 4ull * n + 15) & ~15ull;
+  Layout B;   // rec_off | rec_len (uploaded) | outs | n_outs | specs | status | uint32 spill_used[n] (brought back)
+  const uint64_t b_off = B.take(8ull * n), b_len = B.take(8ull * n);
+  const uint64_t b_outs = B.take(sizeof(b200tfs_output) * (uint64_t)n * stride), b_nouts = B.take(4ull * n);
+  const uint64_t b_specs = B.take(sizeof(b200tfs_model_spec) * (uint64_t)n), b_status = B.take(4ull * n);
+  const uint64_t b_spill = B.take(4ull * n), total = B.end;
   int rc;
   if ((rc = grow_dev(c, c->scratch_dev, total))) return rc;
   if ((rc = grow_host(c, c->scratch_host, total))) return rc;
@@ -1250,13 +1278,14 @@ extern "C" int b200tfs_unpack_outputs(b200tfs_ctx* c, const void* arena_dev, int
 namespace {
 struct FusedLayout { uint64_t outs, nouts, specs, status, vstatus, total; };
 FusedLayout fused_layout(int32_t n) {
+  Layout R;
   FusedLayout L;
-  L.outs = 0;
-  L.nouts = L.outs + sizeof(b200tfs_output) * (uint64_t)n * kFusedMaxOutputs;
-  L.specs = (L.nouts + 4ull * n + 15) & ~15ull;
-  L.status = L.specs + sizeof(b200tfs_model_spec) * (uint64_t)n;
-  L.vstatus = (L.status + 4ull * n + 15) & ~15ull;     // b200tfs_set_decode_varints: one status word per (record, output) slot
-  L.total = (L.vstatus + 4ull * n * kFusedMaxOutputs + 15) & ~15ull;
+  L.outs = R.take(sizeof(b200tfs_output) * (uint64_t)n * kFusedMaxOutputs);
+  L.nouts = R.take(4ull * n);
+  L.specs = R.take(sizeof(b200tfs_model_spec) * (uint64_t)n);
+  L.status = R.take(4ull * n);
+  L.vstatus = R.take(4ull * n * kFusedMaxOutputs);     // b200tfs_set_decode_varints: one status word per (record, output) slot
+  L.total = R.end;
   return L;
 }
 
@@ -1264,17 +1293,41 @@ FusedLayout fused_layout(int32_t n) {
 struct VarPlanLayout { uint64_t jobs, segs, tile_seg, tile_val, group_sum, total, status, n_tiles, bytes; };
 VarPlanLayout var_plan_layout(uint64_t n, uint64_t tile_cap) {
   const uint64_t slots = n * kFusedMaxOutputs;
+  Layout R;
   VarPlanLayout V;
-  V.jobs = 0;
-  V.segs = V.jobs + slots * sizeof(VarJobDev);
-  V.tile_seg = (V.segs + slots * B200TFS_MAX_RUNS * sizeof(VarSeg) + 15) & ~15ull;
-  V.tile_val = (V.tile_seg + 4 * tile_cap + 15) & ~15ull;
-  V.group_sum = (V.tile_val + 4 * tile_cap + 15) & ~15ull;
-  V.total = (V.group_sum + 4 * (tile_cap / kVarGroupTiles + slots + 2) + 15) & ~15ull;
-  V.status = V.total + 8 * slots;
-  V.n_tiles = (V.status + 4 * slots + 15) & ~15ull;
-  V.bytes = V.n_tiles + 16;
+  V.jobs = R.take(slots * sizeof(VarJobDev));
+  V.segs = R.take(slots * B200TFS_MAX_RUNS * sizeof(VarSeg));
+  V.tile_seg = R.take(4 * tile_cap);
+  V.tile_val = R.take(4 * tile_cap);
+  V.group_sum = R.take(4 * (tile_cap / kVarGroupTiles + slots + 2));
+  V.total = R.take(8 * slots);
+  V.status = R.take(4 * slots);
+  V.n_tiles = R.take(16);
+  V.bytes = R.end;
   return V;
+}
+
+// b200tfs_encode_requests_async / b200tfs_encode_example_requests_async leave rec_off[n] | rec_len[n] | status[n] in pinned
+// memory (enc_host), where b200tfs_encode_results reads them
+struct EncResultsLayout { uint64_t rec_off, rec_len, status, bytes; };
+EncResultsLayout enc_results_layout(uint64_t n) {
+  Layout R;
+  EncResultsLayout E;
+  E.rec_off = R.take(8 * n);
+  E.rec_len = R.take(8 * n);
+  E.status = R.take(4 * n);
+  E.bytes = R.end;
+  return E;
+}
+
+// Point the pointers a launch writes its results through at enc_host, grown for n requests
+int bind_enc_results(b200tfs_ctx* c, int32_t n, uint64_t** rec_off, uint64_t** rec_len, int32_t** status) {
+  const EncResultsLayout E = enc_results_layout((uint64_t)n);
+  int rc = grow_host(c, c->enc_host, E.bytes);
+  if (rc) return rc;
+  uint8_t* rh = (uint8_t*)c->enc_host.p;
+  *rec_off = (uint64_t*)(rh + E.rec_off); *rec_len = (uint64_t*)(rh + E.rec_len); *status = (int32_t*)(rh + E.status);
+  return B200TFS_OK;
 }
 }  // namespace
 
@@ -1298,19 +1351,28 @@ static uint32_t decode_vpt(const b200tfs_ctx* c, int32_t n, const uint64_t* rec_
   return pick_vec_per_tile(c, c->decode_cast ? wire_total / 2 : wire_total, c->decode_cast ? 65536 : 262144);
 }
 
+// The parse walk (walker.h) of one record that lies in host memory, up to `max` outputs.  A record the walker's 32-bit cursor
+// cannot hold is B200TFS_E_PARSE, as the kernels find it.  `cur` (optional) is left where the walk ended.
+static int walk_host_record(const void* rec, uint64_t len, int max, b200tfs_output* outs, int* cnt, b200tfs_model_spec* spec,
+                            SpillArea sp = SpillArea{nullptr, 0u, 0u}, Cursor* cur = nullptr) {
+  if (len > 0x7FFFFFFFull) return B200TFS_E_PARSE;
+  Cursor own;
+  Cursor& k = cur ? *cur : own;
+  cur_open_host(k, (const uint8_t*)rec, (uint32_t)len);
+  return walk_response(k, max, outs, cnt, spec, sp);
+}
+
 // Walk record 0 on the host (its bytes are in host memory) and build its template: the launch that follows then takes the
 // template path from its first CTA on.  Returns false when the record does not qualify (the kernel will walk it).
 static bool host_template(const uint8_t* rec0, uint64_t len, uint32_t vpt, uint64_t dst_stride, uint32_t serial, uint32_t cast, uint32_t varints,
                           Template* T) {
   T->in.head.valid = 0;
-  if (!rec0 || len == 0 || len > 0x7FFFFFFFull) return false;
+  if (!rec0 || len == 0) return false;
   b200tfs_output outs[kFusedMaxOutputs + 1];
   b200tfs_model_spec spec;
   int cnt = 0;
   Cursor cur;
-  cur_open_host(cur, rec0, (uint32_t)len);
-  SpillArea sp{nullptr, 0u, 0u};
-  const int st = walk_response(cur, kFusedMaxOutputs, outs, &cnt, &spec, sp);
+  const int st = walk_host_record(rec0, len, kFusedMaxOutputs, outs, &cnt, &spec, SpillArea{nullptr, 0u, 0u}, &cur);
   if (st != B200TFS_OK) return false;
   const uint64_t used = tpl_layout_outputs(outs, cnt, dst_stride, cast, varints);
   for (int k = 0; k < cnt; ++k) if (outs[k].status == B200TFS_E_SIZE) return false;
@@ -1327,14 +1389,11 @@ int b200tfs_decode_slot_bytes(const void* wire_host, int32_t n, const uint64_t* 
   uint64_t most = 0;
   int32_t nv = 0;
   for (int i = 0; i < n; ++i) {
-    if (rec_len[i] > 0x7FFFFFFFull) continue;     // the launch rejects such a record: it gets no slot bytes
     b200tfs_output outs[kFusedMaxOutputs + 1];
     b200tfs_model_spec spec;
     int cnt = 0;
-    Cursor cur;
-    cur_open_host(cur, (const uint8_t*)wire_host + rec_off[i], (uint32_t)rec_len[i]);
-    SpillArea sp{nullptr, 0u, 0u};
-    if (walk_response(cur, kFusedMaxOutputs, outs, &cnt, &spec, sp) != B200TFS_OK) continue;
+    // a record the launch rejects (malformed, or too long for the walker) gets no slot bytes
+    if (walk_host_record((const uint8_t*)wire_host + rec_off[i], rec_len[i], kFusedMaxOutputs, outs, &cnt, &spec) != B200TFS_OK) continue;
     most = std::max(most, tpl_layout_outputs(outs, cnt, ~0ull, 0u, varints ? 1u : 0u));
     for (int k = 0; k < cnt && varints; ++k)
       if (outs[k].status == B200TFS_OK && outs[k].n_elems && dtype_info(outs[k].dtype).kind != VK_FIXED && tpl_gets_range(1u, outs[k].dtype))
@@ -1343,6 +1402,30 @@ int b200tfs_decode_slot_bytes(const void* wire_host, int32_t n, const uint64_t* 
   *slot_bytes = most;
   if (n_varint_outputs) *n_varint_outputs = nv;
   return B200TFS_OK;
+}
+
+// The packed-varint outputs of a table a decode launch published: vdec_plan_kernel builds their decode tables in the region `vd`
+// (var_plan_layout(vp.n, vp.tile_cap)), then the count and emit kernels run over them.  `vp` comes with the table, the wire and
+// the destinations set; rec_off is the host's copy of the record offsets.  vp.status receives the per-slot statuses.
+static int launch_varint_tail(b200tfs_ctx* c, VarPlan& vp, uint8_t* vd, const uint64_t* rec_off) {
+  const VarPlanLayout V = var_plan_layout(vp.n, vp.tile_cap);
+  if (vp.n <= (uint32_t)kFusedInlineRecs) for (uint32_t i = 0; i < vp.n; ++i) vp.off_inl[i] = rec_off[i];
+  vp.jobs = (VarJobDev*)(vd + V.jobs); vp.segs = (VarSeg*)(vd + V.segs); vp.tile_seg = (uint32_t*)(vd + V.tile_seg);
+  vp.tile_val = (uint32_t*)(vd + V.tile_val); vp.group_sum = (uint32_t*)(vd + V.group_sum);
+  vp.total = (unsigned long long*)(vd + V.total); vp.status = (int32_t*)(vd + V.status); vp.n_tiles = (uint32_t*)(vd + V.n_tiles);
+  CU(launch_vdec_plan(vp, c->stream));
+  VarTables tb{};
+  tb.segs = vp.segs; tb.tile_seg = vp.tile_seg; tb.jobs = vp.jobs; tb.n_tiles = vp.tile_cap; tb.n_tiles_dev = vp.n_tiles;
+  CU(launch_vdec_dev(tb, (uint32_t)c->sm_count * 4, c->stream));
+  c->launches += 3;
+  return B200TFS_OK;
+}
+
+// What the varint decode found for one output slot of the table (kVarSlotIdle: a slot it did not take, left as tabulated)
+static void fold_varint_status(b200tfs_output& o, int32_t s) {
+  if (s == kVarSlotIdle) return;
+  o.status = s;
+  o.flags |= B200TFS_OF_DEVICE_VARINT;
 }
 
 // the pipelined host decode of ONE record: launch k covers tiles [tile_lo[k], tile_lo[k+1]) of the full grid (the last one also the
@@ -1432,25 +1515,20 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
       }
       q.inl.tile_start[n] = (uint32_t)grid;
     } else {
-      // tables: cta_rec[grid] | tile_start[n+1] | rec_off[n] | rec_len[n]
       std::vector<uint32_t> ts(n + 1);
       for (int i = 0; i < n; ++i) { ts[i] = (uint32_t)grid; grid += per(rec_len[i]); }
       ts[n] = (uint32_t)grid;
       if (grid > 0x7FFFFFFFull) return fail(B200TFS_E_TOOBIG, "batch needs more than 2^31 tiles");
-      const uint64_t o_ts = (grid * 4 + 15) & ~15ull, o_off = (o_ts + 4ull * (n + 1) + 15) & ~15ull, o_len = o_off + 8ull * n;
-      const uint64_t image = o_len + 8ull * n;
-      Slot* slot;
-      int rc2;
-      if ((rc2 = claim_slot(c, image, &slot))) return rc2;
-      uint8_t* h = (uint8_t*)slot->host.p;
-      uint32_t* cr = (uint32_t*)h;
-      for (int i = 0; i < n; ++i) for (uint32_t t = ts[i]; t < ts[i + 1]; ++t) cr[t] = (uint32_t)i;
-      memcpy(h + o_ts, ts.data(), 4ull * (n + 1));
-      memcpy(h + o_off, rec_off, 8ull * n);
-      memcpy(h + o_len, rec_len, 8ull * n);
-      if ((rc2 = upload_slot(c, slot, image))) return rc2;
-      uint8_t* sd = (uint8_t*)slot->dev.p;
-      q.cta_rec = (const uint32_t*)sd; q.tile_start = (const uint32_t*)(sd + o_ts);
+      Layout T;   // cta_rec[grid] | tile_start[n+1] | rec_off[n] | rec_len[n]
+      const uint64_t o_cr = T.take(4 * grid), o_ts = T.take(4ull * (n + 1)), o_off = T.take(8ull * n), o_len = T.take(8ull * n);
+      uint8_t* sd;
+      int rc2 = upload_image(c, T.end, {{o_ts, ts.data(), 4ull * (n + 1)}, {o_off, rec_off, 8ull * n}, {o_len, rec_len, 8ull * n}}, &sd, nullptr,
+                             [&](uint8_t* h, uint8_t*) {
+                               uint32_t* cr = (uint32_t*)(h + o_cr);
+                               for (int i = 0; i < n; ++i) for (uint32_t t = ts[i]; t < ts[i + 1]; ++t) cr[t] = (uint32_t)i;
+                             });
+      if (rc2) return rc2;
+      q.cta_rec = (const uint32_t*)(sd + o_cr); q.tile_start = (const uint32_t*)(sd + o_ts);
       q.rec_off = (const uint64_t*)(sd + o_off); q.rec_len = (const uint64_t*)(sd + o_len);
     }
     if (grid > 0x7FFFFFFFull) return fail(B200TFS_E_TOOBIG, "batch needs more than 2^31 tiles");
@@ -1515,22 +1593,12 @@ static int decode_launch(b200tfs_ctx* c, const void* arena_dev, int32_t n, const
   c->fused_varints = fp.varints != 0;
   if (fp.varints) {
     // plan -> count -> emit over the table the launch(es) above published, then the per-output statuses to pinned memory
-    const VarPlanLayout V = var_plan_layout((uint64_t)n, var_tile_cap);
-    uint8_t* vd = (uint8_t*)c->vdec_dev.p;
     VarPlan vp{};
     vp.outs = fp.outs; vp.n_outs = fp.n_outs; vp.rec_status = fp.status;
     vp.w = fp.w; vp.rec_off = fp.rec_off;
-    if (n <= kFusedInlineRecs) for (int i = 0; i < n; ++i) vp.off_inl[i] = rec_off[i];
     vp.dst = fp.dst; vp.dst_stride = dst_stride; vp.n = (uint32_t)n; vp.tile_cap = (uint32_t)var_tile_cap;
-    vp.jobs = (VarJobDev*)(vd + V.jobs); vp.segs = (VarSeg*)(vd + V.segs); vp.tile_seg = (uint32_t*)(vd + V.tile_seg);
-    vp.tile_val = (uint32_t*)(vd + V.tile_val); vp.group_sum = (uint32_t*)(vd + V.group_sum);
-    vp.total = (unsigned long long*)(vd + V.total); vp.status = (int32_t*)(vd + V.status); vp.n_tiles = (uint32_t*)(vd + V.n_tiles);
-    CU(launch_vdec_plan(vp, c->stream));
-    VarTables tb{};
-    tb.segs = vp.segs; tb.tile_seg = vp.tile_seg; tb.jobs = vp.jobs; tb.n_tiles = vp.tile_cap; tb.n_tiles_dev = vp.n_tiles;
-    CU(launch_vdec_dev(tb, (uint32_t)c->sm_count * 4, c->stream));
+    if ((rc = launch_varint_tail(c, vp, (uint8_t*)c->vdec_dev.p, rec_off))) return rc;
     CU(cudaMemcpyAsync((uint8_t*)c->fused_host.p + L.vstatus, vp.status, 4ull * n * kFusedMaxOutputs, cudaMemcpyDeviceToHost, c->stream));
-    c->launches += 3;
   }
   c->fused_n = n;
   if (!c->capturing) { CU(cudaEventRecord(c->tpl_event, c->stream)); c->tpl_event_pending = true; }
@@ -1576,13 +1644,8 @@ int b200tfs_decode_results(b200tfs_ctx* c, int32_t n, b200tfs_output* outs, int3
     const int32_t* no = (const int32_t*)(h + L.nouts);
     const int32_t* vs = (const int32_t*)(h + L.vstatus);
     for (int r = 0; r < n; ++r)
-      for (int k = 0; k < no[r] && rs[r] == B200TFS_OK && k < kFusedMaxOutputs; ++k) {
-        b200tfs_output& o = outs[(size_t)r * kFusedMaxOutputs + k];
-        const int32_t s = vs[(size_t)r * kFusedMaxOutputs + k];
-        if (s == kVarSlotIdle) continue;
-        o.status = s;
-        o.flags |= B200TFS_OF_DEVICE_VARINT;
-      }
+      for (int k = 0; k < no[r] && rs[r] == B200TFS_OK && k < kFusedMaxOutputs; ++k)
+        fold_varint_status(outs[(size_t)r * kFusedMaxOutputs + k], vs[(size_t)r * kFusedMaxOutputs + k]);
   }
   if (n_outs) memcpy(n_outs, h + L.nouts, 4ull * n);
   if (specs) memcpy(specs, h + L.specs, sizeof(b200tfs_model_spec) * (uint64_t)n);
@@ -1978,13 +2041,16 @@ int b200tfs_encode_requests_host(b200tfs_ctx* c, int32_t n, const b200tfs_reques
   return B200TFS_OK;
 }
 
-static int stage_wire(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, uint64_t* span) {
+// Give a host wire its place in stage_dev, `shift` bytes in, and copy it there unless `copy` is false (the caller copies it in
+// pieces).  *span receives the bytes the records cover.
+static int stage_wire(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, uint64_t* span,
+                      uint64_t shift = 0, bool copy = true) {
   uint64_t hi = 0;
   for (int i = 0; i < n; ++i) hi = std::max(hi, rec_off[i] + rec_len[i]);
   int rc = grow_dev(c, c->stage_dev, hi + 64);
   if (rc) return rc;
-  if (hi) CU(cudaMemcpyAsync(c->stage_dev.p, wire_host, hi, cudaMemcpyHostToDevice, c->stream));
-  c->stage_shift = 0;
+  c->stage_shift = shift;
+  if (hi && copy) CU(cudaMemcpyAsync((uint8_t*)c->stage_dev.p + shift, wire_host, hi, cudaMemcpyHostToDevice, c->stream));
   *span = hi;
   return B200TFS_OK;
 }
@@ -2032,11 +2098,16 @@ int b200tfs_decode_responses_host_async(b200tfs_ctx* c, const void* wire_host, i
     for (uint32_t q = 1; q < T.in.head.n_chunks; ++q) if (T.in.chunk[q].len > T.in.chunk[big].len) big = q;
     if (T.in.head.n_chunks) shift = (16 - ((rec_off[0] + T.in.chunk[big].wire_off) & 15)) & 15;
   }
-  uint64_t hi = 0;
-  for (int i = 0; i < n; ++i) hi = std::max(hi, rec_off[i] + rec_len[i]);
-  int rc = grow_dev(c, c->stage_dev, hi + 64);
+  // One large record whose values lie in one fixed-width chunk: slices of tiles, pipelined like the encode (wire bytes of slice
+  // k+1 travel H2D while slice k is decoded and the tensor bytes of slice k-1 travel D2H).  The kernel skips its framing verdict:
+  // the template was built from these very bytes, and a slice runs before the record's tail has arrived.
+  const TplChunk& ch = T.in.chunk[0];
+  const uint64_t tile_bytes = 16ull * vpt;
+  const bool sliced = have && n == 1 && c->pipe_min && rec_len[0] >= c->pipe_min && !c->opt_no_inline && T.in.head.n_chunks == 1 &&
+                      !ch.is_varint && (ch.op == OP_COPY || ch.op == OP_QUIET_DST) && ch.n_tiles >= 2 && ch.n_tiles == T.in.head.total_tiles;
+  uint64_t hi;
+  int rc = stage_wire(c, wire_host, n, rec_off, rec_len, &hi, shift, !sliced);
   if (rc) return rc;
-  c->stage_shift = shift;
   // a pinned destination is written by the kernel itself (posted PCIe writes): no staging buffer, no device-to-host copy
   uint8_t* dst_direct = (c->opt_direct_out && c->pipe_min) ? device_view_of_host(dst_host) : nullptr;
   if (dst_direct && ((uintptr_t)dst_direct & 255)) dst_direct = nullptr;
@@ -2044,13 +2115,7 @@ int b200tfs_decode_responses_host_async(b200tfs_ctx* c, const void* wire_host, i
   uint8_t* dst_dev = dst_direct ? dst_direct : (uint8_t*)c->arena_dev.p;
   if (dst_direct) c->direct_calls += 1;
   uint8_t* wire_dev = (uint8_t*)c->stage_dev.p + shift;
-  // One large record whose values lie in one fixed-width chunk: slices of tiles, pipelined like the encode (wire bytes of slice
-  // k+1 travel H2D while slice k is decoded and the tensor bytes of slice k-1 travel D2H).  The kernel skips its framing verdict:
-  // the template was built from these very bytes, and a slice runs before the record's tail has arrived.
-  const TplChunk& ch = T.in.chunk[0];
-  const uint64_t tile_bytes = 16ull * vpt;
-  if (have && n == 1 && c->pipe_min && rec_len[0] >= c->pipe_min && !c->opt_no_inline && T.in.head.n_chunks == 1 && !ch.is_varint &&
-      (ch.op == OP_COPY || ch.op == OP_QUIET_DST) && ch.n_tiles >= 2 && ch.n_tiles == T.in.head.total_tiles) {
+  if (sliced) {
     DecodeSlices sl;
     sl.K = (int)std::min<uint64_t>(std::min<uint64_t>(c->pipe_max, ch.n_tiles),
                                    std::max<uint64_t>(2, rec_len[0] / std::max<uint64_t>(c->pipe_min, 1ull << 18)));
@@ -2087,7 +2152,6 @@ int b200tfs_decode_responses_host_async(b200tfs_ctx* c, const void* wire_host, i
     c->pipelined_calls += 1;
     return B200TFS_OK;
   }
-  if (hi) CU(cudaMemcpyAsync(wire_dev, wire_host, hi, cudaMemcpyHostToDevice, c->stream));
   if ((rc = decode_launch(c, wire_dev, n, rec_off, rec_len, dst_dev, dst_stride, vpt, have ? &T : nullptr))) return rc;
   if (!dst_direct) CU(cudaMemcpyAsync(dst_host, c->arena_dev.p, dst_stride * (uint64_t)n, cudaMemcpyDeviceToHost, c->stream));
   return B200TFS_OK;
@@ -2141,17 +2205,13 @@ static int concat_check_keys(int32_t n_keys, const b200tfs_concat_key* keys) {
 int b200tfs_response_keys(const void* rec_host, uint64_t rec_len, int32_t cap, uint64_t* key_off, uint32_t* key_len, int32_t* count) {
   if (!count || cap < 0 || (cap && (!key_off || !key_len)) || (rec_len && !rec_host)) return fail(B200TFS_E_ARG, "bad arguments");
   *count = 0;
-  if (rec_len > 0x7FFFFFFFull) return B200TFS_E_PARSE;
   std::vector<b200tfs_output> outs;
   for (int max = 16;; max *= 2) {   // PredictResponse.FromString has no limit on the map size
     outs.assign((size_t)max + 1, b200tfs_output{});
     b200tfs_model_spec spec;
     int cnt = 0;
-    Cursor cur;
-    cur_open_host(cur, (const uint8_t*)rec_host, (uint32_t)rec_len);
     std::vector<SpillEntry> spill(4096);
-    SpillArea sp{spill.data(), (uint32_t)spill.size(), 0u};
-    const int st = walk_response(cur, max, outs.data(), &cnt, &spec, sp);
+    const int st = walk_host_record(rec_host, rec_len, max, outs.data(), &cnt, &spec, SpillArea{spill.data(), (uint32_t)spill.size(), 0u});
     if (st == B200TFS_E_SIZE && max < (1 << 20)) continue;
     if (st != B200TFS_OK && st != B200TFS_E_SPILL) return st;   // a spill only concerns dims / runs: the keys are all there
     *count = cnt;
@@ -2177,15 +2237,10 @@ int b200tfs_concat_layout(const void* wire_host, int32_t n, const uint64_t* rec_
   for (int r = 0; r < n; ++r) {
     b200tfs_output outs[kFusedMaxOutputs + 1];
     b200tfs_model_spec spec;
-    int cnt = 0, st = B200TFS_E_PARSE;
+    int cnt = 0;
     const uint8_t* rec = (const uint8_t*)wire_host + rec_off[r];
-    if (rec_len[r] <= 0x7FFFFFFFull) {
-      Cursor cur;
-      cur_open_host(cur, rec, (uint32_t)rec_len[r]);
-      SpillArea sp{nullptr, 0u, 0u};
-      st = walk_response(cur, kFusedMaxOutputs, outs, &cnt, &spec, sp);
-      if (st == B200TFS_E_SPILL || st == B200TFS_E_SIZE) st = B200TFS_E_NONCANONICAL;
-    }
+    int st = walk_host_record(rec, rec_len[r], kFusedMaxOutputs, outs, &cnt, &spec);
+    if (st == B200TFS_E_SPILL || st == B200TFS_E_SIZE) st = B200TFS_E_NONCANONICAL;
     for (int k = 0; k < n_keys; ++k) {
       if (done[k]) continue;
       b200tfs_concat_key& K = keys[k];
@@ -2220,24 +2275,27 @@ int b200tfs_concat_layout(const void* wire_host, int32_t n, const uint64_t* rec_
 
 namespace {
 // device scratch of b200tfs_decode_concat for n records, n_keys keys, tile_cap move tiles and var_tile_cap varint tiles
-struct ConcatLayout { uint64_t outs, nouts, specs, status, spill, kst, match, plan, plan_tiles, vouts, vnouts, vstatus, var, bytes; };
+struct ConcatLayout { uint64_t outs, nouts, specs, status, spill, kst, match, plan, plan_tiles, vouts, vnouts, vstatus, var, var_status, bytes; };
 ConcatLayout concat_layout(uint64_t n, uint64_t n_keys, uint64_t tile_cap, uint64_t var_tile_cap) {
-  auto up = [](uint64_t x) { return (x + 255) & ~255ull; };
+  const PlanGeometry g = plan_geometry(n * n_keys * B200TFS_MAX_RUNS, tile_cap, 0);   // concat_plan_kernel's plan image
+  const VarPlanLayout V = var_plan_layout(n, var_tile_cap);
+  Layout R;
   ConcatLayout L;
-  L.outs = 0;
-  L.nouts = up(L.outs + sizeof(b200tfs_output) * n * (kFusedMaxOutputs + 1));
-  L.specs = up(L.nouts + 4 * n);
-  L.status = up(L.specs + sizeof(b200tfs_model_spec) * n);
-  L.spill = up(L.status + 4 * n);
-  L.kst = up(L.spill + 4 * n);
-  L.match = up(L.kst + 4 * n * n_keys);
-  L.plan = up(L.match + 4 * n * n_keys);
-  L.plan_tiles = ((((sizeof(PlanHeader) + 15) & ~15ull) + n * n_keys * B200TFS_MAX_RUNS * sizeof(MoveItem) + 15) & ~15ull);
-  L.vouts = up(L.plan + L.plan_tiles + tile_cap * sizeof(TileRef));
-  L.vnouts = up(L.vouts + sizeof(b200tfs_output) * n * kFusedMaxOutputs);
-  L.vstatus = up(L.vnouts + 4 * n);
-  L.var = up(L.vstatus + 4 * n);
-  L.bytes = L.var + var_plan_layout(n, var_tile_cap).bytes;
+  L.outs = R.take(sizeof(b200tfs_output) * n * (kFusedMaxOutputs + 1), 256);
+  L.nouts = R.take(4 * n, 256);
+  L.specs = R.take(sizeof(b200tfs_model_spec) * n, 256);
+  L.status = R.take(4 * n, 256);
+  L.spill = R.take(4 * n, 256);
+  L.kst = R.take(4 * n * n_keys, 256);
+  L.match = R.take(4 * n * n_keys, 256);
+  L.plan = R.take(g.end, 256);
+  L.plan_tiles = g.off_tiles;
+  L.vouts = R.take(sizeof(b200tfs_output) * n * kFusedMaxOutputs, 256);
+  L.vnouts = R.take(4 * n, 256);
+  L.vstatus = R.take(4 * n, 256);
+  L.var = R.take(V.bytes, 256);
+  L.var_status = L.var + V.status;
+  L.bytes = R.end;
   return L;
 }
 }  // namespace
@@ -2263,24 +2321,23 @@ int b200tfs_decode_concat(b200tfs_ctx* c, const void* arena_dev, int32_t n, cons
   // rec_off | rec_len | keys | key bytes: one upload (a captured call keeps a private copy)
   uint64_t key_bytes = 0;
   for (int k = 0; k < n_keys; ++k) key_bytes += (uint64_t)keys[k].key_len;
-  const uint64_t o_len = 8ull * n, o_keys = (o_len + 8ull * n + 15) & ~15ull, o_kb = o_keys + sizeof(ConcatKeyDev) * n_keys;
+  Layout K;
+  const uint64_t o_off = K.take(8ull * n), o_len = K.take(8ull * n), o_keys = K.take(sizeof(ConcatKeyDev) * n_keys), o_kb = K.take(key_bytes);
   Slot* slot;
-  if ((rc = claim_slot(c, o_kb + key_bytes + 16, &slot))) return rc;
-  uint8_t* h = (uint8_t*)slot->host.p;
-  uint8_t* sd = (uint8_t*)slot->dev.p;
-  memcpy(h, rec_off, 8ull * n);
-  memcpy(h + o_len, rec_len, 8ull * n);
-  uint64_t at = o_kb;
-  for (int k = 0; k < n_keys; ++k) {
-    ConcatKeyDev kd{sd + at, (uint8_t*)keys[k].dst, keys[k].dst_cap, (uint32_t)keys[k].key_len, 0u};
-    memcpy(h + o_keys + sizeof(ConcatKeyDev) * k, &kd, sizeof kd);
-    if (keys[k].key_len) memcpy(h + at, keys[k].key, (size_t)keys[k].key_len);
-    at += (uint64_t)keys[k].key_len;
-    c->concat_dst[k] = (uint8_t*)keys[k].dst;
-  }
-  if ((rc = upload_slot(c, slot, at))) return rc;
+  uint8_t* sd;
+  rc = upload_image(c, K.end, {{o_off, rec_off, 8ull * n}, {o_len, rec_len, 8ull * n}}, &sd, &slot, [&](uint8_t* h, uint8_t* dev) {
+    uint64_t at = o_kb;
+    for (int k = 0; k < n_keys; ++k) {
+      ConcatKeyDev kd{dev + at, (uint8_t*)keys[k].dst, keys[k].dst_cap, (uint32_t)keys[k].key_len, 0u};
+      memcpy(h + o_keys + sizeof(ConcatKeyDev) * k, &kd, sizeof kd);
+      if (keys[k].key_len) memcpy(h + at, keys[k].key, (size_t)keys[k].key_len);
+      at += (uint64_t)keys[k].key_len;
+    }
+  });
+  if (rc) return rc;
+  for (int k = 0; k < n_keys; ++k) c->concat_dst[k] = (uint8_t*)keys[k].dst;
   uint8_t* d = (uint8_t*)c->concat_dev.p;
-  const uint64_t* off_dev = (const uint64_t*)sd;
+  const uint64_t* off_dev = (const uint64_t*)(sd + o_off);
   CU(launch_parse_responses((const uint8_t*)arena_dev, off_dev, (const uint64_t*)(sd + o_len), n, kFusedMaxOutputs, (b200tfs_output*)(d + L.outs),
                             (int32_t*)(d + L.nouts), (b200tfs_model_spec*)(d + L.specs), (int32_t*)(d + L.status), nullptr, 0u,
                             (uint32_t*)(d + L.spill), c->stream));
@@ -2295,23 +2352,15 @@ int b200tfs_decode_concat(b200tfs_ctx* c, const void* arena_dev, int32_t n, cons
   CU(launch_concat_plan(cp, (uint32_t)tile_cap, c->stream));
   // packed-varint outputs: the single-launch decode's plan / count / emit over the table the plan kernel wrote (its dst_off is
   // the absolute address: dst 0, stride 0)
-  const VarPlanLayout V = var_plan_layout((uint64_t)n, var_tile_cap);
-  uint8_t* vd = d + L.var;
   VarPlan vp{};
   vp.outs = cp.vouts; vp.n_outs = cp.vn_outs; vp.rec_status = cp.vrec_status;
   vp.w = cp.w; vp.rec_off = off_dev;
-  if (n <= kFusedInlineRecs) for (int i = 0; i < n; ++i) vp.off_inl[i] = rec_off[i];
   vp.dst = nullptr; vp.dst_stride = 0; vp.n = (uint32_t)n; vp.tile_cap = (uint32_t)var_tile_cap;
-  vp.jobs = (VarJobDev*)(vd + V.jobs); vp.segs = (VarSeg*)(vd + V.segs); vp.tile_seg = (uint32_t*)(vd + V.tile_seg);
-  vp.tile_val = (uint32_t*)(vd + V.tile_val); vp.group_sum = (uint32_t*)(vd + V.group_sum);
-  vp.total = (unsigned long long*)(vd + V.total); vp.status = (int32_t*)(vd + V.status); vp.n_tiles = (uint32_t*)(vd + V.n_tiles);
-  CU(launch_vdec_plan(vp, c->stream));
-  VarTables tb{};
-  tb.segs = vp.segs; tb.tile_seg = vp.tile_seg; tb.jobs = vp.jobs; tb.n_tiles = vp.tile_cap; tb.n_tiles_dev = vp.n_tiles;
-  CU(launch_vdec_dev(tb, (uint32_t)c->sm_count * 4, c->stream));
+  if ((rc = launch_varint_tail(c, vp, d + L.var, rec_off))) return rc;
   if (slot->done && !c->capturing) { CU(cudaEventRecord(slot->done, c->stream)); slot->pending = true; }   // the kernels read the upload
-  c->launches += 6;
-  c->concat_n = n; c->concat_k = n_keys; c->concat_vouts_off = L.vouts; c->concat_vstat_off = L.var + V.status;
+  c->launches += 3;
+  c->concat_n = n; c->concat_k = n_keys;
+  c->concat_vouts_off = L.vouts; c->concat_vstat_off = L.var_status; c->concat_specs_off = L.specs; c->concat_status_off = L.status;
   return B200TFS_OK;
 }
 
@@ -2333,7 +2382,6 @@ int b200tfs_concat_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_ou
   if (n == 0) return B200TFS_OK;
   CU(cudaSetDevice(c->device));
   CU(cudaStreamSynchronize(c->stream));
-  const ConcatLayout L = concat_layout((uint64_t)n, (uint64_t)n_keys, 0, 0);   // specs and status do not depend on the tile bounds
   const uint8_t* d = (const uint8_t*)c->concat_dev.p;
   if (outs) {
     std::vector<b200tfs_output> v((size_t)n * kFusedMaxOutputs);
@@ -2343,15 +2391,14 @@ int b200tfs_concat_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_ou
     for (int r = 0; r < n; ++r)
       for (int k = 0; k < n_keys; ++k) {
         b200tfs_output o = v[(size_t)r * kFusedMaxOutputs + k];
-        const int32_t s = vs[(size_t)r * kFusedMaxOutputs + k];
-        if (s != kVarSlotIdle) { o.status = s; o.flags |= B200TFS_OF_DEVICE_VARINT; }
+        fold_varint_status(o, vs[(size_t)r * kFusedMaxOutputs + k]);
         o.dst_off -= (uint64_t)(uintptr_t)c->concat_dst[k];
         outs[(size_t)r * n_keys + k] = o;
       }
   }
-  if (specs) CU(cudaMemcpy(specs, d + L.specs, sizeof(b200tfs_model_spec) * (uint64_t)n, cudaMemcpyDeviceToHost));
+  if (specs) CU(cudaMemcpy(specs, d + c->concat_specs_off, sizeof(b200tfs_model_spec) * (uint64_t)n, cudaMemcpyDeviceToHost));
   if (rec_status) {
-    CU(cudaMemcpy(rec_status, d + L.status, 4ull * n, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(rec_status, d + c->concat_status_off, 4ull * n, cudaMemcpyDeviceToHost));
     for (int r = 0; r < n; ++r) if (rec_status[r] == B200TFS_E_SPILL || rec_status[r] == B200TFS_E_SIZE) rec_status[r] = B200TFS_E_NONCANONICAL;
   }
   return B200TFS_OK;

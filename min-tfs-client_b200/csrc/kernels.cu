@@ -1074,10 +1074,10 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
   __shared__ unsigned long long warp_sum[kConcatPlanThreads / 32];
   __shared__ uint32_t ref_rec;
   const uint32_t n = cp.n, nk = cp.n_keys;
-  MoveItem* items = reinterpret_cast<MoveItem*>(cp.plan + ((sizeof(PlanHeader) + 15) & ~15ull));
   const uint64_t n_items = (uint64_t)n * nk * B200TFS_MAX_RUNS;
-  const uint64_t off_tiles = (((sizeof(PlanHeader) + 15) & ~15ull) + n_items * sizeof(MoveItem) + 15) & ~15ull;
-  TileRef* tref = reinterpret_cast<TileRef*>(cp.plan + off_tiles);
+  const PlanGeometry g = plan_geometry(n_items, 0, 0);   // tile refs run from off_tiles to the end of the image; no small items
+  MoveItem* items = reinterpret_cast<MoveItem*>(cp.plan + g.off_items);
+  TileRef* tref = reinterpret_cast<TileRef*>(cp.plan + g.off_tiles);
   uint64_t tile_carry = 0;
   for (uint32_t k = 0; k < nk; ++k) {
     const ConcatKeyDev key = cp.keys[k];
@@ -1168,9 +1168,9 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
     ph.n_items = (uint32_t)n_items;
     ph.n_tiles = (uint32_t)min(tile_carry, (uint64_t)cp.tile_cap);
     ph.vec_per_tile = cp.vpt;
-    ph.off_items = (uint32_t)((sizeof(PlanHeader) + 15) & ~15ull);
-    ph.off_tiles = (uint32_t)off_tiles;
-    ph.off_small = (uint32_t)off_tiles;
+    ph.off_items = (uint32_t)g.off_items;
+    ph.off_tiles = (uint32_t)g.off_tiles;
+    ph.off_small = (uint32_t)g.off_small;
     ph.guard_div = 1;
     *reinterpret_cast<PlanHeader*>(cp.plan) = ph;
   }

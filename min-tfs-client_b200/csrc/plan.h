@@ -57,6 +57,25 @@ struct PlanHeader {
   const uint32_t* guard;
 };
 
+#if defined(__CUDACC__)
+#define B2_PLAN_HD __host__ __device__ __forceinline__
+#else
+#define B2_PLAN_HD inline
+#endif
+
+// Where the tables of a plan image lie: PlanHeader | MoveItem[n_items] | TileRef[n_tile_refs] | SmallItem[n_small], and `end`,
+// where the header blob starts.  The host planner (build_plan), the scratch sizing of b200tfs_decode_concat and
+// concat_plan_kernel, which writes such an image on the device, all take it from here.
+struct PlanGeometry { uint64_t off_items, off_tiles, off_small, end; };
+B2_PLAN_HD PlanGeometry plan_geometry(uint64_t n_items, uint64_t n_tile_refs, uint64_t n_small) {
+  PlanGeometry g;
+  g.off_items = (sizeof(PlanHeader) + 15) & ~15ull;
+  g.off_tiles = g.off_items + n_items * sizeof(MoveItem);
+  g.off_small = (g.off_tiles + n_tile_refs * sizeof(TileRef) + 15) & ~15ull;
+  g.end = g.off_small + n_small * sizeof(SmallItem);
+  return g;
+}
+
 constexpr uint32_t kInlinePlanBytes = 3840;  // fits the classic 4 KB kernel-parameter window
 struct InlinePlan { uint8_t bytes[kInlinePlanBytes]; };
 
@@ -283,11 +302,6 @@ struct FrameTables {
 };
 
 // decode tiles of a chunk [src, src + n): aligned windows of kVarTileBytes starting at src rounded down to 16
-#if defined(__CUDACC__)
-#define B2_PLAN_HD __host__ __device__ __forceinline__
-#else
-#define B2_PLAN_HD inline
-#endif
 B2_PLAN_HD uint64_t var_decode_tiles(const void* src, uint64_t n) {
   return n ? (((uint64_t)((uintptr_t)src & 15) + n + kVarTileBytes - 1) / kVarTileBytes) : 0;
 }

@@ -204,6 +204,18 @@ _FUSED_MOVES = frozenset((1, 2, 8, 18))   # DT_FLOAT, DT_DOUBLE, DT_COMPLEX64, D
 _VARINT_DTYPES = frozenset((3, 4, 5, 6, 9, 10, 14, 17, 19, 22, 23))
 
 
+def _narrowing_cast(out_dtypes: Mapping) -> Optional[int]:
+    """DT_HALF or DT_BFLOAT16 when every requested cast is that one narrowing of float32 (b200tfs_set_decode_cast does it in
+    the decode launch itself), else None."""
+    try:
+        wanted = {int(enum_for_numpy(np.dtype(v).type)) for v in out_dtypes.values()}
+    except (KeyError, ValueError, TypeError):
+        return None
+    if len(wanted) == 1 and next(iter(wanted)) in (int(DT_HALF), int(DT_BFLOAT16)):
+        return next(iter(wanted))
+    return None
+
+
 def _device_varint(o: N.Output) -> bool:
     """A varint output the single-launch decode decoded into its range.  One it decoded with an error, or could not lay out
     (E_SIZE), reads afterwards as the table reads with the switch off - status OK, tabulated only - so that the unpack route
@@ -486,6 +498,31 @@ class Codec:
     def _text(buf: np.ndarray, off: int, length: int) -> str:
         return buf[off: off + length].tobytes().decode("utf-8")
 
+    @staticmethod
+    def _spec(buf: np.ndarray, base: int, s: N.ModelSpec) -> "DecodedSpec":
+        """The model_spec of the record at `base` (the table's offsets are record-relative)."""
+        t = Codec._text
+        return DecodedSpec(t(buf, base + s.name_off, s.name_len), int(s.version), bool(s.has_version),
+                           t(buf, base + s.label_off, s.label_len), t(buf, base + s.signature_off, s.signature_len))
+
+    def _unpack_to_host(self, jobs, rec_offsets) -> List[np.ndarray]:
+        """b200tfs_unpack_outputs_host over (Output, numpy type, dst dtype code, shape) jobs whose records start at
+        `rec_offsets` of the staged wire: one new array per job.  The first job that failed raises - ValueError when the
+        values do not fill the shape."""
+        m = len(jobs)
+        arrays = [np.empty(shape, dtype=np_type) for _, np_type, _, shape in jobs]
+        outs = (N.Output * m)(*[j[0] for j in jobs])
+        dst = (C.c_void_p * m)(*[a.ctypes.data if a.size else None for a in arrays])
+        codes = (C.c_int32 * m)(*[j[2] for j in jobs])
+        status = (C.c_int32 * m)()
+        rec = (C.c_uint64 * m)(*rec_offsets)
+        N.check(self._lib.b200tfs_unpack_outputs_host(self._ctx, m, outs, rec, dst, codes, status))
+        for k, (_, _, _, shape) in enumerate(jobs):
+            if status[k] == N.E_SHAPE:
+                raise ValueError(f"cannot reshape array into shape {shape}")
+            N.check(status[k])
+        return arrays
+
     def parse_predict_responses(self, wires: Sequence[bytes], max_outputs: int = 16) -> List[ParsedResponse]:
         """Run the parse kernel over each PredictResponse; raises DecodeError like ``FromString``.  ``max_outputs`` sizes
         the first attempt only: a response with more outputs is parsed again with a table twice as wide, and so on
@@ -517,10 +554,7 @@ class Codec:
             for j in range(n_outs[i]):
                 o = outs[i * max_outputs + j]
                 table[self._text(buf, base + o.key_off, o.key_len)] = o
-            s = specs[i]
-            spec = DecodedSpec(self._text(buf, base + s.name_off, s.name_len), int(s.version), bool(s.has_version),
-                               self._text(buf, base + s.label_off, s.label_len), self._text(buf, base + s.signature_off, s.signature_len))
-            parsed.append(ParsedResponse(buf, int(off[i]), int(ln[i]), int(status[i]), table, spec))
+            parsed.append(ParsedResponse(buf, int(off[i]), int(ln[i]), int(status[i]), table, self._spec(buf, base, specs[i])))
         return parsed
 
     def _resolve_output(self, o: N.Output, strict: bool, out_dtype):
@@ -601,12 +635,9 @@ class Codec:
                 return fused
         elif out_dtypes and len(wires) and not strict:
             # every requested cast is the same narrowing of float32 (BASELINE config C4): one launch does it (b200tfs_set_decode_cast)
-            try:
-                wanted = {int(enum_for_numpy(np.dtype(v).type)) for v in out_dtypes.values()}
-            except (KeyError, ValueError, TypeError):
-                wanted = set()
-            if len(wanted) == 1 and next(iter(wanted)) in (int(DT_HALF), int(DT_BFLOAT16)):
-                fused = self._decode_fused(wires, strict, cast=(next(iter(wanted)), dict(out_dtypes)))
+            cast_code = _narrowing_cast(out_dtypes)
+            if cast_code is not None:
+                fused = self._decode_fused(wires, strict, cast=(cast_code, dict(out_dtypes)))
                 if fused is not None:
                     return fused
         return self._decode_two_phase(wires, strict, out_dtypes, max_outputs)
@@ -631,19 +662,9 @@ class Codec:
                 np_type, dst_code, shape = self._resolve_output(o, strict, od)
                 jobs.append((i, key, o, np_type, dst_code, shape))
         if jobs:
-            m = len(jobs)
-            outs = (N.Output * m)(*[j[2] for j in jobs])
-            arrays = [np.empty(j[5], dtype=j[3]) for j in jobs]
-            dst = (C.c_void_p * m)(*[a.ctypes.data if a.size else None for a in arrays])
-            codes = (C.c_int32 * m)(*[j[4] for j in jobs])
-            status = (C.c_int32 * m)()
-            rec = (C.c_uint64 * m)(*[parsed[j[0]].offset for j in jobs])
-            N.check(self._lib.b200tfs_unpack_outputs_host(self._ctx, m, outs, rec, dst, codes, status))
-            for k, (i, key, o, np_type, dst_code, shape) in enumerate(jobs):
-                if status[k] == N.E_SHAPE:
-                    raise ValueError(f"cannot reshape array into shape {shape}")
-                N.check(status[k])
-                results[i][0][key] = arrays[k]
+            arrays = self._unpack_to_host([j[2:] for j in jobs], [parsed[j[0]].offset for j in jobs])
+            for (i, key, *_), a in zip(jobs, arrays):
+                results[i][0][key] = a
         return results
 
     def _fused_launch(self, wires: Sequence[bytes], cast_code: int = 0):
@@ -724,11 +745,8 @@ class Codec:
         jobs = []
         for i in range(n):
             base = int(off[i])
-            s = specs[i]
-            spec = DecodedSpec(self._text(buf, base + s.name_off, s.name_len), int(s.version), bool(s.has_version),
-                               self._text(buf, base + s.label_off, s.label_len), self._text(buf, base + s.signature_off, s.signature_len))
             arrays: Dict[str, np.ndarray] = {}
-            results.append((arrays, spec))
+            results.append((arrays, self._spec(buf, base, specs[i])))
             for j in range(n_outs[i]):
                 o = outs[i * K + j]
                 key = self._text(buf, base + o.key_off, o.key_len)
@@ -753,19 +771,9 @@ class Codec:
                 else:
                     jobs.append((i, key, o, np_type, dst_code, shape))
         if jobs:
-            m = len(jobs)
-            o_arr = (N.Output * m)(*[j[2] for j in jobs])
-            made = [np.empty(j[5], dtype=j[3]) for j in jobs]
-            ptrs = (C.c_void_p * m)(*[a.ctypes.data if a.size else None for a in made])
-            codes = (C.c_int32 * m)(*[j[4] for j in jobs])
-            st = (C.c_int32 * m)()
-            rec = (C.c_uint64 * m)(*[int(off[j[0]]) for j in jobs])
-            N.check(self._lib.b200tfs_unpack_outputs_host(self._ctx, m, o_arr, rec, ptrs, codes, st))
-            for k, (i, key, o, np_type, dst_code, shape) in enumerate(jobs):
-                if st[k] == N.E_SHAPE:
-                    raise ValueError(f"cannot reshape array into shape {shape}")
-                N.check(st[k])
-                results[i][0][key] = made[k]
+            made = self._unpack_to_host([j[2:] for j in jobs], [int(off[j[0]]) for j in jobs])
+            for (i, key, *_), a in zip(jobs, made):
+                results[i][0][key] = a
         return results
 
     # ---- batch decode into one tensor per key ------------------------------------------------------
@@ -860,15 +868,9 @@ class Codec:
         kb = [k.encode("utf-8") for k in keys]
         cast_code = 0
         if out_dtypes:
-            if strict:
+            cast_code = None if strict else _narrowing_cast(out_dtypes)
+            if cast_code is None:
                 return None
-            try:
-                wanted = {int(enum_for_numpy(np.dtype(v).type)) for v in out_dtypes.values()}
-            except (KeyError, ValueError, TypeError):
-                return None
-            if len(wanted) != 1 or next(iter(wanted)) not in (int(DT_HALF), int(DT_BFLOAT16)):
-                return None
-            cast_code = next(iter(wanted))
         ck = (N.ConcatKey * nk)()
         for i, k in enumerate(kb):
             ck[i].key, ck[i].key_len = k, len(k)
@@ -960,12 +962,7 @@ class Codec:
                 result[k] = dev[i]
         self.sync()
         self.concat_device_calls += 1
-        spec_list = []
-        for r in range(n):
-            base, s = int(off[r]), specs[r]
-            spec_list.append(DecodedSpec(self._text(buf, base + s.name_off, s.name_len), int(s.version), bool(s.has_version),
-                                         self._text(buf, base + s.label_off, s.label_len), self._text(buf, base + s.signature_off, s.signature_len)))
-        return result, spec_list
+        return result, [self._spec(buf, int(off[r]), specs[r]) for r in range(n)]
 
     @staticmethod
     def _decode_strings(buf: np.ndarray, base: int, o: N.Output, rec_len: int = 0, key: str = "") -> np.ndarray:
@@ -1019,10 +1016,7 @@ class Codec:
         np_type, dst_code, shape = self._resolve_output(o, strict, None)
         if dst_code != int(o.dtype) or np.dtype(np_type) != arr.dtype or tuple(shape) != arr.shape:
             return None
-        s = specs[0]
-        spec = DecodedSpec(self._text(buf, s.name_off, s.name_len), int(s.version), bool(s.has_version),
-                           self._text(buf, s.label_off, s.label_len), self._text(buf, s.signature_off, s.signature_len))
-        return {key: arr}, spec
+        return {key: arr}, self._spec(buf, 0, specs[0])
 
     def decode_tensor_protos(self, wires: Sequence[bytes], *, strict: bool = False, out_dtype=None) -> List[np.ndarray]:
         """``tensor_proto_to_ndarray`` for serialised TensorProto messages."""
@@ -1044,19 +1038,9 @@ class Codec:
             np_type, dst_code, shape = self._resolve_output(o, strict, out_dtype)
             jobs.append((i, o, np_type, dst_code, shape))
         if jobs:
-            m = len(jobs)
-            o_arr = (N.Output * m)(*[j[1] for j in jobs])
-            arrays = [np.empty(j[4], dtype=j[2]) for j in jobs]
-            dst = (C.c_void_p * m)(*[a.ctypes.data if a.size else None for a in arrays])
-            codes = (C.c_int32 * m)(*[j[3] for j in jobs])
-            st = (C.c_int32 * m)()
-            rec = (C.c_uint64 * m)(*[int(off[j[0]]) for j in jobs])
-            N.check(self._lib.b200tfs_unpack_outputs_host(self._ctx, m, o_arr, rec, dst, codes, st))
-            for k, (i, o, np_type, dst_code, shape) in enumerate(jobs):
-                if st[k] == N.E_SHAPE:
-                    raise ValueError(f"cannot reshape array into shape {shape}")
-                N.check(st[k])
-                results[i] = arrays[k]
+            arrays = self._unpack_to_host([j[1:] for j in jobs], [int(off[j[0]]) for j in jobs])
+            for (i, *_), a in zip(jobs, arrays):
+                results[i] = a
         return results  # type: ignore[return-value]
 
 
