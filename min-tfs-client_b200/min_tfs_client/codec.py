@@ -14,6 +14,8 @@ their TensorProto is assembled on the host and spliced into the request by the k
 """
 from __future__ import annotations
 
+import collections
+import contextlib
 import ctypes as C
 import threading
 from typing import Dict, Iterable, List, Mapping, Optional, Sequence, Tuple, Union
@@ -216,18 +218,56 @@ def _narrowing_cast(out_dtypes: Mapping) -> Optional[int]:
     return None
 
 
-def _device_varint(o: N.Output) -> bool:
-    """A varint output the single-launch decode decoded into its range.  One it decoded with an error, or could not lay out
-    (E_SIZE), reads afterwards as the table reads with the switch off - status OK, tabulated only - so that the unpack route
-    finishes it and raises exactly what it raises today."""
-    if o.flags & N.OF_DEVICE_VARINT:
-        if o.status == N.OK:
-            return True
-        o.flags &= ~N.OF_DEVICE_VARINT
-        o.status = N.OK
-    elif o.status == N.E_SIZE and int(o.dtype) in _VARINT_DTYPES:
-        o.status = N.OK     # not laid out: never viewed, the unpack route (or the caller) decodes it
-    return False
+def _narrowing_fits(dtype: int, key, out_dtypes: Mapping) -> bool:
+    """The narrowing cast applies to every float32 output: it is right only when exactly those were asked for."""
+    return (int(dtype) == DT_FLOAT) == (key in out_dtypes)
+
+
+def _to_unpack(o: N.Output, unfinished: int = N.E_SIZE) -> bool:
+    """Make a table entry a device decode did not finish - a varint output it decoded with an error, or status `unfinished`
+    (E_SIZE: no room in the fused launch's slot) - read as the walk tabulated it: status OK, no OF_DEVICE_VARINT.  The unpack
+    route then finishes it and raises what it raises for it.  False for an entry with an error of its own."""
+    if not (o.flags & N.OF_DEVICE_VARINT or o.status in (N.OK, unfinished)):
+        return False
+    o.flags &= ~N.OF_DEVICE_VARINT
+    o.status = N.OK
+    return True
+
+
+def _stored(o: N.Output) -> bool:
+    """Whether the fused launch stored this output in its slot: a dtype it moves itself, or a varint output it decoded.  Decided
+    before _resolve_output, which may raise.  An output the launch did not finish goes to the unpack route."""
+    if o.flags & N.OF_DEVICE_VARINT and o.status == N.OK:
+        return True
+    if o.flags & N.OF_DEVICE_VARINT or o.status == N.E_SIZE:
+        _to_unpack(o)
+        return False
+    return o.status == N.OK and int(o.dtype) in _FUSED_MOVES and bool(o.n_runs and o.n_elems)
+
+
+def _stored_as(o: N.Output, dst_code: int, cast_code: int = 0) -> bool:
+    """Whether the resolved destination dtype is what the launch wrote: the output's own, or the narrowing of a float32 output
+    (strict DT_HALF resolves to half_val read as values, the launch wrote TF's bit patterns)."""
+    return dst_code == int(o.dtype) or bool(cast_code) and int(o.dtype) == DT_FLOAT and dst_code == cast_code
+
+
+def _check_out(key, dst, dtype, shape, contiguous: bool = False):
+    """ValueError unless the caller's destination `dst` (``out={key: dst}``) holds exactly `dtype` and `shape` - and, with
+    `contiguous`, a numpy one is C-contiguous.  Returns (pointer, keep-alive) of a device destination, None for a numpy one."""
+    shape = tuple(shape)
+    if D.is_device_object(dst):
+        ptr, dshape, ddtype, keep = D.device_view(dst)
+        if ddtype != dtype or tuple(dshape) != shape:
+            raise ValueError(f"out[{key!r}]: {ddtype}{tuple(dshape)} does not match the decoded {dtype}{shape}")
+        return ptr, keep
+    if not isinstance(dst, np.ndarray) or dst.dtype != dtype or dst.shape != shape or (contiguous and not dst.flags.c_contiguous):
+        raise ValueError(f"out[{key!r}] does not match the decoded {dtype}{shape}")
+    return None
+
+
+# what one fused launch left on the host: n records staged in buf at off, their outputs in dst (a slot of stride bytes per
+# record), each record's table ({key: Output}) and model_spec
+_Launch = collections.namedtuple("_Launch", "n buf off dst stride tables specs")
 
 
 class OpenResponse:
@@ -235,6 +275,7 @@ class OpenResponse:
 
     def __init__(self, codec, buf, base, dst, table):
         self._codec, self._buf, self._base, self._dst, self.table = codec, buf, base, dst, table
+        self._stored = {k for k, o in table.items() if _stored(o)}
         self._handed = set()
 
     def wire_of(self, key) -> bytes:
@@ -245,12 +286,11 @@ class OpenResponse:
         """The decoded output, or None when the launch did not move it (varint-packed, string, tensor_content only): the
         caller then decodes ``wire_of(key)`` on its own.  Raises what the reference raises for this output."""
         o = self.table[key]
-        dev_varint = _device_varint(o)
-        if not dev_varint and (int(o.dtype) not in _FUSED_MOVES or o.status != N.OK or not o.n_runs or not o.n_elems):
+        if key not in self._stored:
             return None
         np_type, dst_code, shape = self._codec._resolve_output(o, strict, None)
-        if dev_varint and dst_code != int(o.dtype):
-            return None      # strict DT_HALF: the reference reads half_val as values, the launch wrote TF's bit patterns
+        if not _stored_as(o, dst_code):
+            return None
         at = int(o.dst_off)
         arr = self._dst[at: at + int(o.dst_bytes)].view(np_type).reshape(shape)
         if key in self._handed:      # tensor_proto_to_ndarray returns a fresh array per call (tensors.py:46): never alias two results
@@ -505,23 +545,32 @@ class Codec:
         return DecodedSpec(t(buf, base + s.name_off, s.name_len), int(s.version), bool(s.has_version),
                            t(buf, base + s.label_off, s.label_len), t(buf, base + s.signature_off, s.signature_len))
 
-    def _unpack_to_host(self, jobs, rec_offsets) -> List[np.ndarray]:
-        """b200tfs_unpack_outputs_host over (Output, numpy type, dst dtype code, shape) jobs whose records start at
-        `rec_offsets` of the staged wire: one new array per job.  The first job that failed raises - ValueError when the
-        values do not fill the shape."""
+    @staticmethod
+    def _table(buf: np.ndarray, off, outs, n_outs, width: int, i: int) -> Dict[str, N.Output]:
+        """{key: Output} of record i, from a table of `width` entries per record (its offsets are relative to the record)."""
+        base = int(off[i])
+        return {Codec._text(buf, base + o.key_off, o.key_len): o for o in (outs[i * width + j] for j in range(n_outs[i]))}
+
+    def _unpack_to_host(self, jobs):
+        """b200tfs_unpack_outputs_host over (into, key, Output, numpy type, dst dtype code, shape, record offset) jobs, the
+        record offsets into the staged wire: one new array per job, stored at ``into[key]``.  The first job that failed
+        raises - ValueError when the values do not fill the shape."""
         m = len(jobs)
-        arrays = [np.empty(shape, dtype=np_type) for _, np_type, _, shape in jobs]
-        outs = (N.Output * m)(*[j[0] for j in jobs])
+        if not m:
+            return
+        arrays = [np.empty(j[5], dtype=j[3]) for j in jobs]
+        outs = (N.Output * m)(*[j[2] for j in jobs])
         dst = (C.c_void_p * m)(*[a.ctypes.data if a.size else None for a in arrays])
-        codes = (C.c_int32 * m)(*[j[2] for j in jobs])
+        codes = (C.c_int32 * m)(*[j[4] for j in jobs])
         status = (C.c_int32 * m)()
-        rec = (C.c_uint64 * m)(*rec_offsets)
+        rec = (C.c_uint64 * m)(*[j[6] for j in jobs])
         N.check(self._lib.b200tfs_unpack_outputs_host(self._ctx, m, outs, rec, dst, codes, status))
-        for k, (_, _, _, shape) in enumerate(jobs):
+        for k, j in enumerate(jobs):
             if status[k] == N.E_SHAPE:
-                raise ValueError(f"cannot reshape array into shape {shape}")
+                raise ValueError(f"cannot reshape array into shape {j[5]}")
             N.check(status[k])
-        return arrays
+        for (into, key, *_), a in zip(jobs, arrays):
+            into[key] = a
 
     def parse_predict_responses(self, wires: Sequence[bytes], max_outputs: int = 16) -> List[ParsedResponse]:
         """Run the parse kernel over each PredictResponse; raises DecodeError like ``FromString``.  ``max_outputs`` sizes
@@ -549,12 +598,8 @@ class Codec:
                 from google.protobuf.message import DecodeError
 
                 raise DecodeError(f"Error parsing message (response {i}, status {status[i]})")
-            table = {}
-            base = int(off[i])  # table offsets are relative to the record
-            for j in range(n_outs[i]):
-                o = outs[i * max_outputs + j]
-                table[self._text(buf, base + o.key_off, o.key_len)] = o
-            parsed.append(ParsedResponse(buf, int(off[i]), int(ln[i]), int(status[i]), table, self._spec(buf, base, specs[i])))
+            table = self._table(buf, off, outs, n_outs, max_outputs, i)
+            parsed.append(ParsedResponse(buf, int(off[i]), int(ln[i]), int(status[i]), table, self._spec(buf, int(off[i]), specs[i])))
         return parsed
 
     def _resolve_output(self, o: N.Output, strict: bool, out_dtype):
@@ -629,88 +674,84 @@ class Codec:
         rejects); the default additionally accepts what TF itself emits: ``tensor_content``, rank-0
         tensors, complex pairs, bfloat16, and reads ``half_val`` as bit patterns.
         """
+        fused = None
         if out_dtypes is None and len(wires):
             fused = self._decode_fused(wires, strict)
-            if fused is not None:
-                return fused
-        elif out_dtypes and len(wires) and not strict:
+        elif out_dtypes and len(wires) and not strict and _narrowing_cast(out_dtypes) is not None:
             # every requested cast is the same narrowing of float32 (BASELINE config C4): one launch does it (b200tfs_set_decode_cast)
-            cast_code = _narrowing_cast(out_dtypes)
-            if cast_code is not None:
-                fused = self._decode_fused(wires, strict, cast=(cast_code, dict(out_dtypes)))
-                if fused is not None:
-                    return fused
-        return self._decode_two_phase(wires, strict, out_dtypes, max_outputs)
+            fused = self._decode_fused(wires, strict, dict(out_dtypes))
+        return fused if fused is not None else self._decode_two_phase(wires, strict, out_dtypes, max_outputs)
 
     def _decode_two_phase(self, wires, strict, out_dtypes, max_outputs, keys=None):
         """The parse kernel, then the unpack of every output - of the outputs named in `keys` only, when given (the others are
         neither converted nor checked)."""
         parsed = self.parse_predict_responses(wires, max_outputs=max_outputs)
-        if not parsed:
-            return []
-        jobs = []  # (response idx, key, Output, np_type, dst_code, shape)
+        jobs = []
         results: List[Tuple[Dict[str, np.ndarray], DecodedSpec]] = []
-        for i, pr in enumerate(parsed):
-            results.append(({}, pr.model_spec))
+        for pr in parsed:
+            arrays: Dict[str, np.ndarray] = {}
+            results.append((arrays, pr.model_spec))
             for key, o in pr.outputs.items():
                 if keys is not None and key not in keys:
                     continue
-                od = out_dtypes.get(key) if out_dtypes else None
                 if int(o.dtype) == DT_STRING and o.status == N.OK:
-                    results[i][0][key] = self._decode_strings(pr.wire, pr.offset, o, pr.length, key)
+                    arrays[key] = self._decode_strings(pr.wire, pr.offset, o, pr.length, key)
                     continue
-                np_type, dst_code, shape = self._resolve_output(o, strict, od)
-                jobs.append((i, key, o, np_type, dst_code, shape))
-        if jobs:
-            arrays = self._unpack_to_host([j[2:] for j in jobs], [parsed[j[0]].offset for j in jobs])
-            for (i, key, *_), a in zip(jobs, arrays):
-                results[i][0][key] = a
+                np_type, dst_code, shape = self._resolve_output(o, strict, out_dtypes.get(key) if out_dtypes else None)
+                jobs.append((arrays, key, o, np_type, dst_code, shape, pr.offset))
+        self._unpack_to_host(jobs)
         return results
 
-    def _fused_launch(self, wires: Sequence[bytes], cast_code: int = 0):
-        """H2D of the wire, decode_fused_kernel, D2H of the decoded fixed-width outputs, one synchronise.  None if any
-        record was not tabulated (malformed, or more than FUSED_MAX_OUTPUTS outputs)."""
-        n = len(wires)
-        buf, off, ln = self._pack_wires(wires)
-        K = N.FUSED_MAX_OUTPUTS
-        stride, varints = self._slot_stride(buf, off, ln)
-        dst = np.empty(n * stride, dtype=np.uint8)
+    @contextlib.contextmanager
+    def _decode_modes(self, cast_code: int = 0, varints: bool = False):
+        """The context's narrowing cast and varint decode switched on for the native calls inside, and off after them."""
         if cast_code:
             N.check(self._lib.b200tfs_set_decode_cast(self._ctx, cast_code))
         if varints:
             N.check(self._lib.b200tfs_set_decode_varints(self._ctx, 1))
         try:
-            N.check(self._lib.b200tfs_decode_responses_host_async(self._ctx, buf.ctypes.data, n, off, ln, dst.ctypes.data, stride))
+            yield
         finally:
             if cast_code:
                 N.check(self._lib.b200tfs_set_decode_cast(self._ctx, 0))
             if varints:
                 N.check(self._lib.b200tfs_set_decode_varints(self._ctx, 0))
-        outs = (N.Output * (n * K))()
+
+    def _fused_launch(self, wires: Sequence[bytes], cast_code: int = 0, dst: Optional[np.ndarray] = None,
+                      stride: int = 0) -> Optional["_Launch"]:
+        """H2D of the wire, decode_fused_kernel, D2H of the decoded fixed-width outputs, one synchronise, into slots sized by
+        _slot_stride - or into the caller's page-locked `dst` at `stride`, varint decode off.  None if any record was not
+        tabulated (malformed, or more than FUSED_MAX_OUTPUTS outputs)."""
+        n = len(wires)
+        buf, off, ln = self._pack_wires(wires)
+        varints = False
+        if dst is None:
+            stride, varints = self._slot_stride(buf, off, ln)
+            dst = np.empty(n * stride, dtype=np.uint8)
+        with self._decode_modes(cast_code, varints):
+            N.check(self._lib.b200tfs_decode_responses_host_async(self._ctx, buf.ctypes.data, n, off, ln, dst.ctypes.data, stride))
+        outs = (N.Output * (n * N.FUSED_MAX_OUTPUTS))()
         n_outs = (C.c_int32 * n)()
         specs = (N.ModelSpec * n)()
         status = (C.c_int32 * n)()
         N.check(self._lib.b200tfs_decode_results(self._ctx, n, outs, n_outs, specs, status))   # synchronises
         if any(status[i] != N.OK for i in range(n)):
             return None
-        return n, buf, off, dst, stride, outs, n_outs, specs
+        tables = [self._table(buf, off, outs, n_outs, N.FUSED_MAX_OUTPUTS, i) for i in range(n)]
+        return _Launch(n, buf, off, dst, stride, tables, specs)
 
     def open_predict_response(self, wire: bytes) -> Optional["OpenResponse"]:
         """Decode one PredictResponse now, hand its outputs out later (``PredictResponseView.outputs``): the launch moves
         every fixed-width output; ``OpenResponse.array(key, strict)`` applies the reference's per-output rules on demand."""
         if not len(wire):
             return None
-        launched = self._fused_launch([wire])
-        if launched is None:
+        launch = self._fused_launch([wire])
+        if launch is None:
             return None
-        _, buf, off, dst, _, outs, n_outs, _ = launched
-        table = {}
-        for j in range(n_outs[0]):
-            o = outs[j]
-            table[self._text(buf, int(off[0]) + o.key_off, o.key_len)] = o
-            if o.n_elems and int(o.dtype) in _VARINT_DTYPES:
-                self._seen_varints = True
-        return OpenResponse(self, buf, int(off[0]), dst, table)
+        table = launch.tables[0]
+        if any(o.n_elems and int(o.dtype) in _VARINT_DTYPES for o in table.values()):
+            self._seen_varints = True
+        return OpenResponse(self, launch.buf, int(launch.off[0]), launch.dst, table)
 
     def _slot_stride(self, buf, off, ln) -> Tuple[int, bool]:
         """(dst_stride, decode varints) for the records of ONE call.  Every fixed-width output fits the parent layout's stride
@@ -727,53 +768,41 @@ class Codec:
             return stride, False
         return max(stride, (need.value + 255) & ~255), True
 
-    def _decode_fused(self, wires: Sequence[bytes], strict: bool, cast=None):
+    def _decode_fused(self, wires: Sequence[bytes], strict: bool, cast_keys: Optional[Dict] = None):
         """One launch, one synchronise: tag walk (or framing-template check), destination layout and the move of every
         fixed-width output in ``decode_fused_kernel``; the outputs come back as views of one host buffer.  Once this codec has
         seen varint-packed outputs, the same launch decodes those too (b200tfs_set_decode_varints) and they come back as views
         as well; the ones it cannot finish (TF's padding, strict DT_HALF, rows of unpacked elements, errors) and
         tensor_content-only outputs are unpacked by a second one.  Returns None when
         a record needs the two-phase path (more than eight outputs, a malformed record: that path raises what the
-        reference raises)."""
-        cast_code, cast_keys = cast if cast else (0, {})
-        launched = self._fused_launch(wires, cast_code)
-        if launched is None:
+        reference raises).  `cast_keys`: out_dtypes asking for one narrowing of float32 (b200tfs_set_decode_cast)."""
+        cast_keys = cast_keys or {}
+        cast_code = _narrowing_cast(cast_keys) if cast_keys else 0
+        launch = self._fused_launch(wires, cast_code)
+        if launch is None:
             return None
-        n, buf, off, dst, stride, outs, n_outs, specs = launched
-        K = N.FUSED_MAX_OUTPUTS
         results: List[Tuple[Dict[str, np.ndarray], DecodedSpec]] = []
         jobs = []
-        for i in range(n):
-            base = int(off[i])
+        for i in range(launch.n):
+            base = int(launch.off[i])
             arrays: Dict[str, np.ndarray] = {}
-            results.append((arrays, self._spec(buf, base, specs[i])))
-            for j in range(n_outs[i]):
-                o = outs[i * K + j]
-                key = self._text(buf, base + o.key_off, o.key_len)
+            results.append((arrays, self._spec(launch.buf, base, launch.specs[i])))
+            for key, o in launch.tables[i].items():
                 if int(o.dtype) == DT_STRING and o.status == N.OK:
-                    arrays[key] = self._decode_strings(buf, base, o, len(wires[i]), key)
+                    arrays[key] = self._decode_strings(launch.buf, base, o, len(wires[i]), key)
                     continue
-                if cast_code and ((int(o.dtype) == 1) != (key in cast_keys)):
-                    return None      # the launch narrowed every float32 output: only right when exactly those were asked for
-                unplaced = o.status == N.E_SIZE   # no room in the slot (_slot_stride sizes it so that this does not happen)
-                if unplaced:
-                    o.status = N.OK               # ... as the walk tabulated it: the unpack route decodes it
-                dev_varint = False
+                if cast_code and not _narrowing_fits(o.dtype, key, cast_keys):
+                    return None
                 if int(o.dtype) in _VARINT_DTYPES and o.n_elems:
                     self._seen_varints = True
-                    dev_varint = _device_varint(o)
+                stored = _stored(o)
                 np_type, dst_code, shape = self._resolve_output(o, strict, cast_keys.get(key))
-                if not unplaced and ((dev_varint and dst_code == int(o.dtype)) or
-                                     o.status == N.OK and int(o.dtype) in _FUSED_MOVES and o.n_runs and o.n_elems and
-                                     (dst_code == int(o.dtype) or (cast_code and int(o.dtype) == 1 and dst_code == cast_code))):
-                    at = i * stride + int(o.dst_off)
-                    arrays[key] = dst[at: at + int(o.dst_bytes)].view(np_type).reshape(shape)
+                if stored and _stored_as(o, dst_code, cast_code):
+                    at = i * launch.stride + int(o.dst_off)
+                    arrays[key] = launch.dst[at: at + int(o.dst_bytes)].view(np_type).reshape(shape)
                 else:
-                    jobs.append((i, key, o, np_type, dst_code, shape))
-        if jobs:
-            made = self._unpack_to_host([j[2:] for j in jobs], [int(off[j[0]]) for j in jobs])
-            for (i, key, *_), a in zip(jobs, made):
-                results[i][0][key] = a
+                    jobs.append((arrays, key, o, np_type, dst_code, shape, base))
+        self._unpack_to_host(jobs)
         return results
 
     # ---- batch decode into one tensor per key ------------------------------------------------------
@@ -847,18 +876,13 @@ class Codec:
         dst = out.get(key)
         if dst is None:
             return self.device_array(arr) if device else arr
-        if D.is_device_object(dst):
-            ptr, shape, dtype, _keep = D.device_view(dst)
-            if dtype != arr.dtype or tuple(shape) != arr.shape:
-                raise ValueError(f"out[{key!r}]: {dtype}{tuple(shape)} does not match the decoded {arr.dtype}{arr.shape}")
-            if arr.nbytes:
-                a = np.ascontiguousarray(arr)
-                N.check(self._lib.b200tfs_memcpy_h2d(self._ctx, ptr, a.ctypes.data, a.nbytes))
-                self.sync()
-            return dst
-        if not isinstance(dst, np.ndarray) or dst.dtype != arr.dtype or dst.shape != arr.shape:
-            raise ValueError(f"out[{key!r}] does not match the decoded {arr.dtype}{arr.shape}")
-        np.copyto(dst, arr)
+        view = _check_out(key, dst, arr.dtype, arr.shape)
+        if view is None:
+            np.copyto(dst, arr)
+        elif arr.nbytes:
+            a = np.ascontiguousarray(arr)
+            N.check(self._lib.b200tfs_memcpy_h2d(self._ctx, view[0], a.ctypes.data, a.nbytes))
+            self.sync()
         return dst
 
     def _concat_device(self, wires, buf, off, ln, keys, strict, out_dtypes, device, out):
@@ -882,37 +906,27 @@ class Codec:
                 return None
             if strict and (c.dtype == DT_BFLOAT16 or c.dtype in (DT_COMPLEX64, DT_COMPLEX128)):
                 return None
-            if cast_code and ((c.dtype == DT_FLOAT) != (keys[i] in out_dtypes)):
-                return None       # the narrowing applies to every float32 output: only right when exactly those asked for it
+            if cast_code and not _narrowing_fits(c.dtype, keys[i], out_dtypes):
+                return None
             shapes.append(tuple(int(c.dims[d]) for d in range(c.rank)))
             np_types.append(np.dtype(numpy_for_enum(cast_code if cast_code and c.dtype == DT_FLOAT else int(c.dtype))))
         # destinations: the caller's device arrays, else device arrays of our own (returned, or copied into the host result)
         dev, ptrs, holds = [], [], []
         for i, k in enumerate(keys):
             dst = out.get(k)
-            if dst is not None and D.is_device_object(dst):
-                ptr, shape, dtype, keep = D.device_view(dst)
-                if dtype != np_types[i] or tuple(shape) != shapes[i]:
-                    raise ValueError(f"out[{k!r}]: {dtype}{tuple(shape)} does not match the decoded {np_types[i]}{shapes[i]}")
+            view = None if dst is None else _check_out(k, dst, np_types[i], shapes[i], contiguous=True)
+            if view is not None:
                 dev.append(dst)
-                ptrs.append(ptr)
-                holds.append(keep)
+                ptrs.append(view[0])
+                holds.append(view)
             else:
-                if dst is not None and (not isinstance(dst, np.ndarray) or dst.dtype != np_types[i] or dst.shape != shapes[i] or
-                                        not dst.flags.c_contiguous):
-                    raise ValueError(f"out[{k!r}] does not match the decoded {np_types[i]}{shapes[i]}")
                 a = D.DeviceArray(self, shapes[i], np_types[i])
                 dev.append(a)
                 ptrs.append(a.ptr)
             ck[i].dst, ck[i].dst_cap = ptrs[i], int(ck[i].bytes)
         wire = D.DeviceArray(self, (len(buf),), np.uint8).copy_from_host(buf)
-        if cast_code:
-            N.check(self._lib.b200tfs_set_decode_cast(self._ctx, cast_code))
-        try:
+        with self._decode_modes(cast_code):
             N.check(self._lib.b200tfs_decode_concat(self._ctx, wire.ptr, n, off, ln, nk, ck))
-        finally:
-            if cast_code:
-                N.check(self._lib.b200tfs_set_decode_cast(self._ctx, 0))
         outs, specs, rec_status = (N.Output * (n * nk))(), (N.ModelSpec * n)(), (C.c_int32 * n)()
         N.check(self._lib.b200tfs_concat_results(self._ctx, n, nk, outs, specs, rec_status))   # synchronises
         raw = np.frombuffer(outs, dtype=np.uint8).reshape(n * nk, C.sizeof(N.Output))
@@ -926,14 +940,7 @@ class Codec:
         for j in sorted(redo):
             r, i = divmod(j, nk)
             o = outs[j]
-            if rec_status[r] != N.OK:
-                return None
-            if o.flags & N.OF_DEVICE_VARINT:
-                o.flags &= ~N.OF_DEVICE_VARINT    # finished below by the unpack route, which raises what it raises today
-                o.status = N.OK
-            elif o.status == N.E_NONCANONICAL:
-                o.status = N.OK
-            elif o.status != N.OK:
+            if rec_status[r] != N.OK or not _to_unpack(o, N.E_NONCANONICAL):
                 return None
             _, dst_code, _ = self._resolve_output(o, strict, out_dtypes.get(keys[i]) if out_dtypes else None)
             if o.n_elems:
@@ -990,8 +997,7 @@ class Codec:
             for k, dst in out.items():
                 if k not in arrays:
                     raise KeyError(k)
-                if dst.dtype != arrays[k].dtype or dst.shape != arrays[k].shape:
-                    raise ValueError(f"out[{k!r}]: {dst.dtype}{dst.shape} does not match the decoded {arrays[k].dtype}{arrays[k].shape}")
+                _check_out(k, dst, arrays[k].dtype, arrays[k].shape)
                 np.copyto(dst, arrays[k])
                 arrays[k] = dst
             return arrays, spec
@@ -1002,21 +1008,16 @@ class Codec:
         cap = self._pinned.capacity(arr)
         if cap is None or not len(wire):
             return None
-        buf, off, ln = self._pack_wires([wire])
-        stride = cap & ~255
-        N.check(self._lib.b200tfs_decode_responses_host_async(self._ctx, buf.ctypes.data, 1, off, ln, arr.ctypes.data, stride))
-        K = N.FUSED_MAX_OUTPUTS
-        outs, n_outs, specs, status = (N.Output * K)(), (C.c_int32 * 1)(), (N.ModelSpec * 1)(), (C.c_int32 * 1)()
-        N.check(self._lib.b200tfs_decode_results(self._ctx, 1, outs, n_outs, specs, status))
-        if status[0] != N.OK or n_outs[0] != 1:
+        launch = self._fused_launch([wire], dst=arr, stride=cap & ~255)
+        if launch is None or len(launch.tables[0]) != 1:
             return None                                  # not the single-output case after all: the general path redoes it
-        o = outs[0]
-        if self._text(buf, o.key_off, o.key_len) != key or int(o.dtype) not in _FUSED_MOVES or o.status != N.OK or not o.n_runs or o.dst_off != 0:
+        o = launch.tables[0].get(key)
+        if o is None or not _stored(o) or o.dst_off != 0:
             return None
         np_type, dst_code, shape = self._resolve_output(o, strict, None)
-        if dst_code != int(o.dtype) or np.dtype(np_type) != arr.dtype or tuple(shape) != arr.shape:
+        if not _stored_as(o, dst_code) or np.dtype(np_type) != arr.dtype or tuple(shape) != arr.shape:
             return None
-        return {key: arr}, self._spec(buf, 0, specs[0])
+        return {key: arr}, self._spec(launch.buf, 0, launch.specs[0])
 
     def decode_tensor_protos(self, wires: Sequence[bytes], *, strict: bool = False, out_dtype=None) -> List[np.ndarray]:
         """``tensor_proto_to_ndarray`` for serialised TensorProto messages."""
@@ -1036,11 +1037,8 @@ class Codec:
                 results[i] = self._decode_strings(buf, int(off[i]), o)
                 continue
             np_type, dst_code, shape = self._resolve_output(o, strict, out_dtype)
-            jobs.append((i, o, np_type, dst_code, shape))
-        if jobs:
-            arrays = self._unpack_to_host([j[1:] for j in jobs], [int(off[j[0]]) for j in jobs])
-            for (i, *_), a in zip(jobs, arrays):
-                results[i] = a
+            jobs.append((results, i, o, np_type, dst_code, shape, int(off[i])))
+        self._unpack_to_host(jobs)
         return results  # type: ignore[return-value]
 
 
