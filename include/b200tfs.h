@@ -582,6 +582,52 @@ int b200tfs_encode_example_requests_async(b200tfs_ctx* ctx, int32_t n, const b20
 int b200tfs_encode_example_requests_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, void* wire_host,
                                          uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
 
+/* ---- Classify / Regress responses: a batch of responses into one value or score array ----------------------
+ * What ClassificationResponse.FromString / RegressionResponse.FromString followed by a loop over the result give, concatenated
+ * along the example axis across the n responses: row order is response 0's examples, then response 1's, and so on.
+ *   B200TFS_RESP_REGRESS:  values float32[rows], values[row] = regressions[i].value.
+ *   B200TFS_RESP_CLASSIFY: scores float32[rows * C] (row-major), scores[row * C + c] = classifications[i].classes[c].score, and
+ *                          labels[row * C + c] = where that class's label lies, relative to its record.  C is the class count of
+ *                          the batch's first example; every other example must have C classes too.
+ * Floats come back as the runtime gives them: an absent score / value is +0.0, -0.0 stays -0.0, a signalling NaN is quieted.
+ * Fields in any order, the last of repeated scalar fields wins, unknown fields (groups included) are skipped at every level, a
+ * known field with another wire type is an unknown field, repeated `result` fields merge (their entries concatenate), repeated
+ * model_spec fields merge.  Malformed wire - truncation, tag 0, over-long varints, lengths past the end, wire types 6 / 7,
+ * mismatched groups, a label or model_spec string that is not UTF-8 - is B200TFS_E_PARSE, where FromString raises DecodeError. */
+#define B200TFS_RESP_REGRESS 1
+#define B200TFS_RESP_CLASSIFY 2
+typedef struct b200tfs_label_ref {
+  uint32_t off;         /* label bytes, from the start of the record (0 / 0: the label is empty)                               */
+  uint32_t len;
+} b200tfs_label_ref;
+/* Host only, closed form from the record lengths alone (every Regression, Classifications and Class entry takes at least two
+ * bytes): *max_rows >= the rows of any responses of these lengths, *max_values >= their values (rows for Regress, rows * C for a
+ * Classify batch that decodes).  Either pointer may be NULL.                                                                 */
+int b200tfs_example_response_bound(int32_t kind, int32_t n, const uint64_t* rec_len, uint64_t* max_rows, uint64_t* max_values);
+/* Decode n responses of `kind` lying at rec_off[i]..+rec_len[i] of the device arena.  values_dst (device) holds values_cap floats,
+ * labels_dst (device; Classify only, may be NULL for Regress) labels_cap references.  Asynchronous and CUDA-graph capturable: the
+ * kernels (index, scan, emit; Classify adds a label compare) find the rows on the device, so a graph captured once serves any
+ * responses of the same lengths, and a replay adapts to new row counts.  Stores: values / labels of row r, class c < C only, and
+ * never at or past values_cap / labels_cap; a response whose rows end past them is B200TFS_E_SIZE.  Collect the results with
+ * b200tfs_example_response_results.                                                                                           */
+int b200tfs_decode_example_responses(b200tfs_ctx* ctx, int32_t kind, const void* arena_dev, int32_t n, const uint64_t* rec_off,
+                                     const uint64_t* rec_len, float* values_dst, uint64_t values_cap, b200tfs_label_ref* labels_dst,
+                                     uint64_t labels_cap);
+/* The same for responses in host memory (pinned for an asynchronous copy): the wire is copied to the device inside.  The
+ * destinations are device memory as above.                                                                                   */
+int b200tfs_decode_example_responses_host_async(b200tfs_ctx* ctx, int32_t kind, const void* wire_host, int32_t n,
+                                                const uint64_t* rec_off, const uint64_t* rec_len, float* values_dst,
+                                                uint64_t values_cap, b200tfs_label_ref* labels_dst, uint64_t labels_cap);
+/* Results of the context's most recent b200tfs_decode_example_responses* call (synchronises); any pointer may be NULL.
+ *   per_rec[3 * i + 0 .. 2]: the first row of response i, its rows, its status: B200TFS_OK, B200TFS_E_PARSE, B200TFS_E_SIZE (its
+ *                            rows end past a capacity) or B200TFS_E_SHAPE (an example with another class count than C), in
+ *                            that order of precedence.
+ *   specs[i]:                its model_spec (offsets from the start of its record).
+ *   batch[0 .. 4]:           rows of the batch, C (0 for Regress), same_labels (1: every example lists exactly the labels of the
+ *                            first example, in the same order), the status of the first response that is not B200TFS_OK (or
+ *                            B200TFS_OK), and that response's index (-1 when none).                                              */
+int b200tfs_example_response_results(b200tfs_ctx* ctx, int32_t n, int64_t* per_rec, b200tfs_model_spec* specs, int64_t* batch);
+
 #ifdef __cplusplus
 }
 #endif

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "../../include/b200tfs.h"
+#include "example_walk.h"
 #include "frame.h"
 #include "kernels.h"
 #include "plan.h"
@@ -136,6 +137,9 @@ struct b200tfs_ctx {
   int32_t concat_n = 0, concat_k = 0;   // ... of its most recent call, what b200tfs_concat_results answers for
   uint8_t* concat_dst[B200TFS_CONCAT_MAX_KEYS] = {};
   uint64_t concat_vouts_off = 0, concat_vstat_off = 0, concat_specs_off = 0, concat_status_off = 0;   // its ConcatLayout
+  Growable xr_dev;                      // b200tfs_decode_example_responses: entry slots and per-response tables (XrLayout)
+  Growable xr_host;                     // ... and the results its publish kernel leaves in pinned memory (XrResultsLayout)
+  int32_t xr_n = 0;                     // responses of its most recent call, what b200tfs_example_response_results answers for
 };
 
 // `baked`: the buffer's address ends up inside captured graphs (every context-owned scratch buffer except the plan-upload
@@ -320,6 +324,8 @@ int b200tfs_destroy(b200tfs_ctx* c) {
   if (c->guard_dev.p) cudaFree(c->guard_dev.p);
   if (c->vdec_dev.p) cudaFree(c->vdec_dev.p);
   if (c->concat_dev.p) cudaFree(c->concat_dev.p);
+  if (c->xr_dev.p) cudaFree(c->xr_dev.p);
+  if (c->xr_host.p) cudaFreeHost(c->xr_host.p);
   if (c->enc_host.p) cudaFreeHost(c->enc_host.p);
   if (c->measured_dev.p) cudaFree(c->measured_dev.p);
   if (c->scratch_host.p) cudaFreeHost(c->scratch_host.p);

@@ -22,6 +22,8 @@
 //                      device-side totals, writes every header byte, patches the destinations of the movers behind it.
 //   ex_count / ex_scan / ex_emit / ex_frame_kernel   Classify / Regress requests: a batch of tf.Examples from columnar
 //                      arrays (example_kernels.cuh).
+//   xr_index / xr_scan / xr_emit / xr_compare / xr_publish_kernel   Classify / Regress responses: a batch of responses into
+//                      one value / score array (example_resp_kernels.cuh, walk in example_walk.h).
 //   venc_* / vdec_*    packed-varint encode and decode (int_val / int64_val / uint32_val / uint64_val /
 //                      half_val / bool_val): varint_kernels.cuh.  vdec_plan_kernel + vdec_{count,emit}_dev_kernel decode the
 //                      varint outputs of a single-launch decode from tables built on the device (b200tfs_set_decode_varints).
@@ -43,6 +45,7 @@
 #include "kernels.h"
 #include "plan.h"
 #include "tpl.h"
+#include "example_walk.h"
 #include "walker.h"
 #include "wire.h"
 
@@ -1180,6 +1183,11 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
 // tf.Example requests (Classify / Regress): ex_count / ex_scan / ex_emit / ex_frame
 // ------------------------------------------------------------------------------------------------
 #include "example_kernels.cuh"
+
+// ------------------------------------------------------------------------------------------------
+// Classify / Regress responses: xr_index / xr_scan / xr_emit / xr_compare / xr_publish
+// ------------------------------------------------------------------------------------------------
+#include "example_resp_kernels.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // frame_requests_kernel (plan.h "deferred framing"): one thread per request evaluates the request's values from the job

@@ -47,5 +47,8 @@ cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t
 cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStream_t stream);
 // tf.Example requests (example_kernels.cuh): count + scan (when T.n_tiles), emit, frame; *launched receives how many kernels
 cudaError_t launch_example_requests(const ExTables& T, cudaStream_t stream, uint32_t* launched);
+// Classify / Regress responses (example_resp_kernels.cuh): index, scan, emit, [label compare,] publish; emit_ctas CTAs stride over
+// the rows; *launched receives how many kernels
+cudaError_t launch_example_responses(const XrTables& T, uint32_t emit_ctas, cudaStream_t stream, uint32_t* launched);
 
 }  // namespace b200tfs

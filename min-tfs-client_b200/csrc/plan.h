@@ -359,4 +359,24 @@ B2_PLAN_HD uint64_t ex_example_len(uint64_t F) {
   return 1 + varint_len(x) + x;
 }
 
+// ---- Classify / Regress responses (example_host.inc plans, example_resp_kernels.cuh runs) --------------------------------
+// Every buffer is sized from the record lengths alone: response r owns xr_row_bound(rec_len[r]) entry slots from ent0[r] on.
+constexpr uint32_t kXrIndexWarps = 4;      // responses per index CTA (one warp each)
+constexpr uint32_t kXrEmitThreads = 128;   // emit: one thread per row (a Regression entry or a Classifications example)
+struct XrTables {
+  const uint8_t* w;                        // the arena
+  const uint64_t* rec_off; const uint64_t* rec_len; const uint64_t* ent0;
+  b200tfs_label_ref* ent;                  // {off, len} of every result entry, record-relative
+  uint32_t* rows;                          // entries of every response
+  uint32_t* cls0;                          // Classify: classes of every response's first example
+  int32_t* status;                         // B200TFS_OK / E_PARSE / E_SIZE / E_SHAPE (lowest wins)
+  b200tfs_model_spec* specs;
+  uint64_t* row0;                          // first row of every response (scan)
+  unsigned long long* batch;               // rows, C, first response with rows, same_labels
+  float* values; uint64_t values_cap;
+  b200tfs_label_ref* labels; uint64_t labels_cap;
+  int64_t* per_rec_host; b200tfs_model_spec* specs_host; int64_t* batch_host;   // pinned host memory: read by b200tfs_example_response_results
+  uint32_t n, kind;
+};
+
 }  // namespace b200tfs

@@ -105,6 +105,14 @@ class ExampleRequest(C.Structure):
     ]
 
 
+RESP_REGRESS, RESP_CLASSIFY = 1, 2
+
+
+class LabelRef(C.Structure):
+    """b200tfs_label_ref: a Class label's bytes, from the start of its record."""
+    _fields_ = [("off", C.c_uint32), ("len", C.c_uint32)]
+
+
 _u64p = C.POINTER(C.c_uint64)
 _i32p = C.POINTER(C.c_int32)
 _vp = C.c_void_p
@@ -187,6 +195,11 @@ SIGNATURES = {
     "b200tfs_example_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), _u64p]),
     "b200tfs_encode_example_requests_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), _vp, C.c_uint64]),
     "b200tfs_encode_example_requests_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), _vp, C.c_uint64, _u64p, _u64p]),
+    "b200tfs_example_response_bound": (C.c_int, [C.c_int32, C.c_int32, _u64p, _u64p, _u64p]),
+    "b200tfs_decode_example_responses": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64, _vp, C.c_uint64]),
+    "b200tfs_decode_example_responses_host_async": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64, _vp,
+                                                              C.c_uint64]),
+    "b200tfs_example_response_results": (C.c_int, [_vp, C.c_int32, C.POINTER(C.c_int64), C.POINTER(ModelSpec), C.POINTER(C.c_int64)]),
 }
 
 _lib = None

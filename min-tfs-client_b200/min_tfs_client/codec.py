@@ -299,6 +299,34 @@ class OpenResponse:
         return arr
 
 
+class RegressionBatch:
+    """A batch of RegressionResponses decoded into one array: ``values`` float32 ``[rows]`` (response 0's regressions, then
+    response 1's, ...), ``counts`` int64 ``[n]`` (regressions per response), ``specs`` (a ``DecodedSpec`` per response)."""
+
+    __slots__ = ("values", "counts", "specs")
+
+    def __init__(self, values, counts, specs):
+        self.values, self.counts, self.specs = values, counts, specs
+
+
+class ClassificationBatch:
+    """A batch of ClassificationResponses decoded into one array: ``scores`` float32 ``[rows, C]``, ``counts`` int64 ``[n]``,
+    ``specs``; ``class_labels`` is the list of the C labels when every example lists the same labels in the same order (else
+    None), and ``labels()`` gives every example's labels."""
+
+    __slots__ = ("scores", "counts", "specs", "class_labels", "_rows")
+
+    def __init__(self, scores, counts, specs, class_labels, rows):
+        self.scores, self.counts, self.specs, self.class_labels, self._rows = scores, counts, specs, class_labels, rows
+
+    def labels(self) -> List[List[str]]:
+        """Per example, the labels of its classes (a callable: the common case decodes only C strings)."""
+        rows = self._rows
+        if callable(rows):
+            rows = self._rows = rows()
+        return [list(r) for r in rows]
+
+
 class ParsedResponse:
     """Table the parse kernel produced for one PredictResponse: where every output's values lie."""
 
@@ -327,6 +355,9 @@ class Codec:
         self._seen_varints = False
         # decode_predict_responses_concat calls the device route finished (the others were decoded response by response)
         self.concat_device_calls = 0
+        # decode_regression_responses / decode_classification_responses calls the device route finished
+        self.example_response_device_calls = 0
+        self._xr_scratch = None       # their device destinations when the result goes to host memory: (values, labels)
 
     def close(self):
         if getattr(self, "_ctx", None):
@@ -970,6 +1001,133 @@ class Codec:
         self.sync()
         self.concat_device_calls += 1
         return result, [self._spec(buf, int(off[r]), specs[r]) for r in range(n)]
+
+    # ---- Classify / Regress responses ------------------------------------------------------------------
+    def decode_regression_responses(self, wires: Sequence[bytes], *, device: bool = False, out=None) -> RegressionBatch:
+        """Decode a batch of RegressionResponses into one float32 array of every regression's value, response after response -
+        ``np.array([r.value for w in wires for r in RegressionResponse.FromString(w).result.regressions], np.float32)`` bit
+        for bit, raising what FromString raises.  ``device=True``: ``values`` is a ``DeviceArray`` (of the used rows);
+        ``out=``: a C-contiguous float32 device array or numpy / ``pinned_empty`` array of at least ``rows`` elements, of
+        which ``out[:rows]`` is returned (nothing is written into it when the call raises)."""
+        return self._decode_example_responses(N.RESP_REGRESS, wires, device, out)
+
+    def decode_classification_responses(self, wires: Sequence[bytes], *, device: bool = False, out=None) -> ClassificationBatch:
+        """Decode a batch of ClassificationResponses into one float32 ``[rows, C]`` array of scores - ``np.array([[c.score for c
+        in cl.classes] for w in wires for cl in ClassificationResponse.FromString(w).result.classifications], np.float32)``
+        bit for bit - raising what FromString raises, and ValueError when the examples disagree on the number of classes C.
+        ``device`` and ``out`` (at least ``rows`` rows of C columns) as for ``decode_regression_responses``."""
+        return self._decode_example_responses(N.RESP_CLASSIFY, wires, device, out)
+
+    def _xr_buffers(self, values: int, labels: int):
+        """The codec's own device destinations, grown to hold `values` floats and `labels` label references."""
+        have = self._xr_scratch
+        if have is None or have[0].nbytes < 4 * values or have[1].nbytes < C.sizeof(N.LabelRef) * labels:
+            v = max(values, have[0].nbytes // 4 if have else 0)
+            lab = max(labels, have[1].nbytes // C.sizeof(N.LabelRef) if have else 0)
+            self._xr_scratch = have = (D.DeviceArray(self, (max(v, 1),), np.float32), D.DeviceArray(self, (max(lab, 1), 2), np.uint32))
+        return have
+
+    def _decode_example_responses(self, kind, wires, device, out):
+        n = len(wires)
+        cls = kind == N.RESP_CLASSIFY
+        if n == 0:
+            return self._example_batch_host(kind, wires, device, out)
+        buf, off, ln = self._pack_wires(wires)
+        max_rows, max_values = C.c_uint64(), C.c_uint64()
+        N.check(self._lib.b200tfs_example_response_bound(kind, n, ln, C.byref(max_rows), C.byref(max_values)))
+        mv = int(max_values.value)
+        # the kernels write the codec's scratch; the result reaches the caller's destination only once the batch has decoded
+        scratch_v, scratch_l = self._xr_buffers(mv, mv if cls else 0)
+        vptr, lptr, lcap = scratch_v.ptr, (scratch_l.ptr if cls else None), (mv if cls else 0)
+        N.check(self._lib.b200tfs_decode_example_responses_host_async(self._ctx, kind, buf.ctypes.data, n, off, ln, vptr, mv, lptr, lcap))
+        per, specs, batch = (C.c_int64 * (3 * n))(), (N.ModelSpec * n)(), (C.c_int64 * 5)()
+        N.check(self._lib.b200tfs_example_response_results(self._ctx, n, per, specs, batch))   # synchronises
+        rows, ncls, same, status = int(batch[0]), int(batch[1]), bool(batch[2]), int(batch[3])
+        if status != N.OK:      # a response the device route does not decode: the definition itself, response by response
+            return self._example_batch_host(kind, wires, device, out)
+        counts = np.array([per[3 * i + 1] for i in range(n)], dtype=np.int64)
+        spec_list = [self._spec(buf, int(off[i]), specs[i]) for i in range(n)]
+        vals = self._example_out((rows, ncls) if cls else (rows,), device, out, src_dev=vptr)
+        if cls:
+            nref = ncls if same else rows * ncls
+            refs = np.empty((nref, 2), np.uint32)
+            if nref:
+                N.check(self._lib.b200tfs_memcpy_d2h(self._ctx, refs.ctypes.data, lptr, refs.nbytes))
+        self.sync()
+        self.example_response_device_calls += 1
+        if not cls:
+            return RegressionBatch(vals, counts, spec_list)
+        row_of = np.repeat(np.arange(n), counts)
+        text = lambda i, k: self._text(buf, int(off[row_of[i]]) + int(refs[i * ncls + k, 0]), int(refs[i * ncls + k, 1]))   # noqa: E731
+        if same:
+            class_labels = [text(0, k) for k in range(ncls)] if rows else []
+            return ClassificationBatch(vals, counts, spec_list, class_labels, lambda: [class_labels] * rows)
+        return ClassificationBatch(vals, counts, spec_list, None, lambda: [[text(i, k) for k in range(ncls)] for i in range(rows)])
+
+    def _example_out(self, shape, device, out, src_dev=None, host=None):
+        """The decoded float32 array of `shape` - on the device at src_dev, or the host array `host` - delivered where the caller
+        asked: into ``out`` (``out[:rows]`` is returned; a device array that cannot be sliced must have exactly `rows` rows), a new
+        ``DeviceArray`` (device=True) or a new numpy array.  ``out`` is checked before anything is written into it."""
+        rows, nbytes = shape[0], 4 * int(np.prod(shape, dtype=np.int64))
+        if out is not None and D.is_device_object(out):
+            ptr, oshape, odtype, hold = D.device_view(out)
+            sliceable = hasattr(out, "__getitem__")
+            if odtype != np.float32 or len(oshape) != len(shape) or tuple(oshape[1:]) != tuple(shape[1:]) or oshape[0] < rows \
+                    or (not sliceable and oshape[0] != rows):
+                raise ValueError(f"out: {odtype}{tuple(oshape)} cannot take {tuple(shape)} float32 values"
+                                 + ("" if sliceable else " (an array that cannot be sliced must have exactly that shape)"))
+            dst = out
+        elif device and out is None:
+            dst = D.DeviceArray(self, shape, np.float32)
+            ptr = dst.ptr
+        else:
+            if out is not None and (not isinstance(out, np.ndarray) or out.dtype != np.float32 or not out.flags.c_contiguous
+                                    or out.ndim != len(shape) or out.shape[1:] != tuple(shape[1:]) or len(out) < rows):
+                raise ValueError(f"out must be a C-contiguous float32 array of at least {tuple(shape)} (rows first)")
+            arr = np.empty(shape, np.float32) if out is None else out[:rows]
+            if host is not None:
+                arr[...] = host
+            elif nbytes:
+                N.check(self._lib.b200tfs_memcpy_d2h(self._ctx, arr.ctypes.data, src_dev, nbytes))
+                self.sync()
+            return arr
+        if nbytes:
+            if host is not None:
+                a = np.ascontiguousarray(host, dtype=np.float32)
+                N.check(self._lib.b200tfs_memcpy_h2d(self._ctx, ptr, a.ctypes.data, nbytes))
+            else:
+                N.check(self._lib.b200tfs_memcpy_d2d(self._ctx, ptr, src_dev, nbytes))
+            self.sync()
+        return dst[:rows] if dst is out and hasattr(out, "__getitem__") else dst
+
+    def _example_batch_host(self, kind, wires, device, out):
+        """The definition, response by response, with protobuf on the host: what the device route hands over when a response
+        does not decode there (malformed, ragged class counts, rows past the caller's ``out``)."""
+        from tensorflow_serving.apis.classification_pb2 import ClassificationResponse
+        from tensorflow_serving.apis.regression_pb2 import RegressionResponse
+
+        cls = kind == N.RESP_CLASSIFY
+        msgs = [(ClassificationResponse if cls else RegressionResponse).FromString(bytes(w)) for w in wires]
+        specs = []
+        for m in msgs:
+            s = m.model_spec
+            specs.append(DecodedSpec(s.name, s.version.value, s.HasField("version"), s.version_label, s.signature_name))
+        if cls:
+            rows = [cl.classes for m in msgs for cl in m.result.classifications]
+            if len({len(r) for r in rows}) > 1:
+                raise ValueError("examples disagree on the number of classes")
+            ncls = len(rows[0]) if rows else 0
+            vals = np.array([[c.score for c in r] for r in rows], np.float32).reshape(len(rows), ncls)
+            counts = np.array([len(m.result.classifications) for m in msgs], dtype=np.int64)
+            labels = [[c.label for c in r] for r in rows]
+        else:
+            vals = np.array([r.value for m in msgs for r in m.result.regressions], np.float32)
+            counts = np.array([len(m.result.regressions) for m in msgs], dtype=np.int64)
+        res = self._example_out(vals.shape, device, out, host=vals)
+        if not cls:
+            return RegressionBatch(res, counts, specs)
+        same = all(r == labels[0] for r in labels)
+        return ClassificationBatch(res, counts, specs, list(labels[0]) if same and labels else ([] if same else None), labels)
 
     @staticmethod
     def _decode_strings(buf: np.ndarray, base: int, o: N.Output, rec_len: int = 0, key: str = "") -> np.ndarray:

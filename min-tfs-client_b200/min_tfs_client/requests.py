@@ -100,6 +100,71 @@ class PredictResponseView:
         return getattr(self.to_proto(), name)
 
 
+class _ExampleResponseView:
+    """A Classify / Regress response decoded on the GPU on first use; anything the view does not answer itself comes from a
+    real response message parsed on demand."""
+
+    _message = None      # the protobuf class
+
+    def __init__(self, wire: bytes):
+        self._wire = wire
+        self._proto = None
+        self._batch = None
+
+    def to_proto(self):
+        if self._proto is None:
+            self._proto = self._message.FromString(self._wire)
+        return self._proto
+
+    def SerializeToString(self) -> bytes:  # noqa: N802
+        return self._wire
+
+    def __getattr__(self, name):
+        return getattr(self.to_proto(), name)
+
+
+class ClassificationResponseView(_ExampleResponseView):
+    """What ``gpu_classification_response_deserializer`` returns: ``.scores`` (float32 ``[examples, classes]``) and
+    ``.labels()`` decoded by the kernels; ``.result``, ``.model_spec``, ... from a ``ClassificationResponse``."""
+
+    from tensorflow_serving.apis.classification_pb2 import ClassificationResponse as _message
+
+    def _decoded(self):
+        if self._batch is None:
+            self._batch = get_codec().decode_classification_responses([self._wire])
+        return self._batch
+
+    @property
+    def scores(self) -> np.ndarray:
+        return self._decoded().scores
+
+    def labels(self):
+        return self._decoded().labels()
+
+
+class RegressionResponseView(_ExampleResponseView):
+    """What ``gpu_regression_response_deserializer`` returns: ``.values`` (float32 ``[examples]``) decoded by the kernels;
+    ``.result``, ``.model_spec``, ... from a ``RegressionResponse``."""
+
+    from tensorflow_serving.apis.regression_pb2 import RegressionResponse as _message
+
+    @property
+    def values(self) -> np.ndarray:
+        if self._batch is None:
+            self._batch = get_codec().decode_regression_responses([self._wire])
+        return self._batch.values
+
+
+def gpu_classification_response_deserializer(wire: bytes) -> ClassificationResponseView:
+    """``response_deserializer`` for ``channel.unary_unary(CLASSIFY_METHOD, ...)``: bytes -> lazy response view."""
+    return ClassificationResponseView(wire)
+
+
+def gpu_regression_response_deserializer(wire: bytes) -> RegressionResponseView:
+    """``response_deserializer`` for ``channel.unary_unary(REGRESS_METHOD, ...)``: bytes -> lazy response view."""
+    return RegressionResponseView(wire)
+
+
 def gpu_request_serializer(request) -> bytes:
     """``request_serializer`` for ``channel.unary_unary``: (model_name, model_version, input_dict) -> bytes."""
     model_name, model_version, input_dict = request
