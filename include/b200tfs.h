@@ -457,6 +457,55 @@ int b200tfs_decode_concat_host_async(b200tfs_ctx* ctx, const void* wire_host, in
 int b200tfs_concat_results(b200tfs_ctx* ctx, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs,
                            int32_t* rec_status);
 
+/* ---- batch decode into one padded tensor per output (ragged trailing dims) --------------------------
+ * What a caller of a sequence model wants back (per-token logits f32[1, T_r, V], token ids int64[1, T_r], ...): for each requested
+ * key, the outputs of every record concatenated along axis 0 with every other axis padded - record r's output lands in rows
+ * [first_row, first_row + dims[0]) of one tensor of shape [rows, dims[1], ..., dims[rank-1]], at index 0 of every trailing axis, and
+ * every other element of those rows holds the pad element.  As for the concatenated decode, the rows and the trailing dims are
+ * planned on the device, so a replayed CUDA graph adapts to new records.  Only the requested outputs are decoded.              */
+typedef struct b200tfs_pad_key {
+  const char* key;        /* in: map key bytes (not NUL terminated); the keys of one call must be distinct                   */
+  int64_t key_len;
+  void* dst;              /* in: b200tfs_decode_padded*: device destination, 16-byte aligned                                  */
+  uint64_t dst_cap;       /* in: its capacity in bytes - nothing is ever stored at or past dst + dst_cap                      */
+  int32_t dtype;          /* out (b200tfs_padded_layout): DT_* of the first record that has the key                          */
+  int32_t rank;           /* out: its rank.  In (b200tfs_decode_padded*): the destination's rank                              */
+  int64_t dims[B200TFS_MAX_RANK]; /* out: dims[0] = rows of all records together, dims[1..rank) the elementwise maximum of the
+                             records' trailing dims.  In (b200tfs_decode_padded*): dims[1..rank) are the destination's trailing
+                             dims (a caller that captures a graph fixes them once, e.g. at the model's longest sequence)     */
+  uint64_t bytes;         /* out: rows * prod(dims[1..rank)) * element size in memory (2 for float32 with a cast)              */
+  int32_t status;         /* out: as b200tfs_concat_key.status, except that other trailing dims are not an error              */
+  int32_t bad_rec;        /* out: the record `status` is about (-1 when OK)                                                  */
+  uint8_t pad_bits[16];   /* in: the pad element's bit pattern in the destination dtype (little-endian; the first element
+                             size bytes are used)                                                                            */
+} b200tfs_pad_key;
+/* Host only (needs no device): walks the n records in host memory and fills the out fields of keys[0..n_keys).  The first
+ * problem in record order, with b200tfs_concat_layout's codes: E_SHAPE (rank 0, another rank), E_DTYPE, E_KEY, the output's
+ * tabulated error, E_NONCANONICAL (a record the device route cannot tabulate).  cast: 0, or DT_HALF / DT_BFLOAT16.              */
+int b200tfs_padded_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
+                          b200tfs_pad_key* keys, int32_t cast);
+/* Decode n PredictResponses of the device arena into keys[k].dst for every k < n_keys (<= B200TFS_CONCAT_MAX_KEYS; only the in
+ * fields are read).  Asynchronous and CUDA-graph capturable, with no host step between the launches (parse, one-CTA plan,
+ * destination-major emit, packed-varint plan / count / emit - b200tfs_kernel_launches counts six).  The scratch is sized from n,
+ * n_keys and rec_len alone, so a replay over new records of the same lengths re-plans rows and trailing dims.  Float32 outputs are
+ * narrowed per b200tfs_set_decode_cast; values are what b200tfs_decode_concat writes.  Stores: with `pitch` = prod(dims[1..rank))
+ * * element size and rows_used = the rows of the records that got a place, every byte of [0, rows_used * pitch) of keys[k].dst is
+ * written exactly once - values and pads alike - and nothing else, never at or past dst_cap.  A record whose trailing dim exceeds
+ * dims[d], or whose rows would pass dst_cap, is B200TFS_E_SIZE and gets no place.  A packed-varint output whose decode fails
+ * leaves its value elements unspecified (its pads are written).                                                                  */
+int b200tfs_decode_padded(b200tfs_ctx* ctx, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                          int32_t n_keys, const b200tfs_pad_key* keys);
+/* The same for records in host memory: the wire is copied to the device inside (asynchronous; wire_host should be pinned). */
+int b200tfs_decode_padded_host_async(b200tfs_ctx* ctx, const void* wire_host, int32_t n, const uint64_t* rec_off,
+                                     const uint64_t* rec_len, int32_t n_keys, const b200tfs_pad_key* keys);
+/* Results of the context's most recent b200tfs_decode_padded* call (synchronises).  outs[r * n_keys + k]: record r's table entry
+ * for key k - its `dims` are that record's own shape - with dst_off = the byte offset of its first row inside keys[k].dst,
+ * dst_bytes = the bytes of its rows there, and `status` as b200tfs_concat_results words it, except that other trailing dims are not
+ * an error and that packed-varint rows of unpacked elements are B200TFS_E_NONCANONICAL with no place.  specs[r] and rec_status[r]
+ * as b200tfs_parse_responses gives them; any pointer may be NULL.                                                               */
+int b200tfs_padded_results(b200tfs_ctx* ctx, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs,
+                           int32_t* rec_status);
+
 /* ---- CUDA graphs: record a fixed sequence of encode / decode calls once, replay it per request ---
  * Between capture_begin and capture_end the asynchronous entry points (b200tfs_encode_requests,
  * b200tfs_encode_tensor_protos, b200tfs_decode_responses, b200tfs_memcpy_*) only record work; calls

@@ -133,10 +133,17 @@ struct b200tfs_ctx {
   Growable enc_host;                    // b200tfs_encode_requests_async: rec_off | rec_len | status, written by frame_requests_kernel (pinned)
   int32_t enc_n = 0;
   bool has_graphs = false;              // a CUDA graph captured on this context refers to the scratch buffers: they may not move any more
+  // the per-key decodes' most recent call, what their results calls answer for: records, keys, destinations and where the
+  // table, the varint statuses, the specs and the record statuses lie in the scratch buffer
+  struct KeyResults {
+    int32_t n = 0, k = 0;
+    uint8_t* dst[B200TFS_CONCAT_MAX_KEYS] = {};
+    uint64_t vouts = 0, vstat = 0, specs = 0, status = 0;
+  };
   Growable concat_dev;                  // b200tfs_decode_concat: parse table, plan image, varint tables (ConcatLayout)
-  int32_t concat_n = 0, concat_k = 0;   // ... of its most recent call, what b200tfs_concat_results answers for
-  uint8_t* concat_dst[B200TFS_CONCAT_MAX_KEYS] = {};
-  uint64_t concat_vouts_off = 0, concat_vstat_off = 0, concat_specs_off = 0, concat_status_off = 0;   // its ConcatLayout
+  KeyResults concat_res;
+  Growable padded_dev;                  // b200tfs_decode_padded: parse table, descriptors, varint tables (PaddedLayout)
+  KeyResults padded_res;
   Growable xr_dev;                      // b200tfs_decode_example_responses: entry slots and per-response tables (XrLayout)
   Growable xr_host;                     // ... and the results its publish kernel leaves in pinned memory (XrResultsLayout)
   int32_t xr_n = 0;                     // responses of its most recent call, what b200tfs_example_response_results answers for
@@ -324,6 +331,7 @@ int b200tfs_destroy(b200tfs_ctx* c) {
   if (c->guard_dev.p) cudaFree(c->guard_dev.p);
   if (c->vdec_dev.p) cudaFree(c->vdec_dev.p);
   if (c->concat_dev.p) cudaFree(c->concat_dev.p);
+  if (c->padded_dev.p) cudaFree(c->padded_dev.p);
   if (c->xr_dev.p) cudaFree(c->xr_dev.p);
   if (c->xr_host.p) cudaFreeHost(c->xr_host.p);
   if (c->enc_host.p) cudaFreeHost(c->enc_host.p);
@@ -1412,8 +1420,9 @@ int b200tfs_decode_slot_bytes(const void* wire_host, int32_t n, const uint64_t* 
 
 // The packed-varint outputs of a table a decode launch published: vdec_plan_kernel builds their decode tables in the region `vd`
 // (var_plan_layout(vp.n, vp.tile_cap)), then the count and emit kernels run over them.  `vp` comes with the table, the wire and
-// the destinations set; rec_off is the host's copy of the record offsets.  vp.status receives the per-slot statuses.
-static int launch_varint_tail(b200tfs_ctx* c, VarPlan& vp, uint8_t* vd, const uint64_t* rec_off) {
+// the destinations set; rec_off is the host's copy of the record offsets.  vp.status receives the per-slot statuses.  `pad`: the
+// padded decode's element placement (VarPadMap).
+static int launch_varint_tail(b200tfs_ctx* c, VarPlan& vp, uint8_t* vd, const uint64_t* rec_off, const VarPadMap* pad = nullptr) {
   const VarPlanLayout V = var_plan_layout(vp.n, vp.tile_cap);
   if (vp.n <= (uint32_t)kFusedInlineRecs) for (uint32_t i = 0; i < vp.n; ++i) vp.off_inl[i] = rec_off[i];
   vp.jobs = (VarJobDev*)(vd + V.jobs); vp.segs = (VarSeg*)(vd + V.segs); vp.tile_seg = (uint32_t*)(vd + V.tile_seg);
@@ -1422,7 +1431,7 @@ static int launch_varint_tail(b200tfs_ctx* c, VarPlan& vp, uint8_t* vd, const ui
   CU(launch_vdec_plan(vp, c->stream));
   VarTables tb{};
   tb.segs = vp.segs; tb.tile_seg = vp.tile_seg; tb.jobs = vp.jobs; tb.n_tiles = vp.tile_cap; tb.n_tiles_dev = vp.n_tiles;
-  CU(launch_vdec_dev(tb, (uint32_t)c->sm_count * 4, c->stream));
+  CU(launch_vdec_dev(tb, (uint32_t)c->sm_count * 4, c->stream, pad));
   c->launches += 3;
   return B200TFS_OK;
 }
@@ -2197,7 +2206,9 @@ int b200tfs_unpack_outputs_host(b200tfs_ctx* c, int32_t m, const b200tfs_output*
 // ------------------------------------------------------------------------------------------------
 // decode into one tensor per key, concatenated along axis 0
 // ------------------------------------------------------------------------------------------------
-static int concat_check_keys(int32_t n_keys, const b200tfs_concat_key* keys) {
+extern "C++" {
+template <class Key>   // b200tfs_concat_key, b200tfs_pad_key
+static int concat_check_keys(int32_t n_keys, const Key* keys) {
   if (n_keys <= 0 || n_keys > B200TFS_CONCAT_MAX_KEYS || !keys) return fail(B200TFS_E_ARG, "n_keys must be 1..%d", B200TFS_CONCAT_MAX_KEYS);
   for (int k = 0; k < n_keys; ++k) {
     if (keys[k].key_len < 0 || keys[k].key_len > 0xFFFFFFFFll || (keys[k].key_len && !keys[k].key)) return fail(B200TFS_E_ARG, "key %d: bad key", k);
@@ -2207,6 +2218,7 @@ static int concat_check_keys(int32_t n_keys, const b200tfs_concat_key* keys) {
   }
   return B200TFS_OK;
 }
+}  // extern "C++"
 
 int b200tfs_response_keys(const void* rec_host, uint64_t rec_len, int32_t cap, uint64_t* key_off, uint32_t* key_len, int32_t* count) {
   if (!count || cap < 0 || (cap && (!key_off || !key_len)) || (rec_len && !rec_host)) return fail(B200TFS_E_ARG, "bad arguments");
@@ -2226,15 +2238,20 @@ int b200tfs_response_keys(const void* rec_host, uint64_t rec_len, int32_t cap, u
   }
 }
 
-int b200tfs_concat_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
-                          b200tfs_concat_key* keys, int32_t cast) {
+extern "C++" {
+// The host walk of b200tfs_concat_layout and b200tfs_padded_layout: per key, the first problem in record order, the dtype and
+// rank of the first record that has the key, the rows, and the trailing dims - every record's (another one is E_SHAPE) or, with
+// `ragged`, their elementwise maximum.
+template <class Key>
+static int key_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys, Key* keys,
+                      int32_t cast, bool ragged) {
   if (n <= 0 || !wire_host || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
   int rc = concat_check_keys(n_keys, keys);
   if (rc) return rc;
   if (cast != 0 && cast != DT_FLOAT && cast != DT_HALF && cast != DT_BFLOAT16) return fail(B200TFS_E_DTYPE, "cast to dtype %d", cast);
   const uint32_t cst = (cast == DT_HALF || cast == DT_BFLOAT16) ? (uint32_t)cast : 0u;
   for (int k = 0; k < n_keys; ++k) {
-    b200tfs_concat_key& K = keys[k];
+    Key& K = keys[k];
     K.dtype = 0; K.rank = 0; K.bytes = 0; K.status = B200TFS_E_KEY; K.bad_rec = -1;
     for (int d = 0; d < B200TFS_MAX_RANK; ++d) K.dims[d] = 0;
   }
@@ -2249,7 +2266,7 @@ int b200tfs_concat_layout(const void* wire_host, int32_t n, const uint64_t* rec_
     if (st == B200TFS_E_SPILL || st == B200TFS_E_SIZE) st = B200TFS_E_NONCANONICAL;
     for (int k = 0; k < n_keys; ++k) {
       if (done[k]) continue;
-      b200tfs_concat_key& K = keys[k];
+      Key& K = keys[k];
       int32_t s = st;
       const b200tfs_output* o = nullptr;
       if (s == B200TFS_OK) {
@@ -2261,7 +2278,7 @@ int b200tfs_concat_layout(const void* wire_host, int32_t n, const uint64_t* rec_
           else if (o->rank > B200TFS_MAX_RANK) s = B200TFS_E_NONCANONICAL;
           else if (have[k] && o->dtype != K.dtype) s = B200TFS_E_DTYPE;
           else if (have[k] && o->rank != K.rank) s = B200TFS_E_SHAPE;
-          else for (int d = 1; have[k] && d < o->rank; ++d) if (o->dims[d] != K.dims[d]) s = B200TFS_E_SHAPE;
+          else for (int d = 1; have[k] && !ragged && d < o->rank; ++d) if (o->dims[d] != K.dims[d]) s = B200TFS_E_SHAPE;
         }
       }
       if (s != B200TFS_OK) { K.status = s; K.bad_rec = r; done[k] = 1; continue; }
@@ -2272,11 +2289,31 @@ int b200tfs_concat_layout(const void* wire_host, int32_t n, const uint64_t* rec_
         K.dims[0] = 0;
       }
       K.dims[0] += o->dims[0];
-      K.bytes += tpl_narrows(cst, o->dtype) ? o->n_elems * 2 : o->dst_bytes;
+      for (int d = 1; ragged && d < o->rank; ++d) K.dims[d] = std::max(K.dims[d], o->dims[d]);
+      if (!ragged) K.bytes += tpl_narrows(cst, o->dtype) ? o->n_elems * 2 : o->dst_bytes;
     }
   }
-  for (int k = 0; k < n_keys; ++k) if (!done[k]) keys[k].status = B200TFS_OK;
+  for (int k = 0; k < n_keys; ++k) {
+    Key& K = keys[k];
+    if (!done[k]) K.status = B200TFS_OK;
+    if (ragged && K.status == B200TFS_OK) {
+      uint64_t b = (uint64_t)K.dims[0] * (tpl_narrows(cst, K.dtype) ? 2u : dtype_info(K.dtype).elem_size);
+      for (int d = 1; d < K.rank; ++d) b *= (uint64_t)K.dims[d];
+      K.bytes = b;
+    }
+  }
   return B200TFS_OK;
+}
+}  // extern "C++"
+
+int b200tfs_concat_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
+                          b200tfs_concat_key* keys, int32_t cast) {
+  return key_layout(wire_host, n, rec_off, rec_len, n_keys, keys, cast, false);
+}
+
+int b200tfs_padded_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
+                          b200tfs_pad_key* keys, int32_t cast) {
+  return key_layout(wire_host, n, rec_off, rec_len, n_keys, keys, cast, true);
 }
 
 namespace {
@@ -2341,7 +2378,7 @@ int b200tfs_decode_concat(b200tfs_ctx* c, const void* arena_dev, int32_t n, cons
     }
   });
   if (rc) return rc;
-  for (int k = 0; k < n_keys; ++k) c->concat_dst[k] = (uint8_t*)keys[k].dst;
+  for (int k = 0; k < n_keys; ++k) c->concat_res.dst[k] = (uint8_t*)keys[k].dst;
   uint8_t* d = (uint8_t*)c->concat_dev.p;
   const uint64_t* off_dev = (const uint64_t*)(sd + o_off);
   CU(launch_parse_responses((const uint8_t*)arena_dev, off_dev, (const uint64_t*)(sd + o_len), n, kFusedMaxOutputs, (b200tfs_output*)(d + L.outs),
@@ -2365,8 +2402,8 @@ int b200tfs_decode_concat(b200tfs_ctx* c, const void* arena_dev, int32_t n, cons
   if ((rc = launch_varint_tail(c, vp, d + L.var, rec_off))) return rc;
   if (slot->done && !c->capturing) { CU(cudaEventRecord(slot->done, c->stream)); slot->pending = true; }   // the kernels read the upload
   c->launches += 3;
-  c->concat_n = n; c->concat_k = n_keys;
-  c->concat_vouts_off = L.vouts; c->concat_vstat_off = L.var_status; c->concat_specs_off = L.specs; c->concat_status_off = L.status;
+  c->concat_res.n = n; c->concat_res.k = n_keys;
+  c->concat_res.vouts = L.vouts; c->concat_res.vstat = L.var_status; c->concat_res.specs = L.specs; c->concat_res.status = L.status;
   return B200TFS_OK;
 }
 
@@ -2381,33 +2418,162 @@ int b200tfs_decode_concat_host_async(b200tfs_ctx* c, const void* wire_host, int3
   return b200tfs_decode_concat(c, c->stage_dev.p, n, rec_off, rec_len, n_keys, keys);
 }
 
-int b200tfs_concat_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs, int32_t* rec_status) {
+// The results of a per-key decode (`R` of its most recent call, its scratch at `base`), as b200tfs_concat_results describes them
+static int key_results(b200tfs_ctx* c, const b200tfs_ctx::KeyResults& R, const uint8_t* base, const char* what, int32_t n, int32_t n_keys,
+                       b200tfs_output* outs, b200tfs_model_spec* specs, int32_t* rec_status) {
   if (!c || n < 0 || n_keys < 0) return fail(B200TFS_E_ARG, "bad arguments");
   if (c->capturing) return fail(B200TFS_E_ARG, "cannot collect results during graph capture");
-  if (n != c->concat_n || n_keys != c->concat_k) return fail(B200TFS_E_ARG, "the last b200tfs_decode_concat had %d records and %d keys", c->concat_n, c->concat_k);
+  if (n != R.n || n_keys != R.k) return fail(B200TFS_E_ARG, "the last %s had %d records and %d keys", what, R.n, R.k);
   if (n == 0) return B200TFS_OK;
   CU(cudaSetDevice(c->device));
   CU(cudaStreamSynchronize(c->stream));
-  const uint8_t* d = (const uint8_t*)c->concat_dev.p;
+  const uint8_t* d = base;
   if (outs) {
     std::vector<b200tfs_output> v((size_t)n * kFusedMaxOutputs);
     std::vector<int32_t> vs((size_t)n * kFusedMaxOutputs);
-    CU(cudaMemcpy(v.data(), d + c->concat_vouts_off, sizeof(b200tfs_output) * v.size(), cudaMemcpyDeviceToHost));
-    CU(cudaMemcpy(vs.data(), d + c->concat_vstat_off, 4 * vs.size(), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(v.data(), d + R.vouts, sizeof(b200tfs_output) * v.size(), cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(vs.data(), d + R.vstat, 4 * vs.size(), cudaMemcpyDeviceToHost));
     for (int r = 0; r < n; ++r)
       for (int k = 0; k < n_keys; ++k) {
         b200tfs_output o = v[(size_t)r * kFusedMaxOutputs + k];
         fold_varint_status(o, vs[(size_t)r * kFusedMaxOutputs + k]);
-        o.dst_off -= (uint64_t)(uintptr_t)c->concat_dst[k];
+        o.dst_off -= (uint64_t)(uintptr_t)R.dst[k];
         outs[(size_t)r * n_keys + k] = o;
       }
   }
-  if (specs) CU(cudaMemcpy(specs, d + c->concat_specs_off, sizeof(b200tfs_model_spec) * (uint64_t)n, cudaMemcpyDeviceToHost));
+  if (specs) CU(cudaMemcpy(specs, d + R.specs, sizeof(b200tfs_model_spec) * (uint64_t)n, cudaMemcpyDeviceToHost));
   if (rec_status) {
-    CU(cudaMemcpy(rec_status, d + c->concat_status_off, 4ull * n, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(rec_status, d + R.status, 4ull * n, cudaMemcpyDeviceToHost));
     for (int r = 0; r < n; ++r) if (rec_status[r] == B200TFS_E_SPILL || rec_status[r] == B200TFS_E_SIZE) rec_status[r] = B200TFS_E_NONCANONICAL;
   }
   return B200TFS_OK;
+}
+
+int b200tfs_concat_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs, int32_t* rec_status) {
+  if (!c) return fail(B200TFS_E_ARG, "bad arguments");
+  return key_results(c, c->concat_res, (const uint8_t*)c->concat_dev.p, "b200tfs_decode_concat", n, n_keys, outs, specs, rec_status);
+}
+
+// ------------------------------------------------------------------------------------------------
+// decode into one padded tensor per key
+// ------------------------------------------------------------------------------------------------
+namespace {
+// device scratch of b200tfs_decode_padded for n records, n_keys keys and var_tile_cap varint tiles
+struct PaddedLayout { uint64_t outs, nouts, specs, status, spill, kst, match, desc, first_row, kout, vouts, vnouts, vstatus, var, var_status, bytes; };
+PaddedLayout padded_layout(uint64_t n, uint64_t n_keys, uint64_t var_tile_cap) {
+  const VarPlanLayout V = var_plan_layout(n, var_tile_cap);
+  Layout R;
+  PaddedLayout L;
+  L.outs = R.take(sizeof(b200tfs_output) * n * (kFusedMaxOutputs + 1), 256);
+  L.nouts = R.take(4 * n, 256);
+  L.specs = R.take(sizeof(b200tfs_model_spec) * n, 256);
+  L.status = R.take(4 * n, 256);
+  L.spill = R.take(4 * n, 256);
+  L.kst = R.take(4 * n * n_keys, 256);
+  L.match = R.take(4 * n * n_keys, 256);
+  L.desc = R.take(sizeof(PadDesc) * n * n_keys, 256);
+  L.first_row = R.take(8 * n * n_keys, 256);
+  L.kout = R.take(sizeof(PadKeyOut) * (n_keys + 1), 256);
+  L.vouts = R.take(sizeof(b200tfs_output) * n * kFusedMaxOutputs, 256);
+  L.vnouts = R.take(4 * n, 256);
+  L.vstatus = R.take(4 * n, 256);
+  L.var = R.take(V.bytes, 256);
+  L.var_status = L.var + V.status;
+  L.bytes = R.end;
+  return L;
+}
+}  // namespace
+
+int b200tfs_decode_padded(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                          int32_t n_keys, const b200tfs_pad_key* keys) {
+  if (!c || n <= 0 || !arena_dev || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
+  int rc = concat_check_keys(n_keys, keys);
+  if (rc) return rc;
+  uint64_t chunk_bound = 0;
+  for (int k = 0; k < n_keys; ++k) {
+    const b200tfs_pad_key& K = keys[k];
+    if (K.dst_cap && !K.dst) return fail(B200TFS_E_ARG, "key %d: dst is NULL", k);
+    if ((uintptr_t)K.dst & 15) return fail(B200TFS_E_ARG, "key %d: dst is not 16-byte aligned", k);
+    if (K.rank < 1 || K.rank > B200TFS_MAX_RANK) return fail(B200TFS_E_ARG, "key %d: rank %d", k, K.rank);
+    uint64_t row = 1;
+    for (int d = 1; d < K.rank; ++d) {
+      if (K.dims[d] < 0 || (K.dims[d] && row > 0xFFFFFFFFull / (uint64_t)K.dims[d])) return fail(B200TFS_E_ARG, "key %d: a row holds 2^32 elements or more", k);
+      row *= (uint64_t)K.dims[d];
+    }
+    chunk_bound += (K.dst_cap + kPadChunkBytes - 1) / kPadChunkBytes;
+  }
+  if (!c->capturing) CU(cudaSetDevice(c->device));
+  uint64_t var_tile_cap = 0;
+  for (int i = 0; i < n; ++i) var_tile_cap += var_record_tile_bound(rec_len[i]);
+  if (var_tile_cap > 0x7FFFFFFFull) return fail(B200TFS_E_TOOBIG, "batch needs more than 2^31 tiles");
+  const PaddedLayout L = padded_layout((uint64_t)n, (uint64_t)n_keys, var_tile_cap);
+  if ((rc = grow_dev(c, c->padded_dev, L.bytes))) return rc;
+  // rec_off | rec_len | keys | key bytes: one upload (a captured call keeps a private copy)
+  uint64_t key_bytes = 0;
+  for (int k = 0; k < n_keys; ++k) key_bytes += (uint64_t)keys[k].key_len;
+  Layout K;
+  const uint64_t o_off = K.take(8ull * n), o_len = K.take(8ull * n), o_keys = K.take(sizeof(PadKeyDev) * n_keys), o_kb = K.take(key_bytes);
+  Slot* slot;
+  uint8_t* sd;
+  rc = upload_image(c, K.end, {{o_off, rec_off, 8ull * n}, {o_len, rec_len, 8ull * n}}, &sd, &slot, [&](uint8_t* h, uint8_t* dev) {
+    uint64_t at = o_kb;
+    for (int k = 0; k < n_keys; ++k) {
+      PadKeyDev kd{};
+      kd.k = ConcatKeyDev{dev + at, (uint8_t*)keys[k].dst, keys[k].dst_cap, (uint32_t)keys[k].key_len, 0u};
+      for (int d = 0; d < B200TFS_MAX_RANK; ++d) kd.dims[d] = keys[k].dims[d];
+      memcpy(kd.pad, keys[k].pad_bits, 16);
+      kd.rank = keys[k].rank;
+      memcpy(h + o_keys + sizeof(PadKeyDev) * k, &kd, sizeof kd);
+      if (keys[k].key_len) memcpy(h + at, keys[k].key, (size_t)keys[k].key_len);
+      at += (uint64_t)keys[k].key_len;
+    }
+  });
+  if (rc) return rc;
+  for (int k = 0; k < n_keys; ++k) c->padded_res.dst[k] = (uint8_t*)keys[k].dst;
+  uint8_t* d = (uint8_t*)c->padded_dev.p;
+  const uint64_t* off_dev = (const uint64_t*)(sd + o_off);
+  CU(launch_parse_responses((const uint8_t*)arena_dev, off_dev, (const uint64_t*)(sd + o_len), n, kFusedMaxOutputs, (b200tfs_output*)(d + L.outs),
+                            (int32_t*)(d + L.nouts), (b200tfs_model_spec*)(d + L.specs), (int32_t*)(d + L.status), nullptr, 0u,
+                            (uint32_t*)(d + L.spill), c->stream));
+  PaddedPlan pp{};
+  ConcatPlan& cp = pp.cp;
+  cp.w = (const uint8_t*)arena_dev; cp.rec_off = off_dev; cp.outs = (const b200tfs_output*)(d + L.outs);
+  cp.n_outs = (const int32_t*)(d + L.nouts); cp.rec_status = (const int32_t*)(d + L.status);
+  cp.n = (uint32_t)n; cp.n_keys = (uint32_t)n_keys; cp.out_stride = kFusedMaxOutputs + 1; cp.cast = c->decode_cast;
+  cp.kst = (int32_t*)(d + L.kst); cp.match = (int32_t*)(d + L.match);
+  cp.vouts = (b200tfs_output*)(d + L.vouts); cp.vn_outs = (int32_t*)(d + L.vnouts); cp.vrec_status = (int32_t*)(d + L.vstatus);
+  pp.keys = (const PadKeyDev*)(sd + o_keys);
+  pp.desc = (PadDesc*)(d + L.desc); pp.first_row = (uint64_t*)(d + L.first_row); pp.kout = (PadKeyOut*)(d + L.kout);
+  const uint32_t emit_grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(chunk_bound, (uint64_t)c->sm_count * 8));
+  CU(launch_padded(pp, emit_grid, c->stream));
+  // packed-varint outputs: the single-launch decode's plan / count, and an emit that stores every element at its padded position
+  VarPlan vp{};
+  vp.outs = cp.vouts; vp.n_outs = cp.vn_outs; vp.rec_status = cp.vrec_status;
+  vp.w = cp.w; vp.rec_off = off_dev;
+  vp.dst = nullptr; vp.dst_stride = 0; vp.n = (uint32_t)n; vp.tile_cap = (uint32_t)var_tile_cap;
+  const VarPadMap pm{pp.desc, pp.keys, (uint32_t)n_keys, 0u};
+  if ((rc = launch_varint_tail(c, vp, d + L.var, rec_off, &pm))) return rc;
+  if (slot->done && !c->capturing) { CU(cudaEventRecord(slot->done, c->stream)); slot->pending = true; }   // the kernels read the upload
+  c->launches += 3;
+  c->padded_res.n = n; c->padded_res.k = n_keys;
+  c->padded_res.vouts = L.vouts; c->padded_res.vstat = L.var_status; c->padded_res.specs = L.specs; c->padded_res.status = L.status;
+  return B200TFS_OK;
+}
+
+int b200tfs_decode_padded_host_async(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                                     int32_t n_keys, const b200tfs_pad_key* keys) {
+  if (!c || n <= 0 || !wire_host || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
+  if (c->capturing) return fail(B200TFS_E_ARG, "capture b200tfs_decode_padded over a device arena instead");
+  CU(cudaSetDevice(c->device));
+  uint64_t span;
+  int rc = stage_wire(c, wire_host, n, rec_off, rec_len, &span);
+  if (rc) return rc;
+  return b200tfs_decode_padded(c, c->stage_dev.p, n, rec_off, rec_len, n_keys, keys);
+}
+
+int b200tfs_padded_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs, int32_t* rec_status) {
+  if (!c) return fail(B200TFS_E_ARG, "bad arguments");
+  return key_results(c, c->padded_res, (const uint8_t*)c->padded_dev.p, "b200tfs_decode_padded", n, n_keys, outs, specs, rec_status);
 }
 
 }  // extern "C"

@@ -1073,6 +1073,36 @@ __device__ __forceinline__ uint64_t concat_scan(uint64_t v, uint64_t& carry, uns
   return before + inc - v;
 }
 
+// pass A of the key plans (concat_plan_kernel, padded_plan_kernel): the key in each record's table, and the record's own verdict
+// on it, into cp.kst / cp.match; *ref_rec (shared, n on entry) receives the first record that decoded the key
+__device__ __forceinline__ void plan_match_key(const ConcatPlan& cp, const uint8_t* kb, uint32_t key_len, uint32_t k, uint32_t* ref_rec) {
+  const uint32_t n = cp.n, nk = cp.n_keys;
+  for (uint32_t r = threadIdx.x; r < n; r += kConcatPlanThreads) {
+    int32_t st = cp.rec_status[r], m = -1;
+    if (st == B200TFS_E_SPILL || st == B200TFS_E_SIZE) st = B200TFS_E_NONCANONICAL;   // more than the table holds: another route
+    if (st == B200TFS_OK) {
+      const b200tfs_output* t = cp.outs + (size_t)r * cp.out_stride;
+      const uint8_t* rec = cp.w + cp.rec_off[r];
+      for (int32_t j = 0; j < cp.n_outs[r] && m < 0; ++j) {
+        if (t[j].key_len != key_len) continue;
+        bool same = true;
+        for (uint32_t i = 0; i < key_len && same; ++i) same = rec[t[j].key_off + i] == kb[i];
+        if (same) m = j;
+      }
+      if (m < 0) st = B200TFS_E_KEY;
+      else {
+        const b200tfs_output& o = t[m];
+        st = o.status;
+        if (st == B200TFS_OK && o.rank == 0) st = B200TFS_E_SHAPE;
+        if (st == B200TFS_OK && o.rank > B200TFS_MAX_RANK) st = B200TFS_E_NONCANONICAL;
+      }
+    }
+    cp.kst[(size_t)r * nk + k] = st;
+    cp.match[(size_t)r * nk + k] = m;
+    if (st == B200TFS_OK) atomicMin(ref_rec, r);
+  }
+}
+
 __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const __grid_constant__ ConcatPlan cp) {
   __shared__ unsigned long long warp_sum[kConcatPlanThreads / 32];
   __shared__ uint32_t ref_rec;
@@ -1086,31 +1116,7 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
     const ConcatKeyDev key = cp.keys[k];
     if (threadIdx.x == 0) ref_rec = n;
     __syncthreads();
-    // pass A: the key in each record's table, and the record's own verdict on it
-    for (uint32_t r = threadIdx.x; r < n; r += kConcatPlanThreads) {
-      int32_t st = cp.rec_status[r], m = -1;
-      if (st == B200TFS_E_SPILL || st == B200TFS_E_SIZE) st = B200TFS_E_NONCANONICAL;   // more than the table holds: another route
-      if (st == B200TFS_OK) {
-        const b200tfs_output* t = cp.outs + (size_t)r * cp.out_stride;
-        const uint8_t* rec = cp.w + cp.rec_off[r];
-        for (int32_t j = 0; j < cp.n_outs[r] && m < 0; ++j) {
-          if (t[j].key_len != key.key_len) continue;
-          bool same = true;
-          for (uint32_t i = 0; i < key.key_len && same; ++i) same = rec[t[j].key_off + i] == key.key[i];
-          if (same) m = j;
-        }
-        if (m < 0) st = B200TFS_E_KEY;
-        else {
-          const b200tfs_output& o = t[m];
-          st = o.status;
-          if (st == B200TFS_OK && o.rank == 0) st = B200TFS_E_SHAPE;
-          if (st == B200TFS_OK && o.rank > B200TFS_MAX_RANK) st = B200TFS_E_NONCANONICAL;
-        }
-      }
-      cp.kst[(size_t)r * nk + k] = st;
-      cp.match[(size_t)r * nk + k] = m;
-      if (st == B200TFS_OK) atomicMin(&ref_rec, r);
-    }
+    plan_match_key(cp, key.key, key.key_len, k, &ref_rec);
     __syncthreads();
     const uint32_t rr = ref_rec;
     const b200tfs_output* ro = rr < n ? cp.outs + (size_t)rr * cp.out_stride + cp.match[(size_t)rr * nk + k] : nullptr;
@@ -1178,6 +1184,11 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
     *reinterpret_cast<PlanHeader*>(cp.plan) = ph;
   }
 }
+
+// ------------------------------------------------------------------------------------------------
+// decode into one padded tensor per key: padded_plan_kernel / padded_emit_kernel
+// ------------------------------------------------------------------------------------------------
+#include "padded_kernels.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // tf.Example requests (Classify / Regress): ex_count / ex_scan / ex_emit / ex_frame
@@ -1396,12 +1407,22 @@ cudaError_t launch_vdec_plan(const VarPlan& vp, cudaStream_t stream) {
   vdec_plan_kernel<<<1, kVarPlanThreads, 0, stream>>>(vp);
   return cudaGetLastError();
 }
-cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t stream) {
+cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t stream, const VarPadMap* pm) {
   const uint32_t per = kVarThreads / 32;
   vdec_count_dev_kernel<<<std::max(1u, std::min((tb.n_tiles + per - 1) / per, max_ctas)), kVarThreads, 0, stream>>>(tb);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
-  vdec_emit_dev_kernel<<<std::max(1u, std::min(tb.n_tiles, max_ctas)), kVarThreads, 0, stream>>>(tb);
+  const uint32_t grid = std::max(1u, std::min(tb.n_tiles, max_ctas));
+  if (pm) vdec_emit_padded_kernel<<<grid, kVarThreads, 0, stream>>>(tb, *pm);
+  else vdec_emit_dev_kernel<<<grid, kVarThreads, 0, stream>>>(tb);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_padded(const PaddedPlan& pp, uint32_t emit_grid, cudaStream_t stream) {
+  padded_plan_kernel<<<1, kConcatPlanThreads, 0, stream>>>(pp);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return e;
+  padded_emit_kernel<<<std::max(1u, emit_grid), kPadEmitThreads, 0, stream>>>(pp);
   return cudaGetLastError();
 }
 

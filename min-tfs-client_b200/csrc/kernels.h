@@ -41,10 +41,13 @@ cudaError_t launch_vdec_emit(const VarTables& tb, cudaStream_t stream);
 // packed-varint outputs of the single-launch decode: the plan kernel, then count + emit over the tables it built (tb.n_tiles is
 // the host's bound, tb.n_tiles_dev the real count; each kernel runs at most max_ctas CTAs and strides over the tiles)
 cudaError_t launch_vdec_plan(const VarPlan& vp, cudaStream_t stream);
-cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t stream);
+// (pm: the padded decode's emit, every element at its padded position)
+cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t stream, const VarPadMap* pm = nullptr);
 // b200tfs_decode_concat: concat_plan_kernel, then move_kernel over the plan image it wrote, with move_grid CTAs (the host's bound
 // on the tiles; the CTAs past the plan's own count leave at once)
 cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStream_t stream);
+// b200tfs_decode_padded: padded_plan_kernel, then padded_emit_kernel with emit_grid CTAs striding over the chunks
+cudaError_t launch_padded(const PaddedPlan& pp, uint32_t emit_grid, cudaStream_t stream);
 // tf.Example requests (example_kernels.cuh): count + scan (when T.n_tiles), emit, frame; *launched receives how many kernels
 cudaError_t launch_example_requests(const ExTables& T, cudaStream_t stream, uint32_t* launched);
 // Classify / Regress responses (example_resp_kernels.cuh): index, scan, emit, [label compare,] publish; emit_ctas CTAs stride over

@@ -254,6 +254,43 @@ constexpr uint64_t concat_record_tile_bound(uint64_t len, uint64_t tile_bytes, u
   return len / tile_bytes + 1ull + (uint64_t)n_keys * B200TFS_MAX_RUNS;
 }
 
+// ---- decode into one padded tensor per key (b200tfs_decode_padded) ----------------------------------------------------
+// padded_plan_kernel (one CTA) matches the keys with concat_plan_kernel's pass A, checks every record against the first one that
+// decoded the key and against the destination's trailing dims, scans the rows into first rows and writes one PadDesc per
+// (record, key), the per-key summary and the single-launch decode's table for the varint tail (as ConcatPlan::vouts).
+// padded_emit_kernel then writes the destination in chunks of kPadChunkBytes, a grid-stride loop over the chunks of every key.
+constexpr uint32_t kPadEmitThreads = 256;
+constexpr uint32_t kPadEmitVecs = 4;                                  // 16-byte vectors per thread and chunk
+constexpr uint64_t kPadChunkBytes = 16ull * kPadEmitThreads * kPadEmitVecs;
+struct PadKeyDev {
+  ConcatKeyDev k;                  // key bytes, dst, cap
+  int64_t dims[B200TFS_MAX_RANK];  // the destination's trailing dims (dims[0] unused)
+  uint8_t pad[16];                 // the pad element's bits
+  int32_t rank, pad_;
+};
+struct PadDesc {                   // one (record, key): its value runs, its own dims, its rows in the destination
+  b200tfs_run runs[B200TFS_MAX_RUNS];
+  int64_t dims[B200TFS_MAX_RANK];
+  const uint8_t* rec;
+  uint64_t first_row, rows;        // rows 0: no place
+  uint32_t n_runs, pad_;
+};
+struct PadKeyOut {                 // one key after the plan
+  uint64_t rows, pitch;            // rows in use, destination bytes per row
+  uint64_t chunk0;                 // first chunk of the key (entry n_keys: the chunks of every key)
+  uint32_t row_elems, esz, src_esz, op, varint, pad_;
+};
+struct PaddedPlan {
+  ConcatPlan cp;                   // the parse table, scratch and varint table (cp.keys unused)
+  const PadKeyDev* keys;           // [n_keys]
+  PadDesc* desc;                   // [n * n_keys]: record r, key k at r * n_keys + k
+  uint64_t* first_row;             // [n_keys * n]
+  PadKeyOut* kout;                 // [n_keys + 1]
+};
+// the varint tail of the padded decode: job s = r * kFusedMaxOutputs + k (vdec_plan_kernel's slot) stores element e of record r
+// at its padded position - mixed-radix over the record's dims into the destination's - from jb.dst, the record's first row
+struct VarPadMap { const PadDesc* desc; const PadKeyDev* keys; uint32_t n_keys, pad_; };
+
 // ---- deferred framing: the length prefixes of packed-varint inputs computed ON THE DEVICE -----------------------------
 // Every length on the wire precedes its content, and a packed-varint payload's length is only known once the counting
 // kernel has run.  Instead of bringing it to the host (b200tfs_measure: a stream synchronise in the middle of an encode),

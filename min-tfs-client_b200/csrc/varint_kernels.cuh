@@ -422,13 +422,33 @@ __device__ __forceinline__ uint32_t compress28(uint32_t y) {
 // bytes up to and including the first terminator of `t` (terminator flags at bit 7 of each byte) kept, the rest cleared
 __device__ __forceinline__ uint32_t through_terminator(uint32_t t) { return ((t & (0u - t)) << 1) - 1u; }
 
+// the padded position (in elements from the record's first row) of element e of job `job` (VarPadMap)
+__device__ __forceinline__ uint64_t var_pad_index(const VarPadMap& pm, uint32_t job, uint64_t e) {
+  const uint32_t r = job / kFusedMaxOutputs, k = job % kFusedMaxOutputs;
+  const PadDesc& d = pm.desc[(size_t)r * pm.n_keys + k];
+  const PadKeyDev& key = pm.keys[k];
+  uint64_t own_row = 1, dst_row = 1;
+  for (int32_t a = 1; a < key.rank; ++a) { own_row *= (uint64_t)d.dims[a]; dst_row *= (uint64_t)key.dims[a]; }
+  const uint64_t lr = e / own_row;
+  uint64_t x = e - lr * own_row, at = 0, stride = 1;
+  for (int32_t a = key.rank - 1; a >= 1; --a) {
+    const uint64_t q = x / (uint64_t)d.dims[a];
+    at += (x - q * (uint64_t)d.dims[a]) * stride;
+    stride *= (uint64_t)key.dims[a];
+    x = q;
+  }
+  return lr * dst_row + at;
+}
+
 // element j of the tile starts at smraw[start_at[j]]: 12-byte window by funnel shifts, cut after its terminator.
 // Two shapes, chosen per warp: every lane's varint ends inside its first four bytes (values below 2^28:
 // indices, token ids, small counts), or the general branch-free form.  A varint that never terminates inside the
 // chunk is caught by the caller (the chunk's last byte has its continuation bit set); here only the eleven-byte case.
-template <int K>
+// PAD: element idx0 + j goes to its padded position (var_pad_index) instead of the next one in flat order.
+template <int K, bool PAD = false>
 __device__ __forceinline__ int32_t decode_elems(const uint8_t* smraw, const uint16_t* start_at, uint32_t n_here,
-                                                uint8_t* dst, uint64_t idx0, uint64_t n_elems) {
+                                                uint8_t* dst, uint64_t idx0, uint64_t n_elems, const VarPadMap& pm = VarPadMap{},
+                                                uint32_t job = 0) {
   int32_t st = B200TFS_OK;
   const uint64_t room = n_elems > idx0 ? n_elems - idx0 : 0;   // elements of the tensor this tile may still write
   const uint32_t n_store = (uint32_t)min((uint64_t)n_here, room);
@@ -456,7 +476,10 @@ __device__ __forceinline__ int32_t decode_elems(const uint8_t* smraw, const uint
       v_lo = c0 | (c1 << 28);
       v_hi = (c1 >> 4) | (c2 << 24);
     }
-    if (j < n_store) store_decoded<K>(out, j, (uint64_t)v_lo | ((uint64_t)v_hi << 32), &st);
+    if (j < n_store) {
+      if (PAD) store_decoded<K>(dst, var_pad_index(pm, job, idx0 + j), (uint64_t)v_lo | ((uint64_t)v_hi << 32), &st);
+      else store_decoded<K>(out, j, (uint64_t)v_lo | ((uint64_t)v_hi << 32), &st);
+    }
   }
   return st;
 }
@@ -466,7 +489,8 @@ __device__ __forceinline__ int32_t decode_elems(const uint8_t* smraw, const uint
 // finds the varints that START there (previous byte is a terminator - the zero before the chunk's first byte
 // is one); a block scan ranks them; they are compacted into a list so that the decode step hands out
 // ELEMENTS, not byte blocks, to threads: balanced work and coalesced stores.
-__device__ __forceinline__ void vdec_emit_tile(const VarTables& tb, uint32_t t) {
+template <bool PAD = false>
+__device__ __forceinline__ void vdec_emit_tile(const VarTables& tb, uint32_t t, const VarPadMap& pm = VarPadMap{}) {
   constexpr uint32_t kBlocks = kVarTileBytes / 16;             // 512: two per thread
   __shared__ __align__(16) uint8_t smraw[16 + kVarTileBytes + 16];
   __shared__ uint16_t start_at[kVarTileBytes];
@@ -542,17 +566,18 @@ __device__ __forceinline__ void vdec_emit_tile(const VarTables& tb, uint32_t t) 
   const uint64_t idx0 = before + (smraw[15] >> 7);
   if (threadIdx.x == 0 && hi > G && hi <= G + kVarTileBytes && (hi[-1] & 0x80)) atomicMin(jb.status, B200TFS_E_PARSE);   // the chunk's last varint never ends
   int32_t st_local;
+  const uint32_t job = sg.job;
   switch (jb.dtype) {
-    case DT_INT64: case DT_UINT64: st_local = decode_elems<VS_U64>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
-    case DT_INT32: case DT_UINT32: st_local = decode_elems<VS_U32>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
-    case DT_INT16: st_local = decode_elems<VS_I16>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
-    case DT_INT8: st_local = decode_elems<VS_I8>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
-    case DT_UINT16: st_local = decode_elems<VS_U16>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
-    case DT_UINT8: st_local = decode_elems<VS_U8>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
-    case DT_BOOL: st_local = decode_elems<VS_BOOL>(smraw, start_at, n_here, jb.dst, idx0, n_store); break;
+    case DT_INT64: case DT_UINT64: st_local = decode_elems<VS_U64, PAD>(smraw, start_at, n_here, jb.dst, idx0, n_store, pm, job); break;
+    case DT_INT32: case DT_UINT32: st_local = decode_elems<VS_U32, PAD>(smraw, start_at, n_here, jb.dst, idx0, n_store, pm, job); break;
+    case DT_INT16: st_local = decode_elems<VS_I16, PAD>(smraw, start_at, n_here, jb.dst, idx0, n_store, pm, job); break;
+    case DT_INT8: st_local = decode_elems<VS_I8, PAD>(smraw, start_at, n_here, jb.dst, idx0, n_store, pm, job); break;
+    case DT_UINT16: st_local = decode_elems<VS_U16, PAD>(smraw, start_at, n_here, jb.dst, idx0, n_store, pm, job); break;
+    case DT_UINT8: st_local = decode_elems<VS_U8, PAD>(smraw, start_at, n_here, jb.dst, idx0, n_store, pm, job); break;
+    case DT_BOOL: st_local = decode_elems<VS_BOOL, PAD>(smraw, start_at, n_here, jb.dst, idx0, n_store, pm, job); break;
     case DT_HALF: case DT_BFLOAT16:
-      st_local = (jb.flags & kVarFlagHalfAsValue) ? decode_elems<VS_HALF_VALUE>(smraw, start_at, n_here, jb.dst, idx0, n_store)
-                                                  : decode_elems<VS_HALF_BITS>(smraw, start_at, n_here, jb.dst, idx0, n_store);
+      st_local = (jb.flags & kVarFlagHalfAsValue) ? decode_elems<VS_HALF_VALUE, PAD>(smraw, start_at, n_here, jb.dst, idx0, n_store, pm, job)
+                                                  : decode_elems<VS_HALF_BITS, PAD>(smraw, start_at, n_here, jb.dst, idx0, n_store, pm, job);
       break;
     default: st_local = B200TFS_OK; break;
   }
@@ -564,6 +589,14 @@ __global__ void __launch_bounds__(kVarThreads) vdec_emit_dev_kernel(const __grid
   const uint32_t nt = *tb.n_tiles_dev;
   for (uint32_t t = blockIdx.x; t < nt; t += gridDim.x) {
     vdec_emit_tile(tb, t);
+    __syncthreads();
+  }
+}
+// the same for the padded decode (b200tfs_decode_padded): every element goes to its padded position
+__global__ void __launch_bounds__(kVarThreads) vdec_emit_padded_kernel(const __grid_constant__ VarTables tb, const __grid_constant__ VarPadMap pm) {
+  const uint32_t nt = *tb.n_tiles_dev;
+  for (uint32_t t = blockIdx.x; t < nt; t += gridDim.x) {
+    vdec_emit_tile<true>(tb, t, pm);
     __syncthreads();
   }
 }

@@ -85,6 +85,16 @@ class ConcatKey(C.Structure):
     ]
 
 
+class PadKey(C.Structure):
+    """b200tfs_pad_key: one requested output of b200tfs_decode_padded (in: key, dst, dst_cap, rank, dims[1:], pad_bits; out: the
+    layout)."""
+    _fields_ = [
+        ("key", C.c_char_p), ("key_len", C.c_int64), ("dst", C.c_void_p), ("dst_cap", C.c_uint64), ("dtype", C.c_int32),
+        ("rank", C.c_int32), ("dims", C.c_int64 * MAX_RANK), ("bytes", C.c_uint64), ("status", C.c_int32), ("bad_rec", C.c_int32),
+        ("pad_bits", C.c_uint8 * 16),
+    ]
+
+
 F_BROADCAST = 0x10
 
 
@@ -172,6 +182,10 @@ SIGNATURES = {
     "b200tfs_decode_concat": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(ConcatKey)]),
     "b200tfs_decode_concat_host_async": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(ConcatKey)]),
     "b200tfs_concat_results": (C.c_int, [_vp, C.c_int32, C.c_int32, C.POINTER(Output), C.POINTER(ModelSpec), _i32p]),
+    "b200tfs_padded_layout": (C.c_int, [_vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey), C.c_int32]),
+    "b200tfs_decode_padded": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey)]),
+    "b200tfs_decode_padded_host_async": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey)]),
+    "b200tfs_padded_results": (C.c_int, [_vp, C.c_int32, C.c_int32, C.POINTER(Output), C.POINTER(ModelSpec), _i32p]),
     "b200tfs_capture_begin": (C.c_int, [_vp]),
     "b200tfs_capture_end": (C.c_int, [_vp, _vpp]),
     "b200tfs_graph_launch": (C.c_int, [_vp, _vp]),

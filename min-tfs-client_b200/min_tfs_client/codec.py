@@ -355,6 +355,8 @@ class Codec:
         self._seen_varints = False
         # decode_predict_responses_concat calls the device route finished (the others were decoded response by response)
         self.concat_device_calls = 0
+        # decode_predict_responses_padded calls the device route finished
+        self.padded_device_calls = 0
         # decode_regression_responses / decode_classification_responses calls the device route finished
         self.example_response_device_calls = 0
         self._xr_scratch = None       # their device destinations when the result goes to host memory: (values, labels)
@@ -855,6 +857,15 @@ class Codec:
             raise ValueError("need at least one response to concatenate")
         out = dict(out or {})
         buf, off, ln = self._pack_wires(wires)
+        keys, out_dtypes = self._requested(wires, buf, off, ln, keys, out, out_dtypes)
+        fast = self._concat_device(wires, buf, off, ln, keys, strict, out_dtypes, device, out) if len(keys) <= N.CONCAT_MAX_KEYS else None
+        if fast is not None:
+            return fast
+        return self._concat_per_record(wires, keys, strict, out_dtypes, device, out)
+
+    def _requested(self, wires, buf, off, ln, keys, out, out_dtypes):
+        """The requested keys of a per-key batch decode (None: every key of the first response), and out_dtypes restricted to
+        them.  KeyError for a key of `out` that is not requested."""
         if keys is None:
             keys = self._response_keys(buf, int(off[0]), int(ln[0]))
             if keys is None:      # the first response does not parse: the parse raises what the reference raises
@@ -868,10 +879,7 @@ class Codec:
                 raise KeyError(k)
         if out_dtypes:        # only the requested outputs are decoded: entries for other keys play no part
             out_dtypes = {k: v for k, v in out_dtypes.items() if k in keys} or None
-        fast = self._concat_device(wires, buf, off, ln, keys, strict, out_dtypes, device, out) if len(keys) <= N.CONCAT_MAX_KEYS else None
-        if fast is not None:
-            return fast
-        return self._concat_per_record(wires, keys, strict, out_dtypes, device, out)
+        return keys, out_dtypes
 
     def _response_keys(self, buf, base: int, length: int) -> Optional[List[str]]:
         cap = 64
@@ -941,19 +949,8 @@ class Codec:
                 return None
             shapes.append(tuple(int(c.dims[d]) for d in range(c.rank)))
             np_types.append(np.dtype(numpy_for_enum(cast_code if cast_code and c.dtype == DT_FLOAT else int(c.dtype))))
-        # destinations: the caller's device arrays, else device arrays of our own (returned, or copied into the host result)
-        dev, ptrs, holds = [], [], []
-        for i, k in enumerate(keys):
-            dst = out.get(k)
-            view = None if dst is None else _check_out(k, dst, np_types[i], shapes[i], contiguous=True)
-            if view is not None:
-                dev.append(dst)
-                ptrs.append(view[0])
-                holds.append(view)
-            else:
-                a = D.DeviceArray(self, shapes[i], np_types[i])
-                dev.append(a)
-                ptrs.append(a.ptr)
+        dev, ptrs, holds = self._key_destinations(keys, out, shapes, np_types)
+        for i in range(nk):
             ck[i].dst, ck[i].dst_cap = ptrs[i], int(ck[i].bytes)
         wire = D.DeviceArray(self, (len(buf),), np.uint8).copy_from_host(buf)
         with self._decode_modes(cast_code):
@@ -986,6 +983,30 @@ class Codec:
             N.check(self._lib.b200tfs_unpack_outputs(self._ctx, wire.ptr, m, o_arr, rec, dd, codes, st))
             if any(st[q] != N.OK for q in range(m)):
                 return None
+        result = self._key_deliver(keys, out, device, shapes, np_types, dev, ptrs)
+        self.concat_device_calls += 1
+        return result, [self._spec(buf, int(off[r]), specs[r]) for r in range(n)]
+
+    def _key_destinations(self, keys, out, shapes, np_types):
+        """Device destinations of a per-key device decode: the caller's device arrays, else device arrays of our own (returned,
+        or copied into the host result).  Returns (arrays, pointers, keep-alives)."""
+        dev, ptrs, holds = [], [], []
+        for i, k in enumerate(keys):
+            dst = out.get(k)
+            view = None if dst is None else _check_out(k, dst, np_types[i], shapes[i], contiguous=True)
+            if view is not None:
+                dev.append(dst)
+                ptrs.append(view[0])
+                holds.append(view)
+            else:
+                a = D.DeviceArray(self, shapes[i], np_types[i])
+                dev.append(a)
+                ptrs.append(a.ptr)
+        return dev, ptrs, holds
+
+    def _key_deliver(self, keys, out, device, shapes, np_types, dev, ptrs):
+        """{key: result} of a per-key device decode that finished: the caller's device array, the caller's host array or a new
+        one (one device-to-host copy each), or our device array.  Synchronises."""
         result = {}
         for i, k in enumerate(keys):
             dst = out.get(k)
@@ -999,8 +1020,126 @@ class Codec:
             else:
                 result[k] = dev[i]
         self.sync()
-        self.concat_device_calls += 1
-        return result, [self._spec(buf, int(off[r]), specs[r]) for r in range(n)]
+        return result
+
+    # ---- batch decode into one padded tensor per key -----------------------------------------------------
+    def decode_predict_responses_padded(self, wires: Sequence[bytes], keys: Optional[Sequence[str]] = None, *, pad_value=0,
+                                        pad_to: Optional[Mapping] = None, strict: bool = False, out_dtypes: Optional[Mapping] = None,
+                                        device: bool = False, out: Optional[Mapping] = None
+                                        ) -> Tuple[Dict[str, object], Dict[str, np.ndarray], List[DecodedSpec]]:
+        """Decode a batch of PredictResponses with ragged trailing dimensions into ONE padded tensor per output - what
+        ``pad_sequence`` / ``tf.keras.utils.pad_sequences`` give: for every key, the rows of all responses concatenated along axis
+        0, every other axis padded at its end with ``pad_value`` to the batch maximum, or to ``pad_to[key]`` (the trailing dims).
+        Bit for bit, and with the same exceptions, what this does with the per-response decode::
+
+            parts = [decode_predict_responses([w], strict=strict, out_dtypes=out_dtypes)[0][0][key] for w in wires]
+            tail = pad_to[key] if key in pad_to else elementwise max of p.shape[1:]     # rank 0 / other ranks: ValueError
+            res = np.full((sum(p.shape[0] for p in parts), *tail), pad_value, dtype)    # other dtypes: ValueError
+            # part r fills res[r0:r0 + rows_r, :d1, :d2, ...]; a part larger than pad_to: ValueError
+
+        ``keys``, ``strict``, ``out_dtypes``, ``device`` and ``out`` as for ``decode_predict_responses_concat`` (a narrowed output
+        gets the pad converted to the narrowed dtype).  Returns ``({key: tensor}, {key: int64[n, rank] shape of every response's
+        output}, [DecodedSpec per response])``.
+        """
+        n = len(wires)
+        if n == 0:
+            raise ValueError("need at least one response to pad")
+        out = dict(out or {})
+        buf, off, ln = self._pack_wires(wires)
+        keys, out_dtypes = self._requested(wires, buf, off, ln, keys, out, out_dtypes)
+        pad_to = dict(pad_to or {})
+        fast = self._padded_device(wires, buf, off, ln, keys, pad_value, pad_to, strict, out_dtypes, device, out) \
+            if len(keys) <= N.CONCAT_MAX_KEYS else None
+        if fast is not None:
+            return fast
+        return self._padded_per_record(wires, keys, pad_value, pad_to, strict, out_dtypes, device, out)
+
+    def _padded_per_record(self, wires, keys, pad_value, pad_to, strict, out_dtypes, device, out):
+        """The definition itself, response by response and padded with numpy: what the device route hands over when a batch
+        holds a case it does not take (a malformed record, more than FUSED_MAX_OUTPUTS outputs or MAX_RANK dims, TF padding,
+        tensor_content only, strings, packed varints in rows of unpacked elements, any error)."""
+        wanted = set(keys)
+        per = [self._decode_two_phase([w], strict, out_dtypes, 16, wanted)[0] for w in wires]
+        result, shapes = {}, {}
+        for k in keys:
+            parts = [p[0][k] for p in per]
+            rank = parts[0].ndim
+            if rank == 0 or any(a.ndim != rank for a in parts):
+                raise ValueError(f"output {k!r}: every response must have the same rank >= 1 to be padded")
+            if len({a.dtype for a in parts}) > 1:
+                raise ValueError(f"output {k!r}: responses disagree on the dtype ({', '.join(sorted({str(a.dtype) for a in parts}))})")
+            tail = tuple(int(x) for x in pad_to[k]) if k in pad_to else \
+                tuple(max(a.shape[d] for a in parts) for d in range(1, rank))
+            if len(tail) != rank - 1:
+                raise ValueError(f"output {k!r}: pad_to has {len(tail)} trailing dims, the output {rank - 1}")
+            res = np.full((sum(a.shape[0] for a in parts), *tail), pad_value, parts[0].dtype)
+            r0 = 0
+            for a in parts:
+                if any(a.shape[d] > tail[d - 1] for d in range(1, rank)):
+                    raise ValueError(f"output {k!r}: a response of shape {a.shape} does not fit pad_to {tail}")
+                res[(slice(r0, r0 + a.shape[0]),) + tuple(slice(0, d) for d in a.shape[1:])] = a
+                r0 += a.shape[0]
+            if device and res.dtype.kind in "US":
+                raise TypeError(f"output {k!r}: string tensors are decoded on the host")
+            result[k] = self._concat_deliver(k, res, device, out)
+            shapes[k] = np.array([a.shape for a in parts], dtype=np.int64).reshape(len(parts), rank)
+        return result, shapes, [p[1] for p in per]
+
+    def _padded_device(self, wires, buf, off, ln, keys, pad_value, pad_to, strict, out_dtypes, device, out):
+        """The device route (b200tfs_decode_padded): parse, one-CTA plan, destination-major emit, varint decode - or None
+        when the batch holds a case it leaves to the response-by-response route.  The host layout runs first, so nothing is
+        written into `out` for a batch that route then refuses."""
+        n, nk = len(wires), len(keys)
+        kb = [k.encode("utf-8") for k in keys]
+        cast_code = 0
+        if out_dtypes:
+            cast_code = None if strict else _narrowing_cast(out_dtypes)
+            if cast_code is None:
+                return None
+        pk = (N.PadKey * nk)()
+        for i, k in enumerate(kb):
+            pk[i].key, pk[i].key_len = k, len(k)
+        N.check(self._lib.b200tfs_padded_layout(buf.ctypes.data, n, off, ln, nk, pk, cast_code))
+        shapes, np_types, pads = [], [], []
+        for i in range(nk):
+            c = pk[i]
+            # strict DT_HALF: the reference reads half_val as values, the device writes TF's bit patterns
+            if c.status != N.OK or c.dtype == DT_STRING or strict and c.dtype in (DT_HALF, DT_BFLOAT16, DT_COMPLEX64, DT_COMPLEX128):
+                return None
+            if cast_code and not _narrowing_fits(c.dtype, keys[i], out_dtypes):
+                return None
+            tail = tuple(int(c.dims[d]) for d in range(1, c.rank))
+            if keys[i] in pad_to:
+                want = tuple(int(x) for x in pad_to[keys[i]])
+                if len(want) != len(tail) or any(t > w for t, w in zip(tail, want)):
+                    return None   # the definition raises, after decoding every response
+                tail = want
+            np_types.append(np.dtype(numpy_for_enum(cast_code if cast_code and c.dtype == DT_FLOAT else int(c.dtype))))
+            shapes.append((int(c.dims[0]),) + tail)
+            try:
+                pads.append(np.full((1,), pad_value, np_types[i]).tobytes())
+            except Exception:     # noqa: BLE001 - the definition raises it, after decoding every response
+                return None
+        dev, ptrs, holds = self._key_destinations(keys, out, shapes, np_types)
+        if any(p % 16 for p in ptrs):
+            return None           # the emit writes whole 16-byte vectors
+        for i in range(nk):
+            pk[i].dst, pk[i].dst_cap, pk[i].rank = ptrs[i], int(np.prod(shapes[i], dtype=np.int64)) * np_types[i].itemsize, len(shapes[i])
+            for d in range(1, len(shapes[i])):
+                pk[i].dims[d] = shapes[i][d]
+            C.memmove(pk[i].pad_bits, pads[i], len(pads[i]))
+        wire = D.DeviceArray(self, (len(buf),), np.uint8).copy_from_host(buf)
+        with self._decode_modes(cast_code):
+            N.check(self._lib.b200tfs_decode_padded(self._ctx, wire.ptr, n, off, ln, nk, pk))
+        outs, specs, rec_status = (N.Output * (n * nk))(), (N.ModelSpec * n)(), (C.c_int32 * n)()
+        N.check(self._lib.b200tfs_padded_results(self._ctx, n, nk, outs, specs, rec_status))   # synchronises
+        if any(rec_status[r] != N.OK for r in range(n)) or any(outs[j].status != N.OK for j in range(n * nk)):
+            return None
+        rec_shapes = {k: np.array([list(outs[r * nk + i].dims)[: len(shapes[i])] for r in range(n)], dtype=np.int64).reshape(n, len(shapes[i]))
+                      for i, k in enumerate(keys)}
+        result = self._key_deliver(keys, out, device, shapes, np_types, dev, ptrs)
+        self.padded_device_calls += 1
+        return result, rec_shapes, [self._spec(buf, int(off[r]), specs[r]) for r in range(n)]
 
     # ---- Classify / Regress responses ------------------------------------------------------------------
     def decode_regression_responses(self, wires: Sequence[bytes], *, device: bool = False, out=None) -> RegressionBatch:
