@@ -1356,7 +1356,7 @@ cudaError_t launch_decode_fused(const FusedParams& fp, uint32_t grid, cudaStream
       opted[dev] = true;
     }
   }
-  // Tiles of more than one 32 KB chunk (big batches: up to 256 KB per CTA) go through the TMA-staged path, which moved
+  // Tiles of more than one 32 KB chunk (big batches: 64 KB per CTA) go through the TMA-staged path, which moved
   // big batches faster.  One-chunk tiles (a single 4 MiB response) keep the register path and no staging buffers: there
   // the staged path gained little on one stream and lost bandwidth when many lanes overlap.
   if (fp.cast) {
