@@ -396,17 +396,43 @@ __global__ void __launch_bounds__(kVarThreads, 5) vdec_count_dev_kernel(const __
   for (uint32_t t = blockIdx.x * (kVarThreads / 32) + (threadIdx.x >> 5); t < nt; t += gridDim.x * (kVarThreads / 32)) vdec_count_tile(tb, t, lane);
 }
 
+// An output's status in the reference's order: FromString refuses a malformed varint (E_PARSE) before np.array() refuses an
+// out-of-range value (E_RANGE), which comes before reshape() refuses the element count (E_SHAPE).  The numeric codes do not
+// sort that way (E_RANGE < E_PARSE < E_SHAPE), so the status word is raised by rank, not by atomicMin.  Any other code
+// (E_NONCANONICAL from the plan) outranks all three: the job never ran.
+__device__ __forceinline__ uint32_t var_status_rank(int32_t s) {
+  return s == B200TFS_OK ? 0u : s == B200TFS_E_SHAPE ? 1u : s == B200TFS_E_RANGE ? 2u : s == B200TFS_E_PARSE ? 3u : 4u;
+}
+__device__ __forceinline__ void var_status_raise(int32_t* status, int32_t s) {
+  int32_t cur = *reinterpret_cast<volatile int32_t*>(status);
+  while (var_status_rank(s) > var_status_rank(cur)) {
+    const int32_t seen = atomicCAS(status, cur, s);
+    if (seen == cur) break;
+    cur = seen;
+  }
+}
+
 // how a decoded value is stored
 enum VarStore : int { VS_U64, VS_U32, VS_I16, VS_I8, VS_U16, VS_U8, VS_BOOL, VS_HALF_BITS, VS_HALF_VALUE };
+// does the value fit the element type (int_val carries the 16- and 8-bit types as 32-bit ints: np.array() checks the range)
 template <int K>
-__device__ __forceinline__ void store_decoded(uint8_t* d, uint64_t idx, uint64_t v, int32_t* status) {
+__device__ __forceinline__ bool decoded_in_range(uint64_t v) {
+  const int32_t x = (int32_t)(uint32_t)v;
+  if (K == VS_I16) return x >= -32768 && x <= 32767;
+  if (K == VS_I8) return x >= -128 && x <= 127;
+  if (K == VS_U16) return x >= 0 && x <= 65535;
+  if (K == VS_U8) return x >= 0 && x <= 255;
+  return true;
+}
+template <int K>
+__device__ __forceinline__ void store_decoded(uint8_t* d, uint64_t idx, uint64_t v) {
   const int32_t x = (int32_t)(uint32_t)v;
   if (K == VS_U64) reinterpret_cast<uint64_t*>(d)[idx] = v;
   else if (K == VS_U32) reinterpret_cast<uint32_t*>(d)[idx] = (uint32_t)v;
-  else if (K == VS_I16) { if (x < -32768 || x > 32767) *status = B200TFS_E_RANGE; reinterpret_cast<int16_t*>(d)[idx] = (int16_t)x; }
-  else if (K == VS_I8) { if (x < -128 || x > 127) *status = B200TFS_E_RANGE; reinterpret_cast<int8_t*>(d)[idx] = (int8_t)x; }
-  else if (K == VS_U16) { if (x < 0 || x > 65535) *status = B200TFS_E_RANGE; reinterpret_cast<uint16_t*>(d)[idx] = (uint16_t)x; }
-  else if (K == VS_U8) { if (x < 0 || x > 255) *status = B200TFS_E_RANGE; d[idx] = (uint8_t)x; }
+  else if (K == VS_I16) reinterpret_cast<int16_t*>(d)[idx] = (int16_t)x;
+  else if (K == VS_I8) reinterpret_cast<int8_t*>(d)[idx] = (int8_t)x;
+  else if (K == VS_U16) reinterpret_cast<uint16_t*>(d)[idx] = (uint16_t)x;
+  else if (K == VS_U8) d[idx] = (uint8_t)x;
   else if (K == VS_BOOL) d[idx] = v != 0;
   else if (K == VS_HALF_BITS) reinterpret_cast<uint16_t*>(d)[idx] = (uint16_t)v;
   else reinterpret_cast<uint16_t*>(d)[idx] = __half_as_ushort(__int2half_rn(x));
@@ -476,9 +502,12 @@ __device__ __forceinline__ int32_t decode_elems(const uint8_t* smraw, const uint
       v_lo = c0 | (c1 << 28);
       v_hi = (c1 >> 4) | (c2 << 24);
     }
+    const uint64_t v = (uint64_t)v_lo | ((uint64_t)v_hi << 32);
+    // every value is range-checked, stored or not (a wrong element count stores nothing, yet np.array() sees every value)
+    if (j < n_here && !decoded_in_range<K>(v) && st != B200TFS_E_PARSE) st = B200TFS_E_RANGE;
     if (j < n_store) {
-      if (PAD) store_decoded<K>(dst, var_pad_index(pm, job, idx0 + j), (uint64_t)v_lo | ((uint64_t)v_hi << 32), &st);
-      else store_decoded<K>(out, j, (uint64_t)v_lo | ((uint64_t)v_hi << 32), &st);
+      if (PAD) store_decoded<K>(dst, var_pad_index(pm, job, idx0 + j), v);
+      else store_decoded<K>(out, j, v);
     }
   }
   return st;
@@ -498,10 +527,10 @@ __device__ __forceinline__ void vdec_emit_tile(const VarTables& tb, uint32_t t, 
   VarSeg sg;
   VarJobDev jb;
   fetch_tile(tb, t, sg, jb);
-  // element count != prod(shape): reshape() would raise.  The tile still looks for malformed varints (nothing is stored): the
-  // runtime refuses such a message before any reshape, so B200TFS_E_PARSE must win over B200TFS_E_SHAPE (atomicMin does)
+  // element count != prod(shape): reshape() would raise.  The tile still looks for malformed varints and out-of-range values
+  // (nothing is stored): both are refused before any reshape (var_status_raise)
   const bool count_ok = (jb.flags & kVarFlagPadEdge) ? *jb.total <= jb.n_elems : *jb.total == jb.n_elems;
-  if (!count_ok && threadIdx.x == 0) atomicMin(jb.status, B200TFS_E_SHAPE);
+  if (!count_ok && threadIdx.x == 0) var_status_raise(jb.status, B200TFS_E_SHAPE);
   const uint64_t n_store = count_ok ? jb.n_elems : 0;
   const uint64_t share = prefix_share(jb, t - jb.first_tile);
   const uint8_t* lo = sg.src;
@@ -564,7 +593,7 @@ __device__ __forceinline__ void vdec_emit_tile(const VarTables& tb, uint32_t t, 
   // counts those ahead of the tile (+1 when a varint straddles in from the previous tile: it precedes ours but
   // its terminator is here).
   const uint64_t idx0 = before + (smraw[15] >> 7);
-  if (threadIdx.x == 0 && hi > G && hi <= G + kVarTileBytes && (hi[-1] & 0x80)) atomicMin(jb.status, B200TFS_E_PARSE);   // the chunk's last varint never ends
+  if (threadIdx.x == 0 && hi > G && hi <= G + kVarTileBytes && (hi[-1] & 0x80)) var_status_raise(jb.status, B200TFS_E_PARSE);   // the chunk's last varint never ends
   int32_t st_local;
   const uint32_t job = sg.job;
   switch (jb.dtype) {
@@ -581,7 +610,7 @@ __device__ __forceinline__ void vdec_emit_tile(const VarTables& tb, uint32_t t, 
       break;
     default: st_local = B200TFS_OK; break;
   }
-  if (st_local != B200TFS_OK) atomicMin(jb.status, st_local);
+  if (st_local != B200TFS_OK) var_status_raise(jb.status, st_local);
 }
 __global__ void __launch_bounds__(kVarThreads) vdec_emit_kernel(const __grid_constant__ VarTables tb) { vdec_emit_tile(tb, blockIdx.x); }
 // the same over tables vdec_plan_kernel built (grid-stride loop; the barrier keeps the next tile's staging behind this one's reads)

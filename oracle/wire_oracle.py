@@ -167,6 +167,7 @@ def build_predict_response(outputs, model_name="default", version=1, signature="
 
 
 _EXC = {E_SHAPE: ValueError, E_KEY: KeyError, E_RANK0: TypeError, E_RANGE: OverflowError, E_DTYPE: ValueError}
+_RANGE_CHECKED = (4, 5, 6, 17)     # DT_UINT8, DT_INT16, DT_INT8, DT_UINT16: int_val values narrowed by np.array(values, dtype)
 
 
 class ParseError(Exception):
@@ -203,6 +204,13 @@ def _materialise(handle, i, d: _Desc, wire: bytes, half_mode: int, tolerant: boo
                     raise _EXC.get(rc, ValueError)(f"oracle status {rc}")
                 flat[have:] = flat[have - 1]
             return flat.reshape(shape)
+    if status == E_SHAPE and d.dtype in _RANGE_CHECKED:
+        # np.array(values, dtype) refuses an out-of-range value before reshape() refuses the element count
+        have = int(lib().orc_value_count(handle, i))
+        if have > 0:
+            scratch = np.empty(have, dtype=_np_dtype(d.dtype))
+            if lib().orc_write_output(handle, i, half_mode, scratch.ctypes.data) == E_RANGE:
+                raise OverflowError(f"oracle status {E_RANGE}")
     if status != OK:
         raise _EXC.get(status, ValueError)(f"oracle status {status}")
     shape = tuple(d.dims[k] for k in range(d.rank))

@@ -14,7 +14,7 @@ import decode_mutants as D
 from devutil import Dev
 from min_tfs_client import _native as N
 from min_tfs_client.codec import Codec
-from oracle import wire_oracle
+from oracle import ref_port, wire_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -529,6 +529,11 @@ def test_python_errors_are_unchanged(strict):
         response(output("x", 6, [3], [packed([1, 2, 300])])),                # out of range: OverflowError
         response(output("x", 3, [3], [], unpacked=[5, 6, 7])),               # rows of unpacked elements
         response(output("x", 19, [2], [packed([18688, 1])])),                # DT_HALF: values (strict) or bits
+        # more than one error in one output: DecodeError before OverflowError before ValueError
+        response(output("x", 6, [2], [packed([1]) + b"\xac\x82" + b"\x80" * 8 + b"\x00"])),   # 11-byte varint reading 300
+        response(output("x", 6, [4], [packed([1, 2, 300])])),                # out of range and too few values
+        response(output("x", 5, [7], [packed([1, 40000]) + b"\xff" * 10 + b"\x01"])),   # all three
+        response(output("x", 4, [3], [packed([256]), packed([1])])),          # out of range in one chunk, count wrong
     ]
     warm = _classify(np.random.default_rng(6), 1)
 
@@ -541,12 +546,20 @@ def test_python_errors_are_unchanged(strict):
         except (DecodeError, ValueError, OverflowError, KeyError, TypeError, NotImplementedError) as e:
             return ("raise", type(e).__name__)
 
+    def reference(w):
+        try:
+            return ("ok", {k: (v.dtype.str, v.shape, v.tobytes()) for k, v in ref_port.decode_predict_response(w).items()})
+        except (DecodeError, ValueError, OverflowError) as e:
+            return ("raise", type(e).__name__)
+
     fresh, warmed = Codec(0), Codec(0)
     try:
         warmed.decode_predict_responses(warm)
         assert warmed._seen_varints and not fresh._seen_varints
         for w in bad:
             assert outcome(warmed, w) == outcome(fresh, w), w
+            if strict:
+                assert outcome(fresh, w) == reference(w), w
     finally:
         fresh.close()
         warmed.close()
