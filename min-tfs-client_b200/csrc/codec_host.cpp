@@ -140,9 +140,9 @@ struct b200tfs_ctx {
     uint8_t* dst[B200TFS_CONCAT_MAX_KEYS] = {};
     uint64_t vouts = 0, vstat = 0, specs = 0, status = 0;
   };
-  Growable concat_dev;                  // b200tfs_decode_concat: parse table, plan image, varint tables (ConcatLayout)
+  Growable concat_dev;                  // b200tfs_decode_concat: parse table, varint tables, plan image (KeyLayout)
   KeyResults concat_res;
-  Growable padded_dev;                  // b200tfs_decode_padded: parse table, descriptors, varint tables (PaddedLayout)
+  Growable padded_dev;                  // b200tfs_decode_padded: parse table, varint tables, descriptors (KeyLayout)
   KeyResults padded_res;
   Growable xr_dev;                      // b200tfs_decode_example_responses: entry slots and per-response tables (XrLayout)
   Growable xr_host;                     // ... and the results its publish kernel leaves in pinned memory (XrResultsLayout)
@@ -2317,13 +2317,14 @@ int b200tfs_padded_layout(const void* wire_host, int32_t n, const uint64_t* rec_
 }
 
 namespace {
-// device scratch of b200tfs_decode_concat for n records, n_keys keys, tile_cap move tiles and var_tile_cap varint tiles
-struct ConcatLayout { uint64_t outs, nouts, specs, status, spill, kst, match, plan, plan_tiles, vouts, vnouts, vstatus, var, var_status, bytes; };
-ConcatLayout concat_layout(uint64_t n, uint64_t n_keys, uint64_t tile_cap, uint64_t var_tile_cap) {
-  const PlanGeometry g = plan_geometry(n * n_keys * B200TFS_MAX_RUNS, tile_cap, 0);   // concat_plan_kernel's plan image
+// device scratch of a per-key decode (b200tfs_decode_concat, b200tfs_decode_padded) for n records, n_keys keys and var_tile_cap
+// varint tiles: the parse table, the keys' verdicts and matches, the varint tail's table and scratch, then the route's own
+// regions of `sizes` bytes (own[i])
+struct KeyLayout { uint64_t outs, nouts, specs, status, spill, kst, match, vouts, vnouts, vstatus, var, var_status, own[3], bytes; };
+KeyLayout key_scratch(uint64_t n, uint64_t n_keys, uint64_t var_tile_cap, std::initializer_list<uint64_t> sizes) {
   const VarPlanLayout V = var_plan_layout(n, var_tile_cap);
   Layout R;
-  ConcatLayout L;
+  KeyLayout L{};
   L.outs = R.take(sizeof(b200tfs_output) * n * (kFusedMaxOutputs + 1), 256);
   L.nouts = R.take(4 * n, 256);
   L.specs = R.take(sizeof(b200tfs_model_spec) * n, 256);
@@ -2331,55 +2332,71 @@ ConcatLayout concat_layout(uint64_t n, uint64_t n_keys, uint64_t tile_cap, uint6
   L.spill = R.take(4 * n, 256);
   L.kst = R.take(4 * n * n_keys, 256);
   L.match = R.take(4 * n * n_keys, 256);
-  L.plan = R.take(g.end, 256);
-  L.plan_tiles = g.off_tiles;
   L.vouts = R.take(sizeof(b200tfs_output) * n * kFusedMaxOutputs, 256);
   L.vnouts = R.take(4 * n, 256);
   L.vstatus = R.take(4 * n, 256);
   L.var = R.take(V.bytes, 256);
   L.var_status = L.var + V.status;
+  uint64_t* own = L.own;
+  for (uint64_t b : sizes) *own++ = R.take(b, 256);
   L.bytes = R.end;
   return L;
 }
 }  // namespace
 
-int b200tfs_decode_concat(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
-                          int32_t n_keys, const b200tfs_concat_key* keys) {
+extern "C++" {
+// The start of a per-key decode: the argument checks (`check(key, k)`: the route's own checks of key k, after the shared ones),
+// the device, and the varint tail's tile bound
+template <class Key, class Check>
+static int key_begin(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
+                     const Key* keys, uint64_t* var_tile_cap, Check&& check) {
   if (!c || n <= 0 || !arena_dev || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
   int rc = concat_check_keys(n_keys, keys);
   if (rc) return rc;
-  for (int k = 0; k < n_keys; ++k) if (keys[k].dst_cap && !keys[k].dst) return fail(B200TFS_E_ARG, "key %d: dst is NULL", k);
-  if (!c->capturing) CU(cudaSetDevice(c->device));
-  uint64_t wire_total = 0, tile_cap = 0, var_tile_cap = 0;
-  for (int i = 0; i < n; ++i) wire_total += rec_len[i];
-  const uint32_t vpt = pick_vec_per_tile(c, c->decode_cast ? wire_total / 2 : wire_total, 65536);
-  for (int i = 0; i < n; ++i) {
-    tile_cap += concat_record_tile_bound(rec_len[i], 16ull * vpt, (uint32_t)n_keys);
-    var_tile_cap += var_record_tile_bound(rec_len[i]);
+  for (int k = 0; k < n_keys; ++k) {
+    if (keys[k].dst_cap && !keys[k].dst) return fail(B200TFS_E_ARG, "key %d: dst is NULL", k);
+    if ((rc = check(keys[k], k))) return rc;
   }
-  if (tile_cap > 0x7FFFFFFFull || var_tile_cap > 0x7FFFFFFFull) return fail(B200TFS_E_TOOBIG, "batch needs more than 2^31 tiles");
-  const ConcatLayout L = concat_layout((uint64_t)n, (uint64_t)n_keys, tile_cap, var_tile_cap);
-  if (L.plan_tiles > 0xFFFFFFFFull) return fail(B200TFS_E_TOOBIG, "plan image larger than 4 GiB");
-  if ((rc = grow_dev(c, c->concat_dev, L.bytes))) return rc;
+  if (!c->capturing) CU(cudaSetDevice(c->device));
+  uint64_t tiles = 0;
+  for (int i = 0; i < n; ++i) tiles += var_record_tile_bound(rec_len[i]);
+  if (tiles > 0x7FFFFFFFull) return fail(B200TFS_E_TOOBIG, "batch needs more than 2^31 tiles");
+  *var_tile_cap = tiles;
+  return B200TFS_OK;
+}
+
+// A per-key decode on c->stream, around the route's plan: its scratch in `g` (KeyLayout, with the route's regions `own`), one
+// upload of rec_off | rec_len | key records (`dev_key(key, its bytes on the device)`) | key bytes, the parse kernel and the
+// ConcatPlan fields both routes use.  `plan(cp, scratch, layout, device key records, &pad)` launches the route's kernels, which
+// write the single-launch decode's table with absolute dst_off, and may set `pad`, the placement of the varint emit.  Then the
+// varint tail over that table, and `res` becomes this call's.
+template <class Key, class DevKey, class Plan>
+static int key_decode(b200tfs_ctx* c, Growable& g, b200tfs_ctx::KeyResults& res, const void* arena_dev, int32_t n, const uint64_t* rec_off,
+                      const uint64_t* rec_len, int32_t n_keys, const Key* keys, uint64_t var_tile_cap, std::initializer_list<uint64_t> own,
+                      DevKey&& dev_key, Plan&& plan) {
+  using KeyRec = decltype(dev_key(keys[0], (const uint8_t*)nullptr));
+  const KeyLayout L = key_scratch((uint64_t)n, (uint64_t)n_keys, var_tile_cap, own);
+  int rc = grow_dev(c, g, L.bytes);
+  if (rc) return rc;
   // rec_off | rec_len | keys | key bytes: one upload (a captured call keeps a private copy)
   uint64_t key_bytes = 0;
   for (int k = 0; k < n_keys; ++k) key_bytes += (uint64_t)keys[k].key_len;
   Layout K;
-  const uint64_t o_off = K.take(8ull * n), o_len = K.take(8ull * n), o_keys = K.take(sizeof(ConcatKeyDev) * n_keys), o_kb = K.take(key_bytes);
+  const uint64_t o_off = K.take(8ull * n), o_len = K.take(8ull * n), o_keys = K.take(sizeof(KeyRec) * n_keys), o_kb = K.take(key_bytes);
   Slot* slot;
   uint8_t* sd;
   rc = upload_image(c, K.end, {{o_off, rec_off, 8ull * n}, {o_len, rec_len, 8ull * n}}, &sd, &slot, [&](uint8_t* h, uint8_t* dev) {
     uint64_t at = o_kb;
     for (int k = 0; k < n_keys; ++k) {
-      ConcatKeyDev kd{dev + at, (uint8_t*)keys[k].dst, keys[k].dst_cap, (uint32_t)keys[k].key_len, 0u};
-      memcpy(h + o_keys + sizeof(ConcatKeyDev) * k, &kd, sizeof kd);
+      const KeyRec kd = dev_key(keys[k], dev + at);
+      memcpy(h + o_keys + sizeof(KeyRec) * k, &kd, sizeof kd);
       if (keys[k].key_len) memcpy(h + at, keys[k].key, (size_t)keys[k].key_len);
       at += (uint64_t)keys[k].key_len;
     }
   });
   if (rc) return rc;
-  for (int k = 0; k < n_keys; ++k) c->concat_res.dst[k] = (uint8_t*)keys[k].dst;
-  uint8_t* d = (uint8_t*)c->concat_dev.p;
+  for (int k = 0; k < n_keys; ++k) res.dst[k] = (uint8_t*)keys[k].dst;
+  uint8_t* d = (uint8_t*)g.p;
   const uint64_t* off_dev = (const uint64_t*)(sd + o_off);
   CU(launch_parse_responses((const uint8_t*)arena_dev, off_dev, (const uint64_t*)(sd + o_len), n, kFusedMaxOutputs, (b200tfs_output*)(d + L.outs),
                             (int32_t*)(d + L.nouts), (b200tfs_model_spec*)(d + L.specs), (int32_t*)(d + L.status), nullptr, 0u,
@@ -2387,35 +2404,61 @@ int b200tfs_decode_concat(b200tfs_ctx* c, const void* arena_dev, int32_t n, cons
   ConcatPlan cp{};
   cp.w = (const uint8_t*)arena_dev; cp.rec_off = off_dev; cp.outs = (const b200tfs_output*)(d + L.outs);
   cp.n_outs = (const int32_t*)(d + L.nouts); cp.rec_status = (const int32_t*)(d + L.status);
-  cp.keys = (const ConcatKeyDev*)(sd + o_keys);
   cp.n = (uint32_t)n; cp.n_keys = (uint32_t)n_keys; cp.out_stride = kFusedMaxOutputs + 1; cp.cast = c->decode_cast;
-  cp.vpt = vpt; cp.tile_cap = (uint32_t)tile_cap;
-  cp.kst = (int32_t*)(d + L.kst); cp.match = (int32_t*)(d + L.match); cp.plan = d + L.plan;
+  cp.kst = (int32_t*)(d + L.kst); cp.match = (int32_t*)(d + L.match);
   cp.vouts = (b200tfs_output*)(d + L.vouts); cp.vn_outs = (int32_t*)(d + L.vnouts); cp.vrec_status = (int32_t*)(d + L.vstatus);
-  CU(launch_concat_plan(cp, (uint32_t)tile_cap, c->stream));
-  // packed-varint outputs: the single-launch decode's plan / count / emit over the table the plan kernel wrote (its dst_off is
-  // the absolute address: dst 0, stride 0)
+  const VarPadMap* pad = nullptr;
+  if ((rc = plan(cp, d, L, sd + o_keys, &pad))) return rc;
+  // packed-varint outputs: the single-launch decode's plan / count / emit over the table the plan kernel wrote (dst 0, stride 0)
   VarPlan vp{};
   vp.outs = cp.vouts; vp.n_outs = cp.vn_outs; vp.rec_status = cp.vrec_status;
   vp.w = cp.w; vp.rec_off = off_dev;
   vp.dst = nullptr; vp.dst_stride = 0; vp.n = (uint32_t)n; vp.tile_cap = (uint32_t)var_tile_cap;
-  if ((rc = launch_varint_tail(c, vp, d + L.var, rec_off))) return rc;
+  if ((rc = launch_varint_tail(c, vp, d + L.var, rec_off, pad))) return rc;
   if (slot->done && !c->capturing) { CU(cudaEventRecord(slot->done, c->stream)); slot->pending = true; }   // the kernels read the upload
   c->launches += 3;
-  c->concat_res.n = n; c->concat_res.k = n_keys;
-  c->concat_res.vouts = L.vouts; c->concat_res.vstat = L.var_status; c->concat_res.specs = L.specs; c->concat_res.status = L.status;
+  res.n = n; res.k = n_keys;
+  res.vouts = L.vouts; res.vstat = L.var_status; res.specs = L.specs; res.status = L.status;
   return B200TFS_OK;
 }
 
-int b200tfs_decode_concat_host_async(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
-                                     int32_t n_keys, const b200tfs_concat_key* keys) {
+// b200tfs_decode_concat_host_async / b200tfs_decode_padded_host_async: the wire staged on the device, then `decode` (`name`)
+template <class Key>
+static int key_decode_host_async(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                                 int32_t n_keys, const Key* keys, const char* name,
+                                 int (*decode)(b200tfs_ctx*, const void*, int32_t, const uint64_t*, const uint64_t*, int32_t, const Key*)) {
   if (!c || n <= 0 || !wire_host || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
-  if (c->capturing) return fail(B200TFS_E_ARG, "capture b200tfs_decode_concat over a device arena instead");
+  if (c->capturing) return fail(B200TFS_E_ARG, "capture %s over a device arena instead", name);
   CU(cudaSetDevice(c->device));
   uint64_t span;
   int rc = stage_wire(c, wire_host, n, rec_off, rec_len, &span);
   if (rc) return rc;
-  return b200tfs_decode_concat(c, c->stage_dev.p, n, rec_off, rec_len, n_keys, keys);
+  return decode(c, c->stage_dev.p, n, rec_off, rec_len, n_keys, keys);
+}
+}  // extern "C++"
+
+int b200tfs_decode_concat(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                          int32_t n_keys, const b200tfs_concat_key* keys) {
+  uint64_t var_tile_cap = 0, tile_cap = 0;
+  int rc = key_begin(c, arena_dev, n, rec_off, rec_len, n_keys, keys, &var_tile_cap, [](const b200tfs_concat_key&, int) { return 0; });
+  if (rc) return rc;
+  const uint32_t vpt = decode_vpt(c, n, rec_len);
+  for (int i = 0; i < n; ++i) tile_cap += concat_record_tile_bound(rec_len[i], 16ull * vpt, (uint32_t)n_keys);
+  if (tile_cap > 0x7FFFFFFFull) return fail(B200TFS_E_TOOBIG, "batch needs more than 2^31 tiles");
+  const PlanGeometry g = plan_geometry((uint64_t)n * (uint64_t)n_keys * B200TFS_MAX_RUNS, tile_cap, 0);   // concat_plan_kernel's plan image
+  if (g.off_tiles > 0xFFFFFFFFull) return fail(B200TFS_E_TOOBIG, "plan image larger than 4 GiB");
+  return key_decode(c, c->concat_dev, c->concat_res, arena_dev, n, rec_off, rec_len, n_keys, keys, var_tile_cap, {g.end},
+                    [](const b200tfs_concat_key& k, const uint8_t* kb) { return ConcatKeyDev{kb, (uint8_t*)k.dst, k.dst_cap, (uint32_t)k.key_len, 0u}; },
+                    [&](ConcatPlan& cp, uint8_t* d, const KeyLayout& L, const uint8_t* kd, const VarPadMap**) -> int {
+                      cp.keys = (const ConcatKeyDev*)kd; cp.vpt = vpt; cp.tile_cap = (uint32_t)tile_cap; cp.plan = d + L.own[0];
+                      CU(launch_concat_plan(cp, (uint32_t)tile_cap, c->stream));
+                      return B200TFS_OK;
+                    });
+}
+
+int b200tfs_decode_concat_host_async(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                                     int32_t n_keys, const b200tfs_concat_key* keys) {
+  return key_decode_host_async(c, wire_host, n, rec_off, rec_len, n_keys, keys, "b200tfs_decode_concat", b200tfs_decode_concat);
 }
 
 // The results of a per-key decode (`R` of its most recent call, its scratch at `base`), as b200tfs_concat_results describes them
@@ -2457,42 +2500,10 @@ int b200tfs_concat_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_ou
 // ------------------------------------------------------------------------------------------------
 // decode into one padded tensor per key
 // ------------------------------------------------------------------------------------------------
-namespace {
-// device scratch of b200tfs_decode_padded for n records, n_keys keys and var_tile_cap varint tiles
-struct PaddedLayout { uint64_t outs, nouts, specs, status, spill, kst, match, desc, first_row, kout, vouts, vnouts, vstatus, var, var_status, bytes; };
-PaddedLayout padded_layout(uint64_t n, uint64_t n_keys, uint64_t var_tile_cap) {
-  const VarPlanLayout V = var_plan_layout(n, var_tile_cap);
-  Layout R;
-  PaddedLayout L;
-  L.outs = R.take(sizeof(b200tfs_output) * n * (kFusedMaxOutputs + 1), 256);
-  L.nouts = R.take(4 * n, 256);
-  L.specs = R.take(sizeof(b200tfs_model_spec) * n, 256);
-  L.status = R.take(4 * n, 256);
-  L.spill = R.take(4 * n, 256);
-  L.kst = R.take(4 * n * n_keys, 256);
-  L.match = R.take(4 * n * n_keys, 256);
-  L.desc = R.take(sizeof(PadDesc) * n * n_keys, 256);
-  L.first_row = R.take(8 * n * n_keys, 256);
-  L.kout = R.take(sizeof(PadKeyOut) * (n_keys + 1), 256);
-  L.vouts = R.take(sizeof(b200tfs_output) * n * kFusedMaxOutputs, 256);
-  L.vnouts = R.take(4 * n, 256);
-  L.vstatus = R.take(4 * n, 256);
-  L.var = R.take(V.bytes, 256);
-  L.var_status = L.var + V.status;
-  L.bytes = R.end;
-  return L;
-}
-}  // namespace
-
 int b200tfs_decode_padded(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
                           int32_t n_keys, const b200tfs_pad_key* keys) {
-  if (!c || n <= 0 || !arena_dev || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
-  int rc = concat_check_keys(n_keys, keys);
-  if (rc) return rc;
-  uint64_t chunk_bound = 0;
-  for (int k = 0; k < n_keys; ++k) {
-    const b200tfs_pad_key& K = keys[k];
-    if (K.dst_cap && !K.dst) return fail(B200TFS_E_ARG, "key %d: dst is NULL", k);
+  uint64_t var_tile_cap = 0, chunk_bound = 0;
+  int rc = key_begin(c, arena_dev, n, rec_off, rec_len, n_keys, keys, &var_tile_cap, [&](const b200tfs_pad_key& K, int k) -> int {
     if ((uintptr_t)K.dst & 15) return fail(B200TFS_E_ARG, "key %d: dst is not 16-byte aligned", k);
     if (K.rank < 1 || K.rank > B200TFS_MAX_RANK) return fail(B200TFS_E_ARG, "key %d: rank %d", k, K.rank);
     uint64_t row = 1;
@@ -2501,74 +2512,38 @@ int b200tfs_decode_padded(b200tfs_ctx* c, const void* arena_dev, int32_t n, cons
       row *= (uint64_t)K.dims[d];
     }
     chunk_bound += (K.dst_cap + kPadChunkBytes - 1) / kPadChunkBytes;
-  }
-  if (!c->capturing) CU(cudaSetDevice(c->device));
-  uint64_t var_tile_cap = 0;
-  for (int i = 0; i < n; ++i) var_tile_cap += var_record_tile_bound(rec_len[i]);
-  if (var_tile_cap > 0x7FFFFFFFull) return fail(B200TFS_E_TOOBIG, "batch needs more than 2^31 tiles");
-  const PaddedLayout L = padded_layout((uint64_t)n, (uint64_t)n_keys, var_tile_cap);
-  if ((rc = grow_dev(c, c->padded_dev, L.bytes))) return rc;
-  // rec_off | rec_len | keys | key bytes: one upload (a captured call keeps a private copy)
-  uint64_t key_bytes = 0;
-  for (int k = 0; k < n_keys; ++k) key_bytes += (uint64_t)keys[k].key_len;
-  Layout K;
-  const uint64_t o_off = K.take(8ull * n), o_len = K.take(8ull * n), o_keys = K.take(sizeof(PadKeyDev) * n_keys), o_kb = K.take(key_bytes);
-  Slot* slot;
-  uint8_t* sd;
-  rc = upload_image(c, K.end, {{o_off, rec_off, 8ull * n}, {o_len, rec_len, 8ull * n}}, &sd, &slot, [&](uint8_t* h, uint8_t* dev) {
-    uint64_t at = o_kb;
-    for (int k = 0; k < n_keys; ++k) {
-      PadKeyDev kd{};
-      kd.k = ConcatKeyDev{dev + at, (uint8_t*)keys[k].dst, keys[k].dst_cap, (uint32_t)keys[k].key_len, 0u};
-      for (int d = 0; d < B200TFS_MAX_RANK; ++d) kd.dims[d] = keys[k].dims[d];
-      memcpy(kd.pad, keys[k].pad_bits, 16);
-      kd.rank = keys[k].rank;
-      memcpy(h + o_keys + sizeof(PadKeyDev) * k, &kd, sizeof kd);
-      if (keys[k].key_len) memcpy(h + at, keys[k].key, (size_t)keys[k].key_len);
-      at += (uint64_t)keys[k].key_len;
-    }
+    return B200TFS_OK;
   });
   if (rc) return rc;
-  for (int k = 0; k < n_keys; ++k) c->padded_res.dst[k] = (uint8_t*)keys[k].dst;
-  uint8_t* d = (uint8_t*)c->padded_dev.p;
-  const uint64_t* off_dev = (const uint64_t*)(sd + o_off);
-  CU(launch_parse_responses((const uint8_t*)arena_dev, off_dev, (const uint64_t*)(sd + o_len), n, kFusedMaxOutputs, (b200tfs_output*)(d + L.outs),
-                            (int32_t*)(d + L.nouts), (b200tfs_model_spec*)(d + L.specs), (int32_t*)(d + L.status), nullptr, 0u,
-                            (uint32_t*)(d + L.spill), c->stream));
-  PaddedPlan pp{};
-  ConcatPlan& cp = pp.cp;
-  cp.w = (const uint8_t*)arena_dev; cp.rec_off = off_dev; cp.outs = (const b200tfs_output*)(d + L.outs);
-  cp.n_outs = (const int32_t*)(d + L.nouts); cp.rec_status = (const int32_t*)(d + L.status);
-  cp.n = (uint32_t)n; cp.n_keys = (uint32_t)n_keys; cp.out_stride = kFusedMaxOutputs + 1; cp.cast = c->decode_cast;
-  cp.kst = (int32_t*)(d + L.kst); cp.match = (int32_t*)(d + L.match);
-  cp.vouts = (b200tfs_output*)(d + L.vouts); cp.vn_outs = (int32_t*)(d + L.vnouts); cp.vrec_status = (int32_t*)(d + L.vstatus);
-  pp.keys = (const PadKeyDev*)(sd + o_keys);
-  pp.desc = (PadDesc*)(d + L.desc); pp.first_row = (uint64_t*)(d + L.first_row); pp.kout = (PadKeyOut*)(d + L.kout);
-  const uint32_t emit_grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(chunk_bound, (uint64_t)c->sm_count * 8));
-  CU(launch_padded(pp, emit_grid, c->stream));
-  // packed-varint outputs: the single-launch decode's plan / count, and an emit that stores every element at its padded position
-  VarPlan vp{};
-  vp.outs = cp.vouts; vp.n_outs = cp.vn_outs; vp.rec_status = cp.vrec_status;
-  vp.w = cp.w; vp.rec_off = off_dev;
-  vp.dst = nullptr; vp.dst_stride = 0; vp.n = (uint32_t)n; vp.tile_cap = (uint32_t)var_tile_cap;
-  const VarPadMap pm{pp.desc, pp.keys, (uint32_t)n_keys, 0u};
-  if ((rc = launch_varint_tail(c, vp, d + L.var, rec_off, &pm))) return rc;
-  if (slot->done && !c->capturing) { CU(cudaEventRecord(slot->done, c->stream)); slot->pending = true; }   // the kernels read the upload
-  c->launches += 3;
-  c->padded_res.n = n; c->padded_res.k = n_keys;
-  c->padded_res.vouts = L.vouts; c->padded_res.vstat = L.var_status; c->padded_res.specs = L.specs; c->padded_res.status = L.status;
-  return B200TFS_OK;
+  const uint64_t pairs = (uint64_t)n * (uint64_t)n_keys;
+  VarPadMap pm{};
+  return key_decode(c, c->padded_dev, c->padded_res, arena_dev, n, rec_off, rec_len, n_keys, keys, var_tile_cap,
+                    {sizeof(PadDesc) * pairs, 8 * pairs, sizeof(PadKeyOut) * (n_keys + 1)},
+                    [](const b200tfs_pad_key& k, const uint8_t* kb) {
+                      PadKeyDev kd{};
+                      kd.k = ConcatKeyDev{kb, (uint8_t*)k.dst, k.dst_cap, (uint32_t)k.key_len, 0u};
+                      for (int d = 0; d < B200TFS_MAX_RANK; ++d) kd.dims[d] = k.dims[d];
+                      memcpy(kd.pad, k.pad_bits, 16);
+                      kd.rank = k.rank;
+                      return kd;
+                    },
+                    [&](ConcatPlan& cp, uint8_t* d, const KeyLayout& L, const uint8_t* kd, const VarPadMap** pad) -> int {
+                      PaddedPlan pp{};
+                      pp.cp = cp;
+                      pp.keys = (const PadKeyDev*)kd;
+                      pp.desc = (PadDesc*)(d + L.own[0]); pp.first_row = (uint64_t*)(d + L.own[1]); pp.kout = (PadKeyOut*)(d + L.own[2]);
+                      const uint32_t emit_grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(chunk_bound, (uint64_t)c->sm_count * 8));
+                      CU(launch_padded(pp, emit_grid, c->stream));
+                      // the varint emit stores every element at its padded position
+                      pm = VarPadMap{pp.desc, pp.keys, (uint32_t)n_keys, 0u};
+                      *pad = &pm;
+                      return B200TFS_OK;
+                    });
 }
 
 int b200tfs_decode_padded_host_async(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
                                      int32_t n_keys, const b200tfs_pad_key* keys) {
-  if (!c || n <= 0 || !wire_host || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
-  if (c->capturing) return fail(B200TFS_E_ARG, "capture b200tfs_decode_padded over a device arena instead");
-  CU(cudaSetDevice(c->device));
-  uint64_t span;
-  int rc = stage_wire(c, wire_host, n, rec_off, rec_len, &span);
-  if (rc) return rc;
-  return b200tfs_decode_padded(c, c->stage_dev.p, n, rec_off, rec_len, n_keys, keys);
+  return key_decode_host_async(c, wire_host, n, rec_off, rec_len, n_keys, keys, "b200tfs_decode_padded", b200tfs_decode_padded);
 }
 
 int b200tfs_padded_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs, int32_t* rec_status) {

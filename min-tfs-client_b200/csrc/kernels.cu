@@ -1103,6 +1103,18 @@ __device__ __forceinline__ void plan_match_key(const ConcatPlan& cp, const uint8
   }
 }
 
+// pass A of key k, called by every thread of the CTA (`ref_rec`: shared scratch): the output of the first record that decoded the
+// key, the reference of pass B, or nullptr when no record did
+__device__ __forceinline__ const b200tfs_output* plan_key_reference(const ConcatPlan& cp, const uint8_t* kb, uint32_t key_len, uint32_t k,
+                                                                    uint32_t* ref_rec) {
+  if (threadIdx.x == 0) *ref_rec = cp.n;
+  __syncthreads();
+  plan_match_key(cp, kb, key_len, k, ref_rec);
+  __syncthreads();
+  const uint32_t rr = *ref_rec;
+  return rr < cp.n ? cp.outs + (size_t)rr * cp.out_stride + cp.match[(size_t)rr * cp.n_keys + k] : nullptr;
+}
+
 __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const __grid_constant__ ConcatPlan cp) {
   __shared__ unsigned long long warp_sum[kConcatPlanThreads / 32];
   __shared__ uint32_t ref_rec;
@@ -1114,12 +1126,7 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
   uint64_t tile_carry = 0;
   for (uint32_t k = 0; k < nk; ++k) {
     const ConcatKeyDev key = cp.keys[k];
-    if (threadIdx.x == 0) ref_rec = n;
-    __syncthreads();
-    plan_match_key(cp, key.key, key.key_len, k, &ref_rec);
-    __syncthreads();
-    const uint32_t rr = ref_rec;
-    const b200tfs_output* ro = rr < n ? cp.outs + (size_t)rr * cp.out_stride + cp.match[(size_t)rr * nk + k] : nullptr;
+    const b200tfs_output* ro = plan_key_reference(cp, key.key, key.key_len, k, &ref_rec);
     // pass B: consistency, offsets, tiles, items
     uint64_t byte_carry = 0;
     for (uint32_t r0 = 0; r0 < n; r0 += kConcatPlanThreads) {      // uniform trip count: the scans have barriers inside

@@ -1,7 +1,7 @@
 // padded_kernels.cuh - b200tfs_decode_padded: a batch of PredictResponses into one padded tensor per requested key (plan.h
 // PaddedPlan; the host side is in codec_host.cpp).  Included by kernels.cu inside namespace b200tfs, after concat_plan_kernel.
 //
-//   padded_plan_kernel  one CTA.  Per key: concat_plan_kernel's pass A (plan_match_key), then every record against the first
+//   padded_plan_kernel  one CTA.  Per key: concat_plan_kernel's pass A (plan_key_reference), then every record against the first
 //                       record that decoded the key (dtype, rank) and against the destination's trailing dims, a block scan of
 //                       dims[0] into first rows, one PadDesc per (record, key) and the single-launch decode's table for the
 //                       varint tail.  Nothing waits on another CTA: a replayed graph re-plans rows and trailing dims.
@@ -52,12 +52,8 @@ __global__ void __launch_bounds__(kConcatPlanThreads) padded_plan_kernel(const _
   uint64_t chunks = 0;
   for (uint32_t k = 0; k < nk; ++k) {
     const PadKeyDev& key = pp.keys[k];
-    if (threadIdx.x == 0) { ref_rec = n; first_over = ~0ull; }
-    __syncthreads();
-    plan_match_key(cp, key.k.key, key.k.key_len, k, &ref_rec);
-    __syncthreads();
-    const uint32_t rr = ref_rec;
-    const b200tfs_output* ro = rr < n ? cp.outs + (size_t)rr * cp.out_stride + cp.match[(size_t)rr * nk + k] : nullptr;
+    if (threadIdx.x == 0) first_over = ~0ull;
+    const b200tfs_output* ro = plan_key_reference(cp, key.k.key, key.k.key_len, k, &ref_rec);
     const int32_t dtype = ro ? ro->dtype : 0, rank = key.rank;
     const DtypeInfo di = dtype_info(dtype);
     const bool narrow = tpl_narrows(cp.cast, dtype), varint = di.kind == VK_VARINT || di.kind == VK_BOOL;

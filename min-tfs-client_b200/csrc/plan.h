@@ -255,9 +255,9 @@ constexpr uint64_t concat_record_tile_bound(uint64_t len, uint64_t tile_bytes, u
 }
 
 // ---- decode into one padded tensor per key (b200tfs_decode_padded) ----------------------------------------------------
-// padded_plan_kernel (one CTA) matches the keys with concat_plan_kernel's pass A, checks every record against the first one that
-// decoded the key and against the destination's trailing dims, scans the rows into first rows and writes one PadDesc per
-// (record, key), the per-key summary and the single-launch decode's table for the varint tail (as ConcatPlan::vouts).
+// padded_plan_kernel (one CTA) matches the keys as concat_plan_kernel does (plan_key_reference), checks every record against the
+// first one that decoded the key and against the destination's trailing dims, scans the rows into first rows and writes one
+// PadDesc per (record, key), the per-key summary and the single-launch decode's table for the varint tail (as ConcatPlan::vouts).
 // padded_emit_kernel then writes the destination in chunks of kPadChunkBytes, a grid-stride loop over the chunks of every key.
 constexpr uint32_t kPadEmitThreads = 256;
 constexpr uint32_t kPadEmitVecs = 4;                                  // 16-byte vectors per thread and chunk

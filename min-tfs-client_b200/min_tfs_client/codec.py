@@ -269,6 +269,10 @@ def _check_out(key, dst, dtype, shape, contiguous: bool = False):
 # record), each record's table ({key: Output}) and model_spec
 _Launch = collections.namedtuple("_Launch", "n buf off dst stride tables specs")
 
+# what a per-key device decode (Codec._key_device) left: its key structs, the wire on the device, the results table, each
+# response's status and DecodedSpec, and the destinations as Codec._key_deliver takes them (holds: their keep-alives)
+_KeyLaunch = collections.namedtuple("_KeyLaunch", "keys wire outs rec_status specs shapes np_types dev ptrs holds")
+
 
 class OpenResponse:
     """One PredictResponse after the fused launch: the table, and the host buffer the fixed-width outputs landed in."""
@@ -852,20 +856,20 @@ class Codec:
         key.  ``out={key: array}`` writes in place: a C-contiguous device array (CUDA array interface / DLPack) or a numpy /
         ``pinned_empty`` array of exactly the result's dtype and shape.  Returns ``({key: tensor}, [DecodedSpec per response])``.
         """
-        n = len(wires)
-        if n == 0:
-            raise ValueError("need at least one response to concatenate")
-        out = dict(out or {})
-        buf, off, ln = self._pack_wires(wires)
-        keys, out_dtypes = self._requested(wires, buf, off, ln, keys, out, out_dtypes)
-        fast = self._concat_device(wires, buf, off, ln, keys, strict, out_dtypes, device, out) if len(keys) <= N.CONCAT_MAX_KEYS else None
+        buf, off, ln, keys, out_dtypes, out = self._requested(wires, keys, out, out_dtypes, "need at least one response to concatenate")
+        fast = self._concat_device(wires, buf, off, ln, keys, strict, out_dtypes, device, out)
         if fast is not None:
             return fast
         return self._concat_per_record(wires, keys, strict, out_dtypes, device, out)
 
-    def _requested(self, wires, buf, off, ln, keys, out, out_dtypes):
-        """The requested keys of a per-key batch decode (None: every key of the first response), and out_dtypes restricted to
-        them.  KeyError for a key of `out` that is not requested."""
+    def _requested(self, wires, keys, out, out_dtypes, empty: str):
+        """The front of a per-key batch decode: the batch staged (_pack_wires), the requested keys (None: every key of the first
+        response), out_dtypes restricted to them and `out` as a dict.  ValueError(`empty`) for an empty batch, KeyError for a
+        key of `out` that is not requested."""
+        if len(wires) == 0:
+            raise ValueError(empty)
+        out = dict(out or {})
+        buf, off, ln = self._pack_wires(wires)
         if keys is None:
             keys = self._response_keys(buf, int(off[0]), int(ln[0]))
             if keys is None:      # the first response does not parse: the parse raises what the reference raises
@@ -879,7 +883,7 @@ class Codec:
                 raise KeyError(k)
         if out_dtypes:        # only the requested outputs are decoded: entries for other keys play no part
             out_dtypes = {k: v for k, v in out_dtypes.items() if k in keys} or None
-        return keys, out_dtypes
+        return buf, off, ln, keys, out_dtypes, out
 
     def _response_keys(self, buf, base: int, length: int) -> Optional[List[str]]:
         cap = 64
@@ -892,24 +896,32 @@ class Codec:
                 return [self._text(buf, base + int(ko[i]), int(kl[i])) for i in range(cnt.value)]
             cap = cnt.value
 
-    def _concat_per_record(self, wires, keys, strict, out_dtypes, device, out):
-        """The definition itself, response by response, for the requested outputs: what the device route hands over when a batch
+    def _per_record(self, wires, keys, strict, out_dtypes, device, out, bad_rank, combine):
+        """The definition itself, response by response, for the requested outputs: what a device route hands over when a batch
         holds a case it does not take (a malformed record, more than FUSED_MAX_OUTPUTS outputs or MAX_RANK dims, TF padding,
-        tensor_content only, strings, mismatches).  Like the device route it converts and checks the requested outputs only."""
+        tensor_content only, strings, mismatches).  Like the device routes it converts and checks the requested outputs only.
+        Per key, the route's rank rule (`bad_rank(key, parts)`: the ValueError's message, or None), one dtype, and the route's
+        tensor of the parts (`combine(key, parts)`)."""
         wanted = set(keys)
         per = [self._decode_two_phase([w], strict, out_dtypes, 16, wanted)[0] for w in wires]
         result = {}
-        for k in dict.fromkeys(keys):
+        for k in keys:
             parts = [p[0][k] for p in per]
-            if any(a.ndim == 0 for a in parts):
-                raise ValueError("zero-dimensional arrays cannot be concatenated")
+            msg = bad_rank(k, parts)
+            if msg:
+                raise ValueError(msg)
             if len({a.dtype for a in parts}) > 1:
                 raise ValueError(f"output {k!r}: responses disagree on the dtype ({', '.join(sorted({str(a.dtype) for a in parts}))})")
-            cat = np.concatenate(parts, axis=0)
-            if device and cat.dtype.kind in "US":
+            arr = combine(k, parts)
+            if device and arr.dtype.kind in "US":
                 raise TypeError(f"output {k!r}: string tensors are decoded on the host")
-            result[k] = self._concat_deliver(k, cat, device, out)
+            result[k] = self._concat_deliver(k, arr, device, out)
         return result, [p[1] for p in per]
+
+    def _concat_per_record(self, wires, keys, strict, out_dtypes, device, out):
+        return self._per_record(wires, keys, strict, out_dtypes, device, out,
+                                lambda k, parts: "zero-dimensional arrays cannot be concatenated" if any(a.ndim == 0 for a in parts) else None,
+                                lambda k, parts: np.concatenate(parts, axis=0))
 
     def _concat_deliver(self, key, arr: np.ndarray, device: bool, out):
         dst = out.get(key)
@@ -924,9 +936,15 @@ class Codec:
             self.sync()
         return dst
 
-    def _concat_device(self, wires, buf, off, ln, keys, strict, out_dtypes, device, out):
-        """The device route (b200tfs_decode_concat): parse, one-CTA plan, move, varint decode - or None when the batch holds
-        a case it leaves to the per-response route."""
+    def _key_device(self, native, wires, buf, off, ln, keys, strict, out_dtypes, out, shape_of, place) -> Optional["_KeyLaunch"]:
+        """A per-key device route up to the results of its decode, or None when the batch holds a case it leaves to the
+        per-response route.  `native`: the route's key struct and its layout, decode and results entry points.  The host layout
+        runs first, so nothing is written into `out` for a batch the route then refuses.  `shape_of(i, key struct, numpy type)`
+        is key i's result shape (None: refused); `place(key structs, pointers, shapes, numpy types)` completes the key structs
+        once the destinations are known (False: refused)."""
+        if len(keys) > N.CONCAT_MAX_KEYS:
+            return None
+        key_type, layout, decode, results = native
         n, nk = len(wires), len(keys)
         kb = [k.encode("utf-8") for k in keys]
         cast_code = 0
@@ -934,58 +952,75 @@ class Codec:
             cast_code = None if strict else _narrowing_cast(out_dtypes)
             if cast_code is None:
                 return None
-        ck = (N.ConcatKey * nk)()
+        ks = (key_type * nk)()
         for i, k in enumerate(kb):
-            ck[i].key, ck[i].key_len = k, len(k)
-        N.check(self._lib.b200tfs_concat_layout(buf.ctypes.data, n, off, ln, nk, ck, cast_code))
+            ks[i].key, ks[i].key_len = k, len(k)
+        N.check(layout(buf.ctypes.data, n, off, ln, nk, ks, cast_code))
         shapes, np_types = [], []
         for i in range(nk):
-            c = ck[i]
-            if c.status != N.OK or c.dtype == DT_STRING:
-                return None
-            if strict and (c.dtype == DT_BFLOAT16 or c.dtype in (DT_COMPLEX64, DT_COMPLEX128)):
+            c = ks[i]
+            if c.status != N.OK or c.dtype == DT_STRING or strict and c.dtype in (DT_BFLOAT16, DT_COMPLEX64, DT_COMPLEX128):
                 return None
             if cast_code and not _narrowing_fits(c.dtype, keys[i], out_dtypes):
                 return None
-            shapes.append(tuple(int(c.dims[d]) for d in range(c.rank)))
             np_types.append(np.dtype(numpy_for_enum(cast_code if cast_code and c.dtype == DT_FLOAT else int(c.dtype))))
+            shape = shape_of(i, c, np_types[i])
+            if shape is None:
+                return None
+            shapes.append(shape)
         dev, ptrs, holds = self._key_destinations(keys, out, shapes, np_types)
-        for i in range(nk):
-            ck[i].dst, ck[i].dst_cap = ptrs[i], int(ck[i].bytes)
+        if not place(ks, ptrs, shapes, np_types):
+            return None
         wire = D.DeviceArray(self, (len(buf),), np.uint8).copy_from_host(buf)
         with self._decode_modes(cast_code):
-            N.check(self._lib.b200tfs_decode_concat(self._ctx, wire.ptr, n, off, ln, nk, ck))
+            N.check(decode(self._ctx, wire.ptr, n, off, ln, nk, ks))
         outs, specs, rec_status = (N.Output * (n * nk))(), (N.ModelSpec * n)(), (C.c_int32 * n)()
-        N.check(self._lib.b200tfs_concat_results(self._ctx, n, nk, outs, specs, rec_status))   # synchronises
-        raw = np.frombuffer(outs, dtype=np.uint8).reshape(n * nk, C.sizeof(N.Output))
+        N.check(results(self._ctx, n, nk, outs, specs, rec_status))   # synchronises
+        return _KeyLaunch(ks, wire, outs, rec_status, [self._spec(buf, int(off[r]), specs[r]) for r in range(n)],
+                          shapes, np_types, dev, ptrs, holds)
+
+    def _concat_device(self, wires, buf, off, ln, keys, strict, out_dtypes, device, out):
+        """The device route (b200tfs_decode_concat): parse, one-CTA plan, move, varint decode - or None when the batch holds
+        a case it leaves to the per-response route."""
+        def place(ck, ptrs, shapes, np_types):
+            for i in range(len(keys)):
+                ck[i].dst, ck[i].dst_cap = ptrs[i], int(ck[i].bytes)
+            return True
+        f = self._key_device((N.ConcatKey, self._lib.b200tfs_concat_layout, self._lib.b200tfs_decode_concat, self._lib.b200tfs_concat_results),
+                             wires, buf, off, ln, keys, strict, out_dtypes, out,
+                             lambda i, c, np_type: tuple(int(c.dims[d]) for d in range(c.rank)), place)
+        if f is None:
+            return None
+        n, nk = len(wires), len(keys)
+        raw = np.frombuffer(f.outs, dtype=np.uint8).reshape(n * nk, C.sizeof(N.Output))
         status = raw[:, N.Output.status.offset: N.Output.status.offset + 4].copy().view(np.int32).ravel()
         redo = set(np.flatnonzero(status != N.OK).tolist())
         if strict:     # the reference reads half_val as VALUES; the device wrote TF's bit patterns
             for i in range(nk):
-                if ck[i].dtype == DT_HALF:
+                if f.keys[i].dtype == DT_HALF:
                     redo.update(r * nk + i for r in range(n))
         jobs = []
         for j in sorted(redo):
             r, i = divmod(j, nk)
-            o = outs[j]
-            if rec_status[r] != N.OK or not _to_unpack(o, N.E_NONCANONICAL):
+            o = f.outs[j]
+            if f.rec_status[r] != N.OK or not _to_unpack(o, N.E_NONCANONICAL):
                 return None
             _, dst_code, _ = self._resolve_output(o, strict, out_dtypes.get(keys[i]) if out_dtypes else None)
             if o.n_elems:
-                jobs.append((j, r, ptrs[i] + int(o.dst_off), dst_code))
+                jobs.append((j, r, f.ptrs[i] + int(o.dst_off), dst_code))
         if jobs:
             m = len(jobs)
-            o_arr = (N.Output * m)(*[outs[j[0]] for j in jobs])
+            o_arr = (N.Output * m)(*[f.outs[j[0]] for j in jobs])
             rec = (C.c_uint64 * m)(*[int(off[j[1]]) for j in jobs])
             dd = (C.c_void_p * m)(*[j[2] for j in jobs])
             codes = (C.c_int32 * m)(*[j[3] for j in jobs])
             st = (C.c_int32 * m)()
-            N.check(self._lib.b200tfs_unpack_outputs(self._ctx, wire.ptr, m, o_arr, rec, dd, codes, st))
+            N.check(self._lib.b200tfs_unpack_outputs(self._ctx, f.wire.ptr, m, o_arr, rec, dd, codes, st))
             if any(st[q] != N.OK for q in range(m)):
                 return None
-        result = self._key_deliver(keys, out, device, shapes, np_types, dev, ptrs)
+        result = self._key_deliver(keys, out, device, f.shapes, f.np_types, f.dev, f.ptrs)
         self.concat_device_calls += 1
-        return result, [self._spec(buf, int(off[r]), specs[r]) for r in range(n)]
+        return result, f.specs
 
     def _key_destinations(self, keys, out, shapes, np_types):
         """Device destinations of a per-key device decode: the caller's device arrays, else device arrays of our own (returned,
@@ -1041,33 +1076,24 @@ class Codec:
         gets the pad converted to the narrowed dtype).  Returns ``({key: tensor}, {key: int64[n, rank] shape of every response's
         output}, [DecodedSpec per response])``.
         """
-        n = len(wires)
-        if n == 0:
-            raise ValueError("need at least one response to pad")
-        out = dict(out or {})
-        buf, off, ln = self._pack_wires(wires)
-        keys, out_dtypes = self._requested(wires, buf, off, ln, keys, out, out_dtypes)
+        buf, off, ln, keys, out_dtypes, out = self._requested(wires, keys, out, out_dtypes, "need at least one response to pad")
         pad_to = dict(pad_to or {})
-        fast = self._padded_device(wires, buf, off, ln, keys, pad_value, pad_to, strict, out_dtypes, device, out) \
-            if len(keys) <= N.CONCAT_MAX_KEYS else None
+        fast = self._padded_device(wires, buf, off, ln, keys, pad_value, pad_to, strict, out_dtypes, device, out)
         if fast is not None:
             return fast
         return self._padded_per_record(wires, keys, pad_value, pad_to, strict, out_dtypes, device, out)
 
     def _padded_per_record(self, wires, keys, pad_value, pad_to, strict, out_dtypes, device, out):
-        """The definition itself, response by response and padded with numpy: what the device route hands over when a batch
-        holds a case it does not take (a malformed record, more than FUSED_MAX_OUTPUTS outputs or MAX_RANK dims, TF padding,
-        tensor_content only, strings, packed varints in rows of unpacked elements, any error)."""
-        wanted = set(keys)
-        per = [self._decode_two_phase([w], strict, out_dtypes, 16, wanted)[0] for w in wires]
-        result, shapes = {}, {}
-        for k in keys:
-            parts = [p[0][k] for p in per]
+        shapes = {}
+
+        def bad_rank(k, parts):
             rank = parts[0].ndim
             if rank == 0 or any(a.ndim != rank for a in parts):
-                raise ValueError(f"output {k!r}: every response must have the same rank >= 1 to be padded")
-            if len({a.dtype for a in parts}) > 1:
-                raise ValueError(f"output {k!r}: responses disagree on the dtype ({', '.join(sorted({str(a.dtype) for a in parts}))})")
+                return f"output {k!r}: every response must have the same rank >= 1 to be padded"
+            return None
+
+        def pad(k, parts):
+            rank = parts[0].ndim
             tail = tuple(int(x) for x in pad_to[k]) if k in pad_to else \
                 tuple(max(a.shape[d] for a in parts) for d in range(1, rank))
             if len(tail) != rank - 1:
@@ -1079,67 +1105,52 @@ class Codec:
                     raise ValueError(f"output {k!r}: a response of shape {a.shape} does not fit pad_to {tail}")
                 res[(slice(r0, r0 + a.shape[0]),) + tuple(slice(0, d) for d in a.shape[1:])] = a
                 r0 += a.shape[0]
-            if device and res.dtype.kind in "US":
-                raise TypeError(f"output {k!r}: string tensors are decoded on the host")
-            result[k] = self._concat_deliver(k, res, device, out)
             shapes[k] = np.array([a.shape for a in parts], dtype=np.int64).reshape(len(parts), rank)
-        return result, shapes, [p[1] for p in per]
+            return res
+        result, specs = self._per_record(wires, keys, strict, out_dtypes, device, out, bad_rank, pad)
+        return result, shapes, specs
 
     def _padded_device(self, wires, buf, off, ln, keys, pad_value, pad_to, strict, out_dtypes, device, out):
         """The device route (b200tfs_decode_padded): parse, one-CTA plan, destination-major emit, varint decode - or None
-        when the batch holds a case it leaves to the response-by-response route.  The host layout runs first, so nothing is
-        written into `out` for a batch that route then refuses."""
-        n, nk = len(wires), len(keys)
-        kb = [k.encode("utf-8") for k in keys]
-        cast_code = 0
-        if out_dtypes:
-            cast_code = None if strict else _narrowing_cast(out_dtypes)
-            if cast_code is None:
-                return None
-        pk = (N.PadKey * nk)()
-        for i, k in enumerate(kb):
-            pk[i].key, pk[i].key_len = k, len(k)
-        N.check(self._lib.b200tfs_padded_layout(buf.ctypes.data, n, off, ln, nk, pk, cast_code))
-        shapes, np_types, pads = [], [], []
-        for i in range(nk):
-            c = pk[i]
-            # strict DT_HALF: the reference reads half_val as values, the device writes TF's bit patterns
-            if c.status != N.OK or c.dtype == DT_STRING or strict and c.dtype in (DT_HALF, DT_BFLOAT16, DT_COMPLEX64, DT_COMPLEX128):
-                return None
-            if cast_code and not _narrowing_fits(c.dtype, keys[i], out_dtypes):
-                return None
+        when the batch holds a case it leaves to the response-by-response route."""
+        pads = []
+
+        def shape_of(i, c, np_type):
+            if strict and c.dtype == DT_HALF:
+                return None   # the reference reads half_val as values, the device writes TF's bit patterns
             tail = tuple(int(c.dims[d]) for d in range(1, c.rank))
             if keys[i] in pad_to:
                 want = tuple(int(x) for x in pad_to[keys[i]])
                 if len(want) != len(tail) or any(t > w for t, w in zip(tail, want)):
                     return None   # the definition raises, after decoding every response
                 tail = want
-            np_types.append(np.dtype(numpy_for_enum(cast_code if cast_code and c.dtype == DT_FLOAT else int(c.dtype))))
-            shapes.append((int(c.dims[0]),) + tail)
             try:
-                pads.append(np.full((1,), pad_value, np_types[i]).tobytes())
+                pads.append(np.full((1,), pad_value, np_type).tobytes())
             except Exception:     # noqa: BLE001 - the definition raises it, after decoding every response
                 return None
-        dev, ptrs, holds = self._key_destinations(keys, out, shapes, np_types)
-        if any(p % 16 for p in ptrs):
-            return None           # the emit writes whole 16-byte vectors
-        for i in range(nk):
-            pk[i].dst, pk[i].dst_cap, pk[i].rank = ptrs[i], int(np.prod(shapes[i], dtype=np.int64)) * np_types[i].itemsize, len(shapes[i])
-            for d in range(1, len(shapes[i])):
-                pk[i].dims[d] = shapes[i][d]
-            C.memmove(pk[i].pad_bits, pads[i], len(pads[i]))
-        wire = D.DeviceArray(self, (len(buf),), np.uint8).copy_from_host(buf)
-        with self._decode_modes(cast_code):
-            N.check(self._lib.b200tfs_decode_padded(self._ctx, wire.ptr, n, off, ln, nk, pk))
-        outs, specs, rec_status = (N.Output * (n * nk))(), (N.ModelSpec * n)(), (C.c_int32 * n)()
-        N.check(self._lib.b200tfs_padded_results(self._ctx, n, nk, outs, specs, rec_status))   # synchronises
-        if any(rec_status[r] != N.OK for r in range(n)) or any(outs[j].status != N.OK for j in range(n * nk)):
+            return (int(c.dims[0]),) + tail
+
+        def place(pk, ptrs, shapes, np_types):
+            if any(p % 16 for p in ptrs):
+                return False      # the emit writes whole 16-byte vectors
+            for i in range(len(keys)):
+                pk[i].dst, pk[i].dst_cap, pk[i].rank = ptrs[i], int(np.prod(shapes[i], dtype=np.int64)) * np_types[i].itemsize, len(shapes[i])
+                for d in range(1, len(shapes[i])):
+                    pk[i].dims[d] = shapes[i][d]
+                C.memmove(pk[i].pad_bits, pads[i], len(pads[i]))
+            return True
+        f = self._key_device((N.PadKey, self._lib.b200tfs_padded_layout, self._lib.b200tfs_decode_padded, self._lib.b200tfs_padded_results),
+                             wires, buf, off, ln, keys, strict, out_dtypes, out, shape_of, place)
+        if f is None:
             return None
-        rec_shapes = {k: np.array([list(outs[r * nk + i].dims)[: len(shapes[i])] for r in range(n)], dtype=np.int64).reshape(n, len(shapes[i]))
+        n, nk = len(wires), len(keys)
+        if any(f.rec_status[r] != N.OK for r in range(n)) or any(f.outs[j].status != N.OK for j in range(n * nk)):
+            return None
+        rec_shapes = {k: np.array([list(f.outs[r * nk + i].dims)[: len(f.shapes[i])] for r in range(n)], dtype=np.int64).reshape(n, len(f.shapes[i]))
                       for i, k in enumerate(keys)}
-        result = self._key_deliver(keys, out, device, shapes, np_types, dev, ptrs)
+        result = self._key_deliver(keys, out, device, f.shapes, f.np_types, f.dev, f.ptrs)
         self.padded_device_calls += 1
-        return result, rec_shapes, [self._spec(buf, int(off[r]), specs[r]) for r in range(n)]
+        return result, rec_shapes, f.specs
 
     # ---- Classify / Regress responses ------------------------------------------------------------------
     def decode_regression_responses(self, wires: Sequence[bytes], *, device: bool = False, out=None) -> RegressionBatch:

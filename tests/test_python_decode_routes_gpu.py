@@ -2,8 +2,8 @@
 
 For every case below - float, varint, string and mixed outputs, more than eight outputs, malformed records, TF padding,
 tensor_content, strict DT_HALF, ``out_dtypes`` narrowing, pinned and ordinary ``out=``, ``open_predict_response`` +
-``OpenResponse.array`` and the concatenated decode - the test records what comes back (dtype, shape and a digest of the
-bytes, or the exception type), whether each returned array is a view of the launch's host buffer, a fresh array or the
+``OpenResponse.array`` and the concatenated and padded decodes - the test records what comes back (dtype, shape and a digest
+of the bytes, or the exception type), whether each returned array is a view of the launch's host buffer, a fresh array or the
 caller's ``out=`` array, how far ``kernel_launches()``, ``concat_device_calls`` and ``b200tfs_decode_stats`` advance, and how
 many times each native decode entry point runs.  Each case runs twice on a fresh codec, and twice again on a codec that has
 already seen varint outputs (``_seen_varints``), so that the templates the first call leaves and the varint switch are
@@ -29,7 +29,8 @@ pytestmark = pytest.mark.gpu
 COUNTED = ("b200tfs_decode_responses_host_async", "b200tfs_decode_results", "b200tfs_parse_responses_host",
            "b200tfs_parse_tensor_protos_host", "b200tfs_unpack_outputs_host", "b200tfs_unpack_outputs", "b200tfs_set_decode_cast",
            "b200tfs_set_decode_varints", "b200tfs_decode_slot_bytes", "b200tfs_response_keys", "b200tfs_concat_layout",
-           "b200tfs_decode_concat", "b200tfs_concat_results", "b200tfs_memcpy_h2d", "b200tfs_memcpy_d2h")
+           "b200tfs_decode_concat", "b200tfs_concat_results", "b200tfs_padded_layout", "b200tfs_decode_padded",
+           "b200tfs_padded_results", "b200tfs_memcpy_h2d", "b200tfs_memcpy_d2h")
 
 build = wire_oracle.build_predict_response
 rng = np.random.default_rng(20261016)
@@ -123,6 +124,29 @@ def _concat(wires, out=None, **kw):
     return run
 
 
+def _padded(wires, out=None, **kw):
+    """``out`` values: (shape, dtype, where) with where False (numpy), True (device array) or "torch" (a torch tensor 8 bytes
+    past a 16-byte boundary: the device route refuses it), returned as a host copy."""
+    def run(c):
+        dst = {}
+        for k, (shape, dtype, where) in (out or {}).items():
+            if where == "torch":
+                import torch
+
+                dst[k] = torch.from_numpy(np.zeros(int(np.prod(shape)) + 1, dtype)).cuda()[1:].view(*shape)
+            else:
+                dst[k] = c.device_array(np.zeros(shape, dtype)) if where else np.zeros(shape, dtype)
+        res = c.decode_predict_responses_padded(wires, out=dst or None, **kw)
+        for k, v in dst.items():
+            if not isinstance(v, (np.ndarray, DV.DeviceArray)):
+                res[0][k] = v.cpu().numpy()
+        return res, [v for v in dst.values() if isinstance(v, (np.ndarray, DV.DeviceArray))]
+    return run
+
+
+RAGGED = build([("scores", F32[:3, :2] + 1), ("d", F64[:2])])
+WIDE = build([("scores", Y[:2, :7]), ("d", F64)])
+
 CASES = {}
 for name, w in SINGLES.items():
     for strict in (False, True):
@@ -185,6 +209,43 @@ CASES.update({
     "concat_out_mismatch": _concat([FLOATS, FLOATS2], out={"scores": ((15, 5), np.float32, False)}),
     "concat_out_device_mismatch": _concat([FLOATS, FLOATS2], out={"scores": ((16, 5), np.float64, True)}),
     "concat_out_strings_mismatch": _concat([STRINGS, STRINGS], out={"a": ((3,), np.float32, False)}),
+    "padded_floats": _padded([FLOATS, FLOATS2, FLOATS]),
+    "padded_floats_device": _padded([FLOATS, FLOATS2, FLOATS], device=True),
+    "padded_ragged": _padded([FLOATS, RAGGED, WIDE]),
+    "padded_ragged_device": _padded([FLOATS, RAGGED, WIDE], device=True),
+    "padded_pad_value": _padded([FLOATS, RAGGED, WIDE], pad_value=-1.5),
+    "padded_pad_value_bad": _padded([FLOATS, RAGGED], pad_value="x"),
+    "padded_pad_to": _padded([FLOATS, RAGGED, WIDE], pad_to={"scores": (9,)}),
+    "padded_pad_to_small": _padded([FLOATS, RAGGED, WIDE], pad_to={"scores": (5,)}),
+    "padded_pad_to_rank": _padded([FLOATS, RAGGED], pad_to={"scores": (9, 2)}),
+    "padded_mixed": _padded([MIXED, MIXED2]),
+    "padded_mixed_device": _padded([MIXED, MIXED2], device=True),
+    "padded_mixed_strict": _padded([MIXED, MIXED2], strict=True),
+    "padded_keys": _padded([MIXED, MIXED2], keys=["d", "classes"]),
+    "padded_varint": _padded([VARINT, VARINT]),
+    "padded_strings": _padded([STRINGS, STRINGS]),
+    "padded_strings_device": _padded([STRINGS, STRINGS], device=True),
+    "padded_half": _padded([HALF, HALF]),
+    "padded_half_strict": _padded([HALF, HALF], strict=True),
+    "padded_narrow": _padded([NARROW, NARROW], out_dtypes={"f": np.float16, "g": np.float16}),
+    "padded_narrow_partial": _padded([NARROW, NARROW], out_dtypes={"f": np.float16}),
+    "padded_narrow_strict": _padded([NARROW, NARROW], out_dtypes={"f": np.float16, "g": np.float16}, strict=True),
+    "padded_many": _padded([MANY, MANY]),
+    "padded_rank0": _padded([RANK0, RANK0]),
+    "padded_pad": _padded([PAD, PAD]),
+    "padded_content": _padded([CONTENT, CONTENT]),
+    "padded_varint_rows": _padded([VARINT_BAD["rows"], VARINT_BAD["rows"]]),
+    "padded_varint_few": _padded([VARINT_BAD["few"], VARINT_BAD["few"]]),
+    "padded_varint_range": _padded([VARINT_BAD["range"], VARINT_BAD["range"]]),
+    "padded_truncated_first": _padded([TRUNCATED, MIXED]),
+    "padded_truncated_second": _padded([MIXED, TRUNCATED]),
+    "padded_dtype_disagrees": _padded([FLOATS, build([("scores", F32.astype(np.float64)), ("d", F64)])]),
+    "padded_out_numpy": _padded([FLOATS, FLOATS2], out={"scores": ((16, 5), np.float32, False)}),
+    "padded_out_device": _padded([FLOATS, FLOATS2], out={"scores": ((16, 5), np.float32, True), "d": ((6,), np.float64, True)}),
+    "padded_out_unaligned": _padded([FLOATS, FLOATS2], out={"d": ((6,), np.float64, "torch")}),
+    "padded_out_mismatch": _padded([FLOATS, FLOATS2], out={"scores": ((15, 5), np.float32, False)}),
+    "padded_out_device_mismatch": _padded([FLOATS, FLOATS2], out={"scores": ((16, 5), np.float64, True)}),
+    "padded_out_strings_mismatch": _padded([STRINGS, STRINGS], out={"a": ((3,), np.float32, False)}),
     "tensor_protos": lambda c: (c.decode_tensor_protos([SEEDS["t_f32"], SEEDS["t_i32"], SEEDS["t_f64_content"]]), []),
     "tensor_protos_strict": lambda c: (c.decode_tensor_protos([SEEDS["t_f32"], SEEDS["t_i32"], SEEDS["t_f64_content"]], strict=True), []),
     "parse": lambda c: ([sorted(p.keys()) for p in c.parse_predict_responses([FLOATS, MANY, STRINGS])], []),
@@ -1596,6 +1657,376 @@ EXPECTED = {
         'warm': [
             {'calls': {'b200tfs_decode_responses_host_async': 2, 'b200tfs_decode_results': 2, 'b200tfs_decode_slot_bytes': 1, 'b200tfs_unpack_outputs_host': 1}, 'concat_device_calls': 0, 'launches': 2, 'result': ['ok', [[['y', ['array', '<f4', [0], 'da39a3ee5e6b', 'out']]], ['spec', 'default', 1, True, '', 'serving_default']]], 'seen_varints': True, 'stats': [2, 0, 0]},
             {'calls': {'b200tfs_decode_responses_host_async': 2, 'b200tfs_decode_results': 2, 'b200tfs_decode_slot_bytes': 1, 'b200tfs_unpack_outputs_host': 1}, 'concat_device_calls': 0, 'launches': 2, 'result': ['ok', [[['y', ['array', '<f4', [0], 'da39a3ee5e6b', 'out']]], ['spec', 'default', 1, True, '', 'serving_default']]], 'seen_varints': True, 'stats': [2, 0, 0]},
+        ],
+    },
+    'padded_content': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['c', ['array', '<f4', [16, 5], '0faa8a48c67b', 'fresh']]], [['c', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['c', ['array', '<f4', [16, 5], '0faa8a48c67b', 'fresh']]], [['c', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['c', ['array', '<f4', [16, 5], '0faa8a48c67b', 'fresh']]], [['c', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['c', ['array', '<f4', [16, 5], '0faa8a48c67b', 'fresh']]], [['c', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_dtype_disagrees': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_floats': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [24, 5], '907117f39572', 'fresh']], ['d', ['array', '<f8', [9], 'ac70ecbf4f0c', 'fresh']]], [['scores', ['array', '<i8', [3, 2], '8d1645f09d1d', 'fresh']], ['d', ['array', '<i8', [3, 1], 'de29d662a270', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [24, 5], '907117f39572', 'fresh']], ['d', ['array', '<f8', [9], 'ac70ecbf4f0c', 'fresh']]], [['scores', ['array', '<i8', [3, 2], '8d1645f09d1d', 'fresh']], ['d', ['array', '<i8', [3, 1], 'de29d662a270', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [24, 5], '907117f39572', 'fresh']], ['d', ['array', '<f8', [9], 'ac70ecbf4f0c', 'fresh']]], [['scores', ['array', '<i8', [3, 2], '8d1645f09d1d', 'fresh']], ['d', ['array', '<i8', [3, 1], 'de29d662a270', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [24, 5], '907117f39572', 'fresh']], ['d', ['array', '<f8', [9], 'ac70ecbf4f0c', 'fresh']]], [['scores', ['array', '<i8', [3, 2], '8d1645f09d1d', 'fresh']], ['d', ['array', '<i8', [3, 1], 'de29d662a270', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_floats_device': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [24, 5], '907117f39572', 'device']], ['d', ['device', '<f8', [9], 'ac70ecbf4f0c', 'device']]], [['scores', ['array', '<i8', [3, 2], '8d1645f09d1d', 'fresh']], ['d', ['array', '<i8', [3, 1], 'de29d662a270', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [24, 5], '907117f39572', 'device']], ['d', ['device', '<f8', [9], 'ac70ecbf4f0c', 'device']]], [['scores', ['array', '<i8', [3, 2], '8d1645f09d1d', 'fresh']], ['d', ['array', '<i8', [3, 1], 'de29d662a270', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [24, 5], '907117f39572', 'device']], ['d', ['device', '<f8', [9], 'ac70ecbf4f0c', 'device']]], [['scores', ['array', '<i8', [3, 2], '8d1645f09d1d', 'fresh']], ['d', ['array', '<i8', [3, 1], 'de29d662a270', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [24, 5], '907117f39572', 'device']], ['d', ['device', '<f8', [9], 'ac70ecbf4f0c', 'device']]], [['scores', ['array', '<i8', [3, 2], '8d1645f09d1d', 'fresh']], ['d', ['array', '<i8', [3, 1], 'de29d662a270', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_half': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['h', ['array', '<f2', [12], 'd7d38c467a05', 'fresh']], ['f', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']]], [['h', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['f', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['h', ['array', '<f2', [12], 'd7d38c467a05', 'fresh']], ['f', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']]], [['h', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['f', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['h', ['array', '<f2', [12], 'd7d38c467a05', 'fresh']], ['f', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']]], [['h', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['f', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['h', ['array', '<f2', [12], 'd7d38c467a05', 'fresh']], ['f', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']]], [['h', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['f', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_half_strict': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['h', ['array', '<f2', [12], 'a612ac46cb97', 'fresh']], ['f', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']]], [['h', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['f', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['h', ['array', '<f2', [12], 'a612ac46cb97', 'fresh']], ['f', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']]], [['h', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['f', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['h', ['array', '<f2', [12], 'a612ac46cb97', 'fresh']], ['f', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']]], [['h', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['f', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['h', ['array', '<f2', [12], 'a612ac46cb97', 'fresh']], ['f', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']]], [['h', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['f', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_keys': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']], ['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']]], [['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']], ['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']], ['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']]], [['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']], ['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']], ['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']]], [['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']], ['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']], ['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']]], [['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']], ['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_many': {
+        'cold': [
+            {'calls': {'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['o0', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']], ['o1', ['array', '<f4', [10], '9bd4809dc080', 'fresh']], ['o2', ['array', '<f4', [10], '603b11843256', 'fresh']], ['o3', ['array', '<f4', [10], '12388578a29e', 'fresh']], ['o4', ['array', '<f4', [10], '50493d3f1088', 'fresh']], ['o5', ['array', '<f4', [10], '159f97f92d1a', 'fresh']], ['o6', ['array', '<f4', [10], '4d18a2bb7161', 'fresh']], ['o7', ['array', '<f4', [10], '361fa970ef6e', 'fresh']], ['o8', ['array', '<f4', [10], '2b195ee6133a', 'fresh']]], [['o0', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o1', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o2', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o3', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o4', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o5', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o6', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o7', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o8', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['o0', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']], ['o1', ['array', '<f4', [10], '9bd4809dc080', 'fresh']], ['o2', ['array', '<f4', [10], '603b11843256', 'fresh']], ['o3', ['array', '<f4', [10], '12388578a29e', 'fresh']], ['o4', ['array', '<f4', [10], '50493d3f1088', 'fresh']], ['o5', ['array', '<f4', [10], '159f97f92d1a', 'fresh']], ['o6', ['array', '<f4', [10], '4d18a2bb7161', 'fresh']], ['o7', ['array', '<f4', [10], '361fa970ef6e', 'fresh']], ['o8', ['array', '<f4', [10], '2b195ee6133a', 'fresh']]], [['o0', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o1', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o2', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o3', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o4', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o5', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o6', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o7', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o8', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['o0', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']], ['o1', ['array', '<f4', [10], '9bd4809dc080', 'fresh']], ['o2', ['array', '<f4', [10], '603b11843256', 'fresh']], ['o3', ['array', '<f4', [10], '12388578a29e', 'fresh']], ['o4', ['array', '<f4', [10], '50493d3f1088', 'fresh']], ['o5', ['array', '<f4', [10], '159f97f92d1a', 'fresh']], ['o6', ['array', '<f4', [10], '4d18a2bb7161', 'fresh']], ['o7', ['array', '<f4', [10], '361fa970ef6e', 'fresh']], ['o8', ['array', '<f4', [10], '2b195ee6133a', 'fresh']]], [['o0', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o1', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o2', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o3', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o4', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o5', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o6', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o7', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o8', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['o0', ['array', '<f4', [10], '978ac77ea8bf', 'fresh']], ['o1', ['array', '<f4', [10], '9bd4809dc080', 'fresh']], ['o2', ['array', '<f4', [10], '603b11843256', 'fresh']], ['o3', ['array', '<f4', [10], '12388578a29e', 'fresh']], ['o4', ['array', '<f4', [10], '50493d3f1088', 'fresh']], ['o5', ['array', '<f4', [10], '159f97f92d1a', 'fresh']], ['o6', ['array', '<f4', [10], '4d18a2bb7161', 'fresh']], ['o7', ['array', '<f4', [10], '361fa970ef6e', 'fresh']], ['o8', ['array', '<f4', [10], '2b195ee6133a', 'fresh']]], [['o0', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o1', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o2', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o3', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o4', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o5', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o6', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o7', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['o8', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_mixed': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']], ['scores', ['array', '<f4', [10, 5], '61c2992f9901', 'fresh']], ['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']], ['scores', ['array', '<f4', [10, 5], '61c2992f9901', 'fresh']], ['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']], ['scores', ['array', '<f4', [10, 5], '61c2992f9901', 'fresh']], ['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']], ['scores', ['array', '<f4', [10, 5], '61c2992f9901', 'fresh']], ['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_mixed_device': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['device', '<i8', [10, 5], 'db935af57046', 'device']], ['scores', ['device', '<f4', [10, 5], '61c2992f9901', 'device']], ['d', ['device', '<f8', [4, 1], '29fc26da5c1c', 'device']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['device', '<i8', [10, 5], 'db935af57046', 'device']], ['scores', ['device', '<f4', [10, 5], '61c2992f9901', 'device']], ['d', ['device', '<f8', [4, 1], '29fc26da5c1c', 'device']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['device', '<i8', [10, 5], 'db935af57046', 'device']], ['scores', ['device', '<f4', [10, 5], '61c2992f9901', 'device']], ['d', ['device', '<f8', [4, 1], '29fc26da5c1c', 'device']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['device', '<i8', [10, 5], 'db935af57046', 'device']], ['scores', ['device', '<f4', [10, 5], '61c2992f9901', 'device']], ['d', ['device', '<f8', [4, 1], '29fc26da5c1c', 'device']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_mixed_strict': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']], ['scores', ['array', '<f4', [10, 5], '61c2992f9901', 'fresh']], ['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']], ['scores', ['array', '<f4', [10, 5], '61c2992f9901', 'fresh']], ['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']], ['scores', ['array', '<f4', [10, 5], '61c2992f9901', 'fresh']], ['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['classes', ['array', '<i8', [10, 5], 'db935af57046', 'fresh']], ['scores', ['array', '<f4', [10, 5], '61c2992f9901', 'fresh']], ['d', ['array', '<f8', [4, 1], '29fc26da5c1c', 'fresh']]], [['classes', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['scores', ['array', '<i8', [2, 2], '4a72c2d2a443', 'fresh']], ['d', ['array', '<i8', [2, 2], '8a9fb03e4ef2', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_narrow': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1, 'b200tfs_set_decode_cast': 2}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f2', [198], '01c90ef1748f', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1, 'b200tfs_set_decode_cast': 2}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f2', [198], '01c90ef1748f', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1, 'b200tfs_set_decode_cast': 2}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f2', [198], '01c90ef1748f', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1, 'b200tfs_set_decode_cast': 2}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f2', [198], '01c90ef1748f', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_narrow_partial': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 10, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f4', [198], 'ea065140f6b0', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 10, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f4', [198], 'ea065140f6b0', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 10, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f4', [198], 'ea065140f6b0', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 10, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f4', [198], 'ea065140f6b0', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_narrow_strict': {
+        'cold': [
+            {'calls': {'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f2', [198], '01c90ef1748f', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f2', [198], '01c90ef1748f', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f2', [198], '01c90ef1748f', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['f', ['array', '<f2', [60, 7], '1ef8d77aafaa', 'fresh']], ['g', ['array', '<f2', [198], '01c90ef1748f', 'fresh']], ['ids', ['array', '<i8', [100], '4b0fdc7daed0', 'fresh']]], [['f', ['array', '<i8', [2, 2], 'e64d738ca8ff', 'fresh']], ['g', ['array', '<i8', [2, 1], '706e0b8d481d', 'fresh']], ['ids', ['array', '<i8', [2, 1], '5835af0410d0', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_out_device': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 3, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [16, 5], '9808d3628a01', 'out']], ['d', ['device', '<f8', [6], '9f573d120c9b', 'out']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 3, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [16, 5], '9808d3628a01', 'out']], ['d', ['device', '<f8', [6], '9f573d120c9b', 'out']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 3, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [16, 5], '9808d3628a01', 'out']], ['d', ['device', '<f8', [6], '9f573d120c9b', 'out']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 3, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [16, 5], '9808d3628a01', 'out']], ['d', ['device', '<f8', [6], '9f573d120c9b', 'out']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_out_device_mismatch': {
+        'cold': [
+            {'calls': {'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 0, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 0, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 0, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 0, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_out_mismatch': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 0, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 0, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 0, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 0, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_out_numpy': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [16, 5], '9808d3628a01', 'out']], ['d', ['array', '<f8', [6], '9f573d120c9b', 'fresh']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [16, 5], '9808d3628a01', 'out']], ['d', ['array', '<f8', [6], '9f573d120c9b', 'fresh']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [16, 5], '9808d3628a01', 'out']], ['d', ['array', '<f8', [6], '9f573d120c9b', 'fresh']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [16, 5], '9808d3628a01', 'out']], ['d', ['array', '<f8', [6], '9f573d120c9b', 'fresh']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_out_strings_mismatch': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_out_unaligned': {
+        'cold': [
+            {'calls': {'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['scores', ['array', '<f4', [16, 5], '9808d3628a01', 'fresh']], ['d', ['array', '<f8', [6], '9f573d120c9b', 'fresh']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['scores', ['array', '<f4', [16, 5], '9808d3628a01', 'fresh']], ['d', ['array', '<f8', [6], '9f573d120c9b', 'fresh']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['scores', ['array', '<f4', [16, 5], '9808d3628a01', 'fresh']], ['d', ['array', '<f8', [6], '9f573d120c9b', 'fresh']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['ok', [[['scores', ['array', '<f4', [16, 5], '9808d3628a01', 'fresh']], ['d', ['array', '<f8', [6], '9f573d120c9b', 'fresh']]], [['scores', ['array', '<i8', [2, 2], '825a637d87fb', 'fresh']], ['d', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_pad': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['p', ['array', '<f4', [12], 'bb69489226a6', 'fresh']], ['z', ['array', '<f4', [8], 'de8a847bff8c', 'fresh']]], [['p', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['z', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['p', ['array', '<f4', [12], 'bb69489226a6', 'fresh']], ['z', ['array', '<f4', [8], 'de8a847bff8c', 'fresh']]], [['p', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['z', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['p', ['array', '<f4', [12], 'bb69489226a6', 'fresh']], ['z', ['array', '<f4', [8], 'de8a847bff8c', 'fresh']]], [['p', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['z', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['p', ['array', '<f4', [12], 'bb69489226a6', 'fresh']], ['z', ['array', '<f4', [8], 'de8a847bff8c', 'fresh']]], [['p', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['z', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_pad_to': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 9], '301b6605a03b', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 9], '301b6605a03b', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 9], '301b6605a03b', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 9], '301b6605a03b', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_pad_to_rank': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_pad_to_small': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 3, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 3}, 'concat_device_calls': 0, 'launches': 6, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 3, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 3}, 'concat_device_calls': 0, 'launches': 6, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 3, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 3}, 'concat_device_calls': 0, 'launches': 6, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 3, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 3}, 'concat_device_calls': 0, 'launches': 6, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_pad_value': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 7], '1cbc08700a7e', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 7], '1cbc08700a7e', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 7], '1cbc08700a7e', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 7], '1cbc08700a7e', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_pad_value_bad': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_ragged': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 7], 'c3e1f8c53e49', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 7], 'c3e1f8c53e49', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 7], 'c3e1f8c53e49', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 2, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['array', '<f4', [13, 7], 'c3e1f8c53e49', 'fresh']], ['d', ['array', '<f8', [8], '1744000061fe', 'fresh']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_ragged_device': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [13, 7], 'c3e1f8c53e49', 'device']], ['d', ['device', '<f8', [8], '1744000061fe', 'device']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [13, 7], 'c3e1f8c53e49', 'device']], ['d', ['device', '<f8', [8], '1744000061fe', 'device']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [13, 7], 'c3e1f8c53e49', 'device']], ['d', ['device', '<f8', [8], '1744000061fe', 'device']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['scores', ['device', '<f4', [13, 7], 'c3e1f8c53e49', 'device']], ['d', ['device', '<f8', [8], '1744000061fe', 'device']]], [['scores', ['array', '<i8', [3, 2], 'b7c568c51e44', 'fresh']], ['d', ['array', '<i8', [3, 1], '46970c330957', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_rank0': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 4, 'result': ['raise', 'ValueError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_strings': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['ok', [[['a', ['array', '<f4', [8], '7e0c4ddcde8e', 'fresh']], ['ids', ['array', '<i8', [12], 'b1e1d436fa4c', 'fresh']], ['m', ['array', '|b1', [10], '86cd1efe8a37', 'fresh']], ['s', ['array', '<U3', [4], '45a441b904fa', 'fresh']]], [['a', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']], ['ids', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['m', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['s', ['array', '<i8', [2, 1], '21fdd1ec71ba', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['ok', [[['a', ['array', '<f4', [8], '7e0c4ddcde8e', 'fresh']], ['ids', ['array', '<i8', [12], 'b1e1d436fa4c', 'fresh']], ['m', ['array', '|b1', [10], '86cd1efe8a37', 'fresh']], ['s', ['array', '<U3', [4], '45a441b904fa', 'fresh']]], [['a', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']], ['ids', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['m', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['s', ['array', '<i8', [2, 1], '21fdd1ec71ba', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['ok', [[['a', ['array', '<f4', [8], '7e0c4ddcde8e', 'fresh']], ['ids', ['array', '<i8', [12], 'b1e1d436fa4c', 'fresh']], ['m', ['array', '|b1', [10], '86cd1efe8a37', 'fresh']], ['s', ['array', '<U3', [4], '45a441b904fa', 'fresh']]], [['a', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']], ['ids', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['m', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['s', ['array', '<i8', [2, 1], '21fdd1ec71ba', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['ok', [[['a', ['array', '<f4', [8], '7e0c4ddcde8e', 'fresh']], ['ids', ['array', '<i8', [12], 'b1e1d436fa4c', 'fresh']], ['m', ['array', '|b1', [10], '86cd1efe8a37', 'fresh']], ['s', ['array', '<U3', [4], '45a441b904fa', 'fresh']]], [['a', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']], ['ids', ['array', '<i8', [2, 1], '61434fbc6460', 'fresh']], ['m', ['array', '<i8', [2, 1], '37089f813939', 'fresh']], ['s', ['array', '<i8', [2, 1], '21fdd1ec71ba', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_strings_device': {
+        'cold': [
+            {'calls': {'b200tfs_memcpy_h2d': 3, 'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['raise', 'TypeError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_memcpy_h2d': 3, 'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['raise', 'TypeError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_memcpy_h2d': 3, 'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['raise', 'TypeError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_memcpy_h2d': 3, 'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 12, 'result': ['raise', 'TypeError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_truncated_first': {
+        'cold': [
+            {'calls': {'b200tfs_parse_responses_host': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 1, 'result': ['raise', 'DecodeError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_parse_responses_host': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 1, 'result': ['raise', 'DecodeError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_parse_responses_host': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 1, 'result': ['raise', 'DecodeError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_parse_responses_host': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 1, 'result': ['raise', 'DecodeError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_truncated_second': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['raise', 'DecodeError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['raise', 'DecodeError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['raise', 'DecodeError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['raise', 'DecodeError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_varint': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['ids', ['array', '<i8', [6, 7], 'b1151a4651e4', 'fresh']], ['mask', ['array', '|b1', [18], '80e4d63ffc4a', 'fresh']], ['small', ['array', '<i4', [10], 'eee5b0893685', 'fresh']]], [['ids', ['array', '<i8', [2, 2], '1e1a11cce185', 'fresh']], ['mask', ['array', '<i8', [2, 1], '23b8f6f42560', 'fresh']], ['small', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['ids', ['array', '<i8', [6, 7], 'b1151a4651e4', 'fresh']], ['mask', ['array', '|b1', [18], '80e4d63ffc4a', 'fresh']], ['small', ['array', '<i4', [10], 'eee5b0893685', 'fresh']]], [['ids', ['array', '<i8', [2, 2], '1e1a11cce185', 'fresh']], ['mask', ['array', '<i8', [2, 1], '23b8f6f42560', 'fresh']], ['small', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['ids', ['array', '<i8', [6, 7], 'b1151a4651e4', 'fresh']], ['mask', ['array', '|b1', [18], '80e4d63ffc4a', 'fresh']], ['small', ['array', '<i4', [10], 'eee5b0893685', 'fresh']]], [['ids', ['array', '<i8', [2, 2], '1e1a11cce185', 'fresh']], ['mask', ['array', '<i8', [2, 1], '23b8f6f42560', 'fresh']], ['small', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_d2h': 3, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_response_keys': 1}, 'concat_device_calls': 0, 'launches': 6, 'result': ['ok', [[['ids', ['array', '<i8', [6, 7], 'b1151a4651e4', 'fresh']], ['mask', ['array', '|b1', [18], '80e4d63ffc4a', 'fresh']], ['small', ['array', '<i4', [10], 'eee5b0893685', 'fresh']]], [['ids', ['array', '<i8', [2, 2], '1e1a11cce185', 'fresh']], ['mask', ['array', '<i8', [2, 1], '23b8f6f42560', 'fresh']], ['small', ['array', '<i8', [2, 1], '37089f813939', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_varint_few': {
+        'cold': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['x', ['array', '<i8', [8], 'd1b4082d226e', 'fresh']]], [['x', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['x', ['array', '<i8', [8], 'd1b4082d226e', 'fresh']]], [['x', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['x', ['array', '<i8', [8], 'd1b4082d226e', 'fresh']]], [['x', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_padded_layout': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 8, 'result': ['ok', [[['x', ['array', '<i8', [8], 'd1b4082d226e', 'fresh']]], [['x', ['array', '<i8', [2, 1], 'a385649cbb41', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_varint_range': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_parse_responses_host': 1, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 1}, 'concat_device_calls': 0, 'launches': 10, 'result': ['raise', 'OverflowError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_parse_responses_host': 1, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 1}, 'concat_device_calls': 0, 'launches': 10, 'result': ['raise', 'OverflowError'], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_parse_responses_host': 1, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 1}, 'concat_device_calls': 0, 'launches': 10, 'result': ['raise', 'OverflowError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_parse_responses_host': 1, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 1}, 'concat_device_calls': 0, 'launches': 10, 'result': ['raise', 'OverflowError'], 'seen_varints': True, 'stats': [0, 0, 0]},
+        ],
+    },
+    'padded_varint_rows': {
+        'cold': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 16, 'result': ['ok', [[['x', ['array', '<i4', [6], 'bc820beafeab', 'fresh']]], [['x', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 16, 'result': ['ok', [[['x', ['array', '<i4', [6], 'bc820beafeab', 'fresh']]], [['x', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': False, 'stats': [0, 0, 0]},
+        ],
+        'warm': [
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 16, 'result': ['ok', [[['x', ['array', '<i4', [6], 'bc820beafeab', 'fresh']]], [['x', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
+            {'calls': {'b200tfs_decode_padded': 1, 'b200tfs_memcpy_h2d': 1, 'b200tfs_padded_layout': 1, 'b200tfs_padded_results': 1, 'b200tfs_parse_responses_host': 2, 'b200tfs_response_keys': 1, 'b200tfs_unpack_outputs_host': 2}, 'concat_device_calls': 0, 'launches': 16, 'result': ['ok', [[['x', ['array', '<i4', [6], 'bc820beafeab', 'fresh']]], [['x', ['array', '<i8', [2, 1], '7590cbf3642e', 'fresh']]], [['spec', 'default', 1, True, '', 'serving_default'], ['spec', 'default', 1, True, '', 'serving_default']]]], 'seen_varints': True, 'stats': [0, 0, 0]},
         ],
     },
     'parse': {
