@@ -341,8 +341,8 @@ int b200tfs_unpack_outputs(b200tfs_ctx* ctx, const void* arena_dev, int32_t m, c
  * collect the table afterwards with b200tfs_decode_results (which synchronises).
  * Each launch remembers the framing of its record 0; records of the next launch that carry the same
  * framing skip the tag walk.  One corner is reported rather than decoded: a record that has exactly
- * that record's LENGTH but other framing, and whose values are spread over more 32 KB..256 KB tiles
- * than that record's, gets B200TFS_E_NONCANONICAL; decode it with the next launch (which starts
+ * that record's LENGTH but other framing, and whose values are spread over more tiles (32 KB or 64 KB
+ * each, or B200TFS_TILE_BYTES) than that record's, gets B200TFS_E_NONCANONICAL; decode it with the next launch (which starts
  * without a remembered framing) or with b200tfs_parse_responses + b200tfs_unpack_outputs.
  * The launch stores only into [dst_off, dst_off + dst_bytes) of the B200TFS_OK fixed-width outputs of B200TFS_OK records:
  * every other byte of every slot - all of it for a record that did not decode - keeps what the caller left there.
