@@ -451,7 +451,7 @@ int b200tfs_cast_supported(int32_t src, int32_t wire) {
 // wire-size arithmetic and header bytes
 // ------------------------------------------------------------------------------------------------
 static bool request_needs_deferred(const b200tfs_request& r);                  // varint_host.inc
-static int deferred_slot_bound(const b200tfs_request& r, uint64_t* bound);     // varint_host.inc
+static int deferred_arena_size(int32_t n, const b200tfs_request* reqs, uint64_t* bytes);   // varint_host.inc
 
 namespace {
 
@@ -459,31 +459,82 @@ constexpr uint64_t kProtoLimit = 0x7FFFFFFFull;  // protobuf's 2 GiB message lim
 
 struct TensorLayout {
   uint64_t n_elems = 0;
-  uint64_t payload_len = 0;  // bytes of the values field body on the wire (0: field omitted)
+  uint64_t payload_len = 0;  // bytes of the values field body on the wire (0: field omitted, or not known yet: unmeasured)
   uint64_t header_len = 0;   // bytes before the payload
   uint32_t op = OP_COPY;     // MoveOp for fixed-width payloads
   bool varint = false;       // payload produced by the varint kernels
+  bool unmeasured = false;   // a packed-varint payload the deferred encode counts on the device: the header ends at the values
+                             // tag, and the length behind it is the framing kernel's to write
   uint32_t field = 0;        // field number the values go into
   uint64_t shape_len = 0;    // bytes of the TensorShapeProto body
   DtypeInfo src_info{}, wire_info{};
 };
 
-// the header_len bytes in front of a tensor's payload, written at w: 08 vi(dtype) 12 vi(shape_len)
-// {12 vi(dim_len) [08 vi(size)]}* [tag vi(payload_len)]
-uint8_t* write_tensor_header(const b200tfs_tensor& t, const struct TensorLayout& L, uint8_t* w) {
-  *w++ = 0x08; w += put_varint(w, (uint64_t)(uint32_t)t.wire_dtype);
-  *w++ = 0x12; w += put_varint(w, L.shape_len);
-  for (int i = 0; i < t.rank; ++i) {
-    const uint64_t d = (uint64_t)t.dims[i];
-    *w++ = 0x12;
-    if (d) { *w++ = (uint8_t)(1 + varint_len(d)); *w++ = 0x08; w += put_varint(w, d); }
-    else *w++ = 0x00;  // Dim(size=0) is an empty sub-message (Q2)
+// Where the framing writers below put their bytes: raw stores at `w` (the immediate planner writes the blob in place), or a
+// DeferredBuilder (varint_host.inc), which also takes Pending lengths - values its framing program computes on the device
+struct RawOut {
+  uint8_t* w;
+  void byte(uint8_t b) { *w++ = b; }
+  void varint(uint64_t v) { w += put_varint(w, v); }
+  void bytes(const void* p, size_t n) { if (n) { memcpy(w, p, n); w += n; } }
+};
+
+// model_spec{ 0A vi name [12 vi {08 vi(version)}] } of a PredictRequest or a tf.Example request
+struct SpecLayout {
+  uint64_t body = 0, version_len = 0;
+  uint64_t field() const { return 1 + varint_len(body) + body; }   // with its tag and length
+};
+
+template <class Req>
+int spec_layout(const Req& r, SpecLayout* S) {
+  if (r.model_name_len < 0 || (r.model_name_len && !r.model_name)) return fail(B200TFS_E_ARG, "bad model_name");
+  *S = SpecLayout{};
+  if (r.model_name_len) S->body += 1 + varint_len((uint64_t)r.model_name_len) + (uint64_t)r.model_name_len;
+  if (r.has_version) {
+    S->version_len = r.version ? 1 + varint_len((uint64_t)r.version) : 0;
+    S->body += 2 + S->version_len;
   }
-  if (L.payload_len) { w += put_varint(w, tag_of(L.field, WT_LEN)); w += put_varint(w, L.payload_len); }
-  return w;
+  return B200TFS_OK;
 }
 
-int tensor_layout(const b200tfs_tensor& t, TensorLayout* L, std::vector<uint8_t>* hdr) {
+template <class Out, class Req>
+void write_model_spec(Out& o, const Req& r, const SpecLayout& S) {
+  o.byte(0x0A); o.varint(S.body);
+  if (r.model_name_len) { o.byte(0x0A); o.varint((uint64_t)r.model_name_len); o.bytes(r.model_name, (size_t)r.model_name_len); }
+  if (r.has_version) {
+    o.byte(0x12); o.byte((uint8_t)S.version_len);
+    if (r.version) { o.byte(0x08); o.varint((uint64_t)r.version); }
+  }
+}
+
+// a map entry's header: 12 vi(entry_len) 0A vi(key_len) key 12 vi(tp_len)
+template <class Out, class Len>
+void write_entry_header(Out& o, const b200tfs_tensor& t, Len entry_len, Len tp_len) {
+  o.byte(0x12); o.varint(entry_len);
+  o.byte(0x0A); o.varint((uint64_t)t.key_len); o.bytes(t.key, (size_t)t.key_len);
+  o.byte(0x12); o.varint(tp_len);
+}
+
+// the header_len bytes in front of a tensor's payload: 08 vi(dtype) 12 vi(shape_len) {12 vi(dim_len) [08 vi(size)]}*
+// [tag vi(payload_len)] - an unmeasured payload's tag without its length; nothing for a pre-serialised TensorProto
+template <class Out>
+void write_tensor_header(Out& o, const b200tfs_tensor& t, const TensorLayout& L) {
+  if (t.flags & B200TFS_F_PRESERIALIZED) return;
+  o.byte(0x08); o.varint((uint64_t)(uint32_t)t.wire_dtype);
+  o.byte(0x12); o.varint(L.shape_len);
+  for (int i = 0; i < t.rank; ++i) {
+    const uint64_t d = (uint64_t)t.dims[i];
+    o.byte(0x12);
+    if (d) { o.byte((uint8_t)(1 + varint_len(d))); o.byte(0x08); o.varint(d); }
+    else o.byte(0x00);  // Dim(size=0) is an empty sub-message (Q2)
+  }
+  if (L.payload_len || L.unmeasured) o.varint(tag_of(L.field, WT_LEN));
+  if (L.payload_len) o.varint(L.payload_len);
+}
+
+// `deferred`: lay out for b200tfs_encode_requests_async, which counts every packed-varint payload on the device whatever
+// packed_len says; anywhere else such a payload must have been measured
+int tensor_layout(const b200tfs_tensor& t, TensorLayout* L, std::vector<uint8_t>* hdr, bool deferred = false) {
   *L = TensorLayout{};   // layouts are reused from request to request (request_layout): no field may survive
   if (t.flags & B200TFS_F_PRESERIALIZED) {  // an already serialised TensorProto: all payload, no header
     if (t.packed_len > kProtoLimit) return fail(B200TFS_E_TOOBIG, "serialised TensorProto exceeds 2 GiB");
@@ -529,9 +580,10 @@ int tensor_layout(const b200tfs_tensor& t, TensorLayout* L, std::vector<uint8_t>
         break;
       default:  // VK_VARINT
         L->varint = true;
-        if (n && t.packed_len == 0)
+        L->unmeasured = n && deferred;
+        if (n && !deferred && t.packed_len == 0)
           return fail(B200TFS_E_ARG, "varint dtype %d: packed_len not set, call b200tfs_measure first", t.wire_dtype);
-        L->payload_len = n ? t.packed_len : 0;
+        L->payload_len = n && !deferred ? t.packed_len : 0;
         break;
     }
   }
@@ -539,13 +591,15 @@ int tensor_layout(const b200tfs_tensor& t, TensorLayout* L, std::vector<uint8_t>
   uint64_t shape_len = 0;
   for (int i = 0; i < t.rank; ++i) shape_len += 2 + (t.dims[i] ? 1 + varint_len((uint64_t)t.dims[i]) : 0);
   uint64_t hl = 1 + varint_len((uint64_t)(uint32_t)t.wire_dtype) + 1 + varint_len(shape_len) + shape_len;
-  if (L->payload_len) hl += varint_len(tag_of(field, WT_LEN)) + varint_len(L->payload_len);
+  if (L->payload_len || L->unmeasured) hl += varint_len(tag_of(field, WT_LEN));
+  if (L->payload_len) hl += varint_len(L->payload_len);
   L->header_len = hl; L->field = field; L->shape_len = shape_len;
   if (hdr) {   // one resize, then raw writes
     const size_t base = hdr->size();
     hdr->resize(base + hl);
-    if ((uint64_t)(write_tensor_header(t, *L, hdr->data() + base) - (hdr->data() + base)) != hl)
-      return fail(B200TFS_E_ARG, "internal: header length mismatch");
+    RawOut o{hdr->data() + base};
+    write_tensor_header(o, t, *L);
+    if ((uint64_t)(o.w - (hdr->data() + base)) != hl) return fail(B200TFS_E_ARG, "internal: header length mismatch");
   }
   return B200TFS_OK;
 }
@@ -728,16 +782,20 @@ struct RequestLayout {
   std::vector<TensorLayout> tl;
   std::vector<int32_t> perm;
   std::vector<uint64_t> tp_len, entry_len;
-  uint64_t spec_len = 0, version_len = 0, total = 0;
+  SpecLayout spec;
+  uint64_t total = 0;
   uint64_t prefix = 0;        // bytes in front of the message: gRPC's 5-byte frame header when asked for
   uint64_t largest_off = 0;
   std::vector<uint64_t> payload_off;
 };
 
-int request_layout(const b200tfs_request& r, RequestLayout* R) {
+// Validates request r, orders its keys and lays it out.  `deferred` (b200tfs_encode_requests_async): packed-varint inputs are
+// unmeasured, and the record's total - which then depends on lengths the device counts - is checked on the device.
+int request_layout(const b200tfs_request& r, RequestLayout* R, bool deferred = false) {
   if (r.n_inputs < 0) return fail(B200TFS_E_ARG, "n_inputs < 0");
   if (r.n_inputs && !r.inputs) return fail(B200TFS_E_ARG, "inputs is NULL");
-  if (r.model_name_len < 0 || (r.model_name_len && !r.model_name)) return fail(B200TFS_E_ARG, "bad model_name");
+  int rc = spec_layout(r, &R->spec);
+  if (rc) return rc;
   const int n = r.n_inputs;
   R->tl.resize(n); R->perm.resize(n); R->tp_len.resize(n); R->entry_len.resize(n); R->payload_off.resize(n);
   // (no heap traffic for the usual handful of inputs: this runs once per request of a batch)
@@ -754,28 +812,18 @@ int request_layout(const b200tfs_request& r, RequestLayout* R) {
     keys[i] = r.inputs[i].key ? r.inputs[i].key : "";
     lens[i] = r.inputs[i].key_len;
   }
-  int rc = B200TFS_OK;
   if (n == 1 && (r.order == B200TFS_ORDER_GIVEN || r.order == B200TFS_ORDER_UPB || r.order == B200TFS_ORDER_BYTES)) R->perm[0] = 0;
   else rc = order_keys(n, keys, lens, r.order, R->perm.data());
   if (rc) return rc;
-  // model_spec{ 0A vi name  [12 vi {08 vi(version)}] }
-  uint64_t spec = 0;
-  if (r.model_name_len) spec += 1 + varint_len((uint64_t)r.model_name_len) + (uint64_t)r.model_name_len;
-  R->version_len = 0;
-  if (r.has_version) {
-    R->version_len = r.version ? 1 + varint_len((uint64_t)r.version) : 0;
-    spec += 2 + R->version_len;
-  }
-  R->spec_len = spec;
   if (r.flags & ~B200TFS_RF_GRPC_FRAME) return fail(B200TFS_E_ARG, "unknown request flags 0x%x", (unsigned)r.flags);
   R->prefix = (r.flags & B200TFS_RF_GRPC_FRAME) ? 5 : 0;
-  uint64_t total = R->prefix + 1 + varint_len(spec) + spec;
+  uint64_t total = R->prefix + R->spec.field();
   uint64_t largest = 0;
   R->largest_off = 0;
   for (int j = 0; j < n; ++j) {
     const b200tfs_tensor& t = r.inputs[R->perm[j]];
     TensorLayout& L = R->tl[j];
-    if ((rc = tensor_layout(t, &L, nullptr))) return rc;
+    if ((rc = tensor_layout(t, &L, nullptr, deferred))) return rc;
     uint64_t tp = L.header_len + L.payload_len;
     if (tp > kProtoLimit) return fail(B200TFS_E_TOOBIG, "TensorProto of %llu bytes exceeds 2 GiB", (unsigned long long)tp);
     R->tp_len[j] = tp;
@@ -787,7 +835,7 @@ int request_layout(const b200tfs_request& r, RequestLayout* R) {
     if (L.payload_len > largest) { largest = L.payload_len; R->largest_off = payload_off; }
     total += 1 + varint_len(el) + el;
   }
-  if (total - R->prefix > kProtoLimit)
+  if (!deferred && total - R->prefix > kProtoLimit)
     return fail(B200TFS_E_TOOBIG, "PredictRequest of %llu bytes exceeds protobuf's 2 GiB limit", (unsigned long long)(total - R->prefix));
   R->total = total;
   return B200TFS_OK;
@@ -802,32 +850,21 @@ int plan_request(const b200tfs_request& r, const RequestLayout& R, uint8_t* rec,
   const size_t base = pb.blob.size();
   pb.blob.resize(base + frame);
   uint8_t* const w0 = pb.blob.data() + base;
-  uint8_t* w = w0;
+  RawOut o{w0};
   size_t mark = base;     // blob offset where the pending header run starts
   uint8_t* cursor = rec;  // where that run will land
   if (R.prefix) {         // gRPC length-prefixed message: compressed-flag 0, big-endian uint32 length
     const uint64_t m = R.total - R.prefix;
-    *w++ = 0; *w++ = (uint8_t)(m >> 24); *w++ = (uint8_t)(m >> 16); *w++ = (uint8_t)(m >> 8); *w++ = (uint8_t)m;
+    o.byte(0); o.byte((uint8_t)(m >> 24)); o.byte((uint8_t)(m >> 16)); o.byte((uint8_t)(m >> 8)); o.byte((uint8_t)m);
   }
-  *w++ = 0x0A; w += put_varint(w, R.spec_len);
-  if (r.model_name_len) {
-    *w++ = 0x0A; w += put_varint(w, (uint64_t)r.model_name_len);
-    memcpy(w, r.model_name, (size_t)r.model_name_len); w += r.model_name_len;
-  }
-  if (r.has_version) {
-    *w++ = 0x12; *w++ = (uint8_t)R.version_len;
-    if (r.version) { *w++ = 0x08; w += put_varint(w, (uint64_t)r.version); }
-  }
+  write_model_spec(o, r, R.spec);
   for (int j = 0; j < r.n_inputs; ++j) {
     const b200tfs_tensor& t = r.inputs[R.perm[j]];
     const TensorLayout& L = R.tl[j];
-    *w++ = 0x12; w += put_varint(w, R.entry_len[j]);
-    *w++ = 0x0A; w += put_varint(w, (uint64_t)t.key_len);
-    if (t.key_len) { memcpy(w, t.key, (size_t)t.key_len); w += t.key_len; }
-    *w++ = 0x12; w += put_varint(w, R.tp_len[j]);
-    if (!(t.flags & B200TFS_F_PRESERIALIZED)) w = write_tensor_header(t, L, w);
+    write_entry_header(o, t, R.entry_len[j], R.tp_len[j]);
+    write_tensor_header(o, t, L);
     if (L.payload_len) {
-      const size_t at = base + (size_t)(w - w0), run = at - mark;
+      const size_t at = base + (size_t)(o.w - w0), run = at - mark;
       pb.header(cursor, mark, run);
       cursor += run;
       int rc = plan_tensor(t, L, cursor, pb);
@@ -836,9 +873,9 @@ int plan_request(const b200tfs_request& r, const RequestLayout& R, uint8_t* rec,
       mark = at;
     }
   }
-  const size_t end = base + (size_t)(w - w0), run = end - mark;
+  const size_t end = base + (size_t)(o.w - w0), run = end - mark;
   if (run) { pb.header(cursor, mark, run); cursor += run; }
-  if ((uint64_t)(w - w0) != frame || (uint64_t)(cursor - rec) != R.total) return fail(B200TFS_E_ARG, "internal: request length mismatch");
+  if ((uint64_t)(o.w - w0) != frame || (uint64_t)(cursor - rec) != R.total) return fail(B200TFS_E_ARG, "internal: request length mismatch");
   return B200TFS_OK;
 }
 
@@ -921,17 +958,8 @@ int b200tfs_request_arena_size(int32_t n, const b200tfs_request* reqs, uint64_t*
   // gets a slot for its worst case; measured batches are sized exactly, as b200tfs_encode_requests lays them out
   bool deferred = false;
   for (int i = 0; i < n && !deferred; ++i) deferred = request_needs_deferred(reqs[i]);
+  if (deferred) return deferred_arena_size(n, reqs, bytes);
   uint64_t cursor = 0;
-  if (deferred) {
-    for (int i = 0; i < n; ++i) {
-      uint64_t bound = 0;
-      int rc = deferred_slot_bound(reqs[i], &bound);
-      if (rc) return rc;
-      cursor = ((cursor + 255) & ~255ull) + bound + 128;
-    }
-    *bytes = (cursor + 255) & ~255ull;
-    return B200TFS_OK;
-  }
   RequestLayout R;
   for (int i = 0; i < n; ++i) {
     int rc = request_layout(reqs[i], &R);
