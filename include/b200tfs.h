@@ -83,6 +83,8 @@ extern "C" {
                                          host hands over DT_STRING tensors, tensors.py:24): spliced in verbatim        */
 #define B200TFS_F_DEVICE_DATA 0x8u    /* *_host entry points only: `data` of THIS tensor is a device pointer already (a tensor
                                          that lives in HBM - the usual case for a model's activations): it is not staged      */
+#define B200TFS_F_BROADCAST 0x10u     /* b200tfs_feature.flags: a 0-d column, whose one row is repeated in every example.
+                                         b200tfs_tensor.flags (b200tfs_encode_padded_requests_async): the same tensor in every request */
 
 /* ---- decode flags (b200tfs_output.flags, set by the parser) ----------------------------------- */
 #define B200TFS_OF_TENSOR_CONTENT 0x1u /* values arrived in tensor_content                                        */
@@ -506,6 +508,41 @@ int b200tfs_decode_padded_host_async(b200tfs_ctx* ctx, const void* wire_host, in
 int b200tfs_padded_results(b200tfs_ctx* ctx, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs,
                            int32_t* rec_status);
 
+/* ---- batch encode of PredictRequests cut out of one padded tensor per input ------------------------
+ * The inverse of b200tfs_decode_padded: request r's tensor for a padded input P of shape [R, D_1, ..., D_{m-1}] is the box
+ * P[r0 : r0 + S[r,0], :S[r,1], ..., :S[r,m-1]], r0 = S[0,0] + ... + S[r-1,0], where S (int64[n, m] in device memory, or int64[n] row
+ * counts with every trailing dim full) gives each request's shape.  The bytes are what b200tfs_encode_requests writes for the
+ * request of those boxes.  Each input's b200tfs_tensor describes the padded tensor (device `data`, `dims` = [R, D_1, ...], dtypes,
+ * flags, key); with B200TFS_F_BROADCAST (0x10, the b200tfs_feature flag) in its flags it is the same tensor, dims as given (any
+ * rank, 0 included), in every request.  The shapes are only read on the device, so a replayed CUDA graph re-plans rows, boxes,
+ * framing and record offsets from whatever the shapes tables and the tensors hold then.                                        */
+typedef struct b200tfs_pad_input {
+  const int64_t* shapes;  /* b200tfs_encode_padded_requests_async: device int64[n, cols]; b200tfs_padded_request_frame: host, the one
+                             request's `cols` entries.  Ignored for a B200TFS_F_BROADCAST input                                         */
+  int32_t cols;           /* the input's rank (full shapes) or 1 (row counts)                                                        */
+  int32_t pad_;
+} b200tfs_pad_input;
+/* Host only, closed form from n and the padded shapes: arena bytes that always hold the n records (per padded input the whole
+ * tensor's payload - 10 bytes per element for the packed-varint dtypes - since the boxes partition its rows; per request the
+ * largest framing these dims allow plus 256 + 128 bytes of placement; broadcast payloads n times).                               */
+int b200tfs_padded_request_arena_size(int32_t n, const b200tfs_request* req, uint64_t* bytes);
+/* Encode the n requests into the device arena (256-byte aligned, arena_cap bytes).  `req` gives the model spec, order, flags and
+ * inputs (at most B200TFS_CONCAT_MAX_KEYS padded and B200TFS_CONCAT_MAX_KEYS broadcast inputs, ranks 1..B200TFS_MAX_RANK - 0 too
+ * for broadcast - no DT_STRING: B200TFS_E_ARG / B200TFS_E_DTYPE), in[i] the shapes of req->inputs[i].  Kernels only (plan, varint
+ * count, layout, frame, move, varint emit; b200tfs_kernel_launches counts them): never synchronises and can be captured.  Records
+ * are placed one behind the other in request order, each slot 256-byte aligned with the largest payload 128-byte aligned.
+ * Collect rec_off / rec_len and the first per-request error with b200tfs_encode_results: B200TFS_E_SHAPE (a negative dim, a
+ * trailing dim past the padded one), B200TFS_E_SIZE (rows past R: that request and every later one), B200TFS_E_TOOBIG (over
+ * 2 GiB).  A request with an error gets rec_len 0 and no bytes; stores go only into [rec_off, rec_off + rec_len) of the others. */
+int b200tfs_encode_padded_requests_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_request* req, const b200tfs_pad_input* in,
+                                         void* arena_dev, uint64_t arena_cap);
+/* What the framing kernels do for ONE request, run on the host (the same inline code; needs no device): in[i].shapes points at the
+ * request's host shape row for req->inputs[i], packed_len[i] stands in for the counted packed length of a packed-varint input.
+ * Writes every framing byte of the record at its wire position in buf (the payload ranges are left alone), and reports the record
+ * length and, per input, where its payload starts and how long it is.  The request's rows start at row 0 of each padded input.     */
+int b200tfs_padded_request_frame(const b200tfs_request* req, const b200tfs_pad_input* in, const uint64_t* packed_len, void* buf,
+                                 uint64_t cap, uint64_t* rec_len, uint64_t* payload_off, uint64_t* payload_len);
+
 /* ---- CUDA graphs: record a fixed sequence of encode / decode calls once, replay it per request ---
  * Between capture_begin and capture_end the asynchronous entry points (b200tfs_encode_requests,
  * b200tfs_encode_tensor_protos, b200tfs_decode_responses, b200tfs_memcpy_*) only record work; calls
@@ -586,7 +623,6 @@ int b200tfs_unpack_outputs_host(b200tfs_ctx* ctx, int32_t m, const b200tfs_outpu
  * quieted; float64 rounded to nearest even, NaN -> sign | 0x7FC00000 | (mantissa >> 29); float16 widened exactly, NaNs quieted.
  * Integer and bool columns become int64_list: sign-extended, uint64 wraps (2**64-1 is written as -1), a bool byte != 0 is 1.
  * A row of 0 elements still writes its empty list.  Strings (bytes_list) are not taken: such requests are assembled on the host. */
-#define B200TFS_F_BROADCAST 0x10u     /* b200tfs_feature.flags: a 0-d column, whose one row is repeated in every example            */
 typedef struct b200tfs_feature {
   const void* data;     /* n_examples rows of row_elems elements (one row with B200TFS_F_BROADCAST), C-contiguous, native order,
                            aligned to the element size; a DEVICE pointer for the _async entry point                              */

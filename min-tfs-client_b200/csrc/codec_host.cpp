@@ -22,6 +22,7 @@
 #include "../../include/b200tfs.h"
 #include "example_walk.h"
 #include "frame.h"
+#include "framing.h"
 #include "kernels.h"
 #include "plan.h"
 #include "tpl.h"
@@ -147,6 +148,7 @@ struct b200tfs_ctx {
   Growable xr_dev;                      // b200tfs_decode_example_responses: entry slots and per-response tables (XrLayout)
   Growable xr_host;                     // ... and the results its publish kernel leaves in pinned memory (XrResultsLayout)
   int32_t xr_n = 0;                     // responses of its most recent call, what b200tfs_example_response_results answers for
+  Growable unpad_dev;                   // b200tfs_encode_padded_requests_async: boxes, varint jobs and counters, move plan (UnpadLayout)
 };
 
 // `baked`: the buffer's address ends up inside captured graphs (every context-owned scratch buffer except the plan-upload
@@ -333,6 +335,7 @@ int b200tfs_destroy(b200tfs_ctx* c) {
   if (c->concat_dev.p) cudaFree(c->concat_dev.p);
   if (c->padded_dev.p) cudaFree(c->padded_dev.p);
   if (c->xr_dev.p) cudaFree(c->xr_dev.p);
+  if (c->unpad_dev.p) cudaFree(c->unpad_dev.p);
   if (c->xr_host.p) cudaFreeHost(c->xr_host.p);
   if (c->enc_host.p) cudaFreeHost(c->enc_host.p);
   if (c->measured_dev.p) cudaFree(c->measured_dev.p);
@@ -457,34 +460,7 @@ namespace {
 
 constexpr uint64_t kProtoLimit = 0x7FFFFFFFull;  // protobuf's 2 GiB message limit
 
-struct TensorLayout {
-  uint64_t n_elems = 0;
-  uint64_t payload_len = 0;  // bytes of the values field body on the wire (0: field omitted, or not known yet: unmeasured)
-  uint64_t header_len = 0;   // bytes before the payload
-  uint32_t op = OP_COPY;     // MoveOp for fixed-width payloads
-  bool varint = false;       // payload produced by the varint kernels
-  bool unmeasured = false;   // a packed-varint payload the deferred encode counts on the device: the header ends at the values
-                             // tag, and the length behind it is the framing kernel's to write
-  uint32_t field = 0;        // field number the values go into
-  uint64_t shape_len = 0;    // bytes of the TensorShapeProto body
-  DtypeInfo src_info{}, wire_info{};
-};
-
-// Where the framing writers below put their bytes: raw stores at `w` (the immediate planner writes the blob in place), or a
-// DeferredBuilder (varint_host.inc), which also takes Pending lengths - values its framing program computes on the device
-struct RawOut {
-  uint8_t* w;
-  void byte(uint8_t b) { *w++ = b; }
-  void varint(uint64_t v) { w += put_varint(w, v); }
-  void bytes(const void* p, size_t n) { if (n) { memcpy(w, p, n); w += n; } }
-};
-
-// model_spec{ 0A vi name [12 vi {08 vi(version)}] } of a PredictRequest or a tf.Example request
-struct SpecLayout {
-  uint64_t body = 0, version_len = 0;
-  uint64_t field() const { return 1 + varint_len(body) + body; }   // with its tag and length
-};
-
+// model_spec's layout (framing.h writes it)
 template <class Req>
 int spec_layout(const Req& r, SpecLayout* S) {
   if (r.model_name_len < 0 || (r.model_name_len && !r.model_name)) return fail(B200TFS_E_ARG, "bad model_name");
@@ -495,41 +471,6 @@ int spec_layout(const Req& r, SpecLayout* S) {
     S->body += 2 + S->version_len;
   }
   return B200TFS_OK;
-}
-
-template <class Out, class Req>
-void write_model_spec(Out& o, const Req& r, const SpecLayout& S) {
-  o.byte(0x0A); o.varint(S.body);
-  if (r.model_name_len) { o.byte(0x0A); o.varint((uint64_t)r.model_name_len); o.bytes(r.model_name, (size_t)r.model_name_len); }
-  if (r.has_version) {
-    o.byte(0x12); o.byte((uint8_t)S.version_len);
-    if (r.version) { o.byte(0x08); o.varint((uint64_t)r.version); }
-  }
-}
-
-// a map entry's header: 12 vi(entry_len) 0A vi(key_len) key 12 vi(tp_len)
-template <class Out, class Len>
-void write_entry_header(Out& o, const b200tfs_tensor& t, Len entry_len, Len tp_len) {
-  o.byte(0x12); o.varint(entry_len);
-  o.byte(0x0A); o.varint((uint64_t)t.key_len); o.bytes(t.key, (size_t)t.key_len);
-  o.byte(0x12); o.varint(tp_len);
-}
-
-// the header_len bytes in front of a tensor's payload: 08 vi(dtype) 12 vi(shape_len) {12 vi(dim_len) [08 vi(size)]}*
-// [tag vi(payload_len)] - an unmeasured payload's tag without its length; nothing for a pre-serialised TensorProto
-template <class Out>
-void write_tensor_header(Out& o, const b200tfs_tensor& t, const TensorLayout& L) {
-  if (t.flags & B200TFS_F_PRESERIALIZED) return;
-  o.byte(0x08); o.varint((uint64_t)(uint32_t)t.wire_dtype);
-  o.byte(0x12); o.varint(L.shape_len);
-  for (int i = 0; i < t.rank; ++i) {
-    const uint64_t d = (uint64_t)t.dims[i];
-    o.byte(0x12);
-    if (d) { o.byte((uint8_t)(1 + varint_len(d))); o.byte(0x08); o.varint(d); }
-    else o.byte(0x00);  // Dim(size=0) is an empty sub-message (Q2)
-  }
-  if (L.payload_len || L.unmeasured) o.varint(tag_of(L.field, WT_LEN));
-  if (L.payload_len) o.varint(L.payload_len);
 }
 
 // `deferred`: lay out for b200tfs_encode_requests_async, which counts every packed-varint payload on the device whatever
@@ -588,8 +529,7 @@ int tensor_layout(const b200tfs_tensor& t, TensorLayout* L, std::vector<uint8_t>
     }
   }
   if (L->payload_len > kProtoLimit) return fail(B200TFS_E_TOOBIG, "payload of %llu bytes exceeds protobuf's 2 GiB limit", (unsigned long long)L->payload_len);
-  uint64_t shape_len = 0;
-  for (int i = 0; i < t.rank; ++i) shape_len += 2 + (t.dims[i] ? 1 + varint_len((uint64_t)t.dims[i]) : 0);
+  const uint64_t shape_len = shape_body_len(t.rank, t.dims);
   uint64_t hl = 1 + varint_len((uint64_t)(uint32_t)t.wire_dtype) + 1 + varint_len(shape_len) + shape_len;
   if (L->payload_len || L->unmeasured) hl += varint_len(tag_of(field, WT_LEN));
   if (L->payload_len) hl += varint_len(L->payload_len);
@@ -2586,3 +2526,4 @@ int b200tfs_padded_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_ou
 // ------------------------------------------------------------------------------------------------
 #include "varint_host.inc"
 #include "example_host.inc"
+#include "unpad_host.inc"

@@ -45,6 +45,7 @@
 #include "kernels.h"
 #include "plan.h"
 #include "tpl.h"
+#include "unpad.h"
 #include "example_walk.h"
 #include "walker.h"
 #include "wire.h"
@@ -1206,6 +1207,11 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
 // Classify / Regress responses: xr_index / xr_scan / xr_emit / xr_compare / xr_publish
 // ------------------------------------------------------------------------------------------------
 #include "example_resp_kernels.cuh"
+
+// ------------------------------------------------------------------------------------------------
+// PredictRequests cut out of padded tensors: unpad_plan / unpad_len / unpad_layout / unpad_frame / move / unpad_emit
+// ------------------------------------------------------------------------------------------------
+#include "unpad_kernels.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // frame_requests_kernel (plan.h "deferred framing"): one thread per request evaluates the request's values from the job

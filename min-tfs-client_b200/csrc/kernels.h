@@ -5,6 +5,7 @@
 
 #include "../../include/b200tfs.h"
 #include "plan.h"
+#include "unpad.h"
 
 namespace b200tfs {
 
@@ -53,5 +54,8 @@ cudaError_t launch_example_requests(const ExTables& T, cudaStream_t stream, uint
 // Classify / Regress responses (example_resp_kernels.cuh): index, scan, emit, [label compare,] publish; emit_ctas CTAs stride over
 // the rows; *launched receives how many kernels
 cudaError_t launch_example_responses(const XrTables& T, uint32_t emit_ctas, cudaStream_t stream, uint32_t* launched);
+// PredictRequests cut out of padded tensors (unpad_kernels.cuh): plan, [varint count,] layout, frame, move over move_grid CTAs (the
+// host's bound on the tiles), [varint emit]; *launched receives how many kernels
+cudaError_t launch_unpad(const UnpadPlan& up, uint32_t move_grid, cudaStream_t stream, uint32_t* launched);
 
 }  // namespace b200tfs

@@ -1,0 +1,296 @@
+// unpad_kernels.cuh - b200tfs_encode_padded_requests_async (unpad.h): n PredictRequests cut out of one padded tensor per input,
+// planned on the device.  Included by kernels.cu inside namespace b200tfs, after the move engine, the varint kernels and
+// concat_scan.  Launch order, no host step between them:
+//   unpad_plan_kernel    one CTA: every request's boxes from the shapes tables, rows block-scanned into first rows, statuses;
+//                        the packed-varint jobs and their tile table, counters zeroed
+//   unpad_len_kernel     the varint bytes of every tile (venc_len over the boxes; only with a packed-varint input)
+//   unpad_layout_kernel  one CTA: record lengths from the dims and payload lengths, a scan over the slots into rec_off, the
+//                        move plan (items with their final destinations, tile table), the varint jobs' destinations, results
+//   unpad_frame_kernel   one thread per request: the framing (framing.h writers through unpad_write)
+//   move_kernel          the fixed-width boxes over the plan image unpad_layout_kernel wrote
+//   unpad_emit_kernel    the varints (venc_emit over the boxes; only with a packed-varint input)
+
+// one element of `esz` bytes, widened like ldg_elem
+__device__ __forceinline__ uint64_t unpad_ld(const uint8_t* p, uint32_t esz, uint32_t sgn) {
+  switch (esz * 2 + (sgn ? 1 : 0)) {
+    case 2: return ldg_elem<1, false>(p);
+    case 3: return ldg_elem<1, true>(p);
+    case 4: return ldg_elem<2, false>(p);
+    case 5: return ldg_elem<2, true>(p);
+    case 8: return ldg_elem<4, false>(p);
+    case 9: return ldg_elem<4, true>(p);
+    default: return ldg_elem<8, false>(p);
+  }
+}
+
+// elements [e0, e0 + cnt) of a box, striped as load_striped loads them: a box that is one stretch of the source takes load_striped
+// itself; a box of several runs reads element k at its padded position
+__device__ __forceinline__ void unpad_load_striped(const UnpadIn& in, const UnpadBox& b, uint64_t e0, uint32_t cnt, uint64_t (&v)[kVarPerThread]) {
+  const uint8_t* base = in.src + b.src_off;
+  if (b.n_runs <= 1) { load_striped(base, e0, cnt, in.src_esz, in.is_signed, v); return; }
+#pragma unroll
+  for (uint32_t i = 0; i < kVarPerThread; ++i) {
+    const uint32_t k = i * kVarThreads + threadIdx.x;
+    v[i] = 0;
+    if (k < cnt) {
+      const uint64_t e = e0 + k, q = e / b.run;
+      v[i] = unpad_ld(base + (unpad_run_start(in, b, q) + (e - q * b.run)) * in.src_esz, in.src_esz, in.is_signed);
+    }
+  }
+}
+
+struct UnpadTile { UnpadIn in; UnpadBox b; VarJobDev jb; uint32_t s; };
+__device__ __forceinline__ void unpad_fetch(const UnpadPlan& up, uint32_t t, UnpadTile& T) {
+  T.s = up.tile_job[t];
+  T.jb = up.jobs[T.s];
+  const uint32_t r = T.s / up.n_var, j = up.var_in[T.s - r * up.n_var];
+  T.in = up.ins[j];
+  T.b = up.box[(size_t)r * up.F.n_in + j];
+}
+
+__global__ void __launch_bounds__(kConcatPlanThreads) unpad_plan_kernel(const __grid_constant__ UnpadPlan up) {
+  __shared__ unsigned long long warp_sum[kConcatPlanThreads / 32];
+  const uint32_t n = up.n, ni = up.F.n_in;
+  uint64_t row_carry[kUnpadMaxInputs];
+  for (uint32_t j = 0; j < kUnpadMaxInputs; ++j) row_carry[j] = 0;
+  __shared__ unsigned long long var_cut;    // first tile of the first job past the host's bound (never with it)
+  if (threadIdx.x == 0) var_cut = ~0ull;
+  __syncthreads();
+  uint64_t tile_carry = 0, group_carry = 0;
+  for (uint32_t r0 = 0; r0 < n; r0 += kConcatPlanThreads) {       // uniform trip counts: the scans have barriers inside
+    const uint32_t r = r0 + threadIdx.x;
+    const bool live = r < n;
+    int32_t st = B200TFS_OK;
+    for (uint32_t j = 0; j < ni; ++j) {
+      const UnpadIn& in = up.ins[j];
+      UnpadBox b{};
+      int32_t s = B200TFS_OK;
+      if (live) s = unpad_box(in, in.shapes ? in.shapes + (size_t)r * in.cols : nullptr, &b);
+      if (in.shapes) {
+        const uint64_t rows = live ? (uint64_t)b.dims[0] : 0;   // a bad trailing dim keeps its rows: the requests behind it stay put
+        const uint64_t first = concat_scan(rows, row_carry[j], warp_sum);
+        if (live && s == B200TFS_OK && first + rows > (uint64_t)in.dims[0]) s = B200TFS_E_SIZE;
+        uint64_t pitch = in.src_esz;
+        for (int32_t d = 1; d < in.rank; ++d) pitch *= (uint64_t)in.dims[d];
+        b.src_off = first * pitch;
+      }
+      if (live) {
+        if (st == B200TFS_OK) st = s;
+        up.box[(size_t)r * ni + j] = b;
+      }
+    }
+    if (live) up.st[r] = st;
+    for (uint32_t v = 0; v < up.n_var; ++v) {
+      const uint32_t j = up.var_in[v];
+      const uint64_t ne = (live && st == B200TFS_OK) ? up.box[(size_t)r * ni + j].n_elems : 0;
+      const uint64_t tiles = (ne + kVarTileElems - 1) / kVarTileElems, groups = (tiles + kVarGroupTiles - 1) / kVarGroupTiles;
+      const uint64_t first = concat_scan(tiles, tile_carry, warp_sum);
+      const uint64_t group0 = concat_scan(groups, group_carry, warp_sum);   // every job's counter groups apart from all others
+      // past the bound (never: unpad_bounds): tiles only grow in scan order, so such jobs are a suffix - their requests get
+      // B200TFS_E_SIZE, and the tile count stops at the first one
+      const bool over = first + tiles > up.var_tile_cap || group0 + groups > up.var_group_cap;
+      if (over) atomicMin(&var_cut, (unsigned long long)first);
+      if (live) {
+        const uint64_t s = (uint64_t)r * up.n_var + v;
+        if (over) { st = B200TFS_E_SIZE; up.st[r] = st; }
+        const UnpadIn& in = up.ins[j];
+        VarJobDev jb{};
+        jb.dst = up.arena;                       // parked until unpad_layout_kernel places the record
+        jb.n_elems = over ? 0 : ne;
+        jb.tile_val = up.tile_val + first;
+        jb.group_sum = up.group_sum + group0;
+        jb.total = up.total + s;
+        jb.dtype = in.wire_dtype;
+        jb.elem_size = in.src_esz;
+        jb.is_signed = in.is_signed;
+        jb.first_tile = (uint32_t)first;
+        jb.n_tiles = (uint32_t)tiles;
+        if (!over) {
+          for (uint64_t i = 0; i < tiles; ++i) up.tile_job[first + i] = (uint32_t)s;
+          for (uint64_t g = 0; g < groups; ++g) jb.group_sum[g] = 0;
+        }
+        *jb.total = 0;
+        up.jobs[s] = jb;
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) *up.n_var_tiles = (uint32_t)min(min(tile_carry, (uint64_t)var_cut), (uint64_t)up.var_tile_cap);
+}
+
+__global__ void __launch_bounds__(kVarThreads) unpad_len_kernel(const __grid_constant__ UnpadPlan up) {
+  __shared__ VarShared sh;
+  const uint32_t t = blockIdx.x;
+  if (t >= *up.n_var_tiles) return;
+  UnpadTile T;
+  unpad_fetch(up, t, T);
+  const uint64_t e0 = (uint64_t)(t - T.jb.first_tile) * kVarTileElems;
+  const uint32_t cnt = (uint32_t)min((uint64_t)kVarTileElems, T.jb.n_elems - e0);
+  uint64_t v[kVarPerThread];
+  unpad_load_striped(T.in, T.b, e0, cnt, v);
+  uint32_t sum = 0;
+#pragma unroll
+  for (uint32_t i = 0; i < kVarPerThread; ++i) sum += vlen64(v[i]) & ((i * kVarThreads + threadIdx.x < cnt) ? ~0u : 0u);
+  const uint32_t total = block_sum_t0(sum, sh);
+  if (threadIdx.x == 0) publish_tile(T.jb, t - T.jb.first_tile, total);
+}
+
+// fixed-width moves of one (request, input): one item for a box that is one stretch of the source (the engine's vector path), else
+// one gathered item per index of the axes above lo - 1, each a row of dims[lo - 1] pieces of `run` elements
+struct UnpadItems { uint64_t items, per_item_runs, item_bytes; uint32_t tiles_per_item; };
+__device__ __forceinline__ UnpadItems unpad_items(const UnpadIn& in, const UnpadBox& b, uint32_t vpt) {
+  UnpadItems I{0, 0, 0, 0};
+  if (in.varint || !b.n_elems) return I;
+  I.per_item_runs = b.n_runs <= 1 ? 1 : (uint64_t)b.dims[b.lo - 1];
+  I.items = b.n_runs <= 1 ? 1 : b.n_runs / I.per_item_runs;
+  I.item_bytes = I.per_item_runs * b.run * in.wire_esz;
+  I.tiles_per_item = tiles_for(I.item_bytes, vpt);
+  return I;
+}
+
+__global__ void __launch_bounds__(kConcatPlanThreads) unpad_layout_kernel(const __grid_constant__ UnpadPlan up) {
+  __shared__ unsigned long long warp_sum[kConcatPlanThreads / 32];
+  const uint32_t n = up.n, ni = up.F.n_in;
+  const PlanGeometry g = plan_geometry(up.item_cap, up.tile_cap, 0);
+  MoveItem* items = reinterpret_cast<MoveItem*>(up.plan + g.off_items);
+  TileRef* tref = reinterpret_cast<TileRef*>(up.plan + g.off_tiles);
+  __shared__ unsigned long long tile_cut;   // first tile of the first request past the host's bounds (never with them)
+  if (threadIdx.x == 0) tile_cut = ~0ull;
+  __syncthreads();
+  uint64_t slot_carry = 0, item_carry = 0, tile_carry = 0;
+  for (uint32_t r0 = 0; r0 < n; r0 += kConcatPlanThreads) {
+    const uint32_t r = r0 + threadIdx.x;
+    const bool live = r < n;
+    int32_t st = live ? up.st[r] : B200TFS_E_ARG;
+    UnpadBox* B = up.box + (size_t)r * ni;
+    uint64_t poff[kUnpadMaxInputs];
+    uint64_t len = 0, largest_off = 0, n_items = 0, n_tiles = 0;
+    if (st == B200TFS_OK) {
+      for (uint32_t j = 0, v = 0; j < ni; ++j) {
+        const UnpadIn& in = up.ins[j];
+        const uint64_t ne = B[j].n_elems;
+        B[j].payload = in.varint ? (ne ? (uint64_t)up.total[(size_t)r * up.n_var + v] : 0) : ne * in.wire_esz;
+        v += in.varint;
+      }
+      int32_t s2;
+      len = unpad_layout(up.F, up.ins, B, poff, &largest_off, &s2);
+      st = s2;
+    }
+    const uint64_t pad = (128 - (largest_off & 127)) & 127;
+    const uint64_t slot = st == B200TFS_OK ? (pad + len + 255) & ~255ull : 0;
+    const uint64_t at = concat_scan(slot, slot_carry, warp_sum);
+    if (st == B200TFS_OK && at + pad + len > up.arena_cap) st = B200TFS_E_SIZE;   // never with b200tfs_padded_request_arena_size bytes
+    if (st == B200TFS_OK)
+      for (uint32_t j = 0; j < ni; ++j) {
+        const UnpadItems I = unpad_items(up.ins[j], B[j], up.vpt);
+        n_items += I.items;
+        n_tiles += I.items * I.tiles_per_item;
+      }
+    const uint64_t first_item = concat_scan(n_items, item_carry, warp_sum);
+    const uint64_t first_tile = concat_scan(n_tiles, tile_carry, warp_sum);
+    if (!live) continue;
+    // Past the host's bounds (never: unpad_bounds).  Item and tile starts only grow, so the requests past them are a suffix: they get
+    // B200TFS_E_SIZE and no moves, and the plan stops at the first one's tiles - every tile in front of it has its reference written.
+    if (first_item + n_items > up.item_cap || first_tile + n_tiles > up.tile_cap) {
+      st = B200TFS_E_SIZE;
+      atomicMin(&tile_cut, (unsigned long long)first_tile);
+    }
+    const uint64_t rec = at + pad;
+    if (st == B200TFS_OK) {
+      uint64_t it = first_item, tt = first_tile;
+      for (uint32_t j = 0, v = 0; j < ni; ++j) {
+        const UnpadIn& in = up.ins[j];
+        const UnpadBox& b = B[j];
+        uint8_t* dst = up.arena + rec + poff[j];
+        if (in.varint) {
+          VarJobDev& jb = up.jobs[(size_t)r * up.n_var + v];
+          jb.dst = dst; jb.cap = b.payload;
+          ++v;
+          continue;
+        }
+        const UnpadItems I = unpad_items(in, b, up.vpt);
+        uint64_t pitch = in.src_esz;      // source bytes of one index of axis lo - 1
+        for (int32_t d = (int32_t)b.lo; d < in.rank; ++d) pitch *= (uint64_t)in.dims[d];
+        for (uint64_t k = 0; k < I.items; ++k, ++it) {
+          const uint8_t* src = in.src + b.src_off + unpad_run_start(in, b, k * I.per_item_runs) * in.src_esz;
+          const bool gather = b.n_runs > 1;
+          items[it] = MoveItem{src, dst + k * I.item_bytes, I.item_bytes, in.op, I.tiles_per_item,
+                               gather ? (uint32_t)(b.run * in.src_esz) : 0u, gather ? (uint32_t)pitch : 0u};
+          for (uint32_t q = 0; q < I.tiles_per_item; ++q) tref[tt++] = TileRef{(uint32_t)it, q};
+        }
+      }
+    } else {
+      for (uint32_t v = 0; v < up.n_var; ++v) { VarJobDev& jb = up.jobs[(size_t)r * up.n_var + v]; jb.dst = up.arena; jb.cap = 0; }
+    }
+    up.st[r] = st;
+    up.rec_off[r] = st == B200TFS_OK ? rec : 0;
+    up.rec_off[n + r] = st == B200TFS_OK ? len : 0;
+    up.rec_off_host[r] = st == B200TFS_OK ? rec : 0;
+    up.rec_len_host[r] = st == B200TFS_OK ? len : 0;
+    up.status_host[r] = st;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    PlanHeader ph{};
+    ph.n_items = up.item_cap;
+    ph.n_tiles = (uint32_t)min(min(tile_carry, (uint64_t)tile_cut), (uint64_t)up.tile_cap);
+    ph.vec_per_tile = up.vpt;
+    ph.off_items = (uint32_t)g.off_items;
+    ph.off_tiles = (uint32_t)g.off_tiles;
+    ph.off_small = (uint32_t)g.off_small;
+    ph.guard_div = 1;
+    *reinterpret_cast<PlanHeader*>(up.plan) = ph;
+  }
+}
+
+__global__ void __launch_bounds__(kUnpadFrameThreads) unpad_frame_kernel(const __grid_constant__ UnpadPlan up) {
+  const uint32_t r = blockIdx.x * kUnpadFrameThreads + threadIdx.x;
+  if (r >= up.n || up.st[r] != B200TFS_OK) return;
+  RawOut o{up.arena + up.rec_off[r]};
+  unpad_write(o, up.F, up.ins, up.box + (size_t)r * up.F.n_in, up.rec_off[up.n + r] - (up.F.grpc ? 5 : 0), nullptr);
+}
+
+// a box as the source of encode tiles: one stretch of the padded tensor goes through venc_load_tile itself, a box of several runs
+// through the same transpose with the striped elements read at their padded positions
+struct BoxSrc {
+  const UnpadTile& T;
+  __device__ __forceinline__ uint32_t load_tile(uint8_t* smem, const VarJobDev& jb, uint64_t e0, uint32_t cnt, uint64_t (&mine)[kVarPerThread],
+                                                uint32_t& lens) const {
+    if (T.b.n_runs <= 1) {
+      const VarSeg sg{T.in.src + T.b.src_off, jb.n_elems, T.s, jb.first_tile};
+      return venc_load_tile(smem, sg, jb, e0, cnt, mine, lens);
+    }
+    uint64_t v[kVarPerThread];
+    unpad_load_striped(T.in, T.b, e0, cnt, v);
+    return venc_block_tile(smem, cnt, v, mine, lens);
+  }
+};
+
+__global__ void __launch_bounds__(kVarThreads, 5) unpad_emit_kernel(const __grid_constant__ UnpadPlan up) {
+  __shared__ __align__(16) uint8_t smem[kVarImageBytes];
+  __shared__ VarShared sh;
+  const uint32_t t = blockIdx.x;
+  if (t >= *up.n_var_tiles) return;
+  UnpadTile T;
+  unpad_fetch(up, t, T);
+  const uint32_t t_rel = t - T.jb.first_tile;
+  const uint64_t e0 = (uint64_t)t_rel * kVarTileElems;
+  const uint32_t cnt = (uint32_t)min((uint64_t)kVarTileElems, T.jb.n_elems - e0);
+  venc_emit_tile(smem, sh, T.jb, t_rel, e0, cnt, BoxSrc{T});
+}
+
+cudaError_t launch_unpad(const UnpadPlan& up, uint32_t move_grid, cudaStream_t stream, uint32_t* launched) {
+  *launched = 0;
+  if (!up.n) return cudaSuccess;
+  const uint32_t var_grid = up.n_var ? up.var_tile_cap : 0;
+  unpad_plan_kernel<<<1, kConcatPlanThreads, 0, stream>>>(up);
+  ++*launched;
+  if (var_grid) { unpad_len_kernel<<<var_grid, kVarThreads, 0, stream>>>(up); ++*launched; }
+  unpad_layout_kernel<<<1, kConcatPlanThreads, 0, stream>>>(up);
+  unpad_frame_kernel<<<(up.n + kUnpadFrameThreads - 1) / kUnpadFrameThreads, kUnpadFrameThreads, 0, stream>>>(up);
+  *launched += 2;
+  // a plain launch, as in launch_concat_plan: the kernel in front of move_kernel writes its plan header
+  if (move_grid) { move_kernel<<<move_grid, kMoveThreads, 0, stream>>>((const uint8_t*)up.plan); ++*launched; }
+  if (var_grid) { unpad_emit_kernel<<<var_grid, kVarThreads, 0, stream>>>(up); ++*launched; }
+  return cudaGetLastError();
+}

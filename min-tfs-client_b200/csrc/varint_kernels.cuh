@@ -175,6 +175,37 @@ __device__ __forceinline__ uint32_t spread28(uint32_t x) {
 // consecutive elements; the staging image reuses the same shared memory.
 constexpr uint32_t kVarImageBytes = kVarTileElems * 10 + 48;
 
+// The tile's elements, blocked through shared memory: the thread's striped elements (element i * kVarThreads + tid of the tile in
+// v[i], as load_striped loads them) are transposed (16-byte chunks XOR-swizzled by row) so that thread r owns
+// elements [8r, 8r+8); `lens` and the return value as venc_load_tile gives them.  One barrier inside.
+__device__ __forceinline__ uint32_t venc_block_tile(uint8_t* smem, uint32_t cnt, const uint64_t (&v)[kVarPerThread], uint64_t (&mine)[kVarPerThread],
+                                                    uint32_t& lens) {
+  const uint32_t r = threadIdx.x;
+  uint64_t* vals = reinterpret_cast<uint64_t*>(smem);
+  {
+#pragma unroll
+    for (uint32_t i = 0; i < kVarPerThread; ++i) {
+      const uint32_t k = i * kVarThreads + threadIdx.x, r = k >> 3, c = k & 7;
+      vals[r * 8 + ((((c >> 1) ^ (r >> 1)) & 3) << 1) + (c & 1)] = v[i];
+    }
+  }
+  __syncthreads();
+#pragma unroll
+  for (uint32_t j = 0; j < kVarPerThread / 2; ++j) {
+    const uint4 q = *reinterpret_cast<const uint4*>(smem + r * 64 + (((j ^ (r >> 1)) & 3) << 4));
+    mine[2 * j] = (uint64_t)q.x | ((uint64_t)q.y << 32);
+    mine[2 * j + 1] = (uint64_t)q.z | ((uint64_t)q.w << 32);
+  }
+  lens = 0;
+#pragma unroll
+  for (uint32_t i = 0; i < kVarPerThread; ++i) lens |= vlen64(mine[i]) << (4 * i);
+  // elements past the end of the tensor (last tile only) take no room
+  const uint32_t have = min(kVarPerThread, cnt - min(cnt, r * kVarPerThread));
+  lens &= __funnelshift_lc(0xFFFFFFFFu, 0u, 4u * have);
+  const uint32_t pairs = (lens & 0x0F0F0F0Fu) + ((lens >> 4) & 0x0F0F0F0Fu);
+  return (pairs * 0x01010101u) >> 24;
+}
+
 // the tile's elements, blocked: thread r owns elements [8r, 8r+8) of the tile; `lens` = their varint lengths, one nibble each
 // (elements past the end of the tensor: 0); returns the thread's byte count.  One barrier inside.
 __device__ __forceinline__ uint32_t venc_load_tile(uint8_t* smem, const VarSeg& sg, const VarJobDev& jb, uint64_t e0, uint32_t cnt,
@@ -210,31 +241,9 @@ __device__ __forceinline__ uint32_t venc_load_tile(uint8_t* smem, const VarSeg& 
     const uint32_t pairs = (lens & 0x0F0F0F0Fu) + ((lens >> 4) & 0x0F0F0F0Fu);
     return (pairs * 0x01010101u) >> 24;
   }
-  uint64_t* vals = reinterpret_cast<uint64_t*>(smem);
-  {
-    uint64_t v[kVarPerThread];
-    load_striped(sg.src, e0, cnt, jb.elem_size, jb.is_signed, v);
-#pragma unroll
-    for (uint32_t i = 0; i < kVarPerThread; ++i) {
-      const uint32_t k = i * kVarThreads + threadIdx.x, r = k >> 3, c = k & 7;
-      vals[r * 8 + ((((c >> 1) ^ (r >> 1)) & 3) << 1) + (c & 1)] = v[i];
-    }
-  }
-  __syncthreads();
-#pragma unroll
-  for (uint32_t j = 0; j < kVarPerThread / 2; ++j) {
-    const uint4 q = *reinterpret_cast<const uint4*>(smem + r * 64 + (((j ^ (r >> 1)) & 3) << 4));
-    mine[2 * j] = (uint64_t)q.x | ((uint64_t)q.y << 32);
-    mine[2 * j + 1] = (uint64_t)q.z | ((uint64_t)q.w << 32);
-  }
-  lens = 0;
-#pragma unroll
-  for (uint32_t i = 0; i < kVarPerThread; ++i) lens |= vlen64(mine[i]) << (4 * i);
-  // elements past the end of the tensor (last tile only) take no room
-  const uint32_t have = min(kVarPerThread, cnt - min(cnt, r * kVarPerThread));
-  lens &= __funnelshift_lc(0xFFFFFFFFu, 0u, 4u * have);
-  const uint32_t pairs = (lens & 0x0F0F0F0Fu) + ((lens >> 4) & 0x0F0F0F0Fu);
-  return (pairs * 0x01010101u) >> 24;
+  uint64_t v[kVarPerThread];
+  load_striped(sg.src, e0, cnt, jb.elem_size, jb.is_signed, v);
+  return venc_block_tile(smem, cnt, v, mine, lens);
 }
 
 // build the thread's varints in registers and append them, whole 32-bit words at a time, to the shared-memory image at byte
@@ -311,6 +320,39 @@ __device__ __forceinline__ void venc_build_image(uint8_t* smem, const uint64_t (
       if (b >= first && b < f) tail[b] = (uint8_t)(acc >> (8 * b));
   }
   __syncthreads();
+}
+
+// One encode tile of job `jb`: tile t_rel of the job, elements [e0, e0 + cnt) of its source.  The offset comes from the counters,
+// `src.load_tile` (a source's tile load; returns the thread's byte count) fills the registers, then the image and the stores - the
+// body of venc_emit_kernel for a source other than a contiguous segment.  (venc_emit_kernel keeps its own copy: built on this
+// template its stack grew from 56 to 80 bytes and its spills with it.)
+template <class Src>
+__device__ __forceinline__ void venc_emit_tile(uint8_t* smem, VarShared& sh, const VarJobDev& jb, uint32_t t_rel, uint64_t e0, uint32_t cnt,
+                                               const Src& src) {
+  const uint64_t share = prefix_share(jb, t_rel);
+  uint64_t mine[kVarPerThread];
+  uint32_t lens;
+  const uint32_t sum = src.load_tile(smem, jb, e0, cnt, mine, lens);
+  uint32_t total;
+  uint64_t base;
+  uint32_t off = block_scan_sum(sum, &total, share, &base, sh);   // every thread has read its elements before the first barrier inside
+  uint8_t* g = jb.dst + base;                  // first output byte of this tile
+  const uint32_t phase = (uint32_t)((uintptr_t)g & 15);
+  venc_build_image(smem, mine, lens, off + phase);
+  // smem[phase .. phase+total) -> g[0 .. total); whole 16-byte vectors where the tile owns them.  Never past the
+  // payload the header announced (the data changed between b200tfs_measure and the encode: undefined bytes, no overrun)
+  if (base >= jb.cap) return;
+  total = (uint32_t)min((uint64_t)total, jb.cap - base);
+  uint8_t* gbase = g - phase;  // 16-byte aligned
+  const uint32_t lo = phase, hi = phase + total;
+  const uint32_t v_lo = (lo + 15) >> 4, v_hi = hi >> 4;
+  if (v_lo < v_hi) {
+    for (uint32_t v = v_lo + threadIdx.x; v < v_hi; v += kVarThreads) st_stream(gbase + 16 * v, reinterpret_cast<const uint4*>(smem)[v]);
+    for (uint32_t i = lo + threadIdx.x; i < v_lo * 16; i += kVarThreads) gbase[i] = smem[i];
+    for (uint32_t i = v_hi * 16 + threadIdx.x; i < hi; i += kVarThreads) gbase[i] = smem[i];
+  } else {
+    for (uint32_t i = lo + threadIdx.x; i < hi; i += kVarThreads) gbase[i] = smem[i];
+  }
 }
 
 __global__ void __launch_bounds__(kVarThreads, 5) venc_emit_kernel(const __grid_constant__ VarTables tb) {

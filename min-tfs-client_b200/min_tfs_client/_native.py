@@ -115,6 +115,11 @@ class ExampleRequest(C.Structure):
     ]
 
 
+class PadInput(C.Structure):
+    """b200tfs_pad_input: the shapes of one input of b200tfs_encode_padded_requests_async (int64[n, cols]; cols 1: row counts)."""
+    _fields_ = [("shapes", C.c_void_p), ("cols", C.c_int32), ("pad_", C.c_int32)]
+
+
 RESP_REGRESS, RESP_CLASSIFY = 1, 2
 
 
@@ -186,6 +191,9 @@ SIGNATURES = {
     "b200tfs_decode_padded": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey)]),
     "b200tfs_decode_padded_host_async": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey)]),
     "b200tfs_padded_results": (C.c_int, [_vp, C.c_int32, C.c_int32, C.POINTER(Output), C.POINTER(ModelSpec), _i32p]),
+    "b200tfs_padded_request_arena_size": (C.c_int, [C.c_int32, C.POINTER(Request), _u64p]),
+    "b200tfs_encode_padded_requests_async": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), C.POINTER(PadInput), _vp, C.c_uint64]),
+    "b200tfs_padded_request_frame": (C.c_int, [C.POINTER(Request), C.POINTER(PadInput), _u64p, _vp, C.c_uint64, _u64p, _u64p, _u64p]),
     "b200tfs_capture_begin": (C.c_int, [_vp]),
     "b200tfs_capture_end": (C.c_int, [_vp, _vpp]),
     "b200tfs_graph_launch": (C.c_int, [_vp, _vp]),

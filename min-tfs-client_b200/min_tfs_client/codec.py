@@ -361,12 +361,18 @@ class Codec:
         self.concat_device_calls = 0
         # decode_predict_responses_padded calls the device route finished
         self.padded_device_calls = 0
+        # encode_predict_requests_padded calls the device route finished
+        self.padded_encode_device_calls = 0
+        self._pe_arena = None         # their device arena (grows)
         # decode_regression_responses / decode_classification_responses calls the device route finished
         self.example_response_device_calls = 0
         self._xr_scratch = None       # their device destinations when the result goes to host memory: (values, labels)
 
     def close(self):
         if getattr(self, "_ctx", None):
+            if self._pe_arena is not None:
+                self._pe_arena.free()
+                self._pe_arena = None
             self._lib.b200tfs_destroy(self._ctx)
             self._ctx = None
             self._pinned.release()
@@ -503,6 +509,149 @@ class Codec:
         wire = np.empty(cap, dtype=np.uint8)
         N.check(self._lib.b200tfs_encode_requests_host(self._ctx, n, reqs, wire.ctypes.data, cap, off, ln))
         return [wire[off[i]: off[i] + ln[i]].tobytes() for i in range(n)]
+
+    def encode_predict_requests_padded(self, model_name: str, inputs: Mapping, shapes: Mapping, *, model_version: Optional[int] = None,
+                                       broadcast: Optional[Mapping] = None, order="deterministic", wire_dtype=None,
+                                       tensor_content: bool = False, keep_snan: bool = False, grpc_frame: bool = False,
+                                       out=None) -> List[bytes]:
+        """n PredictRequests cut out of one padded tensor per input - the inverse of ``decode_predict_responses_padded``.
+
+        ``inputs[key]`` is a padded tensor ``P`` of shape ``[R, D_1, ..., D_{m-1}]``; ``shapes[key]`` gives each request's shape for it,
+        ``int64[n, m]``, or ``int64[n]`` row counts (every trailing dim full).  Request r gets ``P[r0:r0 + S[r,0], :S[r,1], ...,
+        :S[r,m-1]]`` with ``r0 = S[:r, 0].sum()``, plus every ``broadcast`` tensor as it is; its bytes are what
+        ``encode_predict_request`` returns for that request.  Inputs and shapes may be numpy arrays (pageable or ``pinned_empty``) or
+        device arrays (``__cuda_array_interface__`` / DLPack); device shapes never travel to the host - the rows, boxes and framing
+        are planned by kernels.  A negative dim, a trailing dim past ``D_j``, a shape of another rank, rows past ``R`` or a request
+        count that differs between keys raise ValueError.  DT_STRING inputs, more than 8 padded or 8 broadcast inputs and ranks
+        above 16 are cut on the host and encoded request by request.  ``out="pinned"`` as for ``encode_predict_requests``.
+        """
+        if out is not None and out != "pinned":
+            raise ValueError('out must be None or "pinned"')
+        broadcast = dict(broadcast or {})
+        if set(inputs) != set(shapes):
+            raise ValueError("shapes must have exactly the keys of inputs")
+        if set(inputs) & set(broadcast):
+            raise ValueError("a key cannot be both padded and broadcast")
+        pdims = {k: tuple(D.device_view(v)[1]) if D.is_device_object(v) else np.shape(v) for k, v in inputs.items()}
+        n = None
+        host_shapes = {}
+        for k, s in shapes.items():
+            m = len(pdims[k])
+            if m < 1:
+                raise ValueError(f"input {k!r}: a padded tensor has rank >= 1")
+            shp = tuple(D.device_view(s)[1]) if D.is_device_object(s) else np.shape(s)
+            if len(shp) not in (1, 2) or (len(shp) == 2 and shp[1] != m):
+                raise ValueError(f"shapes of {k!r}: expected int64[n, {m}] or int64[n], got {shp}")
+            if n is not None and shp[0] != n:
+                raise ValueError(f"shapes of {k!r} give {shp[0]} requests, another key {n}")
+            n = shp[0]
+            if not D.is_device_object(s):
+                a = np.asarray(s)
+                if a.dtype.kind not in "iu":
+                    raise ValueError(f"shapes of {k!r} must be integers")
+                a = a.astype(np.int64).reshape(n, -1)
+                if (a < 0).any():
+                    raise ValueError(f"shapes of {k!r}: negative dim")
+                if a.shape[1] > 1 and (a[:, 1:] > np.asarray(pdims[k][1:], dtype=np.int64)).any():
+                    raise ValueError(f"shapes of {k!r}: a trailing dim exceeds the padded tensor's {pdims[k][1:]}")
+                if int(a[:, 0].sum()) > pdims[k][0]:
+                    raise ValueError(f"shapes of {k!r}: {int(a[:, 0].sum())} rows of {pdims[k][0]}")
+                host_shapes[k] = a
+        if not n:
+            return []
+        dtypes = [D.device_view(v)[2] if D.is_device_object(v) else np.asarray(v).dtype for v in list(inputs.values()) + list(broadcast.values())]
+        ranks = list(pdims.values()) + [tuple(D.device_view(v)[1]) if D.is_device_object(v) else np.shape(v) for v in broadcast.values()]
+        if (any(dt.kind in "OUS" for dt in dtypes) or len(inputs) > N.CONCAT_MAX_KEYS or len(broadcast) > N.CONCAT_MAX_KEYS
+                or any(len(r) > N.MAX_RANK for r in ranks)):
+            return self._padded_requests_on_host(model_name, model_version, inputs, shapes, broadcast, n, order=order, wire_dtype=wire_dtype,
+                                                 tensor_content=tensor_content, keep_snan=keep_snan, grpc_frame=grpc_frame, out=out)
+        keep = []
+
+        def dev(v):
+            if D.is_device_object(v):
+                return v
+            a = np.asarray(v)
+            if not a.dtype.isnative:
+                a = a.astype(a.dtype.newbyteorder("="))
+            d = self.device_array(a)
+            keep.append(d)
+            return d
+
+        preps, pins = [], []
+        for k, v in list(inputs.items()) + list(broadcast.items()):
+            kb = k.encode("utf-8") if isinstance(k, str) else bytes(k)
+            wd = wire_dtype.get(k) if isinstance(wire_dtype, Mapping) else wire_dtype
+            p = _Prepared(dev(v), kb, wd, tensor_content, keep_snan)
+            if k in broadcast:
+                p.struct.flags |= N.F_BROADCAST
+                pins.append(N.PadInput(shapes=None, cols=0))
+            else:
+                s = shapes[k]
+                sd = dev(host_shapes[k]) if k in host_shapes else s
+                ptr, shp, sdt, hold = D.device_view(sd)
+                if sdt != np.int64:
+                    raise ValueError(f"device shapes of {k!r} must be int64")
+                keep.append(hold)
+                pins.append(N.PadInput(shapes=ptr, cols=shp[1] if len(shp) == 2 else 1))
+            preps.append(p)
+        arr = (N.Tensor * len(preps))(*[p.struct for p in preps])
+        pin_arr = (N.PadInput * len(pins))(*pins)
+        name = model_name.encode("utf-8") if isinstance(model_name, str) else bytes(model_name)
+        order_code = _ORDER[order] if isinstance(order, str) else int(order)
+        req = N.Request(model_name=name, model_name_len=len(name), has_version=int(model_version is not None), order=order_code,
+                        version=int(model_version) if model_version is not None else 0, n_inputs=len(preps),
+                        flags=N.RF_GRPC_FRAME if grpc_frame else 0, inputs=arr)
+        cap = C.c_uint64()
+        N.check(self._lib.b200tfs_padded_request_arena_size(n, C.byref(req), C.byref(cap)))
+        if self._pe_arena is None or self._pe_arena.nbytes < cap.value:
+            if self._pe_arena is not None:
+                self._pe_arena.free()
+            self._pe_arena = D.DeviceArray(self, (max(int(cap.value), 1),), np.uint8)
+        N.check(self._lib.b200tfs_encode_padded_requests_async(self._ctx, n, C.byref(req), pin_arr, self._pe_arena.ptr, cap.value))
+        off, ln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
+        rc = self._lib.b200tfs_encode_results(self._ctx, n, off, ln)
+        if rc in (N.E_SHAPE, N.E_SIZE):
+            raise ValueError(N.last_error())
+        N.check(rc)
+        end = max(int(off[i]) + int(ln[i]) for i in range(n))
+        pw = self._pinned_wire(end)
+        if end:
+            N.check(self._lib.b200tfs_memcpy_d2h(self._ctx, pw.ptr, self._pe_arena.ptr, end))
+        self.sync()
+        self.padded_encode_device_calls += 1
+        if out == "pinned":
+            return [pw.array[off[i]: off[i] + ln[i]] for i in range(n)]
+        return [pw.array[off[i]: off[i] + ln[i]].tobytes() for i in range(n)]
+
+    def _to_host(self, v) -> np.ndarray:
+        if not D.is_device_object(v):
+            return np.asarray(v)
+        ptr, shape, dtype, _hold = D.device_view(v)
+        a = np.empty(shape, dtype=dtype)
+        if a.nbytes:
+            N.check(self._lib.b200tfs_memcpy_d2h(self._ctx, a.ctypes.data, ptr, a.nbytes))
+            self.sync()
+        return a
+
+    def _padded_requests_on_host(self, model_name, model_version, inputs, shapes, broadcast, n, **kw) -> List[bytes]:
+        """The definition of ``encode_predict_requests_padded``, run on the host: each request's boxes sliced, then encoded."""
+        P = {k: self._to_host(v) for k, v in inputs.items()}
+        S = {k: self._to_host(s).astype(np.int64).reshape(n, -1) for k, s in shapes.items()}
+        B = {k: self._to_host(v) for k, v in broadcast.items()}
+        for k, s in S.items():
+            if (s < 0).any() or (s.shape[1] > 1 and (s[:, 1:] > np.asarray(P[k].shape[1:])).any()) or int(s[:, 0].sum()) > P[k].shape[0]:
+                raise ValueError(f"shapes of {k!r} do not fit the padded tensor {P[k].shape}")
+        r0 = {k: np.concatenate([[0], np.cumsum(s[:, 0])]) for k, s in S.items()}
+        reqs = []
+        for r in range(n):
+            d = {}
+            for k, p in P.items():
+                s = S[k][r]
+                box = (slice(int(r0[k][r]), int(r0[k][r]) + int(s[0])),) + tuple(slice(0, int(x)) for x in s[1:])
+                d[k] = p[box]
+            d.update(B)
+            reqs.append((model_name, model_version, d))
+        return self.encode_predict_requests(reqs, **kw)
 
     def encode_predict_request(self, model_name: str, input_dict: Mapping, model_version: Optional[int] = None, **kw) -> bytes:
         return self.encode_predict_requests([(model_name, model_version, input_dict)], **kw)[0]
