@@ -3,49 +3,48 @@
 // concat_scan.  Launch order, no host step between them:
 //   unpad_plan_kernel    one CTA: every request's boxes from the shapes tables, rows block-scanned into first rows, statuses;
 //                        the packed-varint jobs and their tile table, counters zeroed
-//   unpad_len_kernel     the varint bytes of every tile (venc_len over the boxes; only with a packed-varint input)
+//   unpad_len_kernel     the varint bytes of every tile (venc_len_tile over the boxes; only with a packed-varint input)
 //   unpad_layout_kernel  one CTA: record lengths from the dims and payload lengths, a scan over the slots into rec_off, the
 //                        move plan (items with their final destinations, tile table), the varint jobs' destinations, results
 //   unpad_frame_kernel   one thread per request: the framing (framing.h writers through unpad_write)
 //   move_kernel          the fixed-width boxes over the plan image unpad_layout_kernel wrote
-//   unpad_emit_kernel    the varints (venc_emit over the boxes; only with a packed-varint input)
+//   unpad_emit_kernel    the varints (venc_emit_tile over the boxes; only with a packed-varint input)
 
-// one element of `esz` bytes, widened like ldg_elem
-__device__ __forceinline__ uint64_t unpad_ld(const uint8_t* p, uint32_t esz, uint32_t sgn) {
-  switch (esz * 2 + (sgn ? 1 : 0)) {
-    case 2: return ldg_elem<1, false>(p);
-    case 3: return ldg_elem<1, true>(p);
-    case 4: return ldg_elem<2, false>(p);
-    case 5: return ldg_elem<2, true>(p);
-    case 8: return ldg_elem<4, false>(p);
-    case 9: return ldg_elem<4, true>(p);
-    default: return ldg_elem<8, false>(p);
-  }
-}
+// a box as the source of encode tiles (SegSrc, varint_kernels.cuh): a box that is one stretch of the padded tensor is a segment; a box
+// of several runs reads each element at its padded position and goes through the same transpose
+struct BoxSrc {
+  UnpadIn in;
+  UnpadBox b;
 
-// elements [e0, e0 + cnt) of a box, striped as load_striped loads them: a box that is one stretch of the source takes load_striped
-// itself; a box of several runs reads element k at its padded position
-__device__ __forceinline__ void unpad_load_striped(const UnpadIn& in, const UnpadBox& b, uint64_t e0, uint32_t cnt, uint64_t (&v)[kVarPerThread]) {
-  const uint8_t* base = in.src + b.src_off;
-  if (b.n_runs <= 1) { load_striped(base, e0, cnt, in.src_esz, in.is_signed, v); return; }
+  __device__ __forceinline__ SegSrc seg() const { return SegSrc{in.src + b.src_off, in.src_esz, in.is_signed}; }
+  __device__ __forceinline__ void load_striped(uint64_t e0, uint32_t cnt, uint64_t (&v)[kVarPerThread]) const {
+    if (b.n_runs <= 1) { seg().load_striped(e0, cnt, v); return; }
+    const uint8_t* base = in.src + b.src_off;
 #pragma unroll
-  for (uint32_t i = 0; i < kVarPerThread; ++i) {
-    const uint32_t k = i * kVarThreads + threadIdx.x;
-    v[i] = 0;
-    if (k < cnt) {
-      const uint64_t e = e0 + k, q = e / b.run;
-      v[i] = unpad_ld(base + (unpad_run_start(in, b, q) + (e - q * b.run)) * in.src_esz, in.src_esz, in.is_signed);
+    for (uint32_t i = 0; i < kVarPerThread; ++i) {
+      const uint32_t k = i * kVarThreads + threadIdx.x;
+      v[i] = 0;
+      if (k < cnt) {
+        const uint64_t e = e0 + k, q = e / b.run;
+        v[i] = ldg_elem_rt(base + (unpad_run_start(in, b, q) + (e - q * b.run)) * in.src_esz, in.src_esz, in.is_signed);
+      }
     }
   }
-}
+  __device__ __forceinline__ uint32_t load_tile(uint8_t* smem, uint64_t e0, uint32_t cnt, uint64_t (&mine)[kVarPerThread], uint32_t& lens) const {
+    if (b.n_runs <= 1) return seg().load_tile(smem, e0, cnt, mine, lens);
+    uint64_t v[kVarPerThread];
+    load_striped(e0, cnt, v);
+    return venc_block_tile(smem, cnt, v, mine, lens);
+  }
+};
 
-struct UnpadTile { UnpadIn in; UnpadBox b; VarJobDev jb; uint32_t s; };
-__device__ __forceinline__ void unpad_fetch(const UnpadPlan& up, uint32_t t, UnpadTile& T) {
-  T.s = up.tile_job[t];
-  T.jb = up.jobs[T.s];
-  const uint32_t r = T.s / up.n_var, j = up.var_in[T.s - r * up.n_var];
-  T.in = up.ins[j];
-  T.b = up.box[(size_t)r * up.F.n_in + j];
+// the job of packed-varint tile t, and its box
+__device__ __forceinline__ void unpad_fetch(const UnpadPlan& up, uint32_t t, VarJobDev& jb, BoxSrc& src) {
+  const uint32_t s = up.tile_job[t];
+  jb = up.jobs[s];
+  const uint32_t r = s / up.n_var, j = up.var_in[s - r * up.n_var];
+  src.in = up.ins[j];
+  src.b = up.box[(size_t)r * up.F.n_in + j];
 }
 
 __global__ void __launch_bounds__(kConcatPlanThreads) unpad_plan_kernel(const __grid_constant__ UnpadPlan up) {
@@ -122,17 +121,12 @@ __global__ void __launch_bounds__(kVarThreads) unpad_len_kernel(const __grid_con
   __shared__ VarShared sh;
   const uint32_t t = blockIdx.x;
   if (t >= *up.n_var_tiles) return;
-  UnpadTile T;
-  unpad_fetch(up, t, T);
-  const uint64_t e0 = (uint64_t)(t - T.jb.first_tile) * kVarTileElems;
-  const uint32_t cnt = (uint32_t)min((uint64_t)kVarTileElems, T.jb.n_elems - e0);
-  uint64_t v[kVarPerThread];
-  unpad_load_striped(T.in, T.b, e0, cnt, v);
-  uint32_t sum = 0;
-#pragma unroll
-  for (uint32_t i = 0; i < kVarPerThread; ++i) sum += vlen64(v[i]) & ((i * kVarThreads + threadIdx.x < cnt) ? ~0u : 0u);
-  const uint32_t total = block_sum_t0(sum, sh);
-  if (threadIdx.x == 0) publish_tile(T.jb, t - T.jb.first_tile, total);
+  VarJobDev jb;
+  BoxSrc src;
+  unpad_fetch(up, t, jb, src);
+  const uint32_t t_rel = t - jb.first_tile;
+  const uint64_t e0 = (uint64_t)t_rel * kVarTileElems;
+  venc_len_tile(sh, jb, t_rel, e0, (uint32_t)min((uint64_t)kVarTileElems, jb.n_elems - e0), src);
 }
 
 // fixed-width moves of one (request, input): one item for a box that is one stretch of the source (the engine's vector path), else
@@ -250,33 +244,17 @@ __global__ void __launch_bounds__(kUnpadFrameThreads) unpad_frame_kernel(const _
   unpad_write(o, up.F, up.ins, up.box + (size_t)r * up.F.n_in, up.rec_off[up.n + r] - (up.F.grpc ? 5 : 0), nullptr);
 }
 
-// a box as the source of encode tiles: one stretch of the padded tensor goes through venc_load_tile itself, a box of several runs
-// through the same transpose with the striped elements read at their padded positions
-struct BoxSrc {
-  const UnpadTile& T;
-  __device__ __forceinline__ uint32_t load_tile(uint8_t* smem, const VarJobDev& jb, uint64_t e0, uint32_t cnt, uint64_t (&mine)[kVarPerThread],
-                                                uint32_t& lens) const {
-    if (T.b.n_runs <= 1) {
-      const VarSeg sg{T.in.src + T.b.src_off, jb.n_elems, T.s, jb.first_tile};
-      return venc_load_tile(smem, sg, jb, e0, cnt, mine, lens);
-    }
-    uint64_t v[kVarPerThread];
-    unpad_load_striped(T.in, T.b, e0, cnt, v);
-    return venc_block_tile(smem, cnt, v, mine, lens);
-  }
-};
-
 __global__ void __launch_bounds__(kVarThreads, 5) unpad_emit_kernel(const __grid_constant__ UnpadPlan up) {
   __shared__ __align__(16) uint8_t smem[kVarImageBytes];
   __shared__ VarShared sh;
   const uint32_t t = blockIdx.x;
   if (t >= *up.n_var_tiles) return;
-  UnpadTile T;
-  unpad_fetch(up, t, T);
-  const uint32_t t_rel = t - T.jb.first_tile;
+  VarJobDev jb;
+  BoxSrc src;
+  unpad_fetch(up, t, jb, src);
+  const uint32_t t_rel = t - jb.first_tile;
   const uint64_t e0 = (uint64_t)t_rel * kVarTileElems;
-  const uint32_t cnt = (uint32_t)min((uint64_t)kVarTileElems, T.jb.n_elems - e0);
-  venc_emit_tile(smem, sh, T.jb, t_rel, e0, cnt, BoxSrc{T});
+  venc_emit_tile(smem, sh, jb, t_rel, e0, (uint32_t)min((uint64_t)kVarTileElems, jb.n_elems - e0), src);
 }
 
 cudaError_t launch_unpad(const UnpadPlan& up, uint32_t move_grid, cudaStream_t stream, uint32_t* launched) {

@@ -10,6 +10,9 @@
 //                              appends whole 32-bit words to a shared-memory image of the output that
 //                              has the destination's 16-byte phase, and streams the image out with
 //                              128-bit stores
+//            Each pass is one tile body over a tile source: venc_len_tile and venc_emit_tile.  The two kernels here run
+//            them over contiguous segments (SegSrc), unpad_len_kernel and unpad_emit_kernel over the boxes of a padded
+//            tensor (BoxSrc, unpad_kernels.cuh).
 //   decode:  vdec_count_kernel terminators (bytes with the top bit clear) per tile: an ALIGNED 8 KB window of
 //                              the chunk, one warp per tile, sixteen 128-bit loads in flight per lane
 //            vdec_emit_kernel  offset as above; finds the varint starts of the tile with bit tricks,
@@ -46,6 +49,18 @@ __device__ __forceinline__ uint64_t ldg_elem(const uint8_t* p) {
   if (SZ == 4) { const uint32_t t = __ldg(reinterpret_cast<const uint32_t*>(p)); return SG ? (uint64_t)(int64_t)(int32_t)t : t; }
   return __ldg(reinterpret_cast<const unsigned long long*>(p));
 }
+// the same for an element type known at run time
+__device__ __forceinline__ uint64_t ldg_elem_rt(const uint8_t* p, uint32_t size, uint32_t is_signed) {
+  switch (size * 2 + (is_signed ? 1 : 0)) {
+    case 2: return ldg_elem<1, false>(p);
+    case 3: return ldg_elem<1, true>(p);
+    case 4: return ldg_elem<2, false>(p);
+    case 5: return ldg_elem<2, true>(p);
+    case 8: return ldg_elem<4, false>(p);
+    case 9: return ldg_elem<4, true>(p);
+    default: return ldg_elem<8, false>(p);
+  }
+}
 
 // kVarPerThread elements per thread, striped (element base + i*kVarThreads + tid), ALL loads issued
 // before any use; a full tile takes the branch without predicates (one base address, immediate offsets)
@@ -59,18 +74,6 @@ __device__ __forceinline__ void load_striped_t(const uint8_t* src, uint64_t e0, 
 #pragma unroll
     for (uint32_t i = 0; i < kVarPerThread; ++i)
       v[i] = (i * kVarThreads + threadIdx.x < cnt) ? ldg_elem<SZ, SG>(base + (uint64_t)i * kVarThreads * SZ) : 0ull;
-  }
-}
-__device__ __forceinline__ void load_striped(const uint8_t* src, uint64_t e0, uint32_t cnt, uint32_t size, uint32_t is_signed,
-                                             uint64_t (&v)[kVarPerThread]) {
-  switch (size * 2 + (is_signed ? 1 : 0)) {
-    case 2: load_striped_t<1, false>(src, e0, cnt, v); break;
-    case 3: load_striped_t<1, true>(src, e0, cnt, v); break;
-    case 4: load_striped_t<2, false>(src, e0, cnt, v); break;
-    case 5: load_striped_t<2, true>(src, e0, cnt, v); break;
-    case 8: load_striped_t<4, false>(src, e0, cnt, v); break;
-    case 9: load_striped_t<4, true>(src, e0, cnt, v); break;
-    default: load_striped_t<8, false>(src, e0, cnt, v); break;
   }
 }
 
@@ -145,22 +148,16 @@ __device__ __forceinline__ void publish_tile(const VarJobDev& jb, uint32_t t_rel
   atomicAdd(jb.total, (unsigned long long)total);
 }
 
-// E1: bytes each encode tile will occupy
-__global__ void __launch_bounds__(kVarThreads) venc_len_kernel(const __grid_constant__ VarTables tb) {
-  __shared__ VarShared sh;
-  const uint32_t t = blockIdx.x;
-  VarSeg sg;
-  VarJobDev jb;
-  fetch_tile(tb, t, sg, jb);
-  const uint64_t e0 = (uint64_t)(t - sg.first_tile) * kVarTileElems;
-  const uint32_t cnt = (uint32_t)min((uint64_t)kVarTileElems, sg.n - e0);
+// E1: the bytes tile t_rel of job `jb` will occupy, elements [e0, e0 + cnt) of `src`, into the job's counters
+template <class Src>
+__device__ __forceinline__ void venc_len_tile(VarShared& sh, const VarJobDev& jb, uint32_t t_rel, uint64_t e0, uint32_t cnt, const Src& src) {
   uint64_t v[kVarPerThread];
-  load_striped(sg.src, e0, cnt, jb.elem_size, jb.is_signed, v);
+  src.load_striped(e0, cnt, v);
   uint32_t sum = 0;
 #pragma unroll
   for (uint32_t i = 0; i < kVarPerThread; ++i) sum += vlen64(v[i]) & ((i * kVarThreads + threadIdx.x < cnt) ? ~0u : 0u);
   const uint32_t total = block_sum_t0(sum, sh);
-  if (threadIdx.x == 0) publish_tile(jb, t - jb.first_tile, total);
+  if (threadIdx.x == 0) publish_tile(jb, t_rel, total);
 }
 
 // 28 value bits -> four 7-bit groups, one per byte; bit 7 of every byte is left dirty for the caller's
@@ -176,8 +173,8 @@ __device__ __forceinline__ uint32_t spread28(uint32_t x) {
 constexpr uint32_t kVarImageBytes = kVarTileElems * 10 + 48;
 
 // The tile's elements, blocked through shared memory: the thread's striped elements (element i * kVarThreads + tid of the tile in
-// v[i], as load_striped loads them) are transposed (16-byte chunks XOR-swizzled by row) so that thread r owns
-// elements [8r, 8r+8); `lens` and the return value as venc_load_tile gives them.  One barrier inside.
+// v[i], as a source's load_striped loads them) are transposed (16-byte chunks XOR-swizzled by row) so that thread r owns
+// elements [8r, 8r+8); `lens` and the return value as a source's load_tile gives them.  One barrier inside.
 __device__ __forceinline__ uint32_t venc_block_tile(uint8_t* smem, uint32_t cnt, const uint64_t (&v)[kVarPerThread], uint64_t (&mine)[kVarPerThread],
                                                     uint32_t& lens) {
   const uint32_t r = threadIdx.x;
@@ -206,49 +203,69 @@ __device__ __forceinline__ uint32_t venc_block_tile(uint8_t* smem, uint32_t cnt,
   return (pairs * 0x01010101u) >> 24;
 }
 
-// the tile's elements, blocked: thread r owns elements [8r, 8r+8) of the tile; `lens` = their varint lengths, one nibble each
-// (elements past the end of the tensor: 0); returns the thread's byte count.  One barrier inside.
-__device__ __forceinline__ uint32_t venc_load_tile(uint8_t* smem, const VarSeg& sg, const VarJobDev& jb, uint64_t e0, uint32_t cnt,
-                                                   uint64_t (&mine)[kVarPerThread], uint32_t& lens) {
-  const uint32_t r = threadIdx.x;
-  // 64-bit elements of a full tile whose first byte is 16-byte aligned: every thread loads its own eight consecutive elements
-  // with four 128-bit loads - no shared-memory transpose, no barrier (the four loads of a warp cover 2 KB of consecutive bytes
-  // between them; each sector is fetched once and served from L1 to the neighbouring instruction)
-  const uint8_t* first = sg.src + e0 * 8;
-  if (jb.elem_size == 8 && cnt == kVarTileElems && ((uintptr_t)first & 15) == 0) {
-    const uint4* p = reinterpret_cast<const uint4*>(first) + 4 * r;
-    uint4 q[kVarPerThread / 2];
-#pragma unroll
-    for (uint32_t j = 0; j < kVarPerThread / 2; ++j) q[j] = __ldg(p + j);
-    uint32_t any_hi = 0;
-#pragma unroll
-    for (uint32_t j = 0; j < kVarPerThread / 2; ++j) {
-      mine[2 * j] = (uint64_t)q[j].x | ((uint64_t)q[j].y << 32);
-      mine[2 * j + 1] = (uint64_t)q[j].z | ((uint64_t)q[j].w << 32);
-      any_hi |= q[j].y | q[j].w;
+// Where the elements of an encode tile come from.  A source gives elements [e0, e0 + cnt) of its job in the two forms the passes
+// take them:
+//   load_striped  element i * kVarThreads + tid of the tile in v[i], every load issued before any use (venc_len_tile)
+//   load_tile     blocked: thread r owns elements [8r, 8r+8) of the tile, `lens` = their varint lengths, one nibble each (elements
+//                 past the end of the tensor: 0); returns the thread's byte count.  One barrier inside (venc_emit_tile)
+// SegSrc is a contiguous segment; BoxSrc (unpad_kernels.cuh) a box cut out of a padded tensor.
+struct SegSrc {
+  const uint8_t* src;
+  uint32_t elem_size, is_signed;
+
+  __device__ __forceinline__ void load_striped(uint64_t e0, uint32_t cnt, uint64_t (&v)[kVarPerThread]) const {
+    switch (elem_size * 2 + (is_signed ? 1 : 0)) {
+      case 2: load_striped_t<1, false>(src, e0, cnt, v); break;
+      case 3: load_striped_t<1, true>(src, e0, cnt, v); break;
+      case 4: load_striped_t<2, false>(src, e0, cnt, v); break;
+      case 5: load_striped_t<2, true>(src, e0, cnt, v); break;
+      case 8: load_striped_t<4, false>(src, e0, cnt, v); break;
+      case 9: load_striped_t<4, true>(src, e0, cnt, v); break;
+      default: load_striped_t<8, false>(src, e0, cnt, v); break;
     }
-    lens = 0;
-    if (__all_sync(0xFFFFFFFFu, any_hi == 0u)) {      // the warp's values all fit 32 bits: lengths from the low words alone
-#pragma unroll
-      for (uint32_t i = 0; i < kVarPerThread; ++i) {
-        const uint32_t nb = 32u - (uint32_t)__clz((int)((uint32_t)mine[i] | 1u));
-        lens |= (((nb + 6u) * 37u) >> 8) << (4 * i);
-      }
-    } else {
-#pragma unroll
-      for (uint32_t i = 0; i < kVarPerThread; ++i) lens |= vlen64(mine[i]) << (4 * i);
-    }
-    const uint32_t pairs = (lens & 0x0F0F0F0Fu) + ((lens >> 4) & 0x0F0F0F0Fu);
-    return (pairs * 0x01010101u) >> 24;
   }
-  uint64_t v[kVarPerThread];
-  load_striped(sg.src, e0, cnt, jb.elem_size, jb.is_signed, v);
-  return venc_block_tile(smem, cnt, v, mine, lens);
-}
+
+  __device__ __forceinline__ uint32_t load_tile(uint8_t* smem, uint64_t e0, uint32_t cnt, uint64_t (&mine)[kVarPerThread], uint32_t& lens) const {
+    const uint32_t r = threadIdx.x;
+    // 64-bit elements of a full tile whose first byte is 16-byte aligned: every thread loads its own eight consecutive elements
+    // with four 128-bit loads - no shared-memory transpose, no barrier (the four loads of a warp cover 2 KB of consecutive bytes
+    // between them; each sector is fetched once and served from L1 to the neighbouring instruction)
+    const uint8_t* first = src + e0 * 8;
+    if (elem_size == 8 && cnt == kVarTileElems && ((uintptr_t)first & 15) == 0) {
+      const uint4* p = reinterpret_cast<const uint4*>(first) + 4 * r;
+      uint4 q[kVarPerThread / 2];
+#pragma unroll
+      for (uint32_t j = 0; j < kVarPerThread / 2; ++j) q[j] = __ldg(p + j);
+      uint32_t any_hi = 0;
+#pragma unroll
+      for (uint32_t j = 0; j < kVarPerThread / 2; ++j) {
+        mine[2 * j] = (uint64_t)q[j].x | ((uint64_t)q[j].y << 32);
+        mine[2 * j + 1] = (uint64_t)q[j].z | ((uint64_t)q[j].w << 32);
+        any_hi |= q[j].y | q[j].w;
+      }
+      lens = 0;
+      if (__all_sync(0xFFFFFFFFu, any_hi == 0u)) {      // the warp's values all fit 32 bits: lengths from the low words alone
+#pragma unroll
+        for (uint32_t i = 0; i < kVarPerThread; ++i) {
+          const uint32_t nb = 32u - (uint32_t)__clz((int)((uint32_t)mine[i] | 1u));
+          lens |= (((nb + 6u) * 37u) >> 8) << (4 * i);
+        }
+      } else {
+#pragma unroll
+        for (uint32_t i = 0; i < kVarPerThread; ++i) lens |= vlen64(mine[i]) << (4 * i);
+      }
+      const uint32_t pairs = (lens & 0x0F0F0F0Fu) + ((lens >> 4) & 0x0F0F0F0Fu);
+      return (pairs * 0x01010101u) >> 24;
+    }
+    uint64_t v[kVarPerThread];
+    load_striped(e0, cnt, v);
+    return venc_block_tile(smem, cnt, v, mine, lens);
+  }
+};
 
 // build the thread's varints in registers and append them, whole 32-bit words at a time, to the shared-memory image at byte
 // offset `off`; two barriers inside (every thread must have read its elements out of `smem` before this is called: the
-// block scan between venc_load_tile and here has a barrier)
+// block scan between the source's load_tile and here has a barrier)
 __device__ __forceinline__ void venc_build_image(uint8_t* smem, const uint64_t (&mine)[kVarPerThread], uint32_t lens, uint32_t off) {
   const uint32_t f0 = off & 3;
   const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem);
@@ -322,17 +339,15 @@ __device__ __forceinline__ void venc_build_image(uint8_t* smem, const uint64_t (
   __syncthreads();
 }
 
-// One encode tile of job `jb`: tile t_rel of the job, elements [e0, e0 + cnt) of its source.  The offset comes from the counters,
-// `src.load_tile` (a source's tile load; returns the thread's byte count) fills the registers, then the image and the stores - the
-// body of venc_emit_kernel for a source other than a contiguous segment.  (venc_emit_kernel keeps its own copy: built on this
-// template its stack grew from 56 to 80 bytes and its spills with it.)
+// E2: tile t_rel of job `jb`, elements [e0, e0 + cnt) of `src`.  The offset comes from the counters, src.load_tile fills the
+// registers, then the image and the stores.
 template <class Src>
 __device__ __forceinline__ void venc_emit_tile(uint8_t* smem, VarShared& sh, const VarJobDev& jb, uint32_t t_rel, uint64_t e0, uint32_t cnt,
                                                const Src& src) {
   const uint64_t share = prefix_share(jb, t_rel);
   uint64_t mine[kVarPerThread];
   uint32_t lens;
-  const uint32_t sum = src.load_tile(smem, jb, e0, cnt, mine, lens);
+  const uint32_t sum = src.load_tile(smem, e0, cnt, mine, lens);
   uint32_t total;
   uint64_t base;
   uint32_t off = block_scan_sum(sum, &total, share, &base, sh);   // every thread has read its elements before the first barrier inside
@@ -347,12 +362,23 @@ __device__ __forceinline__ void venc_emit_tile(uint8_t* smem, VarShared& sh, con
   const uint32_t lo = phase, hi = phase + total;
   const uint32_t v_lo = (lo + 15) >> 4, v_hi = hi >> 4;
   if (v_lo < v_hi) {
-    for (uint32_t v = v_lo + threadIdx.x; v < v_hi; v += kVarThreads) st_stream(gbase + 16 * v, reinterpret_cast<const uint4*>(smem)[v]);
+    // stepped by byte offset: stepped by vector index, the unrolled loop kept two more induction variables, and venc_emit_kernel spilled more
+    for (uint32_t o = 16 * (v_lo + threadIdx.x); o < 16 * v_hi; o += 16 * kVarThreads) st_stream(gbase + o, *reinterpret_cast<const uint4*>(smem + o));
     for (uint32_t i = lo + threadIdx.x; i < v_lo * 16; i += kVarThreads) gbase[i] = smem[i];
     for (uint32_t i = v_hi * 16 + threadIdx.x; i < hi; i += kVarThreads) gbase[i] = smem[i];
   } else {
     for (uint32_t i = lo + threadIdx.x; i < hi; i += kVarThreads) gbase[i] = smem[i];
   }
+}
+
+__global__ void __launch_bounds__(kVarThreads) venc_len_kernel(const __grid_constant__ VarTables tb) {
+  __shared__ VarShared sh;
+  const uint32_t t = blockIdx.x;
+  VarSeg sg;
+  VarJobDev jb;
+  fetch_tile(tb, t, sg, jb);
+  const uint64_t e0 = (uint64_t)(t - sg.first_tile) * kVarTileElems;
+  venc_len_tile(sh, jb, t - jb.first_tile, e0, (uint32_t)min((uint64_t)kVarTileElems, sg.n - e0), SegSrc{sg.src, jb.elem_size, jb.is_signed});
 }
 
 __global__ void __launch_bounds__(kVarThreads, 5) venc_emit_kernel(const __grid_constant__ VarTables tb) {
@@ -362,33 +388,8 @@ __global__ void __launch_bounds__(kVarThreads, 5) venc_emit_kernel(const __grid_
   VarSeg sg;
   VarJobDev jb;
   fetch_tile(tb, t, sg, jb);
-  const uint32_t t_rel = t - jb.first_tile;
   const uint64_t e0 = (uint64_t)(t - sg.first_tile) * kVarTileElems;
-  const uint32_t cnt = (uint32_t)min((uint64_t)kVarTileElems, sg.n - e0);
-  const uint64_t share = prefix_share(jb, t_rel);
-  uint64_t mine[kVarPerThread];
-  uint32_t lens;
-  const uint32_t sum = venc_load_tile(smem, sg, jb, e0, cnt, mine, lens);
-  uint32_t total;
-  uint64_t base;
-  uint32_t off = block_scan_sum(sum, &total, share, &base, sh);   // every thread has read its elements before the first barrier inside
-  uint8_t* g = jb.dst + base;                  // first output byte of this tile
-  const uint32_t phase = (uint32_t)((uintptr_t)g & 15);
-  venc_build_image(smem, mine, lens, off + phase);
-  // smem[phase .. phase+total) -> g[0 .. total); whole 16-byte vectors where the tile owns them.  Never past the
-  // payload the header announced (the data changed between b200tfs_measure and the encode: undefined bytes, no overrun)
-  if (base >= jb.cap) return;
-  total = (uint32_t)min((uint64_t)total, jb.cap - base);
-  uint8_t* gbase = g - phase;  // 16-byte aligned
-  const uint32_t lo = phase, hi = phase + total;
-  const uint32_t v_lo = (lo + 15) >> 4, v_hi = hi >> 4;
-  if (v_lo < v_hi) {
-    for (uint32_t v = v_lo + threadIdx.x; v < v_hi; v += kVarThreads) st_stream(gbase + 16 * v, reinterpret_cast<const uint4*>(smem)[v]);
-    for (uint32_t i = lo + threadIdx.x; i < v_lo * 16; i += kVarThreads) gbase[i] = smem[i];
-    for (uint32_t i = v_hi * 16 + threadIdx.x; i < hi; i += kVarThreads) gbase[i] = smem[i];
-  } else {
-    for (uint32_t i = lo + threadIdx.x; i < hi; i += kVarThreads) gbase[i] = smem[i];
-  }
+  venc_emit_tile(smem, sh, jb, t - jb.first_tile, e0, (uint32_t)min((uint64_t)kVarTileElems, sg.n - e0), SegSrc{sg.src, jb.elem_size, jb.is_signed});
 }
 
 // D1: varint terminators (bytes with the top bit clear) per decode tile.  One WARP per tile: sixteen
