@@ -286,8 +286,9 @@ int b200tfs_encode_requests(b200tfs_ctx* ctx, int32_t n, const b200tfs_request* 
 /* The same encode (requests.py:41-48 + PredictRequest.SerializeToString, prediction_service_pb2_grpc.py:52) WITHOUT the host-side
  * measuring pass: inputs of the packed-varint dtypes (constants.py:16-23: int_val, int64_val, ...) may carry packed_len == 0.
  * Their lengths are counted, the length prefixes (and every length that encloses them) written, and the record placed by
- * kernels alone - count -> frame_requests_kernel (one thread per request evaluates the dependent varints, writes the
- * framing, patches the destinations of the payload movers) -> move + emit - so the call never synchronises and can be
+ * kernels alone - count -> frame_requests_kernel (one thread per request runs the framing writers twice: once to count the
+ * record and place it, once to write the framing and patch the destinations of the payload movers) -> move + emit - so the
+ * call never synchronises and can be
  * captured in a CUDA graph (b200tfs_measure cannot).  Every record gets a 256-byte aligned slot sized for its worst case
  * (b200tfs_request_arena_size does that when it sees an unmeasured input) and lies inside it with its largest payload
  * 128-byte aligned; WHERE exactly, and how long it is, is known once the kernels have run: b200tfs_encode_results
@@ -295,10 +296,10 @@ int b200tfs_encode_requests(b200tfs_ctx* ctx, int32_t n, const b200tfs_request* 
 int b200tfs_encode_requests_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_request* reqs, void* arena_dev,
                                   uint64_t arena_cap);
 int b200tfs_encode_results(b200tfs_ctx* ctx, int32_t n, uint64_t* rec_off, uint64_t* rec_len);
-/* What frame_requests_kernel computes for ONE request, run on the host (the same inline code; needs no device): given the
+/* What frame_requests_kernel computes for ONE request, run on the host (the same inline function; needs no device): given the
  * packed length of every packed-varint input (packed_len[i] for inputs[i]; other entries ignored) it writes every framing
  * byte of the record into buf at the place it has on the wire and reports where the record lies (rec_off / rec_len) and,
- * per input, where its payload belongs (payload_off[i] / payload_len[i]; 0 / 0 for an input without values).            */
+ * per input, where the framing writers put its payload (payload_off[i] / payload_len[i]; 0 / 0 for an input without values). */
 int b200tfs_request_frame_deferred(const b200tfs_request* r, const uint64_t* packed_len, void* buf, uint64_t cap,
                                    uint64_t* rec_off, uint64_t* rec_len, uint64_t* payload_off, uint64_t* payload_len);
 

@@ -21,7 +21,6 @@
 
 #include "../../include/b200tfs.h"
 #include "example_walk.h"
-#include "frame.h"
 #include "framing.h"
 #include "kernels.h"
 #include "plan.h"
@@ -521,7 +520,6 @@ int tensor_layout(const b200tfs_tensor& t, TensorLayout* L, std::vector<uint8_t>
         break;
       default:  // VK_VARINT
         L->varint = true;
-        L->unmeasured = n && deferred;
         if (n && !deferred && t.packed_len == 0)
           return fail(B200TFS_E_ARG, "varint dtype %d: packed_len not set, call b200tfs_measure first", t.wire_dtype);
         L->payload_len = n && !deferred ? t.packed_len : 0;
@@ -531,8 +529,7 @@ int tensor_layout(const b200tfs_tensor& t, TensorLayout* L, std::vector<uint8_t>
   if (L->payload_len > kProtoLimit) return fail(B200TFS_E_TOOBIG, "payload of %llu bytes exceeds protobuf's 2 GiB limit", (unsigned long long)L->payload_len);
   const uint64_t shape_len = shape_body_len(t.rank, t.dims);
   uint64_t hl = 1 + varint_len((uint64_t)(uint32_t)t.wire_dtype) + 1 + varint_len(shape_len) + shape_len;
-  if (L->payload_len || L->unmeasured) hl += varint_len(tag_of(field, WT_LEN));
-  if (L->payload_len) hl += varint_len(L->payload_len);
+  if (L->payload_len) hl += varint_len(tag_of(field, WT_LEN)) + varint_len(L->payload_len);
   L->header_len = hl; L->field = field; L->shape_len = shape_len;
   if (hdr) {   // one resize, then raw writes
     const size_t base = hdr->size();
@@ -781,6 +778,29 @@ int request_layout(const b200tfs_request& r, RequestLayout* R, bool deferred = f
   return B200TFS_OK;
 }
 
+// write_request's view of request r for the host planner: the framing goes to the blob, and every payload closes the header run
+// in front of it into the plan
+struct PlannedRequest {
+  const b200tfs_request& r;
+  const RequestLayout& R;
+  PlanBuilder& pb;
+  uint8_t* w0;            // the request's framing in the blob
+  size_t base;            // ... at this blob offset
+  size_t mark;            // blob offset where the pending header run starts
+  uint8_t* cursor;        // where that run will land
+  void spec(RawOut& o) { write_model_spec(o, r, R.spec); }
+  void input(uint32_t j, b200tfs_tensor& t, TensorLayout& L) const { t = r.inputs[R.perm[j]]; L = R.tl[j]; }
+  void payload(RawOut& o, uint32_t, const b200tfs_tensor& t, const TensorLayout& L) {
+    if (!L.payload_len) return;
+    const size_t at = base + (size_t)(o.w - w0), run = at - mark;
+    pb.header(cursor, mark, run);
+    cursor += run;
+    plan_tensor(t, L, cursor, pb);
+    cursor += L.payload_len;
+    mark = at;
+  }
+};
+
 // append the wire bytes of request r to the plan, record at arena + rec_off.  Every framing byte of the request is
 // written into the blob with one resize and raw stores (this runs once per request of a batch); the tensor layouts are
 // the ones request_layout computed.
@@ -791,31 +811,11 @@ int plan_request(const b200tfs_request& r, const RequestLayout& R, uint8_t* rec,
   pb.blob.resize(base + frame);
   uint8_t* const w0 = pb.blob.data() + base;
   RawOut o{w0};
-  size_t mark = base;     // blob offset where the pending header run starts
-  uint8_t* cursor = rec;  // where that run will land
-  if (R.prefix) {         // gRPC length-prefixed message: compressed-flag 0, big-endian uint32 length
-    const uint64_t m = R.total - R.prefix;
-    o.byte(0); o.byte((uint8_t)(m >> 24)); o.byte((uint8_t)(m >> 16)); o.byte((uint8_t)(m >> 8)); o.byte((uint8_t)m);
-  }
-  write_model_spec(o, r, R.spec);
-  for (int j = 0; j < r.n_inputs; ++j) {
-    const b200tfs_tensor& t = r.inputs[R.perm[j]];
-    const TensorLayout& L = R.tl[j];
-    write_entry_header(o, t, R.entry_len[j], R.tp_len[j]);
-    write_tensor_header(o, t, L);
-    if (L.payload_len) {
-      const size_t at = base + (size_t)(o.w - w0), run = at - mark;
-      pb.header(cursor, mark, run);
-      cursor += run;
-      int rc = plan_tensor(t, L, cursor, pb);
-      if (rc) return rc;
-      cursor += L.payload_len;
-      mark = at;
-    }
-  }
-  const size_t end = base + (size_t)(o.w - w0), run = end - mark;
-  if (run) { pb.header(cursor, mark, run); cursor += run; }
-  if ((uint64_t)(o.w - w0) != frame || (uint64_t)(cursor - rec) != R.total) return fail(B200TFS_E_ARG, "internal: request length mismatch");
+  PlannedRequest q{r, R, pb, w0, base, base, rec};
+  write_request(o, q, (uint32_t)r.n_inputs, R.prefix != 0, R.total - R.prefix);
+  const size_t end = base + (size_t)(o.w - w0), run = end - q.mark;
+  if (run) { pb.header(q.cursor, q.mark, run); q.cursor += run; }
+  if ((uint64_t)(o.w - w0) != frame || (uint64_t)(q.cursor - rec) != R.total) return fail(B200TFS_E_ARG, "internal: request length mismatch");
   return B200TFS_OK;
 }
 

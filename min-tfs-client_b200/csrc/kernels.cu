@@ -18,8 +18,8 @@
 //   move_guarded_kernel    the move engine over a host-built plan that stores only for records whose guard word is set.
 //   parse_*_kernel     two-phase decode: one lane per PredictResponse / TensorProto walks the tags and
 //                      tabulates dtype, dims and where the values lie.
-//   frame_requests_kernel  deferred framing (frame.h): one warp per request evaluates the request's framing program from the
-//                      device-side totals, writes every header byte, patches the destinations of the movers behind it.
+//   frame_requests_kernel  deferred framing: one thread per request runs the framing writers (framing.h) over the device-side
+//                      totals, writes every header byte, patches the destinations of the movers behind it.
 //   ex_count / ex_scan / ex_emit / ex_frame_kernel   Classify / Regress requests: a batch of tf.Examples from columnar
 //                      arrays (example_kernels.cuh).
 //   xr_index / xr_scan / xr_emit / xr_compare / xr_publish_kernel   Classify / Regress responses: a batch of responses into
@@ -41,7 +41,7 @@
 #include <algorithm>
 #include <utility>
 
-#include "frame.h"
+#include "framing.h"
 #include "kernels.h"
 #include "plan.h"
 #include "tpl.h"
@@ -1214,62 +1214,22 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
 #include "unpad_kernels.cuh"
 
 // ------------------------------------------------------------------------------------------------
-// frame_requests_kernel (plan.h "deferred framing"): one thread per request evaluates the request's values from the job
-// totals the counting kernel just produced, places the record in its slot (largest payload 128-byte aligned, like the host
-// planner's place_record), writes every framing byte and patches the destinations of the payload movers behind it.
+// frame_requests_kernel (plan.h "deferred framing"): one thread per request runs frame_request (framing.h): the framing writers
+// count the record from the job totals the counting kernel just produced, the record is placed in its slot (largest payload
+// 128-byte aligned, like the host planner's place_record), and a second pass writes every framing byte and patches the
+// destinations of the payload movers behind it.
 // ------------------------------------------------------------------------------------------------
-constexpr uint32_t kFrameWarps = 4;                 // requests per CTA (one warp each)
-constexpr uint32_t kFrameSegs = 64, kFrameVals = 32, kFrameTerms = 64, kFrameBlob = 1024;   // what a warp stages in shared memory
-struct FrameStage {
-  FrameSeg segs[kFrameSegs];
-  FrameVal vals[kFrameVals];
-  FrameTerm terms[kFrameTerms];
-  uint64_t term_total[kFrameTerms];
-  uint64_t val[kFrameVals];
-  uint8_t blob[kFrameBlob];
-};
+constexpr uint32_t kFrameThreads = 128;             // requests per CTA (one thread each)
 
-__global__ void __launch_bounds__(32 * kFrameWarps) frame_requests_kernel(const __grid_constant__ FrameTables ft) {
+__global__ void __launch_bounds__(kFrameThreads) frame_requests_kernel(const __grid_constant__ FrameTables ft) {
   pdl_launch_dependents();       // an independent move plan (PlanHeader::independent) may start right behind us
-  __shared__ FrameStage stage[kFrameWarps];
-  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t r = blockIdx.x * kFrameWarps + warp;
-  if (r >= ft.n) return;
-  const FrameReq rq = ft.reqs[r];                                   // round 1 (every lane: one broadcast load)
-  if (rq.n_seg > kFrameSegs || rq.n_val > kFrameVals || rq.n_term > kFrameTerms || rq.n_blob > kFrameBlob) {
-    if (lane == 0) frame_request(ft, r);                            // an unusually large request: walk the tables in place
-    return;
-  }
-  FrameStage& S = stage[warp];
-  for (uint32_t k = lane; k < rq.n_seg; k += 32) S.segs[k] = ft.segs[rq.first_seg + k];     // round 2: all independent
-  for (uint32_t k = lane; k < rq.n_val; k += 32) S.vals[k] = ft.vals[rq.first_val + k];
-  for (uint32_t k = lane; k < rq.n_term; k += 32) {
-    const FrameTerm t = ft.terms[rq.first_term + k];
-    S.terms[k] = t;
-    S.term_total[k] = 0;
-  }
-  for (uint32_t k = lane; k < rq.n_blob; k += 32) S.blob[k] = ft.blob[rq.first_blob + k];
-  __syncwarp();
-  for (uint32_t k = lane; k < rq.n_term; k += 32)                                            // round 3: the job totals
-    if (S.terms[k].kind == FT_TOTAL) S.term_total[k] = (uint64_t)ft.totals[S.terms[k].idx];
-  for (uint32_t k = 0; k < rq.n_term; ++k)                                                   // ... and the tiny inputs: one element per lane
-    if (S.terms[k].kind == FT_TINY) {                                                        // (warp-uniform branch)
-      const TinyVar t = ft.tiny[S.terms[k].idx];
-      uint32_t len = lane < t.n ? varint_len(tiny_elem(t, lane)) : 0u;
-#pragma unroll
-      for (int d = 16; d; d >>= 1) len += __shfl_xor_sync(0xFFFFFFFFu, len, d);
-      if (lane == 0) S.term_total[k] = len;
-    }
-  __syncwarp();
-  if (lane == 0) {
-    FrameView V{S.segs, S.vals, S.terms, S.term_total, S.blob, S.val};
-    frame_request_run(ft, rq, V, r);
-  }
+  const uint32_t r = blockIdx.x * kFrameThreads + threadIdx.x;
+  if (r < ft.n) frame_request(ft, r);
 }
 
 cudaError_t launch_frame_requests(const FrameTables& ft, cudaStream_t stream) {
   if (!ft.n) return cudaSuccess;
-  frame_requests_kernel<<<(ft.n + kFrameWarps - 1) / kFrameWarps, 32 * kFrameWarps, 0, stream>>>(ft);
+  frame_requests_kernel<<<(ft.n + kFrameThreads - 1) / kFrameThreads, kFrameThreads, 0, stream>>>(ft);
   return cudaGetLastError();
 }
 

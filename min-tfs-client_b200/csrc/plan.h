@@ -294,44 +294,44 @@ struct VarPadMap { const PadDesc* desc; const PadKeyDev* keys; uint32_t n_keys, 
 // ---- deferred framing: the length prefixes of packed-varint inputs computed ON THE DEVICE -----------------------------
 // Every length on the wire precedes its content, and a packed-varint payload's length is only known once the counting
 // kernel has run.  Instead of bringing it to the host (b200tfs_measure: a stream synchronise in the middle of an encode),
-// the host describes each request as a little program - byte runs it knows, varints of VALUES the device evaluates
-// (sums of constants, job totals, other values and the varint lengths of other values), and the payloads whose
-// destinations depend on those values - and frame_requests_kernel (one thread per request) lays the record out, writes the
-// framing and patches the destinations into the move plan / the emit jobs that run right behind it.  No host round trip:
-// the whole encode is asynchronous and CUDA-graph capturable.
-enum FrameSegKind : uint32_t {
-  FS_BYTES = 0,   // a = offset into the frame blob, b = byte count
-  FS_VARINT = 1,  // a = value id (request-local): varint(value)
-  FS_BE32 = 2,    // a = value id: four bytes, big endian (gRPC's message length)
-  FS_ITEM = 3,    // a = MoveItem index, b = its byte count: the payload lands here (dst patched)
-  FS_SMALL = 4,   // a = SmallItem index, b = its byte count: likewise
-  FS_VARJOB = 5,  // a = varint job index, b = value id of its packed length: the varints land here (dst and cap patched)
-  FS_TINYVAR = 6  // a = index into FrameTables::tiny, b = value id of its packed length: a packed-varint input of at most
-                  // kTinyVarElems elements (a label, an id, a few flags) is counted AND written by the framing kernel itself -
-                  // no counting kernel, no emit kernel, no counters to zero for it
-};
-constexpr uint32_t kTinyVarElems = 32;
+// the host uploads what each request's framing is made of - its model_spec bytes, and per input the key, the dims, the wire
+// dtype and where the payload's length comes from - and frame_requests_kernel (one thread per request) runs the framing writers
+// (framing.h write_request) over it: it counts the record, places it in its slot, writes the framing and patches the
+// destinations into the move plan / the emit jobs that run right behind it.  No host round trip: the whole encode is
+// asynchronous and CUDA-graph capturable.
+constexpr uint32_t kTinyVarElems = 32;   // a packed-varint input of at most this many elements (a label, an id, a few flags) is
+                                         // counted AND written by the framing kernel itself: no counting or emit kernel for it
 struct TinyVar { const uint8_t* src; uint32_t n, elem_size, is_signed, pad; };
-struct FrameSeg { uint32_t kind, a, b, pad; };
-enum FrameTermKind : uint32_t { FT_TOTAL = 0, FT_VAL = 1, FT_VLEN = 2, FT_TINY = 3 };   // + total[job], + value[i], + varint_len(value[i]), + packed length of tiny[idx]
-struct FrameTerm { uint32_t kind, idx; };
-struct FrameVal { int64_t c; uint32_t first_term, n_terms; };               // evaluated in order: terms refer to earlier values only
-struct FrameReq {
-  uint32_t first_seg, n_seg, first_val, n_val;
-  uint32_t first_term, n_term, first_blob, n_blob;
-  uint32_t align_seg;       // the payload segment that should start 128-byte aligned (index relative to first_seg), ~0u: none
-  uint32_t anchor_seg;      // ~0u, or an FS_ITEM segment whose first byte the host fixed at anchor_off: the record is laid out around it
-  uint32_t pad0;
+enum DeferredPayload : uint32_t {
+  DP_NONE = 0,    // no payload
+  DP_ITEM = 1,    // MoveItem idx moves it (dst patched)
+  DP_SMALL = 2,   // SmallItem idx moves it (dst patched)
+  DP_JOB = 3,     // varint job idx emits it: its length is totals[idx] (dst and cap patched)
+  DP_TINY = 4     // TinyVar idx: the framing kernel counts and writes it
+};
+struct DeferredIn {         // one input of a request, in wire order
+  uint64_t len;             // payload bytes of DP_ITEM / DP_SMALL
+  uint32_t key_off, key_len;   // key bytes in FrameTables::blob
+  uint32_t dims_off;        // int64 dims[rank] in FrameTables::blob
+  int32_t rank, wire_dtype;
+  uint32_t flags, field;
+  uint32_t kind, idx;       // DeferredPayload and its index
+  uint32_t pad;
+};
+struct DeferredReq {
+  uint32_t spec_off, spec_len;   // the model_spec field (its tag included) in FrameTables::blob
+  uint32_t grpc;                 // gRPC's five-byte length-prefixed-message header in front
+  uint32_t first_in, n_in;
+  uint32_t align_in;             // the input whose payload should start 128-byte aligned (request-local), ~0u: none
+  uint32_t anchor_in;            // ~0u, or a DP_ITEM input whose first byte the host fixed at anchor_off: the record is laid out around it
+  uint32_t pad;
   uint64_t anchor_off;
-  uint32_t total_val;       // value id of the record's byte length (incl. a gRPC prefix)
   uint64_t slot_off, slot_cap;   // where the record may lie inside the arena (worst-case sized by the host)
 };
 struct FrameTables {
-  const FrameReq* reqs; const FrameSeg* segs; const FrameVal* vals; const FrameTerm* terms; const uint8_t* blob;
+  const DeferredReq* reqs; const DeferredIn* ins; const uint8_t* blob;
   const unsigned long long* totals;   // packed length of every varint job (the counting kernel's result), by job index
-  const TinyVar* tiny;                // FS_TINYVAR / FT_TINY
-  uint64_t* scratch_vals;   // one evaluated value per FrameVal
-  uint64_t* scratch_terms;  // one fetched total per FrameTerm (used by the table-walking path)
+  const TinyVar* tiny;                // DP_TINY
   uint8_t* arena;
   MoveItem* items; SmallItem* smalls; VarJobDev* jobs;    // patched
   uint64_t* rec_off; uint64_t* rec_len; int32_t* status;  // pinned host memory: read by b200tfs_encode_results

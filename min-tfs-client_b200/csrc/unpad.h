@@ -88,30 +88,32 @@ struct UnpadFrame {                // what every request's framing has in common
   uint32_t n_in, pad_;
 };
 
-// The framing of one request through `o`, payloads skipped: [00 be32(msg)] model_spec {entry header, tensor header, payload}*.
-// The box payloads must be set; `msg` is the message length (unpad_layout).  payload_off (may be null) receives where each
-// input's payload starts, counted from the first byte written.
-template <class Out>
-B2_HD void unpad_write(Out& o, const UnpadFrame& F, const UnpadIn* ins, const UnpadBox* box, uint64_t msg, uint64_t* payload_off) {
-  const uint64_t o0 = o.pos();
-  if (F.grpc) { o.byte(0); o.byte((uint8_t)(msg >> 24)); o.byte((uint8_t)(msg >> 16)); o.byte((uint8_t)(msg >> 8)); o.byte((uint8_t)msg); }
-  o.bytes(F.blob, F.spec_len);
-  for (uint32_t j = 0; j < F.n_in; ++j) {
+// write_request's view of one request of the padded encode: every input from its box, payloads skipped
+struct UnpadRequest {
+  const UnpadFrame& F;
+  const UnpadIn* ins;
+  const UnpadBox* box;
+  uint64_t* payload_off;           // may be null
+  uint64_t o0;
+  template <class Out> B2_HD void spec(Out& o) { o.bytes(F.blob, F.spec_len); }
+  B2_HD void input(uint32_t j, b200tfs_tensor& t, TensorLayout& L) const {
     const UnpadIn& in = ins[j];
-    b200tfs_tensor t{};
     t.wire_dtype = in.wire_dtype; t.rank = in.rank; t.flags = in.flags; t.dims = box[j].dims;
     t.key = (const char*)F.blob + in.key_off; t.key_len = in.key_len;
-    TensorLayout L;
     L.payload_len = box[j].payload; L.field = in.field; L.shape_len = shape_body_len(in.rank, box[j].dims);
-    CountOut h;
-    write_tensor_header(h, t, L);
-    const uint64_t tp = h.n + L.payload_len;
-    const uint64_t el = 1 + varint_len(in.key_len) + in.key_len + 1 + varint_len(tp) + tp;
-    write_entry_header(o, t, el, tp);
-    write_tensor_header(o, t, L);
+  }
+  template <class Out> B2_HD void payload(Out& o, uint32_t j, const b200tfs_tensor&, const TensorLayout& L) {
     if (payload_off) payload_off[j] = o.pos() - o0;
     o.skip(L.payload_len);
   }
+};
+
+// The framing of one request through `o`, payloads skipped.  The box payloads must be set; `msg` is the message length
+// (unpad_layout).  payload_off (may be null) receives where each input's payload starts, counted from the first byte written.
+template <class Out>
+B2_HD void unpad_write(Out& o, const UnpadFrame& F, const UnpadIn* ins, const UnpadBox* box, uint64_t msg, uint64_t* payload_off) {
+  UnpadRequest q{F, ins, box, payload_off, o.pos()};
+  write_request(o, q, F.n_in, F.grpc != 0, msg);
 }
 
 // Length of the record (gRPC prefix included) and, per input, where its payload starts; *largest_off: the start of the largest

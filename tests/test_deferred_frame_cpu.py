@@ -1,5 +1,5 @@
-"""Deferred framing (b200tfs_encode_requests_async): the framing program the host writes for a request and the code
-frame_requests_kernel runs on it, executed on the HOST (b200tfs_request_frame_deferred - the same inline source), against the
+"""Deferred framing (b200tfs_encode_requests_async): the tables the host writes for a request and the framing code
+frame_requests_kernel runs over them, executed on the HOST (b200tfs_request_frame_deferred - the same inline source), against the
 golden PredictRequests of the unmodified reference - including the ones with packed-varint inputs, whose length prefixes
 depend on lengths only the counting kernel knows (here supplied by numpy)."""
 import ctypes as C

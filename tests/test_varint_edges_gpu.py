@@ -291,15 +291,15 @@ def _results(dev, arena, cap, n):
     return [raw[off[i]: off[i] + ln[i]].tobytes() for i in range(n)]
 
 
-def test_deferred_encode_across_the_tiny_limit_and_the_frame_staging(dev):
+def test_deferred_encode_across_the_tiny_limit_and_a_large_request(dev):
     rng = np.random.default_rng(16)
     batch = [("m", 3, [("ids", mixed(9, n, rng))]) for n in (V.TINY - 1, V.TINY, V.TINY + 1, V.ENC_TILE + 1)]
     batch.append(("m", None, [("a", mixed(3, V.TINY, rng)), ("b", mixed(6, V.TINY + 1, rng)), ("c", mixed(22, 1, rng))]))
-    # more packed-varint inputs, tiny values and framing than frame_requests_kernel stages in shared memory
-    many = [("t%02d" % i, mixed(9, V.TINY // 8 + 1, rng)) for i in range(V.FRAME_SEGS)]
+    # a large request: a model name over 1 KB and 72 inputs, most of them tiny packed varints, in one record of the batch
+    many = [("t%02d" % i, mixed(9, V.TINY // 8 + 1, rng)) for i in range(64)]
     many += [("u%02d" % i, mixed(3, V.TINY + i, rng)) for i in range(8)]
-    batch.append(("model_" + "n" * (V.FRAME_BLOB + 100), 7, many))
-    assert sum(a.size for _, a in many if a.size <= V.TINY) > V.FRAME_VALS and len(many) > V.FRAME_SEGS // 2
+    batch.append(("model_" + "n" * 1124, 7, many))
+    assert sum(a.size for _, a in many if a.size <= V.TINY) > 32 and len(many) > 32
     rq, keep = _requests(dev, batch)
     arena, cap = _encode_async(dev, rq, len(batch))
     got = _results(dev, arena, cap, len(batch))

@@ -170,8 +170,6 @@ def test_the_mirrored_geometry_matches_the_sources():
     assert re.fullmatch(r"kVarThreads \* (\d+)", _const(plan, "kVarTileBytes")).group(1) == str(V.DEC_TILE // threads)
     assert _const(plan, "kVarGroupTiles") == "kVarThreads" and threads == V.GROUP_TILES
     assert int(_const(plan, "kTinyVarElems")) == V.TINY
-    assert [int(_const(kern, n)) for n in ("kFrameSegs", "kFrameVals", "kFrameTerms", "kFrameBlob")] == \
-        [V.FRAME_SEGS, V.FRAME_VALS, V.FRAME_TERMS, V.FRAME_BLOB]
     body = host[host.index("bool host_measurable_varint("):]
     body = body[: body.index("\n}\n")]
     assert re.findall(r"> (\d+)\)", body) == [str(V.HOST_MEASURE)] * 2

@@ -17,7 +17,6 @@ GROUP_TILES = 256          # kVarGroupTiles: tiles per counter group
 DEC_TILE = 8192            # kVarTileBytes: wire bytes per decode tile (an aligned window)
 TINY = 32                  # kTinyVarElems: inputs this small are framed by the framing kernel itself
 HOST_MEASURE = 4096        # host_measurable_varint: host inputs up to this many elements are measured on the host
-FRAME_SEGS, FRAME_VALS, FRAME_TERMS, FRAME_BLOB = 64, 32, 64, 1024   # frame_requests_kernel's shared-memory staging per warp
 ENC_GROUP_ELEMS = ENC_TILE * GROUP_TILES      # 524 288 elements: the first encode group boundary
 DEC_GROUP_BYTES = DEC_TILE * GROUP_TILES      # 2 MiB of wire: the first decode group boundary
 
