@@ -623,13 +623,15 @@ int b200tfs_unpack_outputs_host(b200tfs_ctx* ctx, int32_t m, const b200tfs_outpu
  * (DT_FLOAT, DT_DOUBLE, DT_HALF) become float_list the way astype(float32) and a Python float make them: float32 signalling NaNs
  * quieted; float64 rounded to nearest even, NaN -> sign | 0x7FC00000 | (mantissa >> 29); float16 widened exactly, NaNs quieted.
  * Integer and bool columns become int64_list: sign-extended, uint64 wraps (2**64-1 is written as -1), a bool byte != 0 is 1.
- * A row of 0 elements still writes its empty list.  Strings (bytes_list) are not taken: such requests are assembled on the host. */
+ * A row of 0 elements still writes its empty list.  Strings (bytes_list) are not taken: such requests are assembled on the host.
+ * A variable-length (ragged) column is a padded one plus a b200tfs_ragged entry (the *_ragged entry points): row_elems is then the
+ * padded row, and example i takes only the first lengths[i] * unit elements of its row.                                          */
 typedef struct b200tfs_feature {
   const void* data;     /* n_examples rows of row_elems elements (one row with B200TFS_F_BROADCAST), C-contiguous, native order,
                            aligned to the element size; a DEVICE pointer for the _async entry point                              */
   int32_t src_dtype;    /* DT_FLOAT / DT_DOUBLE / DT_HALF / DT_INT8..64 / DT_UINT8..64 / DT_BOOL; others: B200TFS_E_DTYPE         */
   uint32_t flags;       /* B200TFS_F_DEVICE_DATA (the _host entry point: `data` is in HBM already), B200TFS_F_BROADCAST           */
-  int64_t row_elems;    /* elements per example                                                                                 */
+  int64_t row_elems;    /* elements per example (a ragged column: its padded row, max_len * unit)                              */
   const char* key;      /* feature name bytes (UTF-8, not NUL terminated)                                                       */
   int64_t key_len;
 } b200tfs_feature;
@@ -648,10 +650,12 @@ typedef struct b200tfs_example_request {
 
 /* Exact wire length (host, closed form) of a request without integer columns - replaces building the request with
  * requests.py examples_from_input_dict / _make_example_request and asking the message for ByteSize().  A request with an
- * integer column: B200TFS_E_ARG (its length depends on the values).  Over 2 GiB: B200TFS_E_TOOBIG.                       */
+ * integer column: B200TFS_E_ARG (its length depends on the values).  Over 2 GiB: B200TFS_E_TOOBIG.  This is the DENSE size:
+ * it knows nothing of ragged lengths, so a caller with a ragged column sizes with b200tfs_example_arena_size instead.       */
 int b200tfs_example_request_size(const b200tfs_example_request* r, uint64_t* total_len);
 /* Arena bytes b200tfs_encode_example_requests_async needs: one 256-byte aligned slot per request, sized for its worst case
- * (10 bytes per integer element).  A request that cannot stay under 2 GiB whatever its values: B200TFS_E_TOOBIG.       */
+ * (10 bytes per integer element).  A request that cannot stay under 2 GiB whatever its values: B200TFS_E_TOOBIG.  It serves the
+ * _ragged entry points unchanged: a ragged column is described by its padded row_elems, and that worst case bounds every length. */
 int b200tfs_example_arena_size(int32_t n, const b200tfs_example_request* reqs, uint64_t* bytes);
 /* Encode n requests from DEVICE columns into the device arena (256-byte aligned; b200tfs_example_arena_size bytes) - what
  * requests.py examples_from_input_dict + _make_example_request + SerializeToString(deterministic=True) produce.  Kernels only:
@@ -667,6 +671,30 @@ int b200tfs_encode_example_requests_async(b200tfs_ctx* ctx, int32_t n, const b20
  * _make_example_request + SerializeToString.                                                                              */
 int b200tfs_encode_example_requests_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, void* wire_host,
                                          uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
+
+/* Variable-length columns (what a tf.Example model parses as VarLenFeature / RaggedFeature): one entry per feature of every
+ * request, in request-then-feature order (the order of reqs[r].features), parallel to the features as b200tfs_pad_input is to the
+ * inputs of a padded encode.  lengths == NULL: a dense column.  Otherwise feature.row_elems == max_len * unit (B200TFS_E_ARG
+ * when not, when max_len or unit is negative, or on a B200TFS_F_BROADCAST feature) and example i's values are the first
+ * lengths[i] * unit elements of its padded row; unit (the elements of one step of the ragged dimension) may be 0.         */
+typedef struct b200tfs_ragged {
+  const int64_t* lengths;   /* int64[n_examples], 8-byte aligned; device memory for the _async entry point                       */
+  int64_t max_len;          /* L, the padded length                                                                               */
+  int64_t unit;             /* elements per step of the ragged dimension (the product of the inner dims)                        */
+  uint32_t flags;           /* B200TFS_F_DEVICE_DATA: the _host entry point finds the lengths in HBM already                      */
+  int32_t pad_;
+} b200tfs_ragged;
+/* b200tfs_encode_example_requests_async with ragged columns (ragged == NULL: that call itself).  The lengths are only read on the
+ * device, so a replayed CUDA graph follows whatever they hold then.  A length outside [0, max_len] gives that request
+ * B200TFS_E_SHAPE in b200tfs_encode_results (rec_off = rec_len = 0); the kernels clamp it first, so no read leaves the padded
+ * row and no write leaves the request's slot, and the other requests of the call are unaffected.                           */
+int b200tfs_encode_example_requests_ragged_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs,
+                                                 const b200tfs_ragged* ragged, void* arena_dev, uint64_t arena_cap);
+/* b200tfs_encode_example_requests_host with ragged columns (ragged == NULL: that call itself).  Host lengths are copied to the
+ * device with the columns, and checked on the host first (B200TFS_E_SHAPE before anything is launched).                      */
+int b200tfs_encode_example_requests_ragged_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs,
+                                                const b200tfs_ragged* ragged, void* wire_host, uint64_t wire_cap, uint64_t* rec_off,
+                                                uint64_t* rec_len);
 
 /* ---- Classify / Regress responses: a batch of responses into one value or score array ----------------------
  * What ClassificationResponse.FromString / RegressionResponse.FromString followed by a loop over the result give, concatenated

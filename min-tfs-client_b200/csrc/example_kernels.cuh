@@ -1,9 +1,9 @@
 // example_kernels.cuh - Classify / Regress requests: a batch of tf.Examples from columnar arrays (plan.h ExTables; planned by
 // example_host.inc).  Included by kernels.cu inside namespace b200tfs, after concat_scan.
 //
-//   ex_count_kernel  requests with an integer column: one warp per example finds the packed length of every integer row, then
-//                    the example's byte length through its nested lengths (list <- Feature <- map entry <- Features <- Example);
-//                    one CTA per kExTile examples leaves their sum in tile_sum
+//   ex_count_kernel  requests whose size depends on their values (an integer or a ragged column): one warp per example finds
+//                    the packed length of every integer row, then the example's byte length through its nested lengths (list <-
+//                    Feature <- map entry <- Features <- Example); one CTA per kExTile examples leaves their sum in tile_sum
 //   ex_scan_kernel   the same tiles: the tile's offset is the sum of the tiles before it in its request (read, never waited
 //                    for: the count kernel has finished), then a block scan of the example sizes gives every example's offset
 //   ex_emit_kernel   one CTA per contiguous range of examples, i.e. of wire: warps write whole examples (framing, converted float
@@ -11,6 +11,9 @@
 //                    vectors; an example larger than the image is written in place by one warp
 //   ex_frame_kernel  one warp per request: the examples' total, the request prefix in front of the anchor, rec_off / rec_len /
 //                    status to pinned memory
+//
+// count, emit and the example writer take kRagged: a call with a ragged column launches the `true` instantiations, in which a
+// ragged column's row ends after ex_elems elements; every other call runs the `false` ones, which read row_elems as before.
 //
 // What the reference does here: requests.py examples_from_input_dict (a Python loop per example and per feature) and the
 // protobuf runtime serialising the ClassificationRequest / RegressionRequest it filled.
@@ -35,8 +38,17 @@ __device__ __forceinline__ uint64_t ex_int(const ExFeat& f, const uint8_t* p) {
     default: return *reinterpret_cast<const unsigned long long*>(p);
   }
 }
+// elements of example i's row: a ragged column's length, clamped to [0, max_len] (the count kernel flags one that was not), in
+// steps of `unit`; row_elems for a dense column
+template <bool kRagged>
+__device__ __forceinline__ uint64_t ex_elems(const ExFeat& f, uint64_t i) {
+  if (!kRagged || !f.lengths) return f.row_elems;
+  const int64_t l = f.lengths[i];
+  return (l < 0 ? 0ull : min((uint64_t)l, f.max_len)) * f.unit;
+}
+template <bool kRagged>
 __device__ __forceinline__ uint64_t ex_payload(const ExTables& T, const ExReq& q, const ExFeat& f, uint64_t i) {
-  return f.op < EXO_INT ? 4 * f.row_elems : T.L[q.L0 + i * q.n_int + f.lcol];
+  return f.op < EXO_INT ? 4 * ex_elems<kRagged>(f, i) : T.L[q.L0 + i * q.n_int + f.lcol];
 }
 __device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
 #pragma unroll
@@ -45,6 +57,7 @@ __device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
 }
 
 // Example i of request q, written by the calling warp at w (shared or global memory).
+template <bool kRagged>
 __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, uint8_t* w) {
   const uint32_t lane = threadIdx.x & 31;
   uint64_t F = 0, hl;
@@ -52,7 +65,7 @@ __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, 
     uint64_t e = 0;
     if (c + lane < q.n_feat) {
       const ExFeat& f = T.feats[q.first_feat + c + lane];
-      e = ex_entry_len(ex_payload(T, q, f, i), f.key_len, &hl);
+      e = ex_entry_len(ex_payload<kRagged>(T, q, f, i), f.key_len, &hl);
     }
     F += warp_sum64(e);
   }
@@ -70,7 +83,7 @@ __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, 
     hl = 0;
     if (k < q.n_feat) {
       const ExFeat f = T.feats[q.first_feat + k];
-      P = ex_payload(T, q, f, i);
+      P = ex_payload<kRagged>(T, q, f, i);
       e = ex_entry_len(P, f.key_len, &hl);
     }
     uint64_t inc = e;
@@ -99,19 +112,20 @@ __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, 
       if (!Ps) continue;
       const ExFeat f = T.feats[q.first_feat + c + s];
       const uint8_t* row = f.data + i * f.row_stride;
+      const uint64_t ne = ex_elems<kRagged>(f, i);
       uint8_t* d = w + ps;
       if (f.op < EXO_INT) {
-        for (uint64_t j = lane; j < f.row_elems; j += 32) {
+        for (uint64_t j = lane; j < ne; j += 32) {
           const uint32_t b = ex_float_bits(f, row, j);
           d[4 * j] = (uint8_t)b; d[4 * j + 1] = (uint8_t)(b >> 8); d[4 * j + 2] = (uint8_t)(b >> 16); d[4 * j + 3] = (uint8_t)(b >> 24);
         }
       } else {
         uint64_t base = 0;
-        for (uint64_t j0 = 0; j0 < f.row_elems; j0 += 32) {
+        for (uint64_t j0 = 0; j0 < ne; j0 += 32) {
           const uint64_t j = j0 + lane;
           uint64_t v = 0;
           uint32_t len = 0;
-          if (j < f.row_elems) { v = ex_int(f, row + j * f.esz); len = vlen64(v); }
+          if (j < ne) { v = ex_int(f, row + j * f.esz); len = vlen64(v); }
           uint32_t incl = len;
 #pragma unroll
           for (int dd = 1; dd < 32; dd <<= 1) {
@@ -127,6 +141,7 @@ __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, 
   }
 }
 
+template <bool kRagged>
 __global__ void __launch_bounds__(kExTile) ex_count_kernel(const __grid_constant__ ExTables T) {
   __shared__ unsigned long long warp_sum[kExTile / 32];
   const ExSpan sp = T.tiles[blockIdx.x];
@@ -137,11 +152,16 @@ __global__ void __launch_bounds__(kExTile) ex_count_kernel(const __grid_constant
     uint64_t F = 0, hl;
     for (uint32_t k = 0; k < q.n_feat; ++k) {
       const ExFeat f = T.feats[q.first_feat + k];
-      uint64_t P = 4 * f.row_elems;
+      const uint64_t ne = ex_elems<kRagged>(f, i);
+      if (kRagged && f.lengths && lane == 0) {      // compared, never multiplied: 2^62 must not wrap into range
+        const int64_t l = f.lengths[i];
+        if (l < 0 || (uint64_t)l > f.max_len) T.bad[sp.req] = 1;
+      }
+      uint64_t P = 4 * ne;
       if (f.op >= EXO_INT) {
         const uint8_t* row = f.data + i * f.row_stride;
         uint64_t s = 0;
-        for (uint64_t j = lane; j < f.row_elems; j += 32) s += vlen64(ex_int(f, row + j * f.esz));
+        for (uint64_t j = lane; j < ne; j += 32) s += vlen64(ex_int(f, row + j * f.esz));
         P = warp_sum64(s);
         if (lane == 0) T.L[q.L0 + i * q.n_int + f.lcol] = P;
       }
@@ -170,12 +190,20 @@ __global__ void __launch_bounds__(kExTile) ex_scan_kernel(const __grid_constant_
   if (i < sp.e1) T.off[q.ex0 + i] = o;
 }
 
-// where example i of request q starts / ends, from the anchor
-__device__ __forceinline__ uint64_t ex_start(const ExTables& T, const ExReq& q, uint64_t i) {
-  return q.n_int ? T.off[q.ex0 + i] : i * q.fixed_size;
+// Does the scan place request q's examples?  Exactly when fixed_size == 0; without a ragged column that is when the request has an
+// integer column, and the dense instantiation keeps that test (on sm_90a the other one costs its emit kernel 10 registers).
+template <bool kRagged>
+__device__ __forceinline__ bool ex_counted(const ExReq& q) {
+  return kRagged ? q.fixed_size == 0 : q.n_int != 0;
 }
+// where example i of request q starts / ends, from the anchor
+template <bool kRagged>
+__device__ __forceinline__ uint64_t ex_start(const ExTables& T, const ExReq& q, uint64_t i) {
+  return ex_counted<kRagged>(q) ? T.off[q.ex0 + i] : i * q.fixed_size;
+}
+template <bool kRagged>
 __device__ __forceinline__ uint64_t ex_end(const ExTables& T, const ExReq& q, uint64_t i) {
-  return q.n_int ? T.off[q.ex0 + i] + T.S[q.ex0 + i] : (i + 1) * q.fixed_size;
+  return ex_counted<kRagged>(q) ? T.off[q.ex0 + i] + T.S[q.ex0 + i] : (i + 1) * q.fixed_size;
 }
 
 // Store arena bytes [lo, hi) from the image img of the wire that starts at arena offset ws (16-byte aligned): the whole aligned
@@ -189,6 +217,7 @@ __device__ __forceinline__ void ex_flush(uint8_t* arena, const uint8_t* img, uin
   for (uint64_t x = b + threadIdx.x; x < hi; x += blockDim.x) arena[x] = img[x - ws];
 }
 
+template <bool kRagged>
 __global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_constant__ ExTables T) {
   __shared__ __align__(16) uint8_t img[kExStage + 16];
   __shared__ uint64_t next;
@@ -197,7 +226,7 @@ __global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_co
   const ExReq q = T.reqs[sp.req];
   const uint32_t warp = threadIdx.x >> 5;
   const uint64_t A = q.anchor;
-  uint64_t lo = A + ex_start(T, q, sp.e0);   // first byte not stored yet
+  uint64_t lo = A + ex_start<kRagged>(T, q, sp.e0);   // first byte not stored yet
   uint64_t ws = lo & ~15ull;                 // arena offset of img[0]
   uint64_t i = sp.e0;
   while (i < sp.e1) {
@@ -205,16 +234,16 @@ __global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_co
       uint64_t g = i, h = sp.e1;
       while (g < h) {
         const uint64_t m = (g + h + 1) / 2;
-        if (A + ex_end(T, q, m - 1) - ws <= kExStage) g = m; else h = m - 1;
+        if (A + ex_end<kRagged>(T, q, m - 1) - ws <= kExStage) g = m; else h = m - 1;
       }
       next = g;
     }
     __syncthreads();
     const uint64_t j = next;
     if (j > i) {
-      for (uint64_t e = i + warp; e < j; e += kWarps) ex_write_example(T, q, e, img + (A + ex_start(T, q, e) - ws));
+      for (uint64_t e = i + warp; e < j; e += kWarps) ex_write_example<kRagged>(T, q, e, img + (A + ex_start<kRagged>(T, q, e) - ws));
       __syncthreads();
-      const uint64_t be = A + ex_end(T, q, j - 1), cut = be & ~15ull;
+      const uint64_t be = A + ex_end<kRagged>(T, q, j - 1), cut = be & ~15ull;
       if (cut > ws) {                        // store every whole vector; the partial one moves to the front of the image
         ex_flush(T.arena, img, ws, lo, cut);
         const uint8_t t = threadIdx.x < be - cut ? img[cut - ws + threadIdx.x] : 0;
@@ -224,15 +253,15 @@ __global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_co
       }
       i = j;
     } else {                                 // example i alone is larger than the image: one warp writes it in place
-      ex_flush(T.arena, img, ws, lo, A + ex_start(T, q, i));
-      if (warp == 0) ex_write_example(T, q, i, T.arena + A + ex_start(T, q, i));
-      lo = A + ex_end(T, q, i);
+      ex_flush(T.arena, img, ws, lo, A + ex_start<kRagged>(T, q, i));
+      if (warp == 0) ex_write_example<kRagged>(T, q, i, T.arena + A + ex_start<kRagged>(T, q, i));
+      lo = A + ex_end<kRagged>(T, q, i);
       ws = lo & ~15ull;
       ++i;
     }
     __syncthreads();
   }
-  ex_flush(T.arena, img, ws, lo, A + ex_end(T, q, sp.e1 - 1));
+  ex_flush(T.arena, img, ws, lo, A + ex_end<kRagged>(T, q, sp.e1 - 1));
 }
 
 constexpr uint32_t kExFrameWarps = 4;
@@ -241,7 +270,7 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __gr
   if (r >= T.n_req) return;
   const ExReq q = T.reqs[r];
   uint64_t el = 0;
-  if (q.n_int) {
+  if (!q.fixed_size) {
     for (uint32_t k = lane; k < q.n_tiles; k += 32) el += T.tile_sum[q.first_tile + k];
     el = warp_sum64(el);
   } else {
@@ -252,7 +281,8 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __gr
   const uint64_t input = 1 + varint_len(el) + el, msg = q.spec_len + 1 + varint_len(input) + input;
   const uint64_t pre = (q.grpc ? 5 : 0) + q.spec_len + 1 + varint_len(input) + 1 + varint_len(el);
   int32_t st = B200TFS_OK;
-  if (msg > 0x7FFFFFFFull) st = B200TFS_E_TOOBIG;
+  if (T.bad && T.bad[r]) st = B200TFS_E_SHAPE;
+  else if (msg > 0x7FFFFFFFull) st = B200TFS_E_TOOBIG;
   else if (q.anchor + el > q.slot_end) st = B200TFS_E_SIZE;
   T.status[r] = st;
   T.rec_off[r] = st ? 0 : q.anchor - pre;
@@ -267,12 +297,18 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __gr
 
 cudaError_t launch_example_requests(const ExTables& T, cudaStream_t stream, uint32_t* launched) {
   *launched = 0;
+  const bool ragged = T.bad != nullptr;
   if (T.n_tiles) {
-    ex_count_kernel<<<T.n_tiles, kExTile, 0, stream>>>(T);
+    if (ragged) ex_count_kernel<true><<<T.n_tiles, kExTile, 0, stream>>>(T);
+    else ex_count_kernel<false><<<T.n_tiles, kExTile, 0, stream>>>(T);
     ex_scan_kernel<<<T.n_tiles, kExTile, 0, stream>>>(T);
     *launched += 2;
   }
-  if (T.n_spans) { ex_emit_kernel<<<T.n_spans, kExEmitThreads, 0, stream>>>(T); *launched += 1; }
+  if (T.n_spans) {
+    if (ragged) ex_emit_kernel<true><<<T.n_spans, kExEmitThreads, 0, stream>>>(T);
+    else ex_emit_kernel<false><<<T.n_spans, kExEmitThreads, 0, stream>>>(T);
+    *launched += 1;
+  }
   if (T.n_req) { ex_frame_kernel<<<(T.n_req + kExFrameWarps - 1) / kExFrameWarps, 32 * kExFrameWarps, 0, stream>>>(T); *launched += 1; }
   return cudaGetLastError();
 }

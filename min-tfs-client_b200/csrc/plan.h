@@ -345,8 +345,9 @@ B2_PLAN_HD uint64_t var_decode_tiles(const void* src, uint64_t n) {
 
 // ---- tf.Example requests (example_host.inc plans, example_kernels.cuh runs) ----------------------------------------------
 // One request's examples start at a host-fixed anchor inside its slot; the request prefix is written in front of them once
-// their total is known.  Requests with an integer column get their example sizes from the count kernel and their offsets
-// from the scan kernel (tiles of kExTile examples); float-only requests have one closed-form example size.
+// their total is known.  Requests whose size depends on their values (an integer or a ragged column) get their example sizes
+// from the count kernel and their offsets from the scan kernel (tiles of kExTile examples); the others have one closed-form
+// example size.
 enum ExOp : uint32_t { EXO_F32 = 0, EXO_F64 = 1, EXO_F16 = 2, EXO_INT = 3, EXO_BOOL = 4 };
 constexpr uint32_t kExTile = kConcatPlanThreads;   // examples per count / scan CTA (one thread each in the scan)
 constexpr uint32_t kExEmitThreads = 256;
@@ -358,15 +359,18 @@ struct ExFeat {             // one column of one request, in wire order
   uint32_t op, esz, sgn;    // ExOp, element size in memory, sign-extend (EXO_INT)
   uint32_t key_off, key_len;   // key bytes in ExTables::blob
   uint32_t lcol;            // integer columns: column of the request's length table
+  const int64_t* lengths;   // a ragged column: example i takes min(max(lengths[i], 0), max_len) * unit elements; NULL: dense
+  uint64_t max_len, unit;   // row_elems == max_len * unit
 };
 struct ExReq {
-  uint32_t first_feat, n_feat, n_int;   // n_int == 0: float-only, every example is fixed_size bytes
+  uint32_t first_feat, n_feat, n_int;   // integer columns (their entries per example in ExTables::L)
   uint32_t spec_off, spec_len;          // the model_spec field (tag included) in ExTables::blob
   uint32_t grpc;                        // gRPC's five-byte length-prefixed-message header in front
-  uint32_t first_tile, n_tiles;         // count / scan tiles (integer requests)
+  uint32_t first_tile, n_tiles;         // count / scan tiles (requests whose size depends on their values)
   uint64_t n_ex, ex0;                   // examples, and the first one's index in the per-example tables of the call
   uint64_t L0;                          // first entry of the request in ExTables::L (n_ex * n_int entries)
-  uint64_t fixed_size;                  // float-only: bytes of one example in the example_list (its tag included)
+  uint64_t fixed_size;                  // bytes of every example in the example_list (its tag included); 0: the size depends on
+                                        // the values (an integer or a ragged column), S and off hold each example's
   uint64_t anchor, slot_end;            // arena offsets: where example 0 starts, where the slot ends
 };
 struct ExSpan { uint32_t req, pad; uint64_t e0, e1; };   // a CTA's examples [e0, e1) of request `req`
@@ -375,9 +379,11 @@ struct ExTables {
   const ExSpan* tiles;                  // count / scan CTAs
   const ExSpan* spans;                  // emit CTAs
   uint64_t* L;                          // packed length of every (example, integer column)
-  uint64_t* S;                          // bytes of every example of an integer request
+  uint64_t* S;                          // bytes of every example of a request whose size depends on its values
   uint64_t* off;                        // its offset from the anchor
   unsigned long long* tile_sum;         // bytes of every tile's examples
+  int32_t* bad;                         // a call with a ragged column: per request, nonzero when a length was out of range
+                                        // (zeroed by the host in every call); NULL otherwise
   uint8_t* arena;
   uint64_t* rec_off; uint64_t* rec_len; int32_t* status;   // pinned host memory: read by b200tfs_encode_results
   uint32_t n_req, n_tiles, n_spans;

@@ -115,6 +115,12 @@ class ExampleRequest(C.Structure):
     ]
 
 
+class Ragged(C.Structure):
+    """b200tfs_ragged: the lengths of one variable-length tf.Example column (NULL lengths: a dense column); example i takes the
+    first lengths[i] * unit of its row's max_len * unit elements."""
+    _fields_ = [("lengths", C.c_void_p), ("max_len", C.c_int64), ("unit", C.c_int64), ("flags", C.c_uint32), ("pad_", C.c_int32)]
+
+
 class PadInput(C.Structure):
     """b200tfs_pad_input: the shapes of one input of b200tfs_encode_padded_requests_async (int64[n, cols]; cols 1: row counts)."""
     _fields_ = [("shapes", C.c_void_p), ("cols", C.c_int32), ("pad_", C.c_int32)]
@@ -217,6 +223,10 @@ SIGNATURES = {
     "b200tfs_example_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), _u64p]),
     "b200tfs_encode_example_requests_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), _vp, C.c_uint64]),
     "b200tfs_encode_example_requests_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), _vp, C.c_uint64, _u64p, _u64p]),
+    "b200tfs_encode_example_requests_ragged_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), _vp,
+                                                               C.c_uint64]),
+    "b200tfs_encode_example_requests_ragged_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), _vp,
+                                                              C.c_uint64, _u64p, _u64p]),
     "b200tfs_example_response_bound": (C.c_int, [C.c_int32, C.c_int32, _u64p, _u64p, _u64p]),
     "b200tfs_decode_example_responses": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64, _vp, C.c_uint64]),
     "b200tfs_decode_example_responses_host_async": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64, _vp,

@@ -136,31 +136,77 @@ _EXAMPLE_DTYPES = {np.dtype(t): _validated_enum(np.empty(0, t)) for t in (
     np.float16, np.float32, np.float64, np.int8, np.int16, np.int32, np.int64, np.uint8, np.uint16, np.uint32, np.uint64, np.bool_)}
 
 
+class RaggedColumn:
+    """A variable-length tf.Example column - what a model parses as ``VarLenFeature`` / ``RaggedFeature``: a click history, the
+    token ids of a query, multi-hot ids.  Example i's feature holds ``values[i, :lengths[i]].ravel()``, converted as a dense row is.
+
+    ``values`` has shape ``[n, L, *inner]`` (rank >= 2): a numpy array (pageable or ``pinned_empty``) or a device array
+    (``__cuda_array_interface__`` / DLPack).  ``lengths`` is ``int[n]``: a numpy array of any integer dtype, whose values must lie
+    in ``0..L`` (ValueError here), or a device array of int64, whose values the encode kernels check (ValueError from the encode).
+    """
+
+    __slots__ = ("values", "lengths", "shape", "lengths_on_device")
+
+    def __init__(self, values, lengths):
+        shape = tuple(D.device_view(values)[1]) if D.is_device_object(values) else np.shape(values)
+        if len(shape) < 2:
+            raise ValueError(f"ragged values have shape [n, L, *inner] (rank >= 2), got {shape}")
+        self.lengths_on_device = D.is_device_object(lengths)
+        if self.lengths_on_device:
+            _, lshape, ldtype, _ = D.device_view(lengths)
+            if ldtype != np.int64:
+                raise ValueError(f"device ragged lengths must be int64, got {ldtype}")
+        else:
+            lengths = np.asarray(lengths)
+            if lengths.dtype.kind not in "iu":
+                raise ValueError(f"ragged lengths must be integers, got {lengths.dtype}")
+            lshape = lengths.shape
+        if tuple(lshape) != shape[:1]:
+            raise ValueError(f"ragged lengths of shape {tuple(lshape)} for values of {shape[0]} examples")
+        if not self.lengths_on_device:
+            if ((lengths < 0) | (lengths > shape[1])).any():
+                raise ValueError(f"ragged lengths must lie in 0..{shape[1]}")
+            lengths = np.ascontiguousarray(lengths, dtype=np.int64)
+        self.values, self.lengths, self.shape = values, lengths, shape
+
+    @property
+    def ndim(self) -> int:
+        return len(self.shape)
+
+    def row(self, i: int) -> np.ndarray:
+        """Example i's values, ``[lengths[i], *inner]`` (host arrays)."""
+        return np.asarray(self.values)[i, :int(self.lengths[i])]
+
+
 def _example_columns(input_dict: Mapping):
-    """(n_examples, [(Feature, keep-alive), ...]) for the device route, or None for a request ``examples_from_input_dict``
-    assembles on the host (str / bytes columns, dtypes without a device conversion - which it rejects or converts itself).
-    Raises the ValueError ``examples_from_input_dict`` raises for disagreeing example counts, and for device arrays of a dtype
-    the device route does not take."""
+    """(n_examples, [(Feature, keep-alive, key, Ragged or None), ...]) for the device route, or None for a request
+    ``examples_from_input_dict`` assembles on the host (str / bytes columns, dtypes without a device conversion - which it rejects
+    or converts itself).  A ``RaggedColumn`` gives the Feature of its padded ``values`` (``row_elems = L * unit``) and a Ragged
+    entry for its lengths.  Raises the ValueError ``examples_from_input_dict`` raises for disagreeing example counts, and for
+    device arrays of a dtype the device route does not take."""
     cols = []
     for k, v in input_dict.items():
         key = k.encode("utf-8") if isinstance(k, str) else bytes(k)
+        rag = v if isinstance(v, RaggedColumn) else None
+        if rag is not None:
+            v = rag.values
         if D.is_device_object(v):
             ptr, shape, dtype, hold = D.device_view(v)
             if dtype not in _EXAMPLE_DTYPES:
                 raise ValueError(f"input {k!r}: device arrays of dtype {dtype} have no tf.Example feature kind on the device")
-            cols.append((key, ptr, shape, dtype, hold, True))
+            cols.append((key, ptr, shape, dtype, hold, True, rag))
         else:
             a = np.asarray(v)
             dtype = a.dtype.newbyteorder("=")
             if dtype not in _EXAMPLE_DTYPES:
                 return None
-            cols.append((key, None, a.shape, dtype, a, False))
-    rows = {shape[0] for _, _, shape, _, _, _ in cols if len(shape)}
+            cols.append((key, None, a.shape, dtype, a, False, rag))
+    rows = {shape[0] for _, _, shape, _, _, _, _ in cols if len(shape)}
     if len(rows) > 1:
         raise ValueError(f"inputs disagree on the number of examples: {sorted(rows)}")
     n = rows.pop() if rows else (1 if cols else 0)
     preps = []
-    for key, ptr, shape, dtype, hold, on_device in cols:
+    for key, ptr, shape, dtype, hold, on_device, rag in cols:
         row_elems = int(np.prod(shape[1:], dtype=np.int64)) if len(shape) else 1
         flags = 0 if len(shape) else N.F_BROADCAST
         if on_device:
@@ -171,7 +217,17 @@ def _example_columns(input_dict: Mapping):
         size = int(np.prod(shape, dtype=np.int64))
         f = N.Feature(data=ptr if size else None, src_dtype=_EXAMPLE_DTYPES[dtype], flags=flags, row_elems=row_elems,
                       key=key, key_len=len(key))
-        preps.append((f, hold, key))
+        g = None
+        if rag is not None:
+            if rag.lengths_on_device:
+                lptr, _, _, lhold = D.device_view(rag.lengths)
+            else:
+                lhold = rag.lengths
+                lptr = lhold.ctypes.data
+            g = N.Ragged(lengths=lptr or None, max_len=shape[1], unit=int(np.prod(shape[2:], dtype=np.int64)),
+                         flags=N.F_DEVICE_DATA if rag.lengths_on_device else 0)
+            hold = (hold, lhold)
+        preps.append((f, hold, key, g))
     return n, preps
 
 
@@ -664,14 +720,15 @@ class Codec:
         The bytes equal ``_make_example_request(...).SerializeToString(deterministic=True)`` of the request
         ``examples_from_input_dict`` builds - one tf.Example per row, 0-d arrays repeated in every example - with
         ``order="deterministic"``, or list every example's features in insertion order with ``order="given"``.  Values may be
-        numpy arrays (pageable or ``pinned_empty``) or device arrays (``__cuda_array_interface__`` / DLPack).  A request with a
-        str / bytes column (or a dtype the device route does not take) is assembled on the host by ``examples_from_input_dict``,
-        in deterministic order; device arrays of such dtypes raise ValueError.
+        numpy arrays (pageable or ``pinned_empty``) or device arrays (``__cuda_array_interface__`` / DLPack), and a value may be a
+        ``RaggedColumn``: example i then holds only the first ``lengths[i]`` steps of its padded row (device lengths out of range
+        raise ValueError).  A request with a str / bytes column (or a dtype the device route does not take) is assembled on the
+        host by ``examples_from_input_dict``, in deterministic order; device arrays of such dtypes raise ValueError.
         """
         order_code = _ORDER[order] if isinstance(order, str) else int(order)
         items = list(requests)
         out: List[Optional[bytes]] = [None] * len(items)
-        keep, structs, dev_idx = [], [], []
+        keep, structs, dev_idx, ragged = [], [], [], []
         for i, (model_name, model_version, input_dict) in enumerate(items):
             cols = _example_columns(input_dict)
             if cols is None:
@@ -685,6 +742,7 @@ class Codec:
                                             n_examples=n, n_features=len(preps), flags=N.RF_GRPC_FRAME if grpc_frame else 0,
                                             features=feats))
             keep.append((preps, feats, name))
+            ragged += [p[3] or N.Ragged() for p in preps]
             dev_idx.append(i)
         if dev_idx:
             m = len(dev_idx)
@@ -693,7 +751,11 @@ class Codec:
             N.check(self._lib.b200tfs_example_arena_size(m, reqs, C.byref(cap)))
             wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
             off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
-            N.check(self._lib.b200tfs_encode_example_requests_host(self._ctx, m, reqs, wire.ctypes.data, cap.value, off, ln))
+            if any(g.lengths for g in ragged):
+                rg = (N.Ragged * len(ragged))(*ragged)
+                N.check(self._lib.b200tfs_encode_example_requests_ragged_host(self._ctx, m, reqs, rg, wire.ctypes.data, cap.value, off, ln))
+            else:
+                N.check(self._lib.b200tfs_encode_example_requests_host(self._ctx, m, reqs, wire.ctypes.data, cap.value, off, ln))
             for j, i in enumerate(dev_idx):
                 out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
         return out  # type: ignore[return-value]

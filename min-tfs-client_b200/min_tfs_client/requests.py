@@ -18,7 +18,7 @@ from typing import Dict, Optional
 
 import numpy as np
 
-from .codec import get_codec
+from .codec import RaggedColumn, get_codec
 from .tensors import WireTensor
 
 PREDICT_METHOD = "/tensorflow.serving.PredictionService/Predict"
@@ -32,13 +32,14 @@ def examples_from_input_dict(input_dict: Dict[str, np.ndarray]):
 
     Row i of every array is example i: ``feature[k]`` holds the row's values flattened - ``float_list`` for floating
     dtypes, ``int64_list`` for integers and bools, ``bytes_list`` for str / bytes (``coerce_to_bytes``).  0-d arrays are
-    repeated in every example; all other arrays must agree on their first dimension.
+    repeated in every example; all other arrays must agree on their first dimension.  A ``RaggedColumn`` gives example i
+    only ``values[i, :lengths[i]]``.
     """
     from tensorflow_serving.apis.input_pb2 import Input
 
     from .tensors import coerce_to_bytes
 
-    arrays = {k: np.asarray(v) for k, v in input_dict.items()}
+    arrays = {k: v if isinstance(v, RaggedColumn) else np.asarray(v) for k, v in input_dict.items()}
     rows = {a.shape[0] for a in arrays.values() if a.ndim}
     if len(rows) > 1:
         raise ValueError(f"inputs disagree on the number of examples: {sorted(rows)}")
@@ -48,7 +49,7 @@ def examples_from_input_dict(input_dict: Dict[str, np.ndarray]):
     for i in range(n):
         ex = inp.example_list.examples.add()
         for k, a in arrays.items():
-            row = a if a.ndim == 0 else a[i]
+            row = a.row(i) if isinstance(a, RaggedColumn) else a if a.ndim == 0 else a[i]
             feat = ex.features.feature[k]
             if row.dtype.kind == "f":
                 feat.float_list.value.extend(np.asarray(row, dtype=np.float32).ravel().tolist())

@@ -4,14 +4,21 @@ Workloads (one request each unless stated):
   W1  65 536 examples x {dense f32[64]}                                   float-only: closed-form offsets, no count / scan
   W2  16 384 examples x {dense f32[64], ids int64[8] in 0..50 000, age f32}
   W3  256 requests of 64 examples shaped like W2
+  V1  16 384 examples x {history int64 ragged [16384, 64], lengths uniform in 0..64, values in 0..50 000; dense f32[64]}
+  V2  65 536 examples x {emb f32 ragged [65536, 64], lengths uniform in 1..64}   float-only, but counted and scanned (beside W1)
+  V3  4 096 examples x {tokens int32 ragged [4096, 512], lengths geometric with mean ~40, capped at 512}   worst-case emit spans
+  V4  256 requests of 64 examples shaped like V1
 Legs: the _async entry point eager (device columns -> device arena), the same captured once as a CUDA graph and replayed,
 _host from pinned columns (copies both ways included), and examples_from_input_dict + SerializeToString(deterministic=True)
 on one host core.  CUDA events over >= 20 calls after warm-up, three runs each; bytes = column bytes read + wire bytes
 written; the share is of the H100 SXM data sheet's 3.35 TB/s.  W1 is set beside the Predict encode (b200tfs_encode_requests_async)
 of the same f32[65536, 64] as one tensor, and W2 is split by kernel with torch.profiler in a run of its own.  Every leg's
 bytes are checked against the host path after its timed region.  Needs a GPU; --json PATH also writes every number there.
+The V workloads (ragged columns, b200tfs_encode_example_requests_ragged_*) count the values their lengths use, not the padded
+columns, and the lengths; their host path builds the request one example at a time from the unchanged dense code, as a user
+without ragged columns would.  --profile V1,V3 runs only the per-kernel split of the named workloads (profiler on).
 
-  python tools/example_probe.py [--calls 20] [--runs 3] [--json PATH]
+  python tools/example_probe.py [--calls 20] [--runs 3] [--workloads W1,V1,...] [--profile V1,V3] [--json PATH]
 """
 import argparse
 import ctypes as C
@@ -27,8 +34,8 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(REPO, "min-tfs-client_b200"))
 
 from min_tfs_client import _native as N  # noqa: E402
-from min_tfs_client.codec import Codec, _example_columns  # noqa: E402
-from min_tfs_client.requests import TensorServingClient  # noqa: E402
+from min_tfs_client.codec import Codec, RaggedColumn, _example_columns  # noqa: E402
+from min_tfs_client.requests import TensorServingClient, examples_from_input_dict  # noqa: E402
 from tensorflow_serving.apis.classification_pb2 import ClassificationRequest  # noqa: E402
 
 PEAK = 3.35e12
@@ -38,11 +45,52 @@ def workloads(rng):
     def w2(n):
         return {"dense": rng.standard_normal((n, 64)).astype(np.float32), "ids": rng.integers(0, 50_000, (n, 8)),
                 "age": rng.standard_normal(n).astype(np.float32)}
-    return {"W1": [{"dense": rng.standard_normal((65536, 64)).astype(np.float32)}], "W2": [w2(16384)], "W3": [w2(64) for _ in range(256)]}
+    def v1(n):
+        return {"history": RaggedColumn(rng.integers(0, 50_000, (n, 64)), rng.integers(0, 65, n)),
+                "dense": rng.standard_normal((n, 64)).astype(np.float32)}
+    return {"W1": lambda: [{"dense": rng.standard_normal((65536, 64)).astype(np.float32)}], "W2": lambda: [w2(16384)],
+            "W3": lambda: [w2(64) for _ in range(256)],
+            "V1": lambda: [v1(16384)],
+            "V2": lambda: [{"emb": RaggedColumn(rng.standard_normal((65536, 64)).astype(np.float32), rng.integers(1, 65, 65536))}],
+            "V3": lambda: [{"tokens": RaggedColumn(rng.integers(0, 32_000, (4096, 512), dtype=np.int32),
+                                                   np.minimum(rng.geometric(1 / 40, 4096), 512))}],
+            "V4": lambda: [v1(64) for _ in range(256)]}
 
 
 def host_ref(d):
-    return TensorServingClient._make_example_request(None, ClassificationRequest, "model", d, 1).SerializeToString(deterministic=True)
+    """the host path: examples_from_input_dict + SerializeToString; with ragged columns one example at a time (each example the
+    one examples_from_input_dict makes of that example's rows), merged in order"""
+    if not any(isinstance(v, RaggedColumn) for v in d.values()):
+        return TensorServingClient._make_example_request(None, ClassificationRequest, "model", d, 1).SerializeToString(deterministic=True)
+    req = TensorServingClient._make_example_request(None, ClassificationRequest, "model", {}, 1)
+    n = next(v.shape[0] for v in d.values() if isinstance(v, RaggedColumn))
+    for i in range(n):
+        one = {k: v.values[i:i + 1, :int(v.lengths[i])] if isinstance(v, RaggedColumn) else v if np.ndim(v) == 0 else v[i:i + 1]
+               for k, v in d.items()}
+        req.input.example_list.examples.extend(examples_from_input_dict(one).example_list.examples)
+    return req.SerializeToString(deterministic=True)
+
+
+def arrays(d):
+    """the host arrays a request reads, in column order: values, then the lengths of a ragged column"""
+    for v in d.values():
+        if isinstance(v, RaggedColumn):
+            yield v.values
+            yield v.lengths
+        else:
+            yield v
+
+
+def used_bytes(d):
+    """column bytes the encode needs: a ragged column's used values and its lengths, every other column whole"""
+    b = 0
+    for v in d.values():
+        if isinstance(v, RaggedColumn):
+            unit = int(np.prod(v.shape[2:], dtype=np.int64))
+            b += int(v.lengths.sum()) * unit * v.values.itemsize + v.lengths.nbytes
+        else:
+            b += np.asarray(v).nbytes
+    return b
 
 
 class Ctx:
@@ -79,24 +127,52 @@ def timed_host(fn, calls):
 
 
 def build(dicts, device_ptrs=None):
-    keep, structs = [], []
+    """(requests, ragged entries or None when no column is ragged, keep-alive); device_ptrs[r]: the arrays(d) of request r in HBM"""
+    keep, structs, ragged = [], [], []
     for r, d in enumerate(dicts):
         n, preps = _example_columns(d)
         feats = (N.Feature * len(preps))(*[p[0] for p in preps])
+        rg = [p[3] or N.Ragged() for p in preps]
         if device_ptrs is not None:
-            for k, f in enumerate(feats):
-                f.data = device_ptrs[r][k]
+            ptrs = iter(device_ptrs[r])
+            for f, g in zip(feats, rg):
+                f.data = next(ptrs)
                 f.flags |= N.F_DEVICE_DATA
+                if g.lengths:
+                    g.lengths = next(ptrs)
+                    g.flags = N.F_DEVICE_DATA
+        ragged += rg
         structs.append(N.ExampleRequest(model_name=b"model", model_name_len=5, has_version=1, order=N.ORDER_UPB, version=1,
                                         n_examples=n, n_features=len(preps), flags=0, features=feats))
         keep.append((preps, feats))
-    return (N.ExampleRequest * len(structs))(*structs), keep
+    rga = (N.Ragged * len(ragged))(*ragged) if any(g.lengths for g in ragged) else None
+    return (N.ExampleRequest * len(structs))(*structs), rga, keep
+
+
+def profile_split(lib, g, eager, calls):
+    """per-kernel device time of `calls` eager encodes, profiler on"""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+
+    torch.cuda.init()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(calls):
+            eager()
+        N.check(lib.b200tfs_sync(g.ctx))
+    split = {}
+    for e in prof.key_averages():
+        if "ex_" in e.key:
+            total = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
+            split[e.key] = {"count": e.count, "avg_us": total / max(e.count, 1)}
+    return split
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--runs", type=int, default=3)
+    ap.add_argument("--workloads", default="W1,W2,W3,V1,V2,V3,V4", help="comma-separated workloads to run")
+    ap.add_argument("--profile", default="", help="only the per-kernel split of these workloads (comma-separated)")
     ap.add_argument("--json", metavar="PATH", help="write every number of the run to PATH as JSON")
     args = ap.parse_args()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -106,22 +182,24 @@ def main():
     lib = N.load()
     codec = Codec(0)
     out = {"card": card, "calls": args.calls, "runs": args.runs, "workloads": {}}
-    for name, dicts in W.items():
+    profile_only = [w for w in args.profile.split(",") if w]
+    for name in (profile_only or args.workloads.split(",")):
+        dicts = W[name]()
         g = Ctx()       # a context per workload: the graph captured below pins its scratch buffers
         refs = [host_ref(d) for d in dicts]
-        col_bytes = sum(a.nbytes for d in dicts for a in d.values())
+        col_bytes = sum(used_bytes(d) for d in dicts)
         wire_bytes = sum(len(w) for w in refs)
         moved = col_bytes + wire_bytes
         # device columns
         ptrs = []
         for d in dicts:
             row = []
-            for a in d.values():
+            for a in arrays(d):
                 p = g.malloc(a.nbytes)
                 N.check(lib.b200tfs_memcpy_h2d(g.ctx, p, a.ctypes.data, a.nbytes))
                 row.append(p)
             ptrs.append(row)
-        reqs, keep = build(dicts, ptrs)
+        reqs, rga, keep = build(dicts, ptrs)
         n = len(dicts)
         cap = C.c_uint64()
         N.check(lib.b200tfs_example_arena_size(n, reqs, C.byref(cap)))
@@ -129,7 +207,19 @@ def main():
         off, ln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
 
         def eager():
-            N.check(lib.b200tfs_encode_example_requests_async(g.ctx, n, reqs, arena, cap.value))
+            if rga is None:
+                N.check(lib.b200tfs_encode_example_requests_async(g.ctx, n, reqs, arena, cap.value))
+            else:
+                N.check(lib.b200tfs_encode_example_requests_ragged_async(g.ctx, n, reqs, rga, arena, cap.value))
+
+        if profile_only:
+            for _ in range(3):
+                eager()
+            N.check(lib.b200tfs_sync(g.ctx))
+            split = profile_split(lib, g, eager, args.calls)
+            out[f"{name}_kernels"] = split
+            print(name, "kernels", json.dumps(split), flush=True)
+            continue
 
         def check_arena():
             N.check(lib.b200tfs_encode_results(g.ctx, n, off, ln))
@@ -156,14 +246,20 @@ def main():
         check_arena()
         N.check(lib.b200tfs_graph_destroy(ge))
         # _host from pinned columns (another context: the graph above pins this one's scratch buffers)
-        pinned = [{k: codec.pinned_empty(a.shape, a.dtype) for k, a in d.items()} for d in dicts]
-        for p, d in zip(pinned, dicts):
-            for k in d:
-                p[k][...] = d[k]
-        hreqs, hkeep = build(pinned)
+        def pin(a):
+            p = codec.pinned_empty(np.shape(a), np.asarray(a).dtype)
+            p[...] = a
+            return p
+        pinned = [{k: RaggedColumn(pin(v.values), pin(v.lengths)) if isinstance(v, RaggedColumn) else pin(v) for k, v in d.items()}
+                  for d in dicts]
+        hreqs, hrga, hkeep = build(pinned)
         wire = N.PinnedBuffer(cap.value)
         hoff, hln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
-        host = lambda: N.check(lib.b200tfs_encode_example_requests_host(codec.ctx, n, hreqs, wire.ptr, cap.value, hoff, hln))  # noqa: E731
+        if hrga is None:
+            host = lambda: N.check(lib.b200tfs_encode_example_requests_host(codec.ctx, n, hreqs, wire.ptr, cap.value, hoff, hln))  # noqa: E731
+        else:
+            host = lambda: N.check(lib.b200tfs_encode_example_requests_ragged_host(codec.ctx, n, hreqs, hrga, wire.ptr, cap.value,  # noqa: E731
+                                                                                    hoff, hln))
         for _ in range(3):
             host()
         res["host_pinned_us"] = [timed_host(host, args.calls) for _ in range(args.runs)]
@@ -198,19 +294,7 @@ def main():
             out["predict_same_bytes_async_us"] = [g.timed(pe, args.calls) for _ in range(args.runs)]
             print("predict W1-bytes", out["predict_same_bytes_async_us"], flush=True)
         if name == "W2":     # per-kernel split, profiler on, in a run of its own
-            import torch
-            from torch.profiler import ProfilerActivity, profile
-
-            torch.cuda.init()
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                for _ in range(args.calls):
-                    eager()
-                N.check(lib.b200tfs_sync(g.ctx))
-            split = {}
-            for e in prof.key_averages():
-                if "ex_" in e.key:
-                    total = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
-                    split[e.key] = {"count": e.count, "avg_us": total / max(e.count, 1)}
+            split = profile_split(lib, g, eager, args.calls)
             out["W2_kernels"] = split
             print("W2 kernels", json.dumps(split), flush=True)
     if args.json:
