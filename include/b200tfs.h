@@ -696,6 +696,36 @@ int b200tfs_encode_example_requests_ragged_host(b200tfs_ctx* ctx, int32_t n, con
                                                 const b200tfs_ragged* ragged, void* wire_host, uint64_t wire_cap, uint64_t* rec_off,
                                                 uint64_t* rec_len);
 
+/* What message carries a request's examples: one entry per request, parallel to reqs (targets == NULL: every request LIST).
+ *   B200TFS_EXAMPLES_LIST:           the ClassificationRequest / RegressionRequest above (key ignored).
+ *   B200TFS_EXAMPLES_PREDICT_STRING: a PredictRequest with one input, `key`, a DT_STRING tensor of shape [n_examples] whose
+ *                                    string_val holds every example serialised (the input of a model that runs tf.io.parse_example,
+ *                                    e.g. a TFX or Estimator export's serving_default).  Its bytes are those of
+ *                                    PredictRequest{model_spec, inputs[key] = TensorProto{dtype: DT_STRING, tensor_shape {dim {size:
+ *                                    n}}, string_val: [e.SerializeToString(deterministic=True) for e in the examples]}}
+ *                                    serialised with SerializeToString(deterministic=True); each example's bytes are exactly its
+ *                                    bytes in the example_list.
+ * A call may mix both.  An unknown kind, a negative key_len or a NULL key with key_len > 0: B200TFS_E_ARG; a key over 2 GiB:
+ * B200TFS_E_TOOBIG - checked before the context is looked at.                                                                  */
+#define B200TFS_EXAMPLES_LIST 0
+#define B200TFS_EXAMPLES_PREDICT_STRING 1
+typedef struct b200tfs_example_target {
+  int32_t kind;             /* B200TFS_EXAMPLES_*                                                                                 */
+  int32_t pad_;
+  const char* key;          /* PREDICT_STRING: the input's key bytes (UTF-8, not NUL terminated)                                  */
+  int64_t key_len;
+} b200tfs_example_target;
+/* b200tfs_example_request_size, b200tfs_example_arena_size, b200tfs_encode_example_requests_ragged_async and
+ * b200tfs_encode_example_requests_ragged_host with targets (target / targets == NULL: those calls themselves).                  */
+int b200tfs_example_target_request_size(const b200tfs_example_request* r, const b200tfs_example_target* target, uint64_t* total_len);
+int b200tfs_example_target_arena_size(int32_t n, const b200tfs_example_request* reqs, const b200tfs_example_target* targets,
+                                      uint64_t* bytes);
+int b200tfs_encode_example_targets_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                         const b200tfs_example_target* targets, void* arena_dev, uint64_t arena_cap);
+int b200tfs_encode_example_targets_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                        const b200tfs_example_target* targets, void* wire_host, uint64_t wire_cap, uint64_t* rec_off,
+                                        uint64_t* rec_len);
+
 /* ---- Classify / Regress responses: a batch of responses into one value or score array ----------------------
  * What ClassificationResponse.FromString / RegressionResponse.FromString followed by a loop over the result give, concatenated
  * along the example axis across the n responses: row order is response 0's examples, then response 1's, and so on.

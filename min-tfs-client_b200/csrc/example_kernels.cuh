@@ -8,15 +8,17 @@
 //                    for: the count kernel has finished), then a block scan of the example sizes gives every example's offset
 //   ex_emit_kernel   one CTA per contiguous range of examples, i.e. of wire: warps write whole examples (framing, converted float
 //                    rows, int64 varints) into a shared-memory image of the wire, which the CTA stores with aligned 128-bit
-//                    vectors; an example larger than the image is written in place by one warp
-//   ex_frame_kernel  one warp per request: the examples' total, the request prefix in front of the anchor, rec_off / rec_len /
-//                    status to pinned memory
+//                    vectors; an example larger than the image is written in place by one warp.  ex_emit_predict_kernel is the
+//                    same for the spans of Predict requests, whose examples start with the string_val tag
+//   ex_frame_kernel  one warp per request: the examples' total, the request prefix in front of the anchor (an example_list or
+//                    a Predict string_val, plan.h ExReq), rec_off / rec_len / status to pinned memory
 //
 // count, emit and the example writer take kRagged: a call with a ragged column launches the `true` instantiations, in which a
 // ragged column's row ends after ex_elems elements; every other call runs the `false` ones, which read row_elems as before.
 //
 // What the reference does here: requests.py examples_from_input_dict (a Python loop per example and per feature) and the
-// protobuf runtime serialising the ClassificationRequest / RegressionRequest it filled.
+// protobuf runtime serialising the ClassificationRequest / RegressionRequest it filled, or every example and then the
+// PredictRequest whose DT_STRING input holds them.
 
 // float32 bits of element j of a float row: what astype(float32) and the trip through a Python float give
 __device__ __forceinline__ uint32_t ex_f64_to_f32_bits(uint64_t d) {
@@ -56,8 +58,9 @@ __device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
   return v;
 }
 
-// Example i of request q, written by the calling warp at w (shared or global memory).
-template <bool kRagged>
+// Example i of request q, written by the calling warp at w (shared or global memory), behind the tag kTag: 0A
+// (ExampleList.examples) or 42 (TensorProto.string_val).
+template <bool kRagged, uint8_t kTag>
 __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, uint8_t* w) {
   const uint32_t lane = threadIdx.x & 31;
   uint64_t F = 0, hl;
@@ -72,7 +75,7 @@ __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, 
   const uint64_t X = 1 + varint_len(F) + F;
   uint64_t pos = 2 + varint_len(X) + varint_len(F);
   if (lane == 0) {
-    w[0] = 0x0A;
+    w[0] = kTag;
     const uint32_t p = 1 + put_varint(w + 1, X);
     w[p] = 0x0A;
     put_varint(w + p + 1, F);
@@ -217,8 +220,8 @@ __device__ __forceinline__ void ex_flush(uint8_t* arena, const uint8_t* img, uin
   for (uint64_t x = b + threadIdx.x; x < hi; x += blockDim.x) arena[x] = img[x - ws];
 }
 
-template <bool kRagged>
-__global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_constant__ ExTables T) {
+template <bool kRagged, uint8_t kTag>
+__device__ __forceinline__ void ex_emit(const ExTables& T) {
   __shared__ __align__(16) uint8_t img[kExStage + 16];
   __shared__ uint64_t next;
   constexpr uint32_t kWarps = kExEmitThreads / 32;
@@ -241,7 +244,7 @@ __global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_co
     __syncthreads();
     const uint64_t j = next;
     if (j > i) {
-      for (uint64_t e = i + warp; e < j; e += kWarps) ex_write_example<kRagged>(T, q, e, img + (A + ex_start<kRagged>(T, q, e) - ws));
+      for (uint64_t e = i + warp; e < j; e += kWarps) ex_write_example<kRagged, kTag>(T, q, e, img + (A + ex_start<kRagged>(T, q, e) - ws));
       __syncthreads();
       const uint64_t be = A + ex_end<kRagged>(T, q, j - 1), cut = be & ~15ull;
       if (cut > ws) {                        // store every whole vector; the partial one moves to the front of the image
@@ -254,7 +257,7 @@ __global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_co
       i = j;
     } else {                                 // example i alone is larger than the image: one warp writes it in place
       ex_flush(T.arena, img, ws, lo, A + ex_start<kRagged>(T, q, i));
-      if (warp == 0) ex_write_example<kRagged>(T, q, i, T.arena + A + ex_start<kRagged>(T, q, i));
+      if (warp == 0) ex_write_example<kRagged, kTag>(T, q, i, T.arena + A + ex_start<kRagged>(T, q, i));
       lo = A + ex_end<kRagged>(T, q, i);
       ws = lo & ~15ull;
       ++i;
@@ -262,6 +265,16 @@ __global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_co
     __syncthreads();
   }
   ex_flush(T.arena, img, ws, lo, A + ex_end<kRagged>(T, q, sp.e1 - 1));
+}
+
+// The tag is a template argument, so the example_list kernels keep the registers they had before Predict requests existed.
+template <bool kRagged>
+__global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_constant__ ExTables T) {
+  ex_emit<kRagged, 0x0A>(T);
+}
+template <bool kRagged>
+__global__ void __launch_bounds__(kExEmitThreads) ex_emit_predict_kernel(const __grid_constant__ ExTables T) {
+  ex_emit<kRagged, 0x42>(T);
 }
 
 constexpr uint32_t kExFrameWarps = 4;
@@ -276,23 +289,32 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __gr
   } else {
     el = q.n_ex * q.fixed_size;
   }
-  if (lane) return;
-  // [00 be32(msg)] model_spec 12 vi(input) 0A vi(example_list) | examples...
-  const uint64_t input = 1 + varint_len(el) + el, msg = q.spec_len + 1 + varint_len(input) + input;
-  const uint64_t pre = (q.grpc ? 5 : 0) + q.spec_len + 1 + varint_len(input) + 1 + varint_len(el);
+  // [00 be32(msg)] spec 12 vi(outer) mid inner_tag vi(inner) head | examples...   (plan.h ExReq)
+  const uint64_t inner = q.head_len + el, outer = q.mid_len + 1 + varint_len(inner) + inner;
+  const uint64_t msg = q.spec_len + 1 + varint_len(outer) + outer;
+  const uint64_t pre = (q.grpc ? 5 : 0) + msg - el;
   int32_t st = B200TFS_OK;
   if (T.bad && T.bad[r]) st = B200TFS_E_SHAPE;
   else if (msg > 0x7FFFFFFFull) st = B200TFS_E_TOOBIG;
   else if (q.anchor + el > q.slot_end) st = B200TFS_E_SIZE;
-  T.status[r] = st;
-  T.rec_off[r] = st ? 0 : q.anchor - pre;
-  T.rec_len[r] = st ? 0 : pre + el;
+  if (lane == 0) {
+    T.status[r] = st;
+    T.rec_off[r] = st ? 0 : q.anchor - pre;
+    T.rec_len[r] = st ? 0 : pre + el;
+  }
   if (st) return;
   uint8_t* w = T.arena + q.anchor - pre;
-  if (q.grpc) { *w++ = 0; *w++ = (uint8_t)(msg >> 24); *w++ = (uint8_t)(msg >> 16); *w++ = (uint8_t)(msg >> 8); *w++ = (uint8_t)msg; }
-  for (uint32_t b = 0; b < q.spec_len; ++b) *w++ = T.blob[q.spec_off + b];
-  *w++ = 0x12; w += put_varint(w, input);
-  *w++ = 0x0A; put_varint(w, el);
+  // the host-written bytes (spec, mid, head: one run in the blob) by the whole warp, the headers between them by lane 0
+  const uint32_t at_spec = q.grpc ? 5 : 0, at_outer = at_spec + q.spec_len, at_mid = at_outer + 1 + varint_len(outer);
+  const uint32_t at_inner = at_mid + q.mid_len, at_head = at_inner + 1 + varint_len(inner);
+  for (uint32_t k = lane; k < q.spec_len + q.mid_len + q.head_len; k += 32) {
+    const uint32_t d = k < q.spec_len ? at_spec + k : k < q.spec_len + q.mid_len ? at_mid + (k - q.spec_len) : at_head + (k - q.spec_len - q.mid_len);
+    w[d] = T.blob[q.spec_off + k];
+  }
+  if (lane) return;
+  if (q.grpc) { w[0] = 0; w[1] = (uint8_t)(msg >> 24); w[2] = (uint8_t)(msg >> 16); w[3] = (uint8_t)(msg >> 8); w[4] = (uint8_t)msg; }
+  w[at_outer] = 0x12; put_varint(w + at_outer + 1, outer);
+  w[at_inner] = (uint8_t)q.inner_tag; put_varint(w + at_inner + 1, inner);
 }
 
 cudaError_t launch_example_requests(const ExTables& T, cudaStream_t stream, uint32_t* launched) {
@@ -304,9 +326,17 @@ cudaError_t launch_example_requests(const ExTables& T, cudaStream_t stream, uint
     ex_scan_kernel<<<T.n_tiles, kExTile, 0, stream>>>(T);
     *launched += 2;
   }
-  if (T.n_spans) {
-    if (ragged) ex_emit_kernel<true><<<T.n_spans, kExEmitThreads, 0, stream>>>(T);
-    else ex_emit_kernel<false><<<T.n_spans, kExEmitThreads, 0, stream>>>(T);
+  const uint32_t n_list = T.n_spans - T.n_predict_spans;
+  if (n_list) {
+    if (ragged) ex_emit_kernel<true><<<n_list, kExEmitThreads, 0, stream>>>(T);
+    else ex_emit_kernel<false><<<n_list, kExEmitThreads, 0, stream>>>(T);
+    *launched += 1;
+  }
+  if (T.n_predict_spans) {    // the spans of the Predict requests come last
+    ExTables P = T;
+    P.spans += n_list;
+    if (ragged) ex_emit_predict_kernel<true><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
+    else ex_emit_predict_kernel<false><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
     *launched += 1;
   }
   if (T.n_req) { ex_frame_kernel<<<(T.n_req + kExFrameWarps - 1) / kExFrameWarps, 32 * kExFrameWarps, 0, stream>>>(T); *launched += 1; }

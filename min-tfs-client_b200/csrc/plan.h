@@ -362,9 +362,14 @@ struct ExFeat {             // one column of one request, in wire order
   const int64_t* lengths;   // a ragged column: example i takes min(max(lengths[i], 0), max_len) * unit elements; NULL: dense
   uint64_t max_len, unit;   // row_elems == max_len * unit
 };
+// The prefix the frame kernel writes in front of the examples, for both targets:
+//   [00 be32(msg)] spec 12 vi(outer) mid inner_tag vi(inner) head | examples
+//   example_list (Classify / Regress):  outer = Input, mid and head empty, inner_tag 0A, inner = ExampleList
+//   Predict string_val:                 outer = the inputs map entry, mid = 0A vi(klen) key, inner_tag 12, inner = TensorProto,
+//                                       head = 08 07 12 vi(shape) {tensor_shape: dim {size: n}}
 struct ExReq {
   uint32_t first_feat, n_feat, n_int;   // integer columns (their entries per example in ExTables::L)
-  uint32_t spec_off, spec_len;          // the model_spec field (tag included) in ExTables::blob
+  uint32_t spec_off, spec_len;          // the model_spec field (tag included) in ExTables::blob, followed there by mid and head
   uint32_t grpc;                        // gRPC's five-byte length-prefixed-message header in front
   uint32_t first_tile, n_tiles;         // count / scan tiles (requests whose size depends on their values)
   uint64_t n_ex, ex0;                   // examples, and the first one's index in the per-example tables of the call
@@ -372,12 +377,14 @@ struct ExReq {
   uint64_t fixed_size;                  // bytes of every example in the example_list (its tag included); 0: the size depends on
                                         // the values (an integer or a ragged column), S and off hold each example's
   uint64_t anchor, slot_end;            // arena offsets: where example 0 starts, where the slot ends
+  uint32_t mid_len, head_len, inner_tag, pad;   // the Predict prefix above (example_list: 0, 0, 0A); last, because among the
+                                                // fields the emit kernel reads they cost ex_emit_kernel<false> 12 registers
 };
 struct ExSpan { uint32_t req, pad; uint64_t e0, e1; };   // a CTA's examples [e0, e1) of request `req`
 struct ExTables {
   const ExReq* reqs; const ExFeat* feats; const uint8_t* blob;
   const ExSpan* tiles;                  // count / scan CTAs
-  const ExSpan* spans;                  // emit CTAs
+  const ExSpan* spans;                  // emit CTAs: those of the example_list requests, then the n_predict_spans of the Predict ones
   uint64_t* L;                          // packed length of every (example, integer column)
   uint64_t* S;                          // bytes of every example of a request whose size depends on its values
   uint64_t* off;                        // its offset from the anchor
@@ -386,7 +393,7 @@ struct ExTables {
                                         // (zeroed by the host in every call); NULL otherwise
   uint8_t* arena;
   uint64_t* rec_off; uint64_t* rec_len; int32_t* status;   // pinned host memory: read by b200tfs_encode_results
-  uint32_t n_req, n_tiles, n_spans;
+  uint32_t n_req, n_tiles, n_spans, n_predict_spans;
 };
 // Bytes of one feature map entry (its tag included) whose list payload is P bytes; *hl receives those in front of the payload:
 //   0A vi(entry) 0A vi(klen) key 12 vi(Feature) {12 float_list | 1A int64_list} vi(list) [0A vi(P) payload]
@@ -396,7 +403,8 @@ B2_PLAN_HD uint64_t ex_entry_len(uint64_t P, uint64_t klen, uint64_t* hl) {
   *hl = 1 + varint_len(entry) + entry - P;
   return 1 + varint_len(entry) + entry;
 }
-// bytes of one example in the example_list (its tag included) whose map entries add up to F bytes: 0A vi(X) 0A vi(F) entries
+// bytes of one example in the example_list or string_val (its tag included) whose map entries add up to F bytes:
+// {0A | 42} vi(X) 0A vi(F) entries
 B2_PLAN_HD uint64_t ex_example_len(uint64_t F) {
   const uint64_t x = 1 + varint_len(F) + F;
   return 1 + varint_len(x) + x;

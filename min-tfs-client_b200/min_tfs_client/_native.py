@@ -121,6 +121,15 @@ class Ragged(C.Structure):
     _fields_ = [("lengths", C.c_void_p), ("max_len", C.c_int64), ("unit", C.c_int64), ("flags", C.c_uint32), ("pad_", C.c_int32)]
 
 
+EXAMPLES_LIST, EXAMPLES_PREDICT_STRING = 0, 1
+
+
+class ExampleTarget(C.Structure):
+    """b200tfs_example_target: what carries one request's examples - a ClassificationRequest / RegressionRequest (EXAMPLES_LIST)
+    or a PredictRequest whose input ``key`` is a DT_STRING vector of the serialized examples (EXAMPLES_PREDICT_STRING)."""
+    _fields_ = [("kind", C.c_int32), ("pad_", C.c_int32), ("key", C.c_char_p), ("key_len", C.c_int64)]
+
+
 class PadInput(C.Structure):
     """b200tfs_pad_input: the shapes of one input of b200tfs_encode_padded_requests_async (int64[n, cols]; cols 1: row counts)."""
     _fields_ = [("shapes", C.c_void_p), ("cols", C.c_int32), ("pad_", C.c_int32)]
@@ -227,6 +236,12 @@ SIGNATURES = {
                                                                C.c_uint64]),
     "b200tfs_encode_example_requests_ragged_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), _vp,
                                                               C.c_uint64, _u64p, _u64p]),
+    "b200tfs_example_target_request_size": (C.c_int, [C.POINTER(ExampleRequest), C.POINTER(ExampleTarget), _u64p]),
+    "b200tfs_example_target_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), C.POINTER(ExampleTarget), _u64p]),
+    "b200tfs_encode_example_targets_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged),
+                                                       C.POINTER(ExampleTarget), _vp, C.c_uint64]),
+    "b200tfs_encode_example_targets_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged),
+                                                      C.POINTER(ExampleTarget), _vp, C.c_uint64, _u64p, _u64p]),
     "b200tfs_example_response_bound": (C.c_int, [C.c_int32, C.c_int32, _u64p, _u64p, _u64p]),
     "b200tfs_decode_example_responses": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64, _vp, C.c_uint64]),
     "b200tfs_decode_example_responses_host_async": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64, _vp,

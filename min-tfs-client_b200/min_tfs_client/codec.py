@@ -231,14 +231,30 @@ def _example_columns(input_dict: Mapping):
     return n, preps
 
 
-def _host_example_request(model_name, model_version, input_dict, grpc_frame: bool) -> bytes:
-    """A request with a column the device route does not take, as ``examples_from_input_dict`` and protobuf make it."""
-    from tensorflow_serving.apis.classification_pb2 import ClassificationRequest
+def _host_example_request(model_name, model_version, input_dict, grpc_frame: bool, predict_input=None) -> bytes:
+    """A request with a column the device route does not take, as ``examples_from_input_dict`` and protobuf make it: a
+    ClassificationRequest, or with ``predict_input`` a PredictRequest whose input of that key is the DT_STRING ``[n]`` tensor of
+    the examples, each serialized with ``deterministic=True``."""
+    from .requests import TensorServingClient, examples_from_input_dict
 
-    from .requests import TensorServingClient
+    if predict_input is None:
+        from tensorflow_serving.apis.classification_pb2 import ClassificationRequest
 
-    wire = TensorServingClient._make_example_request(None, ClassificationRequest, model_name, input_dict, model_version) \
-        .SerializeToString(deterministic=True)
+        req = TensorServingClient._make_example_request(None, ClassificationRequest, model_name, input_dict, model_version)
+    else:
+        from tensorflow_serving.apis.predict_pb2 import PredictRequest
+
+        req = PredictRequest()
+        req.model_spec.name = model_name
+        if model_version is not None:
+            req.model_spec.version.value = model_version
+        examples = examples_from_input_dict(input_dict).example_list.examples
+        key = predict_input.decode("utf-8") if isinstance(predict_input, bytes) else predict_input
+        t = req.inputs[key]
+        t.dtype = DT_STRING
+        t.tensor_shape.dim.add().size = len(examples)
+        t.string_val.extend(e.SerializeToString(deterministic=True) for e in examples)
+    wire = req.SerializeToString(deterministic=True)
     return (b"\x00" + len(wire).to_bytes(4, "big") + wire) if grpc_frame else wire
 
 
@@ -713,9 +729,12 @@ class Codec:
         return self.encode_predict_requests([(model_name, model_version, input_dict)], **kw)[0]
 
     def encode_example_requests(self, requests: Iterable[Tuple[str, Optional[int], Mapping]], *, order="deterministic",
-                                grpc_frame: bool = False) -> List[bytes]:
+                                grpc_frame: bool = False, predict_input=None) -> List[bytes]:
         """Each item is ``(model_name, model_version, input_dict)``; returns one ClassificationRequest / RegressionRequest wire
-        per item (the two messages share their field numbers, so the bytes serve both RPCs).
+        per item (the two messages share their field numbers, so the bytes serve both RPCs).  With ``predict_input`` (a str or
+        bytes key) each wire is instead a PredictRequest for a model that parses serialized tf.Examples: its one input of that
+        key is a DT_STRING tensor of shape ``[n]`` whose ``string_val`` holds every example, serialized as the protobuf runtime
+        serializes it with ``deterministic=True``.
 
         The bytes equal ``_make_example_request(...).SerializeToString(deterministic=True)`` of the request
         ``examples_from_input_dict`` builds - one tf.Example per row, 0-d arrays repeated in every example - with
@@ -726,13 +745,17 @@ class Codec:
         host by ``examples_from_input_dict``, in deterministic order; device arrays of such dtypes raise ValueError.
         """
         order_code = _ORDER[order] if isinstance(order, str) else int(order)
+        target = None
+        if predict_input is not None:
+            pkey = predict_input.encode("utf-8") if isinstance(predict_input, str) else bytes(predict_input)
+            target = N.ExampleTarget(kind=N.EXAMPLES_PREDICT_STRING, key=pkey, key_len=len(pkey))
         items = list(requests)
         out: List[Optional[bytes]] = [None] * len(items)
         keep, structs, dev_idx, ragged = [], [], [], []
         for i, (model_name, model_version, input_dict) in enumerate(items):
             cols = _example_columns(input_dict)
             if cols is None:
-                out[i] = _host_example_request(model_name, model_version, input_dict, grpc_frame)
+                out[i] = _host_example_request(model_name, model_version, input_dict, grpc_frame, predict_input)
                 continue
             n, preps = cols
             feats = (N.Feature * max(len(preps), 1))(*[p[0] for p in preps])
@@ -748,14 +771,12 @@ class Codec:
             m = len(dev_idx)
             reqs = (N.ExampleRequest * m)(*structs)
             cap = C.c_uint64()
-            N.check(self._lib.b200tfs_example_arena_size(m, reqs, C.byref(cap)))
+            tg = (N.ExampleTarget * m)(*[target] * m) if target is not None else None
+            N.check(self._lib.b200tfs_example_target_arena_size(m, reqs, tg, C.byref(cap)))
             wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
             off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
-            if any(g.lengths for g in ragged):
-                rg = (N.Ragged * len(ragged))(*ragged)
-                N.check(self._lib.b200tfs_encode_example_requests_ragged_host(self._ctx, m, reqs, rg, wire.ctypes.data, cap.value, off, ln))
-            else:
-                N.check(self._lib.b200tfs_encode_example_requests_host(self._ctx, m, reqs, wire.ctypes.data, cap.value, off, ln))
+            rg = (N.Ragged * len(ragged))(*ragged) if any(g.lengths for g in ragged) else None
+            N.check(self._lib.b200tfs_encode_example_targets_host(self._ctx, m, reqs, rg, tg, wire.ctypes.data, cap.value, off, ln))
             for j, i in enumerate(dev_idx):
                 out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
         return out  # type: ignore[return-value]

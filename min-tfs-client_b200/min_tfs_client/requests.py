@@ -178,6 +178,14 @@ def gpu_example_request_serializer(request) -> bytes:
     return get_codec().encode_example_requests([request])[0]
 
 
+def gpu_predict_examples_serializer(request) -> bytes:
+    """``request_serializer`` for ``channel.unary_unary(PREDICT_METHOD, ...)`` to a model that parses serialized tf.Examples:
+    (model_name, model_version, input_dict, input_key) -> a PredictRequest whose input ``input_key`` is the DT_STRING ``[n]``
+    tensor of the examples ``examples_from_input_dict`` builds, each serialized with ``deterministic=True``, packed on the GPU."""
+    model_name, model_version, input_dict, input_key = request
+    return get_codec().encode_example_requests([(model_name, model_version, input_dict)], predict_input=input_key)[0]
+
+
 def gpu_response_deserializer(wire: bytes) -> PredictResponseView:
     """``response_deserializer`` for ``channel.unary_unary``: bytes -> lazy response view."""
     return PredictResponseView(wire)
@@ -206,6 +214,15 @@ class TensorServingClient:
     def predict_request(self, model_name: str, input_dict: Dict[str, np.ndarray], timeout: int = 60,
                         model_version: Optional[int] = None) -> PredictResponseView:
         return self._predict((model_name, model_version, input_dict), timeout)
+
+    def predict_examples_request(self, model_name: str, input_dict: Dict[str, np.ndarray], input_key: str = "examples",
+                                 timeout: int = 60, model_version: Optional[int] = None) -> PredictResponseView:
+        """Predict on a model whose signature takes serialized tf.Examples (a DT_STRING vector it parses with
+        ``tf.io.parse_example``, e.g. a TFX Trainer or Estimator export's ``serving_default``): one example per row of
+        ``input_dict`` as ``examples_from_input_dict`` builds it, sent as input ``input_key``."""
+        call = self._channel.unary_unary(PREDICT_METHOD, request_serializer=gpu_predict_examples_serializer,
+                                         response_deserializer=gpu_response_deserializer)
+        return call((model_name, model_version, input_dict, input_key), timeout)
 
     def _make_example_request(self, request_pb, model_name, input_dict, model_version):
         request = request_pb()

@@ -8,6 +8,8 @@ Workloads (one request each unless stated):
   V2  65 536 examples x {emb f32 ragged [65536, 64], lengths uniform in 1..64}   float-only, but counted and scanned (beside W1)
   V3  4 096 examples x {tokens int32 ragged [4096, 512], lengths geometric with mean ~40, capped at 512}   worst-case emit spans
   V4  256 requests of 64 examples shaped like V1
+  W1P, W2P, V1P  W1, W2 and V1 framed for Predict: a PredictRequest whose input "examples" is the DT_STRING [n] vector of the
+      serialized examples (b200tfs_encode_example_targets_*), each run beside its Classify form
 Legs: the _async entry point eager (device columns -> device arena), the same captured once as a CUDA graph and replayed,
 _host from pinned columns (copies both ways included), and examples_from_input_dict + SerializeToString(deterministic=True)
 on one host core.  CUDA events over >= 20 calls after warm-up, three runs each; bytes = column bytes read + wire bytes
@@ -16,7 +18,9 @@ of the same f32[65536, 64] as one tensor, and W2 is split by kernel with torch.p
 bytes are checked against the host path after its timed region.  Needs a GPU; --json PATH also writes every number there.
 The V workloads (ragged columns, b200tfs_encode_example_requests_ragged_*) count the values their lengths use, not the padded
 columns, and the lengths; their host path builds the request one example at a time from the unchanged dense code, as a user
-without ragged columns would.  --profile V1,V3 runs only the per-kernel split of the named workloads (profiler on).
+without ragged columns would.  The P workloads' host path is the one a Predict user has today: examples_from_input_dict,
+SerializeToString(deterministic=True) of every example, string_val.extend and the PredictRequest's SerializeToString.
+--profile V1,V3 runs only the per-kernel split of the named workloads (profiler on).
 
   python tools/example_probe.py [--calls 20] [--runs 3] [--workloads W1,V1,...] [--profile V1,V3] [--json PATH]
 """
@@ -36,7 +40,9 @@ sys.path.insert(0, os.path.join(REPO, "min-tfs-client_b200"))
 from min_tfs_client import _native as N  # noqa: E402
 from min_tfs_client.codec import Codec, RaggedColumn, _example_columns  # noqa: E402
 from min_tfs_client.requests import TensorServingClient, examples_from_input_dict  # noqa: E402
+from tensorflow.core.framework import types_pb2  # noqa: E402
 from tensorflow_serving.apis.classification_pb2 import ClassificationRequest  # noqa: E402
+from tensorflow_serving.apis.predict_pb2 import PredictRequest  # noqa: E402
 
 PEAK = 3.35e12
 
@@ -54,21 +60,37 @@ def workloads(rng):
             "V2": lambda: [{"emb": RaggedColumn(rng.standard_normal((65536, 64)).astype(np.float32), rng.integers(1, 65, 65536))}],
             "V3": lambda: [{"tokens": RaggedColumn(rng.integers(0, 32_000, (4096, 512), dtype=np.int32),
                                                    np.minimum(rng.geometric(1 / 40, 4096), 512))}],
-            "V4": lambda: [v1(64) for _ in range(256)]}
+            "V4": lambda: [v1(64) for _ in range(256)],
+            "W1P": lambda: [{"dense": rng.standard_normal((65536, 64)).astype(np.float32)}], "W2P": lambda: [w2(16384)],
+            "V1P": lambda: [v1(16384)]}
 
 
-def host_ref(d):
+def host_ref(d, predict=False):
     """the host path: examples_from_input_dict + SerializeToString; with ragged columns one example at a time (each example the
-    one examples_from_input_dict makes of that example's rows), merged in order"""
-    if not any(isinstance(v, RaggedColumn) for v in d.values()):
-        return TensorServingClient._make_example_request(None, ClassificationRequest, "model", d, 1).SerializeToString(deterministic=True)
-    req = TensorServingClient._make_example_request(None, ClassificationRequest, "model", {}, 1)
-    n = next(v.shape[0] for v in d.values() if isinstance(v, RaggedColumn))
-    for i in range(n):
-        one = {k: v.values[i:i + 1, :int(v.lengths[i])] if isinstance(v, RaggedColumn) else v if np.ndim(v) == 0 else v[i:i + 1]
-               for k, v in d.items()}
-        req.input.example_list.examples.extend(examples_from_input_dict(one).example_list.examples)
-    return req.SerializeToString(deterministic=True)
+    one examples_from_input_dict makes of that example's rows), merged in order.  predict: every example serialized into the
+    string_val of a PredictRequest's DT_STRING input "examples" instead"""
+    if predict and not any(isinstance(v, RaggedColumn) for v in d.values()):
+        examples = examples_from_input_dict(d).example_list.examples
+    elif not any(isinstance(v, RaggedColumn) for v in d.values()):
+        req = TensorServingClient._make_example_request(None, ClassificationRequest, "model", d, 1)
+    else:
+        req = TensorServingClient._make_example_request(None, ClassificationRequest, "model", {}, 1)
+        n = next(v.shape[0] for v in d.values() if isinstance(v, RaggedColumn))
+        for i in range(n):
+            one = {k: v.values[i:i + 1, :int(v.lengths[i])] if isinstance(v, RaggedColumn) else v if np.ndim(v) == 0 else v[i:i + 1]
+                   for k, v in d.items()}
+            req.input.example_list.examples.extend(examples_from_input_dict(one).example_list.examples)
+        examples = req.input.example_list.examples
+    if not predict:
+        return req.SerializeToString(deterministic=True)
+    pr = PredictRequest()
+    pr.model_spec.name = "model"
+    pr.model_spec.version.value = 1
+    t = pr.inputs["examples"]
+    t.dtype = types_pb2.DT_STRING
+    t.tensor_shape.dim.add().size = len(examples)
+    t.string_val.extend(e.SerializeToString(deterministic=True) for e in examples)
+    return pr.SerializeToString(deterministic=True)
 
 
 def arrays(d):
@@ -171,7 +193,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--runs", type=int, default=3)
-    ap.add_argument("--workloads", default="W1,W2,W3,V1,V2,V3,V4", help="comma-separated workloads to run")
+    ap.add_argument("--workloads", default="W1,W1P,W2,W2P,W3,V1,V1P,V2,V3,V4", help="comma-separated workloads to run")
     ap.add_argument("--profile", default="", help="only the per-kernel split of these workloads (comma-separated)")
     ap.add_argument("--json", metavar="PATH", help="write every number of the run to PATH as JSON")
     args = ap.parse_args()
@@ -185,8 +207,9 @@ def main():
     profile_only = [w for w in args.profile.split(",") if w]
     for name in (profile_only or args.workloads.split(",")):
         dicts = W[name]()
+        predict = name.endswith("P")
         g = Ctx()       # a context per workload: the graph captured below pins its scratch buffers
-        refs = [host_ref(d) for d in dicts]
+        refs = [host_ref(d, predict) for d in dicts]
         col_bytes = sum(used_bytes(d) for d in dicts)
         wire_bytes = sum(len(w) for w in refs)
         moved = col_bytes + wire_bytes
@@ -201,13 +224,16 @@ def main():
             ptrs.append(row)
         reqs, rga, keep = build(dicts, ptrs)
         n = len(dicts)
+        tg = (N.ExampleTarget * n)(*[N.ExampleTarget(kind=N.EXAMPLES_PREDICT_STRING, key=b"examples", key_len=8)] * n) if predict else None
         cap = C.c_uint64()
-        N.check(lib.b200tfs_example_arena_size(n, reqs, C.byref(cap)))
+        N.check(lib.b200tfs_example_target_arena_size(n, reqs, tg, C.byref(cap)))
         arena = g.malloc(cap.value)
         off, ln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
 
         def eager():
-            if rga is None:
+            if predict:
+                N.check(lib.b200tfs_encode_example_targets_async(g.ctx, n, reqs, rga, tg, arena, cap.value))
+            elif rga is None:
                 N.check(lib.b200tfs_encode_example_requests_async(g.ctx, n, reqs, arena, cap.value))
             else:
                 N.check(lib.b200tfs_encode_example_requests_ragged_async(g.ctx, n, reqs, rga, arena, cap.value))
@@ -255,7 +281,10 @@ def main():
         hreqs, hrga, hkeep = build(pinned)
         wire = N.PinnedBuffer(cap.value)
         hoff, hln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
-        if hrga is None:
+        if predict:
+            host = lambda: N.check(lib.b200tfs_encode_example_targets_host(codec.ctx, n, hreqs, hrga, tg, wire.ptr, cap.value,  # noqa: E731
+                                                                            hoff, hln))
+        elif hrga is None:
             host = lambda: N.check(lib.b200tfs_encode_example_requests_host(codec.ctx, n, hreqs, wire.ptr, cap.value, hoff, hln))  # noqa: E731
         else:
             host = lambda: N.check(lib.b200tfs_encode_example_requests_ragged_host(codec.ctx, n, hreqs, hrga, wire.ptr, cap.value,  # noqa: E731
@@ -269,7 +298,7 @@ def main():
         for _ in range(args.runs):
             t0 = time.perf_counter()
             for d in dicts:
-                host_ref(d)
+                host_ref(d, predict)
             runs.append((time.perf_counter() - t0) * 1e6)
         res["protobuf_host_us"] = runs
         for leg in ("async_us", "graph_us", "host_pinned_us", "protobuf_host_us"):
