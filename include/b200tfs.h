@@ -623,13 +623,15 @@ int b200tfs_unpack_outputs_host(b200tfs_ctx* ctx, int32_t m, const b200tfs_outpu
  * (DT_FLOAT, DT_DOUBLE, DT_HALF) become float_list the way astype(float32) and a Python float make them: float32 signalling NaNs
  * quieted; float64 rounded to nearest even, NaN -> sign | 0x7FC00000 | (mantissa >> 29); float16 widened exactly, NaNs quieted.
  * Integer and bool columns become int64_list: sign-extended, uint64 wraps (2**64-1 is written as -1), a bool byte != 0 is 1.
- * A row of 0 elements still writes its empty list.  Strings (bytes_list) are not taken: such requests are assembled on the host.
+ * A row of 0 elements still writes its empty list.  Strings (bytes_list) are taken as DT_STRING columns with a b200tfs_bytes
+ * entry (the *_example_columns_* entry points, below); without one a DT_STRING column is B200TFS_E_DTYPE.
  * A variable-length (ragged) column is a padded one plus a b200tfs_ragged entry (the *_ragged entry points): row_elems is then the
  * padded row, and example i takes only the first lengths[i] * unit elements of its row.                                          */
 typedef struct b200tfs_feature {
   const void* data;     /* n_examples rows of row_elems elements (one row with B200TFS_F_BROADCAST), C-contiguous, native order,
                            aligned to the element size; a DEVICE pointer for the _async entry point                              */
-  int32_t src_dtype;    /* DT_FLOAT / DT_DOUBLE / DT_HALF / DT_INT8..64 / DT_UINT8..64 / DT_BOOL; others: B200TFS_E_DTYPE         */
+  int32_t src_dtype;    /* DT_FLOAT / DT_DOUBLE / DT_HALF / DT_INT8..64 / DT_UINT8..64 / DT_BOOL, DT_STRING with a b200tfs_bytes
+                           entry; others: B200TFS_E_DTYPE                                                                        */
   uint32_t flags;       /* B200TFS_F_DEVICE_DATA (the _host entry point: `data` is in HBM already), B200TFS_F_BROADCAST           */
   int64_t row_elems;    /* elements per example (a ragged column: its padded row, max_len * unit)                              */
   const char* key;      /* feature name bytes (UTF-8, not NUL terminated)                                                       */
@@ -725,6 +727,42 @@ int b200tfs_encode_example_targets_async(b200tfs_ctx* ctx, int32_t n, const b200
 int b200tfs_encode_example_targets_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
                                         const b200tfs_example_target* targets, void* wire_host, uint64_t wire_cap, uint64_t* rec_off,
                                         uint64_t* rec_len);
+
+/* String columns (bytes_list), laid out as Arrow / cuDF hold them: one byte buffer and int64 offsets.  One entry per feature of
+ * every request, in request-then-feature order, parallel to the features as b200tfs_ragged is.  offsets == NULL: not a bytes
+ * column.  Otherwise the feature has src_dtype DT_STRING, `data` is the byte buffer (data_len bytes, any alignment) and row_elems
+ * counts the strings of one example: string j is data[offsets[j], offsets[j+1]), the n_examples * row_elems strings (row_elems
+ * with B200TFS_F_BROADCAST) fill the rows in order, and offsets[0] need not be 0 (a sliced column).  With a b200tfs_ragged entry
+ * example i takes the first lengths[i] * unit strings of its padded row of max_len * unit.  Each string becomes one value of
+ * the example's bytes_list; a row of no strings still writes its empty list.
+ * The offsets of example i's row, starting at string b = i * row_elems (0 with B200TFS_F_BROADCAST), are read for its l_i
+ * strings and for the next row's start, and must satisfy
+ *     0 <= offsets[b] <= offsets[b+1] <= ... <= offsets[b + l_i] <= offsets[b + row_elems] <= data_len,
+ * so that the rows are disjoint and in order: a request's strings take at most data_len bytes (n_examples * data_len broadcast),
+ * which is what its arena slot is sized for.  Host offsets that break this: B200TFS_E_SHAPE before anything is launched.  Device
+ * offsets are checked by the kernels: that request gets B200TFS_E_SHAPE in b200tfs_encode_results (rec_off = rec_len = 0), every
+ * offset is clamped first, so no read leaves [data, data + data_len) and no write leaves the request's slot, and the other
+ * requests of the call are unaffected.  A DT_STRING feature without an entry: B200TFS_E_DTYPE; an entry on another dtype, a
+ * negative data_len, offsets not 8-byte aligned or unknown flags: B200TFS_E_ARG - checked before the context is looked at.      */
+typedef struct b200tfs_bytes {
+  const int64_t* offsets;   /* int64[strings + 1], 8-byte aligned; device memory for the _async entry point                      */
+  int64_t data_len;         /* bytes of the buffer the offsets index (cuDF's int32 offsets must be widened to int64 first)      */
+  uint32_t flags;           /* B200TFS_F_DEVICE_DATA: the _host entry point finds the offsets in HBM already (the data has its own
+                               flag on the feature)                                                                              */
+  int32_t pad_;
+} b200tfs_bytes;
+/* b200tfs_example_target_arena_size, b200tfs_encode_example_targets_async and b200tfs_encode_example_targets_host with bytes
+ * columns (bytes == NULL: those calls themselves).  The slot of a request with a bytes column is sized from its data_len and
+ * 11 bytes per string instead of a per-example worst case; the kernels count and place every example, and a replayed CUDA graph
+ * follows whatever the data, offsets and lengths hold then.  Host data and offsets are copied to the device with the columns.   */
+int b200tfs_example_columns_arena_size(int32_t n, const b200tfs_example_request* reqs, const b200tfs_bytes* bytes,
+                                       const b200tfs_example_target* targets, uint64_t* bytes_out);
+int b200tfs_encode_example_columns_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                         const b200tfs_bytes* bytes, const b200tfs_example_target* targets, void* arena_dev,
+                                         uint64_t arena_cap);
+int b200tfs_encode_example_columns_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                        const b200tfs_bytes* bytes, const b200tfs_example_target* targets, void* wire_host,
+                                        uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
 
 /* ---- Classify / Regress responses: a batch of responses into one value or score array ----------------------
  * What ClassificationResponse.FromString / RegressionResponse.FromString followed by a loop over the result give, concatenated

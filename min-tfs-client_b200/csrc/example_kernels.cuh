@@ -13,8 +13,10 @@
 //   ex_frame_kernel  one warp per request: the examples' total, the request prefix in front of the anchor (an example_list or
 //                    a Predict string_val, plan.h ExReq), rec_off / rec_len / status to pinned memory
 //
-// count, emit and the example writer take kRagged: a call with a ragged column launches the `true` instantiations, in which a
-// ragged column's row ends after ex_elems elements; every other call runs the `false` ones, which read row_elems as before.
+// count, emit and the example writer take an ExMode: a call with a bytes column launches the kExColumns instantiations, a call
+// with a ragged numeric column (and none of bytes) the kExRagged ones, in which a ragged column's row ends after ex_elems
+// elements; every other call runs the kExDense ones, which read row_elems as before.  kExColumns takes ragged rows too, and
+// bytes rows: a row's strings are cut from one byte buffer by int64 offsets (ex_str_ends), one string per lane.
 //
 // What the reference does here: requests.py examples_from_input_dict (a Python loop per example and per feature) and the
 // protobuf runtime serialising the ClassificationRequest / RegressionRequest it filled, or every example and then the
@@ -42,15 +44,20 @@ __device__ __forceinline__ uint64_t ex_int(const ExFeat& f, const uint8_t* p) {
 }
 // elements of example i's row: a ragged column's length, clamped to [0, max_len] (the count kernel flags one that was not), in
 // steps of `unit`; row_elems for a dense column
-template <bool kRagged>
+template <int kMode>
 __device__ __forceinline__ uint64_t ex_elems(const ExFeat& f, uint64_t i) {
-  if (!kRagged || !f.lengths) return f.row_elems;
+  if (kMode == kExDense || !f.lengths) return f.row_elems;
   const int64_t l = f.lengths[i];
   return (l < 0 ? 0ull : min((uint64_t)l, f.max_len)) * f.unit;
 }
-template <bool kRagged>
+template <int kMode>
 __device__ __forceinline__ uint64_t ex_payload(const ExTables& T, const ExReq& q, const ExFeat& f, uint64_t i) {
-  return f.op < EXO_INT ? 4 * ex_elems<kRagged>(f, i) : T.L[q.L0 + i * q.n_int + f.lcol];
+  return f.op < EXO_INT ? 4 * ex_elems<kMode>(f, i) : T.L[q.L0 + i * q.n_int + f.lcol];
+}
+// the map entry of a feature whose list payload is P bytes
+template <int kMode>
+__device__ __forceinline__ uint64_t ex_feat_entry_len(const ExFeat& f, uint64_t P, uint64_t* hl) {
+  return kMode == kExColumns && f.op == EXO_BYTES ? ex_bytes_entry_len(P, f.key_len, hl) : ex_entry_len(P, f.key_len, hl);
 }
 __device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
 #pragma unroll
@@ -58,9 +65,106 @@ __device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
   return v;
 }
 
+// ---- bytes rows ----
+// Example i's row of a bytes column is strings b .. b + ne of the column (b = i * row_stride), and the kernels read offsets
+// o[b .. b + ne] and o[b + row_elems], the next row's start.  A valid row has 0 <= o[b] <= ... <= o[b + ne] <= o[b + row_elems]
+// <= data_len, so the rows of a valid request are disjoint and in order.  Count and emit both see the offsets through
+// ex_str_ends: the row is clamped to [lo, hi] = [o[b], o[b + row_elems]] clamped into [0, data_len] (hi >= lo, and at most 4 GiB
+// past lo: no request under 2 GiB has a longer row), and every offset into [lo, hi] with a running maximum.  So both kernels
+// agree on every length, whatever the offsets hold, and no read leaves [data, data + data_len).
+__device__ __forceinline__ uint64_t ex_clamp_off(int64_t v, uint64_t lo, uint64_t hi) {
+  return v < 0 ? lo : min(max((uint64_t)v, lo), hi);
+}
+__device__ __forceinline__ void ex_row_bounds(const ExFeat& f, uint64_t b, uint64_t* lo, uint64_t* hi) {
+  *lo = ex_clamp_off(f.offsets[b], 0, f.data_len);
+  *hi = min(ex_clamp_off(f.offsets[b + f.row_elems], *lo, f.data_len), *lo + ((uint64_t)1 << 32));
+}
+// Warp-collective, over strings j0 .. j0 + 31 of a row (lane: string j0 + lane, < ne): the end of the lane's string, and through
+// *start its start; *carry (the end of string j0 - 1, lo for j0 = 0) moves on to the end of string j0 + 31.
+__device__ __forceinline__ uint64_t ex_str_ends(const ExFeat& f, uint64_t b, uint64_t ne, uint64_t j0, uint64_t lo, uint64_t hi,
+                                                uint64_t* carry, uint64_t* start) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t j = j0 + lane;
+  uint64_t e = j < ne ? ex_clamp_off(f.offsets[b + j + 1], lo, hi) : hi;
+  e = max(e, *carry);
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint64_t x = __shfl_up_sync(0xFFFFFFFFu, e, d);
+    if (lane >= (uint32_t)d) e = max(e, x);
+  }
+  const uint64_t s = __shfl_up_sync(0xFFFFFFFFu, e, 1);
+  *start = lane ? s : *carry;
+  *carry = __shfl_sync(0xFFFFFFFFu, e, 31);
+  return e;
+}
+// Strings at most this long are copied by their own lane; a longer one by the whole warp.
+constexpr uint64_t kExWarpCopy = 64;
+// Example i's bytes row at d, its list payload (L) already known: the {0A vi(len) bytes} field of every string.
+__device__ __forceinline__ void ex_write_bytes(const ExFeat& f, uint64_t i, uint64_t ne, uint8_t* d) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t b = i * f.row_stride;
+  uint64_t lo, hi, carry, base = 0;
+  ex_row_bounds(f, b, &lo, &hi);
+  carry = lo;
+  for (uint64_t j0 = 0; j0 < ne; j0 += 32) {
+    uint64_t s;
+    const uint64_t e = ex_str_ends(f, b, ne, j0, lo, hi, &carry, &s);
+    const uint64_t len = j0 + lane < ne ? e - s : 0;
+    const uint64_t sz = j0 + lane < ne ? 1 + varint_len(len) + len : 0;
+    uint64_t incl = sz;
+#pragma unroll
+    for (int dd = 1; dd < 32; dd <<= 1) {
+      const uint64_t x = __shfl_up_sync(0xFFFFFFFFu, incl, dd);
+      if (lane >= (uint32_t)dd) incl += x;
+    }
+    uint8_t* h = d + base + incl - sz;
+    const uint8_t* src = f.data + s;
+    if (sz) {
+      *h++ = 0x0A; h += put_varint(h, len);
+      if (len <= kExWarpCopy)
+        for (uint64_t k = 0; k < len; ++k) h[k] = src[k];
+    }
+    uint32_t big = __ballot_sync(0xFFFFFFFFu, len > kExWarpCopy);
+    while (big) {                             // the long strings of this chunk, each by the whole warp
+      const int l = __ffs(big) - 1;
+      big &= big - 1;
+      const uint64_t n = __shfl_sync(0xFFFFFFFFu, len, l);
+      uint8_t* dl = (uint8_t*)__shfl_sync(0xFFFFFFFFu, (unsigned long long)h, l);
+      const uint8_t* sl = (const uint8_t*)__shfl_sync(0xFFFFFFFFu, (unsigned long long)src, l);
+      for (uint64_t k = lane; k < n; k += 32) dl[k] = sl[k];
+    }
+    base += __shfl_sync(0xFFFFFFFFu, incl, 31);
+  }
+}
+// The list payload of example i's bytes row (what ex_write_bytes writes), by the whole warp; flags request r in T.bad when the
+// row breaks the offset rule.
+__device__ __forceinline__ uint64_t ex_count_bytes(const ExTables& T, uint32_t r, const ExFeat& f, uint64_t i, uint64_t ne) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t b = i * f.row_stride;
+  uint64_t lo, hi, carry, sum = 0;
+  ex_row_bounds(f, b, &lo, &hi);
+  carry = lo;
+  bool bad = false;
+  for (uint64_t j0 = 0; j0 < ne; j0 += 32) {
+    uint64_t s;
+    const uint64_t e = ex_str_ends(f, b, ne, j0, lo, hi, &carry, &s);
+    const uint64_t j = j0 + lane;
+    if (j < ne) {
+      sum += 1 + varint_len(e - s) + (e - s);
+      bad |= f.offsets[b + j + 1] < f.offsets[b + j];
+    }
+  }
+  if (lane == 0) {
+    const int64_t o0 = f.offsets[b], on = f.offsets[b + ne], nx = f.offsets[b + f.row_elems];
+    bad |= o0 < 0 || on > nx || nx > (int64_t)f.data_len;
+  }
+  if (__any_sync(0xFFFFFFFFu, bad) && lane == 0) T.bad[r] = 1;
+  return warp_sum64(sum);
+}
+
 // Example i of request q, written by the calling warp at w (shared or global memory), behind the tag kTag: 0A
 // (ExampleList.examples) or 42 (TensorProto.string_val).
-template <bool kRagged, uint8_t kTag>
+template <int kMode, uint8_t kTag>
 __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, uint8_t* w) {
   const uint32_t lane = threadIdx.x & 31;
   uint64_t F = 0, hl;
@@ -68,7 +172,7 @@ __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, 
     uint64_t e = 0;
     if (c + lane < q.n_feat) {
       const ExFeat& f = T.feats[q.first_feat + c + lane];
-      e = ex_entry_len(ex_payload<kRagged>(T, q, f, i), f.key_len, &hl);
+      e = ex_feat_entry_len<kMode>(f, ex_payload<kMode>(T, q, f, i), &hl);
     }
     F += warp_sum64(e);
   }
@@ -86,8 +190,8 @@ __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, 
     hl = 0;
     if (k < q.n_feat) {
       const ExFeat f = T.feats[q.first_feat + k];
-      P = ex_payload<kRagged>(T, q, f, i);
-      e = ex_entry_len(P, f.key_len, &hl);
+      P = ex_payload<kMode>(T, q, f, i);
+      e = ex_feat_entry_len<kMode>(f, P, &hl);
     }
     uint64_t inc = e;
 #pragma unroll
@@ -96,17 +200,18 @@ __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, 
       if (lane >= (uint32_t)d) inc += x;
     }
     const uint64_t at = pos + inc - e;
-    if (k < q.n_feat) {       // 0A vi(entry) 0A vi(klen) key 12 vi(Feature) {12|1A} vi(list) [0A vi(P)]
+    if (k < q.n_feat) {       // 0A vi(entry) 0A vi(klen) key 12 vi(Feature) {12|1A} vi(list) [0A vi(P)]   (bytes: 0A vi(P))
       const ExFeat& f = T.feats[q.first_feat + k];
-      const uint64_t list = P ? 1 + varint_len(P) + P : 0, feature = 1 + varint_len(list) + list;
+      const bool str = kMode == kExColumns && f.op == EXO_BYTES;
+      const uint64_t list = str ? P : P ? 1 + varint_len(P) + P : 0, feature = 1 + varint_len(list) + list;
       uint8_t* h = w + at;
       const uint64_t entry = 1 + varint_len(f.key_len) + f.key_len + 1 + varint_len(feature) + feature;
       *h++ = 0x0A; h += put_varint(h, entry);
       *h++ = 0x0A; h += put_varint(h, f.key_len);
       for (uint32_t b = 0; b < f.key_len; ++b) *h++ = T.blob[f.key_off + b];
       *h++ = 0x12; h += put_varint(h, feature);
-      *h++ = f.op < EXO_INT ? 0x12 : 0x1A; h += put_varint(h, list);
-      if (P) { *h++ = 0x0A; put_varint(h, P); }
+      *h++ = str ? 0x0A : f.op < EXO_INT ? 0x12 : 0x1A; h += put_varint(h, list);
+      if (P && !str) { *h++ = 0x0A; put_varint(h, P); }
     }
     const uint32_t nk = min(32u, q.n_feat - c);
     for (uint32_t s = 0; s < nk; ++s) {             // the rows, one after the other, by the whole warp
@@ -115,9 +220,11 @@ __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, 
       if (!Ps) continue;
       const ExFeat f = T.feats[q.first_feat + c + s];
       const uint8_t* row = f.data + i * f.row_stride;
-      const uint64_t ne = ex_elems<kRagged>(f, i);
+      const uint64_t ne = ex_elems<kMode>(f, i);
       uint8_t* d = w + ps;
-      if (f.op < EXO_INT) {
+      if (kMode == kExColumns && f.op == EXO_BYTES) {
+        ex_write_bytes(f, i, ne, d);
+      } else if (f.op < EXO_INT) {
         for (uint64_t j = lane; j < ne; j += 32) {
           const uint32_t b = ex_float_bits(f, row, j);
           d[4 * j] = (uint8_t)b; d[4 * j + 1] = (uint8_t)(b >> 8); d[4 * j + 2] = (uint8_t)(b >> 16); d[4 * j + 3] = (uint8_t)(b >> 24);
@@ -144,7 +251,7 @@ __device__ void ex_write_example(const ExTables& T, const ExReq& q, uint64_t i, 
   }
 }
 
-template <bool kRagged>
+template <int kMode>
 __global__ void __launch_bounds__(kExTile) ex_count_kernel(const __grid_constant__ ExTables T) {
   __shared__ unsigned long long warp_sum[kExTile / 32];
   const ExSpan sp = T.tiles[blockIdx.x];
@@ -155,20 +262,23 @@ __global__ void __launch_bounds__(kExTile) ex_count_kernel(const __grid_constant
     uint64_t F = 0, hl;
     for (uint32_t k = 0; k < q.n_feat; ++k) {
       const ExFeat f = T.feats[q.first_feat + k];
-      const uint64_t ne = ex_elems<kRagged>(f, i);
-      if (kRagged && f.lengths && lane == 0) {      // compared, never multiplied: 2^62 must not wrap into range
+      const uint64_t ne = ex_elems<kMode>(f, i);
+      if (kMode != kExDense && f.lengths && lane == 0) {      // compared, never multiplied: 2^62 must not wrap into range
         const int64_t l = f.lengths[i];
         if (l < 0 || (uint64_t)l > f.max_len) T.bad[sp.req] = 1;
       }
       uint64_t P = 4 * ne;
-      if (f.op >= EXO_INT) {
+      if (kMode == kExColumns && f.op == EXO_BYTES) {
+        P = ex_count_bytes(T, sp.req, f, i, ne);
+        if (lane == 0) T.L[q.L0 + i * q.n_int + f.lcol] = P;
+      } else if (f.op >= EXO_INT) {
         const uint8_t* row = f.data + i * f.row_stride;
         uint64_t s = 0;
         for (uint64_t j = lane; j < ne; j += 32) s += vlen64(ex_int(f, row + j * f.esz));
         P = warp_sum64(s);
         if (lane == 0) T.L[q.L0 + i * q.n_int + f.lcol] = P;
       }
-      F += ex_entry_len(P, f.key_len, &hl);
+      F += ex_feat_entry_len<kMode>(f, P, &hl);
     }
     const uint64_t S = ex_example_len(F);
     if (lane == 0) { T.S[q.ex0 + i] = S; mine += S; }
@@ -195,18 +305,18 @@ __global__ void __launch_bounds__(kExTile) ex_scan_kernel(const __grid_constant_
 
 // Does the scan place request q's examples?  Exactly when fixed_size == 0; without a ragged column that is when the request has an
 // integer column, and the dense instantiation keeps that test (on sm_90a the other one costs its emit kernel 10 registers).
-template <bool kRagged>
+template <int kMode>
 __device__ __forceinline__ bool ex_counted(const ExReq& q) {
-  return kRagged ? q.fixed_size == 0 : q.n_int != 0;
+  return kMode != kExDense ? q.fixed_size == 0 : q.n_int != 0;
 }
 // where example i of request q starts / ends, from the anchor
-template <bool kRagged>
+template <int kMode>
 __device__ __forceinline__ uint64_t ex_start(const ExTables& T, const ExReq& q, uint64_t i) {
-  return ex_counted<kRagged>(q) ? T.off[q.ex0 + i] : i * q.fixed_size;
+  return ex_counted<kMode>(q) ? T.off[q.ex0 + i] : i * q.fixed_size;
 }
-template <bool kRagged>
+template <int kMode>
 __device__ __forceinline__ uint64_t ex_end(const ExTables& T, const ExReq& q, uint64_t i) {
-  return ex_counted<kRagged>(q) ? T.off[q.ex0 + i] + T.S[q.ex0 + i] : (i + 1) * q.fixed_size;
+  return ex_counted<kMode>(q) ? T.off[q.ex0 + i] + T.S[q.ex0 + i] : (i + 1) * q.fixed_size;
 }
 
 // Store arena bytes [lo, hi) from the image img of the wire that starts at arena offset ws (16-byte aligned): the whole aligned
@@ -220,7 +330,7 @@ __device__ __forceinline__ void ex_flush(uint8_t* arena, const uint8_t* img, uin
   for (uint64_t x = b + threadIdx.x; x < hi; x += blockDim.x) arena[x] = img[x - ws];
 }
 
-template <bool kRagged, uint8_t kTag>
+template <int kMode, uint8_t kTag>
 __device__ __forceinline__ void ex_emit(const ExTables& T) {
   __shared__ __align__(16) uint8_t img[kExStage + 16];
   __shared__ uint64_t next;
@@ -229,7 +339,10 @@ __device__ __forceinline__ void ex_emit(const ExTables& T) {
   const ExReq q = T.reqs[sp.req];
   const uint32_t warp = threadIdx.x >> 5;
   const uint64_t A = q.anchor;
-  uint64_t lo = A + ex_start<kRagged>(T, q, sp.e0);   // first byte not stored yet
+  // a bytes request whose offsets broke the rule can count more bytes than its slot holds (it gets B200TFS_E_SHAPE): a span
+  // that would end past the slot writes nothing
+  if (kMode == kExColumns && A + ex_end<kMode>(T, q, sp.e1 - 1) > q.slot_end) return;
+  uint64_t lo = A + ex_start<kMode>(T, q, sp.e0);   // first byte not stored yet
   uint64_t ws = lo & ~15ull;                 // arena offset of img[0]
   uint64_t i = sp.e0;
   while (i < sp.e1) {
@@ -237,16 +350,16 @@ __device__ __forceinline__ void ex_emit(const ExTables& T) {
       uint64_t g = i, h = sp.e1;
       while (g < h) {
         const uint64_t m = (g + h + 1) / 2;
-        if (A + ex_end<kRagged>(T, q, m - 1) - ws <= kExStage) g = m; else h = m - 1;
+        if (A + ex_end<kMode>(T, q, m - 1) - ws <= kExStage) g = m; else h = m - 1;
       }
       next = g;
     }
     __syncthreads();
     const uint64_t j = next;
     if (j > i) {
-      for (uint64_t e = i + warp; e < j; e += kWarps) ex_write_example<kRagged, kTag>(T, q, e, img + (A + ex_start<kRagged>(T, q, e) - ws));
+      for (uint64_t e = i + warp; e < j; e += kWarps) ex_write_example<kMode, kTag>(T, q, e, img + (A + ex_start<kMode>(T, q, e) - ws));
       __syncthreads();
-      const uint64_t be = A + ex_end<kRagged>(T, q, j - 1), cut = be & ~15ull;
+      const uint64_t be = A + ex_end<kMode>(T, q, j - 1), cut = be & ~15ull;
       if (cut > ws) {                        // store every whole vector; the partial one moves to the front of the image
         ex_flush(T.arena, img, ws, lo, cut);
         const uint8_t t = threadIdx.x < be - cut ? img[cut - ws + threadIdx.x] : 0;
@@ -256,25 +369,25 @@ __device__ __forceinline__ void ex_emit(const ExTables& T) {
       }
       i = j;
     } else {                                 // example i alone is larger than the image: one warp writes it in place
-      ex_flush(T.arena, img, ws, lo, A + ex_start<kRagged>(T, q, i));
-      if (warp == 0) ex_write_example<kRagged, kTag>(T, q, i, T.arena + A + ex_start<kRagged>(T, q, i));
-      lo = A + ex_end<kRagged>(T, q, i);
+      ex_flush(T.arena, img, ws, lo, A + ex_start<kMode>(T, q, i));
+      if (warp == 0) ex_write_example<kMode, kTag>(T, q, i, T.arena + A + ex_start<kMode>(T, q, i));
+      lo = A + ex_end<kMode>(T, q, i);
       ws = lo & ~15ull;
       ++i;
     }
     __syncthreads();
   }
-  ex_flush(T.arena, img, ws, lo, A + ex_end<kRagged>(T, q, sp.e1 - 1));
+  ex_flush(T.arena, img, ws, lo, A + ex_end<kMode>(T, q, sp.e1 - 1));
 }
 
 // The tag is a template argument, so the example_list kernels keep the registers they had before Predict requests existed.
-template <bool kRagged>
+template <int kMode>
 __global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_constant__ ExTables T) {
-  ex_emit<kRagged, 0x0A>(T);
+  ex_emit<kMode, 0x0A>(T);
 }
-template <bool kRagged>
+template <int kMode>
 __global__ void __launch_bounds__(kExEmitThreads) ex_emit_predict_kernel(const __grid_constant__ ExTables T) {
-  ex_emit<kRagged, 0x42>(T);
+  ex_emit<kMode, 0x42>(T);
 }
 
 constexpr uint32_t kExFrameWarps = 4;
@@ -317,26 +430,28 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __gr
   w[at_inner] = (uint8_t)q.inner_tag; put_varint(w + at_inner + 1, inner);
 }
 
-cudaError_t launch_example_requests(const ExTables& T, cudaStream_t stream, uint32_t* launched) {
+cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t stream, uint32_t* launched) {
   *launched = 0;
-  const bool ragged = T.bad != nullptr;
   if (T.n_tiles) {
-    if (ragged) ex_count_kernel<true><<<T.n_tiles, kExTile, 0, stream>>>(T);
-    else ex_count_kernel<false><<<T.n_tiles, kExTile, 0, stream>>>(T);
+    if (mode == kExColumns) ex_count_kernel<kExColumns><<<T.n_tiles, kExTile, 0, stream>>>(T);
+    else if (mode == kExRagged) ex_count_kernel<kExRagged><<<T.n_tiles, kExTile, 0, stream>>>(T);
+    else ex_count_kernel<kExDense><<<T.n_tiles, kExTile, 0, stream>>>(T);
     ex_scan_kernel<<<T.n_tiles, kExTile, 0, stream>>>(T);
     *launched += 2;
   }
   const uint32_t n_list = T.n_spans - T.n_predict_spans;
   if (n_list) {
-    if (ragged) ex_emit_kernel<true><<<n_list, kExEmitThreads, 0, stream>>>(T);
-    else ex_emit_kernel<false><<<n_list, kExEmitThreads, 0, stream>>>(T);
+    if (mode == kExColumns) ex_emit_kernel<kExColumns><<<n_list, kExEmitThreads, 0, stream>>>(T);
+    else if (mode == kExRagged) ex_emit_kernel<kExRagged><<<n_list, kExEmitThreads, 0, stream>>>(T);
+    else ex_emit_kernel<kExDense><<<n_list, kExEmitThreads, 0, stream>>>(T);
     *launched += 1;
   }
   if (T.n_predict_spans) {    // the spans of the Predict requests come last
     ExTables P = T;
     P.spans += n_list;
-    if (ragged) ex_emit_predict_kernel<true><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
-    else ex_emit_predict_kernel<false><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
+    if (mode == kExColumns) ex_emit_predict_kernel<kExColumns><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
+    else if (mode == kExRagged) ex_emit_predict_kernel<kExRagged><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
+    else ex_emit_predict_kernel<kExDense><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
     *launched += 1;
   }
   if (T.n_req) { ex_frame_kernel<<<(T.n_req + kExFrameWarps - 1) / kExFrameWarps, 32 * kExFrameWarps, 0, stream>>>(T); *launched += 1; }

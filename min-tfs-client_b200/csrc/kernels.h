@@ -50,7 +50,7 @@ cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStr
 // b200tfs_decode_padded: padded_plan_kernel, then padded_emit_kernel with emit_grid CTAs striding over the chunks
 cudaError_t launch_padded(const PaddedPlan& pp, uint32_t emit_grid, cudaStream_t stream);
 // tf.Example requests (example_kernels.cuh): count + scan (when T.n_tiles), emit, frame; *launched receives how many kernels
-cudaError_t launch_example_requests(const ExTables& T, cudaStream_t stream, uint32_t* launched);
+cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t stream, uint32_t* launched);
 // Classify / Regress responses (example_resp_kernels.cuh): index, scan, emit, [label compare,] publish; emit_ctas CTAs stride over
 // the rows; *launched receives how many kernels
 cudaError_t launch_example_responses(const XrTables& T, uint32_t emit_ctas, cudaStream_t stream, uint32_t* launched);

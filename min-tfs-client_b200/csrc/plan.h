@@ -347,8 +347,10 @@ B2_PLAN_HD uint64_t var_decode_tiles(const void* src, uint64_t n) {
 // One request's examples start at a host-fixed anchor inside its slot; the request prefix is written in front of them once
 // their total is known.  Requests whose size depends on their values (an integer or a ragged column) get their example sizes
 // from the count kernel and their offsets from the scan kernel (tiles of kExTile examples); the others have one closed-form
-// example size.
-enum ExOp : uint32_t { EXO_F32 = 0, EXO_F64 = 1, EXO_F16 = 2, EXO_INT = 3, EXO_BOOL = 4 };
+// example size.  A bytes column (EXO_BYTES, only in calls that run the kExColumns kernels) is counted like an integer one.
+enum ExOp : uint32_t { EXO_F32 = 0, EXO_F64 = 1, EXO_F16 = 2, EXO_INT = 3, EXO_BOOL = 4, EXO_BYTES = 5 };
+// which instantiation of the count and emit kernels a call runs: no variable-length column, a ragged numeric column, a bytes column
+enum ExMode : int { kExDense = 0, kExRagged = 1, kExColumns = 2 };
 constexpr uint32_t kExTile = kConcatPlanThreads;   // examples per count / scan CTA (one thread each in the scan)
 constexpr uint32_t kExEmitThreads = 256;
 constexpr uint32_t kExStage = 16384;               // shared-memory image of the wire one emit batch writes
@@ -361,6 +363,8 @@ struct ExFeat {             // one column of one request, in wire order
   uint32_t lcol;            // integer columns: column of the request's length table
   const int64_t* lengths;   // a ragged column: example i takes min(max(lengths[i], 0), max_len) * unit elements; NULL: dense
   uint64_t max_len, unit;   // row_elems == max_len * unit
+  const int64_t* offsets;   // EXO_BYTES: string j is data[offsets[j], offsets[j+1]); example i's row starts at string i * row_stride
+  uint64_t data_len;        // (row_stride = row_elems, or 0 for a broadcast column).  Last: the dense and ragged kernels never read them
 };
 // The prefix the frame kernel writes in front of the examples, for both targets:
 //   [00 be32(msg)] spec 12 vi(outer) mid inner_tag vi(inner) head | examples
@@ -385,12 +389,12 @@ struct ExTables {
   const ExReq* reqs; const ExFeat* feats; const uint8_t* blob;
   const ExSpan* tiles;                  // count / scan CTAs
   const ExSpan* spans;                  // emit CTAs: those of the example_list requests, then the n_predict_spans of the Predict ones
-  uint64_t* L;                          // packed length of every (example, integer column)
+  uint64_t* L;                          // packed length of every (example, integer column), or list length (bytes column)
   uint64_t* S;                          // bytes of every example of a request whose size depends on its values
   uint64_t* off;                        // its offset from the anchor
   unsigned long long* tile_sum;         // bytes of every tile's examples
-  int32_t* bad;                         // a call with a ragged column: per request, nonzero when a length was out of range
-                                        // (zeroed by the host in every call); NULL otherwise
+  int32_t* bad;                         // a call with a ragged or bytes column: per request, nonzero when a length or a string
+                                        // offset was out of range (zeroed by the host in every call); NULL otherwise
   uint8_t* arena;
   uint64_t* rec_off; uint64_t* rec_len; int32_t* status;   // pinned host memory: read by b200tfs_encode_results
   uint32_t n_req, n_tiles, n_spans, n_predict_spans;
@@ -399,6 +403,14 @@ struct ExTables {
 //   0A vi(entry) 0A vi(klen) key 12 vi(Feature) {12 float_list | 1A int64_list} vi(list) [0A vi(P) payload]
 B2_PLAN_HD uint64_t ex_entry_len(uint64_t P, uint64_t klen, uint64_t* hl) {
   const uint64_t list = P ? 1 + varint_len(P) + P : 0, feature = 1 + varint_len(list) + list;
+  const uint64_t entry = 1 + varint_len(klen) + klen + 1 + varint_len(feature) + feature;
+  *hl = 1 + varint_len(entry) + entry - P;
+  return 1 + varint_len(entry) + entry;
+}
+// The same for a bytes_list, whose repeated strings are not packed: its list is the P bytes of {0A vi(len) bytes} fields.
+//   0A vi(entry) 0A vi(klen) key 12 vi(Feature) 0A vi(P) {0A vi(len) bytes}*
+B2_PLAN_HD uint64_t ex_bytes_entry_len(uint64_t P, uint64_t klen, uint64_t* hl) {
+  const uint64_t feature = 1 + varint_len(P) + P;
   const uint64_t entry = 1 + varint_len(klen) + klen + 1 + varint_len(feature) + feature;
   *hl = 1 + varint_len(entry) + entry - P;
   return 1 + varint_len(entry) + entry;

@@ -121,6 +121,12 @@ class Ragged(C.Structure):
     _fields_ = [("lengths", C.c_void_p), ("max_len", C.c_int64), ("unit", C.c_int64), ("flags", C.c_uint32), ("pad_", C.c_int32)]
 
 
+class Bytes(C.Structure):
+    """b200tfs_bytes: the int64 offsets of one string (bytes_list) tf.Example column (NULL offsets: not a bytes column); string j
+    is data[offsets[j]:offsets[j+1]] of the feature's byte buffer of data_len bytes."""
+    _fields_ = [("offsets", C.c_void_p), ("data_len", C.c_int64), ("flags", C.c_uint32), ("pad_", C.c_int32)]
+
+
 EXAMPLES_LIST, EXAMPLES_PREDICT_STRING = 0, 1
 
 
@@ -241,6 +247,12 @@ SIGNATURES = {
     "b200tfs_encode_example_targets_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged),
                                                        C.POINTER(ExampleTarget), _vp, C.c_uint64]),
     "b200tfs_encode_example_targets_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged),
+                                                      C.POINTER(ExampleTarget), _vp, C.c_uint64, _u64p, _u64p]),
+    "b200tfs_example_columns_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Bytes), C.POINTER(ExampleTarget),
+                                                     _u64p]),
+    "b200tfs_encode_example_columns_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                       C.POINTER(ExampleTarget), _vp, C.c_uint64]),
+    "b200tfs_encode_example_columns_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
                                                       C.POINTER(ExampleTarget), _vp, C.c_uint64, _u64p, _u64p]),
     "b200tfs_example_response_bound": (C.c_int, [C.c_int32, C.c_int32, _u64p, _u64p, _u64p]),
     "b200tfs_decode_example_responses": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64, _vp, C.c_uint64]),

@@ -136,19 +136,104 @@ _EXAMPLE_DTYPES = {np.dtype(t): _validated_enum(np.empty(0, t)) for t in (
     np.float16, np.float32, np.float64, np.int8, np.int16, np.int32, np.int64, np.uint8, np.uint16, np.uint32, np.uint64, np.bool_)}
 
 
+class BytesColumn:
+    """A string tf.Example column (``bytes_list``) laid out as Arrow / cuDF hold one: a byte buffer ``data`` (``uint8[data_len]``)
+    and ``offsets`` (``int[m + 1]``), string j being ``data[offsets[j]:offsets[j + 1]]``.  The m strings fill ``shape`` (default
+    ``(m,)``) in C order: row i, ``shape[1:]`` strings, is example i's list; ``shape=()`` is one string repeated in every example,
+    as a 0-d array is.  ``offsets[0]`` need not be 0 (a sliced column).
+
+    Both may be numpy arrays (pageable or ``pinned_empty``; host offsets of any integer dtype) or device arrays
+    (``__cuda_array_interface__`` / DLPack), so a GPU dataframe's string column is encoded where it lies; device offsets must be
+    int64 (widen cuDF's int32 offsets first).  Each example's offsets must rise inside ``0..data_len``: host offsets are checked
+    by the encode before anything runs, device ones by the kernels, and either way a request that breaks this raises ValueError.
+    A ``RaggedColumn`` of a ``BytesColumn`` of shape ``[n, L, *inner]`` gives example i its first ``lengths[i]`` steps.
+    ``from_array`` builds one from a numpy str / bytes array.
+    """
+
+    __slots__ = ("data", "offsets", "shape", "data_len", "data_on_device", "offsets_on_device")
+
+    def __init__(self, data, offsets, shape=None):
+        self.data_on_device = D.is_device_object(data)
+        if self.data_on_device:
+            _, dshape, ddtype, _ = D.device_view(data)
+            if ddtype != np.uint8 or len(dshape) != 1:
+                raise ValueError(f"string data must be a uint8 vector, got {ddtype} of shape {tuple(dshape)}")
+            data_len = int(dshape[0])
+        else:
+            data = np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else np.asarray(data)
+            if data.dtype != np.uint8 or data.ndim != 1:
+                raise ValueError(f"string data must be a uint8 vector, got {data.dtype} of shape {data.shape}")
+            data = np.require(data, requirements="C")
+            data_len = data.size
+        self.offsets_on_device = D.is_device_object(offsets)
+        if self.offsets_on_device:
+            _, oshape, odtype, _ = D.device_view(offsets)
+            if odtype != np.int64:
+                raise ValueError(f"device string offsets must be int64, got {odtype} (cast cuDF's int32 offsets to int64 first)")
+            oshape = tuple(oshape)
+        else:
+            offsets = np.asarray(offsets)
+            if offsets.dtype.kind not in "iu":
+                raise ValueError(f"string offsets must be integers, got {offsets.dtype}")
+            if offsets.dtype == np.uint64 and offsets.size and offsets.max() > np.iinfo(np.int64).max:
+                raise ValueError("string offsets exceed int64")
+            offsets = np.require(offsets.astype(np.int64, copy=False), requirements="CA")
+            oshape = offsets.shape
+        if len(oshape) != 1 or oshape[0] < 1:
+            raise ValueError(f"string offsets are a vector of at least one entry, got shape {oshape}")
+        shape = (oshape[0] - 1,) if shape is None else tuple(int(x) for x in shape)
+        if int(np.prod(shape, dtype=np.int64)) != oshape[0] - 1:
+            raise ValueError(f"{oshape[0] - 1} strings do not fill shape {shape}")
+        self.data, self.offsets, self.shape, self.data_len = data, offsets, shape, data_len
+
+    @classmethod
+    def from_array(cls, a) -> "BytesColumn":
+        """The strings of a numpy str (``U``) or bytes (``S``) array, as ``examples_from_input_dict`` makes them: trailing NULs
+        dropped (inner ones kept), str encoded as UTF-8 (a lone surrogate raises ``UnicodeEncodeError``)."""
+        a = np.asarray(a)
+        if a.dtype.kind == "U":
+            enc = np.asarray(np.char.encode(a, "utf-8"))
+        elif a.dtype.kind == "S":
+            enc = a
+        else:
+            raise ValueError(f"BytesColumn.from_array takes str or bytes arrays, got {a.dtype}")
+        m, w = enc.size, enc.dtype.itemsize
+        cells = np.ascontiguousarray(enc).reshape(m).view(np.uint8).reshape(m, w)
+        nz = cells != 0
+        lens = np.where(nz.any(axis=1), w - np.argmax(nz[:, ::-1], axis=1), 0) if w else np.zeros(m, np.int64)
+        data = cells[np.arange(w) < lens[:, None]]
+        offsets = np.zeros(m + 1, np.int64)
+        np.cumsum(lens, out=offsets[1:])
+        return cls(data, offsets, a.shape)
+
+    @property
+    def ndim(self) -> int:
+        return len(self.shape)
+
+    def strings(self, i: int, count: Optional[int] = None) -> List[bytes]:
+        """The first ``count`` (default: all) strings of example i (host arrays)."""
+        row = int(np.prod(self.shape[1:], dtype=np.int64)) if self.shape else 1
+        base = i * row if self.shape else 0
+        o = np.asarray(self.offsets)[base: base + (row if count is None else count) + 1].tolist()
+        d = np.asarray(self.data)
+        return [d[o[j]: o[j + 1]].tobytes() for j in range(len(o) - 1)]
+
+
 class RaggedColumn:
     """A variable-length tf.Example column - what a model parses as ``VarLenFeature`` / ``RaggedFeature``: a click history, the
     token ids of a query, multi-hot ids.  Example i's feature holds ``values[i, :lengths[i]].ravel()``, converted as a dense row is.
 
-    ``values`` has shape ``[n, L, *inner]`` (rank >= 2): a numpy array (pageable or ``pinned_empty``) or a device array
-    (``__cuda_array_interface__`` / DLPack).  ``lengths`` is ``int[n]``: a numpy array of any integer dtype, whose values must lie
-    in ``0..L`` (ValueError here), or a device array of int64, whose values the encode kernels check (ValueError from the encode).
+    ``values`` has shape ``[n, L, *inner]`` (rank >= 2): a numpy array (pageable or ``pinned_empty``), a device array
+    (``__cuda_array_interface__`` / DLPack) or a ``BytesColumn`` of that shape.  ``lengths`` is ``int[n]``: a numpy array of any
+    integer dtype, whose values must lie in ``0..L`` (ValueError here), or a device array of int64, whose values the encode kernels
+    check (ValueError from the encode).
     """
 
     __slots__ = ("values", "lengths", "shape", "lengths_on_device")
 
     def __init__(self, values, lengths):
-        shape = tuple(D.device_view(values)[1]) if D.is_device_object(values) else np.shape(values)
+        shape = values.shape if isinstance(values, BytesColumn) else \
+            tuple(D.device_view(values)[1]) if D.is_device_object(values) else np.shape(values)
         if len(shape) < 2:
             raise ValueError(f"ragged values have shape [n, L, *inner] (rank >= 2), got {shape}")
         self.lengths_on_device = D.is_device_object(lengths)
@@ -177,20 +262,33 @@ class RaggedColumn:
         """Example i's values, ``[lengths[i], *inner]`` (host arrays)."""
         return np.asarray(self.values)[i, :int(self.lengths[i])]
 
+    def strings(self, i: int) -> List[bytes]:
+        """Example i's strings, when the values are a ``BytesColumn`` (host arrays)."""
+        return self.values.strings(i, int(self.lengths[i]) * int(np.prod(self.shape[2:], dtype=np.int64)))
+
+
+class _ExampleColumn(tuple):
+    """(Feature, keep-alive, key, Ragged or None), and ``bytes_entry``: the Bytes entry of a string column (None otherwise)."""
+
+    bytes_entry = None
+
 
 def _example_columns(input_dict: Mapping):
-    """(n_examples, [(Feature, keep-alive, key, Ragged or None), ...]) for the device route, or None for a request
-    ``examples_from_input_dict`` assembles on the host (str / bytes columns, dtypes without a device conversion - which it rejects
-    or converts itself).  A ``RaggedColumn`` gives the Feature of its padded ``values`` (``row_elems = L * unit``) and a Ragged
-    entry for its lengths.  Raises the ValueError ``examples_from_input_dict`` raises for disagreeing example counts, and for
-    device arrays of a dtype the device route does not take."""
+    """(n_examples, [_ExampleColumn (Feature, keep-alive, key, Ragged or None), ...]) for the device route, or None for a request
+    ``examples_from_input_dict`` assembles on the host (numpy str / bytes columns, dtypes without a device conversion - which it
+    rejects or converts itself).  A ``RaggedColumn`` gives the Feature of its padded ``values`` (``row_elems = L * unit``) and a
+    Ragged entry for its lengths; a ``BytesColumn`` a DT_STRING Feature of its byte buffer and a Bytes entry for its offsets.
+    Raises the ValueError ``examples_from_input_dict`` raises for disagreeing example counts, and for device arrays of a dtype the
+    device route does not take."""
     cols = []
     for k, v in input_dict.items():
         key = k.encode("utf-8") if isinstance(k, str) else bytes(k)
         rag = v if isinstance(v, RaggedColumn) else None
         if rag is not None:
             v = rag.values
-        if D.is_device_object(v):
+        if isinstance(v, BytesColumn):
+            cols.append((key, None, v.shape, None, v, v.data_on_device, rag))
+        elif D.is_device_object(v):
             ptr, shape, dtype, hold = D.device_view(v)
             if dtype not in _EXAMPLE_DTYPES:
                 raise ValueError(f"input {k!r}: device arrays of dtype {dtype} have no tf.Example feature kind on the device")
@@ -211,12 +309,30 @@ def _example_columns(input_dict: Mapping):
         flags = 0 if len(shape) else N.F_BROADCAST
         if on_device:
             flags |= N.F_DEVICE_DATA
+        b = None
+        if isinstance(hold, BytesColumn):
+            col = hold
+            if col.data_on_device:
+                ptr, _, _, dhold = D.device_view(col.data)
+            else:
+                dhold = col.data
+                ptr = dhold.ctypes.data
+            if col.offsets_on_device:
+                optr, _, _, ohold = D.device_view(col.offsets)
+            else:
+                ohold = col.offsets
+                optr = ohold.ctypes.data
+            b = N.Bytes(offsets=optr, data_len=col.data_len, flags=N.F_DEVICE_DATA if col.offsets_on_device else 0)
+            f = N.Feature(data=ptr if col.data_len else None, src_dtype=DT_STRING, flags=flags, row_elems=row_elems, key=key,
+                          key_len=len(key))
+            hold = (dhold, ohold)
         else:
-            hold = np.require(hold.astype(dtype, copy=False), requirements="CA")
-            ptr = hold.ctypes.data
-        size = int(np.prod(shape, dtype=np.int64))
-        f = N.Feature(data=ptr if size else None, src_dtype=_EXAMPLE_DTYPES[dtype], flags=flags, row_elems=row_elems,
-                      key=key, key_len=len(key))
+            if not on_device:
+                hold = np.require(hold.astype(dtype, copy=False), requirements="CA")
+                ptr = hold.ctypes.data
+            size = int(np.prod(shape, dtype=np.int64))
+            f = N.Feature(data=ptr if size else None, src_dtype=_EXAMPLE_DTYPES[dtype], flags=flags, row_elems=row_elems,
+                          key=key, key_len=len(key))
         g = None
         if rag is not None:
             if rag.lengths_on_device:
@@ -227,7 +343,9 @@ def _example_columns(input_dict: Mapping):
             g = N.Ragged(lengths=lptr or None, max_len=shape[1], unit=int(np.prod(shape[2:], dtype=np.int64)),
                          flags=N.F_DEVICE_DATA if rag.lengths_on_device else 0)
             hold = (hold, lhold)
-        preps.append((f, hold, key, g))
+        col = _ExampleColumn((f, hold, key, g))
+        col.bytes_entry = b
+        preps.append(col)
     return n, preps
 
 
@@ -741,8 +859,10 @@ class Codec:
         ``order="deterministic"``, or list every example's features in insertion order with ``order="given"``.  Values may be
         numpy arrays (pageable or ``pinned_empty``) or device arrays (``__cuda_array_interface__`` / DLPack), and a value may be a
         ``RaggedColumn``: example i then holds only the first ``lengths[i]`` steps of its padded row (device lengths out of range
-        raise ValueError).  A request with a str / bytes column (or a dtype the device route does not take) is assembled on the
-        host by ``examples_from_input_dict``, in deterministic order; device arrays of such dtypes raise ValueError.
+        raise ValueError).  String features are encoded on the device from a ``BytesColumn`` (offsets that break its rule raise
+        ValueError), which ``BytesColumn.from_array`` makes of a numpy str / bytes array.  A request with a numpy str / bytes
+        column (or a dtype the device route does not take) is assembled on the host by ``examples_from_input_dict``, in
+        deterministic order; device arrays of such dtypes raise ValueError.
         """
         order_code = _ORDER[order] if isinstance(order, str) else int(order)
         target = None
@@ -751,7 +871,7 @@ class Codec:
             target = N.ExampleTarget(kind=N.EXAMPLES_PREDICT_STRING, key=pkey, key_len=len(pkey))
         items = list(requests)
         out: List[Optional[bytes]] = [None] * len(items)
-        keep, structs, dev_idx, ragged = [], [], [], []
+        keep, structs, dev_idx, ragged, strs = [], [], [], [], []
         for i, (model_name, model_version, input_dict) in enumerate(items):
             cols = _example_columns(input_dict)
             if cols is None:
@@ -766,17 +886,19 @@ class Codec:
                                             features=feats))
             keep.append((preps, feats, name))
             ragged += [p[3] or N.Ragged() for p in preps]
+            strs += [p.bytes_entry or N.Bytes() for p in preps]
             dev_idx.append(i)
         if dev_idx:
             m = len(dev_idx)
             reqs = (N.ExampleRequest * m)(*structs)
             cap = C.c_uint64()
             tg = (N.ExampleTarget * m)(*[target] * m) if target is not None else None
-            N.check(self._lib.b200tfs_example_target_arena_size(m, reqs, tg, C.byref(cap)))
+            bs = (N.Bytes * len(strs))(*strs) if any(b.offsets for b in strs) else None
+            N.check(self._lib.b200tfs_example_columns_arena_size(m, reqs, bs, tg, C.byref(cap)))
             wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
             off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
             rg = (N.Ragged * len(ragged))(*ragged) if any(g.lengths for g in ragged) else None
-            N.check(self._lib.b200tfs_encode_example_targets_host(self._ctx, m, reqs, rg, tg, wire.ctypes.data, cap.value, off, ln))
+            N.check(self._lib.b200tfs_encode_example_columns_host(self._ctx, m, reqs, rg, bs, tg, wire.ctypes.data, cap.value, off, ln))
             for j, i in enumerate(dev_idx):
                 out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
         return out  # type: ignore[return-value]

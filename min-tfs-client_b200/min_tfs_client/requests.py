@@ -18,7 +18,7 @@ from typing import Dict, Optional
 
 import numpy as np
 
-from .codec import RaggedColumn, get_codec
+from .codec import BytesColumn, RaggedColumn, get_codec
 from .tensors import WireTensor
 
 PREDICT_METHOD = "/tensorflow.serving.PredictionService/Predict"
@@ -33,13 +33,13 @@ def examples_from_input_dict(input_dict: Dict[str, np.ndarray]):
     Row i of every array is example i: ``feature[k]`` holds the row's values flattened - ``float_list`` for floating
     dtypes, ``int64_list`` for integers and bools, ``bytes_list`` for str / bytes (``coerce_to_bytes``).  0-d arrays are
     repeated in every example; all other arrays must agree on their first dimension.  A ``RaggedColumn`` gives example i
-    only ``values[i, :lengths[i]]``.
+    only ``values[i, :lengths[i]]``.  A ``BytesColumn`` (or a ``RaggedColumn`` of one) gives example i its strings, as they are.
     """
     from tensorflow_serving.apis.input_pb2 import Input
 
     from .tensors import coerce_to_bytes
 
-    arrays = {k: v if isinstance(v, RaggedColumn) else np.asarray(v) for k, v in input_dict.items()}
+    arrays = {k: v if isinstance(v, (RaggedColumn, BytesColumn)) else np.asarray(v) for k, v in input_dict.items()}
     rows = {a.shape[0] for a in arrays.values() if a.ndim}
     if len(rows) > 1:
         raise ValueError(f"inputs disagree on the number of examples: {sorted(rows)}")
@@ -49,8 +49,11 @@ def examples_from_input_dict(input_dict: Dict[str, np.ndarray]):
     for i in range(n):
         ex = inp.example_list.examples.add()
         for k, a in arrays.items():
-            row = a.row(i) if isinstance(a, RaggedColumn) else a if a.ndim == 0 else a[i]
             feat = ex.features.feature[k]
+            if isinstance(a, BytesColumn) or isinstance(a, RaggedColumn) and isinstance(a.values, BytesColumn):
+                feat.bytes_list.value.extend(a.strings(i))
+                continue
+            row = a.row(i) if isinstance(a, RaggedColumn) else a if a.ndim == 0 else a[i]
             if row.dtype.kind == "f":
                 feat.float_list.value.extend(np.asarray(row, dtype=np.float32).ravel().tolist())
             elif row.dtype.kind in "iub":
@@ -219,7 +222,8 @@ class TensorServingClient:
                                  timeout: int = 60, model_version: Optional[int] = None) -> PredictResponseView:
         """Predict on a model whose signature takes serialized tf.Examples (a DT_STRING vector it parses with
         ``tf.io.parse_example``, e.g. a TFX Trainer or Estimator export's ``serving_default``): one example per row of
-        ``input_dict`` as ``examples_from_input_dict`` builds it, sent as input ``input_key``."""
+        ``input_dict`` as ``examples_from_input_dict`` builds it, sent as input ``input_key``.  Values may be ``RaggedColumn`` and
+        ``BytesColumn`` columns, encoded on the GPU like the numeric ones."""
         call = self._channel.unary_unary(PREDICT_METHOD, request_serializer=gpu_predict_examples_serializer,
                                          response_deserializer=gpu_response_deserializer)
         return call((model_name, model_version, input_dict, input_key), timeout)

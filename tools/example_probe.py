@@ -8,7 +8,10 @@ Workloads (one request each unless stated):
   V2  65 536 examples x {emb f32 ragged [65536, 64], lengths uniform in 1..64}   float-only, but counted and scanned (beside W1)
   V3  4 096 examples x {tokens int32 ragged [4096, 512], lengths geometric with mean ~40, capped at 512}   worst-case emit spans
   V4  256 requests of 64 examples shaped like V1
-  W1P, W2P, V1P  W1, W2 and V1 framed for Predict: a PredictRequest whose input "examples" is the DT_STRING [n] vector of the
+  B1  65 536 examples x {country: 1 string of 2 B, tags: [n, 4] strings of 3-12 B, dense f32[16]}   bytes columns
+  B2  16 384 examples x {query: 1 UTF-8 string of 100-400 B, ids int64[8] in 0..50 000}
+  B3  256 requests of 64 examples shaped like B1
+  W1P, W2P, V1P, B1P  W1, W2, V1 and B1 framed for Predict: a PredictRequest whose input "examples" is the DT_STRING [n] vector of the
       serialized examples (b200tfs_encode_example_targets_*), each run beside its Classify form
 Legs: the _async entry point eager (device columns -> device arena), the same captured once as a CUDA graph and replayed,
 _host from pinned columns (copies both ways included), and examples_from_input_dict + SerializeToString(deterministic=True)
@@ -20,6 +23,8 @@ The V workloads (ragged columns, b200tfs_encode_example_requests_ragged_*) count
 columns, and the lengths; their host path builds the request one example at a time from the unchanged dense code, as a user
 without ragged columns would.  The P workloads' host path is the one a Predict user has today: examples_from_input_dict,
 SerializeToString(deterministic=True) of every example, string_val.extend and the PredictRequest's SerializeToString.
+The B workloads (BytesColumn columns, b200tfs_encode_example_columns_*) count the string bytes and offsets; their host path runs
+examples_from_input_dict over the equivalent numpy str / bytes arrays, which BytesColumn.from_array turns into the columns.
 --profile V1,V3 runs only the per-kernel split of the named workloads (profiler on).
 
   python tools/example_probe.py [--calls 20] [--runs 3] [--workloads W1,V1,...] [--profile V1,V3] [--json PATH]
@@ -38,7 +43,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(REPO, "min-tfs-client_b200"))
 
 from min_tfs_client import _native as N  # noqa: E402
-from min_tfs_client.codec import Codec, RaggedColumn, _example_columns  # noqa: E402
+from min_tfs_client.codec import BytesColumn, Codec, RaggedColumn, _example_columns  # noqa: E402
 from min_tfs_client.requests import TensorServingClient, examples_from_input_dict  # noqa: E402
 from tensorflow.core.framework import types_pb2  # noqa: E402
 from tensorflow_serving.apis.classification_pb2 import ClassificationRequest  # noqa: E402
@@ -54,6 +59,15 @@ def workloads(rng):
     def v1(n):
         return {"history": RaggedColumn(rng.integers(0, 50_000, (n, 64)), rng.integers(0, 65, n)),
                 "dense": rng.standard_normal((n, 64)).astype(np.float32)}
+    def tags(n):
+        cells = rng.integers(97, 123, (n, 4, 12), dtype=np.uint8)
+        cells[np.arange(12) >= rng.integers(3, 13, (n, 4, 1))] = 0
+        return cells.view("S12").reshape(n, 4)
+    def b1(n):
+        return {"country": np.array([b"us", b"de", b"fr", b"jp", b"br"])[rng.integers(0, 5, n)], "tags": tags(n),
+                "dense": rng.standard_normal((n, 16)).astype(np.float32)}
+    words = ["".join(rng.choice(list("abcdefghij klmnop\u00e9\u00fc"), int(rng.integers(100, 400)))) for _ in range(1000)]
+    queries = np.array([w.encode("utf-8")[:400].decode("utf-8", "ignore") for w in words])
     return {"W1": lambda: [{"dense": rng.standard_normal((65536, 64)).astype(np.float32)}], "W2": lambda: [w2(16384)],
             "W3": lambda: [w2(64) for _ in range(256)],
             "V1": lambda: [v1(16384)],
@@ -62,7 +76,14 @@ def workloads(rng):
                                                    np.minimum(rng.geometric(1 / 40, 4096), 512))}],
             "V4": lambda: [v1(64) for _ in range(256)],
             "W1P": lambda: [{"dense": rng.standard_normal((65536, 64)).astype(np.float32)}], "W2P": lambda: [w2(16384)],
-            "V1P": lambda: [v1(16384)]}
+            "V1P": lambda: [v1(16384)],
+            "B1": lambda: [b1(65536)], "B1P": lambda: [b1(65536)], "B3": lambda: [b1(64) for _ in range(256)],
+            "B2": lambda: [{"query": queries[rng.integers(0, 1000, 16384)], "ids": rng.integers(0, 50_000, (16384, 8))}]}
+
+
+def columns(d):
+    """the device route's columns of a workload: numpy str / bytes arrays as BytesColumn"""
+    return {k: BytesColumn.from_array(v) if isinstance(v, np.ndarray) and v.dtype.kind in "US" else v for k, v in d.items()}
 
 
 def host_ref(d, predict=False):
@@ -99,6 +120,9 @@ def arrays(d):
         if isinstance(v, RaggedColumn):
             yield v.values
             yield v.lengths
+        elif isinstance(v, BytesColumn):
+            yield v.data
+            yield v.offsets
         else:
             yield v
 
@@ -110,6 +134,8 @@ def used_bytes(d):
         if isinstance(v, RaggedColumn):
             unit = int(np.prod(v.shape[2:], dtype=np.int64))
             b += int(v.lengths.sum()) * unit * v.values.itemsize + v.lengths.nbytes
+        elif isinstance(v, BytesColumn):
+            b += v.data_len + v.offsets.nbytes
         else:
             b += np.asarray(v).nbytes
     return b
@@ -149,26 +175,33 @@ def timed_host(fn, calls):
 
 
 def build(dicts, device_ptrs=None):
-    """(requests, ragged entries or None when no column is ragged, keep-alive); device_ptrs[r]: the arrays(d) of request r in HBM"""
-    keep, structs, ragged = [], [], []
+    """(requests, ragged entries or None when no column is ragged, bytes entries or None when no column is one, keep-alive);
+    device_ptrs[r]: the arrays(d) of request r in HBM"""
+    keep, structs, ragged, strs = [], [], [], []
     for r, d in enumerate(dicts):
         n, preps = _example_columns(d)
         feats = (N.Feature * len(preps))(*[p[0] for p in preps])
         rg = [p[3] or N.Ragged() for p in preps]
+        bs = [p.bytes_entry or N.Bytes() for p in preps]
         if device_ptrs is not None:
             ptrs = iter(device_ptrs[r])
-            for f, g in zip(feats, rg):
+            for f, g, b in zip(feats, rg, bs):
                 f.data = next(ptrs)
                 f.flags |= N.F_DEVICE_DATA
+                if b.offsets:
+                    b.offsets = next(ptrs)
+                    b.flags = N.F_DEVICE_DATA
                 if g.lengths:
                     g.lengths = next(ptrs)
                     g.flags = N.F_DEVICE_DATA
         ragged += rg
+        strs += bs
         structs.append(N.ExampleRequest(model_name=b"model", model_name_len=5, has_version=1, order=N.ORDER_UPB, version=1,
                                         n_examples=n, n_features=len(preps), flags=0, features=feats))
         keep.append((preps, feats))
     rga = (N.Ragged * len(ragged))(*ragged) if any(g.lengths for g in ragged) else None
-    return (N.ExampleRequest * len(structs))(*structs), rga, keep
+    bsa = (N.Bytes * len(strs))(*strs) if any(b.offsets for b in strs) else None
+    return (N.ExampleRequest * len(structs))(*structs), rga, bsa, keep
 
 
 def profile_split(lib, g, eager, calls):
@@ -193,7 +226,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--runs", type=int, default=3)
-    ap.add_argument("--workloads", default="W1,W1P,W2,W2P,W3,V1,V1P,V2,V3,V4", help="comma-separated workloads to run")
+    ap.add_argument("--workloads", default="W1,W1P,W2,W2P,W3,V1,V1P,V2,V3,V4,B1,B1P,B2,B3", help="comma-separated workloads to run")
     ap.add_argument("--profile", default="", help="only the per-kernel split of these workloads (comma-separated)")
     ap.add_argument("--json", metavar="PATH", help="write every number of the run to PATH as JSON")
     args = ap.parse_args()
@@ -206,10 +239,11 @@ def main():
     out = {"card": card, "calls": args.calls, "runs": args.runs, "workloads": {}}
     profile_only = [w for w in args.profile.split(",") if w]
     for name in (profile_only or args.workloads.split(",")):
-        dicts = W[name]()
+        host_dicts = W[name]()
+        dicts = [columns(d) for d in host_dicts]
         predict = name.endswith("P")
         g = Ctx()       # a context per workload: the graph captured below pins its scratch buffers
-        refs = [host_ref(d, predict) for d in dicts]
+        refs = [host_ref(d, predict) for d in host_dicts]
         col_bytes = sum(used_bytes(d) for d in dicts)
         wire_bytes = sum(len(w) for w in refs)
         moved = col_bytes + wire_bytes
@@ -222,16 +256,18 @@ def main():
                 N.check(lib.b200tfs_memcpy_h2d(g.ctx, p, a.ctypes.data, a.nbytes))
                 row.append(p)
             ptrs.append(row)
-        reqs, rga, keep = build(dicts, ptrs)
+        reqs, rga, bsa, keep = build(dicts, ptrs)
         n = len(dicts)
         tg = (N.ExampleTarget * n)(*[N.ExampleTarget(kind=N.EXAMPLES_PREDICT_STRING, key=b"examples", key_len=8)] * n) if predict else None
         cap = C.c_uint64()
-        N.check(lib.b200tfs_example_target_arena_size(n, reqs, tg, C.byref(cap)))
+        N.check(lib.b200tfs_example_columns_arena_size(n, reqs, bsa, tg, C.byref(cap)))
         arena = g.malloc(cap.value)
         off, ln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
 
         def eager():
-            if predict:
+            if bsa is not None:
+                N.check(lib.b200tfs_encode_example_columns_async(g.ctx, n, reqs, rga, bsa, tg, arena, cap.value))
+            elif predict:
                 N.check(lib.b200tfs_encode_example_targets_async(g.ctx, n, reqs, rga, tg, arena, cap.value))
             elif rga is None:
                 N.check(lib.b200tfs_encode_example_requests_async(g.ctx, n, reqs, arena, cap.value))
@@ -276,12 +312,20 @@ def main():
             p = codec.pinned_empty(np.shape(a), np.asarray(a).dtype)
             p[...] = a
             return p
-        pinned = [{k: RaggedColumn(pin(v.values), pin(v.lengths)) if isinstance(v, RaggedColumn) else pin(v) for k, v in d.items()}
-                  for d in dicts]
-        hreqs, hrga, hkeep = build(pinned)
+        def pin_col(v):
+            if isinstance(v, RaggedColumn):
+                return RaggedColumn(pin(v.values), pin(v.lengths))
+            if isinstance(v, BytesColumn):
+                return BytesColumn(pin(v.data), pin(v.offsets), v.shape)
+            return pin(v)
+        pinned = [{k: pin_col(v) for k, v in d.items()} for d in dicts]
+        hreqs, hrga, hbsa, hkeep = build(pinned)
         wire = N.PinnedBuffer(cap.value)
         hoff, hln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
-        if predict:
+        if hbsa is not None:
+            host = lambda: N.check(lib.b200tfs_encode_example_columns_host(codec.ctx, n, hreqs, hrga, hbsa, tg, wire.ptr, cap.value,  # noqa: E731
+                                                                            hoff, hln))
+        elif predict:
             host = lambda: N.check(lib.b200tfs_encode_example_targets_host(codec.ctx, n, hreqs, hrga, tg, wire.ptr, cap.value,  # noqa: E731
                                                                             hoff, hln))
         elif hrga is None:
@@ -297,7 +341,7 @@ def main():
         runs = []
         for _ in range(args.runs):
             t0 = time.perf_counter()
-            for d in dicts:
+            for d in host_dicts:
                 host_ref(d, predict)
             runs.append((time.perf_counter() - t0) * 1e6)
         res["protobuf_host_us"] = runs
@@ -322,10 +366,10 @@ def main():
                 pe()
             out["predict_same_bytes_async_us"] = [g.timed(pe, args.calls) for _ in range(args.runs)]
             print("predict W1-bytes", out["predict_same_bytes_async_us"], flush=True)
-        if name == "W2":     # per-kernel split, profiler on, in a run of its own
+        if name in ("W2", "B1", "B2"):     # per-kernel split, profiler on, in a run of its own
             split = profile_split(lib, g, eager, args.calls)
-            out["W2_kernels"] = split
-            print("W2 kernels", json.dumps(split), flush=True)
+            out[f"{name}_kernels"] = split
+            print(name, "kernels", json.dumps(split), flush=True)
     if args.json:
         with open(args.json, "w") as f:
             json.dump(out, f, indent=1)
