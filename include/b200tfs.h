@@ -183,7 +183,7 @@ typedef struct b200tfs_output {
   uint64_t msg_len;
   uint64_t n_elems;     /* prod(dims)                                                           */
   uint64_t dst_bytes;   /* n_elems * element size of `dtype` in memory                          */
-  uint64_t n_strings;   /* string_val occurrences (strings are unpacked on the host)            */
+  uint64_t n_strings;   /* string_val occurrences (unpacked on the host, or by b200tfs_decode_concat_strings) */
   uint64_t dst_off;     /* b200tfs_decode_responses: where the values were written, from the
                            record's destination slot dst_dev + i*dst_stride                    */
   int32_t status;       /* B200TFS_OK, or the error tensor_proto_to_ndarray raises for it       */
@@ -416,7 +416,8 @@ typedef struct b200tfs_concat_key {
   int32_t rank;           /* out: rank of the concatenated tensor                                                     */
   int64_t dims[B200TFS_MAX_RANK]; /* out: dims[0] = rows of all records together, the rest those of every record      */
   uint64_t bytes;         /* out: bytes of the concatenated tensor in memory (2 per float32 element with a cast)      */
-  int32_t status;         /* out: B200TFS_OK (also for a DT_STRING key: bytes 0, decoded on the host) or the first
+  int32_t status;         /* out: B200TFS_OK (also for a DT_STRING key: bytes 0, decoded on the host - or, with
+                             b200tfs_concat_strings entries, bytes of its int64 offsets) or the first
                              problem in record order: the record's error (E_PARSE, ...,
                              E_NONCANONICAL for a record the device route cannot tabulate: more than
                              B200TFS_FUSED_MAX_OUTPUTS outputs, rank > B200TFS_MAX_RANK, more than B200TFS_MAX_RUNS runs),
@@ -450,7 +451,8 @@ int b200tfs_decode_concat_host_async(b200tfs_ctx* ctx, const void* wire_host, in
  * output's error; B200TFS_E_KEY (no such key); B200TFS_E_DTYPE / B200TFS_E_SHAPE (dtype / rank / trailing dims differ from the
  * first record that decoded the key; rank 0); B200TFS_E_SIZE (its rows end past dst_cap); B200TFS_E_NONCANONICAL, which is
  * either a packed-varint output in rows of unpacked elements (its place [dst_off, dst_off + dst_bytes) is reserved; finish it
- * with b200tfs_unpack_outputs there), a string output (nothing reserved: strings are decoded on the host), or a record the
+ * with b200tfs_unpack_outputs there), a string output of a call without b200tfs_concat_strings entries (nothing reserved: such
+ * strings are decoded on the host; see b200tfs_decode_concat_strings for the string pairs of a call with them), or a record the
  * device parse cannot tabulate (more than B200TFS_FUSED_MAX_OUTPUTS outputs, rank > B200TFS_MAX_RANK, more than
  * B200TFS_MAX_RUNS runs; nothing reserved).  Outputs the tolerant decode would accept although their table entry is an error -
  * tensor_content only, fewer fixed-width values than the shape holds (TF's padding) - keep that error (B200TFS_E_SHAPE) and
@@ -459,6 +461,45 @@ int b200tfs_decode_concat_host_async(b200tfs_ctx* ctx, const void* wire_host, in
  * b200tfs_parse_responses gives them; any pointer may be NULL.                                                           */
 int b200tfs_concat_results(b200tfs_ctx* ctx, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs,
                            int32_t* rec_status);
+
+/* DT_STRING outputs of the same decode, as offset-indexed byte columns (the Arrow / cuDF layout b200tfs_bytes reads): for a key
+ * whose outputs are DT_STRING, the string_val elements of every record, in record order, as raw bytes (no UTF-8 check; NULs and
+ * high bytes kept).  With m strings of D bytes in all, keys[k].dst receives int64 offsets[m + 1] (offsets[0] = 0, string j is
+ * data[offsets[j], offsets[j + 1])) and the entry's `data` the D bytes.  The offsets take the key's own dst / dst_cap so that
+ * b200tfs_output.dst_off keeps its meaning: the byte offset of the record's first offset entry (8 * its first string).  One entry
+ * per key, parallel to keys; entries of keys whose outputs are not DT_STRING are ignored.                                         */
+typedef struct b200tfs_concat_strings {
+  void* data;             /* in: device destination of the key's string bytes                                                  */
+  uint64_t data_cap;      /* in: its capacity in bytes - nothing is ever stored at or past data + data_cap                     */
+  uint64_t strings;       /* out (b200tfs_concat_strings_layout): m, the strings of every record together                     */
+  uint64_t data_bytes;    /* out: D, their bytes                                                                               */
+} b200tfs_concat_strings;
+/* b200tfs_concat_layout with entries (strings == NULL: that call itself).  A DT_STRING key that lays out gets `strings` and
+ * `data_bytes`, and keys[k].bytes = 8 * (strings + 1), the offsets' size.  A record whose string_val elements the device walk
+ * does not find in its last `value` occurrence (a map entry that carries its TensorProto in several, which the runtime merges)
+ * is B200TFS_E_NONCANONICAL: that batch is decoded on the host.                                                                  */
+int b200tfs_concat_strings_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
+                                  b200tfs_concat_key* keys, b200tfs_concat_strings* strings, int32_t cast);
+/* Host only, closed form from the record lengths alone, for a caller that captures a graph once: every string_val element takes at
+ * least two bytes of wire and its bytes lie in the wire, so one key of any records of these lengths has at most *max_strings
+ * strings (offsets of 8 * (*max_strings + 1) bytes) and *max_data_bytes bytes.  Either pointer may be NULL.                    */
+int b200tfs_concat_strings_bound(int32_t n, const uint64_t* rec_len, uint64_t* max_strings, uint64_t* max_data_bytes);
+/* b200tfs_decode_concat with entries (strings == NULL: that call itself).  Still asynchronous and CUDA-graph capturable with no
+ * host step between the launches: the plan places every (record, string key)'s offsets, then four kernels (index: a warp per
+ * pair walks its string_val elements; scan: one CTA places their bytes; copy; fix: the final offsets) follow the plan and come
+ * ahead of the varint tail - b200tfs_kernel_launches counts ten.  The scratch is sized from n, n_keys and rec_len alone, so a
+ * replay over new records of the same lengths re-plans string counts and byte offsets.  b200tfs_concat_results reports each
+ * (record, string key): B200TFS_OK with dst_off = 8 * its first string and dst_bytes = 8 * its strings; B200TFS_E_SIZE when its
+ * offsets (up to and including the entry behind its last string) would end past dst_cap or its bytes past data_cap; or
+ * B200TFS_E_NONCANONICAL when its string_val elements do not all lie in its last `value` occurrence (decode that batch on the
+ * host).  Stores: for the OK pairs, their offset entries and bytes, and offsets[m] behind the last OK pair of the key; the entries
+ * of a pair that ends B200TFS_E_SIZE for its bytes or B200TFS_E_NONCANONICAL may hold scratch values.  Nothing at or past dst_cap
+ * or data_cap.                                                                                                                     */
+int b200tfs_decode_concat_strings(b200tfs_ctx* ctx, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                                  int32_t n_keys, const b200tfs_concat_key* keys, const b200tfs_concat_strings* strings);
+int b200tfs_decode_concat_strings_host_async(b200tfs_ctx* ctx, const void* wire_host, int32_t n, const uint64_t* rec_off,
+                                             const uint64_t* rec_len, int32_t n_keys, const b200tfs_concat_key* keys,
+                                             const b200tfs_concat_strings* strings);
 
 /* ---- batch decode into one padded tensor per output (ragged trailing dims) --------------------------
  * What a caller of a sequence model wants back (per-token logits f32[1, T_r, V], token ids int64[1, T_r], ...): for each requested

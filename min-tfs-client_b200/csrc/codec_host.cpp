@@ -24,6 +24,7 @@
 #include "framing.h"
 #include "kernels.h"
 #include "plan.h"
+#include "string_walk.h"
 #include "tpl.h"
 #include "walker.h"
 #include "wire.h"
@@ -2209,10 +2210,11 @@ int b200tfs_response_keys(const void* rec_host, uint64_t rec_len, int32_t cap, u
 extern "C++" {
 // The host walk of b200tfs_concat_layout and b200tfs_padded_layout: per key, the first problem in record order, the dtype and
 // rank of the first record that has the key, the rows, and the trailing dims - every record's (another one is E_SHAPE) or, with
-// `ragged`, their elementwise maximum.
-template <class Key>
+// `ragged`, their elementwise maximum.  `on_out(k, record, its length, output)` sees every output that passes those checks and
+// may refuse it with a status.
+template <class Key, class OnOut>
 static int key_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys, Key* keys,
-                      int32_t cast, bool ragged) {
+                      int32_t cast, bool ragged, OnOut&& on_out) {
   if (n <= 0 || !wire_host || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
   int rc = concat_check_keys(n_keys, keys);
   if (rc) return rc;
@@ -2247,6 +2249,7 @@ static int key_layout(const void* wire_host, int32_t n, const uint64_t* rec_off,
           else if (have[k] && o->dtype != K.dtype) s = B200TFS_E_DTYPE;
           else if (have[k] && o->rank != K.rank) s = B200TFS_E_SHAPE;
           else for (int d = 1; have[k] && !ragged && d < o->rank; ++d) if (o->dims[d] != K.dims[d]) s = B200TFS_E_SHAPE;
+          if (s == B200TFS_OK) s = on_out(k, rec, rec_len[r], *o);
         }
       }
       if (s != B200TFS_OK) { K.status = s; K.bad_rec = r; done[k] = 1; continue; }
@@ -2276,12 +2279,56 @@ static int key_layout(const void* wire_host, int32_t n, const uint64_t* rec_off,
 
 int b200tfs_concat_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
                           b200tfs_concat_key* keys, int32_t cast) {
-  return key_layout(wire_host, n, rec_off, rec_len, n_keys, keys, cast, false);
+  return b200tfs_concat_strings_layout(wire_host, n, rec_off, rec_len, n_keys, keys, nullptr, cast);
+}
+
+namespace {
+struct StrTally {
+  uint64_t bytes = 0;
+  void operator()(uint64_t, uint32_t, uint32_t len) { bytes += len; }
+};
+}  // namespace
+
+int b200tfs_concat_strings_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
+                                  b200tfs_concat_key* keys, b200tfs_concat_strings* strings, int32_t cast) {
+  if (strings && n_keys > 0 && n_keys <= B200TFS_CONCAT_MAX_KEYS)
+    for (int k = 0; k < n_keys; ++k) strings[k].strings = strings[k].data_bytes = 0;
+  const int rc = key_layout(wire_host, n, rec_off, rec_len, n_keys, keys, cast, false,
+                            [&](int k, const uint8_t* rec, uint64_t len, const b200tfs_output& o) -> int32_t {
+                              if (!strings || dtype_info(o.dtype).kind != VK_STRING) return B200TFS_OK;
+                              // the walk of str_index_kernel: the strings of the entry's last `value` occurrence
+                              Cursor c;
+                              cur_open_host(c, rec, (uint32_t)len);
+                              c.p = (uint32_t)o.msg_off;
+                              c.end = (uint32_t)(o.msg_off + o.msg_len);
+                              StrTally t;
+                              const uint64_t found = walk_strings(c, t);
+                              if (c.err || found != o.n_strings) return B200TFS_E_NONCANONICAL;
+                              strings[k].strings += found;
+                              strings[k].data_bytes += t.bytes;
+                              return B200TFS_OK;
+                            });
+  if (rc || !strings) return rc;
+  for (int k = 0; k < n_keys; ++k) {
+    if (keys[k].status == B200TFS_OK && dtype_info(keys[k].dtype).kind == VK_STRING) keys[k].bytes = 8 * (strings[k].strings + 1);
+    else strings[k].strings = strings[k].data_bytes = 0;
+  }
+  return B200TFS_OK;
+}
+
+int b200tfs_concat_strings_bound(int32_t n, const uint64_t* rec_len, uint64_t* max_strings, uint64_t* max_data_bytes) {
+  if (n < 0 || (n && !rec_len)) return fail(B200TFS_E_ARG, "bad arguments");
+  uint64_t s = 0, b = 0;
+  for (int i = 0; i < n; ++i) { s += str_count_bound(rec_len[i]); b += rec_len[i]; }
+  if (max_strings) *max_strings = s;
+  if (max_data_bytes) *max_data_bytes = b;
+  return B200TFS_OK;
 }
 
 int b200tfs_padded_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
                           b200tfs_pad_key* keys, int32_t cast) {
-  return key_layout(wire_host, n, rec_off, rec_len, n_keys, keys, cast, true);
+  return key_layout(wire_host, n, rec_off, rec_len, n_keys, keys, cast, true,
+                    [](int, const uint8_t*, uint64_t, const b200tfs_output&) -> int32_t { return B200TFS_OK; });
 }
 
 namespace {
@@ -2335,7 +2382,7 @@ static int key_begin(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uin
 
 // A per-key decode on c->stream, around the route's plan: its scratch in `g` (KeyLayout, with the route's regions `own`), one
 // upload of rec_off | rec_len | key records (`dev_key(key, its bytes on the device)`) | key bytes, the parse kernel and the
-// ConcatPlan fields both routes use.  `plan(cp, scratch, layout, device key records, &pad)` launches the route's kernels, which
+// ConcatPlan fields both routes use.  `plan(cp, scratch, layout, device key records, device rec_len, &pad)` launches the route's kernels, which
 // write the single-launch decode's table with absolute dst_off, and may set `pad`, the placement of the varint emit.  Then the
 // varint tail over that table, and `res` becomes this call's.
 template <class Key, class DevKey, class Plan>
@@ -2376,7 +2423,7 @@ static int key_decode(b200tfs_ctx* c, Growable& g, b200tfs_ctx::KeyResults& res,
   cp.kst = (int32_t*)(d + L.kst); cp.match = (int32_t*)(d + L.match);
   cp.vouts = (b200tfs_output*)(d + L.vouts); cp.vn_outs = (int32_t*)(d + L.vnouts); cp.vrec_status = (int32_t*)(d + L.vstatus);
   const VarPadMap* pad = nullptr;
-  if ((rc = plan(cp, d, L, sd + o_keys, &pad))) return rc;
+  if ((rc = plan(cp, d, L, sd + o_keys, (const uint64_t*)(sd + o_len), &pad))) return rc;
   // packed-varint outputs: the single-launch decode's plan / count / emit over the table the plan kernel wrote (dst 0, stride 0)
   VarPlan vp{};
   vp.outs = cp.vouts; vp.n_outs = cp.vn_outs; vp.rec_status = cp.vrec_status;
@@ -2407,26 +2454,61 @@ static int key_decode_host_async(b200tfs_ctx* c, const void* wire_host, int32_t 
 
 int b200tfs_decode_concat(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
                           int32_t n_keys, const b200tfs_concat_key* keys) {
+  return b200tfs_decode_concat_strings(c, arena_dev, n, rec_off, rec_len, n_keys, keys, nullptr);
+}
+
+int b200tfs_decode_concat_strings(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                                  int32_t n_keys, const b200tfs_concat_key* keys, const b200tfs_concat_strings* strings) {
   uint64_t var_tile_cap = 0, tile_cap = 0;
-  int rc = key_begin(c, arena_dev, n, rec_off, rec_len, n_keys, keys, &var_tile_cap, [](const b200tfs_concat_key&, int) { return 0; });
+  int rc = key_begin(c, arena_dev, n, rec_off, rec_len, n_keys, keys, &var_tile_cap, [&](const b200tfs_concat_key&, int k) -> int {
+    if (strings && strings[k].data_cap && !strings[k].data) return fail(B200TFS_E_ARG, "key %d: string data is NULL", k);
+    return B200TFS_OK;
+  });
   if (rc) return rc;
   const uint32_t vpt = decode_vpt(c, n, rec_len);
   for (int i = 0; i < n; ++i) tile_cap += concat_record_tile_bound(rec_len[i], 16ull * vpt, (uint32_t)n_keys);
   if (tile_cap > 0x7FFFFFFFull) return fail(B200TFS_E_TOOBIG, "batch needs more than 2^31 tiles");
   const PlanGeometry g = plan_geometry((uint64_t)n * (uint64_t)n_keys * B200TFS_MAX_RUNS, tile_cap, 0);   // concat_plan_kernel's plan image
   if (g.off_tiles > 0xFFFFFFFFull) return fail(B200TFS_E_TOOBIG, "plan image larger than 4 GiB");
-  return key_decode(c, c->concat_dev, c->concat_res, arena_dev, n, rec_off, rec_len, n_keys, keys, var_tile_cap, {g.end},
-                    [](const b200tfs_concat_key& k, const uint8_t* kb) { return ConcatKeyDev{kb, (uint8_t*)k.dst, k.dst_cap, (uint32_t)k.key_len, 0u}; },
-                    [&](ConcatPlan& cp, uint8_t* d, const KeyLayout& L, const uint8_t* kd, const VarPadMap**) -> int {
-                      cp.keys = (const ConcatKeyDev*)kd; cp.vpt = vpt; cp.tile_cap = (uint32_t)tile_cap; cp.plan = d + L.own[0];
-                      CU(launch_concat_plan(cp, (uint32_t)tile_cap, c->stream));
-                      return B200TFS_OK;
-                    });
+  // the string pairs' scratch: bytes | data0 | chunk0 (n_keys * n each) | n_chunks
+  const uint64_t pairs = (uint64_t)n * (uint64_t)n_keys, str_bytes = 24 * pairs + 8;
+  uint64_t chunk_bound = 0;
+  for (int i = 0; strings && i < n; ++i) chunk_bound += (uint64_t)n_keys * (str_count_bound(rec_len[i]) / kStrChunk + 1);
+  const auto plan = [&](ConcatPlan& cp, uint8_t* d, const KeyLayout& L, const uint8_t* kd, const uint64_t* len_dev, const VarPadMap**) -> int {
+    cp.keys = (const ConcatKeyDev*)kd; cp.vpt = vpt; cp.tile_cap = (uint32_t)tile_cap; cp.plan = d + L.own[0];
+    CU(launch_concat_plan(cp, (uint32_t)tile_cap, c->stream, strings != nullptr));
+    if (!strings) return B200TFS_OK;
+    StrTables T{};
+    for (int k = 0; k < n_keys; ++k) T.keys[k] = StrKeyDev{(uint8_t*)strings[k].data, strings[k].data_cap};
+    T.w = cp.w; T.rec_off = cp.rec_off; T.rec_len = len_dev; T.vouts = cp.vouts;
+    T.bytes = (uint64_t*)(d + L.own[1]); T.data0 = T.bytes + pairs; T.chunk0 = T.data0 + pairs; T.n_chunks = T.chunk0 + pairs;
+    T.n = (uint32_t)n; T.n_keys = (uint32_t)n_keys;
+    const uint64_t grid = std::min<uint64_t>((chunk_bound + kStrThreads / 32 - 1) / (kStrThreads / 32), (uint64_t)c->sm_count * 8);
+    CU(launch_concat_strings(T, (uint32_t)grid, c->stream));
+    c->launches += 4;
+    return B200TFS_OK;
+  };
+  const auto dev_key = [](const b200tfs_concat_key& k, const uint8_t* kb) { return ConcatKeyDev{kb, (uint8_t*)k.dst, k.dst_cap, (uint32_t)k.key_len, 0u}; };
+  if (strings)
+    return key_decode(c, c->concat_dev, c->concat_res, arena_dev, n, rec_off, rec_len, n_keys, keys, var_tile_cap, {g.end, str_bytes}, dev_key, plan);
+  return key_decode(c, c->concat_dev, c->concat_res, arena_dev, n, rec_off, rec_len, n_keys, keys, var_tile_cap, {g.end}, dev_key, plan);
 }
 
 int b200tfs_decode_concat_host_async(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
                                      int32_t n_keys, const b200tfs_concat_key* keys) {
   return key_decode_host_async(c, wire_host, n, rec_off, rec_len, n_keys, keys, "b200tfs_decode_concat", b200tfs_decode_concat);
+}
+
+int b200tfs_decode_concat_strings_host_async(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off,
+                                             const uint64_t* rec_len, int32_t n_keys, const b200tfs_concat_key* keys,
+                                             const b200tfs_concat_strings* strings) {
+  if (!c || n <= 0 || !wire_host || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
+  if (c->capturing) return fail(B200TFS_E_ARG, "capture b200tfs_decode_concat_strings over a device arena instead");
+  CU(cudaSetDevice(c->device));
+  uint64_t span;
+  int rc = stage_wire(c, wire_host, n, rec_off, rec_len, &span);
+  if (rc) return rc;
+  return b200tfs_decode_concat_strings(c, c->stage_dev.p, n, rec_off, rec_len, n_keys, keys, strings);
 }
 
 // The results of a per-key decode (`R` of its most recent call, its scratch at `base`), as b200tfs_concat_results describes them
@@ -2495,7 +2577,7 @@ int b200tfs_decode_padded(b200tfs_ctx* c, const void* arena_dev, int32_t n, cons
                       kd.rank = k.rank;
                       return kd;
                     },
-                    [&](ConcatPlan& cp, uint8_t* d, const KeyLayout& L, const uint8_t* kd, const VarPadMap** pad) -> int {
+                    [&](ConcatPlan& cp, uint8_t* d, const KeyLayout& L, const uint8_t* kd, const uint64_t*, const VarPadMap** pad) -> int {
                       PaddedPlan pp{};
                       pp.cp = cp;
                       pp.keys = (const PadKeyDev*)kd;

@@ -44,6 +44,7 @@
 #include "framing.h"
 #include "kernels.h"
 #include "plan.h"
+#include "string_walk.h"
 #include "tpl.h"
 #include "unpad.h"
 #include "example_walk.h"
@@ -1116,7 +1117,10 @@ __device__ __forceinline__ const b200tfs_output* plan_key_reference(const Concat
   return rr < cp.n ? cp.outs + (size_t)rr * cp.out_stride + cp.match[(size_t)rr * cp.n_keys + k] : nullptr;
 }
 
-__global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const __grid_constant__ ConcatPlan cp) {
+// kStrings: the DT_STRING outputs get places too (b200tfs_decode_concat_strings): 8 * n_strings bytes of int64 offsets, and one
+// more entry behind them, in the key's destination; string_kernels.cuh fills them.  Without it they are left to the host.
+template <bool kStrings>
+__device__ __forceinline__ void concat_plan_body(const ConcatPlan& cp) {
   __shared__ unsigned long long warp_sum[kConcatPlanThreads / 32];
   __shared__ uint32_t ref_rec;
   const uint32_t n = cp.n, nk = cp.n_keys;
@@ -1134,7 +1138,7 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
       const uint32_t r = r0 + threadIdx.x;
       int32_t st = B200TFS_E_ARG;
       const b200tfs_output* o = nullptr;
-      uint64_t bytes = 0;
+      uint64_t bytes = 0, tail = 0;
       if (r < n) {
         st = cp.kst[(size_t)r * nk + k];
         const int32_t m = cp.match[(size_t)r * nk + k];
@@ -1144,11 +1148,13 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
           else if (o->rank != ro->rank) st = B200TFS_E_SHAPE;
           else for (int32_t d = 1; d < o->rank; ++d) if (o->dims[d] != ro->dims[d]) st = B200TFS_E_SHAPE;
         }
-        if (st == B200TFS_OK && dtype_info(o->dtype).kind == VK_STRING) st = B200TFS_E_NONCANONICAL;   // strings are decoded on the host
-        if (st == B200TFS_OK) bytes = tpl_narrows(cp.cast, o->dtype) ? o->n_elems * 2 : o->dst_bytes;
+        const bool str = st == B200TFS_OK && dtype_info(o->dtype).kind == VK_STRING;
+        if (str && !kStrings) st = B200TFS_E_NONCANONICAL;   // strings are decoded on the host
+        if (st == B200TFS_OK) bytes = str ? 8 * o->n_strings : tpl_narrows(cp.cast, o->dtype) ? o->n_elems * 2 : o->dst_bytes;
+        if (kStrings && str) tail = 8;                       // the entry behind the record's last string
       }
       const uint64_t off = concat_scan(bytes, byte_carry, warp_sum);
-      if (st == B200TFS_OK && off + bytes > key.cap) st = B200TFS_E_SIZE;
+      if (st == B200TFS_OK && off + bytes + tail > key.cap) st = B200TFS_E_SIZE;
       uint32_t tiles = 0;
       const bool narrow = st == B200TFS_OK && tpl_narrows(cp.cast, o->dtype);
       if (st == B200TFS_OK && bytes && dtype_info(o->dtype).kind == VK_FIXED)   // OK fixed-width outputs with elements have value runs
@@ -1192,6 +1198,16 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const _
     *reinterpret_cast<PlanHeader*>(cp.plan) = ph;
   }
 }
+
+__global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_kernel(const __grid_constant__ ConcatPlan cp) { concat_plan_body<false>(cp); }
+__global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_strings_kernel(const __grid_constant__ ConcatPlan cp) {
+  concat_plan_body<true>(cp);
+}
+
+// ------------------------------------------------------------------------------------------------
+// DT_STRING keys of the concatenated decode: str_index / str_scan / str_copy / str_fix
+// ------------------------------------------------------------------------------------------------
+#include "string_kernels.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // decode into one padded tensor per key: padded_plan_kernel / padded_emit_kernel
@@ -1340,8 +1356,9 @@ cudaError_t launch_decode_fused(const FusedParams& fp, uint32_t grid, cudaStream
   return launch_pdl(decode_fused_kernel, grid, kMoveThreads, 0, stream, fp);
 }
 
-cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStream_t stream) {
-  concat_plan_kernel<<<1, kConcatPlanThreads, 0, stream>>>(cp);
+cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStream_t stream, bool strings) {
+  if (strings) concat_plan_strings_kernel<<<1, kConcatPlanThreads, 0, stream>>>(cp);
+  else concat_plan_kernel<<<1, kConcatPlanThreads, 0, stream>>>(cp);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess || !move_grid) return e;
   // a plain launch: move_kernel reads PlanHeader::independent before it waits on the kernel in front of it, and here that kernel

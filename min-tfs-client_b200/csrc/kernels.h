@@ -46,7 +46,11 @@ cudaError_t launch_vdec_plan(const VarPlan& vp, cudaStream_t stream);
 cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t stream, const VarPadMap* pm = nullptr);
 // b200tfs_decode_concat: concat_plan_kernel, then move_kernel over the plan image it wrote, with move_grid CTAs (the host's bound
 // on the tiles; the CTAs past the plan's own count leave at once)
-cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStream_t stream);
+// (strings: concat_plan_strings_kernel, which places the DT_STRING outputs' offsets too)
+cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStream_t stream, bool strings = false);
+// b200tfs_decode_concat_strings, behind launch_concat_plan: index, scan, copy and fix (string_kernels.cuh); the index runs a warp
+// per (record, key), copy and fix run grid CTAs striding over the chunks
+cudaError_t launch_concat_strings(const StrTables& T, uint32_t grid, cudaStream_t stream);
 // b200tfs_decode_padded: padded_plan_kernel, then padded_emit_kernel with emit_grid CTAs striding over the chunks
 cudaError_t launch_padded(const PaddedPlan& pp, uint32_t emit_grid, cudaStream_t stream);
 // tf.Example requests (example_kernels.cuh): count + scan (when T.n_tiles), emit, frame; *launched receives how many kernels

@@ -254,6 +254,30 @@ constexpr uint64_t concat_record_tile_bound(uint64_t len, uint64_t tile_bytes, u
   return len / tile_bytes + 1ull + (uint64_t)n_keys * B200TFS_MAX_RUNS;
 }
 
+// ---- DT_STRING keys of the concatenated decode as byte columns (b200tfs_decode_concat_strings) -------------------------
+// concat_plan_strings_kernel scans 8 * n_strings of every (record, string key) into dst_off, the record's first offset entry.
+// Then (string_kernels.cuh): str_index_kernel - a warp per pair walks its string_val elements (string_walk.h) and packs each
+// one's record-relative wire offset (high 32 bits) and its byte position within the record's strings (low 32 bits) into the
+// offset entry the string owns, and leaves the pair's byte total; str_scan_kernel - one CTA places every pair's bytes in the
+// key's data and numbers the copy chunks (kStrChunk strings each); str_copy_kernel - a lane per short string, the warp for long
+// ones; str_fix_kernel - the offsets' final values, in a launch of its own because the copy reads the entry behind each string.
+constexpr uint32_t kStrChunk = 256;         // strings per copy chunk (eight per lane)
+constexpr uint32_t kStrLaneMax = 64;        // strings up to this many bytes are copied by one lane, longer ones by the warp
+constexpr uint32_t kStrThreads = 256;       // threads per CTA of the index, copy and fix kernels
+struct StrKeyDev { uint8_t* data; uint64_t cap; };
+struct StrTables {
+  const uint8_t* w;                // wire arena
+  const uint64_t* rec_off;         // [n], device
+  const uint64_t* rec_len;         // [n], device
+  b200tfs_output* vouts;           // the plan's table: record r, key k at r * kFusedMaxOutputs + k (dst_off absolute)
+  StrKeyDev keys[B200TFS_CONCAT_MAX_KEYS];   // the keys' string data (in the kernel parameters: a replay reads them as captured)
+  uint64_t* bytes;                 // [n_keys * n]: the pair's string bytes (index)
+  uint64_t* data0;                 // [n_keys * n]: its first byte in the key's data (scan)
+  uint64_t* chunk0;                // [n_keys * n]: its first copy chunk (scan; key-major, so it rises through the array)
+  uint64_t* n_chunks;              // [1]: chunks of every pair
+  uint32_t n, n_keys;
+};
+
 // ---- decode into one padded tensor per key (b200tfs_decode_padded) ----------------------------------------------------
 // padded_plan_kernel (one CTA) matches the keys as concat_plan_kernel does (plan_key_reference), checks every record against the
 // first one that decoded the key and against the destination's trailing dims, scans the rows into first rows and writes one

@@ -85,6 +85,12 @@ class ConcatKey(C.Structure):
     ]
 
 
+class ConcatStrings(C.Structure):
+    """b200tfs_concat_strings: the byte buffer of one DT_STRING key of b200tfs_decode_concat_strings, whose int64 offsets go to the
+    key's dst (in: data, data_cap; out of b200tfs_concat_strings_layout: strings, data_bytes)."""
+    _fields_ = [("data", C.c_void_p), ("data_cap", C.c_uint64), ("strings", C.c_uint64), ("data_bytes", C.c_uint64)]
+
+
 class PadKey(C.Structure):
     """b200tfs_pad_key: one requested output of b200tfs_decode_padded (in: key, dst, dst_cap, rank, dims[1:], pad_bits; out: the
     layout)."""
@@ -208,6 +214,13 @@ SIGNATURES = {
     "b200tfs_decode_concat": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(ConcatKey)]),
     "b200tfs_decode_concat_host_async": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(ConcatKey)]),
     "b200tfs_concat_results": (C.c_int, [_vp, C.c_int32, C.c_int32, C.POINTER(Output), C.POINTER(ModelSpec), _i32p]),
+    "b200tfs_concat_strings_layout": (C.c_int, [_vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(ConcatKey), C.POINTER(ConcatStrings),
+                                                C.c_int32]),
+    "b200tfs_concat_strings_bound": (C.c_int, [C.c_int32, _u64p, _u64p, _u64p]),
+    "b200tfs_decode_concat_strings": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(ConcatKey),
+                                                C.POINTER(ConcatStrings)]),
+    "b200tfs_decode_concat_strings_host_async": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(ConcatKey),
+                                                           C.POINTER(ConcatStrings)]),
     "b200tfs_padded_layout": (C.c_int, [_vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey), C.c_int32]),
     "b200tfs_decode_padded": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey)]),
     "b200tfs_decode_padded_host_async": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey)]),

@@ -463,6 +463,9 @@ _Launch = collections.namedtuple("_Launch", "n buf off dst stride tables specs")
 # response's status and DecodedSpec, and the destinations as Codec._key_deliver takes them (holds: their keep-alives)
 _KeyLaunch = collections.namedtuple("_KeyLaunch", "keys wire outs rec_status specs shapes np_types dev ptrs holds")
 
+# one response's DT_STRING output as the runtime gives it: string_val's raw bytes and the shape (-1 inferred)
+_RawStrings = collections.namedtuple("_RawStrings", "strings shape")
+
 
 class OpenResponse:
     """One PredictResponse after the fused launch: the table, and the host buffer the fixed-width outputs landed in."""
@@ -1073,9 +1076,9 @@ class Codec:
             fused = self._decode_fused(wires, strict, dict(out_dtypes))
         return fused if fused is not None else self._decode_two_phase(wires, strict, out_dtypes, max_outputs)
 
-    def _decode_two_phase(self, wires, strict, out_dtypes, max_outputs, keys=None):
+    def _decode_two_phase(self, wires, strict, out_dtypes, max_outputs, keys=None, raw_strings=False):
         """The parse kernel, then the unpack of every output - of the outputs named in `keys` only, when given (the others are
-        neither converted nor checked)."""
+        neither converted nor checked).  `raw_strings`: string outputs as _RawStrings instead of numpy str arrays."""
         parsed = self.parse_predict_responses(wires, max_outputs=max_outputs)
         jobs = []
         results: List[Tuple[Dict[str, np.ndarray], DecodedSpec]] = []
@@ -1085,8 +1088,16 @@ class Codec:
             for key, o in pr.outputs.items():
                 if keys is not None and key not in keys:
                     continue
+                if raw_strings and int(o.dtype) == DT_STRING and o.status == N.E_SHAPE:
+                    raise ValueError(f"output {key!r}: {int(o.n_strings)} strings do not fill its shape")
                 if int(o.dtype) == DT_STRING and o.status == N.OK:
-                    arrays[key] = self._decode_strings(pr.wire, pr.offset, o, pr.length, key)
+                    if raw_strings:
+                        proto = self._string_proto(pr.wire, pr.offset, o, pr.length, key)
+                        strs = list(proto.string_val)
+                        shape = np.empty(len(strs), np.uint8).reshape(tuple(int(d.size) for d in proto.tensor_shape.dim)).shape
+                        arrays[key] = _RawStrings(strs, shape)
+                    else:
+                        arrays[key] = self._decode_strings(pr.wire, pr.offset, o, pr.length, key)
                     continue
                 np_type, dst_code, shape = self._resolve_output(o, strict, out_dtypes.get(key) if out_dtypes else None)
                 jobs.append((arrays, key, o, np_type, dst_code, shape, pr.offset))
@@ -1198,8 +1209,8 @@ class Codec:
 
     # ---- batch decode into one tensor per key ------------------------------------------------------
     def decode_predict_responses_concat(self, wires: Sequence[bytes], keys: Optional[Sequence[str]] = None, *, strict: bool = False,
-                                        out_dtypes: Optional[Mapping] = None, device: bool = False,
-                                        out: Optional[Mapping] = None) -> Tuple[Dict[str, object], List[DecodedSpec]]:
+                                        out_dtypes: Optional[Mapping] = None, device: bool = False, out: Optional[Mapping] = None,
+                                        string_columns: bool = False) -> Tuple[Dict[str, object], List[DecodedSpec]]:
         """Decode a batch of PredictResponses into ONE tensor per output: for every key, the outputs of all responses
         concatenated along axis 0 - ``np.concatenate([decode_predict_responses([w], ...)[0][0][key] for w in wires], axis=0)``,
         bit for bit and with the same exceptions, except that outputs of different dtypes raise ValueError instead of being
@@ -1209,12 +1220,19 @@ class Codec:
         ``torch.as_tensor(a, device="cuda")`` takes them without a copy); otherwise numpy arrays, one device-to-host copy per
         key.  ``out={key: array}`` writes in place: a C-contiguous device array (CUDA array interface / DLPack) or a numpy /
         ``pinned_empty`` array of exactly the result's dtype and shape.  Returns ``({key: tensor}, [DecodedSpec per response])``.
+
+        ``string_columns=True``: every DT_STRING output comes back as a ``BytesColumn`` - the raw bytes of every response's
+        ``string_val`` (no UTF-8 check, NULs and high bytes kept), concatenated in response order, with ``offsets`` int64[m + 1]
+        from 0 and the concatenated shape - decoded on the device in the same call as the numeric outputs (``DeviceArray`` data and
+        offsets with ``device=True``, numpy arrays otherwise).  Such a column feeds ``encode_example_requests`` directly.  ``out``
+        naming a string output raises ValueError.  Without it, string outputs are numpy str arrays decoded on the host (and
+        ``device=True`` raises TypeError for them).
         """
         buf, off, ln, keys, out_dtypes, out = self._requested(wires, keys, out, out_dtypes, "need at least one response to concatenate")
-        fast = self._concat_device(wires, buf, off, ln, keys, strict, out_dtypes, device, out)
+        fast = self._concat_device(wires, buf, off, ln, keys, strict, out_dtypes, device, out, string_columns)
         if fast is not None:
             return fast
-        return self._concat_per_record(wires, keys, strict, out_dtypes, device, out)
+        return self._concat_per_record(wires, keys, strict, out_dtypes, device, out, string_columns)
 
     def _requested(self, wires, keys, out, out_dtypes, empty: str):
         """The front of a per-key batch decode: the batch staged (_pack_wires), the requested keys (None: every key of the first
@@ -1250,17 +1268,20 @@ class Codec:
                 return [self._text(buf, base + int(ko[i]), int(kl[i])) for i in range(cnt.value)]
             cap = cnt.value
 
-    def _per_record(self, wires, keys, strict, out_dtypes, device, out, bad_rank, combine):
+    def _per_record(self, wires, keys, strict, out_dtypes, device, out, bad_rank, combine, string_columns=False):
         """The definition itself, response by response, for the requested outputs: what a device route hands over when a batch
         holds a case it does not take (a malformed record, more than FUSED_MAX_OUTPUTS outputs or MAX_RANK dims, TF padding,
         tensor_content only, strings, mismatches).  Like the device routes it converts and checks the requested outputs only.
         Per key, the route's rank rule (`bad_rank(key, parts)`: the ValueError's message, or None), one dtype, and the route's
-        tensor of the parts (`combine(key, parts)`)."""
+        tensor of the parts (`combine(key, parts)`).  `string_columns`: string outputs become BytesColumns of their raw bytes."""
         wanted = set(keys)
-        per = [self._decode_two_phase([w], strict, out_dtypes, 16, wanted)[0] for w in wires]
+        per = [self._decode_two_phase([w], strict, out_dtypes, 16, wanted, string_columns)[0] for w in wires]
         result = {}
         for k in keys:
             parts = [p[0][k] for p in per]
+            if any(isinstance(a, _RawStrings) for a in parts):
+                result[k] = self._string_column(k, parts, device, out)
+                continue
             msg = bad_rank(k, parts)
             if msg:
                 raise ValueError(msg)
@@ -1272,10 +1293,30 @@ class Codec:
             result[k] = self._concat_deliver(k, arr, device, out)
         return result, [p[1] for p in per]
 
-    def _concat_per_record(self, wires, keys, strict, out_dtypes, device, out):
+    def _concat_per_record(self, wires, keys, strict, out_dtypes, device, out, string_columns=False):
         return self._per_record(wires, keys, strict, out_dtypes, device, out,
                                 lambda k, parts: "zero-dimensional arrays cannot be concatenated" if any(a.ndim == 0 for a in parts) else None,
-                                lambda k, parts: np.concatenate(parts, axis=0))
+                                lambda k, parts: np.concatenate(parts, axis=0), string_columns)
+
+    def _string_column(self, key, parts, device: bool, out) -> BytesColumn:
+        """The per-response route's BytesColumn of one string output, with the concatenation's errors (ValueError: rank 0, another
+        dtype, another rank or other trailing dims)."""
+        if key in out:
+            raise ValueError(f"output {key!r}: out= does not take string columns")
+        if any(isinstance(a, _RawStrings) and len(a.shape) == 0 or not isinstance(a, _RawStrings) and a.ndim == 0 for a in parts):
+            raise ValueError("zero-dimensional arrays cannot be concatenated")
+        if not all(isinstance(a, _RawStrings) for a in parts):
+            raise ValueError(f"output {key!r}: responses disagree on the dtype")
+        if len({a.shape[1:] for a in parts}) > 1 or len({len(a.shape) for a in parts}) > 1:
+            raise ValueError(f"output {key!r}: all the input array dimensions except for the concatenation axis must match exactly")
+        strs = [b for a in parts for b in a.strings]
+        offsets = np.zeros(len(strs) + 1, np.int64)
+        np.cumsum(np.fromiter(map(len, strs), np.int64, len(strs)), out=offsets[1:])
+        data = np.frombuffer(b"".join(strs), np.uint8)
+        shape = (sum(a.shape[0] for a in parts),) + tuple(parts[0].shape[1:])
+        if device:
+            return BytesColumn(self.device_array(data), self.device_array(offsets), shape)
+        return BytesColumn(data.copy(), offsets, shape)
 
     def _concat_deliver(self, key, arr: np.ndarray, device: bool, out):
         dst = out.get(key)
@@ -1290,12 +1331,14 @@ class Codec:
             self.sync()
         return dst
 
-    def _key_device(self, native, wires, buf, off, ln, keys, strict, out_dtypes, out, shape_of, place) -> Optional["_KeyLaunch"]:
+    def _key_device(self, native, wires, buf, off, ln, keys, strict, out_dtypes, out, shape_of, place,
+                    strings: bool = False) -> Optional["_KeyLaunch"]:
         """A per-key device route up to the results of its decode, or None when the batch holds a case it leaves to the
         per-response route.  `native`: the route's key struct and its layout, decode and results entry points.  The host layout
         runs first, so nothing is written into `out` for a batch the route then refuses.  `shape_of(i, key struct, numpy type)`
         is key i's result shape (None: refused); `place(key structs, pointers, shapes, numpy types)` completes the key structs
-        once the destinations are known (False: refused)."""
+        once the destinations are known (False: refused).  `strings`: DT_STRING keys are the route's too (their destination is
+        int64 offsets, which `shape_of` sizes), except that `out` may not name one (ValueError)."""
         if len(keys) > N.CONCAT_MAX_KEYS:
             return None
         key_type, layout, decode, results = native
@@ -1313,11 +1356,16 @@ class Codec:
         shapes, np_types = [], []
         for i in range(nk):
             c = ks[i]
-            if c.status != N.OK or c.dtype == DT_STRING or strict and c.dtype in (DT_BFLOAT16, DT_COMPLEX64, DT_COMPLEX128):
+            if c.status != N.OK or c.dtype == DT_STRING and not strings or strict and c.dtype in (DT_BFLOAT16, DT_COMPLEX64, DT_COMPLEX128):
                 return None
+            if c.dtype == DT_STRING and keys[i] in out:
+                raise ValueError(f"output {keys[i]!r}: out= does not take string columns")
             if cast_code and not _narrowing_fits(c.dtype, keys[i], out_dtypes):
                 return None
-            np_types.append(np.dtype(numpy_for_enum(cast_code if cast_code and c.dtype == DT_FLOAT else int(c.dtype))))
+            if c.dtype == DT_STRING:
+                np_types.append(np.dtype(np.int64))
+            else:
+                np_types.append(np.dtype(numpy_for_enum(cast_code if cast_code and c.dtype == DT_FLOAT else int(c.dtype))))
             shape = shape_of(i, c, np_types[i])
             if shape is None:
                 return None
@@ -1333,19 +1381,38 @@ class Codec:
         return _KeyLaunch(ks, wire, outs, rec_status, [self._spec(buf, int(off[r]), specs[r]) for r in range(n)],
                           shapes, np_types, dev, ptrs, holds)
 
-    def _concat_device(self, wires, buf, off, ln, keys, strict, out_dtypes, device, out):
+    def _concat_device(self, wires, buf, off, ln, keys, strict, out_dtypes, device, out, string_columns=False):
         """The device route (b200tfs_decode_concat): parse, one-CTA plan, move, varint decode - or None when the batch holds
-        a case it leaves to the per-response route."""
+        a case it leaves to the per-response route.  `string_columns`: with b200tfs_concat_strings entries (string index, scan,
+        copy and fix kernels) when a requested key is DT_STRING."""
+        nk = len(keys)
+        sc = (N.ConcatStrings * nk)() if string_columns else None
+        data = {}
+        lib = self._lib
+
+        def has_strings(ck):
+            return any(ck[i].dtype == DT_STRING and ck[i].status == N.OK for i in range(nk))
+
         def place(ck, ptrs, shapes, np_types):
-            for i in range(len(keys)):
+            for i in range(nk):
                 ck[i].dst, ck[i].dst_cap = ptrs[i], int(ck[i].bytes)
+                if ck[i].dtype == DT_STRING:
+                    data[i] = D.DeviceArray(self, (int(sc[i].data_bytes),), np.uint8)
+                    sc[i].data, sc[i].data_cap = data[i].ptr, int(sc[i].data_bytes)
             return True
-        f = self._key_device((N.ConcatKey, self._lib.b200tfs_concat_layout, self._lib.b200tfs_decode_concat, self._lib.b200tfs_concat_results),
-                             wires, buf, off, ln, keys, strict, out_dtypes, out,
-                             lambda i, c, np_type: tuple(int(c.dims[d]) for d in range(c.rank)), place)
+        if string_columns:
+            native = (N.ConcatKey, lambda *a: lib.b200tfs_concat_strings_layout(*a[:6], sc, a[6]),
+                      lambda *a: lib.b200tfs_decode_concat_strings(*a, sc if has_strings(a[6]) else None), lib.b200tfs_concat_results)
+        else:
+            native = (N.ConcatKey, lib.b200tfs_concat_layout, lib.b200tfs_decode_concat, lib.b200tfs_concat_results)
+        f = self._key_device(native, wires, buf, off, ln, keys, strict, out_dtypes, out,
+                             lambda i, c, np_type: (int(sc[i].strings) + 1,) if c.dtype == DT_STRING else tuple(int(c.dims[d]) for d in range(c.rank)),
+                             place, strings=string_columns)
         if f is None:
             return None
-        n, nk = len(wires), len(keys)
+        n = len(wires)
+        if any(f.outs[r * nk + i].status != N.OK for i in data for r in range(n)):
+            return None       # E_NONCANONICAL (a TensorProto in several `value` occurrences): the per-response route
         raw = np.frombuffer(f.outs, dtype=np.uint8).reshape(n * nk, C.sizeof(N.Output))
         status = raw[:, N.Output.status.offset: N.Output.status.offset + 4].copy().view(np.int32).ravel()
         redo = set(np.flatnonzero(status != N.OK).tolist())
@@ -1373,6 +1440,10 @@ class Codec:
             if any(st[q] != N.OK for q in range(m)):
                 return None
         result = self._key_deliver(keys, out, device, f.shapes, f.np_types, f.dev, f.ptrs)
+        for i, a in data.items():
+            c = f.keys[i]
+            shape = tuple(int(c.dims[d]) for d in range(c.rank))
+            result[keys[i]] = BytesColumn(a if device else a.copy_to_host(), result[keys[i]], shape)
         self.concat_device_calls += 1
         return result, f.specs
 
@@ -1635,6 +1706,13 @@ class Codec:
 
     @staticmethod
     def _decode_strings(buf: np.ndarray, base: int, o: N.Output, rec_len: int = 0, key: str = "") -> np.ndarray:
+        proto = Codec._string_proto(buf, base, o, rec_len, key)
+        shape = tuple(int(d.size) for d in proto.tensor_shape.dim)     # the host message is at hand: any rank
+        return np.array([e for e in proto.string_val], dtype=np.str_).reshape(*shape)
+
+    @staticmethod
+    def _string_proto(buf: np.ndarray, base: int, o: N.Output, rec_len: int = 0, key: str = ""):
+        """The TensorProto of a string output, as the runtime merges it."""
         from tensorflow.core.framework.tensor_pb2 import TensorProto
 
         proto = TensorProto.FromString(buf[base + o.msg_off: base + o.msg_off + o.msg_len].tobytes())
@@ -1644,8 +1722,7 @@ class Codec:
             from tensorflow_serving.apis.predict_pb2 import PredictResponse
 
             proto = PredictResponse.FromString(buf[base: base + rec_len].tobytes()).outputs[key]
-        shape = tuple(int(d.size) for d in proto.tensor_shape.dim)     # the host message is at hand: any rank
-        return np.array([e for e in proto.string_val], dtype=np.str_).reshape(*shape)
+        return proto
 
     def decode_predict_response(self, wire: bytes, *, out: Optional[Mapping[str, np.ndarray]] = None, **kw) -> Tuple[Dict[str, np.ndarray], DecodedSpec]:
         """One response.  ``out={key: array}``: the named outputs are written into the caller's arrays (dtype and shape must
