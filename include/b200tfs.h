@@ -584,6 +584,33 @@ int b200tfs_encode_padded_requests_async(b200tfs_ctx* ctx, int32_t n, const b200
  * length and, per input, where its payload starts and how long it is.  The request's rows start at row 0 of each padded input.     */
 int b200tfs_padded_request_frame(const b200tfs_request* req, const b200tfs_pad_input* in, const uint64_t* packed_len, void* buf,
                                  uint64_t cap, uint64_t* rec_len, uint64_t* payload_off, uint64_t* payload_len);
+/* The same three with DT_STRING inputs from string columns (the b200tfs_bytes layout below; bytes == NULL: those calls
+ * themselves).  bytes[i] goes with req->inputs[i]; offsets == NULL: not a string column.  A string input has src_dtype and
+ * wire_dtype DT_STRING, `data` is its byte buffer (data_len bytes, device memory for the _async call), `offsets` device int64[m + 1]
+ * for the m strings that fill `dims` in C order, and offsets[0] need not be 0 (a sliced column).  It is cut into boxes like any
+ * padded input (or is the same tensor in every request with B200TFS_F_BROADCAST), and each string of a box becomes one string_val
+ * value of its raw bytes, in C order (a box of no strings writes no string_val).
+ * A request's box reads, in this order, the offset of its first row's start, both ends of every string of the box, and its last
+ * row's end (a broadcast input: every offset), and they must satisfy
+ *     0 <= each offset <= data_len, and no offset read is smaller than the one read before it,
+ * so that the boxes of a call take disjoint byte ranges: the arena holds per padded string input data_len + 11 * strings bytes, per
+ * broadcast one n * (data_len + 11 * strings).  The kernels check this, and clamp every offset into [0, data_len] first, so no read
+ * leaves [data, data + data_len); a request that breaks it gets B200TFS_E_SHAPE in b200tfs_encode_results and no bytes (no store
+ * leaves [rec_off, rec_off + rec_len) of the others).  Such a request can let its neighbours read overlapping bytes, so that the
+ * good requests together need more than the arena bound: the later ones then get B200TFS_E_SIZE rather than their bytes.  Offsets that no box reads are never looked at.  A replayed CUDA graph
+ * follows new shapes, data and offsets as long as data_len and the column's dims stay the same.  A call with a string input
+ * launches two kernels more (string count and string emit).  In b200tfs_padded_request_frame_columns packed_len[i] stands in for
+ * the counted bytes of a string input's values (sum of 1 + varint(len) + len), as for a packed-varint input, and the offsets are not
+ * read.  A DT_STRING input without an entry: B200TFS_E_DTYPE; an entry on another dtype, a wire dtype other than DT_STRING,
+ * B200TFS_F_TENSOR_CONTENT / B200TFS_F_KEEP_SNAN on a string input, offsets not 8-byte aligned, a negative data_len or bytes flags
+ * other than B200TFS_F_DEVICE_DATA: B200TFS_E_ARG - all checked before the context's device is used.                            */
+struct b200tfs_bytes;   /* defined with the tf.Example string columns, below */
+int b200tfs_padded_request_columns_arena_size(int32_t n, const b200tfs_request* req, const struct b200tfs_bytes* bytes, uint64_t* out);
+int b200tfs_encode_padded_requests_columns_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_request* req, const b200tfs_pad_input* in,
+                                                 const struct b200tfs_bytes* bytes, void* arena_dev, uint64_t arena_cap);
+int b200tfs_padded_request_frame_columns(const b200tfs_request* req, const b200tfs_pad_input* in, const struct b200tfs_bytes* bytes,
+                                         const uint64_t* packed_len, void* buf, uint64_t cap, uint64_t* rec_len,
+                                         uint64_t* payload_off, uint64_t* payload_len);
 
 /* ---- CUDA graphs: record a fixed sequence of encode / decode calls once, replay it per request ---
  * Between capture_begin and capture_end the asynchronous entry points (b200tfs_encode_requests,

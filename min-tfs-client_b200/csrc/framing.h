@@ -19,7 +19,8 @@ struct TensorLayout {
   uint64_t header_len = 0;   // bytes before the payload
   uint32_t op = OP_COPY;     // MoveOp for fixed-width payloads
   bool varint = false;       // payload produced by the varint kernels
-  uint32_t field = 0;        // field number the values go into
+  uint32_t field = 0;        // field number the values go into; F_STRING: repeated string_val, each value its own 42 vi(len)
+                             // bytes field, so the payload (all of them) has no enclosing tag and length
   uint64_t shape_len = 0;    // bytes of the TensorShapeProto body
   DtypeInfo src_info{}, wire_info{};
 };
@@ -83,7 +84,7 @@ B2_HD uint64_t shape_body_len(int32_t rank, const int64_t* dims) {
 }
 
 // the header_len bytes in front of a tensor's payload: 08 vi(dtype) 12 vi(shape_len) {12 vi(dim_len) [08 vi(size)]}*
-// [tag vi(payload_len)]; nothing for a pre-serialised TensorProto
+// [tag vi(payload_len)] (not for string_val, whose values carry their own tags); nothing for a pre-serialised TensorProto
 template <class Out>
 B2_HD void write_tensor_header(Out& o, const b200tfs_tensor& t, const TensorLayout& L) {
   if (t.flags & B200TFS_F_PRESERIALIZED) return;
@@ -95,7 +96,7 @@ B2_HD void write_tensor_header(Out& o, const b200tfs_tensor& t, const TensorLayo
     if (d) { o.byte((uint8_t)(1 + varint_len(d))); o.byte(0x08); o.varint(d); }
     else o.byte(0x00);  // Dim(size=0) is an empty sub-message (Q2)
   }
-  if (L.payload_len) { o.varint(tag_of(L.field, WT_LEN)); o.varint(L.payload_len); }
+  if (L.payload_len && L.field != F_STRING) { o.varint(tag_of(L.field, WT_LEN)); o.varint(L.payload_len); }
 }
 
 // element e of a tiny packed-varint input, widened to 64 bits the way the protobuf runtime widens it (sign-extended if signed)

@@ -29,15 +29,22 @@ struct UnpadIn {                   // one input of every request, in wire (key) 
   uint32_t src_esz, wire_esz;      // element size in memory / wire bytes per element (fixed width and bool)
   uint32_t varint, is_signed, field;
   uint32_t key_off, key_len;       // key bytes in the blob
-  uint32_t pad_;
+  uint32_t str;                    // string input str - 1 (0: none) - a DT_STRING column (b200tfs_bytes), its offsets and data_len in
+                                   // UnpadPlan::str_cols: src is its byte buffer, element e is string e (src_esz 1, so a box's
+                                   // src_off counts strings), field F_STRING
+};
+
+struct UnpadStrCol {               // the offsets of a string input (kept out of UnpadIn, which the varint kernels copy per thread)
+  const int64_t* offsets;          // device int64[strings + 1]
+  int64_t data_len;                // bytes of the input's src
 };
 
 struct UnpadBox {                  // one (request, input)
   int64_t dims[B200TFS_MAX_RANK];  // the request's shape for the input
-  uint64_t src_off;                // byte offset of its first element in the source
+  uint64_t src_off;                // byte offset of its first element in the source (string column: index of its first string)
   uint64_t n_elems;
   uint64_t run, n_runs;            // n_runs runs of `run` elements (see above); n_runs <= 1: one contiguous stretch
-  uint64_t payload;                // wire bytes of its values (varints: the counted total)
+  uint64_t payload;                // wire bytes of its values (varints: the counted total; strings: sum of 1 + vi(len) + len)
   uint32_t lo, pad_;
 };
 
@@ -81,6 +88,36 @@ B2_HD uint64_t unpad_run_start(const UnpadIn& in, const UnpadBox& b, uint64_t q)
   }
   return off;
 }
+
+// ---- string columns --------------------------------------------------------------------------------------------------------
+// A box of a string column reads, in element order, the offset of its first row's start, both ends of every string of the box and
+// its last row's end; these must never decrease and stay within [0, data_len] (a broadcast input reads every offset).  When every
+// request of the call follows the rule, the boxes take disjoint byte ranges and the padded inputs' strings fit in data_len bytes.
+// The count and emit kernels see every offset through unpad_str_off: clamped into [0, data_len], so both agree on every length
+// whatever the offsets hold and no read leaves the buffer; a box whose offsets break the rule gets B200TFS_E_SHAPE and writes
+// nothing.  Such a request can also let the good ones on either side of it read overlapping bytes (its last row's end below its
+// first row's start), so that together they need more than the arena bound: the layout kernel's arena_cap check then gives the
+// later ones B200TFS_E_SIZE instead of their bytes - never a store outside the good records.
+B2_HD uint64_t unpad_str_off(const UnpadStrCol& c, uint64_t i, bool* ok) {
+  const int64_t v = c.offsets[i];
+  if (v < 0 || v > c.data_len) *ok = false;
+  return v < 0 ? 0 : v > c.data_len ? (uint64_t)c.data_len : (uint64_t)v;
+}
+// column index of string e of box b (src_off: the box's first string)
+B2_HD uint64_t unpad_str_index(const UnpadIn& in, const UnpadBox& b, uint64_t e) {
+  if (b.n_runs <= 1) return b.src_off + e;
+  const uint64_t q = e / b.run;
+  return b.src_off + unpad_run_start(in, b, q) + (e - q * b.run);
+}
+// the offset indexes of box b's first row's start and last row's end (broadcast: the whole column)
+B2_HD void unpad_str_rows(const UnpadIn& in, const UnpadBox& b, uint64_t* first, uint64_t* end) {
+  uint64_t w = 1;
+  for (int32_t d = 1; d < in.rank; ++d) w *= (uint64_t)in.dims[d];
+  *first = in.shapes ? b.src_off : 0;
+  *end = in.shapes ? b.src_off + (uint64_t)b.dims[0] * w : b.n_elems;
+}
+// wire bytes of one string_val value of `len` bytes: 42 vi(len) bytes
+B2_HD uint64_t unpad_str_wire(uint64_t len) { return 1 + varint_len(len) + len; }
 
 struct UnpadFrame {                // what every request's framing has in common
   const uint8_t* blob;             // model_spec field (its tag included) at 0, then the keys
@@ -153,6 +190,17 @@ struct UnpadPlan {
   unsigned long long* total;       // [n * n_var]
   uint32_t* n_var_tiles;           // [1]
   uint32_t var_tile_cap, var_group_cap;
+  // string jobs (request r, string input k: r * n_str + k), in tables of their own shaped like the varint ones: a tile is
+  // kVarThreads strings, tile_val its wire bytes (saturated at 2^32 - 1), total the box's payload
+  uint32_t n_str, str_tile_cap, str_group_cap, pad2_;
+  uint8_t str_in[kUnpadMaxInputs]; // input index of string input k
+  const UnpadStrCol* str_cols;     // [n_str]
+  VarJobDev* str_jobs;             // [n * n_str]
+  uint32_t* str_tile_job;          // [str_tile_cap]
+  uint32_t* str_tile_val;          // [str_tile_cap]
+  uint32_t* str_group_sum;         // [str_group_cap]
+  unsigned long long* str_total;   // [n * n_str]
+  uint32_t* n_str_tiles;           // [1]
   // move plan: PlanHeader | MoveItem[item_cap] | TileRef[tile_cap]
   uint8_t* plan;
   uint32_t item_cap, tile_cap, vpt, pad_;

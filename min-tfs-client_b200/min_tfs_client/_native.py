@@ -228,6 +228,11 @@ SIGNATURES = {
     "b200tfs_padded_request_arena_size": (C.c_int, [C.c_int32, C.POINTER(Request), _u64p]),
     "b200tfs_encode_padded_requests_async": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), C.POINTER(PadInput), _vp, C.c_uint64]),
     "b200tfs_padded_request_frame": (C.c_int, [C.POINTER(Request), C.POINTER(PadInput), _u64p, _vp, C.c_uint64, _u64p, _u64p, _u64p]),
+    "b200tfs_padded_request_columns_arena_size": (C.c_int, [C.c_int32, C.POINTER(Request), C.POINTER(Bytes), _u64p]),
+    "b200tfs_encode_padded_requests_columns_async": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), C.POINTER(PadInput), C.POINTER(Bytes),
+                                                               _vp, C.c_uint64]),
+    "b200tfs_padded_request_frame_columns": (C.c_int, [C.POINTER(Request), C.POINTER(PadInput), C.POINTER(Bytes), _u64p, _vp, C.c_uint64,
+                                                       _u64p, _u64p, _u64p]),
     "b200tfs_capture_begin": (C.c_int, [_vp]),
     "b200tfs_capture_end": (C.c_int, [_vp, _vpp]),
     "b200tfs_graph_launch": (C.c_int, [_vp, _vp]),

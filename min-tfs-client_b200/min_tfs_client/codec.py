@@ -65,12 +65,86 @@ def _string_tensor_proto_bytes(arr: np.ndarray) -> bytes:
     return proto.SerializeToString()
 
 
+def _bytes_tensor_proto_bytes(col: "BytesColumn") -> bytes:
+    """Host assembly of the DT_STRING TensorProto of a host ``BytesColumn``: one string_val value of raw bytes per string."""
+    from tensorflow.core.framework.tensor_pb2 import TensorProto
+    from tensorflow.core.framework.tensor_shape_pb2 import TensorShapeProto
+
+    proto = TensorProto(dtype=DT_STRING, tensor_shape=TensorShapeProto(dim=[TensorShapeProto.Dim(size=d) for d in col.shape]))
+    o, d = col.offsets.tolist(), col.data
+    proto.string_val.extend(d[o[j]: o[j + 1]].tobytes() for j in range(len(o) - 1))
+    return proto.SerializeToString()
+
+
+def _string_wire_dtype(key, wire_dtype) -> None:
+    """ValueError when the wire dtype given for a string column is not DT_STRING."""
+    if wire_dtype is not None and _as_enum(wire_dtype) != DT_STRING:
+        raise ValueError(f"input {key!r}: a BytesColumn goes on the wire as DT_STRING, not {wire_dtype!r}")
+
+
+def _check_host_offsets(key, col: "BytesColumn") -> None:
+    """The offsets rule for host offsets, over the whole column: they never decrease and stay within ``0..data_len``."""
+    if col.offsets_on_device:
+        return
+    o = col.offsets
+    if o[0] < 0 or o[-1] > col.data_len or (o.size > 1 and (np.diff(o) < 0).any()):
+        raise ValueError(f"input {key!r}: string offsets must rise within 0..{col.data_len}")
+
+
+def _bytes_box(key, col: "BytesColumn", r0: int, row) -> "BytesColumn":
+    """The strings of the box ``[r0 : r0 + row[0], :row[1], ...]`` of a padded host ``BytesColumn`` (``row``: a request's shape
+    row, or its row count with every trailing dim full), in C order, as a column of their raw bytes.  Checks the offsets rule for
+    the box alone - its first row's start, both ends of each of its strings, its last row's end never decrease and stay within
+    ``0..data_len`` (ValueError) - as the device route does.  Work and memory are proportional to the box."""
+    dims = col.shape
+    bd = (int(row[0]),) + (tuple(int(x) for x in row[1:]) if len(row) > 1 else tuple(int(d) for d in dims[1:]))
+    st = [int(np.prod(dims[a + 1:], dtype=np.int64)) for a in range(len(dims))]     # elements of one index of each axis
+    idx = np.asarray(r0 * st[0], np.int64)
+    for b, s in zip(bd, st):
+        idx = idx[..., None] + np.arange(b, dtype=np.int64) * s
+    flat = idx.ravel()
+    o = col.offsets
+    seq = np.concatenate([o[r0 * st[0]: r0 * st[0] + 1], np.stack([o[flat], o[flat + 1]], 1).ravel(),
+                          o[(r0 + bd[0]) * st[0]: (r0 + bd[0]) * st[0] + 1]])
+    if seq[0] < 0 or seq[-1] > col.data_len or (np.diff(seq) < 0).any():
+        raise ValueError(f"input {key!r}: the string offsets of a request's box must rise within 0..{col.data_len}")
+    lens = o[flat + 1] - o[flat]
+    offsets = np.zeros(flat.size + 1, np.int64)
+    np.cumsum(lens, out=offsets[1:])
+    at = np.repeat(o[flat] - offsets[:-1], lens) + np.arange(int(offsets[-1]), dtype=np.int64)
+    return BytesColumn(np.asarray(col.data)[at], offsets, bd)
+
+
+class _PaddedString:
+    """The Tensor struct of a string column of the padded encode (what the call reads of a _Prepared)."""
+
+    __slots__ = ("key", "dims", "struct")
+
+    def __init__(self, key: bytes, shape):
+        self.key = key
+        self.dims = (C.c_int64 * max(len(shape), 1))(*shape)
+        self.struct = None
+
+
 class _Prepared:
     """One input readied for the C ABI; keeps every buffer the Tensor struct points at alive."""
 
     __slots__ = ("array", "dims", "key", "struct", "on_device", "nbytes", "ndim", "size", "itemsize", "kind")
 
     def __init__(self, value, key: bytes, wire_dtype, tensor_content: bool, keep_snan: bool):
+        if isinstance(value, BytesColumn):
+            # raw strings, assembled on the host like a numpy str tensor (tensor_content / keep_snan do not apply to strings)
+            if value.data_on_device or value.offsets_on_device:
+                raise ValueError(f"input {key!r}: a BytesColumn of device arrays is encoded by encode_predict_requests_padded; "
+                                 "encode_predict_requests takes host arrays")
+            _string_wire_dtype(key, wire_dtype)
+            _check_host_offsets(key, value)
+            blob = np.frombuffer(_bytes_tensor_proto_bytes(value), dtype=np.uint8)
+            self.on_device, self.array, self.dims, self.key = False, blob, (C.c_int64 * 1)(0), key
+            self.struct = N.Tensor(data=blob.ctypes.data if blob.size else None, src_dtype=DT_STRING, wire_dtype=DT_STRING, rank=0,
+                                   flags=N.F_PRESERIALIZED, dims=self.dims, key=key, key_len=len(key), packed_len=blob.size)
+            self.nbytes, self.ndim, self.size, self.itemsize, self.kind = int(blob.size), 1, int(blob.size), 1, "u"
+            return
         self.on_device = D.is_device_object(value)
         if self.on_device:
             # a tensor that already lives in HBM (CUDA array interface / DLPack): encoded in place, no host-to-device copy
@@ -668,7 +742,11 @@ class Codec:
         header in front (for a transport that writes HTTP/2 DATA frames itself; grpc-python adds it on its own).
         Inputs may be numpy arrays (pageable or ``pinned_empty``) or device arrays (``__cuda_array_interface__`` / DLPack: no
         host-to-device copy).  ``out="pinned"`` returns uint8 views of the codec's page-locked landing buffer instead of ``bytes``
-        objects (no copy on the host; valid until the next encode on this codec).
+        objects (no copy on the host; valid until the next encode on this codec).  A DT_STRING input may be a numpy str array
+        (UTF-8, as the reference) or a ``BytesColumn`` of host arrays: a DT_STRING tensor of its shape whose ``string_val`` holds
+        each string's raw bytes (NULs and high bytes kept), so binary data such as an encoded image can be sent; its offsets must
+        rise within ``0..data_len`` and ``wire_dtype`` must be DT_STRING if given (ValueError).  A ``BytesColumn`` of device arrays
+        raises ValueError: ``encode_predict_requests_padded`` encodes those on the device.
         """
         keep, structs = self._build_requests(list(requests), order, wire_dtype, tensor_content, keep_snan, grpc_frame)
         n = len(structs)
@@ -715,8 +793,15 @@ class Codec:
         ``encode_predict_request`` returns for that request.  Inputs and shapes may be numpy arrays (pageable or ``pinned_empty``) or
         device arrays (``__cuda_array_interface__`` / DLPack); device shapes never travel to the host - the rows, boxes and framing
         are planned by kernels.  A negative dim, a trailing dim past ``D_j``, a shape of another rank, rows past ``R`` or a request
-        count that differs between keys raise ValueError.  DT_STRING inputs, more than 8 padded or 8 broadcast inputs and ranks
-        above 16 are cut on the host and encoded request by request.  ``out="pinned"`` as for ``encode_predict_requests``.
+        count that differs between keys raise ValueError.  ``out="pinned"`` as for ``encode_predict_requests``.
+
+        A string input is a ``BytesColumn`` (padded or broadcast, its data and offsets on the host or the device): each string of a
+        box becomes one ``string_val`` value of its raw bytes (NULs and high bytes kept), cut and framed on the device beside the
+        numeric inputs; ``wire_dtype`` other than DT_STRING for it raises ValueError.  The offsets a request reads - its first row's
+        start, both ends of every string of its box, its last row's end (a broadcast column: every offset) - must never decrease and
+        stay within ``0..data_len``.  Host offsets are checked over the whole column before anything runs; device offsets are checked
+        by the kernels, only where a box reads them; either way a break raises ValueError.  Numpy str / bytes / object inputs, more
+        than 8 padded or 8 broadcast inputs and ranks above 16 are cut on the host and encoded request by request.
         """
         if out is not None and out != "pinned":
             raise ValueError('out must be None or "pinned"')
@@ -725,7 +810,14 @@ class Codec:
             raise ValueError("shapes must have exactly the keys of inputs")
         if set(inputs) & set(broadcast):
             raise ValueError("a key cannot be both padded and broadcast")
-        pdims = {k: tuple(D.device_view(v)[1]) if D.is_device_object(v) else np.shape(v) for k, v in inputs.items()}
+        def dims_of(v):
+            return v.shape if isinstance(v, BytesColumn) else tuple(D.device_view(v)[1]) if D.is_device_object(v) else np.shape(v)
+
+        pdims = {k: dims_of(v) for k, v in inputs.items()}
+        for k, v in list(inputs.items()) + list(broadcast.items()):
+            if isinstance(v, BytesColumn):
+                _string_wire_dtype(k, wire_dtype.get(k) if isinstance(wire_dtype, Mapping) else wire_dtype)
+                _check_host_offsets(k, v)
         n = None
         host_shapes = {}
         for k, s in shapes.items():
@@ -752,8 +844,9 @@ class Codec:
                 host_shapes[k] = a
         if not n:
             return []
-        dtypes = [D.device_view(v)[2] if D.is_device_object(v) else np.asarray(v).dtype for v in list(inputs.values()) + list(broadcast.values())]
-        ranks = list(pdims.values()) + [tuple(D.device_view(v)[1]) if D.is_device_object(v) else np.shape(v) for v in broadcast.values()]
+        dtypes = [D.device_view(v)[2] if D.is_device_object(v) else np.asarray(v).dtype for v in list(inputs.values()) + list(broadcast.values())
+                  if not isinstance(v, BytesColumn)]
+        ranks = list(pdims.values()) + [dims_of(v) for v in broadcast.values()]
         if (any(dt.kind in "OUS" for dt in dtypes) or len(inputs) > N.CONCAT_MAX_KEYS or len(broadcast) > N.CONCAT_MAX_KEYS
                 or any(len(r) > N.MAX_RANK for r in ranks)):
             return self._padded_requests_on_host(model_name, model_version, inputs, shapes, broadcast, n, order=order, wire_dtype=wire_dtype,
@@ -770,11 +863,16 @@ class Codec:
             keep.append(d)
             return d
 
-        preps, pins = [], []
+        preps, pins, strs = [], [], []
         for k, v in list(inputs.items()) + list(broadcast.items()):
             kb = k.encode("utf-8") if isinstance(k, str) else bytes(k)
             wd = wire_dtype.get(k) if isinstance(wire_dtype, Mapping) else wire_dtype
-            p = _Prepared(dev(v), kb, wd, tensor_content, keep_snan)
+            if isinstance(v, BytesColumn):
+                p, b = self._padded_string_input(v, kb, keep)
+                strs.append(b)
+            else:
+                p = _Prepared(dev(v), kb, wd, tensor_content, keep_snan)
+                strs.append(N.Bytes())
             if k in broadcast:
                 p.struct.flags |= N.F_BROADCAST
                 pins.append(N.PadInput(shapes=None, cols=0))
@@ -795,12 +893,20 @@ class Codec:
                         version=int(model_version) if model_version is not None else 0, n_inputs=len(preps),
                         flags=N.RF_GRPC_FRAME if grpc_frame else 0, inputs=arr)
         cap = C.c_uint64()
-        N.check(self._lib.b200tfs_padded_request_arena_size(n, C.byref(req), C.byref(cap)))
+        bs = (N.Bytes * len(strs))(*strs) if any(b.offsets for b in strs) else None
+        if bs is None:
+            N.check(self._lib.b200tfs_padded_request_arena_size(n, C.byref(req), C.byref(cap)))
+        else:
+            N.check(self._lib.b200tfs_padded_request_columns_arena_size(n, C.byref(req), bs, C.byref(cap)))
         if self._pe_arena is None or self._pe_arena.nbytes < cap.value:
             if self._pe_arena is not None:
                 self._pe_arena.free()
             self._pe_arena = D.DeviceArray(self, (max(int(cap.value), 1),), np.uint8)
-        N.check(self._lib.b200tfs_encode_padded_requests_async(self._ctx, n, C.byref(req), pin_arr, self._pe_arena.ptr, cap.value))
+        if bs is None:
+            N.check(self._lib.b200tfs_encode_padded_requests_async(self._ctx, n, C.byref(req), pin_arr, self._pe_arena.ptr, cap.value))
+        else:
+            N.check(self._lib.b200tfs_encode_padded_requests_columns_async(self._ctx, n, C.byref(req), pin_arr, bs, self._pe_arena.ptr,
+                                                                            cap.value))
         off, ln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
         rc = self._lib.b200tfs_encode_results(self._ctx, n, off, ln)
         if rc in (N.E_SHAPE, N.E_SIZE):
@@ -816,7 +922,31 @@ class Codec:
             return [pw.array[off[i]: off[i] + ln[i]] for i in range(n)]
         return [pw.array[off[i]: off[i] + ln[i]].tobytes() for i in range(n)]
 
+    def _padded_string_input(self, col: "BytesColumn", key: bytes, keep: list):
+        """(_Prepared-like holder of the DT_STRING Tensor, Bytes entry) of a string column of the padded encode; host arrays are
+        copied to the device (the kernels read both there)."""
+        def on_device(a, on_dev, dtype):
+            if on_dev:
+                ptr, _, _, hold = D.device_view(a)
+                keep.append(hold)
+                return ptr
+            d = self.device_array(np.ascontiguousarray(a, dtype=dtype))
+            keep.append(d)
+            return d.ptr
+
+        data = on_device(col.data, col.data_on_device, np.uint8) if col.data_len else None
+        offsets = on_device(col.offsets, col.offsets_on_device, np.int64)
+        p = _PaddedString(key, col.shape)
+        p.struct = N.Tensor(data=data, src_dtype=DT_STRING, wire_dtype=DT_STRING, rank=len(col.shape), flags=N.F_DEVICE_DATA,
+                            dims=p.dims, key=key, key_len=len(key), packed_len=0)
+        return p, N.Bytes(offsets=offsets, data_len=col.data_len, flags=N.F_DEVICE_DATA)
+
     def _to_host(self, v) -> np.ndarray:
+        if isinstance(v, BytesColumn):
+            if not (v.data_on_device or v.offsets_on_device):
+                return v
+            data = self._to_host(v.data) if v.data_on_device else v.data
+            return BytesColumn(data, self._to_host(v.offsets) if v.offsets_on_device else v.offsets, v.shape)
         if not D.is_device_object(v):
             return np.asarray(v)
         ptr, shape, dtype, _hold = D.device_view(v)
@@ -831,6 +961,9 @@ class Codec:
         P = {k: self._to_host(v) for k, v in inputs.items()}
         S = {k: self._to_host(s).astype(np.int64).reshape(n, -1) for k, s in shapes.items()}
         B = {k: self._to_host(v) for k, v in broadcast.items()}
+        for k, v in B.items():
+            if isinstance(v, BytesColumn):
+                _check_host_offsets(k, v)   # a broadcast column is read in full; a padded one box by box (_bytes_box)
         for k, s in S.items():
             if (s < 0).any() or (s.shape[1] > 1 and (s[:, 1:] > np.asarray(P[k].shape[1:])).any()) or int(s[:, 0].sum()) > P[k].shape[0]:
                 raise ValueError(f"shapes of {k!r} do not fit the padded tensor {P[k].shape}")
@@ -841,7 +974,7 @@ class Codec:
             for k, p in P.items():
                 s = S[k][r]
                 box = (slice(int(r0[k][r]), int(r0[k][r]) + int(s[0])),) + tuple(slice(0, int(x)) for x in s[1:])
-                d[k] = p[box]
+                d[k] = _bytes_box(k, p, int(r0[k][r]), s) if isinstance(p, BytesColumn) else p[box]
             d.update(B)
             reqs.append((model_name, model_version, d))
         return self.encode_predict_requests(reqs, **kw)

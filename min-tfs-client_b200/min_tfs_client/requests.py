@@ -170,7 +170,9 @@ def gpu_regression_response_deserializer(wire: bytes) -> RegressionResponseView:
 
 
 def gpu_request_serializer(request) -> bytes:
-    """``request_serializer`` for ``channel.unary_unary``: (model_name, model_version, input_dict) -> bytes."""
+    """``request_serializer`` for ``channel.unary_unary``: (model_name, model_version, input_dict) -> bytes.  A DT_STRING input may
+    be a numpy str array (UTF-8, as the reference) or a ``BytesColumn`` of host arrays, whose strings go out as their raw bytes -
+    how a request carries binary data such as encoded images."""
     model_name, model_version, input_dict = request
     return get_codec().encode_predict_request(model_name, input_dict, model_version)
 

@@ -6,6 +6,12 @@ Workloads (sequence and image clients whose batch is already on the GPU):
   U2  256 x f32[1, T_r, 1024] from f32[256, 512, 1024]
   U3  the split of f32[262144, 1024] into 256 x f32[1024, 1024]
   U4  64 x f32[1, H_r, W_r, 3] from f32[64, 512, 512, 3]
+String workloads (DT_STRING inputs from a BytesColumn on the device; --strings runs these alone):
+  T1  1024 x {text: string[rows_r], ids: int64[rows_r]}, rows_r in 1..64, strings of 16..256 bytes
+  T2  256 x text: string[rows_r, S_r1] from string[R, 8], rows_r in 1..32, S_r1 in 1..8, strings of 16..64 bytes
+  T3  64 x image_bytes: string[1], one binary string of 256 KiB - 2 MiB each
+  legs: device (eager and graph, as above), today (a numpy str_ column through the host route; T3 has none: binary data cannot be
+  a str_ array) and protobuf (the requests built and serialized with the protobuf runtime on one host core).
 Legs:
   device  the C call, eager (host call to results, arena ready on the device) and as a replayed CUDA graph
   quo     the status quo: shapes to the host, a synchronise, per-request structs over the device boxes planned on the host, then
@@ -13,7 +19,7 @@ Legs:
   existing  the same b200tfs_encode_requests_async with the requests planned once: the existing encode at equal bytes
   python  Codec.encode_predict_requests_padded (bytes on the host)
   defn    the definition: host slicing, then encode_predict_requests
-Usage: python tools/padded_encode_probe.py [out.json]
+Usage: python tools/padded_encode_probe.py [--strings] [out.json]
 GB/s = (source bytes read + wire bytes written) / time; share of the H100 SXM's 3.35 TB/s.
 """
 import ctypes as C
@@ -26,12 +32,13 @@ import time
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path[:0] = [os.path.join(HERE, "..", "min-tfs-client_b200"), os.path.join(HERE, "..")]
+sys.path[:0] = [os.path.join(HERE, "..", "min-tfs-client_b200"), os.path.join(HERE, ".."), os.path.join(HERE, "..", "tests")]
 
 import torch  # noqa: E402
 
 from min_tfs_client import _native as N  # noqa: E402
-from min_tfs_client.codec import Codec  # noqa: E402
+from min_tfs_client.codec import BytesColumn, Codec  # noqa: E402
+import padded_strings_ref as SR  # noqa: E402
 
 
 def workloads(rng):
@@ -55,6 +62,125 @@ def timed(fn, reps):
     return (time.perf_counter() - t) / reps, out
 
 
+def string_workloads(rng):
+    """(name, strings, dims, shapes, numeric padded inputs, text strings?) of T1-T3"""
+    def text(m, lo, hi):
+        lens = rng.integers(lo, hi + 1, m)
+        letters = rng.integers(97, 123, int(lens.sum())).astype(np.uint8).tobytes()
+        off = np.concatenate([[0], np.cumsum(lens)])
+        return [letters[off[j]: off[j + 1]] for j in range(m)]
+    rows = rng.integers(1, 65, 1024).astype(np.int64)
+    R = int(rows.sum())
+    yield "T1", text(R, 16, 256), (R,), rows, {"ids": rng.integers(0, 1 << 40, R)}, True
+    rows = rng.integers(1, 33, 256).astype(np.int64)
+    R = int(rows.sum())
+    yield "T2", text(R * 8, 16, 64), (R, 8), np.stack([rows, rng.integers(1, 9, 256)], 1), {}, True
+    sizes = rng.integers(256 << 10, (2 << 20) + 1, 64)
+    yield "T3", [rng.integers(0, 256, int(k)).astype(np.uint8).tobytes() for k in sizes], (64,), np.ones(64, np.int64), {}, False
+
+
+def run_strings(codec, lib, rng, out):
+    for name, strs, dims, shapes, numeric, is_text in string_workloads(rng):
+        n = len(shapes)
+        key = "image_bytes" if name == "T3" else "text"
+        lens = np.array([len(x) for x in strs], np.int64)
+        offs = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+        data_h = np.frombuffer(b"".join(strs), np.uint8)
+        data, offsets = torch.from_numpy(data_h.copy()).cuda(), torch.from_numpy(offs).cuda()
+        col = BytesColumn(data, offsets, dims)
+        num = {k: torch.from_numpy(v).cuda() for k, v in numeric.items()}
+        S = {key: torch.from_numpy(np.ascontiguousarray(shapes)).cuda(), **{k: torch.from_numpy(np.ascontiguousarray(shapes.reshape(n, -1)[:, 0])).cuda()
+                                                                             for k in numeric}}
+        ref = SR.reference_requests("m", 1, {key: (strs, dims), **numeric}, {k: s.cpu().numpy() for k, s in S.items()}, {})
+        # source bytes: the strings of the boxes, their offsets and the numeric boxes; wire bytes: the requests
+        box_bytes, box_strs, r0 = 0, 0, 0
+        for r in range(n):
+            row = shapes.reshape(n, -1)[r]
+            bs, _ = SR.box_strings(list(range(len(strs))), dims, r0, row)
+            box_bytes += int(lens[bs].sum())
+            box_strs += len(bs)
+            r0 += int(row[0])
+        src = box_bytes + 16 * box_strs + sum(8 * int(shapes.reshape(n, -1)[:, 0].sum()) for _ in numeric)
+        wire_bytes = sum(len(w) for w in ref)
+        reps = 5
+        res = {}
+        # the C call, eager and as a replayed graph
+        keep, structs, pins, bts = [], [], [], []
+        for k, t in [(key, None)] + list(num.items()):
+            if t is None:
+                d = (C.c_int64 * len(dims))(*dims)
+                structs.append(N.Tensor(data=data.data_ptr(), src_dtype=7, wire_dtype=7, rank=len(dims), flags=N.F_DEVICE_DATA, dims=d,
+                                        key=k.encode(), key_len=len(k), packed_len=0))
+                bts.append(N.Bytes(offsets=offsets.data_ptr(), data_len=data_h.size, flags=N.F_DEVICE_DATA))
+            else:
+                d = (C.c_int64 * 1)(t.shape[0])
+                structs.append(N.Tensor(data=t.data_ptr(), src_dtype=9, wire_dtype=9, rank=1, flags=N.F_DEVICE_DATA, dims=d, key=k.encode(),
+                                        key_len=len(k), packed_len=0))
+                bts.append(N.Bytes())
+            keep.append(d)
+            pins.append(N.PadInput(shapes=S[k].data_ptr(), cols=S[k].shape[1] if S[k].dim() == 2 else 1))
+        arr = (N.Tensor * len(structs))(*structs)
+        req = N.Request(model_name=b"m", model_name_len=1, has_version=1, order=N.ORDER_UPB, version=1, n_inputs=len(structs), flags=0, inputs=arr)
+        pin_arr, bt_arr = (N.PadInput * len(pins))(*pins), (N.Bytes * len(bts))(*bts)
+        cap = C.c_uint64()
+        N.check(lib.b200tfs_padded_request_columns_arena_size(n, C.byref(req), bt_arr, C.byref(cap)))
+        gc = Codec(0)
+        mem = C.c_void_p()
+        N.check(lib.b200tfs_malloc(gc.ctx, cap.value, C.byref(mem)))
+        arena = mem.value
+        off, ln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
+
+        def wires():
+            N.check(lib.b200tfs_encode_results(gc.ctx, n, off, ln))
+            end = max(int(off[i]) + int(ln[i]) for i in range(n))
+            host = np.empty(end, np.uint8)
+            N.check(lib.b200tfs_memcpy_d2h(gc.ctx, host.ctypes.data, arena, end))
+            gc.sync()
+            return [host[off[i]: off[i] + ln[i]].tobytes() for i in range(n)]
+
+        def eager():
+            N.check(lib.b200tfs_encode_padded_requests_columns_async(gc.ctx, n, C.byref(req), pin_arr, bt_arr, arena, cap.value))
+            gc.sync()
+
+        res["device"], _ = timed(eager, reps)
+        assert wires() == ref, f"{name}: device bytes differ"
+        N.check(lib.b200tfs_capture_begin(gc.ctx))
+        N.check(lib.b200tfs_encode_padded_requests_columns_async(gc.ctx, n, C.byref(req), pin_arr, bt_arr, arena, cap.value))
+        g = C.c_void_p()
+        N.check(lib.b200tfs_capture_end(gc.ctx, C.byref(g)))
+
+        def replay():
+            N.check(lib.b200tfs_graph_launch(gc.ctx, g.value))
+            gc.sync()
+
+        res["graph"], _ = timed(replay, reps)
+        assert wires() == ref, f"{name}: graph replay bytes differ"
+        N.check(lib.b200tfs_graph_destroy(g.value))
+        N.check(lib.b200tfs_free(gc.ctx, arena))
+        gc.close()
+        dt, got = timed(lambda: codec.encode_predict_requests_padded("m", {key: col, **num}, S, model_version=1), reps)
+        assert got == ref, f"{name}: python bytes differ"
+        res["python"] = dt
+        if is_text:     # today's route: a numpy str_ column, sliced and encoded request by request on the host
+            a = np.array([x.decode() for x in strs]).reshape(dims)
+            hs = {k: s.cpu().numpy() for k, s in S.items()}
+            dt, got = timed(lambda: codec._padded_requests_on_host("m", 1, {key: a, **numeric}, hs, {}, n), 1)
+            assert got == ref, f"{name}: today's bytes differ"
+            res["today"] = dt
+        hs = {k: s.cpu().numpy() for k, s in S.items()}
+        dt, got = timed(lambda: SR.reference_requests("m", 1, {key: (strs, dims), **numeric}, hs, {}), 1)
+        assert got == ref
+        res["protobuf"] = dt
+        line = {"workload": name, "n": n, "src_bytes": src, "wire_bytes": wire_bytes}
+        for leg, t in res.items():
+            gbs = (src + wire_bytes) / t / 1e9
+            line[leg] = {"us": round(t * 1e6, 1), "GB/s": round(gbs, 2)}
+        print(json.dumps(line))
+        out["workloads"][name] = line
+        del data, offsets, col, num, S
+        torch.cuda.empty_cache()
+
+
 def main():
     q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     print("card:", q)
@@ -62,7 +188,10 @@ def main():
     lib = N.load()
     rng = np.random.default_rng(0)
     out = {"card": q, "workloads": {}}
-    for name, inputs, shapes, contiguous in workloads(rng):
+    only_strings = "--strings" in sys.argv
+    args = [a for a in sys.argv[1:] if a != "--strings"]
+    run_strings(codec, lib, np.random.default_rng(1), out)
+    for name, inputs, shapes, contiguous in ([] if only_strings else workloads(rng)):
         torch.cuda.synchronize()
         S = {k: torch.from_numpy(shapes[:, :t.dim()] if shapes.ndim == 2 else shapes).cuda().contiguous() for k, t in inputs.items()}
         src = 0
@@ -186,8 +315,8 @@ def main():
         out["workloads"][name] = line
         del inputs, S
         torch.cuda.empty_cache()
-    if len(sys.argv) > 1:      # a JSON copy of the lines
-        with open(sys.argv[1], "w") as f:
+    if args:      # a JSON copy of the lines
+        with open(args[0], "w") as f:
             json.dump(out, f, indent=1)
     codec.close()
 
