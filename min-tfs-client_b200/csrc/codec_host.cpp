@@ -2603,6 +2603,23 @@ int b200tfs_padded_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_ou
 
 }  // extern "C"
 
+// The checks a string column's b200tfs_bytes entry takes in every route that reads one (B200TFS_E_ARG).  `what` and the arguments
+// behind it, a printf format such as "input %d", name the column in the message; they are formatted only for a refusal.
+static int bytes_entry_check(const b200tfs_bytes& b, const void* data, const char* what, ...) {
+  char msg[64];
+  if (b.flags & ~B200TFS_F_DEVICE_DATA) snprintf(msg, sizeof msg, "unknown bytes flags 0x%x", (unsigned)b.flags);
+  else if (b.data_len < 0) snprintf(msg, sizeof msg, "negative data_len %lld", (long long)b.data_len);
+  else if (b.data_len && !data) snprintf(msg, sizeof msg, "data pointer is NULL");
+  else if ((uintptr_t)b.offsets & 7) snprintf(msg, sizeof msg, "string offsets must be 8-byte aligned");
+  else return B200TFS_OK;
+  char name[64];
+  va_list ap;
+  va_start(ap, what);
+  vsnprintf(name, sizeof name, what, ap);
+  va_end(ap);
+  return fail(B200TFS_E_ARG, "%s: %s", name, msg);
+}
+
 // ------------------------------------------------------------------------------------------------
 // varint dtypes (phase 2: kernels in kernels.cu; wired here)
 // ------------------------------------------------------------------------------------------------

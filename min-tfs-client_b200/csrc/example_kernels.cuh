@@ -97,8 +97,6 @@ __device__ __forceinline__ uint64_t ex_str_ends(const ExFeat& f, uint64_t b, uin
   *carry = __shfl_sync(0xFFFFFFFFu, e, 31);
   return e;
 }
-// Strings at most this long are copied by their own lane; a longer one by the whole warp.
-constexpr uint64_t kExWarpCopy = 64;
 // Example i's bytes row at d, its list payload (L) already known: the {0A vi(len) bytes} field of every string.
 __device__ __forceinline__ void ex_write_bytes(const ExFeat& f, uint64_t i, uint64_t ne, uint8_t* d) {
   const uint32_t lane = threadIdx.x & 31;
@@ -110,7 +108,7 @@ __device__ __forceinline__ void ex_write_bytes(const ExFeat& f, uint64_t i, uint
     uint64_t s;
     const uint64_t e = ex_str_ends(f, b, ne, j0, lo, hi, &carry, &s);
     const uint64_t len = j0 + lane < ne ? e - s : 0;
-    const uint64_t sz = j0 + lane < ne ? 1 + varint_len(len) + len : 0;
+    const uint64_t sz = j0 + lane < ne ? string_value_len(len) : 0;
     uint64_t incl = sz;
 #pragma unroll
     for (int dd = 1; dd < 32; dd <<= 1) {
@@ -118,21 +116,8 @@ __device__ __forceinline__ void ex_write_bytes(const ExFeat& f, uint64_t i, uint
       if (lane >= (uint32_t)dd) incl += x;
     }
     uint8_t* h = d + base + incl - sz;
-    const uint8_t* src = f.data + s;
-    if (sz) {
-      *h++ = 0x0A; h += put_varint(h, len);
-      if (len <= kExWarpCopy)
-        for (uint64_t k = 0; k < len; ++k) h[k] = src[k];
-    }
-    uint32_t big = __ballot_sync(0xFFFFFFFFu, len > kExWarpCopy);
-    while (big) {                             // the long strings of this chunk, each by the whole warp
-      const int l = __ffs(big) - 1;
-      big &= big - 1;
-      const uint64_t n = __shfl_sync(0xFFFFFFFFu, len, l);
-      uint8_t* dl = (uint8_t*)__shfl_sync(0xFFFFFFFFu, (unsigned long long)h, l);
-      const uint8_t* sl = (const uint8_t*)__shfl_sync(0xFFFFFFFFu, (unsigned long long)src, l);
-      for (uint64_t k = lane; k < n; k += 32) dl[k] = sl[k];
-    }
+    if (sz) { *h++ = 0x0A; h += put_varint(h, len); }
+    warp_copy_strings(h, f.data + s, len, sz != 0, UINT64_MAX);
     base += __shfl_sync(0xFFFFFFFFu, incl, 31);
   }
 }
@@ -150,7 +135,7 @@ __device__ __forceinline__ uint64_t ex_count_bytes(const ExTables& T, uint32_t r
     const uint64_t e = ex_str_ends(f, b, ne, j0, lo, hi, &carry, &s);
     const uint64_t j = j0 + lane;
     if (j < ne) {
-      sum += 1 + varint_len(e - s) + (e - s);
+      sum += string_value_len(e - s);
       bad |= f.offsets[b + j + 1] < f.offsets[b + j];
     }
   }

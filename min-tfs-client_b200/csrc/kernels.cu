@@ -44,6 +44,7 @@
 #include "framing.h"
 #include "kernels.h"
 #include "plan.h"
+#include "strcol.h"
 #include "string_walk.h"
 #include "tpl.h"
 #include "unpad.h"

@@ -262,7 +262,6 @@ constexpr uint64_t concat_record_tile_bound(uint64_t len, uint64_t tile_bytes, u
 // key's data and numbers the copy chunks (kStrChunk strings each); str_copy_kernel - a lane per short string, the warp for long
 // ones; str_fix_kernel - the offsets' final values, in a launch of its own because the copy reads the entry behind each string.
 constexpr uint32_t kStrChunk = 256;         // strings per copy chunk (eight per lane)
-constexpr uint32_t kStrLaneMax = 64;        // strings up to this many bytes are copied by one lane, longer ones by the warp
 constexpr uint32_t kStrThreads = 256;       // threads per CTA of the index, copy and fix kernels
 struct StrKeyDev { uint8_t* data; uint64_t cap; };
 struct StrTables {

@@ -9,7 +9,8 @@
 //                     writes past the n_strings entries the plan reserved.
 //   str_scan_kernel   one CTA: per key, a block scan of the byte totals gives each pair its first data byte (B200TFS_E_SIZE past
 //                     data_cap) and the chunks of kStrChunk strings their numbers; offsets[m] behind the key's last OK pair
-//   str_copy_kernel   a warp per chunk, striding: a lane per string of at most kStrLaneMax bytes, the warp for longer ones
+//   str_copy_kernel   a warp per chunk, striding: a lane per string of at most kStrLaneCopy bytes, the warp for longer ones
+//                     (warp_copy_strings, strcol.h)
 //   str_fix_kernel    the same chunks: every entry becomes its string's first byte in the key's data.  Separate from the copy,
 //                     which reads the entry behind each string for its length.
 
@@ -117,19 +118,7 @@ __global__ void __launch_bounds__(kStrThreads) str_copy_kernel(const __grid_cons
         pos = (uint32_t)e;
         len = (j + 1 < cnt ? (uint32_t)slot[j + 1] : end) - pos;
       }
-      const bool mine = len <= kStrLaneMax;
-      if (mine)
-#pragma unroll 1
-        for (uint32_t b = 0; b < len; ++b) dst[pos + b] = rec[src + b];
-      uint32_t longs = __ballot_sync(0xFFFFFFFFu, !mine);
-#pragma unroll 1
-      while (longs) {
-        const int l = __ffs(longs) - 1;
-        longs &= longs - 1;
-        const uint32_t s = __shfl_sync(0xFFFFFFFFu, src, l), at = __shfl_sync(0xFFFFFFFFu, pos, l), m = __shfl_sync(0xFFFFFFFFu, len, l);
-#pragma unroll 4
-        for (uint32_t b = lane; b < m; b += 32) dst[at + b] = rec[s + b];
-      }
+      warp_copy_strings(dst + pos, rec + src, len, j < cnt, UINT64_MAX);
     }
   }
 }

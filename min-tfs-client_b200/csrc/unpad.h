@@ -116,8 +116,6 @@ B2_HD void unpad_str_rows(const UnpadIn& in, const UnpadBox& b, uint64_t* first,
   *first = in.shapes ? b.src_off : 0;
   *end = in.shapes ? b.src_off + (uint64_t)b.dims[0] * w : b.n_elems;
 }
-// wire bytes of one string_val value of `len` bytes: 42 vi(len) bytes
-B2_HD uint64_t unpad_str_wire(uint64_t len) { return 1 + varint_len(len) + len; }
 
 struct UnpadFrame {                // what every request's framing has in common
   const uint8_t* blob;             // model_spec field (its tag included) at 0, then the keys

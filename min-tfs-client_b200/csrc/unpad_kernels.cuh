@@ -354,7 +354,7 @@ __global__ void __launch_bounds__(kVarThreads) unpad_str_count_kernel(const __gr
     const uint64_t before = unpad_str_off(col, e ? unpad_str_index(in, b, e - 1) + 1 : first, &ok);
     if (before > s0) ok = false;
     if (e + 1 == jb.n_elems && s0 + len > unpad_str_off(col, end, &ok)) ok = false;
-    size = unpad_str_wire(len);
+    size = string_value_len(len);
   }
   if (t_rel == 0 && threadIdx.x == 0 && unpad_str_off(col, first, &ok) > unpad_str_off(col, end, &ok)) ok = false;   // empty boxes too
   uint32_t unused;
@@ -367,21 +367,8 @@ __global__ void __launch_bounds__(kVarThreads) unpad_str_count_kernel(const __gr
   }
 }
 
-// Strings at most this long are copied by their own thread, up to kUnpadStrBlockCopy by their warp, longer ones by the CTA.
-constexpr uint64_t kUnpadStrLaneCopy = 64;
+// Strings up to kStrLaneCopy bytes are copied by their own thread, up to kUnpadStrBlockCopy by their warp, longer ones by the CTA.
 constexpr uint64_t kUnpadStrBlockCopy = 16384;
-
-// bytes [0, m) of src to dst by `n` threads (this one is `i`), 16 bytes per thread and step
-__device__ __forceinline__ void unpad_copy(uint8_t* dst, const uint8_t* src, uint64_t m, uint32_t i, uint32_t n) {
-#pragma unroll 1
-  for (uint64_t a = (uint64_t)i * 16; a < m; a += (uint64_t)n * 16) {
-    uint8_t v[16];
-#pragma unroll
-    for (int k = 0; k < 16; ++k) v[k] = a + k < m ? __ldg(src + a + k) : 0;
-#pragma unroll
-    for (int k = 0; k < 16; ++k) if (a + k < m) dst[a + k] = v[k];
-  }
-}
 
 __global__ void __launch_bounds__(kVarThreads) unpad_str_emit_kernel(const __grid_constant__ UnpadPlan up) {
   __shared__ VarShared sh;
@@ -394,13 +381,13 @@ __global__ void __launch_bounds__(kVarThreads) unpad_str_emit_kernel(const __gri
   uint32_t r;
   if (!unpad_str_fetch(up, blockIdx.x, jb, in, col, b, r)) return;   // the layout kernel's final statuses: a bad request writes nothing
   if (threadIdx.x == 0) n_long = 0;
-  const uint32_t lane = threadIdx.x & 31, t_rel = blockIdx.x - jb.first_tile;
+  const uint32_t t_rel = blockIdx.x - jb.first_tile;
   const uint64_t e = (uint64_t)t_rel * kVarThreads + threadIdx.x;
   bool ok = true;
   uint64_t s0 = 0, len = 0, size = 0;
   if (e < jb.n_elems) {
     len = unpad_str_span(in, col, b, e, &s0, &ok);   // the lengths the count read
-    size = unpad_str_wire(len);
+    size = string_value_len(len);
   }
   uint32_t tile_total;
   uint64_t base;
@@ -412,19 +399,8 @@ __global__ void __launch_bounds__(kVarThreads) unpad_str_emit_kernel(const __gri
     o.byte(0x42);
     o.varint(len);
     d = o.w;
-    if (len <= kUnpadStrLaneCopy)
-      for (uint64_t k = 0; k < len; ++k) d[k] = in.src[s0 + k];
   }
-  const bool warp_copy = mine && len > kUnpadStrLaneCopy && len <= kUnpadStrBlockCopy;
-  uint32_t longs = __ballot_sync(0xFFFFFFFFu, warp_copy);
-#pragma unroll 1
-  while (longs) {
-    const int l = __ffs(longs) - 1;
-    longs &= longs - 1;
-    const uint8_t* src = in.src + __shfl_sync(0xFFFFFFFFu, s0, l);
-    uint8_t* dst = (uint8_t*)__shfl_sync(0xFFFFFFFFu, (unsigned long long)(uintptr_t)d, l);
-    unpad_copy(dst, src, __shfl_sync(0xFFFFFFFFu, len, l), lane, 32);
-  }
+  warp_copy_strings(d, in.src + s0, len, mine, kUnpadStrBlockCopy);
   if (mine && len > kUnpadStrBlockCopy) {
     const uint32_t q = atomicAdd(&n_long, 1u);
     long_src[q] = s0; long_dst[q] = (uint64_t)(uintptr_t)d; long_len[q] = len;
@@ -432,7 +408,7 @@ __global__ void __launch_bounds__(kVarThreads) unpad_str_emit_kernel(const __gri
   __syncthreads();
 #pragma unroll 1
   for (uint32_t q = 0; q < n_long; ++q)
-    unpad_copy((uint8_t*)(uintptr_t)long_dst[q], in.src + long_src[q], long_len[q], threadIdx.x, kVarThreads);
+    copy_bytes((uint8_t*)(uintptr_t)long_dst[q], in.src + long_src[q], long_len[q], threadIdx.x, kVarThreads);
 }
 
 cudaError_t launch_unpad(const UnpadPlan& up, uint32_t move_grid, cudaStream_t stream, uint32_t* launched) {

@@ -292,6 +292,25 @@ class BytesColumn:
         d = np.asarray(self.data)
         return [d[o[j]: o[j + 1]].tobytes() for j in range(len(o) - 1)]
 
+    def _bind(self, keep: list, upload=None):
+        """(data pointer, or None when ``data_len`` is 0; the ``N.Bytes`` entry of the offsets) for the C ABI.  Every array the two
+        point at is appended to ``keep``.  With ``upload`` (a Codec), host arrays are first copied to its device."""
+        def ptr(a, on_device, dtype):
+            if on_device:
+                p, _, _, hold = D.device_view(a)
+            elif upload is not None:
+                hold = upload.device_array(np.ascontiguousarray(a, dtype=dtype))
+                p = hold.ptr
+            else:
+                hold, p = a, a.ctypes.data
+            keep.append(hold)
+            return p
+
+        data = ptr(self.data, self.data_on_device, np.uint8) if self.data_len else None
+        offsets = ptr(self.offsets, self.offsets_on_device, np.int64)
+        flags = N.F_DEVICE_DATA if self.offsets_on_device or upload is not None else 0
+        return data, N.Bytes(offsets=offsets, data_len=self.data_len, flags=flags)
+
 
 class RaggedColumn:
     """A variable-length tf.Example column - what a model parses as ``VarLenFeature`` / ``RaggedFeature``: a click history, the
@@ -385,21 +404,9 @@ def _example_columns(input_dict: Mapping):
             flags |= N.F_DEVICE_DATA
         b = None
         if isinstance(hold, BytesColumn):
-            col = hold
-            if col.data_on_device:
-                ptr, _, _, dhold = D.device_view(col.data)
-            else:
-                dhold = col.data
-                ptr = dhold.ctypes.data
-            if col.offsets_on_device:
-                optr, _, _, ohold = D.device_view(col.offsets)
-            else:
-                ohold = col.offsets
-                optr = ohold.ctypes.data
-            b = N.Bytes(offsets=optr, data_len=col.data_len, flags=N.F_DEVICE_DATA if col.offsets_on_device else 0)
-            f = N.Feature(data=ptr if col.data_len else None, src_dtype=DT_STRING, flags=flags, row_elems=row_elems, key=key,
-                          key_len=len(key))
-            hold = (dhold, ohold)
+            col, hold = hold, []
+            ptr, b = col._bind(hold)
+            f = N.Feature(data=ptr, src_dtype=DT_STRING, flags=flags, row_elems=row_elems, key=key, key_len=len(key))
         else:
             if not on_device:
                 hold = np.require(hold.astype(dtype, copy=False), requirements="CA")
@@ -925,21 +932,11 @@ class Codec:
     def _padded_string_input(self, col: "BytesColumn", key: bytes, keep: list):
         """(_Prepared-like holder of the DT_STRING Tensor, Bytes entry) of a string column of the padded encode; host arrays are
         copied to the device (the kernels read both there)."""
-        def on_device(a, on_dev, dtype):
-            if on_dev:
-                ptr, _, _, hold = D.device_view(a)
-                keep.append(hold)
-                return ptr
-            d = self.device_array(np.ascontiguousarray(a, dtype=dtype))
-            keep.append(d)
-            return d.ptr
-
-        data = on_device(col.data, col.data_on_device, np.uint8) if col.data_len else None
-        offsets = on_device(col.offsets, col.offsets_on_device, np.int64)
+        data, b = col._bind(keep, upload=self)
         p = _PaddedString(key, col.shape)
         p.struct = N.Tensor(data=data, src_dtype=DT_STRING, wire_dtype=DT_STRING, rank=len(col.shape), flags=N.F_DEVICE_DATA,
                             dims=p.dims, key=key, key_len=len(key), packed_len=0)
-        return p, N.Bytes(offsets=offsets, data_len=col.data_len, flags=N.F_DEVICE_DATA)
+        return p, b
 
     def _to_host(self, v) -> np.ndarray:
         if isinstance(v, BytesColumn):

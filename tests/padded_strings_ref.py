@@ -58,20 +58,6 @@ def box_strings(strings, dims, r0, row):
     return [strings[i] for i in idx.ravel().tolist()], bd
 
 
-def string_payload(strings) -> bytes:
-    """The string_val values on the wire: 42 vi(len) bytes per string."""
-    out = bytearray()
-    for s in strings:
-        out.append(0x42)
-        n = len(s)
-        while n >= 0x80:
-            out.append((n & 0x7F) | 0x80)
-            n >>= 7
-        out.append(n)
-        out += s
-    return bytes(out)
-
-
 def reference_requests(name, version, padded: dict, shapes: dict, broadcast: dict, order="deterministic", grpc=False):
     """Every request's wire.  padded / broadcast values: numpy arrays, or (strings, dims) of a string column; shapes: int[n, m] or
     int[n] per padded key."""

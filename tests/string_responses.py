@@ -1,5 +1,6 @@
 """PredictResponses with DT_STRING outputs, and the definition of their concatenated byte column, for the string decode tests
-(tests/test_concat_strings_cpu.py, tests/test_concat_strings_gpu.py).
+(tests/test_concat_strings_cpu.py, tests/test_concat_strings_gpu.py); strings_body is also the string_val payload the padded encode
+tests expect (tests/test_padded_strings_cpu.py).
 
 The definition: for a requested key, record r contributes S_r = list(PredictResponse.FromString(w_r).outputs[key].string_val)
 (raw bytes) of shape dims_r (one -1 inferred); the column has shape (sum_r dims_r[0], *dims[1:]), int64 offsets[m + 1] from 0 and
@@ -16,6 +17,7 @@ DT_FLOAT, DT_STRING, DT_INT64 = 1, 7, 9
 
 
 def strings_body(strs: Sequence[bytes]) -> bytes:
+    """The string_val values on the wire: 42 vi(len) bytes per string."""
     return b"".join(G.ld(0x42, s) for s in strs)
 
 

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 import padded_strings_ref as R
+import string_responses as SR
 from min_tfs_client import _native as N
 from tensorflow.core.framework import types_pb2
 
@@ -88,7 +89,7 @@ def _check(padded, rows, broadcast, order="deterministic", grpc=False, version=3
         v = padded[k] if k in padded else broadcast[k]
         if isinstance(v, tuple):
             strs = R.box_strings(v[2], v[3], 0, rows[k])[0] if k in padded else v[2]
-            payloads[k] = R.string_payload(strs)
+            payloads[k] = SR.strings_body(strs)
             packed.append(len(payloads[k]))
         else:
             box = v[(slice(0, int(rows[k][0])),) + tuple(slice(0, int(x)) for x in rows[k][1:])] if k in padded else v
