@@ -518,7 +518,9 @@ typedef struct b200tfs_pad_key {
                              records' trailing dims.  In (b200tfs_decode_padded*): dims[1..rank) are the destination's trailing
                              dims (a caller that captures a graph fixes them once, e.g. at the model's longest sequence)     */
   uint64_t bytes;         /* out: rows * prod(dims[1..rank)) * element size in memory (2 for float32 with a cast)              */
-  int32_t status;         /* out: as b200tfs_concat_key.status, except that other trailing dims are not an error              */
+  int32_t status;         /* out: as b200tfs_concat_key.status, except that other trailing dims are not an error (a DT_STRING
+                             key: OK with bytes 0, decoded on the host - or, with b200tfs_padded_strings entries, bytes of
+                             its int64 offsets)                                                                              */
   int32_t bad_rec;        /* out: the record `status` is about (-1 when OK)                                                  */
   uint8_t pad_bits[16];   /* in: the pad element's bit pattern in the destination dtype (little-endian; the first element
                              size bytes are used)                                                                            */
@@ -549,6 +551,48 @@ int b200tfs_decode_padded_host_async(b200tfs_ctx* ctx, const void* wire_host, in
  * as b200tfs_parse_responses gives them; any pointer may be NULL.                                                               */
 int b200tfs_padded_results(b200tfs_ctx* ctx, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs,
                            int32_t* rec_status);
+
+/* DT_STRING outputs of the same decode, as one padded offset-indexed byte column per key (the b200tfs_bytes layout): for a key whose
+ * outputs are DT_STRING, position (row, i_1, ..., i_{rank-1}) of the [rows, dims[1], ..., dims[rank-1]] destination holds, in C
+ * order, record r's string at (row - first_row, i_1, ...) when every index lies inside its own dims, and the pad string otherwise
+ * (raw bytes; no UTF-8 check).  With m = rows * prod(dims[1..rank)) positions, keys[k].dst receives int64 offsets[m + 1]
+ * (offsets[0] = 0, position p is data[offsets[p], offsets[p + 1])) and the entry's `data` the bytes, so that
+ * b200tfs_output.dst_off keeps its meaning: the byte offset of the record's first row, 8 bytes per position.  One entry per key,
+ * parallel to keys; entries of keys whose outputs are not DT_STRING are ignored, and so are those keys' pad_bits.              */
+typedef struct b200tfs_padded_strings {
+  void* data;             /* in: device destination of the key's string bytes                                                  */
+  uint64_t data_cap;      /* in: its capacity in bytes - nothing is ever stored at or past data + data_cap                     */
+  const void* pad;        /* in: the pad string's bytes in host memory (copied inside the call; NULL when pad_len is 0)        */
+  uint64_t pad_len;       /* in: its length                                                                                    */
+  uint64_t strings;       /* out (b200tfs_padded_strings_layout): the records' own strings together                            */
+  uint64_t data_bytes;    /* out: their bytes                                                                                  */
+} b200tfs_padded_strings;
+/* b200tfs_padded_layout with entries (strings == NULL: that call itself).  A DT_STRING key that lays out gets `strings` and
+ * `data_bytes`, and keys[k].bytes = 8 * (m + 1), the offsets' size, with m = dims[0] * prod(dims[1..rank)) of the elementwise
+ * maximum.  Its column then takes data_bytes + (m - strings) * pad_len data bytes; with other trailing dims D (pad_to), m is
+ * dims[0] * prod(D).  A record whose string_val elements the device walk does not find in its last `value` occurrence is
+ * B200TFS_E_NONCANONICAL, as for b200tfs_concat_strings_layout.  For a caller that captures a graph once with trailing dims D and
+ * at most R rows: offsets of 8 * (R * prod(D) + 1) bytes and max_data_bytes + R * prod(D) * pad_len data bytes hold any records
+ * of the same lengths (max_data_bytes from b200tfs_concat_strings_bound).                                                     */
+int b200tfs_padded_strings_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
+                                  b200tfs_pad_key* keys, b200tfs_padded_strings* strings, int32_t cast);
+/* b200tfs_decode_padded with entries (strings == NULL: that call itself).  Still asynchronous and CUDA-graph capturable with no host
+ * step between the launches: the plan places every (record, string key)'s rows as for a numeric key, then four kernels (index: a
+ * warp per pair walks its string_val elements and notes each at its padded position; scan: one CTA places every record's bytes,
+ * its own and its pads'; copy: strings and pads, destination-major; fix: the final offsets of the own strings) come ahead of the
+ * varint tail - b200tfs_kernel_launches counts ten.  The scratch is sized from n, n_keys and rec_len alone: a replay over new
+ * records of the same lengths re-plans rows, string counts and bytes.  b200tfs_padded_results reports each (record, string key):
+ * B200TFS_OK with dst_off / dst_bytes of its rows; B200TFS_E_SIZE when its rows would end past dst_cap (the entry behind them
+ * included), its bytes past data_cap, or a trailing dim exceeds the destination's - it gets no place, and the rows in use end at
+ * the first record that ends B200TFS_E_SIZE for its bytes; or B200TFS_E_NONCANONICAL when its string_val elements do not all lie
+ * in its last `value` occurrence (its rows then hold the pad string: decode that batch on the host).  Stores: with rows_used the
+ * rows in use, every offset entry of [0, rows_used * prod(dims[1..rank))] and every data byte of those rows, each once; the
+ * entries of a record that ends B200TFS_E_SIZE for its bytes may hold scratch values.  Nothing at or past dst_cap or data_cap. */
+int b200tfs_decode_padded_strings(b200tfs_ctx* ctx, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                                  int32_t n_keys, const b200tfs_pad_key* keys, const b200tfs_padded_strings* strings);
+int b200tfs_decode_padded_strings_host_async(b200tfs_ctx* ctx, const void* wire_host, int32_t n, const uint64_t* rec_off,
+                                             const uint64_t* rec_len, int32_t n_keys, const b200tfs_pad_key* keys,
+                                             const b200tfs_padded_strings* strings);
 
 /* ---- batch encode of PredictRequests cut out of one padded tensor per input ------------------------
  * The inverse of b200tfs_decode_padded: request r's tensor for a padded input P of shape [R, D_1, ..., D_{m-1}] is the box

@@ -2287,6 +2287,21 @@ struct StrTally {
   uint64_t bytes = 0;
   void operator()(uint64_t, uint32_t, uint32_t len) { bytes += len; }
 };
+
+// the walk of the index kernels over DT_STRING output o of a record: the strings of the entry's last `value` occurrence, added to
+// *strings and *bytes, or B200TFS_E_NONCANONICAL when that is not all of them
+int32_t tally_strings(const uint8_t* rec, uint64_t len, const b200tfs_output& o, uint64_t* strings, uint64_t* bytes) {
+  Cursor c;
+  cur_open_host(c, rec, (uint32_t)len);
+  c.p = (uint32_t)o.msg_off;
+  c.end = (uint32_t)(o.msg_off + o.msg_len);
+  StrTally t;
+  const uint64_t found = walk_strings(c, t);
+  if (c.err || found != o.n_strings) return B200TFS_E_NONCANONICAL;
+  *strings += found;
+  *bytes += t.bytes;
+  return B200TFS_OK;
+}
 }  // namespace
 
 int b200tfs_concat_strings_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
@@ -2296,17 +2311,7 @@ int b200tfs_concat_strings_layout(const void* wire_host, int32_t n, const uint64
   const int rc = key_layout(wire_host, n, rec_off, rec_len, n_keys, keys, cast, false,
                             [&](int k, const uint8_t* rec, uint64_t len, const b200tfs_output& o) -> int32_t {
                               if (!strings || dtype_info(o.dtype).kind != VK_STRING) return B200TFS_OK;
-                              // the walk of str_index_kernel: the strings of the entry's last `value` occurrence
-                              Cursor c;
-                              cur_open_host(c, rec, (uint32_t)len);
-                              c.p = (uint32_t)o.msg_off;
-                              c.end = (uint32_t)(o.msg_off + o.msg_len);
-                              StrTally t;
-                              const uint64_t found = walk_strings(c, t);
-                              if (c.err || found != o.n_strings) return B200TFS_E_NONCANONICAL;
-                              strings[k].strings += found;
-                              strings[k].data_bytes += t.bytes;
-                              return B200TFS_OK;
+                              return tally_strings(rec, len, o, &strings[k].strings, &strings[k].data_bytes);
                             });
   if (rc || !strings) return rc;
   for (int k = 0; k < n_keys; ++k) {
@@ -2327,15 +2332,37 @@ int b200tfs_concat_strings_bound(int32_t n, const uint64_t* rec_len, uint64_t* m
 
 int b200tfs_padded_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
                           b200tfs_pad_key* keys, int32_t cast) {
-  return key_layout(wire_host, n, rec_off, rec_len, n_keys, keys, cast, true,
-                    [](int, const uint8_t*, uint64_t, const b200tfs_output&) -> int32_t { return B200TFS_OK; });
+  return b200tfs_padded_strings_layout(wire_host, n, rec_off, rec_len, n_keys, keys, nullptr, cast);
+}
+
+int b200tfs_padded_strings_layout(const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len, int32_t n_keys,
+                                  b200tfs_pad_key* keys, b200tfs_padded_strings* strings, int32_t cast) {
+  if (strings && n_keys > 0 && n_keys <= B200TFS_CONCAT_MAX_KEYS)
+    for (int k = 0; k < n_keys; ++k) strings[k].strings = strings[k].data_bytes = 0;
+  const int rc = key_layout(wire_host, n, rec_off, rec_len, n_keys, keys, cast, true,
+                            [&](int k, const uint8_t* rec, uint64_t len, const b200tfs_output& o) -> int32_t {
+                              if (!strings || dtype_info(o.dtype).kind != VK_STRING) return B200TFS_OK;
+                              return tally_strings(rec, len, o, &strings[k].strings, &strings[k].data_bytes);
+                            });
+  if (rc || !strings) return rc;
+  for (int k = 0; k < n_keys; ++k) {
+    b200tfs_pad_key& K = keys[k];
+    if (K.status == B200TFS_OK && dtype_info(K.dtype).kind == VK_STRING) {
+      uint64_t m = (uint64_t)K.dims[0];
+      for (int d = 1; d < K.rank; ++d) m *= (uint64_t)K.dims[d];
+      K.bytes = 8 * (m + 1);
+    } else {
+      strings[k].strings = strings[k].data_bytes = 0;
+    }
+  }
+  return B200TFS_OK;
 }
 
 namespace {
 // device scratch of a per-key decode (b200tfs_decode_concat, b200tfs_decode_padded) for n records, n_keys keys and var_tile_cap
 // varint tiles: the parse table, the keys' verdicts and matches, the varint tail's table and scratch, then the route's own
 // regions of `sizes` bytes (own[i])
-struct KeyLayout { uint64_t outs, nouts, specs, status, spill, kst, match, vouts, vnouts, vstatus, var, var_status, own[3], bytes; };
+struct KeyLayout { uint64_t outs, nouts, specs, status, spill, kst, match, vouts, vnouts, vstatus, var, var_status, own[4], bytes; };
 KeyLayout key_scratch(uint64_t n, uint64_t n_keys, uint64_t var_tile_cap, std::initializer_list<uint64_t> sizes) {
   const VarPlanLayout V = var_plan_layout(n, var_tile_cap);
   Layout R;
@@ -2385,17 +2412,21 @@ static int key_begin(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uin
 // ConcatPlan fields both routes use.  `plan(cp, scratch, layout, device key records, device rec_len, &pad)` launches the route's kernels, which
 // write the single-launch decode's table with absolute dst_off, and may set `pad`, the placement of the varint emit.  Then the
 // varint tail over that table, and `res` becomes this call's.
+// `extra`: n_extra more host byte ranges (the padded string decode's pad strings), uploaded behind the key bytes; extra[i].dev
+// receives where range i lies on the device before `plan` runs.
+struct HostBytes { const void* p; uint64_t len; const uint8_t* dev; };
 template <class Key, class DevKey, class Plan>
 static int key_decode(b200tfs_ctx* c, Growable& g, b200tfs_ctx::KeyResults& res, const void* arena_dev, int32_t n, const uint64_t* rec_off,
                       const uint64_t* rec_len, int32_t n_keys, const Key* keys, uint64_t var_tile_cap, std::initializer_list<uint64_t> own,
-                      DevKey&& dev_key, Plan&& plan) {
+                      DevKey&& dev_key, Plan&& plan, HostBytes* extra = nullptr, int n_extra = 0) {
   using KeyRec = decltype(dev_key(keys[0], (const uint8_t*)nullptr));
   const KeyLayout L = key_scratch((uint64_t)n, (uint64_t)n_keys, var_tile_cap, own);
   int rc = grow_dev(c, g, L.bytes);
   if (rc) return rc;
-  // rec_off | rec_len | keys | key bytes: one upload (a captured call keeps a private copy)
+  // rec_off | rec_len | keys | key bytes | extra: one upload (a captured call keeps a private copy)
   uint64_t key_bytes = 0;
   for (int k = 0; k < n_keys; ++k) key_bytes += (uint64_t)keys[k].key_len;
+  for (int i = 0; i < n_extra; ++i) key_bytes += extra[i].len;
   Layout K;
   const uint64_t o_off = K.take(8ull * n), o_len = K.take(8ull * n), o_keys = K.take(sizeof(KeyRec) * n_keys), o_kb = K.take(key_bytes);
   Slot* slot;
@@ -2407,6 +2438,11 @@ static int key_decode(b200tfs_ctx* c, Growable& g, b200tfs_ctx::KeyResults& res,
       memcpy(h + o_keys + sizeof(KeyRec) * k, &kd, sizeof kd);
       if (keys[k].key_len) memcpy(h + at, keys[k].key, (size_t)keys[k].key_len);
       at += (uint64_t)keys[k].key_len;
+    }
+    for (int i = 0; i < n_extra; ++i) {
+      if (extra[i].len) memcpy(h + at, extra[i].p, (size_t)extra[i].len);
+      extra[i].dev = dev + at;
+      at += extra[i].len;
     }
   });
   if (rc) return rc;
@@ -2552,8 +2588,16 @@ int b200tfs_concat_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_ou
 // ------------------------------------------------------------------------------------------------
 int b200tfs_decode_padded(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
                           int32_t n_keys, const b200tfs_pad_key* keys) {
-  uint64_t var_tile_cap = 0, chunk_bound = 0;
+  return b200tfs_decode_padded_strings(c, arena_dev, n, rec_off, rec_len, n_keys, keys, nullptr);
+}
+
+int b200tfs_decode_padded_strings(b200tfs_ctx* c, const void* arena_dev, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                                  int32_t n_keys, const b200tfs_pad_key* keys, const b200tfs_padded_strings* strings) {
+  uint64_t var_tile_cap = 0, chunk_bound = 0, pos_bound = 0;
   int rc = key_begin(c, arena_dev, n, rec_off, rec_len, n_keys, keys, &var_tile_cap, [&](const b200tfs_pad_key& K, int k) -> int {
+    if (strings && strings[k].data_cap && !strings[k].data) return fail(B200TFS_E_ARG, "key %d: string data is NULL", k);
+    if (strings && strings[k].pad_len && !strings[k].pad) return fail(B200TFS_E_ARG, "key %d: pad string is NULL", k);
+    pos_bound += K.dst_cap / 8;
     if ((uintptr_t)K.dst & 15) return fail(B200TFS_E_ARG, "key %d: dst is not 16-byte aligned", k);
     if (K.rank < 1 || K.rank > B200TFS_MAX_RANK) return fail(B200TFS_E_ARG, "key %d: rank %d", k, K.rank);
     uint64_t row = 1;
@@ -2567,33 +2611,60 @@ int b200tfs_decode_padded(b200tfs_ctx* c, const void* arena_dev, int32_t n, cons
   if (rc) return rc;
   const uint64_t pairs = (uint64_t)n * (uint64_t)n_keys;
   VarPadMap pm{};
+  HostBytes pads[B200TFS_CONCAT_MAX_KEYS];   // the pad strings, uploaded with the keys
+  for (int k = 0; strings && k < n_keys; ++k) pads[k] = HostBytes{strings[k].pad, strings[k].pad_len, nullptr};
+  const auto plan = [&](ConcatPlan& cp, uint8_t* d, const KeyLayout& L, const uint8_t* kd, const uint64_t* len_dev, const VarPadMap** pad) -> int {
+    PaddedPlan pp{};
+    pp.cp = cp;
+    pp.keys = (const PadKeyDev*)kd;
+    pp.desc = (PadDesc*)(d + L.own[0]); pp.first_row = (uint64_t*)(d + L.own[1]); pp.kout = (PadKeyOut*)(d + L.own[2]);
+    const uint32_t emit_grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(chunk_bound, (uint64_t)c->sm_count * 8));
+    CU(launch_padded(pp, emit_grid, c->stream, strings != nullptr));
+    // the varint emit stores every element at its padded position
+    pm = VarPadMap{pp.desc, pp.keys, (uint32_t)n_keys, 0u};
+    *pad = &pm;
+    if (!strings) return B200TFS_OK;
+    PadStrTables T{};
+    T.pp = pp;
+    T.rec_len = len_dev;
+    for (int k = 0; k < n_keys; ++k) T.keys[k] = PadStrKeyDev{(uint8_t*)strings[k].data, strings[k].data_cap, pads[k].dev, pads[k].len};
+    T.bytes = (uint64_t*)(d + L.own[3]); T.data0 = T.bytes + pairs; T.pos0 = T.data0 + pairs;
+    const uint64_t grid = std::min<uint64_t>((pos_bound + kStrThreads - 1) / kStrThreads, (uint64_t)c->sm_count * 8);
+    CU(launch_padded_strings(T, (uint32_t)grid, c->stream));
+    c->launches += 4;
+    return B200TFS_OK;
+  };
+  const auto dev_key = [](const b200tfs_pad_key& k, const uint8_t* kb) {
+    PadKeyDev kd{};
+    kd.k = ConcatKeyDev{kb, (uint8_t*)k.dst, k.dst_cap, (uint32_t)k.key_len, 0u};
+    for (int d = 0; d < B200TFS_MAX_RANK; ++d) kd.dims[d] = k.dims[d];
+    memcpy(kd.pad, k.pad_bits, 16);
+    kd.rank = k.rank;
+    return kd;
+  };
+  if (strings)   // the string pairs' scratch: bytes | data0 (n_keys * n each) | pos0 (n_keys + 1)
+    return key_decode(c, c->padded_dev, c->padded_res, arena_dev, n, rec_off, rec_len, n_keys, keys, var_tile_cap,
+                      {sizeof(PadDesc) * pairs, 8 * pairs, sizeof(PadKeyOut) * (n_keys + 1), 16 * pairs + 8ull * (n_keys + 1)}, dev_key, plan,
+                      pads, n_keys);
   return key_decode(c, c->padded_dev, c->padded_res, arena_dev, n, rec_off, rec_len, n_keys, keys, var_tile_cap,
-                    {sizeof(PadDesc) * pairs, 8 * pairs, sizeof(PadKeyOut) * (n_keys + 1)},
-                    [](const b200tfs_pad_key& k, const uint8_t* kb) {
-                      PadKeyDev kd{};
-                      kd.k = ConcatKeyDev{kb, (uint8_t*)k.dst, k.dst_cap, (uint32_t)k.key_len, 0u};
-                      for (int d = 0; d < B200TFS_MAX_RANK; ++d) kd.dims[d] = k.dims[d];
-                      memcpy(kd.pad, k.pad_bits, 16);
-                      kd.rank = k.rank;
-                      return kd;
-                    },
-                    [&](ConcatPlan& cp, uint8_t* d, const KeyLayout& L, const uint8_t* kd, const uint64_t*, const VarPadMap** pad) -> int {
-                      PaddedPlan pp{};
-                      pp.cp = cp;
-                      pp.keys = (const PadKeyDev*)kd;
-                      pp.desc = (PadDesc*)(d + L.own[0]); pp.first_row = (uint64_t*)(d + L.own[1]); pp.kout = (PadKeyOut*)(d + L.own[2]);
-                      const uint32_t emit_grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(chunk_bound, (uint64_t)c->sm_count * 8));
-                      CU(launch_padded(pp, emit_grid, c->stream));
-                      // the varint emit stores every element at its padded position
-                      pm = VarPadMap{pp.desc, pp.keys, (uint32_t)n_keys, 0u};
-                      *pad = &pm;
-                      return B200TFS_OK;
-                    });
+                    {sizeof(PadDesc) * pairs, 8 * pairs, sizeof(PadKeyOut) * (n_keys + 1)}, dev_key, plan);
 }
 
 int b200tfs_decode_padded_host_async(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
                                      int32_t n_keys, const b200tfs_pad_key* keys) {
   return key_decode_host_async(c, wire_host, n, rec_off, rec_len, n_keys, keys, "b200tfs_decode_padded", b200tfs_decode_padded);
+}
+
+int b200tfs_decode_padded_strings_host_async(b200tfs_ctx* c, const void* wire_host, int32_t n, const uint64_t* rec_off,
+                                             const uint64_t* rec_len, int32_t n_keys, const b200tfs_pad_key* keys,
+                                             const b200tfs_padded_strings* strings) {
+  if (!c || n <= 0 || !wire_host || !rec_off || !rec_len) return fail(B200TFS_E_ARG, "bad arguments");
+  if (c->capturing) return fail(B200TFS_E_ARG, "capture b200tfs_decode_padded_strings over a device arena instead");
+  CU(cudaSetDevice(c->device));
+  uint64_t span;
+  int rc = stage_wire(c, wire_host, n, rec_off, rec_len, &span);
+  if (rc) return rc;
+  return b200tfs_decode_padded_strings(c, c->stage_dev.p, n, rec_off, rec_len, n_keys, keys, strings);
 }
 
 int b200tfs_padded_results(b200tfs_ctx* c, int32_t n, int32_t n_keys, b200tfs_output* outs, b200tfs_model_spec* specs, int32_t* rec_status) {

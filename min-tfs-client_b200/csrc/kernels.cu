@@ -1211,7 +1211,8 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_strings_kernel
 #include "string_kernels.cuh"
 
 // ------------------------------------------------------------------------------------------------
-// decode into one padded tensor per key: padded_plan_kernel / padded_emit_kernel
+// decode into one padded tensor per key: padded_plan_kernel / padded_emit_kernel, and for DT_STRING keys pad_str_index /
+// pad_str_scan / pad_str_copy / pad_str_fix
 // ------------------------------------------------------------------------------------------------
 #include "padded_kernels.cuh"
 
@@ -1409,8 +1410,9 @@ cudaError_t launch_vdec_dev(const VarTables& tb, uint32_t max_ctas, cudaStream_t
   return cudaGetLastError();
 }
 
-cudaError_t launch_padded(const PaddedPlan& pp, uint32_t emit_grid, cudaStream_t stream) {
-  padded_plan_kernel<<<1, kConcatPlanThreads, 0, stream>>>(pp);
+cudaError_t launch_padded(const PaddedPlan& pp, uint32_t emit_grid, cudaStream_t stream, bool strings) {
+  if (strings) padded_plan_strings_kernel<<<1, kConcatPlanThreads, 0, stream>>>(pp);
+  else padded_plan_kernel<<<1, kConcatPlanThreads, 0, stream>>>(pp);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
   padded_emit_kernel<<<std::max(1u, emit_grid), kPadEmitThreads, 0, stream>>>(pp);

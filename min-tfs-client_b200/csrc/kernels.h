@@ -52,7 +52,11 @@ cudaError_t launch_concat_plan(const ConcatPlan& cp, uint32_t move_grid, cudaStr
 // per (record, key), copy and fix run grid CTAs striding over the chunks
 cudaError_t launch_concat_strings(const StrTables& T, uint32_t grid, cudaStream_t stream);
 // b200tfs_decode_padded: padded_plan_kernel, then padded_emit_kernel with emit_grid CTAs striding over the chunks
-cudaError_t launch_padded(const PaddedPlan& pp, uint32_t emit_grid, cudaStream_t stream);
+// (strings: padded_plan_strings_kernel, which places the DT_STRING outputs' offsets too)
+cudaError_t launch_padded(const PaddedPlan& pp, uint32_t emit_grid, cudaStream_t stream, bool strings = false);
+// b200tfs_decode_padded_strings, behind launch_padded: index, scan, copy and fix (padded_kernels.cuh); the index runs a warp per
+// (record, key), copy and fix run grid CTAs striding over the positions
+cudaError_t launch_padded_strings(const PadStrTables& T, uint32_t grid, cudaStream_t stream);
 // tf.Example requests (example_kernels.cuh): count + scan (when T.n_tiles), emit, frame; *launched receives how many kernels
 cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t stream, uint32_t* launched);
 // Classify / Regress responses (example_resp_kernels.cuh): index, scan, emit, [label compare,] publish; emit_ctas CTAs stride over

@@ -301,7 +301,7 @@ struct PadDesc {                   // one (record, key): its value runs, its own
 struct PadKeyOut {                 // one key after the plan
   uint64_t rows, pitch;            // rows in use, destination bytes per row
   uint64_t chunk0;                 // first chunk of the key (entry n_keys: the chunks of every key)
-  uint32_t row_elems, esz, src_esz, op, varint, pad_;
+  uint32_t row_elems, esz, src_esz, op, varint, str;   // str: a DT_STRING key (padded_plan_strings_kernel), no chunks
 };
 struct PaddedPlan {
   ConcatPlan cp;                   // the parse table, scratch and varint table (cp.keys unused)
@@ -313,6 +313,24 @@ struct PaddedPlan {
 // the varint tail of the padded decode: job s = r * kFusedMaxOutputs + k (vdec_plan_kernel's slot) stores element e of record r
 // at its padded position - mixed-radix over the record's dims into the destination's - from jb.dst, the record's first row
 struct VarPadMap { const PadDesc* desc; const PadKeyDev* keys; uint32_t n_keys, pad_; };
+
+// ---- DT_STRING keys of the padded decode as padded byte columns (b200tfs_decode_padded_strings) --------------------------
+// padded_plan_strings_kernel places a string key's rows as any other key's, 8 bytes (one offset entry) per position.  Then
+// (padded_kernels.cuh): pad_str_index_kernel - a warp per pair walks its string_val elements and packs
+// each one's record-relative wire offset and byte position within the record's own strings into the offset entry of its padded
+// position, and leaves the pair's own bytes; pad_str_scan_kernel - one CTA places every record's bytes (own strings plus pad_len
+// per pad position) in the key's data, cuts the rows in use at the first record past data_cap and numbers the positions;
+// pad_str_copy_kernel - destination-major, a lane per position: its own string or the pad, and the final offset of a pad position;
+// pad_str_fix_kernel - the final offsets of the own strings, in a launch of its own because the copy reads those entries.
+struct PadStrKeyDev { uint8_t* data; uint64_t cap; const uint8_t* pad; uint64_t pad_len; };
+struct PadStrTables {
+  PaddedPlan pp;                   // the plan's tables (PadKeyOut::rows of a string key: its rows in use, after the scan)
+  const uint64_t* rec_len;         // [n], device
+  PadStrKeyDev keys[B200TFS_CONCAT_MAX_KEYS];   // in the kernel parameters: a replay reads them as captured
+  uint64_t* bytes;                 // [n_keys * n]: the pair's own string bytes (index)
+  uint64_t* data0;                 // [n_keys * n]: its first byte in the key's data (scan)
+  uint64_t* pos0;                  // [n_keys + 1]: the key's first position among the positions in use of every key (scan)
+};
 
 // ---- deferred framing: the length prefixes of packed-varint inputs computed ON THE DEVICE -----------------------------
 // Every length on the wire precedes its content, and a packed-varint payload's length is only known once the counting

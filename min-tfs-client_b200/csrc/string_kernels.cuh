@@ -14,12 +14,19 @@
 //   str_fix_kernel    the same chunks: every entry becomes its string's first byte in the key's data.  Separate from the copy,
 //                     which reads the entry behind each string for its length.
 
+// The index kernels' sink (walk_strings): string j's entry goes to slot[place(j)] - here entry j; the padded decode's index kernel
+// (padded_kernels.cuh) places it at its padded position.
+struct StrPlaceSame {
+  __device__ __forceinline__ uint64_t operator()(uint64_t j) const { return j; }
+};
+template <class Place = StrPlaceSame>
 struct StrIndexSink {
   uint64_t* slot;
-  uint64_t cap;   // entries the plan reserved (n_strings)
+  uint64_t cap;   // strings the plan reserved entries for (n_strings)
   uint32_t pos;   // bytes of the strings so far
+  Place place;
   __device__ __forceinline__ void operator()(uint64_t j, uint32_t off, uint32_t len) {
-    if (j < cap) slot[j] = ((uint64_t)off << 32) | pos;
+    if (j < cap) slot[place(j)] = ((uint64_t)off << 32) | pos;
     pos += len;
   }
 };
@@ -37,7 +44,7 @@ __global__ void __launch_bounds__(kStrThreads) str_index_kernel(const __grid_con
     cur_open(c, T.w + T.rec_off[r], (uint32_t)T.rec_len[r], lines[warp]);
     c.p = (uint32_t)o.msg_off;
     c.end = (uint32_t)(o.msg_off + o.msg_len);
-    StrIndexSink sink{reinterpret_cast<uint64_t*>((uintptr_t)o.dst_off), o.n_strings, 0u};
+    StrIndexSink<> sink{reinterpret_cast<uint64_t*>((uintptr_t)o.dst_off), o.n_strings, 0u, {}};
     const uint64_t found = walk_strings(c, sink);
     if (c.err || found != o.n_strings) o.status = B200TFS_E_NONCANONICAL;
     else total = sink.pos;

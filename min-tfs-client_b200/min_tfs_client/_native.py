@@ -101,6 +101,13 @@ class PadKey(C.Structure):
     ]
 
 
+class PaddedStrings(C.Structure):
+    """b200tfs_padded_strings: the byte buffer and pad string of one DT_STRING key of b200tfs_decode_padded_strings, whose int64
+    offsets go to the key's dst (in: data, data_cap, pad, pad_len; out of b200tfs_padded_strings_layout: strings, data_bytes)."""
+    _fields_ = [("data", C.c_void_p), ("data_cap", C.c_uint64), ("pad", C.c_void_p), ("pad_len", C.c_uint64), ("strings", C.c_uint64),
+                ("data_bytes", C.c_uint64)]
+
+
 F_BROADCAST = 0x10
 
 
@@ -225,6 +232,12 @@ SIGNATURES = {
     "b200tfs_decode_padded": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey)]),
     "b200tfs_decode_padded_host_async": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey)]),
     "b200tfs_padded_results": (C.c_int, [_vp, C.c_int32, C.c_int32, C.POINTER(Output), C.POINTER(ModelSpec), _i32p]),
+    "b200tfs_padded_strings_layout": (C.c_int, [_vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey), C.POINTER(PaddedStrings),
+                                                C.c_int32]),
+    "b200tfs_decode_padded_strings": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey),
+                                                C.POINTER(PaddedStrings)]),
+    "b200tfs_decode_padded_strings_host_async": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(PadKey),
+                                                           C.POINTER(PaddedStrings)]),
     "b200tfs_padded_request_arena_size": (C.c_int, [C.c_int32, C.POINTER(Request), _u64p]),
     "b200tfs_encode_padded_requests_async": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), C.POINTER(PadInput), _vp, C.c_uint64]),
     "b200tfs_padded_request_frame": (C.c_int, [C.POINTER(Request), C.POINTER(PadInput), _u64p, _vp, C.c_uint64, _u64p, _u64p, _u64p]),

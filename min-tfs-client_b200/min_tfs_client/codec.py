@@ -1398,19 +1398,20 @@ class Codec:
                 return [self._text(buf, base + int(ko[i]), int(kl[i])) for i in range(cnt.value)]
             cap = cnt.value
 
-    def _per_record(self, wires, keys, strict, out_dtypes, device, out, bad_rank, combine, string_columns=False):
+    def _per_record(self, wires, keys, strict, out_dtypes, device, out, bad_rank, combine, string_column=None):
         """The definition itself, response by response, for the requested outputs: what a device route hands over when a batch
         holds a case it does not take (a malformed record, more than FUSED_MAX_OUTPUTS outputs or MAX_RANK dims, TF padding,
         tensor_content only, strings, mismatches).  Like the device routes it converts and checks the requested outputs only.
         Per key, the route's rank rule (`bad_rank(key, parts)`: the ValueError's message, or None), one dtype, and the route's
-        tensor of the parts (`combine(key, parts)`).  `string_columns`: string outputs become BytesColumns of their raw bytes."""
+        tensor of the parts (`combine(key, parts)`).  `string_column(key, parts)`: the route's BytesColumn of string outputs, whose
+        parts are then _RawStrings of their raw bytes (None: numpy str arrays)."""
         wanted = set(keys)
-        per = [self._decode_two_phase([w], strict, out_dtypes, 16, wanted, string_columns)[0] for w in wires]
+        per = [self._decode_two_phase([w], strict, out_dtypes, 16, wanted, string_column is not None)[0] for w in wires]
         result = {}
         for k in keys:
             parts = [p[0][k] for p in per]
             if any(isinstance(a, _RawStrings) for a in parts):
-                result[k] = self._string_column(k, parts, device, out)
+                result[k] = string_column(k, parts)
                 continue
             msg = bad_rank(k, parts)
             if msg:
@@ -1426,7 +1427,8 @@ class Codec:
     def _concat_per_record(self, wires, keys, strict, out_dtypes, device, out, string_columns=False):
         return self._per_record(wires, keys, strict, out_dtypes, device, out,
                                 lambda k, parts: "zero-dimensional arrays cannot be concatenated" if any(a.ndim == 0 for a in parts) else None,
-                                lambda k, parts: np.concatenate(parts, axis=0), string_columns)
+                                lambda k, parts: np.concatenate(parts, axis=0),
+                                (lambda k, parts: self._string_column(k, parts, device, out)) if string_columns else None)
 
     def _string_column(self, key, parts, device: bool, out) -> BytesColumn:
         """The per-response route's BytesColumn of one string output, with the concatenation's errors (ValueError: rank 0, another
@@ -1439,11 +1441,13 @@ class Codec:
             raise ValueError(f"output {key!r}: responses disagree on the dtype")
         if len({a.shape[1:] for a in parts}) > 1 or len({len(a.shape) for a in parts}) > 1:
             raise ValueError(f"output {key!r}: all the input array dimensions except for the concatenation axis must match exactly")
-        strs = [b for a in parts for b in a.strings]
+        return self._bytes_column([b for a in parts for b in a.strings], (sum(a.shape[0] for a in parts),) + tuple(parts[0].shape[1:]),
+                                  device)
+
+    def _bytes_column(self, strs, shape, device: bool) -> BytesColumn:
         offsets = np.zeros(len(strs) + 1, np.int64)
         np.cumsum(np.fromiter(map(len, strs), np.int64, len(strs)), out=offsets[1:])
         data = np.frombuffer(b"".join(strs), np.uint8)
-        shape = (sum(a.shape[0] for a in parts),) + tuple(parts[0].shape[1:])
         if device:
             return BytesColumn(self.device_array(data), self.device_array(offsets), shape)
         return BytesColumn(data.copy(), offsets, shape)
@@ -1615,7 +1619,8 @@ class Codec:
     # ---- batch decode into one padded tensor per key -----------------------------------------------------
     def decode_predict_responses_padded(self, wires: Sequence[bytes], keys: Optional[Sequence[str]] = None, *, pad_value=0,
                                         pad_to: Optional[Mapping] = None, strict: bool = False, out_dtypes: Optional[Mapping] = None,
-                                        device: bool = False, out: Optional[Mapping] = None
+                                        device: bool = False, out: Optional[Mapping] = None, string_columns: bool = False,
+                                        string_pad: bytes = b""
                                         ) -> Tuple[Dict[str, object], Dict[str, np.ndarray], List[DecodedSpec]]:
         """Decode a batch of PredictResponses with ragged trailing dimensions into ONE padded tensor per output - what
         ``pad_sequence`` / ``tf.keras.utils.pad_sequences`` give: for every key, the rows of all responses concatenated along axis
@@ -1630,15 +1635,39 @@ class Codec:
         ``keys``, ``strict``, ``out_dtypes``, ``device`` and ``out`` as for ``decode_predict_responses_concat`` (a narrowed output
         gets the pad converted to the narrowed dtype).  Returns ``({key: tensor}, {key: int64[n, rank] shape of every response's
         output}, [DecodedSpec per response])``.
+
+        ``string_columns=True``: every DT_STRING output comes back as a padded ``BytesColumn`` of shape ``(rows, *tail)`` - in C
+        order, each position inside a response's own dims holds that response's raw ``string_val`` bytes (no UTF-8 check, NULs
+        and high bytes kept) and every other position of its rows holds ``string_pad`` (``bytes``) - with ``offsets`` int64[m + 1]
+        from 0, decoded on the device in the same call as the numeric outputs (``DeviceArray`` data and offsets with
+        ``device=True``, numpy arrays otherwise), with the errors above.  The column and the shapes table feed
+        ``encode_predict_requests_padded`` directly.  ``out`` naming a string output raises ValueError.  Without it, string
+        outputs are decoded on the host into numpy str arrays (and ``device=True`` raises TypeError for them).
         """
         buf, off, ln, keys, out_dtypes, out = self._requested(wires, keys, out, out_dtypes, "need at least one response to pad")
         pad_to = dict(pad_to or {})
-        fast = self._padded_device(wires, buf, off, ln, keys, pad_value, pad_to, strict, out_dtypes, device, out)
+        string_pad = bytes(string_pad)
+        fast = self._padded_device(wires, buf, off, ln, keys, pad_value, pad_to, strict, out_dtypes, device, out, string_columns,
+                                   string_pad)
         if fast is not None:
             return fast
-        return self._padded_per_record(wires, keys, pad_value, pad_to, strict, out_dtypes, device, out)
+        return self._padded_per_record(wires, keys, pad_value, pad_to, strict, out_dtypes, device, out, string_columns, string_pad)
 
-    def _padded_per_record(self, wires, keys, pad_value, pad_to, strict, out_dtypes, device, out):
+    @staticmethod
+    def _padded_tail(k, pad_to, rank: int, dims) -> Tuple[int, ...]:
+        """The trailing dims of key k's padded tensor: pad_to[k], else the elementwise maximum of the parts' `dims` (ValueError:
+        pad_to of another rank)."""
+        tail = tuple(int(x) for x in pad_to[k]) if k in pad_to else tuple(max(s[d] for s in dims) for d in range(1, rank))
+        if len(tail) != rank - 1:
+            raise ValueError(f"output {k!r}: pad_to has {len(tail)} trailing dims, the output {rank - 1}")
+        return tail
+
+    @staticmethod
+    def _padded_fits(k, tail, shape) -> None:
+        if any(shape[d] > tail[d - 1] for d in range(1, len(shape))):
+            raise ValueError(f"output {k!r}: a response of shape {shape} does not fit pad_to {tail}")
+
+    def _padded_per_record(self, wires, keys, pad_value, pad_to, strict, out_dtypes, device, out, string_columns=False, string_pad=b""):
         shapes = {}
 
         def bad_rank(k, parts):
@@ -1649,26 +1678,50 @@ class Codec:
 
         def pad(k, parts):
             rank = parts[0].ndim
-            tail = tuple(int(x) for x in pad_to[k]) if k in pad_to else \
-                tuple(max(a.shape[d] for a in parts) for d in range(1, rank))
-            if len(tail) != rank - 1:
-                raise ValueError(f"output {k!r}: pad_to has {len(tail)} trailing dims, the output {rank - 1}")
+            tail = self._padded_tail(k, pad_to, rank, [a.shape for a in parts])
             res = np.full((sum(a.shape[0] for a in parts), *tail), pad_value, parts[0].dtype)
             r0 = 0
             for a in parts:
-                if any(a.shape[d] > tail[d - 1] for d in range(1, rank)):
-                    raise ValueError(f"output {k!r}: a response of shape {a.shape} does not fit pad_to {tail}")
+                self._padded_fits(k, tail, a.shape)
                 res[(slice(r0, r0 + a.shape[0]),) + tuple(slice(0, d) for d in a.shape[1:])] = a
                 r0 += a.shape[0]
             shapes[k] = np.array([a.shape for a in parts], dtype=np.int64).reshape(len(parts), rank)
             return res
-        result, specs = self._per_record(wires, keys, strict, out_dtypes, device, out, bad_rank, pad)
+
+        def string_column(k, parts):
+            """The padded BytesColumn of string output k, with the padded decode's errors."""
+            if k in out:
+                raise ValueError(f"output {k!r}: out= does not take string columns")
+            if not all(isinstance(a, _RawStrings) for a in parts):
+                raise ValueError(f"output {k!r}: responses disagree on the dtype")
+            rank = len(parts[0].shape)
+            if rank == 0 or any(len(a.shape) != rank for a in parts):
+                raise ValueError(f"output {k!r}: every response must have the same rank >= 1 to be padded")
+            tail = self._padded_tail(k, pad_to, rank, [a.shape for a in parts])
+            res = np.empty((sum(a.shape[0] for a in parts), *tail), object)
+            res.fill(string_pad)
+            r0 = 0
+            for a in parts:
+                self._padded_fits(k, tail, a.shape)
+                own = np.empty(len(a.strings), object)
+                own[:] = a.strings
+                res[(slice(r0, r0 + a.shape[0]),) + tuple(slice(0, d) for d in a.shape[1:])] = own.reshape(a.shape)
+                r0 += a.shape[0]
+            shapes[k] = np.array([a.shape for a in parts], dtype=np.int64).reshape(len(parts), rank)
+            return self._bytes_column(res.ravel().tolist(), res.shape, device)
+        result, specs = self._per_record(wires, keys, strict, out_dtypes, device, out, bad_rank, pad,
+                                         string_column if string_columns else None)
         return result, shapes, specs
 
-    def _padded_device(self, wires, buf, off, ln, keys, pad_value, pad_to, strict, out_dtypes, device, out):
+    def _padded_device(self, wires, buf, off, ln, keys, pad_value, pad_to, strict, out_dtypes, device, out, string_columns=False,
+                       string_pad=b""):
         """The device route (b200tfs_decode_padded): parse, one-CTA plan, destination-major emit, varint decode - or None
-        when the batch holds a case it leaves to the response-by-response route."""
-        pads = []
+        when the batch holds a case it leaves to the response-by-response route.  `string_columns`: with b200tfs_padded_strings
+        entries (string index, scan, copy and fix kernels) when a requested key is DT_STRING."""
+        nk = len(keys)
+        pads, columns, data = [], {}, {}
+        ps = (N.PaddedStrings * nk)() if string_columns else None
+        lib = self._lib
 
         def shape_of(i, c, np_type):
             if strict and c.dtype == DT_HALF:
@@ -1679,6 +1732,10 @@ class Codec:
                 if len(want) != len(tail) or any(t > w for t, w in zip(tail, want)):
                     return None   # the definition raises, after decoding every response
                 tail = want
+            if c.dtype == DT_STRING:   # its destination is the column's int64 offsets
+                columns[i] = (int(c.dims[0]),) + tail
+                pads.append(b"")
+                return (int(np.prod(columns[i], dtype=np.int64)) + 1,)
             try:
                 pads.append(np.full((1,), pad_value, np_type).tobytes())
             except Exception:     # noqa: BLE001 - the definition raises it, after decoding every response
@@ -1688,22 +1745,35 @@ class Codec:
         def place(pk, ptrs, shapes, np_types):
             if any(p % 16 for p in ptrs):
                 return False      # the emit writes whole 16-byte vectors
-            for i in range(len(keys)):
-                pk[i].dst, pk[i].dst_cap, pk[i].rank = ptrs[i], int(np.prod(shapes[i], dtype=np.int64)) * np_types[i].itemsize, len(shapes[i])
-                for d in range(1, len(shapes[i])):
-                    pk[i].dims[d] = shapes[i][d]
+            for i in range(nk):
+                shape = columns.get(i, shapes[i])
+                pk[i].dst, pk[i].dst_cap, pk[i].rank = ptrs[i], int(np.prod(shapes[i], dtype=np.int64)) * np_types[i].itemsize, len(shape)
+                for d in range(1, len(shape)):
+                    pk[i].dims[d] = shape[d]
                 C.memmove(pk[i].pad_bits, pads[i], len(pads[i]))
+                if i in columns:
+                    m = shapes[i][0] - 1
+                    cap = int(ps[i].data_bytes) + (m - int(ps[i].strings)) * len(string_pad)
+                    data[i] = D.DeviceArray(self, (cap,), np.uint8)
+                    ps[i].data, ps[i].data_cap, ps[i].pad, ps[i].pad_len = data[i].ptr, cap, C.cast(C.c_char_p(string_pad), C.c_void_p), len(string_pad)
             return True
-        f = self._key_device((N.PadKey, self._lib.b200tfs_padded_layout, self._lib.b200tfs_decode_padded, self._lib.b200tfs_padded_results),
-                             wires, buf, off, ln, keys, strict, out_dtypes, out, shape_of, place)
+        if string_columns:
+            native = (N.PadKey, lambda *a: lib.b200tfs_padded_strings_layout(*a[:6], ps, a[6]),
+                      lambda *a: lib.b200tfs_decode_padded_strings(*a, ps if columns else None), lib.b200tfs_padded_results)
+        else:
+            native = (N.PadKey, lib.b200tfs_padded_layout, lib.b200tfs_decode_padded, lib.b200tfs_padded_results)
+        f = self._key_device(native, wires, buf, off, ln, keys, strict, out_dtypes, out, shape_of, place, strings=string_columns)
         if f is None:
             return None
-        n, nk = len(wires), len(keys)
+        n = len(wires)
         if any(f.rec_status[r] != N.OK for r in range(n)) or any(f.outs[j].status != N.OK for j in range(n * nk)):
             return None
-        rec_shapes = {k: np.array([list(f.outs[r * nk + i].dims)[: len(f.shapes[i])] for r in range(n)], dtype=np.int64).reshape(n, len(f.shapes[i]))
+        ranks = [len(columns.get(i, f.shapes[i])) for i in range(nk)]
+        rec_shapes = {k: np.array([list(f.outs[r * nk + i].dims)[: ranks[i]] for r in range(n)], dtype=np.int64).reshape(n, ranks[i])
                       for i, k in enumerate(keys)}
         result = self._key_deliver(keys, out, device, f.shapes, f.np_types, f.dev, f.ptrs)
+        for i, a in data.items():
+            result[keys[i]] = BytesColumn(a if device else a.copy_to_host(), result[keys[i]], columns[i])
         self.padded_device_calls += 1
         return result, rec_shapes, f.specs
 
