@@ -819,8 +819,8 @@ int b200tfs_encode_example_requests_ragged_host(b200tfs_ctx* ctx, int32_t n, con
  *                                    n}}, string_val: [e.SerializeToString(deterministic=True) for e in the examples]}}
  *                                    serialised with SerializeToString(deterministic=True); each example's bytes are exactly its
  *                                    bytes in the example_list.
- * A call may mix both.  An unknown kind, a negative key_len or a NULL key with key_len > 0: B200TFS_E_ARG; a key over 2 GiB:
- * B200TFS_E_TOOBIG - checked before the context is looked at.                                                                  */
+ * A call may mix both, and B200TFS_EXAMPLES_PREDICT_ELWC (below), which needs a context.  An unknown kind, a negative key_len
+ * or a NULL key with key_len > 0: B200TFS_E_ARG; a key over 2 GiB: B200TFS_E_TOOBIG - checked before the context is looked at. */
 #define B200TFS_EXAMPLES_LIST 0
 #define B200TFS_EXAMPLES_PREDICT_STRING 1
 typedef struct b200tfs_example_target {
@@ -875,6 +875,54 @@ int b200tfs_encode_example_columns_async(b200tfs_ctx* ctx, int32_t n, const b200
 int b200tfs_encode_example_columns_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
                                         const b200tfs_bytes* bytes, const b200tfs_example_target* targets, void* wire_host,
                                         uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
+
+/* A shared context (tensorflow.serving.ExampleListWithContext, Input field 2): one context Example for the whole request next to
+ * its examples - the input of a ranking or recommendation model, whose per-query features then travel once instead of in every
+ * candidate.  One entry per request, parallel to reqs (contexts == NULL: no request has one).  present == 0: the request is the
+ * one the calls above encode.  present == 1:
+ *   B200TFS_EXAMPLES_LIST:         the ClassificationRequest / RegressionRequest {model_spec, input {example_list_with_context
+ *                                  {examples, context}}}, what requests.py examples_with_context_from_input_dict builds;
+ *   B200TFS_EXAMPLES_PREDICT_ELWC: a PredictRequest whose one input `key` is a DT_STRING tensor of shape [1] whose string_val is
+ *                                  that ExampleListWithContext serialised (TF-Ranking's serving input, one query per request):
+ *                                  PredictRequest{model_spec, inputs[key] = TensorProto{dtype: DT_STRING, tensor_shape {dim {size:
+ *                                  1}}, string_val: [elwc.SerializeToString(deterministic=True)]}}.
+ * Both serialised with SerializeToString(deterministic=True); the ExampleListWithContext bytes are the same in both, and its
+ * examples are those of the example_list.  The context Example's feature k holds all of context feature k's row_elems values
+ * (`data` holds exactly one row; n_examples plays no part), converted as an example's are, listed in the request's `order`; a
+ * context of no features is an empty Example (wire 12 00).  It comes after the examples on the wire:
+ *     ... 12 vi(elwc) {0A vi(ex) ex}* 12 vi(ctx) 0A vi(F) entries
+ * A context's DT_STRING features take b200tfs_bytes entries (context_bytes: one per feature of every present context, in
+ * request-then-feature order) under the rule above with n_examples = 1; its slot grows by its worst case (10 bytes per integer
+ * element, data_len + 11 per string).  Refused before the context is looked at: present not 0 or 1, a negative n_features, NULL
+ * features with n_features > 0, a B200TFS_F_BROADCAST context feature, PREDICT_STRING with present == 1 and PREDICT_ELWC without
+ * (B200TFS_E_ARG); a DT_STRING context feature without a bytes entry (B200TFS_E_DTYPE); host offsets that break the rule
+ * (B200TFS_E_SHAPE, _host).  Device offsets of a context are checked by the kernels as an example's are: that request gets
+ * B200TFS_E_SHAPE in b200tfs_encode_results, and no write leaves its slot.                                                   */
+#define B200TFS_EXAMPLES_PREDICT_ELWC 2
+typedef struct b200tfs_example_context {
+  const b200tfs_feature* features;   /* host array; each feature's data is one row of row_elems values, placed as b200tfs_feature
+                                        says for the entry point                                                                 */
+  int32_t n_features;
+  int32_t present;                   /* 0: no context; 1: this one (an empty one with n_features == 0)                            */
+} b200tfs_example_context;
+/* b200tfs_example_target_request_size with a context (context == NULL: that call itself): the exact length, in closed form,
+ * when no integer or bytes column appears in the examples or the context (B200TFS_E_ARG otherwise).                          */
+int b200tfs_example_context_request_size(const b200tfs_example_request* r, const b200tfs_example_target* target,
+                                         const b200tfs_example_context* context, uint64_t* total_len);
+/* b200tfs_example_columns_arena_size, b200tfs_encode_example_columns_async and b200tfs_encode_example_columns_host with contexts
+ * (contexts == NULL: those calls themselves, which call these).  A call with contexts launches the count and scan kernels over
+ * the contexts that have an integer or bytes column too, and its frame kernel writes each context behind its examples.         */
+int b200tfs_example_context_arena_size(int32_t n, const b200tfs_example_request* reqs, const b200tfs_bytes* bytes,
+                                       const b200tfs_example_target* targets, const b200tfs_example_context* contexts,
+                                       const b200tfs_bytes* context_bytes, uint64_t* bytes_out);
+int b200tfs_encode_example_contexts_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                          const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                          const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes, void* arena_dev,
+                                          uint64_t arena_cap);
+int b200tfs_encode_example_contexts_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                         const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                         const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes, void* wire_host,
+                                         uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
 
 /* ---- Classify / Regress responses: a batch of responses into one value or score array ----------------------
  * What ClassificationResponse.FromString / RegressionResponse.FromString followed by a loop over the result give, concatenated

@@ -11,7 +11,9 @@
 //                    vectors; an example larger than the image is written in place by one warp.  ex_emit_predict_kernel is the
 //                    same for the spans of Predict requests, whose examples start with the string_val tag
 //   ex_frame_kernel  one warp per request: the examples' total, the request prefix in front of the anchor (an example_list or
-//                    a Predict string_val, plan.h ExReq), rec_off / rec_len / status to pinned memory
+//                    a Predict string_val, plan.h ExReq), rec_off / rec_len / status to pinned memory.  A call with contexts
+//                    (ExampleListWithContext, plan.h ExCtxRef) runs ex_frame_context_kernel instead, whose warp also writes its
+//                    request's context behind the examples; count and scan size the contexts as one-example entries
 //
 // count, emit and the example writer take an ExMode: a call with a bytes column launches the kExColumns instantiations, a call
 // with a ragged numeric column (and none of bytes) the kExRagged ones, in which a ragged column's row ends after ex_elems
@@ -376,10 +378,9 @@ __global__ void __launch_bounds__(kExEmitThreads) ex_emit_predict_kernel(const _
 }
 
 constexpr uint32_t kExFrameWarps = 4;
-__global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __grid_constant__ ExTables T) {
-  const uint32_t r = blockIdx.x * kExFrameWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (r >= T.n_req) return;
-  const ExReq q = T.reqs[r];
+// the bytes of request q's examples, by the calling warp
+__device__ __forceinline__ uint64_t ex_examples_len(const ExTables& T, const ExReq& q) {
+  const uint32_t lane = threadIdx.x & 31;
   uint64_t el = 0;
   if (!q.fixed_size) {
     for (uint32_t k = lane; k < q.n_tiles; k += 32) el += T.tile_sum[q.first_tile + k];
@@ -387,20 +388,29 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __gr
   } else {
     el = q.n_ex * q.fixed_size;
   }
-  // [00 be32(msg)] spec 12 vi(outer) mid inner_tag vi(inner) head | examples...   (plan.h ExReq)
-  const uint64_t inner = q.head_len + el, outer = q.mid_len + 1 + varint_len(inner) + inner;
+  return el;
+}
+// Request r's status, and when it is B200TFS_OK its prefix in front of the anchor, by the calling warp: el bytes of examples and
+// `tail` bytes behind them (a context field), nested once more in a string_val with `nest` (Predict-ELWC).  bad: a length or an
+// offset the request reads was out of range.
+__device__ __forceinline__ int32_t ex_frame_request(const ExTables& T, const ExReq& q, uint32_t r, uint64_t el, uint64_t tail,
+                                                    bool nest, bool bad) {
+  const uint32_t lane = threadIdx.x & 31;
+  // [00 be32(msg)] spec 12 vi(outer) mid inner_tag vi(inner) head [42 vi(body)] | body   (plan.h ExReq, ExCtxRef)
+  const uint64_t body = el + tail, nested = nest ? 1 + varint_len(body) + body : body;
+  const uint64_t inner = q.head_len + nested, outer = q.mid_len + 1 + varint_len(inner) + inner;
   const uint64_t msg = q.spec_len + 1 + varint_len(outer) + outer;
-  const uint64_t pre = (q.grpc ? 5 : 0) + msg - el;
+  const uint64_t pre = (q.grpc ? 5 : 0) + msg - body;
   int32_t st = B200TFS_OK;
-  if (T.bad && T.bad[r]) st = B200TFS_E_SHAPE;
+  if (bad) st = B200TFS_E_SHAPE;
   else if (msg > 0x7FFFFFFFull) st = B200TFS_E_TOOBIG;
-  else if (q.anchor + el > q.slot_end) st = B200TFS_E_SIZE;
+  else if (q.anchor + body > q.slot_end) st = B200TFS_E_SIZE;
   if (lane == 0) {
     T.status[r] = st;
     T.rec_off[r] = st ? 0 : q.anchor - pre;
-    T.rec_len[r] = st ? 0 : pre + el;
+    T.rec_len[r] = st ? 0 : pre + body;
   }
-  if (st) return;
+  if (st) return st;
   uint8_t* w = T.arena + q.anchor - pre;
   // the host-written bytes (spec, mid, head: one run in the blob) by the whole warp, the headers between them by lane 0
   const uint32_t at_spec = q.grpc ? 5 : 0, at_outer = at_spec + q.spec_len, at_mid = at_outer + 1 + varint_len(outer);
@@ -409,13 +419,45 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __gr
     const uint32_t d = k < q.spec_len ? at_spec + k : k < q.spec_len + q.mid_len ? at_mid + (k - q.spec_len) : at_head + (k - q.spec_len - q.mid_len);
     w[d] = T.blob[q.spec_off + k];
   }
-  if (lane) return;
-  if (q.grpc) { w[0] = 0; w[1] = (uint8_t)(msg >> 24); w[2] = (uint8_t)(msg >> 16); w[3] = (uint8_t)(msg >> 8); w[4] = (uint8_t)msg; }
-  w[at_outer] = 0x12; put_varint(w + at_outer + 1, outer);
-  w[at_inner] = (uint8_t)q.inner_tag; put_varint(w + at_inner + 1, inner);
+  if (lane == 0) {
+    if (q.grpc) { w[0] = 0; w[1] = (uint8_t)(msg >> 24); w[2] = (uint8_t)(msg >> 16); w[3] = (uint8_t)(msg >> 8); w[4] = (uint8_t)msg; }
+    w[at_outer] = 0x12; put_varint(w + at_outer + 1, outer);
+    w[at_inner] = (uint8_t)q.inner_tag; put_varint(w + at_inner + 1, inner);
+    if (nest) { w[at_head + q.head_len] = 0x42; put_varint(w + at_head + q.head_len + 1, body); }
+  }
+  return st;
 }
 
-cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t stream, uint32_t* launched) {
+__global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __grid_constant__ ExTables T) {
+  const uint32_t r = blockIdx.x * kExFrameWarps + (threadIdx.x >> 5);
+  if (r >= T.n_req) return;
+  const ExReq q = T.reqs[r];
+  ex_frame_request(T, q, r, ex_examples_len(T, q), 0, false, T.bad && T.bad[r]);
+}
+
+// ex_frame_kernel for a call with contexts (plan.h ExCtxRef): a request with one also takes its context's size into its length,
+// the context's bad flag into its status, and writes the context behind its examples, in place, with the request's warp
+template <int kMode>
+__global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_context_kernel(const __grid_constant__ ExTables T,
+                                                                              const ExCtxRef* __restrict__ ctx) {
+  const uint32_t r = blockIdx.x * kExFrameWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= T.n_req) return;
+  const ExReq q = T.reqs[r];
+  const ExCtxRef c = ctx[r];
+  const uint64_t el = ex_examples_len(T, q);
+  if (c.req == kExNoContext) {
+    ex_frame_request(T, q, r, el, 0, false, T.bad && T.bad[r]);
+    return;
+  }
+  const ExReq x = T.reqs[c.req];
+  const uint64_t cs = x.fixed_size ? x.fixed_size : T.S[x.ex0];    // the context field, its tag included
+  if (ex_frame_request(T, q, r, el, cs, c.nest != 0, T.bad && (T.bad[r] || T.bad[c.req]))) return;
+  uint8_t* w = T.arena + q.anchor + el;
+  if (x.n_feat) ex_write_example<kMode, 0x12>(T, x, 0, w);
+  else if (lane == 0) { w[0] = 0x12; w[1] = 0; }                 // context.SetInParent(): no features map at all
+}
+
+cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t stream, uint32_t* launched, const ExCtxRef* ctx) {
   *launched = 0;
   if (T.n_tiles) {
     if (mode == kExColumns) ex_count_kernel<kExColumns><<<T.n_tiles, kExTile, 0, stream>>>(T);
@@ -439,6 +481,13 @@ cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t st
     else ex_emit_predict_kernel<kExDense><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
     *launched += 1;
   }
-  if (T.n_req) { ex_frame_kernel<<<(T.n_req + kExFrameWarps - 1) / kExFrameWarps, 32 * kExFrameWarps, 0, stream>>>(T); *launched += 1; }
+  if (T.n_req) {
+    const uint32_t grid = (T.n_req + kExFrameWarps - 1) / kExFrameWarps;
+    if (!ctx) ex_frame_kernel<<<grid, 32 * kExFrameWarps, 0, stream>>>(T);
+    else if (mode == kExColumns) ex_frame_context_kernel<kExColumns><<<grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx);
+    else if (mode == kExRagged) ex_frame_context_kernel<kExRagged><<<grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx);
+    else ex_frame_context_kernel<kExDense><<<grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx);
+    *launched += 1;
+  }
   return cudaGetLastError();
 }

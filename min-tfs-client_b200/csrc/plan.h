@@ -426,6 +426,13 @@ struct ExReq {
                                                 // fields the emit kernel reads they cost ex_emit_kernel<false> 12 registers
 };
 struct ExSpan { uint32_t req, pad; uint64_t e0, e1; };   // a CTA's examples [e0, e1) of request `req`
+// A call with contexts (ExampleListWithContext) plans each present context as one more request entry of one example, at an
+// index >= n_req of ExTables::reqs: its features, L entries and count tile are its own (an empty context: no feature, no tile,
+// fixed_size 2, the bytes 12 00).  The frame kernel writes it behind the request's examples, behind the tag 12:
+//   [00 be32(msg)] spec 12 vi(outer) mid 12 vi(inner) head [42 vi(elwc)] | examples... | 12 vi(ctx) 0A vi(F) entries
+// with the ELWC nested in a string_val (`nest`) in the Predict form.  One entry per request of the call.
+constexpr uint32_t kExNoContext = 0xFFFFFFFFu;
+struct ExCtxRef { uint32_t req, nest; };   // the context's entry in ExTables::reqs (kExNoContext: none), Predict-ELWC
 struct ExTables {
   const ExReq* reqs; const ExFeat* feats; const uint8_t* blob;
   const ExSpan* tiles;                  // count / scan CTAs
@@ -434,8 +441,9 @@ struct ExTables {
   uint64_t* S;                          // bytes of every example of a request whose size depends on its values
   uint64_t* off;                        // its offset from the anchor
   unsigned long long* tile_sum;         // bytes of every tile's examples
-  int32_t* bad;                         // a call with a ragged or bytes column: per request, nonzero when a length or a string
-                                        // offset was out of range (zeroed by the host in every call); NULL otherwise
+  int32_t* bad;                         // a call with a ragged or bytes column: per request (and context entry), nonzero when a
+                                        // length or a string offset was out of range (zeroed by the host in every call); NULL
+                                        // otherwise
   uint8_t* arena;
   uint64_t* rec_off; uint64_t* rec_len; int32_t* status;   // pinned host memory: read by b200tfs_encode_results
   uint32_t n_req, n_tiles, n_spans, n_predict_spans;

@@ -140,13 +140,19 @@ class Bytes(C.Structure):
     _fields_ = [("offsets", C.c_void_p), ("data_len", C.c_int64), ("flags", C.c_uint32), ("pad_", C.c_int32)]
 
 
-EXAMPLES_LIST, EXAMPLES_PREDICT_STRING = 0, 1
+EXAMPLES_LIST, EXAMPLES_PREDICT_STRING, EXAMPLES_PREDICT_ELWC = 0, 1, 2
 
 
 class ExampleTarget(C.Structure):
     """b200tfs_example_target: what carries one request's examples - a ClassificationRequest / RegressionRequest (EXAMPLES_LIST)
     or a PredictRequest whose input ``key`` is a DT_STRING vector of the serialized examples (EXAMPLES_PREDICT_STRING)."""
     _fields_ = [("kind", C.c_int32), ("pad_", C.c_int32), ("key", C.c_char_p), ("key_len", C.c_int64)]
+
+
+class ExampleContext(C.Structure):
+    """b200tfs_example_context: one request's shared context Example (present 0: none; 1: ``features``, each one row of all
+    its values), which makes the request an ExampleListWithContext (EXAMPLES_LIST / EXAMPLES_PREDICT_ELWC)."""
+    _fields_ = [("features", C.POINTER(Feature)), ("n_features", C.c_int32), ("present", C.c_int32)]
 
 
 class PadInput(C.Structure):
@@ -285,6 +291,16 @@ SIGNATURES = {
                                                        C.POINTER(ExampleTarget), _vp, C.c_uint64]),
     "b200tfs_encode_example_columns_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
                                                       C.POINTER(ExampleTarget), _vp, C.c_uint64, _u64p, _u64p]),
+    "b200tfs_example_context_request_size": (C.c_int, [C.POINTER(ExampleRequest), C.POINTER(ExampleTarget), C.POINTER(ExampleContext),
+                                                       _u64p]),
+    "b200tfs_example_context_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Bytes), C.POINTER(ExampleTarget),
+                                                     C.POINTER(ExampleContext), C.POINTER(Bytes), _u64p]),
+    "b200tfs_encode_example_contexts_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                        C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes), _vp,
+                                                        C.c_uint64]),
+    "b200tfs_encode_example_contexts_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                       C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes), _vp,
+                                                       C.c_uint64, _u64p, _u64p]),
     "b200tfs_example_response_bound": (C.c_int, [C.c_int32, C.c_int32, _u64p, _u64p, _u64p]),
     "b200tfs_decode_example_responses": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64, _vp, C.c_uint64]),
     "b200tfs_decode_example_responses_host_async": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64, _vp,

@@ -366,18 +366,21 @@ class _ExampleColumn(tuple):
     bytes_entry = None
 
 
-def _example_columns(input_dict: Mapping):
+def _example_columns(input_dict: Mapping, context: bool = False):
     """(n_examples, [_ExampleColumn (Feature, keep-alive, key, Ragged or None), ...]) for the device route, or None for a request
     ``examples_from_input_dict`` assembles on the host (numpy str / bytes columns, dtypes without a device conversion - which it
     rejects or converts itself).  A ``RaggedColumn`` gives the Feature of its padded ``values`` (``row_elems = L * unit``) and a
     Ragged entry for its lengths; a ``BytesColumn`` a DT_STRING Feature of its byte buffer and a Bytes entry for its offsets.
     Raises the ValueError ``examples_from_input_dict`` raises for disagreeing example counts, and for device arrays of a dtype the
-    device route does not take."""
+    device route does not take.  With ``context``, ``input_dict`` is a context: every value is one row of all its values (a
+    ``RaggedColumn`` raises ValueError, as ``examples_with_context_from_input_dict`` does)."""
     cols = []
     for k, v in input_dict.items():
         key = k.encode("utf-8") if isinstance(k, str) else bytes(k)
         rag = v if isinstance(v, RaggedColumn) else None
         if rag is not None:
+            if context:
+                raise ValueError(f"context {k!r}: a RaggedColumn has no place in a context, which has no example axis")
             v = rag.values
         if isinstance(v, BytesColumn):
             cols.append((key, None, v.shape, None, v, v.data_on_device, rag))
@@ -392,6 +395,8 @@ def _example_columns(input_dict: Mapping):
             if dtype not in _EXAMPLE_DTYPES:
                 return None
             cols.append((key, None, a.shape, dtype, a, False, rag))
+    if context:     # one example, whose row is the whole value
+        cols = [(c[0], c[1], (1, int(np.prod(c[2], dtype=np.int64))), *c[3:]) for c in cols]
     rows = {shape[0] for _, _, shape, _, _, _, _ in cols if len(shape)}
     if len(rows) > 1:
         raise ValueError(f"inputs disagree on the number of examples: {sorted(rows)}")
@@ -430,16 +435,18 @@ def _example_columns(input_dict: Mapping):
     return n, preps
 
 
-def _host_example_request(model_name, model_version, input_dict, grpc_frame: bool, predict_input=None) -> bytes:
+def _host_example_request(model_name, model_version, input_dict, grpc_frame: bool, predict_input=None, context_dict=None) -> bytes:
     """A request with a column the device route does not take, as ``examples_from_input_dict`` and protobuf make it: a
     ClassificationRequest, or with ``predict_input`` a PredictRequest whose input of that key is the DT_STRING ``[n]`` tensor of
-    the examples, each serialized with ``deterministic=True``."""
-    from .requests import TensorServingClient, examples_from_input_dict
+    the examples, each serialized with ``deterministic=True``.  With ``context_dict`` the examples and the context form an
+    ExampleListWithContext (``examples_with_context_from_input_dict``): the ClassificationRequest's input, or the one string of a
+    DT_STRING ``[1]`` tensor."""
+    from .requests import TensorServingClient, examples_from_input_dict, examples_with_context_from_input_dict
 
     if predict_input is None:
         from tensorflow_serving.apis.classification_pb2 import ClassificationRequest
 
-        req = TensorServingClient._make_example_request(None, ClassificationRequest, model_name, input_dict, model_version)
+        req = TensorServingClient._make_example_request(None, ClassificationRequest, model_name, input_dict, model_version, context_dict)
     else:
         from tensorflow_serving.apis.predict_pb2 import PredictRequest
 
@@ -447,12 +454,15 @@ def _host_example_request(model_name, model_version, input_dict, grpc_frame: boo
         req.model_spec.name = model_name
         if model_version is not None:
             req.model_spec.version.value = model_version
-        examples = examples_from_input_dict(input_dict).example_list.examples
+        if context_dict is None:
+            values = examples_from_input_dict(input_dict).example_list.examples
+        else:
+            values = [examples_with_context_from_input_dict(input_dict, context_dict).example_list_with_context]
         key = predict_input.decode("utf-8") if isinstance(predict_input, bytes) else predict_input
         t = req.inputs[key]
         t.dtype = DT_STRING
-        t.tensor_shape.dim.add().size = len(examples)
-        t.string_val.extend(e.SerializeToString(deterministic=True) for e in examples)
+        t.tensor_shape.dim.add().size = len(values)
+        t.string_val.extend(e.SerializeToString(deterministic=True) for e in values)
     wire = req.SerializeToString(deterministic=True)
     return (b"\x00" + len(wire).to_bytes(4, "big") + wire) if grpc_frame else wire
 
@@ -979,13 +989,20 @@ class Codec:
     def encode_predict_request(self, model_name: str, input_dict: Mapping, model_version: Optional[int] = None, **kw) -> bytes:
         return self.encode_predict_requests([(model_name, model_version, input_dict)], **kw)[0]
 
-    def encode_example_requests(self, requests: Iterable[Tuple[str, Optional[int], Mapping]], *, order="deterministic",
+    def encode_example_requests(self, requests: Iterable[Tuple], *, order="deterministic",
                                 grpc_frame: bool = False, predict_input=None) -> List[bytes]:
         """Each item is ``(model_name, model_version, input_dict)``; returns one ClassificationRequest / RegressionRequest wire
         per item (the two messages share their field numbers, so the bytes serve both RPCs).  With ``predict_input`` (a str or
         bytes key) each wire is instead a PredictRequest for a model that parses serialized tf.Examples: its one input of that
         key is a DT_STRING tensor of shape ``[n]`` whose ``string_val`` holds every example, serialized as the protobuf runtime
         serializes it with ``deterministic=True``.
+
+        An item may also be ``(model_name, model_version, input_dict, context_dict)`` (``None``: no context), in the same call
+        as the others: the request then carries an ExampleListWithContext, its examples plus one context Example shared by all
+        of them (``examples_with_context_from_input_dict``: the whole of ``context_dict[k]`` is context feature k), the form a
+        ranking model takes.  It is the Classify / Regress request's input, or with ``predict_input`` the one string of a
+        DT_STRING ``[1]`` tensor (TF-Ranking's serving input).  Context values are taken as input values are, but a
+        ``RaggedColumn`` raises ValueError.
 
         The bytes equal ``_make_example_request(...).SerializeToString(deterministic=True)`` of the request
         ``examples_from_input_dict`` builds - one tf.Example per row, 0-d arrays repeated in every example - with
@@ -998,19 +1015,32 @@ class Codec:
         deterministic order; device arrays of such dtypes raise ValueError.
         """
         order_code = _ORDER[order] if isinstance(order, str) else int(order)
-        target = None
+        pkey = None
         if predict_input is not None:
             pkey = predict_input.encode("utf-8") if isinstance(predict_input, str) else bytes(predict_input)
-            target = N.ExampleTarget(kind=N.EXAMPLES_PREDICT_STRING, key=pkey, key_len=len(pkey))
         items = list(requests)
         out: List[Optional[bytes]] = [None] * len(items)
-        keep, structs, dev_idx, ragged, strs = [], [], [], [], []
-        for i, (model_name, model_version, input_dict) in enumerate(items):
+        keep, structs, dev_idx, ragged, strs, targets, contexts, ctx_strs = [], [], [], [], [], [], [], []
+        for i, item in enumerate(items):
+            model_name, model_version, input_dict = item[:3]
+            context_dict = item[3] if len(item) > 3 else None
             cols = _example_columns(input_dict)
-            if cols is None:
-                out[i] = _host_example_request(model_name, model_version, input_dict, grpc_frame, predict_input)
+            ccols = _example_columns(context_dict, context=True) if context_dict is not None else None
+            if cols is None or (context_dict is not None and ccols is None):
+                out[i] = _host_example_request(model_name, model_version, input_dict, grpc_frame, predict_input, context_dict)
                 continue
             n, preps = cols
+            if ccols is None:
+                contexts.append(N.ExampleContext())
+            else:
+                cpreps = ccols[1]
+                cfeats = (N.Feature * max(len(cpreps), 1))(*[p[0] for p in cpreps])
+                keep.append((cpreps, cfeats))
+                contexts.append(N.ExampleContext(features=cfeats, n_features=len(cpreps), present=1))
+                ctx_strs += [p.bytes_entry or N.Bytes() for p in cpreps]
+            if pkey is not None:
+                kind = N.EXAMPLES_PREDICT_STRING if ccols is None else N.EXAMPLES_PREDICT_ELWC
+                targets.append(N.ExampleTarget(kind=kind, key=pkey, key_len=len(pkey)))
             feats = (N.Feature * max(len(preps), 1))(*[p[0] for p in preps])
             name = model_name.encode("utf-8") if isinstance(model_name, str) else bytes(model_name)
             structs.append(N.ExampleRequest(model_name=name, model_name_len=len(name), has_version=int(model_version is not None),
@@ -1025,13 +1055,16 @@ class Codec:
             m = len(dev_idx)
             reqs = (N.ExampleRequest * m)(*structs)
             cap = C.c_uint64()
-            tg = (N.ExampleTarget * m)(*[target] * m) if target is not None else None
+            tg = (N.ExampleTarget * m)(*targets) if targets else None
             bs = (N.Bytes * len(strs))(*strs) if any(b.offsets for b in strs) else None
-            N.check(self._lib.b200tfs_example_columns_arena_size(m, reqs, bs, tg, C.byref(cap)))
+            ct = (N.ExampleContext * m)(*contexts) if any(c.present for c in contexts) else None
+            cb = (N.Bytes * len(ctx_strs))(*ctx_strs) if any(b.offsets for b in ctx_strs) else None
+            N.check(self._lib.b200tfs_example_context_arena_size(m, reqs, bs, tg, ct, cb, C.byref(cap)))
             wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
             off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
             rg = (N.Ragged * len(ragged))(*ragged) if any(g.lengths for g in ragged) else None
-            N.check(self._lib.b200tfs_encode_example_columns_host(self._ctx, m, reqs, rg, bs, tg, wire.ctypes.data, cap.value, off, ln))
+            N.check(self._lib.b200tfs_encode_example_contexts_host(self._ctx, m, reqs, rg, bs, tg, ct, cb, wire.ctypes.data, cap.value,
+                                                                   off, ln))
             for j, i in enumerate(dev_idx):
                 out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
         return out  # type: ignore[return-value]

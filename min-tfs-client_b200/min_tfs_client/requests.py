@@ -37,8 +37,6 @@ def examples_from_input_dict(input_dict: Dict[str, np.ndarray]):
     """
     from tensorflow_serving.apis.input_pb2 import Input
 
-    from .tensors import coerce_to_bytes
-
     arrays = {k: v if isinstance(v, (RaggedColumn, BytesColumn)) else np.asarray(v) for k, v in input_dict.items()}
     rows = {a.shape[0] for a in arrays.values() if a.ndim}
     if len(rows) > 1:
@@ -53,15 +51,48 @@ def examples_from_input_dict(input_dict: Dict[str, np.ndarray]):
             if isinstance(a, BytesColumn) or isinstance(a, RaggedColumn) and isinstance(a.values, BytesColumn):
                 feat.bytes_list.value.extend(a.strings(i))
                 continue
-            row = a.row(i) if isinstance(a, RaggedColumn) else a if a.ndim == 0 else a[i]
-            if row.dtype.kind == "f":
-                feat.float_list.value.extend(np.asarray(row, dtype=np.float32).ravel().tolist())
-            elif row.dtype.kind in "iub":
-                feat.int64_list.value.extend(np.asarray(row, dtype=np.int64).ravel().tolist())
-            elif row.dtype.kind in "US":
-                feat.bytes_list.value.extend(coerce_to_bytes(s) for s in np.asarray(row).ravel().tolist())
-            else:
-                raise ValueError(f"input {k!r}: dtype {row.dtype} has no tf.Example feature kind")
+            _fill_feature(feat, k, a.row(i) if isinstance(a, RaggedColumn) else a if a.ndim == 0 else a[i])
+    return inp
+
+
+def _fill_feature(feat, k, row: np.ndarray) -> None:
+    """``feat`` holds ``row`` flattened in C order: ``float_list`` for floating dtypes, ``int64_list`` for integers and bools,
+    ``bytes_list`` for str / bytes."""
+    from .tensors import coerce_to_bytes
+
+    if row.dtype.kind == "f":
+        feat.float_list.value.extend(np.asarray(row, dtype=np.float32).ravel().tolist())
+    elif row.dtype.kind in "iub":
+        feat.int64_list.value.extend(np.asarray(row, dtype=np.int64).ravel().tolist())
+    elif row.dtype.kind in "US":
+        feat.bytes_list.value.extend(coerce_to_bytes(s) for s in np.asarray(row).ravel().tolist())
+    else:
+        raise ValueError(f"input {k!r}: dtype {row.dtype} has no tf.Example feature kind")
+
+
+def examples_with_context_from_input_dict(input_dict: Dict[str, np.ndarray], context_dict: Dict[str, np.ndarray]):
+    """``Input{example_list_with_context{examples, context}}`` (input.proto ExampleListWithContext): what a ranking or
+    recommendation model takes for Classify / Regress - the candidates' examples, as ``examples_from_input_dict`` builds them, and
+    one context Example shared by all of them.  Context feature ``k`` holds the whole of ``context_dict[k]`` flattened in C order
+    (a 0-d array is one value), converted as an example's values are; a ``BytesColumn`` gives all its strings.  An empty
+    ``context_dict`` is an empty context, which is still sent.  A ``RaggedColumn`` raises ValueError: a context has no example
+    axis."""
+    from tensorflow_serving.apis.input_pb2 import Input
+
+    inp = Input()
+    elwc = inp.example_list_with_context
+    elwc.examples.extend(examples_from_input_dict(input_dict).example_list.examples)
+    elwc.context.SetInParent()
+    for k, v in context_dict.items():
+        if isinstance(v, RaggedColumn):
+            raise ValueError(f"context {k!r}: a RaggedColumn has no place in a context, which has no example axis")
+        feat = elwc.context.features.feature[k]
+        if isinstance(v, BytesColumn):
+            o = np.asarray(v.offsets).tolist()
+            d = np.asarray(v.data)
+            feat.bytes_list.value.extend(d[o[j]: o[j + 1]].tobytes() for j in range(len(o) - 1))
+        else:
+            _fill_feature(feat, k, np.asarray(v))
     return inp
 
 
@@ -179,16 +210,20 @@ def gpu_request_serializer(request) -> bytes:
 
 def gpu_example_request_serializer(request) -> bytes:
     """``request_serializer`` for ``channel.unary_unary(CLASSIFY_METHOD | REGRESS_METHOD, ...)``: (model_name, model_version,
-    input_dict) -> the ClassificationRequest / RegressionRequest bytes ``_make_example_request`` would serialise, packed on the GPU."""
+    input_dict[, context_dict]) -> the ClassificationRequest / RegressionRequest bytes ``_make_example_request`` would serialise,
+    packed on the GPU (with a context_dict that is not None: an ExampleListWithContext)."""
     return get_codec().encode_example_requests([request])[0]
 
 
 def gpu_predict_examples_serializer(request) -> bytes:
     """``request_serializer`` for ``channel.unary_unary(PREDICT_METHOD, ...)`` to a model that parses serialized tf.Examples:
     (model_name, model_version, input_dict, input_key) -> a PredictRequest whose input ``input_key`` is the DT_STRING ``[n]``
-    tensor of the examples ``examples_from_input_dict`` builds, each serialized with ``deterministic=True``, packed on the GPU."""
-    model_name, model_version, input_dict, input_key = request
-    return get_codec().encode_example_requests([(model_name, model_version, input_dict)], predict_input=input_key)[0]
+    tensor of the examples ``examples_from_input_dict`` builds, each serialized with ``deterministic=True``, packed on the GPU.
+    (..., input_key, context_dict) with a context_dict that is not None: the input is instead the DT_STRING ``[1]`` tensor of the
+    one ExampleListWithContext ``examples_with_context_from_input_dict`` builds (TF-Ranking's serving input)."""
+    model_name, model_version, input_dict, input_key = request[:4]
+    context_dict = request[4] if len(request) > 4 else None
+    return get_codec().encode_example_requests([(model_name, model_version, input_dict, context_dict)], predict_input=input_key)[0]
 
 
 def gpu_response_deserializer(wire: bytes) -> PredictResponseView:
@@ -221,40 +256,46 @@ class TensorServingClient:
         return self._predict((model_name, model_version, input_dict), timeout)
 
     def predict_examples_request(self, model_name: str, input_dict: Dict[str, np.ndarray], input_key: str = "examples",
-                                 timeout: int = 60, model_version: Optional[int] = None) -> PredictResponseView:
+                                 timeout: int = 60, model_version: Optional[int] = None, context_dict=None) -> PredictResponseView:
         """Predict on a model whose signature takes serialized tf.Examples (a DT_STRING vector it parses with
         ``tf.io.parse_example``, e.g. a TFX Trainer or Estimator export's ``serving_default``): one example per row of
         ``input_dict`` as ``examples_from_input_dict`` builds it, sent as input ``input_key``.  Values may be ``RaggedColumn`` and
-        ``BytesColumn`` columns, encoded on the GPU like the numeric ones."""
+        ``BytesColumn`` columns, encoded on the GPU like the numeric ones.  With ``context_dict`` the input is one serialized
+        ExampleListWithContext instead (a TF-Ranking model's serving input), the context holding the whole of each value."""
         call = self._channel.unary_unary(PREDICT_METHOD, request_serializer=gpu_predict_examples_serializer,
                                          response_deserializer=gpu_response_deserializer)
-        return call((model_name, model_version, input_dict, input_key), timeout)
+        return call((model_name, model_version, input_dict, input_key, context_dict), timeout)
 
-    def _make_example_request(self, request_pb, model_name, input_dict, model_version):
+    def _make_example_request(self, request_pb, model_name, input_dict, model_version, context_dict=None):
         request = request_pb()
         request.model_spec.name = model_name
         if model_version is not None:
             request.model_spec.version.value = model_version
-        request.input.CopyFrom(examples_from_input_dict(input_dict))
+        if context_dict is None:
+            request.input.CopyFrom(examples_from_input_dict(input_dict))
+        else:
+            request.input.CopyFrom(examples_with_context_from_input_dict(input_dict, context_dict))
         return request
 
     def classification_request(self, model_name: str, input_dict: Dict[str, np.ndarray], timeout: int = 60,
-                               model_version: Optional[int] = None):
-        """Same signature as the reference (requests.py:67-81); returns a ``ClassificationResponse``."""
+                               model_version: Optional[int] = None, context_dict=None):
+        """Same signature as the reference (requests.py:67-81); returns a ``ClassificationResponse``.  With ``context_dict`` the
+        input is an ExampleListWithContext (``examples_with_context_from_input_dict``)."""
         from tensorflow_serving.apis.classification_pb2 import ClassificationRequest, ClassificationResponse
 
         call = self._channel.unary_unary(CLASSIFY_METHOD, request_serializer=ClassificationRequest.SerializeToString,
                                          response_deserializer=ClassificationResponse.FromString)
-        return call(self._make_example_request(ClassificationRequest, model_name, input_dict, model_version), timeout)
+        return call(self._make_example_request(ClassificationRequest, model_name, input_dict, model_version, context_dict), timeout)
 
     def regression_request(self, model_name: str, input_dict: Dict[str, np.ndarray], timeout: int = 60,
-                           model_version: Optional[int] = None):
-        """Same signature as the reference (requests.py:83-97); returns a ``RegressionResponse``."""
+                           model_version: Optional[int] = None, context_dict=None):
+        """Same signature as the reference (requests.py:83-97); returns a ``RegressionResponse``.  With ``context_dict`` the
+        input is an ExampleListWithContext (``examples_with_context_from_input_dict``)."""
         from tensorflow_serving.apis.regression_pb2 import RegressionRequest, RegressionResponse
 
         call = self._channel.unary_unary(REGRESS_METHOD, request_serializer=RegressionRequest.SerializeToString,
                                          response_deserializer=RegressionResponse.FromString)
-        return call(self._make_example_request(RegressionRequest, model_name, input_dict, model_version), timeout)
+        return call(self._make_example_request(RegressionRequest, model_name, input_dict, model_version, context_dict), timeout)
 
     def model_status_request(self, model_name: str, model_version: Optional[int] = None, timeout: Optional[int] = 10):
         """``ModelService/GetModelStatus`` as the reference issues it (requests.py:99-110: the version is set only when truthy)."""

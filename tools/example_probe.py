@@ -13,6 +13,11 @@ Workloads (one request each unless stated):
   B3  256 requests of 64 examples shaped like B1
   W1P, W2P, V1P, B1P  W1, W2, V1 and B1 framed for Predict: a PredictRequest whose input "examples" is the DT_STRING [n] vector of the
       serialized examples (b200tfs_encode_example_targets_*), each run beside its Classify form
+  K1  256 requests x 200 candidates {item f32[32], item_id int64} with a shared context {user f32[256], hist int64[50] in
+      0..50 000, query: 1 string of 35 B}: an ExampleListWithContext (b200tfs_encode_example_contexts_*)
+  K1R the same requests with the user features repeated in every example instead (B200TFS_F_BROADCAST rows, example_list)
+  K1P K1 in the Predict-ELWC form: a PredictRequest whose input "examples" is the DT_STRING [1] serialized ExampleListWithContext
+  K2  4 096 requests x 8 candidates shaped like K1: the context dominates, and each is written by its request's frame warp
 Legs: the _async entry point eager (device columns -> device arena), the same captured once as a CUDA graph and replayed,
 _host from pinned columns (copies both ways included), and examples_from_input_dict + SerializeToString(deterministic=True)
 on one host core.  CUDA events over >= 20 calls after warm-up, three runs each; bytes = column bytes read + wire bytes
@@ -25,6 +30,8 @@ without ragged columns would.  The P workloads' host path is the one a Predict u
 SerializeToString(deterministic=True) of every example, string_val.extend and the PredictRequest's SerializeToString.
 The B workloads (BytesColumn columns, b200tfs_encode_example_columns_*) count the string bytes and offsets; their host path runs
 examples_from_input_dict over the equivalent numpy str / bytes arrays, which BytesColumn.from_array turns into the columns.
+The K workloads' host path is examples_with_context_from_input_dict (K1R: examples_from_input_dict) and SerializeToString; K1R
+counts its repeated rows once, as the kernels read them.
 --profile V1,V3 runs only the per-kernel split of the named workloads (profiler on).
 
   python tools/example_probe.py [--calls 20] [--runs 3] [--workloads W1,V1,...] [--profile V1,V3] [--json PATH]
@@ -44,7 +51,7 @@ sys.path.insert(0, os.path.join(REPO, "min-tfs-client_b200"))
 
 from min_tfs_client import _native as N  # noqa: E402
 from min_tfs_client.codec import BytesColumn, Codec, RaggedColumn, _example_columns  # noqa: E402
-from min_tfs_client.requests import TensorServingClient, examples_from_input_dict  # noqa: E402
+from min_tfs_client.requests import TensorServingClient, examples_from_input_dict, examples_with_context_from_input_dict  # noqa: E402
 from tensorflow.core.framework import types_pb2  # noqa: E402
 from tensorflow_serving.apis.classification_pb2 import ClassificationRequest  # noqa: E402
 from tensorflow_serving.apis.predict_pb2 import PredictRequest  # noqa: E402
@@ -66,6 +73,15 @@ def workloads(rng):
     def b1(n):
         return {"country": np.array([b"us", b"de", b"fr", b"jp", b"br"])[rng.integers(0, 5, n)], "tags": tags(n),
                 "dense": rng.standard_normal((n, 16)).astype(np.float32)}
+    def k1(n, repeated=False):
+        d = {"item": rng.standard_normal((n, 32)).astype(np.float32), "item_id": rng.integers(0, 1 << 40, n)}
+        ctx = {"user": rng.standard_normal(256).astype(np.float32), "hist": rng.integers(0, 50_000, 50),
+               "query": BytesColumn.from_array(np.array(bytes(rng.integers(97, 123, 35, dtype=np.uint8))))}
+        if not repeated:
+            return d, ctx
+        # the rows every example repeats: broadcast views, which build() passes as B200TFS_F_BROADCAST rows
+        d.update(user=np.broadcast_to(ctx["user"], (n, 256)), hist=np.broadcast_to(ctx["hist"], (n, 50)), query=ctx["query"])
+        return d
     words = ["".join(rng.choice(list("abcdefghij klmnop\u00e9\u00fc"), int(rng.integers(100, 400)))) for _ in range(1000)]
     queries = np.array([w.encode("utf-8")[:400].decode("utf-8", "ignore") for w in words])
     return {"W1": lambda: [{"dense": rng.standard_normal((65536, 64)).astype(np.float32)}], "W2": lambda: [w2(16384)],
@@ -78,7 +94,9 @@ def workloads(rng):
             "W1P": lambda: [{"dense": rng.standard_normal((65536, 64)).astype(np.float32)}], "W2P": lambda: [w2(16384)],
             "V1P": lambda: [v1(16384)],
             "B1": lambda: [b1(65536)], "B1P": lambda: [b1(65536)], "B3": lambda: [b1(64) for _ in range(256)],
-            "B2": lambda: [{"query": queries[rng.integers(0, 1000, 16384)], "ids": rng.integers(0, 50_000, (16384, 8))}]}
+            "B2": lambda: [{"query": queries[rng.integers(0, 1000, 16384)], "ids": rng.integers(0, 50_000, (16384, 8))}],
+            "K1": lambda: [k1(200) for _ in range(256)], "K1R": lambda: [k1(200, True) for _ in range(256)],
+            "K1P": lambda: [k1(200) for _ in range(256)], "K2": lambda: [k1(8) for _ in range(4096)]}
 
 
 def columns(d):
@@ -86,11 +104,15 @@ def columns(d):
     return {k: BytesColumn.from_array(v) if isinstance(v, np.ndarray) and v.dtype.kind in "US" else v for k, v in d.items()}
 
 
-def host_ref(d, predict=False):
+def host_ref(d, predict=False, ctx=None):
     """the host path: examples_from_input_dict + SerializeToString; with ragged columns one example at a time (each example the
     one examples_from_input_dict makes of that example's rows), merged in order.  predict: every example serialized into the
-    string_val of a PredictRequest's DT_STRING input "examples" instead"""
-    if predict and not any(isinstance(v, RaggedColumn) for v in d.values()):
+    string_val of a PredictRequest's DT_STRING input "examples" instead.  ctx: an ExampleListWithContext, the Classify input or
+    the one string_val"""
+    if ctx is not None:
+        req = TensorServingClient._make_example_request(None, ClassificationRequest, "model", d, 1, ctx)
+        examples = [req.input.example_list_with_context]
+    elif predict and not any(isinstance(v, RaggedColumn) for v in d.values()):
         examples = examples_from_input_dict(d).example_list.examples
     elif not any(isinstance(v, RaggedColumn) for v in d.values()):
         req = TensorServingClient._make_example_request(None, ClassificationRequest, "model", d, 1)
@@ -131,7 +153,9 @@ def used_bytes(d):
     """column bytes the encode needs: a ragged column's used values and its lengths, every other column whole"""
     b = 0
     for v in d.values():
-        if isinstance(v, RaggedColumn):
+        if isinstance(v, np.ndarray) and v.ndim and not v.strides[0]:     # a repeated row, read once
+            b += v[0].nbytes
+        elif isinstance(v, RaggedColumn):
             unit = int(np.prod(v.shape[2:], dtype=np.int64))
             b += int(v.lengths.sum()) * unit * v.values.itemsize + v.lengths.nbytes
         elif isinstance(v, BytesColumn):
@@ -174,13 +198,17 @@ def timed_host(fn, calls):
     return (time.perf_counter() - t0) * 1e6 / calls
 
 
-def build(dicts, device_ptrs=None):
+def build(dicts, device_ptrs=None, context=False):
     """(requests, ragged entries or None when no column is ragged, bytes entries or None when no column is one, keep-alive);
-    device_ptrs[r]: the arrays(d) of request r in HBM"""
+    device_ptrs[r]: the arrays(d) of request r in HBM.  A column of repeated rows (a broadcast view) is a B200TFS_F_BROADCAST
+    row.  context: the dicts are contexts; the requests' features and n_features make their b200tfs_example_context entries"""
     keep, structs, ragged, strs = [], [], [], []
     for r, d in enumerate(dicts):
-        n, preps = _example_columns(d)
-        feats = (N.Feature * len(preps))(*[p[0] for p in preps])
+        n, preps = _example_columns(d, context=context)
+        feats = (N.Feature * max(len(preps), 1))(*[p[0] for p in preps])
+        for f, v in zip(feats, d.values()):
+            if isinstance(v, np.ndarray) and v.ndim and not v.strides[0]:
+                f.flags |= N.F_BROADCAST
         rg = [p[3] or N.Ragged() for p in preps]
         bs = [p.bytes_entry or N.Bytes() for p in preps]
         if device_ptrs is not None:
@@ -239,33 +267,52 @@ def main():
     out = {"card": card, "calls": args.calls, "runs": args.runs, "workloads": {}}
     profile_only = [w for w in args.profile.split(",") if w]
     for name in (profile_only or args.workloads.split(",")):
-        host_dicts = W[name]()
+        pairs = [x if isinstance(x, tuple) else (x, None) for x in W[name]()]
+        host_dicts = [d for d, _ in pairs]
+        host_ctxs = [c for _, c in pairs]
+        with_ctx = host_ctxs[0] is not None
         dicts = [columns(d) for d in host_dicts]
         predict = name.endswith("P")
         g = Ctx()       # a context per workload: the graph captured below pins its scratch buffers
-        refs = [host_ref(d, predict) for d in host_dicts]
-        col_bytes = sum(used_bytes(d) for d in dicts)
+        refs = [host_ref(d, predict, c) for d, c in pairs]
+        col_bytes = sum(used_bytes(d) for d in dicts) + (sum(used_bytes(c) for c in host_ctxs) if with_ctx else 0)
         wire_bytes = sum(len(w) for w in refs)
         moved = col_bytes + wire_bytes
         # device columns
-        ptrs = []
-        for d in dicts:
-            row = []
-            for a in arrays(d):
-                p = g.malloc(a.nbytes)
-                N.check(lib.b200tfs_memcpy_h2d(g.ctx, p, a.ctypes.data, a.nbytes))
-                row.append(p)
-            ptrs.append(row)
+        def upload(ds):
+            ptrs = []
+            for d in ds:
+                row = []
+                for a in arrays(d):
+                    if isinstance(a, np.ndarray) and a.ndim and not a.strides[0]:
+                        a = np.ascontiguousarray(a[0])          # a repeated row: its one row
+                    p = g.malloc(a.nbytes)
+                    N.check(lib.b200tfs_memcpy_h2d(g.ctx, p, a.ctypes.data, a.nbytes))
+                    row.append(p)
+                ptrs.append(row)
+            return ptrs
+        ptrs = upload(dicts)
         reqs, rga, bsa, keep = build(dicts, ptrs)
         n = len(dicts)
-        tg = (N.ExampleTarget * n)(*[N.ExampleTarget(kind=N.EXAMPLES_PREDICT_STRING, key=b"examples", key_len=8)] * n) if predict else None
+        kind = N.EXAMPLES_PREDICT_ELWC if with_ctx else N.EXAMPLES_PREDICT_STRING
+        tg = (N.ExampleTarget * n)(*[N.ExampleTarget(kind=kind, key=b"examples", key_len=8)] * n) if predict else None
+        def contexts(cdicts, cptrs=None):
+            """(b200tfs_example_context entries, their bytes entries, keep-alive)"""
+            creqs, _, cbsa, ckeep = build(cdicts, cptrs, context=True)
+            ct = (N.ExampleContext * n)(*[N.ExampleContext(features=q.features, n_features=q.n_features, present=1) for q in creqs])
+            return ct, cbsa, (creqs, ckeep)
+        ct = cbsa = None
+        if with_ctx:
+            ct, cbsa, ckeep = contexts(host_ctxs, upload(host_ctxs))
         cap = C.c_uint64()
-        N.check(lib.b200tfs_example_columns_arena_size(n, reqs, bsa, tg, C.byref(cap)))
+        N.check(lib.b200tfs_example_context_arena_size(n, reqs, bsa, tg, ct, cbsa, C.byref(cap)))
         arena = g.malloc(cap.value)
         off, ln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
 
         def eager():
-            if bsa is not None:
+            if with_ctx:
+                N.check(lib.b200tfs_encode_example_contexts_async(g.ctx, n, reqs, rga, bsa, tg, ct, cbsa, arena, cap.value))
+            elif bsa is not None:
                 N.check(lib.b200tfs_encode_example_columns_async(g.ctx, n, reqs, rga, bsa, tg, arena, cap.value))
             elif predict:
                 N.check(lib.b200tfs_encode_example_targets_async(g.ctx, n, reqs, rga, tg, arena, cap.value))
@@ -291,7 +338,7 @@ def main():
                 N.check(lib.b200tfs_sync(g.ctx))
                 assert buf.tobytes() == refs[i], (name, i)
 
-        res = {"column_bytes": col_bytes, "wire_bytes": wire_bytes}
+        res = {"column_bytes": col_bytes, "wire_bytes": wire_bytes, "wire_bytes_per_request": wire_bytes / n}
         for _ in range(3):
             eager()
         N.check(lib.b200tfs_sync(g.ctx))
@@ -313,6 +360,8 @@ def main():
             p[...] = a
             return p
         def pin_col(v):
+            if isinstance(v, np.ndarray) and v.ndim and not v.strides[0]:
+                return np.broadcast_to(pin(v[0]), v.shape)
             if isinstance(v, RaggedColumn):
                 return RaggedColumn(pin(v.values), pin(v.lengths))
             if isinstance(v, BytesColumn):
@@ -322,7 +371,11 @@ def main():
         hreqs, hrga, hbsa, hkeep = build(pinned)
         wire = N.PinnedBuffer(cap.value)
         hoff, hln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
-        if hbsa is not None:
+        if with_ctx:
+            hct, hcbsa, hckeep = contexts([{k: pin_col(v) for k, v in c.items()} for c in host_ctxs])
+            host = lambda: N.check(lib.b200tfs_encode_example_contexts_host(codec.ctx, n, hreqs, hrga, hbsa, tg, hct, hcbsa,  # noqa: E731
+                                                                             wire.ptr, cap.value, hoff, hln))
+        elif hbsa is not None:
             host = lambda: N.check(lib.b200tfs_encode_example_columns_host(codec.ctx, n, hreqs, hrga, hbsa, tg, wire.ptr, cap.value,  # noqa: E731
                                                                             hoff, hln))
         elif predict:
@@ -341,8 +394,8 @@ def main():
         runs = []
         for _ in range(args.runs):
             t0 = time.perf_counter()
-            for d in host_dicts:
-                host_ref(d, predict)
+            for d, c in pairs:
+                host_ref(d, predict, c)
             runs.append((time.perf_counter() - t0) * 1e6)
         res["protobuf_host_us"] = runs
         for leg in ("async_us", "graph_us", "host_pinned_us", "protobuf_host_us"):
@@ -366,7 +419,7 @@ def main():
                 pe()
             out["predict_same_bytes_async_us"] = [g.timed(pe, args.calls) for _ in range(args.runs)]
             print("predict W1-bytes", out["predict_same_bytes_async_us"], flush=True)
-        if name in ("W2", "B1", "B2"):     # per-kernel split, profiler on, in a run of its own
+        if name in ("W2", "B1", "B2", "K1", "K1R", "K2"):     # per-kernel split, profiler on, in a run of its own
             split = profile_split(lib, g, eager, args.calls)
             out[f"{name}_kernels"] = split
             print(name, "kernels", json.dumps(split), flush=True)
