@@ -490,7 +490,9 @@ int b200tfs_concat_strings_bound(int32_t n, const uint64_t* rec_len, uint64_t* m
  * ahead of the varint tail - b200tfs_kernel_launches counts ten.  The scratch is sized from n, n_keys and rec_len alone, so a
  * replay over new records of the same lengths re-plans string counts and byte offsets.  b200tfs_concat_results reports each
  * (record, string key): B200TFS_OK with dst_off = 8 * its first string and dst_bytes = 8 * its strings; B200TFS_E_SIZE when its
- * offsets (up to and including the entry behind its last string) would end past dst_cap or its bytes past data_cap; or
+ * offsets (up to and including the entry behind its last string) would end past dst_cap or its bytes past data_cap (a pair's bytes
+ * hold their place whether or not they fit, so every later pair of the key that decoded, one of no bytes too, starts past
+ * data_cap and is B200TFS_E_SIZE as well); or
  * B200TFS_E_NONCANONICAL when its string_val elements do not all lie in its last `value` occurrence (decode that batch on the
  * host).  Stores: for the OK pairs, their offset entries and bytes, and offsets[m] behind the last OK pair of the key; the entries
  * of a pair that ends B200TFS_E_SIZE for its bytes or B200TFS_E_NONCANONICAL may hold scratch values.  Nothing at or past dst_cap

@@ -11,9 +11,12 @@ the model which edges each case reached.  The kernels' constants are read from t
 Wire, as the runtime serialises it with ``deterministic=True``:
   example      {0A | 42} vi(X) 0A vi(F) entry...              X = Features message, F = the map entries
   entry        0A vi(entry) 0A vi(klen) key 12 vi(feature) {12 float_list | 1A int64_list} vi(list) [0A vi(P) payload]
-               (an empty list: vi(list) = 00 and nothing behind it)
+               (an empty list: vi(list) = 00 and nothing behind it), or for a bytes column (BytesColumn)
+               0A vi(entry) 0A vi(klen) key 12 vi(feature) 0A vi(P) {0A vi(len) bytes}...   (P = 0 for a row of no strings)
   Classify     spec 12 vi(outer) 0A vi(inner) examples        outer = Input, inner = ExampleList
   Predict      spec 12 vi(outer) 0A vi(klen) key 12 vi(inner) 08 07 12 vi(shape) shape examples
+  with context spec 12 vi(outer) 12 vi(elwc) elwc              elwc = examples (tag 0A) 12 vi(X) context
+               (Predict: the map entry's TensorProto is DT_STRING [1] with the elwc as its one string_val)
 """
 import functools
 import os
@@ -21,7 +24,7 @@ import re
 
 import numpy as np
 
-from min_tfs_client.codec import RaggedColumn
+from min_tfs_client.codec import BytesColumn, RaggedColumn
 
 _CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "min-tfs-client_b200", "csrc")
 
@@ -130,6 +133,11 @@ class Col:
     def __init__(self, key, value, n, values=True):
         self.key = key.encode("utf-8") if isinstance(key, str) else bytes(key)
         self.ragged = isinstance(value, RaggedColumn)
+        inner = value.values if self.ragged else value
+        self.is_bytes = isinstance(inner, BytesColumn)
+        if self.is_bytes:
+            self._bytes(inner, value.lengths if self.ragged else None, n, values)
+            return
         a = np.asarray(value.values) if self.ragged else np.asarray(value)
         self.is_float = a.dtype.kind == "f"
         self.dtype = a.dtype
@@ -158,6 +166,34 @@ class Col:
             ends = np.cumsum(self.ne)
             self.P = cs[ends] - cs[ends - self.ne]
 
+    def _bytes(self, col, lengths, n, values):
+        """a bytes_list column (BytesColumn, or a RaggedColumn of one): each example's strings, 0A vi(len) bytes each"""
+        self.is_float, self.dtype = False, np.dtype(np.uint8)
+        shape = tuple(col.shape)
+        self.row_elems = int(np.prod(shape[1:], dtype=np.int64)) if shape else 1
+        if lengths is not None:
+            unit = int(np.prod(shape[2:], dtype=np.int64))
+            self.ne = np.clip(np.asarray(lengths).astype(np.int64), 0, shape[1]) * unit
+        else:
+            self.ne = np.full(n, self.row_elems, np.int64)
+        self.data_len, self.broadcast = int(col.data_len), not shape      # what the host plan sizes the column by
+        if not values:
+            return
+        data, off = np.asarray(col.data), np.asarray(col.offsets).astype(np.int64)
+        stride = 0 if not shape else self.row_elems
+        cells = np.arange(self.row_elems)[None, :]
+        idx = (np.arange(n)[:, None] * stride + cells)[cells < self.ne[:, None]]      # the strings of every row, row after row
+        lens = off[idx + 1] - off[idx]
+        out_start = np.cumsum(lens) - lens
+        strings = data[np.repeat(off[idx] - out_start, lens) + np.arange(int(lens.sum()))]
+        if len(idx):
+            sz, self.payload = _join([_const_piece(len(idx), b"\x0a"), varints(lens), (lens, strings)])
+        else:
+            sz, self.payload = np.zeros(0, np.int64), np.zeros(0, np.uint8)
+        ends = np.cumsum(self.ne)
+        cs = np.concatenate([[0], np.cumsum(sz)])
+        self.P = cs[ends] - cs[ends - self.ne]
+
 
 def upb_order(keys):
     """the map order of the deterministic runtime: bytewise on the common prefix, the longer key first on a tie"""
@@ -169,9 +205,16 @@ def upb_order(keys):
     return sorted(range(len(keys)), key=functools.cmp_to_key(lambda i, j: cmp(keys[i], keys[j]) or i - j))
 
 
+def _rows(v):
+    """example count of a column; None for a 0-d (broadcast) one"""
+    if isinstance(v, RaggedColumn):
+        v = v.values
+    shape = tuple(v.shape) if isinstance(v, BytesColumn) else np.shape(v)
+    return shape[0] if shape else None
+
+
 def n_examples(d):
-    rows = {(v.values if isinstance(v, RaggedColumn) else np.asarray(v)).shape[0] for v in d.values()
-            if isinstance(v, RaggedColumn) or np.ndim(v)}
+    rows = {_rows(v) for v in d.values()} - {None}
     assert len(rows) <= 1
     return rows.pop() if rows else (1 if d else 0)
 
@@ -189,7 +232,8 @@ def nested(cols, n):
     """every nested length of every example: P, list, feature, entry (per column, [n_cols, n]), F, X and S ([n])"""
     P = np.stack([c.P for c in cols]) if cols else np.zeros((0, n), np.int64)
     klen = np.array([len(c.key) for c in cols], np.int64)[:, None]
-    lst = np.where(P > 0, 1 + vlen(P) + P, 0)
+    is_bytes = np.array([c.is_bytes for c in cols], bool)[:, None]
+    lst = np.where(is_bytes, P, np.where(P > 0, 1 + vlen(P) + P, 0))      # a BytesList is its values, unpacked
     feature = 1 + vlen(lst) + lst
     entry = 1 + vlen(klen) + klen + 1 + vlen(feature) + feature
     F = (1 + vlen(entry) + entry).sum(0)
@@ -207,8 +251,11 @@ def example_bytes(d, order="deterministic", tag=0x0A):
     for k, c in enumerate(cols):
         has = c.P > 0
         pieces += [_const_piece(n, b"\x0a"), varints(L["entry"][k]), _const_piece(n, b"\x0a" + vi(len(c.key)) + c.key + b"\x12"),
-                   varints(L["feature"][k]), _const_piece(n, b"\x12" if c.is_float else b"\x1a"), varints(L["list"][k]),
-                   _where(has, _join([_const_piece(int(has.sum()), b"\x0a"), varints(c.P[has])])), (c.P, c.payload)]
+                   varints(L["feature"][k]), _const_piece(n, b"\x0a" if c.is_bytes else b"\x12" if c.is_float else b"\x1a"),
+                   varints(L["list"][k])]
+        if not c.is_bytes:
+            pieces.append(_where(has, _join([_const_piece(int(has.sum()), b"\x0a"), varints(c.P[has])])))
+        pieces.append((c.P, c.payload))
     S, flat = _join(pieces)
     assert (S == L["S"]).all()
     return S, flat
@@ -249,11 +296,39 @@ def prefix(name, version, n, el, key=None, grpc=False) -> bytes:
     return g + spec + b"\x12" + vi(outer) + mid + (b"\x0a" if key is None else b"\x12") + vi(inner) + head
 
 
-def request_bytes(name, version, d, key=None, grpc=False, order="deterministic") -> bytes:
+def _one_example(v):
+    """a context column (the one example's row, as requests.py takes it) as a column of one example"""
+    if isinstance(v, BytesColumn):
+        return v if not v.shape else BytesColumn(v.data, v.offsets, (1,) + tuple(v.shape))
+    a = np.asarray(v)
+    return a if a.ndim == 0 else a[None]
+
+
+def context_bytes(context, order="deterministic") -> bytes:
+    """the ExampleListWithContext.context field (tag 12) of a context dict; 12 00 for an empty one"""
+    if not context:
+        return b"\x12\x00"
+    return example_bytes({k: _one_example(v) for k, v in context.items()}, order, 0x12)[1].tobytes()
+
+
+def request_bytes(name, version, d, key=None, grpc=False, order="deterministic", context=None) -> bytes:
     """the whole request: a ClassificationRequest / RegressionRequest (key None) or a PredictRequest whose input `key` holds
-    the examples; with grpc, behind gRPC's five-byte length-prefixed-message header"""
-    S, flat = example_bytes(d, order, 0x0A if key is None else 0x42)
-    return prefix(name, version, len(S), int(S.sum()), key, grpc) + flat.tobytes()
+    the examples; with grpc, behind gRPC's five-byte length-prefixed-message header.  With a context (a dict, {} included) the
+    examples and the context form an ExampleListWithContext: Input field 2, or the one string_val of the Predict input"""
+    if context is None:
+        S, flat = example_bytes(d, order, 0x0A if key is None else 0x42)
+        return prefix(name, version, len(S), int(S.sum()), key, grpc) + flat.tobytes()
+    elwc = example_bytes(d, order, 0x0A)[1].tobytes() + context_bytes(context, order)
+    spec = model_spec(name, version)
+    if key is None:                                     # Input { example_list_with_context = 2 }
+        outer = b"\x12" + vi(len(elwc)) + elwc
+        msg = spec + b"\x12" + vi(len(outer)) + outer
+    else:                                               # inputs[key] = DT_STRING [1] holding the serialized ELWC
+        kb = key.encode("utf-8") if isinstance(key, str) else bytes(key)
+        tp = predict_head(1) + b"\x42" + vi(len(elwc)) + elwc
+        ent = b"\x0a" + vi(len(kb)) + kb + b"\x12" + vi(len(tp)) + tp
+        msg = spec + b"\x12" + vi(len(ent)) + ent
+    return ((b"\x00" + len(msg).to_bytes(4, "big")) if grpc else b"") + msg
 
 
 def examples_chunk(ex, pattern, i0, i1):
@@ -273,6 +348,12 @@ def _entry_len(P, klen):
     return 1 + len(vi(entry)) + entry
 
 
+def _bytes_entry_len(P, klen):
+    feature = 1 + len(vi(P)) + P
+    entry = 1 + len(vi(klen)) + klen + 1 + len(vi(feature)) + feature
+    return 1 + len(vi(entry)) + entry
+
+
 def _example_len(F):
     x = 1 + len(vi(F)) + F
     return 1 + len(vi(x)) + x
@@ -284,16 +365,30 @@ class ReqPlan:
     def __init__(self, name, version, d, key=None, grpc=False):
         self.n, cols = columns(d, values=False)
         self.n_feat = len(cols)
-        self.has_int = any(not c.is_float for c in cols)
-        self.counted = self.has_int or any(c.ragged for c in cols)
-        f_max = sum(_entry_len((4 if c.is_float else 10) * c.row_elems, len(c.key)) for c in cols)
-        f_min = sum(_entry_len((4 if c.is_float else 1) * c.row_elems, len(c.key)) for c in cols)
+        self.has_int = any(not c.is_float and not c.is_bytes for c in cols)
+        self.has_bytes = any(c.is_bytes for c in cols)
+        self.counted = self.has_int or self.has_bytes or any(c.ragged for c in cols)
+        num = [c for c in cols if not c.is_bytes]
+        f_max = sum(_entry_len((4 if c.is_float else 10) * c.row_elems, len(c.key)) for c in num)
+        f_min = sum(_entry_len((4 if c.is_float else 1) * c.row_elems, len(c.key)) for c in num)
+        # a bytes column: no strings plus 27 bytes of length varints at most, two bytes per string at least
+        f_max += sum(_bytes_entry_len(0, len(c.key)) + 27 for c in cols if c.is_bytes)
+        f_min += sum(_bytes_entry_len(2 * c.row_elems, len(c.key)) for c in cols if c.is_bytes)
         self.ex_max, self.ex_min = _example_len(f_max), _example_len(f_min)
+        self.str_bound, self.ex_expect = 0, self.ex_max
+        if self.has_bytes:        # ex_layout: the strings' bound, and the planner's guess of an example's size for the spans
+            self.ex_max += 18
+            self.ex_expect = self.ex_max
+            for c in cols:
+                if c.is_bytes:
+                    D, R = min(c.data_len, PROTO_LIMIT), c.row_elems
+                    self.str_bound += self.n * R * 11 + (self.n * D if c.broadcast else D)
+                    self.ex_expect += 2 * R + (D if c.broadcast or not self.n else D // self.n)
         self.spec = model_spec(name, version)
         mid, head, _, _, _ = framing(self.spec, self.n, 0, key)
         self.grpc, self.predict = grpc, key is not None
         self.prefix_max = (5 if grpc else 0) + len(self.spec) + len(mid) + len(head) + 22
-        self.per = max(1, K_STAGE // self.ex_max)
+        self.per = max(1, K_STAGE // self.ex_expect)
         self.spans = [(e0, min(e0 + self.per, self.n)) for e0 in range(0, self.n, self.per)]
 
 
@@ -303,7 +398,7 @@ def plan(reqs):
     for q in reqs:
         q.slot_off = (cursor + 255) & ~255
         q.anchor = (q.slot_off + q.prefix_max + 15) & ~15
-        q.slot_end = cursor = q.anchor + q.n * q.ex_max
+        q.slot_end = cursor = q.anchor + q.n * q.ex_max + q.str_bound
         q.first_tile = tiles
         q.n_tiles = -(-q.n // K_TILE) if q.counted else 0
         tiles += q.n_tiles
