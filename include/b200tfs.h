@@ -926,6 +926,43 @@ int b200tfs_encode_example_contexts_host(b200tfs_ctx* ctx, int32_t n, const b200
                                          const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes, void* wire_host,
                                          uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
 
+/* MultiInference (tensorflow.serving.MultiInferenceRequest, inference.proto): several Classify / Regress signatures of one model
+ * over one Input.  One entry per request, parallel to reqs (tasks == NULL: no request has any).  n_tasks == 0: the request is the
+ * one the calls above encode.  n_tasks > 0 (B200TFS_EXAMPLES_LIST only, with or without a context): a MultiInferenceRequest
+ *     [00 be32(msg)] {0A vi(task) 0A vi(spec) <model_spec body> [1A vi(sig) sig] 12 vi(m) method}* 12 vi(input) <Input>
+ * what SerializeToString(deterministic=True) writes: every task's model_spec is the request's (name, version) plus the task's
+ * signature_name, its method_name "tensorflow/serving/classify" or "tensorflow/serving/regress"; the Input is the one the request
+ * has without tasks (an example_list, or an ExampleListWithContext with a context).  The same kernels run.  Refused before the
+ * context is looked at (B200TFS_E_ARG): n_tasks < 0, NULL tasks with n_tasks > 0, n_tasks > 0 with a PREDICT target kind, an
+ * unknown method, a negative signature_len or a NULL signature_name with signature_len > 0.                                    */
+typedef struct b200tfs_inference_task {
+  const char* signature_name;  /* UTF-8, written as given                                                                       */
+  int64_t signature_len;       /* 0: no signature_name field (the server's default signature)                                   */
+  int32_t method;              /* B200TFS_RESP_CLASSIFY / B200TFS_RESP_REGRESS                                                  */
+  int32_t pad_;
+} b200tfs_inference_task;
+typedef struct b200tfs_example_tasks {
+  const b200tfs_inference_task* tasks;   /* host array of n_tasks                                                                */
+  int32_t n_tasks;
+  int32_t pad_;
+} b200tfs_example_tasks;
+/* b200tfs_example_context_request_size, _arena_size, b200tfs_encode_example_contexts_{async,host} with tasks (tasks == NULL: those
+ * calls themselves, which call these).                                                                                          */
+int b200tfs_example_tasks_request_size(const b200tfs_example_request* r, const b200tfs_example_target* target,
+                                       const b200tfs_example_context* context, const b200tfs_example_tasks* tasks, uint64_t* total_len);
+int b200tfs_example_tasks_arena_size(int32_t n, const b200tfs_example_request* reqs, const b200tfs_bytes* bytes,
+                                     const b200tfs_example_target* targets, const b200tfs_example_context* contexts,
+                                     const b200tfs_bytes* context_bytes, const b200tfs_example_tasks* tasks, uint64_t* bytes_out);
+int b200tfs_encode_example_tasks_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                       const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                       const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                       const b200tfs_example_tasks* tasks, void* arena_dev, uint64_t arena_cap);
+int b200tfs_encode_example_tasks_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                      const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                      const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                      const b200tfs_example_tasks* tasks, void* wire_host, uint64_t wire_cap, uint64_t* rec_off,
+                                      uint64_t* rec_len);
+
 /* ---- Classify / Regress responses: a batch of responses into one value or score array ----------------------
  * What ClassificationResponse.FromString / RegressionResponse.FromString followed by a loop over the result give, concatenated
  * along the example axis across the n responses: row order is response 0's examples, then response 1's, and so on.
@@ -971,6 +1008,38 @@ int b200tfs_decode_example_responses_host_async(b200tfs_ctx* ctx, int32_t kind, 
  *                            first example, in the same order), the status of the first response that is not B200TFS_OK (or
  *                            B200TFS_OK), and that response's index (-1 when none).                                              */
 int b200tfs_example_response_results(b200tfs_ctx* ctx, int32_t n, int64_t* per_rec, b200tfs_model_spec* specs, int64_t* batch);
+
+/* ---- MultiInference responses: one value or score array per task ------------------------------------------------------------
+ * n MultiInferenceResponses of a request with n_tasks tasks, kinds[t] (B200TFS_RESP_*) the method of task t.  TF Serving returns
+ * one InferenceResult per task, in task order: task t's rows are those of results[t] across the n responses, decoded as the
+ * Classify / Regress calls above decode a ClassificationResult / RegressionResult (C, labels and same_labels per task).  What
+ * MultiInferenceResponse.FromString gives: each `results` field is its own result; inside one, model_spec fields merge, a oneof
+ * member that occurs again merges (its entries concatenate), a different member clears the one before it; unknown fields and
+ * groups are skipped at every level.  Per response and task, precedence as above: B200TFS_E_PARSE (malformed anywhere in the
+ * response's results up to n_tasks; a malformed entry of a task's own result marks that task), B200TFS_E_SIZE, B200TFS_E_SHAPE
+ * (a result count other than n_tasks - every task of the response -, a result whose member is not the one kinds[t] names - an
+ * empty one included -, or an example with another class count than its task's C).
+ * Host only, closed form: max_rows[t] / max_values[t] (n_tasks entries each; either may be NULL) bound task t as
+ * b200tfs_example_response_bound does.                                                                                        */
+int b200tfs_multi_inference_response_bound(int32_t n_tasks, const int32_t* kinds, int32_t n, const uint64_t* rec_len,
+                                           uint64_t* max_rows, uint64_t* max_values);
+/* Decode into values_dst[t] (device, values_cap[t] floats) and labels_dst[t] (device, labels_cap[t] references; Classify tasks
+ * only, may be NULL) for every task t.  Asynchronous and CUDA-graph capturable: one index kernel (a warp per response) assigns
+ * each result's entries to its task, then every task runs the scan, emit, [compare,] publish kernels of the Classify / Regress
+ * decode.  Scratch is sized from n, n_tasks and the record lengths alone.  Stores as there, per task.                        */
+int b200tfs_decode_multi_inference_responses(b200tfs_ctx* ctx, int32_t n_tasks, const int32_t* kinds, const void* arena_dev, int32_t n,
+                                             const uint64_t* rec_off, const uint64_t* rec_len, float* const* values_dst,
+                                             const uint64_t* values_cap, b200tfs_label_ref* const* labels_dst,
+                                             const uint64_t* labels_cap);
+int b200tfs_decode_multi_inference_responses_host_async(b200tfs_ctx* ctx, int32_t n_tasks, const int32_t* kinds, const void* wire_host,
+                                                        int32_t n, const uint64_t* rec_off, const uint64_t* rec_len,
+                                                        float* const* values_dst, const uint64_t* values_cap,
+                                                        b200tfs_label_ref* const* labels_dst, const uint64_t* labels_cap);
+/* Results of the most recent b200tfs_decode_multi_inference_responses* call (synchronises), task after task: per_rec[3 * (t * n +
+ * i) + 0 .. 2], specs[t * n + i] (the model_spec of response i's result t) and batch[5 * t + 0 .. 4], each as
+ * b200tfs_example_response_results gives them.                                                                               */
+int b200tfs_multi_inference_response_results(b200tfs_ctx* ctx, int32_t n, int32_t n_tasks, int64_t* per_rec, b200tfs_model_spec* specs,
+                                             int64_t* batch);
 
 #ifdef __cplusplus
 }

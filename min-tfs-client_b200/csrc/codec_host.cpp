@@ -148,6 +148,8 @@ struct b200tfs_ctx {
   Growable xr_dev;                      // b200tfs_decode_example_responses: entry slots and per-response tables (XrLayout)
   Growable xr_host;                     // ... and the results its publish kernel leaves in pinned memory (XrResultsLayout)
   int32_t xr_n = 0;                     // responses of its most recent call, what b200tfs_example_response_results answers for
+  Growable mi_dev, mi_host;             // b200tfs_decode_multi_inference_responses: the same, for every task (MiLayout)
+  int32_t mi_n = 0, mi_tasks = 0;       // responses and tasks of its most recent call
   Growable unpad_dev;                   // b200tfs_encode_padded_requests_async: boxes, varint jobs and counters, move plan (UnpadLayout)
 };
 
@@ -337,6 +339,8 @@ int b200tfs_destroy(b200tfs_ctx* c) {
   if (c->xr_dev.p) cudaFree(c->xr_dev.p);
   if (c->unpad_dev.p) cudaFree(c->unpad_dev.p);
   if (c->xr_host.p) cudaFreeHost(c->xr_host.p);
+  if (c->mi_dev.p) cudaFree(c->mi_dev.p);
+  if (c->mi_host.p) cudaFreeHost(c->mi_host.p);
   if (c->enc_host.p) cudaFreeHost(c->enc_host.p);
   if (c->measured_dev.p) cudaFree(c->measured_dev.p);
   if (c->scratch_host.p) cudaFreeHost(c->scratch_host.p);

@@ -24,6 +24,8 @@
 //                      arrays (example_kernels.cuh).
 //   xr_index / xr_scan / xr_emit / xr_compare / xr_publish_kernel   Classify / Regress responses: a batch of responses into
 //                      one value / score array (example_resp_kernels.cuh, walk in example_walk.h).
+//   mi_index_kernel    MultiInference responses: assigns each result's entries to its task, whose view the xr kernels then
+//                      decode (multi_resp_kernels.cuh, walk in multi_walk.h).
 //   venc_* / vdec_*    packed-varint encode and decode (int_val / int64_val / uint32_val / uint64_val /
 //                      half_val / bool_val): varint_kernels.cuh.  vdec_plan_kernel + vdec_{count,emit}_dev_kernel decode the
 //                      varint outputs of a single-launch decode from tables built on the device (b200tfs_set_decode_varints).
@@ -49,6 +51,7 @@
 #include "tpl.h"
 #include "unpad.h"
 #include "example_walk.h"
+#include "multi_walk.h"
 #include "walker.h"
 #include "wire.h"
 
@@ -1225,6 +1228,11 @@ __global__ void __launch_bounds__(kConcatPlanThreads) concat_plan_strings_kernel
 // Classify / Regress responses: xr_index / xr_scan / xr_emit / xr_compare / xr_publish
 // ------------------------------------------------------------------------------------------------
 #include "example_resp_kernels.cuh"
+
+// ------------------------------------------------------------------------------------------------
+// MultiInference responses: mi_index, then the Classify / Regress kernels per task
+// ------------------------------------------------------------------------------------------------
+#include "multi_resp_kernels.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // PredictRequests cut out of padded tensors: unpad_plan / unpad_len / unpad_layout / unpad_frame / move / unpad_emit

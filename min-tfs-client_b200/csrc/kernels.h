@@ -63,6 +63,10 @@ cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t st
 // Classify / Regress responses (example_resp_kernels.cuh): index, scan, emit, [label compare,] publish; emit_ctas CTAs stride over
 // the rows; *launched receives how many kernels
 cudaError_t launch_example_responses(const XrTables& T, uint32_t emit_ctas, cudaStream_t stream, uint32_t* launched);
+// MultiInference responses (multi_resp_kernels.cuh): index, then scan, emit, [label compare,] publish on each of the M.n_tasks
+// views (host array); *launched receives how many kernels
+cudaError_t launch_multi_inference_responses(const MiTables& M, const XrTables* views, uint32_t emit_ctas, cudaStream_t stream,
+                                             uint32_t* launched);
 // PredictRequests cut out of padded tensors (unpad_kernels.cuh): plan, [varint count,] layout, frame, move over move_grid CTAs (the
 // host's bound on the tiles), [varint emit]; *launched receives how many kernels
 cudaError_t launch_unpad(const UnpadPlan& up, uint32_t move_grid, cudaStream_t stream, uint32_t* launched);

@@ -491,4 +491,16 @@ struct XrTables {
   uint32_t n, kind;
 };
 
+// ---- MultiInference responses (example_host.inc plans, multi_resp_kernels.cuh runs) ---------------------------------------
+// Response r owns xr_row_bound(rec_len[r]) entry slots from E0[r] on, shared by its tasks: task t's entries follow task t - 1's.
+// The per-task tables are task-major, [n_tasks][n]; task t's XrTables view points at its rows, and the xr kernels run on it.
+struct MiTables {
+  const uint8_t* w;
+  const uint64_t* rec_off; const uint64_t* rec_len; const uint64_t* E0;
+  const uint32_t* kinds;                   // B200TFS_RESP_* of every task
+  b200tfs_label_ref* ent;
+  uint64_t* ent0; uint32_t* rows; uint32_t* cls0; int32_t* status; b200tfs_model_spec* specs;   // [n_tasks][n]
+  uint32_t n, n_tasks;
+};
+
 }  // namespace b200tfs

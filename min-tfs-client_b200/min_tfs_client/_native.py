@@ -155,6 +155,17 @@ class ExampleContext(C.Structure):
     _fields_ = [("features", C.POINTER(Feature)), ("n_features", C.c_int32), ("present", C.c_int32)]
 
 
+class InferenceTask(C.Structure):
+    """b200tfs_inference_task: one task of a MultiInferenceRequest - a signature (signature_len 0: the server's default) run with
+    the method RESP_CLASSIFY or RESP_REGRESS."""
+    _fields_ = [("signature_name", C.c_char_p), ("signature_len", C.c_int64), ("method", C.c_int32), ("pad_", C.c_int32)]
+
+
+class ExampleTasks(C.Structure):
+    """b200tfs_example_tasks: the tasks of one request (n_tasks 0: not a MultiInferenceRequest)."""
+    _fields_ = [("tasks", C.c_void_p), ("n_tasks", C.c_int32), ("pad_", C.c_int32)]
+
+
 class PadInput(C.Structure):
     """b200tfs_pad_input: the shapes of one input of b200tfs_encode_padded_requests_async (int64[n, cols]; cols 1: row counts)."""
     _fields_ = [("shapes", C.c_void_p), ("cols", C.c_int32), ("pad_", C.c_int32)]
@@ -306,6 +317,23 @@ SIGNATURES = {
     "b200tfs_decode_example_responses_host_async": (C.c_int, [_vp, C.c_int32, _vp, C.c_int32, _u64p, _u64p, _vp, C.c_uint64, _vp,
                                                               C.c_uint64]),
     "b200tfs_example_response_results": (C.c_int, [_vp, C.c_int32, C.POINTER(C.c_int64), C.POINTER(ModelSpec), C.POINTER(C.c_int64)]),
+    "b200tfs_example_tasks_request_size": (C.c_int, [C.POINTER(ExampleRequest), C.POINTER(ExampleTarget), C.POINTER(ExampleContext),
+                                                     C.POINTER(ExampleTasks), _u64p]),
+    "b200tfs_example_tasks_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Bytes), C.POINTER(ExampleTarget),
+                                                   C.POINTER(ExampleContext), C.POINTER(Bytes), C.POINTER(ExampleTasks), _u64p]),
+    "b200tfs_encode_example_tasks_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                     C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                     C.POINTER(ExampleTasks), _vp, C.c_uint64]),
+    "b200tfs_encode_example_tasks_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                    C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                    C.POINTER(ExampleTasks), _vp, C.c_uint64, _u64p, _u64p]),
+    "b200tfs_multi_inference_response_bound": (C.c_int, [C.c_int32, _i32p, C.c_int32, _u64p, _u64p, _u64p]),
+    "b200tfs_decode_multi_inference_responses": (C.c_int, [_vp, C.c_int32, _i32p, _vp, C.c_int32, _u64p, _u64p, _vpp, _u64p, _vpp,
+                                                           _u64p]),
+    "b200tfs_decode_multi_inference_responses_host_async": (C.c_int, [_vp, C.c_int32, _i32p, _vp, C.c_int32, _u64p, _u64p, _vpp,
+                                                                      _u64p, _vpp, _u64p]),
+    "b200tfs_multi_inference_response_results": (C.c_int, [_vp, C.c_int32, C.c_int32, C.POINTER(C.c_int64), C.POINTER(ModelSpec),
+                                                           C.POINTER(C.c_int64)]),
 }
 
 _lib = None

@@ -435,15 +435,18 @@ def _example_columns(input_dict: Mapping, context: bool = False):
     return n, preps
 
 
-def _host_example_request(model_name, model_version, input_dict, grpc_frame: bool, predict_input=None, context_dict=None) -> bytes:
+def _host_example_request(model_name, model_version, input_dict, grpc_frame: bool, predict_input=None, context_dict=None,
+                          tasks=None) -> bytes:
     """A request with a column the device route does not take, as ``examples_from_input_dict`` and protobuf make it: a
     ClassificationRequest, or with ``predict_input`` a PredictRequest whose input of that key is the DT_STRING ``[n]`` tensor of
     the examples, each serialized with ``deterministic=True``.  With ``context_dict`` the examples and the context form an
     ExampleListWithContext (``examples_with_context_from_input_dict``): the ClassificationRequest's input, or the one string of a
-    DT_STRING ``[1]`` tensor."""
-    from .requests import TensorServingClient, examples_from_input_dict, examples_with_context_from_input_dict
+    DT_STRING ``[1]`` tensor.  With ``tasks`` the request is the MultiInferenceRequest ``make_multi_inference_request`` builds."""
+    from .requests import TensorServingClient, examples_from_input_dict, examples_with_context_from_input_dict, make_multi_inference_request
 
-    if predict_input is None:
+    if tasks is not None:
+        req = make_multi_inference_request(model_name, model_version, tasks, input_dict, context_dict)
+    elif predict_input is None:
         from tensorflow_serving.apis.classification_pb2 import ClassificationRequest
 
         req = TensorServingClient._make_example_request(None, ClassificationRequest, model_name, input_dict, model_version, context_dict)
@@ -650,6 +653,7 @@ class Codec:
         self._pe_arena = None         # their device arena (grows)
         # decode_regression_responses / decode_classification_responses calls the device route finished
         self.example_response_device_calls = 0
+        self.multi_inference_device_calls = 0     # MultiInference batches the device route decoded
         self._xr_scratch = None       # their device destinations when the result goes to host memory: (values, labels)
 
     def close(self):
@@ -990,7 +994,7 @@ class Codec:
         return self.encode_predict_requests([(model_name, model_version, input_dict)], **kw)[0]
 
     def encode_example_requests(self, requests: Iterable[Tuple], *, order="deterministic",
-                                grpc_frame: bool = False, predict_input=None) -> List[bytes]:
+                                grpc_frame: bool = False, predict_input=None, tasks=None) -> List[bytes]:
         """Each item is ``(model_name, model_version, input_dict)``; returns one ClassificationRequest / RegressionRequest wire
         per item (the two messages share their field numbers, so the bytes serve both RPCs).  With ``predict_input`` (a str or
         bytes key) each wire is instead a PredictRequest for a model that parses serialized tf.Examples: its one input of that
@@ -1013,8 +1017,24 @@ class Codec:
         ValueError), which ``BytesColumn.from_array`` makes of a numpy str / bytes array.  A request with a numpy str / bytes
         column (or a dtype the device route does not take) is assembled on the host by ``examples_from_input_dict``, in
         deterministic order; device arrays of such dtypes raise ValueError.
+
+        With ``tasks`` - a sequence of ``(signature_name, method_name)``, method_name ``CLASSIFY_METHOD_NAME`` or
+        ``REGRESS_METHOD_NAME`` (requests.py) - every wire is instead the MultiInferenceRequest ``make_multi_inference_request``
+        builds: one InferenceTask per task, each naming the item's model and version and the task's signature (an empty or None
+        one: the server's default), over the Input the item has without tasks.  ``tasks`` with ``predict_input`` raises ValueError.
         """
         order_code = _ORDER[order] if isinstance(order, str) else int(order)
+        task_arr = None
+        if tasks is not None:
+            from .requests import _checked_tasks
+
+            if predict_input is not None:
+                raise ValueError("tasks make a MultiInferenceRequest, which carries an Input, not a Predict input")
+            tasks = _checked_tasks(tasks)
+            sigs = [s.encode("utf-8") for s, _ in tasks]
+            task_arr = (N.InferenceTask * len(tasks))(*[N.InferenceTask(signature_name=s, signature_len=len(s),
+                                                                        method=N.RESP_CLASSIFY if m == _CLASSIFY_NAME else N.RESP_REGRESS)
+                                                        for s, (_, m) in zip(sigs, tasks)])
         pkey = None
         if predict_input is not None:
             pkey = predict_input.encode("utf-8") if isinstance(predict_input, str) else bytes(predict_input)
@@ -1027,7 +1047,7 @@ class Codec:
             cols = _example_columns(input_dict)
             ccols = _example_columns(context_dict, context=True) if context_dict is not None else None
             if cols is None or (context_dict is not None and ccols is None):
-                out[i] = _host_example_request(model_name, model_version, input_dict, grpc_frame, predict_input, context_dict)
+                out[i] = _host_example_request(model_name, model_version, input_dict, grpc_frame, predict_input, context_dict, tasks)
                 continue
             n, preps = cols
             if ccols is None:
@@ -1059,12 +1079,15 @@ class Codec:
             bs = (N.Bytes * len(strs))(*strs) if any(b.offsets for b in strs) else None
             ct = (N.ExampleContext * m)(*contexts) if any(c.present for c in contexts) else None
             cb = (N.Bytes * len(ctx_strs))(*ctx_strs) if any(b.offsets for b in ctx_strs) else None
-            N.check(self._lib.b200tfs_example_context_arena_size(m, reqs, bs, tg, ct, cb, C.byref(cap)))
+            tk = None
+            if task_arr is not None:
+                tk = (N.ExampleTasks * m)(*[N.ExampleTasks(tasks=C.addressof(task_arr), n_tasks=len(task_arr))] * m)
+            N.check(self._lib.b200tfs_example_tasks_arena_size(m, reqs, bs, tg, ct, cb, tk, C.byref(cap)))
             wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
             off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
             rg = (N.Ragged * len(ragged))(*ragged) if any(g.lengths for g in ragged) else None
-            N.check(self._lib.b200tfs_encode_example_contexts_host(self._ctx, m, reqs, rg, bs, tg, ct, cb, wire.ctypes.data, cap.value,
-                                                                   off, ln))
+            N.check(self._lib.b200tfs_encode_example_tasks_host(self._ctx, m, reqs, rg, bs, tg, ct, cb, tk, wire.ctypes.data, cap.value,
+                                                                off, ln))
             for j, i in enumerate(dev_idx):
                 out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
         return out  # type: ignore[return-value]
@@ -1850,9 +1873,16 @@ class Codec:
         N.check(self._lib.b200tfs_decode_example_responses_host_async(self._ctx, kind, buf.ctypes.data, n, off, ln, vptr, mv, lptr, lcap))
         per, specs, batch = (C.c_int64 * (3 * n))(), (N.ModelSpec * n)(), (C.c_int64 * 5)()
         N.check(self._lib.b200tfs_example_response_results(self._ctx, n, per, specs, batch))   # synchronises
-        rows, ncls, same, status = int(batch[0]), int(batch[1]), bool(batch[2]), int(batch[3])
-        if status != N.OK:      # a response the device route does not decode: the definition itself, response by response
+        if int(batch[3]) != N.OK:      # a response the device route does not decode: the definition itself, response by response
             return self._example_batch_host(kind, wires, device, out)
+        res = self._xr_deliver(cls, buf, off, n, per, specs, batch, vptr, lptr, device, out)
+        self.example_response_device_calls += 1
+        return res
+
+    def _xr_deliver(self, cls, buf, off, n, per, specs, batch, vptr, lptr, device, out):
+        """The batch one task of a device decode left: `per`, `specs` and `batch` as b200tfs_example_response_results gives them,
+        its values at vptr and (cls) its label references at lptr on the device."""
+        rows, ncls, same = int(batch[0]), int(batch[1]), bool(batch[2])
         counts = np.array([per[3 * i + 1] for i in range(n)], dtype=np.int64)
         spec_list = [self._spec(buf, int(off[i]), specs[i]) for i in range(n)]
         vals = self._example_out((rows, ncls) if cls else (rows,), device, out, src_dev=vptr)
@@ -1862,7 +1892,6 @@ class Codec:
             if nref:
                 N.check(self._lib.b200tfs_memcpy_d2h(self._ctx, refs.ctypes.data, lptr, refs.nbytes))
         self.sync()
-        self.example_response_device_calls += 1
         if not cls:
             return RegressionBatch(vals, counts, spec_list)
         row_of = np.repeat(np.arange(n), counts)
@@ -1916,26 +1945,93 @@ class Codec:
 
         cls = kind == N.RESP_CLASSIFY
         msgs = [(ClassificationResponse if cls else RegressionResponse).FromString(bytes(w)) for w in wires]
-        specs = []
-        for m in msgs:
-            s = m.model_spec
-            specs.append(DecodedSpec(s.name, s.version.value, s.HasField("version"), s.version_label, s.signature_name))
+        return self._example_batch_of(cls, [m.result for m in msgs], [m.model_spec for m in msgs], device, out)
+
+    def _example_batch_of(self, cls, results, model_specs, device, out):
+        """The batch of parsed ClassificationResults (cls) or RegressionResults and their model_specs, one of each per response."""
+        specs = [DecodedSpec(s.name, s.version.value, s.HasField("version"), s.version_label, s.signature_name) for s in model_specs]
         if cls:
-            rows = [cl.classes for m in msgs for cl in m.result.classifications]
+            rows = [cl.classes for m in results for cl in m.classifications]
             if len({len(r) for r in rows}) > 1:
                 raise ValueError("examples disagree on the number of classes")
             ncls = len(rows[0]) if rows else 0
             vals = np.array([[c.score for c in r] for r in rows], np.float32).reshape(len(rows), ncls)
-            counts = np.array([len(m.result.classifications) for m in msgs], dtype=np.int64)
+            counts = np.array([len(m.classifications) for m in results], dtype=np.int64)
             labels = [[c.label for c in r] for r in rows]
         else:
-            vals = np.array([r.value for m in msgs for r in m.result.regressions], np.float32)
-            counts = np.array([len(m.result.regressions) for m in msgs], dtype=np.int64)
+            vals = np.array([r.value for m in results for r in m.regressions], np.float32)
+            counts = np.array([len(m.regressions) for m in results], dtype=np.int64)
         res = self._example_out(vals.shape, device, out, host=vals)
         if not cls:
             return RegressionBatch(res, counts, specs)
         same = all(r == labels[0] for r in labels)
         return ClassificationBatch(res, counts, specs, list(labels[0]) if same and labels else ([] if same else None), labels)
+
+    # ---- MultiInference responses -----------------------------------------------------------------
+    def decode_multi_inference_responses(self, wires: Sequence[bytes], methods: Sequence[str], *, device: bool = False,
+                                         out=None) -> List[Union[ClassificationBatch, RegressionBatch]]:
+        """Decode a batch of MultiInferenceResponses of a request whose tasks have the method names ``methods``
+        (``CLASSIFY_METHOD_NAME`` / ``REGRESS_METHOD_NAME``, in task order): one ``ClassificationBatch`` or ``RegressionBatch``
+        per task, in task order.  Task t's batch is what ``decode_classification_responses`` / ``decode_regression_responses``
+        give for ``results[t]`` of every response, its specs each result's own model_spec.  Raises what
+        ``MultiInferenceResponse.FromString`` raises, and ValueError when a response has another number of results than
+        ``methods``, when a result is not the one its method names (an empty one included), or when a classify task's examples
+        disagree on the number of classes.  ``device`` as there; ``out`` is None or a sequence parallel to ``methods`` whose
+        entries (None: a new array) follow the rules of ``out`` there."""
+        kinds = [_method_kind(m) for m in methods]
+        T = len(kinds)
+        if not T:
+            raise ValueError("a MultiInference decode needs at least one task")
+        outs = [None] * T if out is None else list(out)
+        if len(outs) != T:
+            raise ValueError(f"out has {len(outs)} entries for {T} tasks")
+        n = len(wires)
+        if n == 0:
+            return self._multi_batch_host(kinds, wires, device, outs)
+        buf, off, ln = self._pack_wires(wires)
+        kv = (C.c_int32 * T)(*kinds)
+        max_rows, max_values = (C.c_uint64 * T)(), (C.c_uint64 * T)()
+        N.check(self._lib.b200tfs_multi_inference_response_bound(T, kv, n, ln, max_rows, max_values))
+        mv = int(max_values[0])           # every task has the same bound
+        cls_of = [k == N.RESP_CLASSIFY for k in kinds]
+        label_at = list(np.cumsum([0] + cls_of[:-1]))     # the classify tasks' places in the label scratch
+        scratch_v, scratch_l = self._xr_buffers(T * mv, sum(cls_of) * mv)
+        vptrs = [scratch_v.ptr + 4 * mv * t for t in range(T)]
+        lptrs = [scratch_l.ptr + C.sizeof(N.LabelRef) * mv * int(label_at[t]) if cls_of[t] else None for t in range(T)]
+        caps = (C.c_uint64 * T)(*[mv] * T)
+        lcaps = (C.c_uint64 * T)(*[mv if c else 0 for c in cls_of])
+        N.check(self._lib.b200tfs_decode_multi_inference_responses_host_async(self._ctx, T, kv, buf.ctypes.data, n, off, ln,
+                                                                              (C.c_void_p * T)(*vptrs), caps, (C.c_void_p * T)(*lptrs),
+                                                                              lcaps))
+        per, specs, batch = (C.c_int64 * (3 * n * T))(), (N.ModelSpec * (n * T))(), (C.c_int64 * (5 * T))()
+        N.check(self._lib.b200tfs_multi_inference_response_results(self._ctx, n, T, per, specs, batch))   # synchronises
+        if any(int(batch[5 * t + 3]) != N.OK for t in range(T)):   # the definition itself, response by response
+            return self._multi_batch_host(kinds, wires, device, outs)
+        res = [self._xr_deliver(cls_of[t], buf, off, n, per[3 * n * t: 3 * n * (t + 1)], specs[n * t: n * (t + 1)],
+                                batch[5 * t: 5 * (t + 1)], vptrs[t], lptrs[t], device, outs[t]) for t in range(T)]
+        self.multi_inference_device_calls += 1
+        return res
+
+    def _multi_batch_host(self, kinds, wires, device, outs):
+        """The definition of ``decode_multi_inference_responses`` with protobuf on the host: what the device route hands over when
+        a response does not decode there."""
+        from tensorflow_serving.apis.inference_pb2 import MultiInferenceResponse
+
+        msgs = [MultiInferenceResponse.FromString(bytes(w)) for w in wires]
+        T = len(kinds)
+        for i, m in enumerate(msgs):
+            if len(m.results) != T:
+                raise ValueError(f"response {i} has {len(m.results)} results for {T} tasks")
+            for t, k in enumerate(kinds):
+                want = "classification_result" if k == N.RESP_CLASSIFY else "regression_result"
+                if m.results[t].WhichOneof("result") != want:
+                    raise ValueError(f"response {i}: result {t} is {m.results[t].WhichOneof('result')}, its task wants {want}")
+        res = []
+        for t, k in enumerate(kinds):
+            cls = k == N.RESP_CLASSIFY
+            body = [m.results[t].classification_result if cls else m.results[t].regression_result for m in msgs]
+            res.append(self._example_batch_of(cls, body, [m.results[t].model_spec for m in msgs], device, outs[t]))
+        return res
 
     @staticmethod
     def _decode_strings(buf: np.ndarray, base: int, o: N.Output, rec_len: int = 0, key: str = "") -> np.ndarray:
@@ -2038,6 +2134,18 @@ def _new_bytes(n: int):
 
 
 _tls = threading.local()
+
+
+_CLASSIFY_NAME, _REGRESS_NAME = "tensorflow/serving/classify", "tensorflow/serving/regress"   # TF's signature_constants
+
+
+def _method_kind(method) -> int:
+    """RESP_CLASSIFY / RESP_REGRESS of a MultiInference task's method name; ValueError for any other."""
+    if method == _CLASSIFY_NAME:
+        return N.RESP_CLASSIFY
+    if method == _REGRESS_NAME:
+        return N.RESP_REGRESS
+    raise ValueError(f"method {method!r} is neither {_CLASSIFY_NAME!r} nor {_REGRESS_NAME!r}")
 
 
 def get_codec(device: int = 0) -> Codec:

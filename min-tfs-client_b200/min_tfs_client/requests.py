@@ -14,7 +14,7 @@ The reference's other three calls are kept as well (requests.py:67-110).  They a
 ``Input{example_list}`` those RPCs define - one ``tf.Example`` per row of ``input_dict`` - and call
 ``PredictionService/Classify`` and ``/Regress``.
 """
-from typing import Dict, Optional
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -24,7 +24,11 @@ from .tensors import WireTensor
 PREDICT_METHOD = "/tensorflow.serving.PredictionService/Predict"
 CLASSIFY_METHOD = "/tensorflow.serving.PredictionService/Classify"
 REGRESS_METHOD = "/tensorflow.serving.PredictionService/Regress"
+MULTI_INFERENCE_METHOD = "/tensorflow.serving.PredictionService/MultiInference"
 MODEL_STATUS_METHOD = "/tensorflow.serving.ModelService/GetModelStatus"
+# the method names of a MultiInference task (TF's signature_constants CLASSIFY_METHOD_NAME / REGRESS_METHOD_NAME)
+CLASSIFY_METHOD_NAME = "tensorflow/serving/classify"
+REGRESS_METHOD_NAME = "tensorflow/serving/regress"
 
 
 def examples_from_input_dict(input_dict: Dict[str, np.ndarray]):
@@ -94,6 +98,45 @@ def examples_with_context_from_input_dict(input_dict: Dict[str, np.ndarray], con
         else:
             _fill_feature(feat, k, np.asarray(v))
     return inp
+
+
+def _checked_tasks(tasks) -> List[Tuple[str, str]]:
+    """The MultiInference tasks ``[(signature_name, method_name), ...]`` with None signatures as "" and bytes ones decoded;
+    ValueError for no task or a method name other than CLASSIFY_METHOD_NAME / REGRESS_METHOD_NAME."""
+    out = []
+    for sig, method in tasks:
+        if method not in (CLASSIFY_METHOD_NAME, REGRESS_METHOD_NAME):
+            raise ValueError(f"task method {method!r} is neither {CLASSIFY_METHOD_NAME!r} nor {REGRESS_METHOD_NAME!r}")
+        out.append(("" if sig is None else sig.decode("utf-8") if isinstance(sig, bytes) else str(sig), method))
+    if not out:
+        raise ValueError("a MultiInferenceRequest needs at least one task")
+    return out
+
+
+def make_multi_inference_request(model_name: str, model_version: Optional[int], tasks: Sequence[Tuple[str, str]],
+                                 input_dict: Dict[str, np.ndarray], context_dict=None):
+    """``MultiInferenceRequest`` (inference.proto) running every task ``(signature_name, method_name)`` of the model over one
+    Input: ``examples_from_input_dict(input_dict)``, or with ``context_dict`` ``examples_with_context_from_input_dict``.  Each
+    task's model_spec names the model, the version (when not None) and the signature (an empty or None one: not set, the server's
+    default); its method_name is ``CLASSIFY_METHOD_NAME`` or ``REGRESS_METHOD_NAME`` (anything else raises ValueError, as does an
+    empty task list).  What ``Codec.encode_example_requests(..., tasks=...)`` encodes on the GPU."""
+    from tensorflow_serving.apis.inference_pb2 import MultiInferenceRequest
+
+    req = MultiInferenceRequest()
+    for sig, method in _checked_tasks(tasks):
+        t = req.tasks.add()
+        t.model_spec.SetInParent()
+        t.model_spec.name = model_name
+        if model_version is not None:
+            t.model_spec.version.value = model_version
+        if sig:
+            t.model_spec.signature_name = sig
+        t.method_name = method
+    if context_dict is None:
+        req.input.CopyFrom(examples_from_input_dict(input_dict))
+    else:
+        req.input.CopyFrom(examples_with_context_from_input_dict(input_dict, context_dict))
+    return req
 
 
 class PredictResponseView:
@@ -226,6 +269,15 @@ def gpu_predict_examples_serializer(request) -> bytes:
     return get_codec().encode_example_requests([(model_name, model_version, input_dict, context_dict)], predict_input=input_key)[0]
 
 
+def gpu_multi_inference_request_serializer(request) -> bytes:
+    """``request_serializer`` for ``channel.unary_unary(MULTI_INFERENCE_METHOD, ...)``: (model_name, model_version, tasks,
+    input_dict[, context_dict]) -> the bytes of ``make_multi_inference_request(...).SerializeToString(deterministic=True)``,
+    packed on the GPU."""
+    model_name, model_version, tasks, input_dict = request[:4]
+    context_dict = request[4] if len(request) > 4 else None
+    return get_codec().encode_example_requests([(model_name, model_version, input_dict, context_dict)], tasks=tasks)[0]
+
+
 def gpu_response_deserializer(wire: bytes) -> PredictResponseView:
     """``response_deserializer`` for ``channel.unary_unary``: bytes -> lazy response view."""
     return PredictResponseView(wire)
@@ -296,6 +348,18 @@ class TensorServingClient:
         call = self._channel.unary_unary(REGRESS_METHOD, request_serializer=RegressionRequest.SerializeToString,
                                          response_deserializer=RegressionResponse.FromString)
         return call(self._make_example_request(RegressionRequest, model_name, input_dict, model_version, context_dict), timeout)
+
+    def multi_inference_request(self, model_name: str, input_dict: Dict[str, np.ndarray], tasks: Sequence[Tuple[str, str]],
+                                timeout: int = 60, model_version: Optional[int] = None, context_dict=None):
+        """``PredictionService/MultiInference``: every task ``(signature_name, method_name)`` of the model - method_name
+        ``CLASSIFY_METHOD_NAME`` or ``REGRESS_METHOD_NAME`` - over one Input, one example per row of ``input_dict`` (with
+        ``context_dict``: an ExampleListWithContext), the request bytes packed on the GPU.  Returns a ``MultiInferenceResponse``
+        (``Codec.decode_multi_inference_responses`` decodes a batch of them on the GPU)."""
+        from tensorflow_serving.apis.inference_pb2 import MultiInferenceResponse
+
+        call = self._channel.unary_unary(MULTI_INFERENCE_METHOD, request_serializer=gpu_multi_inference_request_serializer,
+                                         response_deserializer=MultiInferenceResponse.FromString)
+        return call((model_name, model_version, tasks, input_dict, context_dict), timeout)
 
     def model_status_request(self, model_name: str, model_version: Optional[int] = None, timeout: Optional[int] = 10):
         """``ModelService/GetModelStatus`` as the reference issues it (requests.py:99-110: the version is set only when truthy)."""

@@ -20,6 +20,7 @@ and, for the client's other RPCs (reference requests.py:67-110), host-side messa
   tensorflow/core/example/{feature,example}.proto        tf.Example
   tensorflow_serving/apis/input.proto                    Input{ExampleList}
   tensorflow_serving/apis/{classification,regression}.proto
+  tensorflow_serving/apis/inference.proto                MultiInference{Request,Response}
   tensorflow_serving/apis/get_model_status.proto, tensorflow_serving/util/status.proto,
   tensorflow/core/{lib/core,protobuf}/error_codes.proto
 
@@ -256,6 +257,25 @@ def build_files():
     rs = fd.message_type.add(name="RegressionResponse")
     _field(rs, "model_spec", 2, "msg:.tensorflow.serving.ModelSpec")
     _field(rs, "result", 1, "msg:.tensorflow.serving.RegressionResult")
+    files.append(fd)
+
+    # ---- inference.proto (MultiInference: several Classify / Regress signatures over one Input) -----
+    fd = dpb.FileDescriptorProto(name="tensorflow_serving/apis/inference.proto", package="tensorflow.serving", syntax="proto3",
+                                 dependency=["tensorflow_serving/apis/classification.proto", "tensorflow_serving/apis/input.proto",
+                                             "tensorflow_serving/apis/model.proto", "tensorflow_serving/apis/regression.proto"])
+    it = fd.message_type.add(name="InferenceTask")
+    _field(it, "model_spec", 1, "msg:.tensorflow.serving.ModelSpec")
+    _field(it, "method_name", 2, "string")
+    ir = fd.message_type.add(name="InferenceResult")
+    ir.oneof_decl.add(name="result")
+    _field(ir, "model_spec", 1, "msg:.tensorflow.serving.ModelSpec")
+    _field(ir, "classification_result", 2, "msg:.tensorflow.serving.ClassificationResult", oneof=0)
+    _field(ir, "regression_result", 3, "msg:.tensorflow.serving.RegressionResult", oneof=0)
+    mq = fd.message_type.add(name="MultiInferenceRequest")
+    _field(mq, "tasks", 1, "msg:.tensorflow.serving.InferenceTask", repeated=True)
+    _field(mq, "input", 2, "msg:.tensorflow.serving.Input")
+    ms = fd.message_type.add(name="MultiInferenceResponse")
+    _field(ms, "results", 1, "msg:.tensorflow.serving.InferenceResult", repeated=True)
     files.append(fd)
 
     # ---- error_codes.proto (x2: lib/core re-exports protobuf/) / status.proto / get_model_status.proto ----
