@@ -963,6 +963,60 @@ int b200tfs_encode_example_tasks_host(b200tfs_ctx* ctx, int32_t n, const b200tfs
                                       const b200tfs_example_tasks* tasks, void* wire_host, uint64_t wire_cap, uint64_t* rec_off,
                                       uint64_t* rec_len);
 
+/* SequenceExamples (tensorflow.SequenceExample, example.proto): the input of a model exported with a tf.io.parse_sequence_example
+ * serving input - session and event-history models, TF-Ranking's SequenceExample format.  One entry per request, parallel to reqs
+ * (sequences == NULL: no request has one).  present == 1 with target kind B200TFS_EXAMPLES_PREDICT_SEQUENCE: the request is
+ *     PredictRequest{model_spec, inputs[key] = TensorProto{dtype: DT_STRING, tensor_shape {dim {size: n}}, string_val:
+ *                    [s.SerializeToString(deterministic=True) for s in the n = n_examples sequences]}}
+ * serialised with SerializeToString(deterministic=True) - the PREDICT_STRING prefix, sequences in place of examples:
+ *     42 vi(S) 0A vi(C) {context map entries} 12 vi(G) {0A vi(e) 0A vi(klen) key 12 vi(FL) {0A vi(feat) Feature}*}*
+ * The request's first n_context features are context features: sequence i's context holds them exactly as example i would (row
+ * i, B200TFS_F_BROADCAST rows repeated, b200tfs_ragged and b200tfs_bytes entries as for an example), listed in `order`.  The
+ * other features are feature lists, in `order` as well: each needs a b200tfs_ragged entry whose max_len is its step count T and
+ * whose unit is the elements of one step (row_elems == T * unit).  With lengths == NULL every sequence has T steps, otherwise
+ * sequence i has lengths[i] (a length outside [0, T] is B200TFS_E_SHAPE, host lengths before any launch, device ones in
+ * b200tfs_encode_results).  Step t of sequence i is one Feature (a FeatureList entry, tag 0A) of elements [t * unit, (t + 1) *
+ * unit) of row i, converted as an example's values are; a bytes list's row is strings [i * row_elems, (i + 1) * row_elems) under
+ * the offsets rule of b200tfs_bytes with l_i = lengths[i] * unit.  A list of 0 steps still has its map entry, a step of 0
+ * elements still writes its empty list, and a sequence of no features is 42 04 0A 00 12 00.  A call may mix sequence requests
+ * with every other kind; sequence requests have their own count and emit kernels, and calls without one launch what they did.
+ * Refused before the context is looked at (B200TFS_E_ARG): present not 0 or 1; present == 1 on another kind, PREDICT_SEQUENCE
+ * without present == 1; a sequence request with a present context or with tasks; n_context outside [0, n_features]; a feature
+ * list with B200TFS_F_BROADCAST, without a ragged entry (ragged == NULL), with a negative max_len or unit, unknown ragged flags,
+ * unaligned lengths or row_elems != max_len * unit.  T over 2 GiB, or a request that cannot stay under 2 GiB: B200TFS_E_TOOBIG. */
+#define B200TFS_EXAMPLES_PREDICT_SEQUENCE 3
+typedef struct b200tfs_example_sequence {
+  int32_t present;                   /* 0: not a sequence request; 1: one                                                        */
+  int32_t n_context;                 /* features [0, n_context) of the request are context features, the rest feature lists      */
+} b200tfs_example_sequence;
+/* b200tfs_example_tasks_request_size with sequences (sequence == NULL: that call itself).  The exact length in closed form when no
+ * integer or bytes column and no ragged entry with lengths appears in the request (B200TFS_E_ARG otherwise).                  */
+int b200tfs_example_sequences_request_size(const b200tfs_example_request* r, const b200tfs_example_target* target,
+                                           const b200tfs_example_context* context, const b200tfs_example_tasks* tasks,
+                                           const b200tfs_ragged* ragged, const b200tfs_example_sequence* sequence, uint64_t* total_len);
+/* b200tfs_example_tasks_arena_size with sequences and their ragged entries (both NULL: that call itself).  A sequence's slot takes
+ * its worst case, whatever the values and lengths: T steps of each list, 10 bytes per integer element, data_len + 11 per
+ * string, plus the step headers - so one captured graph serves any values, lengths and offsets.                             */
+int b200tfs_example_sequences_arena_size(int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                         const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                         const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                         const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
+                                         uint64_t* bytes_out);
+/* b200tfs_encode_example_tasks_{async,host} with sequences (sequences == NULL: those calls themselves, which call these).  A call
+ * with a sequence request launches ex_seq_count_kernel over its sequences (one warp each: the context, then every step of every
+ * list; an integer or bytes step's payload goes to a per-step scratch column sized from n and T alone), the unchanged scan over
+ * every tile, and ex_emit_sequence_kernel over its spans; the frame kernel writes its prefix as PREDICT_STRING's.           */
+int b200tfs_encode_example_sequences_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                           const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                           const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                           const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
+                                           void* arena_dev, uint64_t arena_cap);
+int b200tfs_encode_example_sequences_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                          const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                          const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                          const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
+                                          void* wire_host, uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
+
 /* ---- Classify / Regress responses: a batch of responses into one value or score array ----------------------
  * What ClassificationResponse.FromString / RegressionResponse.FromString followed by a loop over the result give, concatenated
  * along the example axis across the n responses: row order is response 0's examples, then response 1's, and so on.

@@ -14,6 +14,8 @@
 //                    a Predict string_val, plan.h ExReq), rec_off / rec_len / status to pinned memory.  A call with contexts
 //                    (ExampleListWithContext, plan.h ExCtxRef) runs ex_frame_context_kernel instead, whose warp also writes its
 //                    request's context behind the examples; count and scan size the contexts as one-example entries
+//   ex_seq_count_kernel, ex_emit_sequence_kernel   SequenceExample requests (plan.h sq_*), only in a call that has one: their
+//                    tiles and spans follow all the others; the scan and frame kernels take them as they take examples
 //
 // count, emit and the example writer take an ExMode: a call with a bytes column launches the kExColumns instantiations, a call
 // with a ragged numeric column (and none of bytes) the kExRagged ones, in which a ragged column's row ends after ex_elems
@@ -275,6 +277,228 @@ __global__ void __launch_bounds__(kExTile) ex_count_kernel(const __grid_constant
   if (threadIdx.x == 0) T.tile_sum[blockIdx.x] = total;
 }
 
+// ---- SequenceExamples (plan.h sq_*): a request's sequences take the place of its examples ----
+// steps of sequence i of feature list f: a length clamped to [0, T] (the count kernel flags one that was not), or T
+__device__ __forceinline__ uint64_t sq_steps(const ExFeat& f, uint64_t i) {
+  if (!f.lengths) return f.max_len;
+  const int64_t l = f.lengths[i];
+  return l < 0 ? 0ull : min((uint64_t)l, f.max_len);
+}
+// ex_str_ends over strings j0 .. min(j0 + 32, ne) - 1 of a step whose last string is ne - 1: *carry moves on to the end of that
+// last string, not to hi, so that the next step starts where this one ends
+__device__ __forceinline__ uint64_t sq_str_ends(const ExFeat& f, uint64_t b, uint64_t ne, uint64_t j0, uint64_t lo, uint64_t hi,
+                                                uint64_t* carry, uint64_t* start) {
+  const uint64_t e = ex_str_ends(f, b, ne, j0, lo, hi, carry, start);
+  *carry = __shfl_sync(0xFFFFFFFFu, e, (uint32_t)min(ne - j0, (uint64_t)32) - 1);
+  return e;
+}
+// the list payload of step t of sequence i of list f (float: closed form; integer and bytes: the count kernel's)
+__device__ __forceinline__ uint64_t sq_payload(const ExTables& T, const ExReq& q, const ExFeat& f, uint64_t i, uint64_t t) {
+  return f.op < EXO_INT ? 4 * f.unit : T.L[q.L0 + i * q.n_int + f.lcol + t];
+}
+// the bytes of sequence i's steps of list f, by the whole warp
+__device__ __forceinline__ uint64_t sq_list_len(const ExTables& T, const ExReq& q, const ExFeat& f, uint64_t i) {
+  const uint64_t steps = sq_steps(f, i);
+  if (f.op < EXO_INT) return steps * sq_step_len(4 * f.unit, false);
+  uint64_t s = 0;
+  for (uint64_t t = threadIdx.x & 31; t < steps; t += 32) s += sq_step_len(sq_payload(T, q, f, i, t), f.op == EXO_BYTES);
+  return warp_sum64(s);
+}
+
+// One warp per sequence: the context as ex_count_kernel counts an example's features, and every step of every list, whose
+// integer or bytes payload goes to its L column; a length or an offset out of range flags the request.
+__global__ void __launch_bounds__(kExTile) ex_seq_count_kernel(const __grid_constant__ ExTables T) {
+  __shared__ unsigned long long warp_sum[kExTile / 32];
+  const ExSpan sp = T.tiles[blockIdx.x];
+  const ExReq q = T.reqs[sp.req];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  uint64_t mine = 0;
+  for (uint64_t i = sp.e0 + warp; i < sp.e1; i += kExTile / 32) {
+    uint64_t C = 0, G = 0, hl;
+    for (uint32_t k = 0; k < q.n_feat; ++k) {
+      const ExFeat f = T.feats[q.first_feat + k];
+      if (f.lengths && lane == 0) {      // compared, never multiplied: 2^62 must not wrap into range
+        const int64_t l = f.lengths[i];
+        if (l < 0 || (uint64_t)l > f.max_len) T.bad[sp.req] = 1;
+      }
+      uint64_t* L = T.L + q.L0 + i * q.n_int + f.lcol;
+      if (k < q.n_ctx) {
+        const uint64_t ne = ex_elems<kExColumns>(f, i);
+        uint64_t P = 4 * ne;
+        if (f.op == EXO_BYTES) {
+          P = ex_count_bytes(T, sp.req, f, i, ne);
+          if (lane == 0) *L = P;
+        } else if (f.op >= EXO_INT) {
+          const uint8_t* row = f.data + i * f.row_stride;
+          uint64_t s = 0;
+          for (uint64_t j = lane; j < ne; j += 32) s += vlen64(ex_int(f, row + j * f.esz));
+          P = warp_sum64(s);
+          if (lane == 0) *L = P;
+        }
+        C += ex_feat_entry_len<kExColumns>(f, P, &hl);
+        continue;
+      }
+      const uint64_t steps = sq_steps(f, i), b = i * f.row_stride;
+      uint64_t FL = 0;
+      if (f.op < EXO_INT) {
+        FL = steps * sq_step_len(4 * f.unit, false);
+      } else if (f.op == EXO_BYTES) {      // ex_count_bytes over the sequence's row, one step after the other
+        uint64_t lo, hi, carry;
+        ex_row_bounds(f, b, &lo, &hi);
+        carry = lo;
+        bool bad = false;
+        for (uint64_t t = 0; t < steps; ++t) {
+          const uint64_t ne = (t + 1) * f.unit;
+          uint64_t P = 0;
+          for (uint64_t j0 = t * f.unit; j0 < ne; j0 += 32) {
+            uint64_t s;
+            const uint64_t e = sq_str_ends(f, b, ne, j0, lo, hi, &carry, &s), j = j0 + lane;
+            if (j < ne) {
+              P += string_value_len(e - s);
+              bad |= f.offsets[b + j + 1] < f.offsets[b + j];
+            }
+          }
+          P = warp_sum64(P);
+          if (lane == 0) L[t] = P;
+          FL += sq_step_len(P, true);
+        }
+        if (lane == 0) {
+          const int64_t o0 = f.offsets[b], on = f.offsets[b + steps * f.unit], nx = f.offsets[b + f.row_elems];
+          bad |= o0 < 0 || on > nx || nx > (int64_t)f.data_len;
+        }
+        if (__any_sync(0xFFFFFFFFu, bad) && lane == 0) T.bad[sp.req] = 1;
+      } else {
+        const uint8_t* row = f.data + b;
+        for (uint64_t t = 0; t < steps; ++t) {
+          uint64_t s = 0;
+          for (uint64_t j = t * f.unit + lane; j < (t + 1) * f.unit; j += 32) s += vlen64(ex_int(f, row + j * f.esz));
+          const uint64_t P = warp_sum64(s);
+          if (lane == 0) L[t] = P;
+          FL += sq_step_len(P, false);
+        }
+      }
+      G += sq_list_entry_len(FL, f.key_len);
+    }
+    const uint64_t S = sq_sequence_len(C, G);
+    if (lane == 0) { T.S[q.ex0 + i] = S; mine += S; }
+  }
+  uint64_t total = 0;
+  concat_scan(mine, total, warp_sum);
+  if (threadIdx.x == 0) T.tile_sum[blockIdx.x] = total;
+}
+
+// Sequence i of request q, written by the calling warp at w behind the tag 42.  The context is written by ex_write_example as an
+// example of the context features, placed so that its `0A vi(C) entries` lands where the sequence has them: the example's own
+// tag and length then lie inside the sequence's `42 vi(S)`, which lane 0 writes over them afterwards.
+__device__ void ex_write_sequence(const ExTables& T, const ExReq& q, uint64_t i, uint8_t* w) {
+  const uint32_t lane = threadIdx.x & 31;
+  uint64_t C = 0, G = 0, hl;
+  for (uint32_t c = 0; c < q.n_ctx; c += 32) {
+    uint64_t e = 0;
+    if (c + lane < q.n_ctx) {
+      const ExFeat& f = T.feats[q.first_feat + c + lane];
+      e = ex_feat_entry_len<kExColumns>(f, ex_payload<kExColumns>(T, q, f, i), &hl);
+    }
+    C += warp_sum64(e);
+  }
+  for (uint32_t k = q.n_ctx; k < q.n_feat; ++k) {
+    const ExFeat& f = T.feats[q.first_feat + k];
+    G += sq_list_entry_len(sq_list_len(T, q, f, i), f.key_len);
+  }
+  const uint64_t X = 1 + varint_len(C) + C + 1 + varint_len(G) + G, ctx_at = 1 + varint_len(X);
+  ExReq qc = q;
+  qc.n_feat = q.n_ctx;
+  const uint64_t xc = 1 + varint_len(C) + C;             // the context example's X
+  ex_write_example<kExColumns, 0x42>(T, qc, i, w + ctx_at - (1 + varint_len(xc)));
+  uint64_t pos = ctx_at + xc;
+  if (lane == 0) {
+    w[0] = 0x42;
+    put_varint(w + 1, X);
+    w[pos] = 0x12;
+    put_varint(w + pos + 1, G);
+  }
+  pos += 1 + varint_len(G);
+  for (uint32_t k = q.n_ctx; k < q.n_feat; ++k) {
+    const ExFeat f = T.feats[q.first_feat + k];
+    const bool str = f.op == EXO_BYTES;
+    const uint64_t FL = sq_list_len(T, q, f, i), steps = sq_steps(f, i);
+    const uint64_t e = 1 + varint_len(f.key_len) + f.key_len + 1 + varint_len(FL) + FL;
+    uint8_t* h = w + pos;        // 0A vi(e) 0A vi(klen) key 12 vi(FL)
+    const uint32_t kat = 2 + varint_len(e) + varint_len(f.key_len);
+    for (uint32_t b = lane; b < f.key_len; b += 32) h[kat + b] = T.blob[f.key_off + b];
+    if (lane == 0) {
+      h[0] = 0x0A; put_varint(h + 1, e);
+      h[kat - 1 - varint_len(f.key_len)] = 0x0A; put_varint(h + kat - varint_len(f.key_len), f.key_len);
+      h[kat + f.key_len] = 0x12; put_varint(h + kat + f.key_len + 1, FL);
+    }
+    pos += kat + f.key_len + 1 + varint_len(FL);
+    const uint8_t* row = f.data + i * f.row_stride;
+    if (f.op < EXO_INT) {        // every step the same size: headers one per lane, then the values one per lane
+      const uint64_t P = 4 * f.unit, list = P ? 1 + varint_len(P) + P : 0, feat = 1 + varint_len(list) + list;
+      const uint64_t sl = 1 + varint_len(feat) + feat, hd = sl - P;
+      for (uint64_t t = lane; t < steps; t += 32) {     // 0A vi(feat) 12 vi(list) [0A vi(P)]
+        uint8_t* s = w + pos + t * sl;
+        *s++ = 0x0A; s += put_varint(s, feat);
+        *s++ = 0x12; s += put_varint(s, list);
+        if (P) { *s++ = 0x0A; put_varint(s, P); }
+      }
+      for (uint64_t j = lane; j < steps * f.unit; j += 32) {
+        const uint64_t t = j / f.unit;
+        const uint32_t v = ex_float_bits(f, row, j);
+        uint8_t* d = w + pos + t * sl + hd + 4 * (j - t * f.unit);
+        d[0] = (uint8_t)v; d[1] = (uint8_t)(v >> 8); d[2] = (uint8_t)(v >> 16); d[3] = (uint8_t)(v >> 24);
+      }
+      pos += steps * sl;
+      continue;
+    }
+    uint64_t lo = 0, hi = 0, carry = 0;
+    const uint64_t b = i * f.row_stride;
+    if (str) { ex_row_bounds(f, b, &lo, &hi); carry = lo; }
+    for (uint64_t t = 0; t < steps; ++t) {     // one step after the other, by the whole warp
+      const uint64_t P = sq_payload(T, q, f, i, t), list = str ? P : P ? 1 + varint_len(P) + P : 0, feat = 1 + varint_len(list) + list;
+      uint8_t* s = w + pos;
+      const uint32_t hd = 1 + varint_len(feat) + (str ? 1 + varint_len(P) : P ? 2 + varint_len(list) + varint_len(P) : 1 + varint_len(list));
+      if (lane == 0) {         // 0A vi(feat) {0A vi(P) | 1A vi(list) [0A vi(P)]}
+        s[0] = 0x0A;
+        uint32_t p = 1 + put_varint(s + 1, feat);
+        s[p++] = str ? 0x0A : 0x1A;
+        p += put_varint(s + p, str ? P : list);
+        if (!str && P) { s[p++] = 0x0A; put_varint(s + p, P); }
+      }
+      uint8_t* d = s + hd;
+      uint64_t base = 0;
+      const uint64_t ne = (t + 1) * f.unit;
+      for (uint64_t j0 = t * f.unit; j0 < ne; j0 += 32) {
+        const uint64_t j = j0 + lane;
+        uint64_t sz = 0, len = 0, st = 0, v = 0;
+        if (str) {
+          const uint64_t en = sq_str_ends(f, b, ne, j0, lo, hi, &carry, &st);
+          len = j < ne ? en - st : 0;
+          sz = j < ne ? string_value_len(len) : 0;
+        } else if (j < ne) {
+          v = ex_int(f, row + j * f.esz);
+          sz = vlen64(v);
+        }
+        uint64_t incl = sz;
+#pragma unroll
+        for (int dd = 1; dd < 32; dd <<= 1) {
+          const uint64_t x = __shfl_up_sync(0xFFFFFFFFu, incl, dd);
+          if (lane >= (uint32_t)dd) incl += x;
+        }
+        uint8_t* o = d + base + incl - sz;
+        if (str) {
+          if (sz) { *o++ = 0x0A; o += put_varint(o, len); }
+          warp_copy_strings(o, f.data + st, len, sz != 0, UINT64_MAX);
+        } else if (sz) {
+          put_varint(o, v);
+        }
+        base += __shfl_sync(0xFFFFFFFFu, incl, 31);
+      }
+      pos += 1 + varint_len(feat) + feat;
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kExTile) ex_scan_kernel(const __grid_constant__ ExTables T) {
   __shared__ unsigned long long warp_sum[kExTile / 32];
   const uint32_t t = blockIdx.x;
@@ -317,7 +541,14 @@ __device__ __forceinline__ void ex_flush(uint8_t* arena, const uint8_t* img, uin
   for (uint64_t x = b + threadIdx.x; x < hi; x += blockDim.x) arena[x] = img[x - ws];
 }
 
-template <int kMode, uint8_t kTag>
+// example i, or with kSeq sequence i, of request q at w
+template <int kMode, uint8_t kTag, bool kSeq>
+__device__ __forceinline__ void ex_write_record(const ExTables& T, const ExReq& q, uint64_t i, uint8_t* w) {
+  if constexpr (kSeq) ex_write_sequence(T, q, i, w);
+  else ex_write_example<kMode, kTag>(T, q, i, w);
+}
+
+template <int kMode, uint8_t kTag, bool kSeq = false>
 __device__ __forceinline__ void ex_emit(const ExTables& T) {
   __shared__ __align__(16) uint8_t img[kExStage + 16];
   __shared__ uint64_t next;
@@ -344,7 +575,7 @@ __device__ __forceinline__ void ex_emit(const ExTables& T) {
     __syncthreads();
     const uint64_t j = next;
     if (j > i) {
-      for (uint64_t e = i + warp; e < j; e += kWarps) ex_write_example<kMode, kTag>(T, q, e, img + (A + ex_start<kMode>(T, q, e) - ws));
+      for (uint64_t e = i + warp; e < j; e += kWarps) ex_write_record<kMode, kTag, kSeq>(T, q, e, img + (A + ex_start<kMode>(T, q, e) - ws));
       __syncthreads();
       const uint64_t be = A + ex_end<kMode>(T, q, j - 1), cut = be & ~15ull;
       if (cut > ws) {                        // store every whole vector; the partial one moves to the front of the image
@@ -357,7 +588,7 @@ __device__ __forceinline__ void ex_emit(const ExTables& T) {
       i = j;
     } else {                                 // example i alone is larger than the image: one warp writes it in place
       ex_flush(T.arena, img, ws, lo, A + ex_start<kMode>(T, q, i));
-      if (warp == 0) ex_write_example<kMode, kTag>(T, q, i, T.arena + A + ex_start<kMode>(T, q, i));
+      if (warp == 0) ex_write_record<kMode, kTag, kSeq>(T, q, i, T.arena + A + ex_start<kMode>(T, q, i));
       lo = A + ex_end<kMode>(T, q, i);
       ws = lo & ~15ull;
       ++i;
@@ -375,6 +606,10 @@ __global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_co
 template <int kMode>
 __global__ void __launch_bounds__(kExEmitThreads) ex_emit_predict_kernel(const __grid_constant__ ExTables T) {
   ex_emit<kMode, 0x42>(T);
+}
+// the spans of the SequenceExample requests, which are always counted (kExColumns places them through off and S)
+__global__ void __launch_bounds__(kExEmitThreads) ex_emit_sequence_kernel(const __grid_constant__ ExTables T) {
+  ex_emit<kExColumns, 0x42, true>(T);
 }
 
 constexpr uint32_t kExFrameWarps = 4;
@@ -457,14 +692,26 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_context_kernel(co
   else if (lane == 0) { w[0] = 0x12; w[1] = 0; }                 // context.SetInParent(): no features map at all
 }
 
-cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t stream, uint32_t* launched, const ExCtxRef* ctx) {
+// n_seq_tiles / n_seq_spans: the count tiles and emit spans of the SequenceExample requests, behind T's n_tiles and n_spans
+cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t stream, uint32_t* launched, const ExCtxRef* ctx,
+                                    uint32_t n_seq_tiles, uint32_t n_seq_spans) {
   *launched = 0;
   if (T.n_tiles) {
     if (mode == kExColumns) ex_count_kernel<kExColumns><<<T.n_tiles, kExTile, 0, stream>>>(T);
     else if (mode == kExRagged) ex_count_kernel<kExRagged><<<T.n_tiles, kExTile, 0, stream>>>(T);
     else ex_count_kernel<kExDense><<<T.n_tiles, kExTile, 0, stream>>>(T);
-    ex_scan_kernel<<<T.n_tiles, kExTile, 0, stream>>>(T);
-    *launched += 2;
+    *launched += 1;
+  }
+  if (n_seq_tiles) {
+    ExTables Q = T;
+    Q.tiles += T.n_tiles;
+    Q.tile_sum += T.n_tiles;
+    ex_seq_count_kernel<<<n_seq_tiles, kExTile, 0, stream>>>(Q);
+    *launched += 1;
+  }
+  if (T.n_tiles + n_seq_tiles) {      // the scan sees every tile: a request's tiles are contiguous, its first_tile global
+    ex_scan_kernel<<<T.n_tiles + n_seq_tiles, kExTile, 0, stream>>>(T);
+    *launched += 1;
   }
   const uint32_t n_list = T.n_spans - T.n_predict_spans;
   if (n_list) {
@@ -479,6 +726,12 @@ cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t st
     if (mode == kExColumns) ex_emit_predict_kernel<kExColumns><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
     else if (mode == kExRagged) ex_emit_predict_kernel<kExRagged><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
     else ex_emit_predict_kernel<kExDense><<<T.n_predict_spans, kExEmitThreads, 0, stream>>>(P);
+    *launched += 1;
+  }
+  if (n_seq_spans) {          // and those of the SequenceExample requests behind them
+    ExTables Q = T;
+    Q.spans += T.n_spans;
+    ex_emit_sequence_kernel<<<n_seq_spans, kExEmitThreads, 0, stream>>>(Q);
     *launched += 1;
   }
   if (T.n_req) {

@@ -422,8 +422,9 @@ struct ExReq {
   uint64_t fixed_size;                  // bytes of every example in the example_list (its tag included); 0: the size depends on
                                         // the values (an integer or a ragged column), S and off hold each example's
   uint64_t anchor, slot_end;            // arena offsets: where example 0 starts, where the slot ends
-  uint32_t mid_len, head_len, inner_tag, pad;   // the Predict prefix above (example_list: 0, 0, 0A); last, because among the
+  uint32_t mid_len, head_len, inner_tag;        // the Predict prefix above (example_list: 0, 0, 0A); last, because among the
                                                 // fields the emit kernel reads they cost ex_emit_kernel<false> 12 registers
+  uint32_t n_ctx;                               // a SequenceExample request: its first n_ctx features (wire order) are context
 };
 struct ExSpan { uint32_t req, pad; uint64_t e0, e1; };   // a CTA's examples [e0, e1) of request `req`
 // A call with contexts (ExampleListWithContext) plans each present context as one more request entry of one example, at an
@@ -468,6 +469,28 @@ B2_PLAN_HD uint64_t ex_bytes_entry_len(uint64_t P, uint64_t klen, uint64_t* hl) 
 // {0A | 42} vi(X) 0A vi(F) entries
 B2_PLAN_HD uint64_t ex_example_len(uint64_t F) {
   const uint64_t x = 1 + varint_len(F) + F;
+  return 1 + varint_len(x) + x;
+}
+
+// ---- SequenceExamples (PREDICT_SEQUENCE requests; ex_seq_count_kernel, ex_emit_sequence_kernel) -------------------------
+// A sequence request is one ExReq whose features [0, n_ctx) are context features (an example's, in wire order) and the rest
+// feature lists, each an ExFeat with max_len = T steps of `unit` elements (row_elems = T * unit; lengths: sequence i has
+// min(max(lengths[i], 0), T) steps, NULL: T).  An integer or bytes list takes T columns of ExTables::L from lcol on, one per step:
+// the step's list payload.  Sequence requests are always counted; their count tiles and emit spans follow all the others.
+//   42 vi(S) 0A vi(C) {context map entries} 12 vi(G) {0A vi(e) 0A vi(klen) key 12 vi(FL) {0A vi(feat) Feature}*}*
+// One step (its 0A tag included) whose Feature holds a list of payload P (bytes: P bytes of {0A vi(len) bytes} fields)
+B2_PLAN_HD uint64_t sq_step_len(uint64_t P, bool bytes) {
+  const uint64_t list = bytes ? P : P ? 1 + varint_len(P) + P : 0, feature = 1 + varint_len(list) + list;
+  return 1 + varint_len(feature) + feature;
+}
+// the FeatureLists map entry (its tag included) of a list whose steps take FL bytes
+B2_PLAN_HD uint64_t sq_list_entry_len(uint64_t FL, uint64_t klen) {
+  const uint64_t e = 1 + varint_len(klen) + klen + 1 + varint_len(FL) + FL;
+  return 1 + varint_len(e) + e;
+}
+// a sequence in the string_val (tag 42 included) whose context entries take C bytes and list entries G
+B2_PLAN_HD uint64_t sq_sequence_len(uint64_t C, uint64_t G) {
+  const uint64_t x = 1 + varint_len(C) + C + 1 + varint_len(G) + G;
   return 1 + varint_len(x) + x;
 }
 

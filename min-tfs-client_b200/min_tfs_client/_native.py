@@ -140,7 +140,7 @@ class Bytes(C.Structure):
     _fields_ = [("offsets", C.c_void_p), ("data_len", C.c_int64), ("flags", C.c_uint32), ("pad_", C.c_int32)]
 
 
-EXAMPLES_LIST, EXAMPLES_PREDICT_STRING, EXAMPLES_PREDICT_ELWC = 0, 1, 2
+EXAMPLES_LIST, EXAMPLES_PREDICT_STRING, EXAMPLES_PREDICT_ELWC, EXAMPLES_PREDICT_SEQUENCE = 0, 1, 2, 3
 
 
 class ExampleTarget(C.Structure):
@@ -164,6 +164,12 @@ class InferenceTask(C.Structure):
 class ExampleTasks(C.Structure):
     """b200tfs_example_tasks: the tasks of one request (n_tasks 0: not a MultiInferenceRequest)."""
     _fields_ = [("tasks", C.c_void_p), ("n_tasks", C.c_int32), ("pad_", C.c_int32)]
+
+
+class ExampleSequence(C.Structure):
+    """b200tfs_example_sequence: one request's SequenceExamples (present 0: none; 1: its first ``n_context`` features are
+    context features, the rest feature lists whose Ragged entries give their steps), for EXAMPLES_PREDICT_SEQUENCE."""
+    _fields_ = [("present", C.c_int32), ("n_context", C.c_int32)]
 
 
 class PadInput(C.Structure):
@@ -327,6 +333,18 @@ SIGNATURES = {
     "b200tfs_encode_example_tasks_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
                                                     C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
                                                     C.POINTER(ExampleTasks), _vp, C.c_uint64, _u64p, _u64p]),
+    "b200tfs_example_sequences_request_size": (C.c_int, [C.POINTER(ExampleRequest), C.POINTER(ExampleTarget), C.POINTER(ExampleContext),
+                                                         C.POINTER(ExampleTasks), C.POINTER(Ragged), C.POINTER(ExampleSequence), _u64p]),
+    "b200tfs_example_sequences_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                       C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                       C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), _u64p]),
+    "b200tfs_encode_example_sequences_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                         C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                         C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), _vp, C.c_uint64]),
+    "b200tfs_encode_example_sequences_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                        C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                        C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), _vp, C.c_uint64, _u64p,
+                                                        _u64p]),
     "b200tfs_multi_inference_response_bound": (C.c_int, [C.c_int32, _i32p, C.c_int32, _u64p, _u64p, _u64p]),
     "b200tfs_decode_multi_inference_responses": (C.c_int, [_vp, C.c_int32, _i32p, _vp, C.c_int32, _u64p, _u64p, _vpp, _u64p, _vpp,
                                                            _u64p]),

@@ -435,6 +435,28 @@ def _example_columns(input_dict: Mapping, context: bool = False):
     return n, preps
 
 
+def _shape_of(v) -> Tuple[int, ...]:
+    if isinstance(v, (BytesColumn, RaggedColumn)):
+        return tuple(v.shape)
+    return tuple(D.device_view(v)[1]) if D.is_device_object(v) else tuple(np.shape(v))
+
+
+def _sequence_count(context_dict: Mapping, feature_list_dict: Mapping) -> int:
+    """The number of SequenceExamples ``context_dict`` and ``feature_list_dict`` hold: the leading dimension of every non-0-d
+    context value and every feature-list value (ValueError when they disagree, or for a feature-list value of rank < 2, which
+    has no step axis); with no such value 1 when either dict is non-empty, else 0."""
+    rows = set()
+    for k, v in feature_list_dict.items():
+        shape = _shape_of(v)
+        if len(shape) < 2:
+            raise ValueError(f"feature list {k!r}: values have shape [n, T, *inner] (rank >= 2), got {shape}")
+        rows.add(shape[0])
+    rows |= {s[0] for s in map(_shape_of, context_dict.values()) if len(s)}
+    if len(rows) > 1:
+        raise ValueError(f"inputs disagree on the number of sequences: {sorted(rows)}")
+    return rows.pop() if rows else (1 if context_dict or feature_list_dict else 0)
+
+
 def _host_example_request(model_name, model_version, input_dict, grpc_frame: bool, predict_input=None, context_dict=None,
                           tasks=None) -> bytes:
     """A request with a column the device route does not take, as ``examples_from_input_dict`` and protobuf make it: a
@@ -1088,6 +1110,72 @@ class Codec:
             rg = (N.Ragged * len(ragged))(*ragged) if any(g.lengths for g in ragged) else None
             N.check(self._lib.b200tfs_encode_example_tasks_host(self._ctx, m, reqs, rg, bs, tg, ct, cb, tk, wire.ctypes.data, cap.value,
                                                                 off, ln))
+            for j, i in enumerate(dev_idx):
+                out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
+        return out  # type: ignore[return-value]
+
+    def encode_sequence_example_requests(self, requests: Iterable[Tuple], *, input_key, order="deterministic",
+                                         grpc_frame: bool = False) -> List[bytes]:
+        """Each item is ``(model_name, model_version, context_dict, feature_list_dict)``; returns one PredictRequest wire per item
+        for a model that parses serialized tf.SequenceExamples: its one input ``input_key`` is the DT_STRING ``[n]`` tensor of the
+        sequences ``requests.sequence_examples_from_input_dict`` builds, each serialized with ``deterministic=True`` - the bytes of
+        ``make_predict_sequence_examples_request(...).SerializeToString(deterministic=True)``.
+
+        Context values are taken as ``encode_example_requests`` takes input values (row i is sequence i's; 0-d values repeated;
+        ``RaggedColumn`` and ``BytesColumn``).  A feature-list value has shape ``[n, T, *inner]``: a numpy, pinned or device
+        array, a ``BytesColumn``, or a ``RaggedColumn`` of either whose sequence i has ``lengths[i]`` steps (device lengths out of
+        range raise ValueError); step t of sequence i is one Feature of ``value[i, t]``.  ``order="given"`` lists the context and
+        the feature lists in insertion order.  An item with a numpy str / bytes value, or a dtype the device route does not take,
+        is assembled on the host by ``make_predict_sequence_examples_request`` (deterministic order); device arrays of such dtypes
+        raise ValueError."""
+        from .requests import make_predict_sequence_examples_request
+
+        order_code = _ORDER[order] if isinstance(order, str) else int(order)
+        pkey = input_key.encode("utf-8") if isinstance(input_key, str) else bytes(input_key)
+        items = list(requests)
+        out: List[Optional[bytes]] = [None] * len(items)
+        keep, structs, dev_idx, ragged, strs, targets, seqs = [], [], [], [], [], [], []
+        for i, (model_name, model_version, context_dict, feature_list_dict) in enumerate(items):
+            n = _sequence_count(context_dict, feature_list_dict)
+            ccols, lcols = _example_columns(context_dict), _example_columns(feature_list_dict)
+            if ccols is None or lcols is None:
+                req = make_predict_sequence_examples_request(model_name, model_version, context_dict, feature_list_dict, pkey.decode("utf-8"))
+                wire = req.SerializeToString(deterministic=True)
+                out[i] = (b"\x00" + len(wire).to_bytes(4, "big") + wire) if grpc_frame else wire
+                continue
+            cpreps, lpreps = ccols[1], lcols[1]
+            # a feature list's steps: T and the elements of one step, from its padded shape
+            lrag = []
+            for p, v in zip(lpreps, feature_list_dict.values()):
+                shape = _shape_of(v)
+                g = p[3] or N.Ragged()
+                g.max_len, g.unit = shape[1], int(np.prod(shape[2:], dtype=np.int64))
+                lrag.append(g)
+            preps = cpreps + lpreps
+            feats = (N.Feature * max(len(preps), 1))(*[p[0] for p in preps])
+            name = model_name.encode("utf-8") if isinstance(model_name, str) else bytes(model_name)
+            structs.append(N.ExampleRequest(model_name=name, model_name_len=len(name), has_version=int(model_version is not None),
+                                            order=order_code, version=int(model_version) if model_version is not None else 0,
+                                            n_examples=n, n_features=len(preps), flags=N.RF_GRPC_FRAME if grpc_frame else 0,
+                                            features=feats))
+            keep.append((preps, feats, name))
+            ragged += [p[3] or N.Ragged() for p in cpreps] + lrag
+            strs += [p.bytes_entry or N.Bytes() for p in preps]
+            targets.append(N.ExampleTarget(kind=N.EXAMPLES_PREDICT_SEQUENCE, key=pkey, key_len=len(pkey)))
+            seqs.append(N.ExampleSequence(present=1, n_context=len(cpreps)))
+            dev_idx.append(i)
+        if dev_idx:
+            m = len(dev_idx)
+            reqs = (N.ExampleRequest * m)(*structs)
+            tg, sq = (N.ExampleTarget * m)(*targets), (N.ExampleSequence * m)(*seqs)
+            rg = (N.Ragged * max(len(ragged), 1))(*ragged)
+            bs = (N.Bytes * len(strs))(*strs) if any(b.offsets for b in strs) else None
+            cap = C.c_uint64()
+            N.check(self._lib.b200tfs_example_sequences_arena_size(m, reqs, rg, bs, tg, None, None, None, sq, C.byref(cap)))
+            wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
+            off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
+            N.check(self._lib.b200tfs_encode_example_sequences_host(self._ctx, m, reqs, rg, bs, tg, None, None, None, sq, wire.ctypes.data,
+                                                                    cap.value, off, ln))
             for j, i in enumerate(dev_idx):
                 out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
         return out  # type: ignore[return-value]

@@ -18,7 +18,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
-from .codec import BytesColumn, RaggedColumn, get_codec
+from .codec import BytesColumn, RaggedColumn, _sequence_count, get_codec
 from .tensors import WireTensor
 
 PREDICT_METHOD = "/tensorflow.serving.PredictionService/Predict"
@@ -98,6 +98,75 @@ def examples_with_context_from_input_dict(input_dict: Dict[str, np.ndarray], con
         else:
             _fill_feature(feat, k, np.asarray(v))
     return inp
+
+
+def _list_steps(a, i: int) -> list:
+    """The steps of sequence i of a feature-list value of shape ``[n, T, *inner]`` (a ``RaggedColumn``: its first ``lengths[i]``):
+    arrays of shape ``inner``, or for a ``BytesColumn`` lists of the step's strings."""
+    vals = a.values if isinstance(a, RaggedColumn) else a
+    steps = int(a.lengths[i]) if isinstance(a, RaggedColumn) else a.shape[1]
+    if isinstance(vals, BytesColumn):
+        unit = int(np.prod(vals.shape[2:], dtype=np.int64))
+        strs = vals.strings(i, steps * unit)
+        return [strs[t * unit:(t + 1) * unit] for t in range(steps)]
+    row = np.asarray(vals)[i]
+    return [row[t] for t in range(steps)]
+
+
+def sequence_examples_from_input_dict(context_dict: Dict[str, np.ndarray], feature_list_dict: Dict[str, np.ndarray]) -> list:
+    """One ``tf.SequenceExample`` per sequence (example.proto, feature.proto FeatureLists): what a model exported with a
+    ``tf.io.parse_sequence_example`` serving input takes.  Context feature ``k`` of sequence i is filled as
+    ``examples_from_input_dict`` fills example i's (row i; a 0-d value repeated in every sequence; ``RaggedColumn`` and
+    ``BytesColumn`` values as there).  A feature-list value has shape ``[n, T, *inner]`` (an array, a ``BytesColumn``, or a
+    ``RaggedColumn`` of either, whose sequence i has ``lengths[i]`` steps): sequence i's ``feature_list[f]`` holds one Feature per
+    step, step t holding ``value[i, t]`` flattened (a bytes value: the step's strings).  A list of no steps still has its entry, and
+    ``context`` and ``feature_lists`` are always set.  n is the leading dimension every non-0-d context value and every feature-list
+    value share (ValueError when they disagree, or for a feature-list value of rank < 2); with none, 1 when a dict is non-empty."""
+    from tensorflow.core.example.example_pb2 import SequenceExample
+
+    n = _sequence_count(context_dict, feature_list_dict)
+    ctx = {k: v if isinstance(v, (RaggedColumn, BytesColumn)) else np.asarray(v) for k, v in context_dict.items()}
+    lists = {k: v if isinstance(v, (RaggedColumn, BytesColumn)) else np.asarray(v) for k, v in feature_list_dict.items()}
+    out = []
+    for i in range(n):
+        s = SequenceExample()
+        s.context.SetInParent()
+        s.feature_lists.SetInParent()
+        for k, a in ctx.items():
+            feat = s.context.feature[k]
+            if isinstance(a, BytesColumn) or isinstance(a, RaggedColumn) and isinstance(a.values, BytesColumn):
+                feat.bytes_list.value.extend(a.strings(i))
+                continue
+            _fill_feature(feat, k, a.row(i) if isinstance(a, RaggedColumn) else a if a.ndim == 0 else a[i])
+        for k, a in lists.items():
+            fl = s.feature_lists.feature_list[k]
+            for step in _list_steps(a, i):
+                if isinstance(step, list):
+                    fl.feature.add().bytes_list.value.extend(step)
+                else:
+                    _fill_feature(fl.feature.add(), k, step)
+        out.append(s)
+    return out
+
+
+def make_predict_sequence_examples_request(model_name: str, model_version: Optional[int], context_dict, feature_list_dict,
+                                           input_key: str):
+    """``PredictRequest`` whose one input ``input_key`` is the DT_STRING ``[n]`` tensor of the sequences
+    ``sequence_examples_from_input_dict`` builds, each serialized with ``deterministic=True`` - what
+    ``Codec.encode_sequence_example_requests`` encodes on the GPU."""
+    from tensorflow.core.framework.types_pb2 import DT_STRING
+    from tensorflow_serving.apis.predict_pb2 import PredictRequest
+
+    req = PredictRequest()
+    req.model_spec.name = model_name
+    if model_version is not None:
+        req.model_spec.version.value = model_version
+    seqs = sequence_examples_from_input_dict(context_dict, feature_list_dict)
+    t = req.inputs[input_key.decode("utf-8") if isinstance(input_key, bytes) else input_key]
+    t.dtype = DT_STRING
+    t.tensor_shape.dim.add().size = len(seqs)
+    t.string_val.extend(s.SerializeToString(deterministic=True) for s in seqs)
+    return req
 
 
 def _checked_tasks(tasks) -> List[Tuple[str, str]]:
@@ -278,6 +347,15 @@ def gpu_multi_inference_request_serializer(request) -> bytes:
     return get_codec().encode_example_requests([(model_name, model_version, input_dict, context_dict)], tasks=tasks)[0]
 
 
+def gpu_predict_sequence_examples_serializer(request) -> bytes:
+    """``request_serializer`` for ``channel.unary_unary(PREDICT_METHOD, ...)`` to a model that parses serialized
+    tf.SequenceExamples: (model_name, model_version, context_dict, feature_list_dict, input_key) -> the bytes of
+    ``make_predict_sequence_examples_request(...).SerializeToString(deterministic=True)``, packed on the GPU."""
+    model_name, model_version, context_dict, feature_list_dict, input_key = request
+    return get_codec().encode_sequence_example_requests([(model_name, model_version, context_dict, feature_list_dict)],
+                                                        input_key=input_key)[0]
+
+
 def gpu_response_deserializer(wire: bytes) -> PredictResponseView:
     """``response_deserializer`` for ``channel.unary_unary``: bytes -> lazy response view."""
     return PredictResponseView(wire)
@@ -317,6 +395,16 @@ class TensorServingClient:
         call = self._channel.unary_unary(PREDICT_METHOD, request_serializer=gpu_predict_examples_serializer,
                                          response_deserializer=gpu_response_deserializer)
         return call((model_name, model_version, input_dict, input_key, context_dict), timeout)
+
+    def predict_sequence_examples_request(self, model_name: str, context_dict, feature_list_dict, input_key: str, timeout: int = 60,
+                                          model_version: Optional[int] = None) -> PredictResponseView:
+        """Predict on a model whose signature takes serialized tf.SequenceExamples (a DT_STRING vector it parses with
+        ``tf.io.parse_sequence_example``: a session or event-history model, or TF-Ranking's SequenceExample format): one sequence
+        per row, as ``sequence_examples_from_input_dict(context_dict, feature_list_dict)`` builds it, sent as input
+        ``input_key`` and packed on the GPU."""
+        call = self._channel.unary_unary(PREDICT_METHOD, request_serializer=gpu_predict_sequence_examples_serializer,
+                                         response_deserializer=gpu_response_deserializer)
+        return call((model_name, model_version, context_dict, feature_list_dict, input_key), timeout)
 
     def _make_example_request(self, request_pb, model_name, input_dict, model_version, context_dict=None):
         request = request_pb()

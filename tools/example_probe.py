@@ -18,6 +18,12 @@ Workloads (one request each unless stated):
   K1R the same requests with the user features repeated in every example instead (B200TFS_F_BROADCAST rows, example_list)
   K1P K1 in the Predict-ELWC form: a PredictRequest whose input "examples" is the DT_STRING [1] serialized ExampleListWithContext
   K2  4 096 requests x 8 candidates shaped like K1: the context dominates, and each is written by its request's frame warp
+  Q1  256 requests x 32 SequenceExamples: context {user f32[64], ids int64[4]}, lists {item_ids int64 ragged T <= 50,
+      item_feats f32[T, 16] ragged} (b200tfs_encode_example_sequences_*, PREDICT_SEQUENCE)
+  Q2  64 requests x 16 queries x 100 documents (TF-Ranking's SequenceExample form): context {query_len int64, query string},
+      lists {doc_f0..doc_f7 f32, doc_title: one string of 5-30 B per step}
+  Q3  256 requests x 16 sequences of 200 steps x 8 float lists of 2 values: about 21 KB each, above the 16 KB emit image
+      (not in the default set; --workloads Q1,Q2,Q3; protobuf is timed once, _host over three calls)
 Legs: the _async entry point eager (device columns -> device arena), the same captured once as a CUDA graph and replayed,
 _host from pinned columns (copies both ways included), and examples_from_input_dict + SerializeToString(deterministic=True)
 on one host core.  CUDA events over >= 20 calls after warm-up, three runs each; bytes = column bytes read + wire bytes
@@ -250,6 +256,115 @@ def profile_split(lib, g, eager, calls):
     return split
 
 
+def sequence_workloads(rng):
+    """the SequenceExample workloads: (context_dict, feature_list_dict) per request, host arrays"""
+    def strs(m, lo, hi):
+        lens = rng.integers(lo, hi + 1, m)
+        return BytesColumn(rng.integers(97, 123, int(lens.sum())).astype(np.uint8), np.concatenate([[0], np.cumsum(lens)]))
+
+    def q1():
+        n, T = 32, 50
+        lens = rng.integers(1, T + 1, n)
+        return ({"user": rng.standard_normal((n, 64)).astype(np.float32), "ids": rng.integers(0, 1 << 40, (n, 4))},
+                {"item_ids": RaggedColumn(rng.integers(0, 1 << 40, (n, T)), lens),
+                 "item_feats": RaggedColumn(rng.standard_normal((n, T, 16)).astype(np.float32), lens)})
+
+    def q2():
+        n, T = 16, 100
+        fl = {f"doc_f{j}": rng.standard_normal((n, T)).astype(np.float32) for j in range(8)}
+        c = strs(n * T, 5, 30)
+        fl["doc_title"] = BytesColumn(c.data, c.offsets, (n, T, 1))
+        return {"query_len": rng.integers(1, 20, n), "query": strs(n, 3, 20)}, fl
+
+    def q3():
+        n, T = 16, 200
+        return {"u": rng.standard_normal((n, 8)).astype(np.float32)}, \
+            {f"l{j}": rng.standard_normal((n, T, 2)).astype(np.float32) for j in range(8)}
+
+    return {"Q1": lambda: [q1() for _ in range(256)], "Q2": lambda: [q2() for _ in range(64)], "Q3": lambda: [q3() for _ in range(256)]}
+
+
+def sequence_workload(name, pairs, args, codec, out):
+    """_async eager, graph replay, _host and protobuf on one core for one SequenceExample workload; bytes compared afterwards"""
+    import torch
+
+    from min_tfs_client.codec import _sequence_count
+    from min_tfs_client.requests import make_predict_sequence_examples_request
+
+    def dev(v):
+        if isinstance(v, RaggedColumn):
+            return RaggedColumn(dev(v.values), torch.from_numpy(np.asarray(v.lengths, np.int64)).cuda())
+        if isinstance(v, BytesColumn):
+            return BytesColumn(torch.from_numpy(v.data).cuda(), torch.from_numpy(v.offsets).cuda(), v.shape)
+        return torch.from_numpy(np.ascontiguousarray(v)).cuda()
+
+    lib = N.load()
+    g = Ctx()
+    keep, structs, ragged, strs, seqs = [], [], [], [], []
+    for ctx, fl in pairs:
+        dctx, dfl = {k: dev(v) for k, v in ctx.items()}, {k: dev(v) for k, v in fl.items()}
+        keep += [dctx, dfl]
+        n = _sequence_count(ctx, fl)
+        _, cp = _example_columns(dctx)
+        _, lp = _example_columns(dfl)
+        rg = [p[3] or N.Ragged() for p in cp]
+        for p, v in zip(lp, fl.values()):
+            r = p[3] or N.Ragged()
+            r.max_len, r.unit = v.shape[1], int(np.prod(v.shape[2:], dtype=np.int64))
+            rg.append(r)
+        preps = cp + lp
+        feats = (N.Feature * len(preps))(*[p[0] for p in preps])
+        keep += [preps, feats]
+        ragged += rg
+        strs += [p.bytes_entry or N.Bytes() for p in preps]
+        structs.append(N.ExampleRequest(model_name=b"model", model_name_len=5, has_version=1, order=N.ORDER_UPB, version=1,
+                                        n_examples=n, n_features=len(preps), flags=0, features=feats))
+        seqs.append(N.ExampleSequence(present=1, n_context=len(cp)))
+    m = len(structs)
+    reqs = (N.ExampleRequest * m)(*structs)
+    rga, bsa = (N.Ragged * len(ragged))(*ragged), (N.Bytes * len(strs))(*strs)
+    tga = (N.ExampleTarget * m)(*[N.ExampleTarget(kind=N.EXAMPLES_PREDICT_SEQUENCE, key=b"sequences", key_len=9)] * m)
+    sqa = (N.ExampleSequence * m)(*seqs)
+    cap = C.c_uint64()
+    N.check(lib.b200tfs_example_sequences_arena_size(m, reqs, rga, bsa, tga, None, None, None, sqa, C.byref(cap)))
+    arena = (g.malloc(cap.value + 256) + 255) & ~255
+
+    def eager():
+        N.check(lib.b200tfs_encode_example_sequences_async(g.ctx, m, reqs, rga, bsa, tga, None, None, None, sqa, arena, cap.value))
+
+    eager()
+    N.check(lib.b200tfs_encode_results(g.ctx, m, None, None))
+    N.check(lib.b200tfs_capture_begin(g.ctx))
+    eager()
+    gr = C.c_void_p()
+    N.check(lib.b200tfs_capture_end(g.ctx, C.byref(gr)))
+    res = {"requests": m, "sequences": sum(s.n_examples for s in structs), "arena_bytes": cap.value}
+    res["async_us"] = min(g.timed(eager, args.calls) for _ in range(args.runs))
+    res["graph_us"] = min(g.timed(lambda: N.check(lib.b200tfs_graph_launch(g.ctx, gr)), args.calls) for _ in range(args.runs))
+    items = [("model", 1, c, f) for c, f in pairs]
+    res["host_us"] = min(timed_host(lambda: codec.encode_sequence_example_requests(items, input_key="sequences"), 3)
+                         for _ in range(args.runs))
+    t0 = time.perf_counter()
+    refs = [make_predict_sequence_examples_request("model", 1, c, f, "sequences").SerializeToString(deterministic=True) for c, f in pairs]
+    res["protobuf_one_core_us"] = (time.perf_counter() - t0) * 1e6
+    res["wire_bytes"] = sum(len(w) for w in refs)
+    # after the timed region: the replayed graph's and the host route's bytes against protobuf
+    off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
+    N.check(lib.b200tfs_graph_launch(g.ctx, gr))
+    N.check(lib.b200tfs_encode_results(g.ctx, m, off, ln))
+    host = np.empty(cap.value, np.uint8)
+    N.check(lib.b200tfs_memcpy_d2h(g.ctx, host.ctypes.data, arena, cap.value))
+    assert all(host[off[r]: off[r] + ln[r]].tobytes() == refs[r] for r in range(m)), name
+    assert codec.encode_sequence_example_requests(items, input_key="sequences") == refs, name
+    sizes = [int(s) for s in ln]
+    res["max_request_bytes"] = max(sizes)
+    N.check(lib.b200tfs_graph_destroy(gr))
+    if name in args.profile.split(","):
+        res["kernels"] = profile_split(lib, g, eager, args.calls)
+    out["workloads"][name] = res
+    print(name, res, flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=20)
@@ -266,7 +381,11 @@ def main():
     codec = Codec(0)
     out = {"card": card, "calls": args.calls, "runs": args.runs, "workloads": {}}
     profile_only = [w for w in args.profile.split(",") if w]
+    Q = sequence_workloads(rng)
     for name in (profile_only or args.workloads.split(",")):
+        if name in Q:
+            sequence_workload(name, Q[name](), args, codec, out)
+            continue
         pairs = [x if isinstance(x, tuple) else (x, None) for x in W[name]()]
         host_dicts = [d for d, _ in pairs]
         host_ctxs = [c for _, c in pairs]
