@@ -151,6 +151,25 @@ typedef struct b200tfs_request {
   const b200tfs_tensor* inputs;
 } b200tfs_request;
 
+/* What a request's model_spec and PredictRequest.output_filter carry beside the name and version, for the _spec entry points
+ * below (one per request, parallel to their reqs[]; NULL: none, the bytes of the entry point without _spec).  Strings are
+ * written as given (UTF-8 by the caller), in field-number order: 0A name | 12 {08 version} | 1A signature_name | 22 version_label.
+ *   signature_len  > 0: ModelSpec.signature_name (field 3); 0: not written (a proto3 scalar: empty is the default)
+ *   version_label_len >= 0: ModelSpec.version_label (field 4, a version_choice oneof member: written even when empty, 22 00);
+ *                     < 0: not set.  A label on a request with has_version is B200TFS_E_ARG.
+ *   output_filter: n_output_filter names, written behind the last inputs entry as {1A vi(len) name}* in the given order (no
+ *                  sorting, no de-duplication; an empty name is 1A 00).
+ * A negative length, a NULL pointer behind a positive length or count: B200TFS_E_ARG.                                          */
+typedef struct b200tfs_request_spec {
+  const char* signature_name;
+  int64_t signature_len;
+  const char* version_label;
+  int64_t version_label_len;
+  const char* const* output_filter;
+  const int64_t* output_filter_len;
+  int64_t n_output_filter;
+} b200tfs_request_spec;
+
 /* Where the values of one output lie on the wire.  The reference iterates the merged repeated field whatever
  * its wire layout (tensors.py:42-46): one packed occurrence, several of them, single unpacked elements, or any
  * mix.  A run is `count` pieces of `len` value bytes each, `stride` bytes apart - one packed occurrence is a run
@@ -264,6 +283,11 @@ int b200tfs_order_keys(int32_t n, const char* const* keys, const int64_t* key_le
  * worst-case slot per record.                                                                       */
 int b200tfs_tensor_arena_size(int32_t n, const b200tfs_tensor* tensors, uint64_t* bytes);
 int b200tfs_request_arena_size(int32_t n, const b200tfs_request* reqs, uint64_t* bytes);
+/* The same three with a b200tfs_request_spec per request (spec / specs: NULL = none; the forms above are these with NULL) */
+int b200tfs_request_size_spec(const b200tfs_request* r, const b200tfs_request_spec* spec, uint64_t* total_len);
+int b200tfs_request_frame_spec(const b200tfs_request* r, const b200tfs_request_spec* spec, void* buf, uint64_t cap, uint64_t* frame_len,
+                               uint64_t* payload_off, uint64_t* payload_len, int32_t* perm);
+int b200tfs_request_arena_size_spec(int32_t n, const b200tfs_request* reqs, const b200tfs_request_spec* specs, uint64_t* bytes);
 
 /* ---- encode (device tensors -> device wire arena) ---------------------------------------------- */
 /* Pass 1 for the varint-packed dtypes (int_val / int64_val / uint32_val / uint64_val / half_val):
@@ -302,6 +326,12 @@ int b200tfs_encode_results(b200tfs_ctx* ctx, int32_t n, uint64_t* rec_off, uint6
  * per input, where the framing writers put its payload (payload_off[i] / payload_len[i]; 0 / 0 for an input without values). */
 int b200tfs_request_frame_deferred(const b200tfs_request* r, const uint64_t* packed_len, void* buf, uint64_t cap,
                                    uint64_t* rec_off, uint64_t* rec_len, uint64_t* payload_off, uint64_t* payload_len);
+/* The same two with a b200tfs_request_spec per request (NULL: none).  The output_filter run lies behind the last payload, so
+ * where it goes depends on the lengths the device counts: frame_requests_kernel copies it there from the host-built bytes. */
+int b200tfs_encode_requests_async_spec(b200tfs_ctx* ctx, int32_t n, const b200tfs_request* reqs, const b200tfs_request_spec* specs,
+                                       void* arena_dev, uint64_t arena_cap);
+int b200tfs_request_frame_deferred_spec(const b200tfs_request* r, const b200tfs_request_spec* spec, const uint64_t* packed_len, void* buf,
+                                        uint64_t cap, uint64_t* rec_off, uint64_t* rec_len, uint64_t* payload_off, uint64_t* payload_len);
 
 /* ---- decode (device wire arena -> table -> device tensors) -------------------------------------- */
 /* Parse n PredictResponse messages lying at rec_off[i]..+rec_len[i] of the device arena.  Runs the
@@ -657,6 +687,16 @@ int b200tfs_encode_padded_requests_columns_async(b200tfs_ctx* ctx, int32_t n, co
 int b200tfs_padded_request_frame_columns(const b200tfs_request* req, const b200tfs_pad_input* in, const struct b200tfs_bytes* bytes,
                                          const uint64_t* packed_len, void* buf, uint64_t cap, uint64_t* rec_len,
                                          uint64_t* payload_off, uint64_t* payload_len);
+/* The same three with one b200tfs_request_spec for every request of the call (NULL: none; the _columns forms are these with
+ * NULL).  The output_filter run follows each record's last payload, so the framing kernels place it from the device shapes. */
+int b200tfs_padded_request_columns_arena_size_spec(int32_t n, const b200tfs_request* req, const struct b200tfs_bytes* bytes,
+                                                   const b200tfs_request_spec* spec, uint64_t* out);
+int b200tfs_encode_padded_requests_columns_async_spec(b200tfs_ctx* ctx, int32_t n, const b200tfs_request* req, const b200tfs_pad_input* in,
+                                                      const struct b200tfs_bytes* bytes, const b200tfs_request_spec* spec, void* arena_dev,
+                                                      uint64_t arena_cap);
+int b200tfs_padded_request_frame_columns_spec(const b200tfs_request* req, const b200tfs_pad_input* in, const struct b200tfs_bytes* bytes,
+                                              const b200tfs_request_spec* spec, const uint64_t* packed_len, void* buf, uint64_t cap,
+                                              uint64_t* rec_len, uint64_t* payload_off, uint64_t* payload_len);
 
 /* ---- CUDA graphs: record a fixed sequence of encode / decode calls once, replay it per request ---
  * Between capture_begin and capture_end the asynchronous entry points (b200tfs_encode_requests,
@@ -693,6 +733,10 @@ int b200tfs_encode_requests_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_requ
 int b200tfs_encode_requests_host_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_request* reqs,
                                        void* wire_host, uint64_t wire_cap, uint64_t* rec_off,
                                        uint64_t* rec_len);
+/* b200tfs_encode_requests_host with a b200tfs_request_spec per request (NULL: none).  The output_filter run is the last framing
+ * bytes of each record, written with the record's other framing (the first slice of a pipelined call).                     */
+int b200tfs_encode_requests_host_spec(b200tfs_ctx* ctx, int32_t n, const b200tfs_request* reqs, const b200tfs_request_spec* specs,
+                                      void* wire_host, uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
 /* Host-buffer form of b200tfs_decode_responses: copies the n responses to the device, runs the fused
  * decode kernel and copies n*dst_stride bytes of decoded values back into dst_host (pinned), all
  * queued asynchronously.  b200tfs_decode_results then synchronises and returns the table.          */
@@ -1016,6 +1060,31 @@ int b200tfs_encode_example_sequences_host(b200tfs_ctx* ctx, int32_t n, const b20
                                           const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
                                           const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
                                           void* wire_host, uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
+/* The _sequences_ entry points with a b200tfs_request_spec per request (spec / specs == NULL: those calls themselves, which call
+ * these).  signature_name and version_label go into the model_spec of every target; a MultiInference task's model_spec is
+ * name | version | the task's signature | label, and a signature_name for the whole request beside tasks is B200TFS_E_ARG.
+ * output_filter exists only on the Predict forms (PREDICT_STRING, PREDICT_ELWC, PREDICT_SEQUENCE), where the frame kernel writes
+ * it behind the examples (and the context); a filter on any other request is B200TFS_E_ARG.                                   */
+int b200tfs_example_specs_request_size(const b200tfs_example_request* r, const b200tfs_example_target* target,
+                                       const b200tfs_example_context* context, const b200tfs_example_tasks* tasks,
+                                       const b200tfs_ragged* ragged, const b200tfs_example_sequence* sequence,
+                                       const b200tfs_request_spec* spec, uint64_t* total_len);
+int b200tfs_example_specs_arena_size(int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                     const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                     const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                     const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
+                                     const b200tfs_request_spec* specs, uint64_t* bytes_out);
+int b200tfs_encode_example_specs_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                       const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                       const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                       const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
+                                       const b200tfs_request_spec* specs, void* arena_dev, uint64_t arena_cap);
+int b200tfs_encode_example_specs_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                      const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                      const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                      const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
+                                      const b200tfs_request_spec* specs, void* wire_host, uint64_t wire_cap, uint64_t* rec_off,
+                                      uint64_t* rec_len);
 
 /* ---- Classify / Regress responses: a batch of responses into one value or score array ----------------------
  * What ClassificationResponse.FromString / RegressionResponse.FromString followed by a loop over the result give, concatenated

@@ -458,21 +458,47 @@ int b200tfs_cast_supported(int32_t src, int32_t wire) {
 // wire-size arithmetic and header bytes
 // ------------------------------------------------------------------------------------------------
 static bool request_needs_deferred(const b200tfs_request& r);                  // varint_host.inc
-static int deferred_arena_size(int32_t n, const b200tfs_request* reqs, uint64_t* bytes);   // varint_host.inc
+static int deferred_arena_size(int32_t n, const b200tfs_request* reqs, const b200tfs_request_spec* specs, uint64_t* bytes);   // varint_host.inc
 
 namespace {
 
 constexpr uint64_t kProtoLimit = 0x7FFFFFFFull;  // protobuf's 2 GiB message limit
 
-// model_spec's layout (framing.h writes it)
+// model_spec's layout (framing.h writes it); `s` (may be null) adds signature_name and version_label
 template <class Req>
-int spec_layout(const Req& r, SpecLayout* S) {
+int spec_layout(const Req& r, SpecLayout* S, const b200tfs_request_spec* s = nullptr) {
   if (r.model_name_len < 0 || (r.model_name_len && !r.model_name)) return fail(B200TFS_E_ARG, "bad model_name");
   *S = SpecLayout{};
   if (r.model_name_len) S->body += 1 + varint_len((uint64_t)r.model_name_len) + (uint64_t)r.model_name_len;
   if (r.has_version) {
     S->version_len = r.version ? 1 + varint_len((uint64_t)r.version) : 0;
     S->body += 2 + S->version_len;
+  }
+  if (!s) return B200TFS_OK;
+  if (s->signature_len < 0 || (s->signature_len && !s->signature_name)) return fail(B200TFS_E_ARG, "bad signature_name");
+  if (s->version_label_len > 0 && !s->version_label) return fail(B200TFS_E_ARG, "bad version_label");
+  if (s->version_label_len >= 0 && r.has_version)
+    return fail(B200TFS_E_ARG, "version and version_label are members of one oneof: set at most one of them");
+  if ((uint64_t)s->signature_len > kProtoLimit || (s->version_label_len > 0 && (uint64_t)s->version_label_len > kProtoLimit))
+    return fail(B200TFS_E_TOOBIG, "signature_name or version_label exceeds protobuf's 2 GiB limit");
+  S->sig = s->signature_name; S->sig_len = (uint64_t)s->signature_len;
+  S->label = s->version_label; S->label_len = s->version_label_len < 0 ? -1 : s->version_label_len;
+  if (S->sig_len) S->body += 1 + varint_len(S->sig_len) + S->sig_len;
+  if (S->label_len >= 0) S->body += 1 + varint_len((uint64_t)S->label_len) + (uint64_t)S->label_len;
+  return B200TFS_OK;
+}
+
+// bytes of the output_filter run framing.h's write_output_filter writes for `s` (may be null)
+int filter_len(const b200tfs_request_spec* s, uint64_t* len) {
+  *len = 0;
+  if (!s) return B200TFS_OK;
+  if (s->n_output_filter < 0 || (s->n_output_filter && (!s->output_filter || !s->output_filter_len)))
+    return fail(B200TFS_E_ARG, "bad output_filter");
+  for (int64_t i = 0; i < s->n_output_filter; ++i) {
+    const int64_t l = s->output_filter_len[i];
+    if (l < 0 || (l && !s->output_filter[i])) return fail(B200TFS_E_ARG, "bad output_filter name %lld", (long long)i);
+    *len += 1 + varint_len((uint64_t)l) + (uint64_t)l;
+    if (*len > kProtoLimit) return fail(B200TFS_E_TOOBIG, "output_filter exceeds protobuf's 2 GiB limit");
   }
   return B200TFS_OK;
 }
@@ -725,6 +751,8 @@ struct RequestLayout {
   std::vector<int32_t> perm;
   std::vector<uint64_t> tp_len, entry_len;
   SpecLayout spec;
+  const b200tfs_request_spec* s = nullptr;   // signature, label and output_filter (may be null)
+  uint64_t tail = 0;          // bytes of the output_filter run behind the last input
   uint64_t total = 0;
   uint64_t prefix = 0;        // bytes in front of the message: gRPC's 5-byte frame header when asked for
   uint64_t largest_off = 0;
@@ -733,11 +761,13 @@ struct RequestLayout {
 
 // Validates request r, orders its keys and lays it out.  `deferred` (b200tfs_encode_requests_async): packed-varint inputs are
 // unmeasured, and the record's total - which then depends on lengths the device counts - is checked on the device.
-int request_layout(const b200tfs_request& r, RequestLayout* R, bool deferred = false) {
+int request_layout(const b200tfs_request& r, const b200tfs_request_spec* s, RequestLayout* R, bool deferred = false) {
   if (r.n_inputs < 0) return fail(B200TFS_E_ARG, "n_inputs < 0");
   if (r.n_inputs && !r.inputs) return fail(B200TFS_E_ARG, "inputs is NULL");
-  int rc = spec_layout(r, &R->spec);
+  int rc = spec_layout(r, &R->spec, s);
   if (rc) return rc;
+  if ((rc = filter_len(s, &R->tail))) return rc;
+  R->s = s;
   const int n = r.n_inputs;
   R->tl.resize(n); R->perm.resize(n); R->tp_len.resize(n); R->entry_len.resize(n); R->payload_off.resize(n);
   // (no heap traffic for the usual handful of inputs: this runs once per request of a batch)
@@ -777,6 +807,7 @@ int request_layout(const b200tfs_request& r, RequestLayout* R, bool deferred = f
     if (L.payload_len > largest) { largest = L.payload_len; R->largest_off = payload_off; }
     total += 1 + varint_len(el) + el;
   }
+  total += R->tail;
   if (!deferred && total - R->prefix > kProtoLimit)
     return fail(B200TFS_E_TOOBIG, "PredictRequest of %llu bytes exceeds protobuf's 2 GiB limit", (unsigned long long)(total - R->prefix));
   R->total = total;
@@ -794,6 +825,7 @@ struct PlannedRequest {
   size_t mark;            // blob offset where the pending header run starts
   uint8_t* cursor;        // where that run will land
   void spec(RawOut& o) { write_model_spec(o, r, R.spec); }
+  void tail(RawOut& o) { write_output_filter(o, R.s); }     // the trailing header run plan_request closes after the last payload
   void input(uint32_t j, b200tfs_tensor& t, TensorLayout& L) const { t = r.inputs[R.perm[j]]; L = R.tl[j]; }
   void payload(RawOut& o, uint32_t, const b200tfs_tensor& t, const TensorLayout& L) {
     if (!L.payload_len) return;
@@ -839,10 +871,12 @@ int b200tfs_tensor_proto_size(const b200tfs_tensor* t, uint64_t* header_len, uin
   return B200TFS_OK;
 }
 
-int b200tfs_request_size(const b200tfs_request* r, uint64_t* total_len) {
+int b200tfs_request_size(const b200tfs_request* r, uint64_t* total_len) { return b200tfs_request_size_spec(r, nullptr, total_len); }
+
+int b200tfs_request_size_spec(const b200tfs_request* r, const b200tfs_request_spec* spec, uint64_t* total_len) {
   if (!r) return fail(B200TFS_E_ARG, "request is NULL");
   RequestLayout R;
-  int rc = request_layout(*r, &R);
+  int rc = request_layout(*r, spec, &R);
   if (rc) return rc;
   if (total_len) *total_len = R.total;
   return B200TFS_OK;
@@ -862,9 +896,14 @@ int b200tfs_tensor_proto_header(const b200tfs_tensor* t, void* buf, uint64_t cap
 
 int b200tfs_request_frame(const b200tfs_request* r, void* buf, uint64_t cap, uint64_t* frame_len, uint64_t* payload_off,
                           uint64_t* payload_len, int32_t* perm) {
+  return b200tfs_request_frame_spec(r, nullptr, buf, cap, frame_len, payload_off, payload_len, perm);
+}
+
+int b200tfs_request_frame_spec(const b200tfs_request* r, const b200tfs_request_spec* spec, void* buf, uint64_t cap, uint64_t* frame_len,
+                               uint64_t* payload_off, uint64_t* payload_len, int32_t* perm) {
   if (!r || !frame_len) return fail(B200TFS_E_ARG, "NULL argument");
   RequestLayout R;
-  int rc = request_layout(*r, &R);
+  int rc = request_layout(*r, spec, &R);
   if (rc) return rc;
   PlanBuilder pb;  // planned against a NULL arena: only the blob (frame bytes in wire order) is used
   if ((rc = plan_request(*r, R, nullptr, pb))) return rc;
@@ -898,16 +937,20 @@ int b200tfs_tensor_arena_size(int32_t n, const b200tfs_tensor* tensors, uint64_t
 }
 
 int b200tfs_request_arena_size(int32_t n, const b200tfs_request* reqs, uint64_t* bytes) {
+  return b200tfs_request_arena_size_spec(n, reqs, nullptr, bytes);
+}
+
+int b200tfs_request_arena_size_spec(int32_t n, const b200tfs_request* reqs, const b200tfs_request_spec* specs, uint64_t* bytes) {
   if (n < 0 || (n && !reqs) || !bytes) return fail(B200TFS_E_ARG, "bad arguments");
   // a batch with an unmeasured packed-varint input (packed_len == 0) is sized for b200tfs_encode_requests_async: every record
   // gets a slot for its worst case; measured batches are sized exactly, as b200tfs_encode_requests lays them out
   bool deferred = false;
   for (int i = 0; i < n && !deferred; ++i) deferred = request_needs_deferred(reqs[i]);
-  if (deferred) return deferred_arena_size(n, reqs, bytes);
+  if (deferred) return deferred_arena_size(n, reqs, specs, bytes);
   uint64_t cursor = 0;
   RequestLayout R;
   for (int i = 0; i < n; ++i) {
-    int rc = request_layout(reqs[i], &R);
+    int rc = request_layout(reqs[i], specs ? specs + i : nullptr, &R);
     if (rc) return rc;
     cursor = place_record(cursor, R.largest_off) + R.total;
   }
@@ -944,8 +987,8 @@ int b200tfs_encode_tensor_protos(b200tfs_ctx* c, int32_t n, const b200tfs_tensor
 }
 
 // lay the batch out in the arena and collect its pieces (b200tfs_encode_requests launches them at once, the pipelined host path in slices)
-static int plan_requests(int32_t n, const b200tfs_request* reqs, void* arena_dev, uint64_t arena_cap, uint64_t* rec_off, uint64_t* rec_len,
-                         PlanBuilder& pb) {
+static int plan_requests(int32_t n, const b200tfs_request* reqs, const b200tfs_request_spec* specs, void* arena_dev, uint64_t arena_cap,
+                         uint64_t* rec_off, uint64_t* rec_len, PlanBuilder& pb) {
   if (n > 16) {   // a batch: one allocation per table instead of a doubling series
     size_t inputs = 0;
     for (int i = 0; i < n; ++i) inputs += (size_t)std::max(reqs[i].n_inputs, 0);
@@ -954,7 +997,7 @@ static int plan_requests(int32_t n, const b200tfs_request* reqs, void* arena_dev
   RequestLayout R;
   uint64_t cursor = 0;
   for (int i = 0; i < n; ++i) {
-    int rc = request_layout(reqs[i], &R);
+    int rc = request_layout(reqs[i], specs ? specs + i : nullptr, &R);
     if (rc) return rc;
     for (int j = 0; j < reqs[i].n_inputs; ++j)
       if (R.tl[j].payload_len && !reqs[i].inputs[R.perm[j]].data) return fail(B200TFS_E_ARG, "request %d: tensor data pointer is NULL", i);
@@ -967,16 +1010,21 @@ static int plan_requests(int32_t n, const b200tfs_request* reqs, void* arena_dev
   return B200TFS_OK;
 }
 
-int b200tfs_encode_requests(b200tfs_ctx* c, int32_t n, const b200tfs_request* reqs, void* arena_dev, uint64_t arena_cap,
-                            uint64_t* rec_off, uint64_t* rec_len) {
+static int encode_requests_spec(b200tfs_ctx* c, int32_t n, const b200tfs_request* reqs, const b200tfs_request_spec* specs, void* arena_dev,
+                                uint64_t arena_cap, uint64_t* rec_off, uint64_t* rec_len) {
   if (!c || n < 0 || (n && (!reqs || !arena_dev || !rec_off || !rec_len))) return fail(B200TFS_E_ARG, "bad arguments");
   if ((uintptr_t)arena_dev & 255) return fail(B200TFS_E_ARG, "arena must be 256-byte aligned");
   CU(cudaSetDevice(c->device));
   PlanBuilder pb;
-  int rc = plan_requests(n, reqs, arena_dev, arena_cap, rec_off, rec_len, pb);
+  int rc = plan_requests(n, reqs, specs, arena_dev, arena_cap, rec_off, rec_len, pb);
   if (rc) return rc;
   if ((rc = launch_plan(c, pb))) return rc;
   return run_varjobs(c, pb);
+}
+
+int b200tfs_encode_requests(b200tfs_ctx* c, int32_t n, const b200tfs_request* reqs, void* arena_dev, uint64_t arena_cap,
+                            uint64_t* rec_off, uint64_t* rec_len) {
+  return encode_requests_spec(c, n, reqs, nullptr, arena_dev, arena_cap, rec_off, rec_len);
 }
 
 // ---- decode ------------------------------------------------------------------------------------
@@ -1934,8 +1982,8 @@ int b200tfs_encode_tensor_protos_host(b200tfs_ctx* c, int32_t n, const b200tfs_t
   return B200TFS_OK;
 }
 
-int b200tfs_encode_requests_host_async(b200tfs_ctx* c, int32_t n, const b200tfs_request* reqs, void* wire_host, uint64_t wire_cap,
-                                       uint64_t* rec_off, uint64_t* rec_len) {
+static int encode_requests_host_async_spec(b200tfs_ctx* c, int32_t n, const b200tfs_request* reqs, const b200tfs_request_spec* specs,
+                                           void* wire_host, uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len) {
   if (!c || n < 0 || (n && (!reqs || !wire_host || !rec_off || !rec_len))) return fail(B200TFS_E_ARG, "bad arguments");
   if (n == 0) return B200TFS_OK;
   CU(cudaSetDevice(c->device));
@@ -1966,7 +2014,7 @@ int b200tfs_encode_requests_host_async(b200tfs_ctx* c, int32_t n, const b200tfs_
   size_t k = 0;
   for (int i = 0; i < n; ++i) { rq[i].inputs = ts.data() + k; k += (size_t)rq[i].n_inputs; }
   uint64_t need = 0;
-  if ((rc = b200tfs_request_arena_size(n, rq.data(), &need))) return rc;
+  if ((rc = b200tfs_request_arena_size_spec(n, rq.data(), specs, &need))) return rc;
   if (try_pipe) {
     // A pinned wire buffer with room for the arena layout (records 256-byte aligned, largest payload 128-byte aligned) is written
     // by the kernels themselves; rec_off then counts from wire_host like always, but record 0 does not start at 0.
@@ -1975,7 +2023,9 @@ int b200tfs_encode_requests_host_async(b200tfs_ctx* c, int32_t n, const b200tfs_
     const bool direct = out_dev != nullptr;
     if (!direct && (rc = grow_dev(c, c->arena_dev, need))) return rc;
     PlanBuilder pb;
-    if ((rc = plan_requests(n, rq.data(), direct ? (void*)out_dev : c->arena_dev.p, direct ? wire_cap : c->arena_dev.cap, rec_off, rec_len, pb))) return rc;
+    if ((rc = plan_requests(n, rq.data(), specs, direct ? (void*)out_dev : c->arena_dev.p, direct ? wire_cap : c->arena_dev.cap, rec_off, rec_len,
+                            pb)))
+      return rc;
     const uint64_t lo = rec_off[0], hi = rec_off[n - 1] + rec_len[n - 1];
     if (!direct && hi - lo > wire_cap) return fail(B200TFS_E_SIZE, "wire buffer too small: need %llu bytes", (unsigned long long)(hi - lo));
     bool done = false;
@@ -1993,12 +2043,17 @@ int b200tfs_encode_requests_host_async(b200tfs_ctx* c, int32_t n, const b200tfs_
     return B200TFS_OK;
   }
   if ((rc = grow_dev(c, c->arena_dev, need))) return rc;
-  if ((rc = b200tfs_encode_requests(c, n, rq.data(), c->arena_dev.p, c->arena_dev.cap, rec_off, rec_len))) return rc;
+  if ((rc = encode_requests_spec(c, n, rq.data(), specs, c->arena_dev.p, c->arena_dev.cap, rec_off, rec_len))) return rc;
   const uint64_t lo = rec_off[0], hi = rec_off[n - 1] + rec_len[n - 1];
   if (hi - lo > wire_cap) return fail(B200TFS_E_SIZE, "wire buffer too small: need %llu bytes", (unsigned long long)(hi - lo));
   CU(cudaMemcpyAsync(wire_host, (uint8_t*)c->arena_dev.p + lo, hi - lo, cudaMemcpyDeviceToHost, c->stream));
   for (int i = 0; i < n; ++i) rec_off[i] -= lo;
   return B200TFS_OK;
+}
+
+int b200tfs_encode_requests_host_async(b200tfs_ctx* c, int32_t n, const b200tfs_request* reqs, void* wire_host, uint64_t wire_cap,
+                                       uint64_t* rec_off, uint64_t* rec_len) {
+  return encode_requests_host_async_spec(c, n, reqs, nullptr, wire_host, wire_cap, rec_off, rec_len);
 }
 
 int b200tfs_pipelined_calls(b200tfs_ctx* c, uint64_t* count) {
@@ -2023,7 +2078,12 @@ int b200tfs_set_pipeline(b200tfs_ctx* c, uint64_t min_bytes, int32_t max_slices)
 
 int b200tfs_encode_requests_host(b200tfs_ctx* c, int32_t n, const b200tfs_request* reqs, void* wire_host, uint64_t wire_cap,
                                  uint64_t* rec_off, uint64_t* rec_len) {
-  int rc = b200tfs_encode_requests_host_async(c, n, reqs, wire_host, wire_cap, rec_off, rec_len);
+  return b200tfs_encode_requests_host_spec(c, n, reqs, nullptr, wire_host, wire_cap, rec_off, rec_len);
+}
+
+int b200tfs_encode_requests_host_spec(b200tfs_ctx* c, int32_t n, const b200tfs_request* reqs, const b200tfs_request_spec* specs,
+                                      void* wire_host, uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len) {
+  int rc = encode_requests_host_async_spec(c, n, reqs, specs, wire_host, wire_cap, rec_off, rec_len);
   if (rc) return rc;
   CU(cudaStreamSynchronize(c->stream));
   return B200TFS_OK;

@@ -626,24 +626,24 @@ __device__ __forceinline__ uint64_t ex_examples_len(const ExTables& T, const ExR
   return el;
 }
 // Request r's status, and when it is B200TFS_OK its prefix in front of the anchor, by the calling warp: el bytes of examples and
-// `tail` bytes behind them (a context field), nested once more in a string_val with `nest` (Predict-ELWC).  bad: a length or an
-// offset the request reads was out of range.
+// `tail` bytes behind them (a context field), nested once more in a string_val with `nest` (Predict-ELWC); then the request's
+// output_filter run (q.tail_len bytes of the blob) behind them.  bad: a length or an offset the request reads was out of range.
 __device__ __forceinline__ int32_t ex_frame_request(const ExTables& T, const ExReq& q, uint32_t r, uint64_t el, uint64_t tail,
                                                     bool nest, bool bad) {
   const uint32_t lane = threadIdx.x & 31;
   // [00 be32(msg)] spec 12 vi(outer) mid inner_tag vi(inner) head [42 vi(body)] | body   (plan.h ExReq, ExCtxRef)
   const uint64_t body = el + tail, nested = nest ? 1 + varint_len(body) + body : body;
   const uint64_t inner = q.head_len + nested, outer = q.mid_len + 1 + varint_len(inner) + inner;
-  const uint64_t msg = q.spec_len + 1 + varint_len(outer) + outer;
-  const uint64_t pre = (q.grpc ? 5 : 0) + msg - body;
+  const uint64_t msg = q.spec_len + 1 + varint_len(outer) + outer + q.tail_len;
+  const uint64_t pre = (q.grpc ? 5 : 0) + msg - body - q.tail_len;
   int32_t st = B200TFS_OK;
   if (bad) st = B200TFS_E_SHAPE;
   else if (msg > 0x7FFFFFFFull) st = B200TFS_E_TOOBIG;
-  else if (q.anchor + body > q.slot_end) st = B200TFS_E_SIZE;
+  else if (q.anchor + body + q.tail_len > q.slot_end) st = B200TFS_E_SIZE;
   if (lane == 0) {
     T.status[r] = st;
     T.rec_off[r] = st ? 0 : q.anchor - pre;
-    T.rec_len[r] = st ? 0 : pre + body;
+    T.rec_len[r] = st ? 0 : pre + body + q.tail_len;
   }
   if (st) return st;
   uint8_t* w = T.arena + q.anchor - pre;
@@ -654,6 +654,8 @@ __device__ __forceinline__ int32_t ex_frame_request(const ExTables& T, const ExR
     const uint32_t d = k < q.spec_len ? at_spec + k : k < q.spec_len + q.mid_len ? at_mid + (k - q.spec_len) : at_head + (k - q.spec_len - q.mid_len);
     w[d] = T.blob[q.spec_off + k];
   }
+  const uint32_t at_tail = q.spec_off + q.spec_len + q.mid_len + q.head_len;
+  for (uint32_t k = lane; k < q.tail_len; k += 32) w[pre + body + k] = T.blob[at_tail + k];
   if (lane == 0) {
     if (q.grpc) { w[0] = 0; w[1] = (uint8_t)(msg >> 24); w[2] = (uint8_t)(msg >> 16); w[3] = (uint8_t)(msg >> 8); w[4] = (uint8_t)msg; }
     w[at_outer] = 0x12; put_varint(w + at_outer + 1, outer);

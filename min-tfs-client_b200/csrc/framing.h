@@ -52,9 +52,14 @@ struct CountOut {
   B2_HD uint64_t pos() const { return n; }
 };
 
-// model_spec{ 0A vi name [12 vi {08 vi(version)}] } of a PredictRequest or a tf.Example request
+// model_spec{ 0A vi name [12 vi {08 vi(version)}] [1A vi signature_name] [22 vi version_label] } of a PredictRequest or a
+// tf.Example request, in field-number order.  signature_name is a proto3 scalar (empty: not written); version_label is a member
+// of the version_choice oneof, so a set label is written even when empty (22 00).  The strings are host memory: the spec is
+// written on the host and copied as bytes by every kernel that places it.
 struct SpecLayout {
   uint64_t body = 0, version_len = 0;
+  const char* sig = nullptr; uint64_t sig_len = 0;
+  const char* label = nullptr; int64_t label_len = -1;   // < 0: no version_label
   B2_HD uint64_t field() const { return 1 + varint_len(body) + body; }   // with its tag and length
 };
 
@@ -65,6 +70,17 @@ B2_HD void write_model_spec(Out& o, const Req& r, const SpecLayout& S) {
   if (r.has_version) {
     o.byte(0x12); o.byte((uint8_t)S.version_len);
     if (r.version) { o.byte(0x08); o.varint((uint64_t)r.version); }
+  }
+  if (S.sig_len) { o.byte(0x1A); o.varint(S.sig_len); o.bytes(S.sig, (size_t)S.sig_len); }
+  if (S.label_len >= 0) { o.byte(0x22); o.varint((uint64_t)S.label_len); o.bytes(S.label, (size_t)S.label_len); }
+}
+
+// PredictRequest.output_filter: {1A vi(len) name}* in the order given (no sorting, no de-duplication), behind the last inputs
+// entry.  Host only, like the spec: the deferred and padded encodes copy these bytes from their blob.
+template <class Out>
+void write_output_filter(Out& o, const b200tfs_request_spec* s) {
+  for (int64_t i = 0; s && i < s->n_output_filter; ++i) {
+    o.byte(0x1A); o.varint((uint64_t)s->output_filter_len[i]); o.bytes(s->output_filter[i], (size_t)s->output_filter_len[i]);
   }
 }
 
@@ -113,9 +129,10 @@ B2_HD uint64_t tiny_total(const TinyVar& t) {
   return s;
 }
 
-// The framing of one PredictRequest through `o`: [00 be32(msg)] model_spec {entry header, tensor header, payload}*.  `Req` supplies
-// what differs between the callers: spec(o) writes the model_spec field, input(j, t, L) fills in input j of the wire order (key,
-// dims, wire dtype, flags; field, payload_len) and payload(o, j, t, L) writes, skips or records its payload_len bytes.
+// The framing of one PredictRequest through `o`: [00 be32(msg)] model_spec {entry header, tensor header, payload}* output_filter.
+// `Req` supplies what differs between the callers: spec(o) writes the model_spec field, input(j, t, L) fills in input j of the
+// wire order (key, dims, wire dtype, flags; field, payload_len), payload(o, j, t, L) writes, skips or records its payload_len
+// bytes and tail(o) writes the output_filter run.
 template <class Out, class Req>
 B2_HD void write_request(Out& o, Req& q, uint32_t n_in, bool grpc, uint64_t msg) {
   if (grpc) { o.byte(0); o.byte((uint8_t)(msg >> 24)); o.byte((uint8_t)(msg >> 16)); o.byte((uint8_t)(msg >> 8)); o.byte((uint8_t)msg); }
@@ -132,6 +149,7 @@ B2_HD void write_request(Out& o, Req& q, uint32_t n_in, bool grpc, uint64_t msg)
     write_tensor_header(o, t, L);
     q.payload(o, j, t, L);
   }
+  q.tail(o);
 }
 
 // ---- the deferred encode (plan.h "deferred framing") ----------------------------------------------------------------------
@@ -145,6 +163,7 @@ struct DeferredRequest {
   DeferredIn in{};                 // the input input() read last
   uint64_t align_at = 0;           // count pass: where input q.align_in's payload starts, from the record's first byte
   template <class Out> B2_HD void spec(Out& o) { o.bytes(ft.blob + q.spec_off, q.spec_len); }
+  template <class Out> B2_HD void tail(Out& o) { o.bytes(ft.blob + q.spec_off + q.spec_len, q.tail_len); }
   B2_HD void input(uint32_t j, b200tfs_tensor& t, TensorLayout& L) {
     in = ft.ins[q.first_in + j];
     t.key = (const char*)ft.blob + in.key_off; t.key_len = in.key_len;

@@ -365,7 +365,7 @@ struct DeferredReq {
   uint32_t first_in, n_in;
   uint32_t align_in;             // the input whose payload should start 128-byte aligned (request-local), ~0u: none
   uint32_t anchor_in;            // ~0u, or a DP_ITEM input whose first byte the host fixed at anchor_off: the record is laid out around it
-  uint32_t pad;
+  uint32_t tail_len;             // the output_filter run, in FrameTables::blob right behind the model_spec field
   uint64_t anchor_off;
   uint64_t slot_off, slot_cap;   // where the record may lie inside the arena (worst-case sized by the host)
 };
@@ -408,7 +408,7 @@ struct ExFeat {             // one column of one request, in wire order
   uint64_t data_len;        // (row_stride = row_elems, or 0 for a broadcast column).  Last: the dense and ragged kernels never read them
 };
 // The prefix the frame kernel writes in front of the examples, for both targets:
-//   [00 be32(msg)] spec 12 vi(outer) mid inner_tag vi(inner) head | examples
+//   [00 be32(msg)] spec 12 vi(outer) mid inner_tag vi(inner) head | examples [output_filter run: Predict only]
 //   example_list (Classify / Regress):  outer = Input, mid and head empty, inner_tag 0A, inner = ExampleList
 //   Predict string_val:                 outer = the inputs map entry, mid = 0A vi(klen) key, inner_tag 12, inner = TensorProto,
 //                                       head = 08 07 12 vi(shape) {tensor_shape: dim {size: n}}
@@ -425,6 +425,8 @@ struct ExReq {
   uint32_t mid_len, head_len, inner_tag;        // the Predict prefix above (example_list: 0, 0, 0A); last, because among the
                                                 // fields the emit kernel reads they cost ex_emit_kernel<false> 12 registers
   uint32_t n_ctx;                               // a SequenceExample request: its first n_ctx features (wire order) are context
+  uint32_t tail_len, pad_;                      // a Predict form's output_filter run, in ExTables::blob behind head, written
+                                                // behind the examples (and the context) by the frame kernel
 };
 struct ExSpan { uint32_t req, pad; uint64_t e0, e1; };   // a CTA's examples [e0, e1) of request `req`
 // A call with contexts (ExampleListWithContext) plans each present context as one more request entry of one example, at an

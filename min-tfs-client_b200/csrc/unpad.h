@@ -118,9 +118,9 @@ B2_HD void unpad_str_rows(const UnpadIn& in, const UnpadBox& b, uint64_t* first,
 }
 
 struct UnpadFrame {                // what every request's framing has in common
-  const uint8_t* blob;             // model_spec field (its tag included) at 0, then the keys
+  const uint8_t* blob;             // model_spec field (its tag included) at 0, the output_filter run, then the keys
   uint32_t spec_len, grpc;         // grpc: gRPC's 5-byte length-prefixed-message header in front
-  uint32_t n_in, pad_;
+  uint32_t n_in, tail_len;         // tail_len: bytes of the output_filter run
 };
 
 // write_request's view of one request of the padded encode: every input from its box, payloads skipped
@@ -131,6 +131,7 @@ struct UnpadRequest {
   uint64_t* payload_off;           // may be null
   uint64_t o0;
   template <class Out> B2_HD void spec(Out& o) { o.bytes(F.blob, F.spec_len); }
+  template <class Out> B2_HD void tail(Out& o) { o.bytes(F.blob + F.spec_len, F.tail_len); }
   B2_HD void input(uint32_t j, b200tfs_tensor& t, TensorLayout& L) const {
     const UnpadIn& in = ins[j];
     t.wire_dtype = in.wire_dtype; t.rank = in.rank; t.flags = in.flags; t.dims = box[j].dims;

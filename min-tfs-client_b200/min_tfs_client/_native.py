@@ -54,6 +54,15 @@ class Request(C.Structure):
     ]
 
 
+class RequestSpec(C.Structure):
+    """b200tfs_request_spec: a request's ModelSpec.signature_name (signature_len 0: not written), ModelSpec.version_label
+    (version_label_len < 0: not set) and PredictRequest.output_filter (n_output_filter names), for the ``_spec`` entry points."""
+    _fields_ = [
+        ("signature_name", C.c_char_p), ("signature_len", C.c_int64), ("version_label", C.c_char_p), ("version_label_len", C.c_int64),
+        ("output_filter", C.POINTER(C.c_char_p)), ("output_filter_len", C.POINTER(C.c_int64)), ("n_output_filter", C.c_int64),
+    ]
+
+
 class Run(C.Structure):
     """b200tfs_run: `count` pieces of `len` value bytes, `stride` bytes apart, from TensorProto field `field`."""
     _fields_ = [("off", C.c_uint64), ("len", C.c_uint32), ("count", C.c_uint32), ("stride", C.c_uint32), ("field", C.c_uint32)]
@@ -224,12 +233,18 @@ SIGNATURES = {
     "b200tfs_order_keys": (C.c_int, [C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_int64), C.c_int32, _i32p]),
     "b200tfs_tensor_arena_size": (C.c_int, [C.c_int32, C.POINTER(Tensor), _u64p]),
     "b200tfs_request_arena_size": (C.c_int, [C.c_int32, C.POINTER(Request), _u64p]),
+    "b200tfs_request_size_spec": (C.c_int, [C.POINTER(Request), C.POINTER(RequestSpec), _u64p]),
+    "b200tfs_request_frame_spec": (C.c_int, [C.POINTER(Request), C.POINTER(RequestSpec), _vp, C.c_uint64, _u64p, _u64p, _u64p, _i32p]),
+    "b200tfs_request_arena_size_spec": (C.c_int, [C.c_int32, C.POINTER(Request), C.POINTER(RequestSpec), _u64p]),
     "b200tfs_measure": (C.c_int, [_vp, C.c_int32, C.POINTER(Tensor)]),
     "b200tfs_encode_tensor_protos": (C.c_int, [_vp, C.c_int32, C.POINTER(Tensor), _vp, C.c_uint64, _u64p, _u64p]),
     "b200tfs_encode_requests": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), _vp, C.c_uint64, _u64p, _u64p]),
     "b200tfs_encode_requests_async": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), _vp, C.c_uint64]),
     "b200tfs_encode_results": (C.c_int, [_vp, C.c_int32, _u64p, _u64p]),
     "b200tfs_request_frame_deferred": (C.c_int, [C.POINTER(Request), _u64p, _vp, C.c_uint64, _u64p, _u64p, _u64p, _u64p]),
+    "b200tfs_encode_requests_async_spec": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), C.POINTER(RequestSpec), _vp, C.c_uint64]),
+    "b200tfs_request_frame_deferred_spec": (C.c_int, [C.POINTER(Request), C.POINTER(RequestSpec), _u64p, _vp, C.c_uint64, _u64p, _u64p,
+                                                      _u64p, _u64p]),
     "b200tfs_parse_responses": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.c_int32, C.POINTER(Output), _i32p,
                                           C.POINTER(ModelSpec), _i32p]),
     "b200tfs_parse_tensor_protos": (C.c_int, [_vp, _vp, C.c_int32, _u64p, _u64p, C.POINTER(Output), _i32p]),
@@ -269,6 +284,12 @@ SIGNATURES = {
                                                                _vp, C.c_uint64]),
     "b200tfs_padded_request_frame_columns": (C.c_int, [C.POINTER(Request), C.POINTER(PadInput), C.POINTER(Bytes), _u64p, _vp, C.c_uint64,
                                                        _u64p, _u64p, _u64p]),
+    "b200tfs_padded_request_columns_arena_size_spec": (C.c_int, [C.c_int32, C.POINTER(Request), C.POINTER(Bytes), C.POINTER(RequestSpec),
+                                                                 _u64p]),
+    "b200tfs_encode_padded_requests_columns_async_spec": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), C.POINTER(PadInput),
+                                                                    C.POINTER(Bytes), C.POINTER(RequestSpec), _vp, C.c_uint64]),
+    "b200tfs_padded_request_frame_columns_spec": (C.c_int, [C.POINTER(Request), C.POINTER(PadInput), C.POINTER(Bytes),
+                                                            C.POINTER(RequestSpec), _u64p, _vp, C.c_uint64, _u64p, _u64p, _u64p]),
     "b200tfs_capture_begin": (C.c_int, [_vp]),
     "b200tfs_capture_end": (C.c_int, [_vp, _vpp]),
     "b200tfs_graph_launch": (C.c_int, [_vp, _vp]),
@@ -276,6 +297,8 @@ SIGNATURES = {
     "b200tfs_wait_event": (C.c_int, [_vp, _vp]),
     "b200tfs_encode_requests_host": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), _vp, C.c_uint64, _u64p, _u64p]),
     "b200tfs_encode_requests_host_async": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), _vp, C.c_uint64, _u64p, _u64p]),
+    "b200tfs_encode_requests_host_spec": (C.c_int, [_vp, C.c_int32, C.POINTER(Request), C.POINTER(RequestSpec), _vp, C.c_uint64, _u64p,
+                                                    _u64p]),
     "b200tfs_pipelined_calls": (C.c_int, [_vp, _u64p]),
     "b200tfs_direct_calls": (C.c_int, [_vp, _u64p]),
     "b200tfs_set_pipeline": (C.c_int, [_vp, C.c_uint64, C.c_int32]),
@@ -345,6 +368,20 @@ SIGNATURES = {
                                                         C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
                                                         C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), _vp, C.c_uint64, _u64p,
                                                         _u64p]),
+    "b200tfs_example_specs_request_size": (C.c_int, [C.POINTER(ExampleRequest), C.POINTER(ExampleTarget), C.POINTER(ExampleContext),
+                                                     C.POINTER(ExampleTasks), C.POINTER(Ragged), C.POINTER(ExampleSequence),
+                                                     C.POINTER(RequestSpec), _u64p]),
+    "b200tfs_example_specs_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                   C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                   C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), C.POINTER(RequestSpec), _u64p]),
+    "b200tfs_encode_example_specs_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                     C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                     C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), C.POINTER(RequestSpec), _vp,
+                                                     C.c_uint64]),
+    "b200tfs_encode_example_specs_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                    C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                    C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), C.POINTER(RequestSpec), _vp,
+                                                    C.c_uint64, _u64p, _u64p]),
     "b200tfs_multi_inference_response_bound": (C.c_int, [C.c_int32, _i32p, C.c_int32, _u64p, _u64p, _u64p]),
     "b200tfs_decode_multi_inference_responses": (C.c_int, [_vp, C.c_int32, _i32p, _vp, C.c_int32, _u64p, _u64p, _vpp, _u64p, _vpp,
                                                            _u64p]),

@@ -192,6 +192,54 @@ class _Prepared:
         self.nbytes, self.ndim, self.size, self.itemsize, self.kind = int(a.nbytes), a.ndim, int(a.size), a.dtype.itemsize, a.dtype.kind
 
 
+def _utf8(what: str, v) -> bytes:
+    """A protobuf string field's bytes: ``str`` as UTF-8, ``bytes`` as given if they are valid UTF-8 (ValueError otherwise, as protobuf
+    refuses them)."""
+    if isinstance(v, str):
+        return v.encode("utf-8")
+    b = bytes(v)
+    try:
+        b.decode("utf-8")
+    except UnicodeDecodeError:
+        raise ValueError(f"{what} {b!r} is not valid UTF-8") from None
+    return b
+
+
+class _RequestSpec:
+    """The signature_name, version_label and output_filter of one encode call as a ``b200tfs_request_spec`` (``struct``) and the
+    bytes its fields point at; ``extra`` bounds the wire bytes they add to a request."""
+
+    __slots__ = ("struct", "keep", "extra")
+
+    def __init__(self, signature_name, version_label, output_filter):
+        sig = b"" if signature_name is None else _utf8("signature_name", signature_name)
+        label = None if version_label is None else _utf8("version_label", version_label)
+        if isinstance(output_filter, (str, bytes)):
+            raise TypeError("output_filter is a sequence of output names, not one name")
+        names = [] if output_filter is None else [_utf8("output_filter name", x) for x in output_filter]
+        ptrs = (C.c_char_p * max(len(names), 1))(*names)
+        lens = (C.c_int64 * max(len(names), 1))(*[len(x) for x in names])
+        self.struct = N.RequestSpec(signature_name=sig, signature_len=len(sig), version_label=label,
+                                    version_label_len=-1 if label is None else len(label), output_filter=ptrs, output_filter_len=lens,
+                                    n_output_filter=len(names))
+        self.keep = (sig, label, names, ptrs, lens)
+        self.extra = 32 + len(sig) + len(label or b"") + sum(11 + len(x) for x in names)
+
+    @staticmethod
+    def of(model_versions, signature_name=None, version_label=None, output_filter=None) -> Optional["_RequestSpec"]:
+        """None when the call sets none of the three (its bytes are then those of a call without them)."""
+        if signature_name is None and version_label is None and output_filter is None:
+            return None
+        if version_label is not None and any(v is not None for v in model_versions):
+            raise ValueError("model_version and version_label are members of one oneof (ModelSpec.version_choice): give at most one")
+        return _RequestSpec(signature_name, version_label, output_filter)
+
+    @staticmethod
+    def array(spec: Optional["_RequestSpec"], n: int):
+        """n copies of the struct for the per-request _spec entry points (None: NULL)."""
+        return None if spec is None else (N.RequestSpec * n)(*([spec.struct] * n))
+
+
 def _wire_bound(p: "_Prepared", tensor_content: bool) -> int:
     """Upper bound of the bytes one prepared tensor occupies on the wire (payload + its own framing)."""
     frame = 64 + 16 * max(p.ndim, 1) + len(p.key)
@@ -458,13 +506,15 @@ def _sequence_count(context_dict: Mapping, feature_list_dict: Mapping) -> int:
 
 
 def _host_example_request(model_name, model_version, input_dict, grpc_frame: bool, predict_input=None, context_dict=None,
-                          tasks=None) -> bytes:
+                          tasks=None, **fields) -> bytes:
     """A request with a column the device route does not take, as ``examples_from_input_dict`` and protobuf make it: a
     ClassificationRequest, or with ``predict_input`` a PredictRequest whose input of that key is the DT_STRING ``[n]`` tensor of
     the examples, each serialized with ``deterministic=True``.  With ``context_dict`` the examples and the context form an
     ExampleListWithContext (``examples_with_context_from_input_dict``): the ClassificationRequest's input, or the one string of a
-    DT_STRING ``[1]`` tensor.  With ``tasks`` the request is the MultiInferenceRequest ``make_multi_inference_request`` builds."""
-    from .requests import TensorServingClient, examples_from_input_dict, examples_with_context_from_input_dict, make_multi_inference_request
+    DT_STRING ``[1]`` tensor.  With ``tasks`` the request is the MultiInferenceRequest ``make_multi_inference_request`` builds.
+    ``fields``: signature_name / version_label / output_filter (``requests.apply_spec_fields``)."""
+    from .requests import (TensorServingClient, apply_spec_fields, examples_from_input_dict, examples_with_context_from_input_dict,
+                           make_multi_inference_request)
 
     if tasks is not None:
         req = make_multi_inference_request(model_name, model_version, tasks, input_dict, context_dict)
@@ -488,7 +538,7 @@ def _host_example_request(model_name, model_version, input_dict, grpc_frame: boo
         t.dtype = DT_STRING
         t.tensor_shape.dim.add().size = len(values)
         t.string_val.extend(e.SerializeToString(deterministic=True) for e in values)
-    wire = req.SerializeToString(deterministic=True)
+    wire = apply_spec_fields(req, model_version, **fields).SerializeToString(deterministic=True)
     return (b"\x00" + len(wire).to_bytes(4, "big") + wire) if grpc_frame else wire
 
 
@@ -776,7 +826,8 @@ class Codec:
 
     def encode_predict_requests(self, requests: Iterable[Tuple[str, Optional[int], Union[Mapping, Sequence]]], *,
                                 order="deterministic", wire_dtype=None, tensor_content: bool = False,
-                                keep_snan: bool = False, grpc_frame: bool = False, out=None) -> List[bytes]:
+                                keep_snan: bool = False, grpc_frame: bool = False, out=None, signature_name=None,
+                                version_label=None, output_filter=None) -> List[bytes]:
         """Each item is ``(model_name, model_version, inputs)``; returns one PredictRequest wire per item.
 
         The bytes equal ``PredictRequest.SerializeToString(deterministic=True)`` of the message the
@@ -790,44 +841,52 @@ class Codec:
         each string's raw bytes (NULs and high bytes kept), so binary data such as an encoded image can be sent; its offsets must
         rise within ``0..data_len`` and ``wire_dtype`` must be DT_STRING if given (ValueError).  A ``BytesColumn`` of device arrays
         raises ValueError: ``encode_predict_requests_padded`` encodes those on the device.
+
+        ``signature_name``, ``version_label`` and ``output_filter`` (a sequence of output names) set ``model_spec.signature_name``,
+        ``model_spec.version_label`` and ``output_filter`` of every request of the call (``str``, or ``bytes`` that are valid UTF-8).
+        ``version_label`` is in a oneof with the version: a request with a ``model_version`` raises ValueError.  None leaves a field
+        unset, and the bytes are those of a call without it.
         """
-        keep, structs = self._build_requests(list(requests), order, wire_dtype, tensor_content, keep_snan, grpc_frame)
+        requests = list(requests)
+        spec = _RequestSpec.of([v for _, v, _ in requests], signature_name, version_label, output_filter)
+        keep, structs = self._build_requests(requests, order, wire_dtype, tensor_content, keep_snan, grpc_frame)
         n = len(structs)
         if n == 0:
             return []
         reqs = (N.Request * n)(*structs)
+        specs = _RequestSpec.array(spec, n)
         if out is not None and out != "pinned":
             raise ValueError('out must be None or "pinned"')
         if n == 1 and out is None:
             # one request whose size is closed-form (no varint-packed input): copy straight into the bytes object
             total = C.c_uint64()
-            if _HAVE_NEW_BYTES and self._lib.b200tfs_request_size(reqs, C.byref(total)) == N.OK:
+            if _HAVE_NEW_BYTES and self._lib.b200tfs_request_size_spec(reqs, specs, C.byref(total)) == N.OK:
                 obj, addr = _new_bytes(int(total.value))
                 off = (C.c_uint64 * 1)()
                 ln = (C.c_uint64 * 1)()
-                N.check(self._lib.b200tfs_encode_requests_host(self._ctx, 1, reqs, addr, total.value, off, ln))
+                N.check(self._lib.b200tfs_encode_requests_host_spec(self._ctx, 1, reqs, specs, addr, total.value, off, ln))
                 if off[0] != 0 or ln[0] != total.value:
                     raise N.NativeError(N.E_ARG, f"encoded length {ln[0]} at {off[0]} does not match the planned {total.value}")
                 return [obj]
         cap = 0
         for preps, _, name in keep:
-            cap += 1024 + len(name)
+            cap += 1024 + len(name) + (spec.extra if spec else 0)
             for p in preps:
                 cap += _wire_bound(p, tensor_content) + 512
         off = (C.c_uint64 * n)()
         ln = (C.c_uint64 * n)()
         if out == "pinned":
             pw = self._pinned_wire(cap)
-            N.check(self._lib.b200tfs_encode_requests_host(self._ctx, n, reqs, pw.ptr, cap, off, ln))
+            N.check(self._lib.b200tfs_encode_requests_host_spec(self._ctx, n, reqs, specs, pw.ptr, cap, off, ln))
             return [pw.array[off[i]: off[i] + ln[i]] for i in range(n)]
         wire = np.empty(cap, dtype=np.uint8)
-        N.check(self._lib.b200tfs_encode_requests_host(self._ctx, n, reqs, wire.ctypes.data, cap, off, ln))
+        N.check(self._lib.b200tfs_encode_requests_host_spec(self._ctx, n, reqs, specs, wire.ctypes.data, cap, off, ln))
         return [wire[off[i]: off[i] + ln[i]].tobytes() for i in range(n)]
 
     def encode_predict_requests_padded(self, model_name: str, inputs: Mapping, shapes: Mapping, *, model_version: Optional[int] = None,
                                        broadcast: Optional[Mapping] = None, order="deterministic", wire_dtype=None,
                                        tensor_content: bool = False, keep_snan: bool = False, grpc_frame: bool = False,
-                                       out=None) -> List[bytes]:
+                                       out=None, signature_name=None, version_label=None, output_filter=None) -> List[bytes]:
         """n PredictRequests cut out of one padded tensor per input - the inverse of ``decode_predict_responses_padded``.
 
         ``inputs[key]`` is a padded tensor ``P`` of shape ``[R, D_1, ..., D_{m-1}]``; ``shapes[key]`` gives each request's shape for it,
@@ -845,9 +904,13 @@ class Codec:
         stay within ``0..data_len``.  Host offsets are checked over the whole column before anything runs; device offsets are checked
         by the kernels, only where a box reads them; either way a break raises ValueError.  Numpy str / bytes / object inputs, more
         than 8 padded or 8 broadcast inputs and ranks above 16 are cut on the host and encoded request by request.
+
+        ``signature_name``, ``version_label`` and ``output_filter`` as for ``encode_predict_requests``: the same for every request.
         """
         if out is not None and out != "pinned":
             raise ValueError('out must be None or "pinned"')
+        named = dict(signature_name=signature_name, version_label=version_label, output_filter=output_filter)
+        spec = _RequestSpec.of([model_version], **named)
         broadcast = dict(broadcast or {})
         if set(inputs) != set(shapes):
             raise ValueError("shapes must have exactly the keys of inputs")
@@ -893,7 +956,7 @@ class Codec:
         if (any(dt.kind in "OUS" for dt in dtypes) or len(inputs) > N.CONCAT_MAX_KEYS or len(broadcast) > N.CONCAT_MAX_KEYS
                 or any(len(r) > N.MAX_RANK for r in ranks)):
             return self._padded_requests_on_host(model_name, model_version, inputs, shapes, broadcast, n, order=order, wire_dtype=wire_dtype,
-                                                 tensor_content=tensor_content, keep_snan=keep_snan, grpc_frame=grpc_frame, out=out)
+                                                 tensor_content=tensor_content, keep_snan=keep_snan, grpc_frame=grpc_frame, out=out, **named)
         keep = []
 
         def dev(v):
@@ -937,19 +1000,14 @@ class Codec:
                         flags=N.RF_GRPC_FRAME if grpc_frame else 0, inputs=arr)
         cap = C.c_uint64()
         bs = (N.Bytes * len(strs))(*strs) if any(b.offsets for b in strs) else None
-        if bs is None:
-            N.check(self._lib.b200tfs_padded_request_arena_size(n, C.byref(req), C.byref(cap)))
-        else:
-            N.check(self._lib.b200tfs_padded_request_columns_arena_size(n, C.byref(req), bs, C.byref(cap)))
+        sp = None if spec is None else C.byref(spec.struct)
+        N.check(self._lib.b200tfs_padded_request_columns_arena_size_spec(n, C.byref(req), bs, sp, C.byref(cap)))
         if self._pe_arena is None or self._pe_arena.nbytes < cap.value:
             if self._pe_arena is not None:
                 self._pe_arena.free()
             self._pe_arena = D.DeviceArray(self, (max(int(cap.value), 1),), np.uint8)
-        if bs is None:
-            N.check(self._lib.b200tfs_encode_padded_requests_async(self._ctx, n, C.byref(req), pin_arr, self._pe_arena.ptr, cap.value))
-        else:
-            N.check(self._lib.b200tfs_encode_padded_requests_columns_async(self._ctx, n, C.byref(req), pin_arr, bs, self._pe_arena.ptr,
-                                                                            cap.value))
+        N.check(self._lib.b200tfs_encode_padded_requests_columns_async_spec(self._ctx, n, C.byref(req), pin_arr, bs, sp, self._pe_arena.ptr,
+                                                                             cap.value))
         off, ln = (C.c_uint64 * n)(), (C.c_uint64 * n)()
         rc = self._lib.b200tfs_encode_results(self._ctx, n, off, ln)
         if rc in (N.E_SHAPE, N.E_SIZE):
@@ -1016,7 +1074,8 @@ class Codec:
         return self.encode_predict_requests([(model_name, model_version, input_dict)], **kw)[0]
 
     def encode_example_requests(self, requests: Iterable[Tuple], *, order="deterministic",
-                                grpc_frame: bool = False, predict_input=None, tasks=None) -> List[bytes]:
+                                grpc_frame: bool = False, predict_input=None, tasks=None, signature_name=None, version_label=None,
+                                output_filter=None) -> List[bytes]:
         """Each item is ``(model_name, model_version, input_dict)``; returns one ClassificationRequest / RegressionRequest wire
         per item (the two messages share their field numbers, so the bytes serve both RPCs).  With ``predict_input`` (a str or
         bytes key) each wire is instead a PredictRequest for a model that parses serialized tf.Examples: its one input of that
@@ -1044,7 +1103,21 @@ class Codec:
         ``REGRESS_METHOD_NAME`` (requests.py) - every wire is instead the MultiInferenceRequest ``make_multi_inference_request``
         builds: one InferenceTask per task, each naming the item's model and version and the task's signature (an empty or None
         one: the server's default), over the Input the item has without tasks.  ``tasks`` with ``predict_input`` raises ValueError.
+
+        ``signature_name`` and ``version_label`` set those model_spec fields of every request (with ``tasks``: the label goes into
+        every task's model_spec, and ``signature_name`` raises ValueError, since each task names its own); ``output_filter`` sets
+        the PredictRequest's output_filter and needs ``predict_input`` (ValueError otherwise).  A label beside a ``model_version``
+        and bytes that are not UTF-8 raise ValueError; None leaves a field unset, and the bytes are those of a call without it.
         """
+        items = list(requests)
+        fields = {k: v for k, v in dict(signature_name=signature_name, version_label=version_label, output_filter=output_filter).items()
+                  if v is not None}
+        if output_filter is not None and predict_input is None:
+            raise ValueError("output_filter is a PredictRequest field: it needs predict_input (a Classify, Regress or MultiInference "
+                             "request has none)")
+        if signature_name is not None and tasks is not None:
+            raise ValueError("a MultiInference request names a signature per task, not one for the whole request")
+        spec = _RequestSpec.of([item[1] for item in items], signature_name, version_label, output_filter)
         order_code = _ORDER[order] if isinstance(order, str) else int(order)
         task_arr = None
         if tasks is not None:
@@ -1060,7 +1133,6 @@ class Codec:
         pkey = None
         if predict_input is not None:
             pkey = predict_input.encode("utf-8") if isinstance(predict_input, str) else bytes(predict_input)
-        items = list(requests)
         out: List[Optional[bytes]] = [None] * len(items)
         keep, structs, dev_idx, ragged, strs, targets, contexts, ctx_strs = [], [], [], [], [], [], [], []
         for i, item in enumerate(items):
@@ -1069,7 +1141,8 @@ class Codec:
             cols = _example_columns(input_dict)
             ccols = _example_columns(context_dict, context=True) if context_dict is not None else None
             if cols is None or (context_dict is not None and ccols is None):
-                out[i] = _host_example_request(model_name, model_version, input_dict, grpc_frame, predict_input, context_dict, tasks)
+                out[i] = _host_example_request(model_name, model_version, input_dict, grpc_frame, predict_input, context_dict, tasks,
+                                               **fields)
                 continue
             n, preps = cols
             if ccols is None:
@@ -1104,18 +1177,20 @@ class Codec:
             tk = None
             if task_arr is not None:
                 tk = (N.ExampleTasks * m)(*[N.ExampleTasks(tasks=C.addressof(task_arr), n_tasks=len(task_arr))] * m)
-            N.check(self._lib.b200tfs_example_tasks_arena_size(m, reqs, bs, tg, ct, cb, tk, C.byref(cap)))
+            rg = (N.Ragged * len(ragged))(*ragged) if any(g.lengths for g in ragged) else None
+            specs = _RequestSpec.array(spec, m)
+            N.check(self._lib.b200tfs_example_specs_arena_size(m, reqs, None, bs, tg, ct, cb, tk, None, specs, C.byref(cap)))
             wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
             off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
-            rg = (N.Ragged * len(ragged))(*ragged) if any(g.lengths for g in ragged) else None
-            N.check(self._lib.b200tfs_encode_example_tasks_host(self._ctx, m, reqs, rg, bs, tg, ct, cb, tk, wire.ctypes.data, cap.value,
-                                                                off, ln))
+            N.check(self._lib.b200tfs_encode_example_specs_host(self._ctx, m, reqs, rg, bs, tg, ct, cb, tk, None, specs, wire.ctypes.data,
+                                                                cap.value, off, ln))
             for j, i in enumerate(dev_idx):
                 out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
         return out  # type: ignore[return-value]
 
     def encode_sequence_example_requests(self, requests: Iterable[Tuple], *, input_key, order="deterministic",
-                                         grpc_frame: bool = False) -> List[bytes]:
+                                         grpc_frame: bool = False, signature_name=None, version_label=None,
+                                         output_filter=None) -> List[bytes]:
         """Each item is ``(model_name, model_version, context_dict, feature_list_dict)``; returns one PredictRequest wire per item
         for a model that parses serialized tf.SequenceExamples: its one input ``input_key`` is the DT_STRING ``[n]`` tensor of the
         sequences ``requests.sequence_examples_from_input_dict`` builds, each serialized with ``deterministic=True`` - the bytes of
@@ -1127,19 +1202,23 @@ class Codec:
         range raise ValueError); step t of sequence i is one Feature of ``value[i, t]``.  ``order="given"`` lists the context and
         the feature lists in insertion order.  An item with a numpy str / bytes value, or a dtype the device route does not take,
         is assembled on the host by ``make_predict_sequence_examples_request`` (deterministic order); device arrays of such dtypes
-        raise ValueError."""
+        raise ValueError.  ``signature_name``, ``version_label`` and ``output_filter`` as for ``encode_predict_requests``."""
         from .requests import make_predict_sequence_examples_request
 
+        items = list(requests)
+        fields = {k: v for k, v in dict(signature_name=signature_name, version_label=version_label, output_filter=output_filter).items()
+                  if v is not None}
+        spec = _RequestSpec.of([item[1] for item in items], signature_name, version_label, output_filter)
         order_code = _ORDER[order] if isinstance(order, str) else int(order)
         pkey = input_key.encode("utf-8") if isinstance(input_key, str) else bytes(input_key)
-        items = list(requests)
         out: List[Optional[bytes]] = [None] * len(items)
         keep, structs, dev_idx, ragged, strs, targets, seqs = [], [], [], [], [], [], []
         for i, (model_name, model_version, context_dict, feature_list_dict) in enumerate(items):
             n = _sequence_count(context_dict, feature_list_dict)
             ccols, lcols = _example_columns(context_dict), _example_columns(feature_list_dict)
             if ccols is None or lcols is None:
-                req = make_predict_sequence_examples_request(model_name, model_version, context_dict, feature_list_dict, pkey.decode("utf-8"))
+                req = make_predict_sequence_examples_request(model_name, model_version, context_dict, feature_list_dict, pkey.decode("utf-8"),
+                                                             **fields)
                 wire = req.SerializeToString(deterministic=True)
                 out[i] = (b"\x00" + len(wire).to_bytes(4, "big") + wire) if grpc_frame else wire
                 continue
@@ -1171,11 +1250,12 @@ class Codec:
             rg = (N.Ragged * max(len(ragged), 1))(*ragged)
             bs = (N.Bytes * len(strs))(*strs) if any(b.offsets for b in strs) else None
             cap = C.c_uint64()
-            N.check(self._lib.b200tfs_example_sequences_arena_size(m, reqs, rg, bs, tg, None, None, None, sq, C.byref(cap)))
+            specs = _RequestSpec.array(spec, m)
+            N.check(self._lib.b200tfs_example_specs_arena_size(m, reqs, rg, bs, tg, None, None, None, sq, specs, C.byref(cap)))
             wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
             off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
-            N.check(self._lib.b200tfs_encode_example_sequences_host(self._ctx, m, reqs, rg, bs, tg, None, None, None, sq, wire.ctypes.data,
-                                                                    cap.value, off, ln))
+            N.check(self._lib.b200tfs_encode_example_specs_host(self._ctx, m, reqs, rg, bs, tg, None, None, None, sq, specs, wire.ctypes.data,
+                                                                cap.value, off, ln))
             for j, i in enumerate(dev_idx):
                 out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
         return out  # type: ignore[return-value]

@@ -149,11 +149,54 @@ def sequence_examples_from_input_dict(context_dict: Dict[str, np.ndarray], featu
     return out
 
 
+class SpecFields(dict):
+    """``signature_name`` / ``version_label`` / ``output_filter`` as the last element of a ``gpu_*_serializer`` request tuple."""
+
+
+def _split_fields(request):
+    """(the request tuple without its SpecFields, the fields as keywords)"""
+    if request and isinstance(request[-1], SpecFields):
+        return tuple(request[:-1]), dict(request[-1])
+    return tuple(request), {}
+
+
+def _fields(signature_name=None, version_label=None, output_filter=None) -> SpecFields:
+    return SpecFields({k: v for k, v in dict(signature_name=signature_name, version_label=version_label,
+                                             output_filter=output_filter).items() if v is not None})
+
+
+def apply_spec_fields(req, model_version=None, signature_name=None, version_label=None, output_filter=None):
+    """Set ``signature_name``, ``version_label`` and ``output_filter`` (None: left unset) on a request protobuf builds: every
+    task's model_spec of a MultiInferenceRequest (whose tasks carry their own signatures), else the request's model_spec.
+    ValueError, as ``Codec`` raises it, for a label beside a version, bytes that are not UTF-8, a filter on a request that is not
+    a PredictRequest and a signature beside tasks."""
+    from .codec import _RequestSpec
+
+    s = _RequestSpec.of([model_version], signature_name, version_label, output_filter)
+    if s is None:
+        return req
+    sig, label, names = s.keep[0], s.keep[1], s.keep[2]
+    multi = req.DESCRIPTOR.name == "MultiInferenceRequest"
+    if multi and signature_name is not None:
+        raise ValueError("a MultiInference request names a signature per task, not one for the whole request")
+    if output_filter is not None and req.DESCRIPTOR.name != "PredictRequest":
+        raise ValueError("output_filter is a PredictRequest field: a Classify, Regress or MultiInference request has none")
+    for spec in [t.model_spec for t in req.tasks] if multi else [req.model_spec]:
+        if sig:
+            spec.signature_name = sig.decode("utf-8")
+        if label is not None:
+            spec.version_label = label.decode("utf-8")
+    if output_filter is not None:
+        req.output_filter.extend(x.decode("utf-8") for x in names)
+    return req
+
+
 def make_predict_sequence_examples_request(model_name: str, model_version: Optional[int], context_dict, feature_list_dict,
-                                           input_key: str):
+                                           input_key: str, *, signature_name=None, version_label=None, output_filter=None):
     """``PredictRequest`` whose one input ``input_key`` is the DT_STRING ``[n]`` tensor of the sequences
     ``sequence_examples_from_input_dict`` builds, each serialized with ``deterministic=True`` - what
-    ``Codec.encode_sequence_example_requests`` encodes on the GPU."""
+    ``Codec.encode_sequence_example_requests`` encodes on the GPU.  ``signature_name``, ``version_label`` and ``output_filter``
+    set those fields (``apply_spec_fields``)."""
     from tensorflow.core.framework.types_pb2 import DT_STRING
     from tensorflow_serving.apis.predict_pb2 import PredictRequest
 
@@ -166,7 +209,7 @@ def make_predict_sequence_examples_request(model_name: str, model_version: Optio
     t.dtype = DT_STRING
     t.tensor_shape.dim.add().size = len(seqs)
     t.string_val.extend(s.SerializeToString(deterministic=True) for s in seqs)
-    return req
+    return apply_spec_fields(req, model_version, signature_name, version_label, output_filter)
 
 
 def _checked_tasks(tasks) -> List[Tuple[str, str]]:
@@ -183,12 +226,15 @@ def _checked_tasks(tasks) -> List[Tuple[str, str]]:
 
 
 def make_multi_inference_request(model_name: str, model_version: Optional[int], tasks: Sequence[Tuple[str, str]],
-                                 input_dict: Dict[str, np.ndarray], context_dict=None):
+                                 input_dict: Dict[str, np.ndarray], context_dict=None, *, signature_name=None, version_label=None,
+                                 output_filter=None):
     """``MultiInferenceRequest`` (inference.proto) running every task ``(signature_name, method_name)`` of the model over one
     Input: ``examples_from_input_dict(input_dict)``, or with ``context_dict`` ``examples_with_context_from_input_dict``.  Each
     task's model_spec names the model, the version (when not None) and the signature (an empty or None one: not set, the server's
     default); its method_name is ``CLASSIFY_METHOD_NAME`` or ``REGRESS_METHOD_NAME`` (anything else raises ValueError, as does an
-    empty task list).  What ``Codec.encode_example_requests(..., tasks=...)`` encodes on the GPU."""
+    empty task list).  What ``Codec.encode_example_requests(..., tasks=...)`` encodes on the GPU.  ``version_label`` goes into every
+    task's model_spec behind its signature; ``signature_name`` (each task names its own) and ``output_filter`` (a PredictRequest
+    field) raise ValueError."""
     from tensorflow_serving.apis.inference_pb2 import MultiInferenceRequest
 
     req = MultiInferenceRequest()
@@ -205,7 +251,7 @@ def make_multi_inference_request(model_name: str, model_version: Optional[int], 
         req.input.CopyFrom(examples_from_input_dict(input_dict))
     else:
         req.input.CopyFrom(examples_with_context_from_input_dict(input_dict, context_dict))
-    return req
+    return apply_spec_fields(req, model_version, signature_name, version_label, output_filter)
 
 
 class PredictResponseView:
@@ -313,18 +359,23 @@ def gpu_regression_response_deserializer(wire: bytes) -> RegressionResponseView:
 
 
 def gpu_request_serializer(request) -> bytes:
-    """``request_serializer`` for ``channel.unary_unary``: (model_name, model_version, input_dict) -> bytes.  A DT_STRING input may
-    be a numpy str array (UTF-8, as the reference) or a ``BytesColumn`` of host arrays, whose strings go out as their raw bytes -
-    how a request carries binary data such as encoded images."""
-    model_name, model_version, input_dict = request
-    return get_codec().encode_predict_request(model_name, input_dict, model_version)
+    """``request_serializer`` for ``channel.unary_unary``: (model_name, model_version, input_dict[, spec]) -> bytes.  A DT_STRING input
+    may be a numpy str array (UTF-8, as the reference) or a ``BytesColumn`` of host arrays, whose strings go out as their raw bytes -
+    how a request carries binary data such as encoded images.  ``spec``, a dict of ``signature_name`` / ``version_label`` /
+    ``output_filter``, sets those fields (``Codec.encode_predict_requests``)."""
+    request, spec = _split_fields(request)
+    model_name, model_version, input_dict = request[:3]
+    spec.update(request[3] if len(request) > 3 else {})
+    return get_codec().encode_predict_request(model_name, input_dict, model_version, **spec)
 
 
 def gpu_example_request_serializer(request) -> bytes:
     """``request_serializer`` for ``channel.unary_unary(CLASSIFY_METHOD | REGRESS_METHOD, ...)``: (model_name, model_version,
     input_dict[, context_dict]) -> the ClassificationRequest / RegressionRequest bytes ``_make_example_request`` would serialise,
-    packed on the GPU (with a context_dict that is not None: an ExampleListWithContext)."""
-    return get_codec().encode_example_requests([request])[0]
+    packed on the GPU (with a context_dict that is not None: an ExampleListWithContext).  A trailing ``SpecFields`` sets
+    ``signature_name`` / ``version_label``."""
+    request, spec = _split_fields(request)
+    return get_codec().encode_example_requests([request], **spec)[0]
 
 
 def gpu_predict_examples_serializer(request) -> bytes:
@@ -333,27 +384,31 @@ def gpu_predict_examples_serializer(request) -> bytes:
     tensor of the examples ``examples_from_input_dict`` builds, each serialized with ``deterministic=True``, packed on the GPU.
     (..., input_key, context_dict) with a context_dict that is not None: the input is instead the DT_STRING ``[1]`` tensor of the
     one ExampleListWithContext ``examples_with_context_from_input_dict`` builds (TF-Ranking's serving input)."""
+    request, spec = _split_fields(request)
     model_name, model_version, input_dict, input_key = request[:4]
     context_dict = request[4] if len(request) > 4 else None
-    return get_codec().encode_example_requests([(model_name, model_version, input_dict, context_dict)], predict_input=input_key)[0]
+    return get_codec().encode_example_requests([(model_name, model_version, input_dict, context_dict)], predict_input=input_key,
+                                               **spec)[0]
 
 
 def gpu_multi_inference_request_serializer(request) -> bytes:
     """``request_serializer`` for ``channel.unary_unary(MULTI_INFERENCE_METHOD, ...)``: (model_name, model_version, tasks,
     input_dict[, context_dict]) -> the bytes of ``make_multi_inference_request(...).SerializeToString(deterministic=True)``,
     packed on the GPU."""
+    request, spec = _split_fields(request)
     model_name, model_version, tasks, input_dict = request[:4]
     context_dict = request[4] if len(request) > 4 else None
-    return get_codec().encode_example_requests([(model_name, model_version, input_dict, context_dict)], tasks=tasks)[0]
+    return get_codec().encode_example_requests([(model_name, model_version, input_dict, context_dict)], tasks=tasks, **spec)[0]
 
 
 def gpu_predict_sequence_examples_serializer(request) -> bytes:
     """``request_serializer`` for ``channel.unary_unary(PREDICT_METHOD, ...)`` to a model that parses serialized
     tf.SequenceExamples: (model_name, model_version, context_dict, feature_list_dict, input_key) -> the bytes of
     ``make_predict_sequence_examples_request(...).SerializeToString(deterministic=True)``, packed on the GPU."""
+    request, spec = _split_fields(request)
     model_name, model_version, context_dict, feature_list_dict, input_key = request
     return get_codec().encode_sequence_example_requests([(model_name, model_version, context_dict, feature_list_dict)],
-                                                        input_key=input_key)[0]
+                                                        input_key=input_key, **spec)[0]
 
 
 def gpu_response_deserializer(wire: bytes) -> PredictResponseView:
@@ -382,11 +437,16 @@ class TensorServingClient:
                                                   response_deserializer=gpu_response_deserializer)
 
     def predict_request(self, model_name: str, input_dict: Dict[str, np.ndarray], timeout: int = 60,
-                        model_version: Optional[int] = None) -> PredictResponseView:
-        return self._predict((model_name, model_version, input_dict), timeout)
+                        model_version: Optional[int] = None, *, signature_name=None, version_label=None,
+                        output_filter=None) -> PredictResponseView:
+        """The reference's signature (requests.py:32-65), plus ``signature_name`` (a signature other than the server's default),
+        ``version_label`` (a labelled version such as ``"canary"``; not with ``model_version``) and ``output_filter`` (only these
+        outputs are computed and returned)."""
+        return self._predict((model_name, model_version, input_dict, _fields(signature_name, version_label, output_filter)), timeout)
 
     def predict_examples_request(self, model_name: str, input_dict: Dict[str, np.ndarray], input_key: str = "examples",
-                                 timeout: int = 60, model_version: Optional[int] = None, context_dict=None) -> PredictResponseView:
+                                 timeout: int = 60, model_version: Optional[int] = None, context_dict=None, *, signature_name=None,
+                                 version_label=None, output_filter=None) -> PredictResponseView:
         """Predict on a model whose signature takes serialized tf.Examples (a DT_STRING vector it parses with
         ``tf.io.parse_example``, e.g. a TFX Trainer or Estimator export's ``serving_default``): one example per row of
         ``input_dict`` as ``examples_from_input_dict`` builds it, sent as input ``input_key``.  Values may be ``RaggedColumn`` and
@@ -394,19 +454,23 @@ class TensorServingClient:
         ExampleListWithContext instead (a TF-Ranking model's serving input), the context holding the whole of each value."""
         call = self._channel.unary_unary(PREDICT_METHOD, request_serializer=gpu_predict_examples_serializer,
                                          response_deserializer=gpu_response_deserializer)
-        return call((model_name, model_version, input_dict, input_key, context_dict), timeout)
+        return call((model_name, model_version, input_dict, input_key, context_dict, _fields(signature_name, version_label, output_filter)),
+                    timeout)
 
     def predict_sequence_examples_request(self, model_name: str, context_dict, feature_list_dict, input_key: str, timeout: int = 60,
-                                          model_version: Optional[int] = None) -> PredictResponseView:
+                                          model_version: Optional[int] = None, *, signature_name=None, version_label=None,
+                                          output_filter=None) -> PredictResponseView:
         """Predict on a model whose signature takes serialized tf.SequenceExamples (a DT_STRING vector it parses with
         ``tf.io.parse_sequence_example``: a session or event-history model, or TF-Ranking's SequenceExample format): one sequence
         per row, as ``sequence_examples_from_input_dict(context_dict, feature_list_dict)`` builds it, sent as input
         ``input_key`` and packed on the GPU."""
         call = self._channel.unary_unary(PREDICT_METHOD, request_serializer=gpu_predict_sequence_examples_serializer,
                                          response_deserializer=gpu_response_deserializer)
-        return call((model_name, model_version, context_dict, feature_list_dict, input_key), timeout)
+        return call((model_name, model_version, context_dict, feature_list_dict, input_key,
+                     _fields(signature_name, version_label, output_filter)), timeout)
 
-    def _make_example_request(self, request_pb, model_name, input_dict, model_version, context_dict=None):
+    def _make_example_request(self, request_pb, model_name, input_dict, model_version, context_dict=None, signature_name=None,
+                              version_label=None):
         request = request_pb()
         request.model_spec.name = model_name
         if model_version is not None:
@@ -415,30 +479,33 @@ class TensorServingClient:
             request.input.CopyFrom(examples_from_input_dict(input_dict))
         else:
             request.input.CopyFrom(examples_with_context_from_input_dict(input_dict, context_dict))
-        return request
+        return apply_spec_fields(request, model_version, signature_name, version_label)
 
     def classification_request(self, model_name: str, input_dict: Dict[str, np.ndarray], timeout: int = 60,
-                               model_version: Optional[int] = None, context_dict=None):
+                               model_version: Optional[int] = None, context_dict=None, *, signature_name=None, version_label=None):
         """Same signature as the reference (requests.py:67-81); returns a ``ClassificationResponse``.  With ``context_dict`` the
         input is an ExampleListWithContext (``examples_with_context_from_input_dict``)."""
         from tensorflow_serving.apis.classification_pb2 import ClassificationRequest, ClassificationResponse
 
         call = self._channel.unary_unary(CLASSIFY_METHOD, request_serializer=ClassificationRequest.SerializeToString,
                                          response_deserializer=ClassificationResponse.FromString)
-        return call(self._make_example_request(ClassificationRequest, model_name, input_dict, model_version, context_dict), timeout)
+        return call(self._make_example_request(ClassificationRequest, model_name, input_dict, model_version, context_dict, signature_name,
+                                               version_label), timeout)
 
     def regression_request(self, model_name: str, input_dict: Dict[str, np.ndarray], timeout: int = 60,
-                           model_version: Optional[int] = None, context_dict=None):
+                           model_version: Optional[int] = None, context_dict=None, *, signature_name=None, version_label=None):
         """Same signature as the reference (requests.py:83-97); returns a ``RegressionResponse``.  With ``context_dict`` the
         input is an ExampleListWithContext (``examples_with_context_from_input_dict``)."""
         from tensorflow_serving.apis.regression_pb2 import RegressionRequest, RegressionResponse
 
         call = self._channel.unary_unary(REGRESS_METHOD, request_serializer=RegressionRequest.SerializeToString,
                                          response_deserializer=RegressionResponse.FromString)
-        return call(self._make_example_request(RegressionRequest, model_name, input_dict, model_version, context_dict), timeout)
+        return call(self._make_example_request(RegressionRequest, model_name, input_dict, model_version, context_dict, signature_name,
+                                               version_label), timeout)
 
     def multi_inference_request(self, model_name: str, input_dict: Dict[str, np.ndarray], tasks: Sequence[Tuple[str, str]],
-                                timeout: int = 60, model_version: Optional[int] = None, context_dict=None):
+                                timeout: int = 60, model_version: Optional[int] = None, context_dict=None, *, signature_name=None,
+                                version_label=None):
         """``PredictionService/MultiInference``: every task ``(signature_name, method_name)`` of the model - method_name
         ``CLASSIFY_METHOD_NAME`` or ``REGRESS_METHOD_NAME`` - over one Input, one example per row of ``input_dict`` (with
         ``context_dict``: an ExampleListWithContext), the request bytes packed on the GPU.  Returns a ``MultiInferenceResponse``
@@ -447,7 +514,7 @@ class TensorServingClient:
 
         call = self._channel.unary_unary(MULTI_INFERENCE_METHOD, request_serializer=gpu_multi_inference_request_serializer,
                                          response_deserializer=MultiInferenceResponse.FromString)
-        return call((model_name, model_version, tasks, input_dict, context_dict), timeout)
+        return call((model_name, model_version, tasks, input_dict, context_dict, _fields(signature_name, version_label)), timeout)
 
     def model_status_request(self, model_name: str, model_version: Optional[int] = None, timeout: Optional[int] = 10):
         """``ModelService/GetModelStatus`` as the reference issues it (requests.py:99-110: the version is set only when truthy)."""
