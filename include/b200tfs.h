@@ -1096,8 +1096,12 @@ int b200tfs_encode_example_specs_host(b200tfs_ctx* ctx, int32_t n, const b200tfs
  * Floats come back as the runtime gives them: an absent score / value is +0.0, -0.0 stays -0.0, a signalling NaN is quieted.
  * Fields in any order, the last of repeated scalar fields wins, unknown fields (groups included) are skipped at every level, a
  * known field with another wire type is an unknown field, repeated `result` fields merge (their entries concatenate), repeated
- * model_spec fields merge.  Malformed wire - truncation, tag 0, over-long varints, lengths past the end, wire types 6 / 7,
- * mismatched groups, a label or model_spec string that is not UTF-8 - is B200TFS_E_PARSE, where FromString raises DecodeError. */
+ * model_spec fields merge.  Malformed wire - truncation, tag 0, a tag written in more than 5 bytes or past 32 bits, over-long
+ * varints, lengths past the end, wire types 6 / 7, mismatched groups, a label or model_spec string that is not UTF-8 - is
+ * B200TFS_E_PARSE, where FromString raises DecodeError.
+ * One divergence: unknown groups nested more than 16 deep are B200TFS_E_PARSE here, while the runtime accepts them up to its
+ * recursion limit of 100 (the message levels above the group included).  Codec.decode_*_responses send such a batch to the host
+ * route, which gives the runtime's answer.                                                                                     */
 #define B200TFS_RESP_REGRESS 1
 #define B200TFS_RESP_CLASSIFY 2
 typedef struct b200tfs_label_ref {
@@ -1141,7 +1145,9 @@ int b200tfs_example_response_results(b200tfs_ctx* ctx, int32_t n, int64_t* per_r
  * groups are skipped at every level.  Per response and task, precedence as above: B200TFS_E_PARSE (malformed anywhere in the
  * response's results up to n_tasks; a malformed entry of a task's own result marks that task), B200TFS_E_SIZE, B200TFS_E_SHAPE
  * (a result count other than n_tasks - every task of the response -, a result whose member is not the one kinds[t] names - an
- * empty one included -, or an example with another class count than its task's C).
+ * empty one included -, or an example with another class count than its task's C).  Tags and groups as above: a tag of more
+ * than 5 bytes is B200TFS_E_PARSE, and so are unknown groups nested more than 16 deep, which the runtime accepts up to its
+ * recursion limit of 100 (Codec.decode_multi_inference_responses sends those to the host route).
  * Host only, closed form: max_rows[t] / max_values[t] (n_tasks entries each; either may be NULL) bound task t as
  * b200tfs_example_response_bound does.                                                                                        */
 int b200tfs_multi_inference_response_bound(int32_t n_tasks, const int32_t* kinds, int32_t n, const uint64_t* rec_len,

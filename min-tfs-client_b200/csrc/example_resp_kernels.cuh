@@ -79,7 +79,7 @@ __device__ __forceinline__ int64_t xr_field_end(const uint8_t* b, uint32_t p, ui
   }
   uint64_t t, v;
   const uint32_t i = xr_varint(b, avail, &t);
-  if (!i) return kXrErr;
+  if (!i || i > 5) return kXrErr;
   if (t > 0xFFFFFFFFull || (t >> 3) == 0) return kXrErr;   // rd_tag
   const uint32_t wt = (uint32_t)t & 7;
   if (wt == WT_I64) return avail - i < 8 ? kXrErr : (int64_t)p + i + 8;

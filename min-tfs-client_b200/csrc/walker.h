@@ -98,12 +98,21 @@ B2_HD uint64_t rd_varint(Cursor& c) {
   return 0;
 }
 
-// tag: must fit 32 bits, field number != 0
+// tag: at most 5 bytes (the runtime refuses a longer one, even of a small value), must fit 32 bits, field number != 0
 B2_HD uint32_t rd_tag(Cursor& c) {
-  const uint64_t t = rd_varint(c);
-  if (c.err) return 0;
-  if (t > 0xFFFFFFFFull || (t >> 3) == 0) { c.err = B200TFS_E_PARSE; return 0; }
-  return (uint32_t)t;
+  uint64_t t = 0;
+#pragma unroll 1
+  for (int i = 0; i < 5; ++i) {
+    if (c.p >= c.end) break;
+    const uint8_t b = rd8(c, c.p++);
+    t |= (uint64_t)(b & 0x7F) << (7 * i);
+    if (!(b & 0x80)) {
+      if (t > 0xFFFFFFFFull || (t >> 3) == 0) break;
+      return (uint32_t)t;
+    }
+  }
+  c.err = B200TFS_E_PARSE;   // truncated, a sixth byte, past 32 bits, or field 0
+  return 0;
 }
 
 // length prefix: bounded by the enclosing message (and by int32, like the runtime)

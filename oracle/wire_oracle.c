@@ -298,9 +298,10 @@ static void skip_value(rd* r, uint64_t tag);
 static void skip_group(rd* r, uint64_t field) {
   for (;;) {
     if (r->p >= r->end) { r->bad = 1; return; }
+    const uint8_t* at = r->p;
     uint64_t t = get_uvar(r);
     if (r->bad) return;
-    if (t > 0xFFFFFFFFu || !(t >> 3)) { r->bad = 1; return; }
+    if (r->p - at > 5 || t > 0xFFFFFFFFu || !(t >> 3)) { r->bad = 1; return; }
     if ((t & 7) == 4) { if ((t >> 3) != field) r->bad = 1; return; }
     skip_value(r, t);
     if (r->bad) return;
@@ -316,9 +317,10 @@ static void skip_value(rd* r, uint64_t tag) {
     default: r->bad = 1;
   }
 }
-static uint64_t get_tag(rd* r) {
+static uint64_t get_tag(rd* r) { /* at most 5 bytes, fits 32 bits, field number != 0 */
+  const uint8_t* at = r->p;
   uint64_t t = get_uvar(r);
-  if (!r->bad && (t > 0xFFFFFFFFu || !(t >> 3))) r->bad = 1;
+  if (!r->bad && (r->p - at > 5 || t > 0xFFFFFFFFu || !(t >> 3))) r->bad = 1;
   return t;
 }
 static int utf8_valid(const uint8_t* s, size_t n) {

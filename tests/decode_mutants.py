@@ -393,13 +393,24 @@ def _rv(b, p):
 
 def length_prefixes(wire: bytes, kind: str):
     """(offset, byte count, value) of every length prefix in a valid record."""
-    found = []
+    return _framing(wire, kind)[0]
+
+
+def tags(wire: bytes, kind: str):
+    """(offset, byte count, value) of every tag in a valid record."""
+    return _framing(wire, kind)[1]
+
+
+def _framing(wire: bytes, kind: str):
+    found, found_tags = [], []
 
     def scan(lo, hi, msg):
         p = lo
         depth = 0
         while p < hi:
+            q = p
             tag, p = _rv(wire, p)
+            found_tags.append((q, p - q, tag))
             wt = tag & 7
             if wt == 0:
                 _, p = _rv(wire, p)
@@ -420,7 +431,7 @@ def length_prefixes(wire: bytes, kind: str):
                 p += n
 
     scan(0, len(wire), kind)
-    return found
+    return found, found_tags
 
 
 # ---- mutants ------------------------------------------------------------------------------------------------------------
@@ -491,6 +502,18 @@ def mutants(s: Seed) -> List[Mutant]:
         long = bytearray(vi(v))
         long[-1] |= 0x80
         add("length_nonminimal", w[:at] + bytes(long) + b"\x00" + w[at + nb:])
+    # tags re-spelt in 5 to 10 bytes (the runtime refuses a tag of more than 5 bytes): the first at every length, a seeded
+    # sample of the others at one length each
+    ts = tags(w, "tensor" if s.tensor else "resp")
+    picks = [(0, k) for k in range(5, 11)]
+    rest = range(1, len(ts)) if len(ts) <= 48 else sorted({len(ts) - 1} | set(int(j) for j in rng.integers(1, len(ts), 46)))
+    picks += [(j, 5 + j % 6) for j in rest]
+    for j, k in picks:
+        at, nb, v = ts[j]
+        if k > nb:
+            long = bytearray(vi(v))
+            long[-1] |= 0x80
+            add("tag_long", w[:at] + bytes(long) + b"\x80" * (k - nb - 1) + b"\x00" + w[at + nb:])
     # the terminator of each packed-varint run
     for o, runs in zip(base.outs, base.runs):
         if not o.flags & N.OF_VARINT:

@@ -151,6 +151,49 @@ def edge_cases():
         ("length_past_end", REGRESS, b"\x0a\x05\x0a\x00"),
         ("truncated_value", REGRESS, b"\x0a\x04\x0a\x02\x0d\x00"),
     ]
+    return cases + long_tag_cases()
+
+
+def long_tag(field: int, wt: int, n: int) -> bytes:
+    """the tag of (field, wt) written in n bytes (n at least its minimal length)"""
+    t = varint(field << 3 | wt)
+    return varint(field << 3 | wt, n - len(t)) if n > len(t) else t
+
+
+def tag_5th_byte(field: int, wt: int, top: int) -> bytes:
+    """a 5-byte tag of (field, wt) whose last byte is `top`: bits 28 and up of the value (0x0F: it still fits 32 bits, 0x10: it
+    does not)"""
+    v = field << 3 | wt
+    return bytes([(v & 0x7F) | 0x80, (v >> 7 & 0x7F) | 0x80, (v >> 14 & 0x7F) | 0x80, (v >> 21 & 0x7F) | 0x80, top])
+
+
+def long_tag_cases():
+    """(name, kind, wire): tags written in 2 to 10 bytes at every level the decode reads one.  The runtime accepts a tag of at
+    most 5 bytes whose value fits 32 bits, and refuses every longer one, whatever its value."""
+    v = f32(1.5)
+    cases = []
+    for n in range(2, 11):
+        e = long_tag(1, LEN, n)
+        cases += [
+            (f"result_tag_{n}_bytes", REGRESS, e + b"\x07" + b"\x0a\x05\x0d" + v),
+            (f"entry_tag_{n}_bytes", REGRESS, serialize([(1, LEN, [(None, RAW, e + b"\x05\x0d" + v), (1, LEN, [(1, I32, v)])])])),
+            (f"value_tag_{n}_bytes", REGRESS, serialize([(1, LEN, [(1, LEN, [(None, RAW, long_tag(1, I32, n) + v)])])])),
+            (f"unknown_tag_{n}_bytes", REGRESS, long_tag(15, VARINT, n) + b"\x01" + serialize(regression_nodes([2.0]))),
+            (f"unknown_body_tag_{n}_bytes", REGRESS, serialize([(1, LEN, [(None, RAW, long_tag(15, I64, n) + b"\1" * 8), (1, LEN, [])])])),
+            (f"group_member_tag_{n}_bytes", REGRESS, serialize([(1, LEN, [(9, SGROUP, b""), (None, RAW, long_tag(1, VARINT, n) + b"\x01"),
+                                                                          (9, EGROUP, b""), (1, LEN, [])])])),
+            (f"class_tag_{n}_bytes", CLASSIFY, serialize([(1, LEN, [(1, LEN, [(None, RAW, e + b"\x03\x0a\x01a"),
+                                                                              (1, LEN, [(1, LEN, b"b")])])])])),
+            (f"label_tag_{n}_bytes", CLASSIFY, serialize([(1, LEN, [(1, LEN, [(1, LEN, [(None, RAW, e + b"\x01a")])])])])),
+        ]
+    for top in (0x0F, 0x10):
+        t = tag_5th_byte(1, LEN, top)            # field (1 | 0x0F << 25) or a value past 32 bits: never an entry
+        cases += [
+            (f"unknown_tag_5th_byte_{top:02x}", REGRESS, t + b"\x00" + serialize(regression_nodes([3.0]))),
+            (f"unknown_body_tag_5th_byte_{top:02x}", REGRESS, serialize([(1, LEN, [(None, RAW, t + b"\x01z"), (1, LEN, [(1, I32, v)])])])),
+            (f"unknown_class_tag_5th_byte_{top:02x}", CLASSIFY, serialize([(1, LEN, [(1, LEN, [(1, LEN, [(None, RAW, t + b"\x00"),
+                                                                                                         (1, LEN, b"a")])])])])),
+        ]
     return cases
 
 

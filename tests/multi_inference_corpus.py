@@ -80,7 +80,31 @@ def edge_cases():
         ("tag_zero", [R], b"\x00\x00"),
         ("length_past_end", [R], b"\x0a\x05\x1a\x00"),
         ("open_group", [R], serialize([result(REG, reg_body([1.0]))]) + bytes([9 << 3 | 3])),
-    ]
+    ] + long_tag_cases()
+
+
+def long_tag_cases():
+    """(name, kinds, wire): tags written in 2 to 10 bytes at every level the decode reads one (the runtime refuses one of more
+    than 5 bytes), and 5-byte tags whose value fits 32 bits or does not."""
+    C, R = CLASSIFY, REGRESS
+    lt = X.long_tag
+    cases = []
+    for n in range(2, 11):
+        cases += [
+            (f"results_tag_{n}_bytes", [R], lt(1, LEN, n) + serialize([result(REG, reg_body([1.0]))])[1:]),   # its 1-byte tag re-spelt
+            (f"member_tag_{n}_bytes", [R], serialize([(1, LEN, spec() + [(None, RAW, lt(REG, LEN, n) + b"\x07\x0a\x05\x0d" + f32(2.0))])])),
+            (f"entry_tag_{n}_bytes", [C], serialize([result(CLS, [(None, RAW, lt(1, LEN, n) + b"\x03\x0a\x01a")] + cls_body([[(b"b", 1.0)]]))])),
+            (f"spec_tag_{n}_bytes", [R], serialize([(1, LEN, [(None, RAW, lt(1, LEN, n) + b"\x03\x0a\x01m"), (REG, LEN, reg_body([1.0]))])])),
+            (f"unknown_tag_{n}_bytes", [R, C], serialize([result(REG, reg_body([1.0]) + [(None, RAW, lt(20, VARINT, n) + b"\x01")]),
+                                                          result(CLS, cls_body(EX2))])),
+        ]
+    for top in (0x0F, 0x10):
+        t = X.tag_5th_byte(1, LEN, top)
+        cases += [
+            (f"unknown_tag_5th_byte_{top:02x}", [R], t + b"\x00" + serialize([result(REG, reg_body([1.0]))])),
+            (f"member_body_tag_5th_byte_{top:02x}", [C], serialize([result(CLS, [(None, RAW, t + b"\x01z")] + cls_body(EX2))])),
+        ]
+    return cases
 
 
 def _bases():
