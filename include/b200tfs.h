@@ -1086,6 +1086,64 @@ int b200tfs_encode_example_specs_host(b200tfs_ctx* ctx, int32_t n, const b200tfs
                                       const b200tfs_request_spec* specs, void* wire_host, uint64_t wire_cap, uint64_t* rec_off,
                                       uint64_t* rec_len);
 
+/* A batch of ExampleListWithContexts, one per query (TF-Ranking's ELWC serving input fed many queries in one Predict call).  One
+ * entry per request, parallel to reqs (lists == NULL: no request has one).  present == 1 with target kind
+ * B200TFS_EXAMPLES_PREDICT_ELWCS: the request is
+ *     PredictRequest{model_spec, inputs[key] = TensorProto{dtype: DT_STRING, tensor_shape {dim {size: Q}}, string_val:
+ *                    [elwc.SerializeToString(deterministic=True) for the Q ExampleListWithContexts]}}
+ * serialised with SerializeToString(deterministic=True), each string being
+ *     42 vi(elwc) {0A vi(ex) ex}* 12 vi(ctx) ctx
+ * Query q's examples are the list_sizes[q] consecutive examples (rows) of the request from sum(list_sizes[0..q)) on, written as
+ * the examples of every other target are; its context is row q of the context features (B200TFS_F_BROADCAST: one row, repeated),
+ * listed in `order`, with b200tfs_ragged and b200tfs_bytes entries (list_ragged / list_bytes: one per context feature of every
+ * present entry, in request-then-feature order; NULL: none) under the rules of the examples' with n_examples = Q.  A context of
+ * no features is an empty Example (12 00).  With Q == 1 the bytes are those of PREDICT_ELWC with that context.  list_sizes are
+ * host values that shape the request as n_examples does: a captured graph replays new values, lengths and offsets, and the same
+ * list sizes.  Refused before the context is looked at (B200TFS_E_ARG): present not 0 or 1; present == 1 on another kind,
+ * PREDICT_ELWCS without it; a present b200tfs_example_context, tasks or a sequence beside it; a negative n_lists or
+ * n_context, NULL list_sizes or context with a count > 0, a negative list size, sum(list_sizes) != n_examples; malformed ragged
+ * or bytes entries.  A request that cannot stay under 2 GiB: B200TFS_E_TOOBIG.  Device lengths or offsets out of range give that
+ * request B200TFS_E_SHAPE in b200tfs_encode_results, and no write leaves its slot.  A call with such a request runs its frame
+ * kernel before the emits (it computes where every query's examples and context go, and writes the query headers), then two
+ * more emit kernels over the queries' examples and the contexts; calls without one launch what they did.                     */
+#define B200TFS_EXAMPLES_PREDICT_ELWCS 4
+typedef struct b200tfs_example_lists {
+  const int64_t* list_sizes;         /* host int64[n_lists]: the examples of every query, each >= 0                              */
+  int64_t n_lists;                   /* Q >= 0                                                                                   */
+  const b200tfs_feature* context;    /* host array of n_context; data: Q rows of row_elems (one with B200TFS_F_BROADCAST)       */
+  int32_t n_context;
+  int32_t present;                   /* 0: not a PREDICT_ELWCS request; 1: one                                                   */
+} b200tfs_example_lists;
+/* The _specs_ entry points with lists (lists == NULL: those calls themselves, which call these).  The request size is exact, in
+ * closed form, when no integer or bytes column and no ragged entry with lengths appears in the examples or the contexts
+ * (B200TFS_E_ARG otherwise).  A request's slot holds its examples' worst case plus, per query, its context's worst case and 6
+ * bytes of header.                                                                                                               */
+int b200tfs_example_lists_request_size(const b200tfs_example_request* r, const b200tfs_example_target* target,
+                                       const b200tfs_example_context* context, const b200tfs_example_tasks* tasks,
+                                       const b200tfs_ragged* ragged, const b200tfs_example_sequence* sequence,
+                                       const b200tfs_request_spec* spec, const b200tfs_example_lists* lists,
+                                       const b200tfs_ragged* list_ragged, uint64_t* total_len);
+int b200tfs_example_lists_arena_size(int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                     const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                     const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                     const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
+                                     const b200tfs_request_spec* specs, const b200tfs_example_lists* lists,
+                                     const b200tfs_ragged* list_ragged, const b200tfs_bytes* list_bytes, uint64_t* bytes_out);
+int b200tfs_encode_example_lists_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                       const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                       const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                       const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
+                                       const b200tfs_request_spec* specs, const b200tfs_example_lists* lists,
+                                       const b200tfs_ragged* list_ragged, const b200tfs_bytes* list_bytes, void* arena_dev,
+                                       uint64_t arena_cap);
+int b200tfs_encode_example_lists_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                      const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                      const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                      const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
+                                      const b200tfs_request_spec* specs, const b200tfs_example_lists* lists,
+                                      const b200tfs_ragged* list_ragged, const b200tfs_bytes* list_bytes, void* wire_host,
+                                      uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
+
 /* ---- Classify / Regress responses: a batch of responses into one value or score array ----------------------
  * What ClassificationResponse.FromString / RegressionResponse.FromString followed by a loop over the result give, concatenated
  * along the example axis across the n responses: row order is response 0's examples, then response 1's, and so on.

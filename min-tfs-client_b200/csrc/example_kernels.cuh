@@ -548,18 +548,19 @@ __device__ __forceinline__ void ex_write_record(const ExTables& T, const ExReq& 
   else ex_write_example<kMode, kTag>(T, q, i, w);
 }
 
-template <int kMode, uint8_t kTag, bool kSeq = false>
-__device__ __forceinline__ void ex_emit(const ExTables& T) {
+// kShift (a PREDICT_ELWCS span, plan.h ExLists): the span's query (its pad) moves its examples by shift[query]
+template <int kMode, uint8_t kTag, bool kSeq = false, bool kShift = false>
+__device__ __forceinline__ void ex_emit(const ExTables& T, const uint64_t* shift = nullptr) {
   __shared__ __align__(16) uint8_t img[kExStage + 16];
   __shared__ uint64_t next;
   constexpr uint32_t kWarps = kExEmitThreads / 32;
   const ExSpan sp = T.spans[blockIdx.x];
   const ExReq q = T.reqs[sp.req];
   const uint32_t warp = threadIdx.x >> 5;
-  const uint64_t A = q.anchor;
+  const uint64_t A = q.anchor + (kShift ? shift[sp.pad] : 0);
   // a bytes request whose offsets broke the rule can count more bytes than its slot holds (it gets B200TFS_E_SHAPE): a span
   // that would end past the slot writes nothing
-  if (kMode == kExColumns && A + ex_end<kMode>(T, q, sp.e1 - 1) > q.slot_end) return;
+  if ((kShift || kMode == kExColumns) && A + ex_end<kMode>(T, q, sp.e1 - 1) > q.slot_end) return;
   uint64_t lo = A + ex_start<kMode>(T, q, sp.e0);   // first byte not stored yet
   uint64_t ws = lo & ~15ull;                 // arena offset of img[0]
   uint64_t i = sp.e0;
@@ -606,6 +607,11 @@ __global__ void __launch_bounds__(kExEmitThreads) ex_emit_kernel(const __grid_co
 template <int kMode>
 __global__ void __launch_bounds__(kExEmitThreads) ex_emit_predict_kernel(const __grid_constant__ ExTables T) {
   ex_emit<kMode, 0x42>(T);
+}
+// the spans of the PREDICT_ELWCS requests: their examples (kTag 0A, ExampleListWithContext.examples) and their contexts (12)
+template <int kMode, uint8_t kTag>
+__global__ void __launch_bounds__(kExEmitThreads) ex_emit_list_kernel(const __grid_constant__ ExTables T, const uint64_t* __restrict__ shift) {
+  ex_emit<kMode, kTag, false, true>(T, shift);
 }
 // the spans of the SequenceExample requests, which are always counted (kExColumns places them through off and S)
 __global__ void __launch_bounds__(kExEmitThreads) ex_emit_sequence_kernel(const __grid_constant__ ExTables T) {
@@ -675,12 +681,9 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_kernel(const __gr
 // ex_frame_kernel for a call with contexts (plan.h ExCtxRef): a request with one also takes its context's size into its length,
 // the context's bad flag into its status, and writes the context behind its examples, in place, with the request's warp
 template <int kMode>
-__global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_context_kernel(const __grid_constant__ ExTables T,
-                                                                              const ExCtxRef* __restrict__ ctx) {
-  const uint32_t r = blockIdx.x * kExFrameWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (r >= T.n_req) return;
+__device__ __forceinline__ void ex_frame_context(const ExTables& T, uint32_t r, const ExCtxRef c) {
+  const uint32_t lane = threadIdx.x & 31;
   const ExReq q = T.reqs[r];
-  const ExCtxRef c = ctx[r];
   const uint64_t el = ex_examples_len(T, q);
   if (c.req == kExNoContext) {
     ex_frame_request(T, q, r, el, 0, false, T.bad && T.bad[r]);
@@ -693,10 +696,69 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_context_kernel(co
   if (x.n_feat) ex_write_example<kMode, 0x12>(T, x, 0, w);
   else if (lane == 0) { w[0] = 0x12; w[1] = 0; }                 // context.SetInParent(): no features map at all
 }
+template <int kMode>
+__global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_context_kernel(const __grid_constant__ ExTables T,
+                                                                              const ExCtxRef* __restrict__ ctx) {
+  const uint32_t r = blockIdx.x * kExFrameWarps + (threadIdx.x >> 5);
+  if (r >= T.n_req) return;
+  ex_frame_context<kMode>(T, r, ctx[r]);
+}
+
+// ex_frame_context_kernel for a call with a PREDICT_ELWCS request (plan.h ExLists), launched after the scan and before the emits:
+// the warp of such a request walks its queries 32 at a time, one per lane.  Query q's examples take E_q bytes from their first
+// contiguous offset, its context C_q (12 00 when empty); a warp scan of 1 + vi(E + C) + E + C gives where its header goes, which
+// the lane writes, and the shifts the list emits move its examples and its context by.  No header leaves the slot, whatever the
+// sizes: a request whose lengths or offsets broke the rules gets B200TFS_E_SHAPE, and its emits stop at the slot's end.
+template <int kMode>
+__global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_lists_kernel(const __grid_constant__ ExTables T,
+                                                                            const ExCtxRef* __restrict__ ctx,
+                                                                            const __grid_constant__ ExLists Ls) {
+  const uint32_t r = blockIdx.x * kExFrameWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= T.n_req) return;
+  const ExCtxRef c = ctx[r];
+  if (c.nest != kExListRef) {
+    ex_frame_context<kMode>(T, r, c);
+    return;
+  }
+  const ExList l = Ls.lists[c.req];
+  const ExReq q = T.reqs[r], x = T.reqs[l.ctx];
+  uint64_t base = 0;            // the bytes of the queries in front of this round
+  for (uint32_t k0 = 0; k0 < l.n_q; k0 += 32) {
+    const uint32_t k = k0 + lane;
+    uint64_t E = 0, C = 0, eo = 0, co = 0, h = 0;
+    if (k < l.n_q) {
+      const ExQuery e = Ls.queries[l.q0 + k];
+      if (e.e1 > e.e0) { eo = ex_start<kMode>(T, q, e.e0); E = ex_end<kMode>(T, q, e.e1 - 1) - eo; }
+      if (x.n_feat) { co = ex_start<kMode>(T, x, k); C = ex_end<kMode>(T, x, k) - co; }
+      else C = 2;
+      h = 1 + varint_len(E + C);
+    }
+    const uint64_t sz = h + E + C;
+    uint64_t inc = sz;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint64_t y = __shfl_up_sync(0xFFFFFFFFu, inc, d);
+      if (lane >= (uint32_t)d) inc += y;
+    }
+    const uint64_t P = base + inc - sz;     // the header, from the anchor
+    if (k < l.n_q) {
+      Ls.shift[l.q0 + k] = P + h - eo;
+      Ls.cshift[l.q0 + k] = P + h + E - co;
+      if (q.anchor + P + sz <= q.slot_end) {
+        uint8_t* w = T.arena + q.anchor + P;
+        w[0] = 0x42;
+        put_varint(w + 1, E + C);
+        if (!x.n_feat) { w[h + E] = 0x12; w[h + E + 1] = 0; }
+      }
+    }
+    base += __shfl_sync(0xFFFFFFFFu, inc, 31);
+  }
+  ex_frame_request(T, q, r, base, 0, false, T.bad && (T.bad[r] || T.bad[l.ctx]));
+}
 
 // n_seq_tiles / n_seq_spans: the count tiles and emit spans of the SequenceExample requests, behind T's n_tiles and n_spans
 cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t stream, uint32_t* launched, const ExCtxRef* ctx,
-                                    uint32_t n_seq_tiles, uint32_t n_seq_spans) {
+                                    uint32_t n_seq_tiles, uint32_t n_seq_spans, const ExLists* lists) {
   *launched = 0;
   if (T.n_tiles) {
     if (mode == kExColumns) ex_count_kernel<kExColumns><<<T.n_tiles, kExTile, 0, stream>>>(T);
@@ -713,6 +775,13 @@ cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t st
   }
   if (T.n_tiles + n_seq_tiles) {      // the scan sees every tile: a request's tiles are contiguous, its first_tile global
     ex_scan_kernel<<<T.n_tiles + n_seq_tiles, kExTile, 0, stream>>>(T);
+    *launched += 1;
+  }
+  const uint32_t frame_grid = (T.n_req + kExFrameWarps - 1) / kExFrameWarps;
+  if (lists && T.n_req) {     // the shifts, before every emit (plan.h ExLists)
+    if (mode == kExColumns) ex_frame_lists_kernel<kExColumns><<<frame_grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx, *lists);
+    else if (mode == kExRagged) ex_frame_lists_kernel<kExRagged><<<frame_grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx, *lists);
+    else ex_frame_lists_kernel<kExDense><<<frame_grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx, *lists);
     *launched += 1;
   }
   const uint32_t n_list = T.n_spans - T.n_predict_spans;
@@ -736,8 +805,26 @@ cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t st
     ex_emit_sequence_kernel<<<n_seq_spans, kExEmitThreads, 0, stream>>>(Q);
     *launched += 1;
   }
+  if (lists) {                // the spans of the PREDICT_ELWCS requests behind those: examples, then contexts
+    ExTables Q = T;
+    Q.spans += T.n_spans + n_seq_spans;
+    if (lists->n_spans) {
+      if (mode == kExColumns) ex_emit_list_kernel<kExColumns, 0x0A><<<lists->n_spans, kExEmitThreads, 0, stream>>>(Q, lists->shift);
+      else if (mode == kExRagged) ex_emit_list_kernel<kExRagged, 0x0A><<<lists->n_spans, kExEmitThreads, 0, stream>>>(Q, lists->shift);
+      else ex_emit_list_kernel<kExDense, 0x0A><<<lists->n_spans, kExEmitThreads, 0, stream>>>(Q, lists->shift);
+      *launched += 1;
+    }
+    Q.spans += lists->n_spans;
+    if (lists->n_ctx_spans) {
+      if (mode == kExColumns) ex_emit_list_kernel<kExColumns, 0x12><<<lists->n_ctx_spans, kExEmitThreads, 0, stream>>>(Q, lists->cshift);
+      else if (mode == kExRagged) ex_emit_list_kernel<kExRagged, 0x12><<<lists->n_ctx_spans, kExEmitThreads, 0, stream>>>(Q, lists->cshift);
+      else ex_emit_list_kernel<kExDense, 0x12><<<lists->n_ctx_spans, kExEmitThreads, 0, stream>>>(Q, lists->cshift);
+      *launched += 1;
+    }
+    return cudaGetLastError();
+  }
   if (T.n_req) {
-    const uint32_t grid = (T.n_req + kExFrameWarps - 1) / kExFrameWarps;
+    const uint32_t grid = frame_grid;
     if (!ctx) ex_frame_kernel<<<grid, 32 * kExFrameWarps, 0, stream>>>(T);
     else if (mode == kExColumns) ex_frame_context_kernel<kExColumns><<<grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx);
     else if (mode == kExRagged) ex_frame_context_kernel<kExRagged><<<grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx);

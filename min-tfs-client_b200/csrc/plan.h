@@ -436,6 +436,21 @@ struct ExSpan { uint32_t req, pad; uint64_t e0, e1; };   // a CTA's examples [e0
 // with the ELWC nested in a string_val (`nest`) in the Predict form.  One entry per request of the call.
 constexpr uint32_t kExNoContext = 0xFFFFFFFFu;
 struct ExCtxRef { uint32_t req, nest; };   // the context's entry in ExTables::reqs (kExNoContext: none), Predict-ELWC
+// A batch of ExampleListWithContexts (PREDICT_ELWCS, one per query) is a request entry over all its examples, whose emit spans
+// never cross a query, and one context entry of Q "examples" over the context columns, one span each.  Both are scanned
+// contiguously; query q then moves by a shift that opens the gaps for the headers and contexts in front of it:
+//   ... 12 vi(inner) head | {42 vi(E_q + C_q) | query q's examples (E_q bytes) | 12 vi(ctx) context q (C_q bytes)}*
+// ex_frame_lists_kernel computes every shift, writes the headers (and the 12 00 of empty contexts) before the emits run.  The
+// request's ExCtxRef is {its index into ExLists::lists, kExListRef}.
+constexpr uint32_t kExListRef = 2;
+struct ExList { uint32_t req, ctx, q0, n_q; };   // the request entry, its context entry, its queries [q0, q0 + n_q)
+struct ExQuery { uint64_t e0, e1; };              // a query's examples [e0, e1) of its request
+struct ExLists {
+  const ExList* lists; const ExQuery* queries;
+  uint64_t* shift;                      // per query: arena offset from the anchor minus the contiguous offset, of its examples
+  uint64_t* cshift;                     // and of its context
+  uint32_t n_lists, n_spans, n_ctx_spans, pad_;   // emit spans behind all others: the examples', then one per non-empty context
+};
 struct ExTables {
   const ExReq* reqs; const ExFeat* feats; const uint8_t* blob;
   const ExSpan* tiles;                  // count / scan CTAs
@@ -473,6 +488,9 @@ B2_PLAN_HD uint64_t ex_example_len(uint64_t F) {
   const uint64_t x = 1 + varint_len(F) + F;
   return 1 + varint_len(x) + x;
 }
+
+// the most bytes of one query's 42 vi(E + C) header (E + C < 2 GiB)
+constexpr uint64_t kExListHeader = 6;
 
 // ---- SequenceExamples (PREDICT_SEQUENCE requests; ex_seq_count_kernel, ex_emit_sequence_kernel) -------------------------
 // A sequence request is one ExReq whose features [0, n_ctx) are context features (an example's, in wire order) and the rest

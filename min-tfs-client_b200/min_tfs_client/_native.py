@@ -149,7 +149,7 @@ class Bytes(C.Structure):
     _fields_ = [("offsets", C.c_void_p), ("data_len", C.c_int64), ("flags", C.c_uint32), ("pad_", C.c_int32)]
 
 
-EXAMPLES_LIST, EXAMPLES_PREDICT_STRING, EXAMPLES_PREDICT_ELWC, EXAMPLES_PREDICT_SEQUENCE = 0, 1, 2, 3
+EXAMPLES_LIST, EXAMPLES_PREDICT_STRING, EXAMPLES_PREDICT_ELWC, EXAMPLES_PREDICT_SEQUENCE, EXAMPLES_PREDICT_ELWCS = 0, 1, 2, 3, 4
 
 
 class ExampleTarget(C.Structure):
@@ -179,6 +179,13 @@ class ExampleSequence(C.Structure):
     """b200tfs_example_sequence: one request's SequenceExamples (present 0: none; 1: its first ``n_context`` features are
     context features, the rest feature lists whose Ragged entries give their steps), for EXAMPLES_PREDICT_SEQUENCE."""
     _fields_ = [("present", C.c_int32), ("n_context", C.c_int32)]
+
+
+class ExampleLists(C.Structure):
+    """b200tfs_example_lists: one request's queries for EXAMPLES_PREDICT_ELWCS (present 0: none; 1: ``n_lists`` ELWCs whose
+    examples are the next ``list_sizes[q]`` rows, and whose contexts are row q of the ``n_context`` ``context`` features)."""
+    _fields_ = [("list_sizes", C.c_void_p), ("n_lists", C.c_int64), ("context", C.POINTER(Feature)), ("n_context", C.c_int32),
+                ("present", C.c_int32)]
 
 
 class PadInput(C.Structure):
@@ -382,6 +389,22 @@ SIGNATURES = {
                                                     C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
                                                     C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), C.POINTER(RequestSpec), _vp,
                                                     C.c_uint64, _u64p, _u64p]),
+    "b200tfs_example_lists_request_size": (C.c_int, [C.POINTER(ExampleRequest), C.POINTER(ExampleTarget), C.POINTER(ExampleContext),
+                                                     C.POINTER(ExampleTasks), C.POINTER(Ragged), C.POINTER(ExampleSequence),
+                                                     C.POINTER(RequestSpec), C.POINTER(ExampleLists), C.POINTER(Ragged), _u64p]),
+    "b200tfs_example_lists_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                   C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                   C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), C.POINTER(RequestSpec),
+                                                   C.POINTER(ExampleLists), C.POINTER(Ragged), C.POINTER(Bytes), _u64p]),
+    "b200tfs_encode_example_lists_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                     C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                     C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), C.POINTER(RequestSpec),
+                                                     C.POINTER(ExampleLists), C.POINTER(Ragged), C.POINTER(Bytes), _vp, C.c_uint64]),
+    "b200tfs_encode_example_lists_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                    C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                    C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), C.POINTER(RequestSpec),
+                                                    C.POINTER(ExampleLists), C.POINTER(Ragged), C.POINTER(Bytes), _vp, C.c_uint64, _u64p,
+                                                    _u64p]),
     "b200tfs_multi_inference_response_bound": (C.c_int, [C.c_int32, _i32p, C.c_int32, _u64p, _u64p, _u64p]),
     "b200tfs_decode_multi_inference_responses": (C.c_int, [_vp, C.c_int32, _i32p, _vp, C.c_int32, _u64p, _u64p, _vpp, _u64p, _vpp,
                                                            _u64p]),

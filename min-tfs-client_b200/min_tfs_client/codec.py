@@ -1260,6 +1260,82 @@ class Codec:
                 out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
         return out  # type: ignore[return-value]
 
+    def encode_elwc_requests(self, requests: Iterable[Tuple], *, input_key, order="deterministic", grpc_frame: bool = False,
+                             signature_name=None, version_label=None, output_filter=None) -> List[bytes]:
+        """Each item is ``(model_name, model_version, context_dict, input_dict, list_sizes)``; returns one PredictRequest wire per
+        item for a TF-Ranking model whose ELWC signature takes a DT_STRING ``[Q]`` vector of serialized ExampleListWithContexts,
+        one per query - the bytes of ``make_predict_elwcs_request(...).SerializeToString(deterministic=True)``.  ``list_sizes``
+        (host integers, Q of them) cuts the rows of ``input_dict`` into the queries' candidate lists; row q of ``context_dict`` is
+        query q's context.
+
+        Values are taken as ``encode_sequence_example_requests`` takes context values (numpy, pinned or device arrays, 0-d values
+        repeated, ``RaggedColumn`` and ``BytesColumn``), on both sides.  ``order="given"`` lists the features in insertion order.
+        An item with a numpy str / bytes value, or a dtype the device route does not take, is assembled on the host by
+        ``make_predict_elwcs_request`` (deterministic order); device arrays of such dtypes raise ValueError, and so do device
+        lengths or offsets out of range.  ``signature_name``, ``version_label`` and ``output_filter`` as for
+        ``encode_predict_requests``.  With one query the bytes equal ``encode_example_requests(..., predict_input=input_key)``'s
+        for that query's context."""
+        from .requests import _list_sizes, make_predict_elwcs_request
+
+        items = list(requests)
+        fields = {k: v for k, v in dict(signature_name=signature_name, version_label=version_label, output_filter=output_filter).items()
+                  if v is not None}
+        spec = _RequestSpec.of([item[1] for item in items], signature_name, version_label, output_filter)
+        order_code = _ORDER[order] if isinstance(order, str) else int(order)
+        pkey = input_key.encode("utf-8") if isinstance(input_key, str) else bytes(input_key)
+        out: List[Optional[bytes]] = [None] * len(items)
+        keep, structs, dev_idx, ragged, strs, lists, lragged, lstrs = [], [], [], [], [], [], [], []
+        for i, (model_name, model_version, context_dict, input_dict, list_sizes) in enumerate(items):
+            sizes = _list_sizes(list_sizes)
+            n, q = int(sizes.sum()), sizes.size
+            for what, d, m in (("input", input_dict, n), ("context", context_dict, q)):
+                for k, v in d.items():
+                    shape = _shape_of(v)
+                    if len(shape) and shape[0] != m:
+                        raise ValueError(f"{what} {k!r} has {shape[0]} rows, not {m}")
+            cols, ccols = _example_columns(input_dict), _example_columns(context_dict)
+            if cols is None or ccols is None or (n and not input_dict):
+                req = make_predict_elwcs_request(model_name, model_version, context_dict, input_dict, sizes, pkey.decode("utf-8"), **fields)
+                wire = req.SerializeToString(deterministic=True)
+                out[i] = (b"\x00" + len(wire).to_bytes(4, "big") + wire) if grpc_frame else wire
+                continue
+            preps, cpreps = cols[1], ccols[1]
+            feats = (N.Feature * max(len(preps), 1))(*[p[0] for p in preps])
+            cfeats = (N.Feature * max(len(cpreps), 1))(*[p[0] for p in cpreps])
+            name = model_name.encode("utf-8") if isinstance(model_name, str) else bytes(model_name)
+            structs.append(N.ExampleRequest(model_name=name, model_name_len=len(name), has_version=int(model_version is not None),
+                                            order=order_code, version=int(model_version) if model_version is not None else 0,
+                                            n_examples=n, n_features=len(preps), flags=N.RF_GRPC_FRAME if grpc_frame else 0,
+                                            features=feats))
+            lists.append(N.ExampleLists(list_sizes=sizes.ctypes.data if q else None, n_lists=q, context=cfeats, n_context=len(cpreps),
+                                        present=1))
+            keep.append((preps, feats, cpreps, cfeats, name, sizes))
+            ragged += [p[3] or N.Ragged() for p in preps]
+            strs += [p.bytes_entry or N.Bytes() for p in preps]
+            lragged += [p[3] or N.Ragged() for p in cpreps]
+            lstrs += [p.bytes_entry or N.Bytes() for p in cpreps]
+            dev_idx.append(i)
+        if dev_idx:
+            m = len(dev_idx)
+            reqs = (N.ExampleRequest * m)(*structs)
+            tg = (N.ExampleTarget * m)(*[N.ExampleTarget(kind=N.EXAMPLES_PREDICT_ELWCS, key=pkey, key_len=len(pkey))] * m)
+            ls = (N.ExampleLists * m)(*lists)
+            rg = (N.Ragged * len(ragged))(*ragged) if any(g.lengths for g in ragged) else None
+            bs = (N.Bytes * len(strs))(*strs) if any(b.offsets for b in strs) else None
+            lrg = (N.Ragged * len(lragged))(*lragged) if any(g.lengths for g in lragged) else None
+            lbs = (N.Bytes * len(lstrs))(*lstrs) if any(b.offsets for b in lstrs) else None
+            cap = C.c_uint64()
+            specs = _RequestSpec.array(spec, m)
+            N.check(self._lib.b200tfs_example_lists_arena_size(m, reqs, None, bs, tg, None, None, None, None, specs, ls, lrg, lbs,
+                                                               C.byref(cap)))
+            wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
+            off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
+            N.check(self._lib.b200tfs_encode_example_lists_host(self._ctx, m, reqs, rg, bs, tg, None, None, None, None, specs, ls, lrg, lbs,
+                                                                wire.ctypes.data, cap.value, off, ln))
+            for j, i in enumerate(dev_idx):
+                out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
+        return out  # type: ignore[return-value]
+
     # ---- decode --------------------------------------------------------------------------------
     def _pack_wires(self, wires: Sequence[bytes]):
         n = len(wires)

@@ -49,14 +49,18 @@ def examples_from_input_dict(input_dict: Dict[str, np.ndarray]):
     inp = Input()
     inp.example_list.SetInParent()
     for i in range(n):
-        ex = inp.example_list.examples.add()
-        for k, a in arrays.items():
-            feat = ex.features.feature[k]
-            if isinstance(a, BytesColumn) or isinstance(a, RaggedColumn) and isinstance(a.values, BytesColumn):
-                feat.bytes_list.value.extend(a.strings(i))
-                continue
-            _fill_feature(feat, k, a.row(i) if isinstance(a, RaggedColumn) else a if a.ndim == 0 else a[i])
+        _fill_example(inp.example_list.examples.add(), arrays, i)
     return inp
+
+
+def _fill_example(ex, arrays: Dict, i: int) -> None:
+    """Example ``ex`` holds row i of every array (0-d arrays: their one value), as ``examples_from_input_dict`` fills it."""
+    for k, a in arrays.items():
+        feat = ex.features.feature[k]
+        if isinstance(a, BytesColumn) or isinstance(a, RaggedColumn) and isinstance(a.values, BytesColumn):
+            feat.bytes_list.value.extend(a.strings(i))
+            continue
+        _fill_feature(feat, k, a.row(i) if isinstance(a, RaggedColumn) else a if a.ndim == 0 else a[i])
 
 
 def _fill_feature(feat, k, row: np.ndarray) -> None:
@@ -147,6 +151,72 @@ def sequence_examples_from_input_dict(context_dict: Dict[str, np.ndarray], featu
                     _fill_feature(fl.feature.add(), k, step)
         out.append(s)
     return out
+
+
+def _list_sizes(list_sizes) -> np.ndarray:
+    """The host int64 vector of a batch's list sizes (ValueError when it is not a 1-D integer array, or has a negative size)."""
+    sizes = np.asarray(list_sizes)
+    if sizes.ndim != 1 or (sizes.size and sizes.dtype.kind not in "iu"):
+        raise ValueError(f"list_sizes is a 1-D integer array, got {sizes.dtype} of shape {sizes.shape}")
+    sizes = np.ascontiguousarray(sizes, dtype=np.int64)
+    if (sizes < 0).any():
+        raise ValueError("list sizes must be >= 0")
+    return sizes
+
+
+def elwcs_from_input_dict(context_dict, input_dict, list_sizes) -> list:
+    """One ``ExampleListWithContext`` per query (input.proto): what TF-Ranking's ELWC serving signature takes as a DT_STRING
+    ``[None]`` vector, one serialized ELWC per query.  ``list_sizes`` is a 1-D integer array of Q sizes >= 0 (Q may be 0), and n
+    their sum.  Example j (j < n) holds row j of every non-0-d value of ``input_dict``, filled as ``examples_from_input_dict``
+    fills it (0-d values repeated; ``RaggedColumn`` and ``BytesColumn`` values as there); query q's examples are the
+    ``list_sizes[q]`` rows from ``sum(list_sizes[:q])`` on.  Context q holds row q of every non-0-d value of ``context_dict``
+    the same way (0-d values repeated, ``RaggedColumn`` and ``BytesColumn`` values allowed), and is always set: an empty
+    ``context_dict`` gives empty contexts.  ValueError when an input value's leading dim is not n, a context value's is not Q,
+    or a list size is negative."""
+    from tensorflow_serving.apis.input_pb2 import ExampleListWithContext
+
+    sizes = _list_sizes(list_sizes)
+    n = int(sizes.sum())
+
+    def rows(d, m, what):
+        arrays = {k: v if isinstance(v, (RaggedColumn, BytesColumn)) else np.asarray(v) for k, v in d.items()}
+        for k, a in arrays.items():
+            if a.ndim and a.shape[0] != m:
+                raise ValueError(f"{what} {k!r} has {a.shape[0]} rows, not {m}")
+        return arrays
+
+    inputs, ctx = rows(input_dict, n, "input"), rows(context_dict, sizes.size, "context")
+    out, s = [], 0
+    for q, m in enumerate(sizes.tolist()):
+        e = ExampleListWithContext()
+        for j in range(s, s + m):
+            _fill_example(e.examples.add(), inputs, j)
+        e.context.SetInParent()
+        _fill_example(e.context, ctx, q)
+        out.append(e)
+        s += m
+    return out
+
+
+def make_predict_elwcs_request(model_name: str, model_version: Optional[int], context_dict, input_dict, list_sizes, input_key: str, *,
+                               signature_name=None, version_label=None, output_filter=None):
+    """``PredictRequest`` whose one input ``input_key`` is the DT_STRING ``[Q]`` tensor of the ExampleListWithContexts
+    ``elwcs_from_input_dict`` builds, each serialized with ``deterministic=True`` - several TF-Ranking queries in one Predict
+    call, what ``Codec.encode_elwc_requests`` encodes on the GPU.  ``signature_name``, ``version_label`` and ``output_filter``
+    set those fields (``apply_spec_fields``)."""
+    from tensorflow.core.framework.types_pb2 import DT_STRING
+    from tensorflow_serving.apis.predict_pb2 import PredictRequest
+
+    req = PredictRequest()
+    req.model_spec.name = model_name
+    if model_version is not None:
+        req.model_spec.version.value = model_version
+    elwcs = elwcs_from_input_dict(context_dict, input_dict, list_sizes)
+    t = req.inputs[input_key.decode("utf-8") if isinstance(input_key, bytes) else input_key]
+    t.dtype = DT_STRING
+    t.tensor_shape.dim.add().size = len(elwcs)
+    t.string_val.extend(e.SerializeToString(deterministic=True) for e in elwcs)
+    return apply_spec_fields(req, model_version, signature_name, version_label, output_filter)
 
 
 class SpecFields(dict):
@@ -411,6 +481,17 @@ def gpu_predict_sequence_examples_serializer(request) -> bytes:
                                                         input_key=input_key, **spec)[0]
 
 
+def gpu_predict_elwcs_serializer(request) -> bytes:
+    """``request_serializer`` for ``channel.unary_unary(PREDICT_METHOD, ...)`` to a TF-Ranking model's ELWC signature:
+    (model_name, model_version, context_dict, input_dict, list_sizes, input_key) -> the bytes of
+    ``make_predict_elwcs_request(...).SerializeToString(deterministic=True)``, packed on the GPU.  A trailing ``SpecFields`` sets
+    ``signature_name`` / ``version_label`` / ``output_filter``."""
+    request, spec = _split_fields(request)
+    model_name, model_version, context_dict, input_dict, list_sizes, input_key = request
+    return get_codec().encode_elwc_requests([(model_name, model_version, context_dict, input_dict, list_sizes)], input_key=input_key,
+                                            **spec)[0]
+
+
 def gpu_response_deserializer(wire: bytes) -> PredictResponseView:
     """``response_deserializer`` for ``channel.unary_unary``: bytes -> lazy response view."""
     return PredictResponseView(wire)
@@ -467,6 +548,17 @@ class TensorServingClient:
         call = self._channel.unary_unary(PREDICT_METHOD, request_serializer=gpu_predict_sequence_examples_serializer,
                                          response_deserializer=gpu_response_deserializer)
         return call((model_name, model_version, context_dict, feature_list_dict, input_key,
+                     _fields(signature_name, version_label, output_filter)), timeout)
+
+    def predict_elwcs_request(self, model_name: str, context_dict, input_dict, list_sizes, input_key: str, timeout: int = 60,
+                              model_version: Optional[int] = None, *, signature_name=None, version_label=None,
+                              output_filter=None) -> PredictResponseView:
+        """Predict on a TF-Ranking model whose signature takes a DT_STRING vector of serialized ExampleListWithContexts, one per
+        query: the Q = ``len(list_sizes)`` ELWCs ``elwcs_from_input_dict(context_dict, input_dict, list_sizes)`` builds, sent as
+        input ``input_key`` in one call and packed on the GPU."""
+        call = self._channel.unary_unary(PREDICT_METHOD, request_serializer=gpu_predict_elwcs_serializer,
+                                         response_deserializer=gpu_response_deserializer)
+        return call((model_name, model_version, context_dict, input_dict, list_sizes, input_key,
                      _fields(signature_name, version_label, output_filter)), timeout)
 
     def _make_example_request(self, request_pb, model_name, input_dict, model_version, context_dict=None, signature_name=None,

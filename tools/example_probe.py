@@ -24,6 +24,12 @@ Workloads (one request each unless stated):
       lists {doc_f0..doc_f7 f32, doc_title: one string of 5-30 B per step}
   Q3  256 requests x 16 sequences of 200 steps x 8 float lists of 2 values: about 21 KB each, above the 16 KB emit image
       (not in the default set; --workloads Q1,Q2,Q3; protobuf is timed once, _host over three calls)
+  K3  64 requests x 16 queries x 100 candidates shaped like K1 (TF-Ranking's ELWC serving input, one ELWC per query): context
+      {user f32[256], hist int64[50], query string} per query (b200tfs_encode_example_lists_*, PREDICT_ELWCS)
+  K3R K3 with a ragged context `query_tokens` int64 [Q, 16], lengths 1..16
+  K4  one request of 1 024 queries x 8 candidates: per-query headers and contexts dominate
+      (not in the default set; --workloads K3,K3R,K4; beside each, the same queries as single-query PREDICT_ELWC requests through
+      Codec.encode_example_requests, what a client sends today; protobuf is timed once, the Python legs over three calls)
 Legs: the _async entry point eager (device columns -> device arena), the same captured once as a CUDA graph and replayed,
 _host from pinned columns (copies both ways included), and examples_from_input_dict + SerializeToString(deterministic=True)
 on one host core.  CUDA events over >= 20 calls after warm-up, three runs each; bytes = column bytes read + wire bytes
@@ -365,6 +371,110 @@ def sequence_workload(name, pairs, args, codec, out):
     print(name, res, flush=True)
 
 
+def elwcs_workloads(rng):
+    """the PREDICT_ELWCS workloads: (context_dict, input_dict, list_sizes) per request, host arrays"""
+    def k3(Q, m, ragged=False):
+        n = Q * m
+        inp = {"item": rng.standard_normal((n, 32)).astype(np.float32), "item_id": rng.integers(0, 1 << 40, n)}
+        q = rng.integers(97, 123, Q * 35).astype(np.uint8)
+        ctx = {"user": rng.standard_normal((Q, 256)).astype(np.float32), "hist": rng.integers(0, 50_000, (Q, 50)),
+               "query": BytesColumn(q, np.arange(Q + 1) * 35)}
+        if ragged:
+            ctx["query_tokens"] = RaggedColumn(rng.integers(0, 30_000, (Q, 16)), rng.integers(1, 17, Q))
+        return ctx, inp, np.full(Q, m, np.int64)
+
+    return {"K3": lambda: [k3(16, 100) for _ in range(64)], "K3R": lambda: [k3(16, 100, True) for _ in range(64)],
+            "K4": lambda: [k3(1024, 8)]}
+
+
+def elwcs_workload(name, items, args, codec, out):
+    """_async eager, graph replay, _host and protobuf on one core for one PREDICT_ELWCS workload, and the same queries as
+    single-query requests through the Python route; bytes compared afterwards"""
+    import torch
+
+    from min_tfs_client.requests import make_predict_elwcs_request
+
+    def dev(v):
+        if isinstance(v, RaggedColumn):
+            return RaggedColumn(dev(v.values), torch.from_numpy(np.asarray(v.lengths, np.int64)).cuda())
+        if isinstance(v, BytesColumn):
+            return BytesColumn(torch.from_numpy(v.data).cuda(), torch.from_numpy(v.offsets).cuda(), v.shape)
+        return torch.from_numpy(np.ascontiguousarray(v)).cuda()
+
+    lib = N.load()
+    g = Ctx()
+    keep, structs, ragged, strs, lists, lragged, lstrs = [], [], [], [], [], [], []
+    for ctx, inp, sizes in items:
+        dctx, dinp = {k: dev(v) for k, v in ctx.items()}, {k: dev(v) for k, v in inp.items()}
+        _, preps = _example_columns(dinp)
+        _, cpreps = _example_columns(dctx)
+        feats = (N.Feature * len(preps))(*[p[0] for p in preps])
+        cfeats = (N.Feature * len(cpreps))(*[p[0] for p in cpreps])
+        keep += [dctx, dinp, preps, cpreps, feats, cfeats, sizes]
+        structs.append(N.ExampleRequest(model_name=b"model", model_name_len=5, has_version=1, order=N.ORDER_UPB, version=1,
+                                        n_examples=int(sizes.sum()), n_features=len(preps), flags=0, features=feats))
+        lists.append(N.ExampleLists(list_sizes=sizes.ctypes.data, n_lists=len(sizes), context=cfeats, n_context=len(cpreps), present=1))
+        ragged += [p[3] or N.Ragged() for p in preps]
+        strs += [p.bytes_entry or N.Bytes() for p in preps]
+        lragged += [p[3] or N.Ragged() for p in cpreps]
+        lstrs += [p.bytes_entry or N.Bytes() for p in cpreps]
+    m = len(structs)
+    reqs, lsa = (N.ExampleRequest * m)(*structs), (N.ExampleLists * m)(*lists)
+    rga, bsa = (N.Ragged * len(ragged))(*ragged), (N.Bytes * len(strs))(*strs)
+    lrga, lbsa = (N.Ragged * len(lragged))(*lragged), (N.Bytes * len(lstrs))(*lstrs)
+    tga = (N.ExampleTarget * m)(*[N.ExampleTarget(kind=N.EXAMPLES_PREDICT_ELWCS, key=b"elwcs", key_len=5)] * m)
+    cap = C.c_uint64()
+    N.check(lib.b200tfs_example_lists_arena_size(m, reqs, rga, bsa, tga, None, None, None, None, None, lsa, lrga, lbsa, C.byref(cap)))
+    arena = (g.malloc(cap.value + 256) + 255) & ~255
+
+    def eager():
+        N.check(lib.b200tfs_encode_example_lists_async(g.ctx, m, reqs, rga, bsa, tga, None, None, None, None, None, lsa, lrga, lbsa,
+                                                       arena, cap.value))
+
+    eager()
+    N.check(lib.b200tfs_encode_results(g.ctx, m, None, None))
+    N.check(lib.b200tfs_capture_begin(g.ctx))
+    eager()
+    gr = C.c_void_p()
+    N.check(lib.b200tfs_capture_end(g.ctx, C.byref(gr)))
+    res = {"requests": m, "queries": sum(len(s) for _, _, s in items), "examples": sum(int(s.sum()) for _, _, s in items),
+           "arena_bytes": cap.value}
+    for _ in range(3):
+        eager()
+    res["async_us"] = min(g.timed(eager, args.calls) for _ in range(args.runs))
+    res["graph_us"] = min(g.timed(lambda: N.check(lib.b200tfs_graph_launch(g.ctx, gr)), args.calls) for _ in range(args.runs))
+    calls = [("model", 1, c, i, s) for c, i, s in items]
+    res["host_us"] = min(timed_host(lambda: codec.encode_elwc_requests(calls, input_key="elwcs"), 3) for _ in range(args.runs))
+    t0 = time.perf_counter()
+    refs = [make_predict_elwcs_request("model", 1, c, i, s, "elwcs").SerializeToString(deterministic=True) for c, i, s in items]
+    res["protobuf_one_core_us"] = (time.perf_counter() - t0) * 1e6
+    res["wire_bytes"] = sum(len(w) for w in refs)
+    # the same queries as single-query Predict-ELWC requests (a ragged context has no such form)
+    if not any(isinstance(v, RaggedColumn) for c, _, _ in items for v in c.values()):
+        single = []
+        for c, inp, sizes in items:
+            s0 = np.concatenate([[0], np.cumsum(sizes)])
+            for q in range(len(sizes)):
+                cq = {k: BytesColumn(v.data, v.offsets[q: q + 2] - 0, (1,)) if isinstance(v, BytesColumn) else v[q] for k, v in c.items()}
+                single.append(("model", 1, {k: v[s0[q]: s0[q + 1]] for k, v in inp.items()}, cq))
+        res["single_query_requests"] = len(single)
+        res["single_query_host_us"] = min(timed_host(lambda: codec.encode_example_requests(single, predict_input="elwcs"), 3)
+                                          for _ in range(args.runs))
+    # after the timed region: the replayed graph's and the host route's bytes against protobuf
+    off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
+    N.check(lib.b200tfs_graph_launch(g.ctx, gr))
+    N.check(lib.b200tfs_encode_results(g.ctx, m, off, ln))
+    host = np.empty(cap.value, np.uint8)
+    N.check(lib.b200tfs_memcpy_d2h(g.ctx, host.ctypes.data, arena, cap.value))
+    assert all(host[off[r]: off[r] + ln[r]].tobytes() == refs[r] for r in range(m)), name
+    assert codec.encode_elwc_requests(calls, input_key="elwcs") == refs, name
+    N.check(lib.b200tfs_graph_destroy(gr))
+    if name in args.profile.split(","):
+        res["kernels"] = profile_split(lib, g, eager, args.calls)
+    out["workloads"][name] = res
+    print(name, res, flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=20)
@@ -382,9 +492,13 @@ def main():
     out = {"card": card, "calls": args.calls, "runs": args.runs, "workloads": {}}
     profile_only = [w for w in args.profile.split(",") if w]
     Q = sequence_workloads(rng)
+    K = elwcs_workloads(rng)
     for name in (profile_only or args.workloads.split(",")):
         if name in Q:
             sequence_workload(name, Q[name](), args, codec, out)
+            continue
+        if name in K:
+            elwcs_workload(name, K[name](), args, codec, out)
             continue
         pairs = [x if isinstance(x, tuple) else (x, None) for x in W[name]()]
         host_dicts = [d for d, _ in pairs]
