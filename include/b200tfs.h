@@ -1099,7 +1099,7 @@ int b200tfs_encode_example_specs_host(b200tfs_ctx* ctx, int32_t n, const b200tfs
  * present entry, in request-then-feature order; NULL: none) under the rules of the examples' with n_examples = Q.  A context of
  * no features is an empty Example (12 00).  With Q == 1 the bytes are those of PREDICT_ELWC with that context.  list_sizes are
  * host values that shape the request as n_examples does: a captured graph replays new values, lengths and offsets, and the same
- * list sizes.  Refused before the context is looked at (B200TFS_E_ARG): present not 0 or 1; present == 1 on another kind,
+ * list sizes (b200tfs_example_device_lists: sizes in device memory, which replays follow).  Refused before the context is looked at (B200TFS_E_ARG): present not 0 or 1; present == 1 on another kind,
  * PREDICT_ELWCS without it; a present b200tfs_example_context, tasks or a sequence beside it; a negative n_lists or
  * n_context, NULL list_sizes or context with a count > 0, a negative list size, sum(list_sizes) != n_examples; malformed ragged
  * or bytes entries.  A request that cannot stay under 2 GiB: B200TFS_E_TOOBIG.  Device lengths or offsets out of range give that
@@ -1108,7 +1108,7 @@ int b200tfs_encode_example_specs_host(b200tfs_ctx* ctx, int32_t n, const b200tfs
  * more emit kernels over the queries' examples and the contexts; calls without one launch what they did.                     */
 #define B200TFS_EXAMPLES_PREDICT_ELWCS 4
 typedef struct b200tfs_example_lists {
-  const int64_t* list_sizes;         /* host int64[n_lists]: the examples of every query, each >= 0                              */
+  const int64_t* list_sizes;         /* host int64[n_lists]: the examples of every query, each >= 0 (NULL: device sizes)         */
   int64_t n_lists;                   /* Q >= 0                                                                                   */
   const b200tfs_feature* context;    /* host array of n_context; data: Q rows of row_elems (one with B200TFS_F_BROADCAST)       */
   int32_t n_context;
@@ -1143,6 +1143,54 @@ int b200tfs_encode_example_lists_host(b200tfs_ctx* ctx, int32_t n, const b200tfs
                                       const b200tfs_request_spec* specs, const b200tfs_example_lists* lists,
                                       const b200tfs_ragged* list_ragged, const b200tfs_bytes* list_bytes, void* wire_host,
                                       uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
+
+/* PREDICT_ELWCS list sizes in device memory, so that a captured graph follows new candidate counts: one entry per request,
+ * parallel to reqs (device_lists == NULL: every request's sizes are host values, the _lists_ calls themselves, which call these).
+ * sizes != NULL on a PREDICT_ELWCS request whose lists entry has list_sizes == NULL: the n_lists sizes are a device int64[n_lists]
+ * (8-byte aligned) that the host never reads.  n_examples is then the capacity N of the example columns, not the sum: query q
+ * takes the sizes[q] rows from sum(sizes[0..q)) on, as with host sizes, and the rows from sum(sizes) on are not sent, so the sizes
+ * and their total may change between replays as long as sum(sizes) <= N.  Those rows are still counted as every row is: their
+ * ragged lengths and string offsets must keep the rules (unused rows of length 0, or offsets equal to the last used offset, do).
+ * The bytes are those of the host-sized request over rows [0, sum(sizes)).  A negative size, or sizes adding up to more than N,
+ * give that request B200TFS_E_SHAPE in b200tfs_encode_results, and no write leaves its slot; the call's other requests are
+ * unaffected.  The slot does not depend on the sizes (N examples' worst case plus Q contexts' and headers'), so the arena size is
+ * what it is for host sizes adding up to N; b200tfs_example_device_lists_request_size, whose size is closed form, refuses a
+ * request with device sizes (B200TFS_E_ARG).  Refused before any launch (B200TFS_E_ARG): sizes != NULL on a request that is
+ * not PREDICT_ELWCS, or beside host list_sizes; a misaligned sizes pointer.  The frame kernel of a call with such a request reads
+ * the sizes, places every query and writes the emit spans of its examples into scratch: ceil(N / per) + Q span slots per request
+ * (per: the examples of one emit span), of which the unused ones are empty.  Calls with none launch what they did.            */
+typedef struct b200tfs_example_device_lists {
+  const int64_t* sizes;              /* device int64[n_lists], or NULL: host list sizes (or not a PREDICT_ELWCS request)         */
+} b200tfs_example_device_lists;
+int b200tfs_example_device_lists_request_size(const b200tfs_example_request* r, const b200tfs_example_target* target,
+                                              const b200tfs_example_context* context, const b200tfs_example_tasks* tasks,
+                                              const b200tfs_ragged* ragged, const b200tfs_example_sequence* sequence,
+                                              const b200tfs_request_spec* spec, const b200tfs_example_lists* lists,
+                                              const b200tfs_ragged* list_ragged, const b200tfs_example_device_lists* device_lists,
+                                              uint64_t* total_len);
+int b200tfs_example_device_lists_arena_size(int32_t n, const b200tfs_example_request* reqs, const b200tfs_ragged* ragged,
+                                            const b200tfs_bytes* bytes, const b200tfs_example_target* targets,
+                                            const b200tfs_example_context* contexts, const b200tfs_bytes* context_bytes,
+                                            const b200tfs_example_tasks* tasks, const b200tfs_example_sequence* sequences,
+                                            const b200tfs_request_spec* specs, const b200tfs_example_lists* lists,
+                                            const b200tfs_ragged* list_ragged, const b200tfs_bytes* list_bytes,
+                                            const b200tfs_example_device_lists* device_lists, uint64_t* bytes_out);
+int b200tfs_encode_example_device_lists_async(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs,
+                                              const b200tfs_ragged* ragged, const b200tfs_bytes* bytes,
+                                              const b200tfs_example_target* targets, const b200tfs_example_context* contexts,
+                                              const b200tfs_bytes* context_bytes, const b200tfs_example_tasks* tasks,
+                                              const b200tfs_example_sequence* sequences, const b200tfs_request_spec* specs,
+                                              const b200tfs_example_lists* lists, const b200tfs_ragged* list_ragged,
+                                              const b200tfs_bytes* list_bytes, const b200tfs_example_device_lists* device_lists,
+                                              void* arena_dev, uint64_t arena_cap);
+int b200tfs_encode_example_device_lists_host(b200tfs_ctx* ctx, int32_t n, const b200tfs_example_request* reqs,
+                                             const b200tfs_ragged* ragged, const b200tfs_bytes* bytes,
+                                             const b200tfs_example_target* targets, const b200tfs_example_context* contexts,
+                                             const b200tfs_bytes* context_bytes, const b200tfs_example_tasks* tasks,
+                                             const b200tfs_example_sequence* sequences, const b200tfs_request_spec* specs,
+                                             const b200tfs_example_lists* lists, const b200tfs_ragged* list_ragged,
+                                             const b200tfs_bytes* list_bytes, const b200tfs_example_device_lists* device_lists,
+                                             void* wire_host, uint64_t wire_cap, uint64_t* rec_off, uint64_t* rec_len);
 
 /* ---- Classify / Regress responses: a batch of responses into one value or score array ----------------------
  * What ClassificationResponse.FromString / RegressionResponse.FromString followed by a loop over the result give, concatenated

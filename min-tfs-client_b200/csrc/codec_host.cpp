@@ -1772,21 +1772,33 @@ struct StagePiece { const uint8_t* dev; const uint8_t* host; uint64_t nb; };
 struct CopyMerger {
   cudaStream_t stream;
   uint8_t* d = nullptr; const uint8_t* h = nullptr; uint64_t n = 0;
+  std::vector<std::pair<uint64_t, uint64_t>> parts;   // the copies merged into [d, d + n): offset from d (and h), bytes
   explicit CopyMerger(cudaStream_t s) : stream(s) {}
   cudaError_t add(const void* dst, const void* src, uint64_t nb) {
     if (!nb) return cudaSuccess;
     if (n && (const uint8_t*)dst >= d + n && (const uint8_t*)dst - (d + n) == (const uint8_t*)src - (h + n) && (const uint8_t*)dst - (d + n) < 256) {
+      parts.push_back({(uint64_t)((const uint8_t*)dst - d), nb});
       n = (uint64_t)((const uint8_t*)dst - d) + nb;      // the gap (alignment padding, equal on both sides) travels along
       return cudaSuccess;
     }
     cudaError_t e = flush();
     d = (uint8_t*)dst; h = (const uint8_t*)src; n = nb;
+    parts.assign(1, {0, nb});
     return e;
   }
+  // Sources that lie at the staging gap from each other need not be one allocation: two page-locked buffers can sit that close,
+  // and the runtime refuses a copy whose host range spans both (cudaErrorInvalidValue).  Such a range is copied part by part.
   cudaError_t flush() {
     cudaError_t e = cudaSuccess;
     if (n) e = cudaMemcpyAsync(d, h, n, cudaMemcpyHostToDevice, stream);
+    if (e == cudaErrorInvalidValue && parts.size() > 1) {
+      cudaGetLastError();
+      e = cudaSuccess;
+      for (size_t i = 0; i < parts.size() && e == cudaSuccess; ++i)
+        e = cudaMemcpyAsync(d + parts[i].first, h + parts[i].first, parts[i].second, cudaMemcpyHostToDevice, stream);
+    }
     n = 0;
+    parts.clear();
     return e;
   }
 };

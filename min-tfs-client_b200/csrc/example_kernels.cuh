@@ -68,6 +68,16 @@ __device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
   for (int d = 16; d; d >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, d);
   return v;
 }
+// the sum of v over this lane and the lanes below it
+__device__ __forceinline__ uint64_t warp_incl_scan64(uint64_t v) {
+  const uint32_t lane = threadIdx.x & 31;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint64_t y = __shfl_up_sync(0xFFFFFFFFu, v, d);
+    if (lane >= (uint32_t)d) v += y;
+  }
+  return v;
+}
 
 // ---- bytes rows ----
 // Example i's row of a bytes column is strings b .. b + ne of the column (b = i * row_stride), and the kernels read offsets
@@ -548,13 +558,15 @@ __device__ __forceinline__ void ex_write_record(const ExTables& T, const ExReq& 
   else ex_write_example<kMode, kTag>(T, q, i, w);
 }
 
-// kShift (a PREDICT_ELWCS span, plan.h ExLists): the span's query (its pad) moves its examples by shift[query]
-template <int kMode, uint8_t kTag, bool kSeq = false, bool kShift = false>
+// kShift (a PREDICT_ELWCS span, plan.h ExLists): the span's query (its pad) moves its examples by shift[query]; kEmpty (the
+// device-planned spans, plan.h ExDevLists): an empty span writes nothing
+template <int kMode, uint8_t kTag, bool kSeq = false, bool kShift = false, bool kEmpty = false>
 __device__ __forceinline__ void ex_emit(const ExTables& T, const uint64_t* shift = nullptr) {
   __shared__ __align__(16) uint8_t img[kExStage + 16];
   __shared__ uint64_t next;
   constexpr uint32_t kWarps = kExEmitThreads / 32;
   const ExSpan sp = T.spans[blockIdx.x];
+  if (kEmpty && sp.e1 <= sp.e0) return;
   const ExReq q = T.reqs[sp.req];
   const uint32_t warp = threadIdx.x >> 5;
   const uint64_t A = q.anchor + (kShift ? shift[sp.pad] : 0);
@@ -612,6 +624,11 @@ __global__ void __launch_bounds__(kExEmitThreads) ex_emit_predict_kernel(const _
 template <int kMode, uint8_t kTag>
 __global__ void __launch_bounds__(kExEmitThreads) ex_emit_list_kernel(const __grid_constant__ ExTables T, const uint64_t* __restrict__ shift) {
   ex_emit<kMode, kTag, false, true>(T, shift);
+}
+// the example spans of the PREDICT_ELWCS requests with device list sizes, which ex_frame_lists_dev_kernel wrote (plan.h ExDevLists)
+template <int kMode>
+__global__ void __launch_bounds__(kExEmitThreads) ex_emit_list_dev_kernel(const __grid_constant__ ExTables T, const uint64_t* __restrict__ shift) {
+  ex_emit<kMode, 0x0A, false, true, true>(T, shift);
 }
 // the spans of the SequenceExample requests, which are always counted (kExColumns places them through off and S)
 __global__ void __launch_bounds__(kExEmitThreads) ex_emit_sequence_kernel(const __grid_constant__ ExTables T) {
@@ -709,10 +726,10 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_context_kernel(co
 // contiguous offset, its context C_q (12 00 when empty); a warp scan of 1 + vi(E + C) + E + C gives where its header goes, which
 // the lane writes, and the shifts the list emits move its examples and its context by.  No header leaves the slot, whatever the
 // sizes: a request whose lengths or offsets broke the rules gets B200TFS_E_SHAPE, and its emits stop at the slot's end.
-template <int kMode>
-__global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_lists_kernel(const __grid_constant__ ExTables T,
-                                                                            const ExCtxRef* __restrict__ ctx,
-                                                                            const __grid_constant__ ExLists Ls) {
+// kDev (D: plan.h ExDevLists): a request with device list sizes takes its queries from a warp scan of the sizes in the same loop,
+// and writes its emit spans, a warp scan of ceil(size / per) placing each query's first one.
+template <int kMode, bool kDev>
+__device__ __forceinline__ void ex_frame_lists(const ExTables& T, const ExCtxRef* ctx, const ExLists& Ls, const ExDevLists* D) {
   const uint32_t r = blockIdx.x * kExFrameWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (r >= T.n_req) return;
   const ExCtxRef c = ctx[r];
@@ -722,12 +739,30 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_lists_kernel(cons
   }
   const ExList l = Ls.lists[c.req];
   const ExReq q = T.reqs[r], x = T.reqs[l.ctx];
+  ExListSizes d{};
+  if constexpr (kDev) d = D->lists[c.req];
   uint64_t base = 0;            // the bytes of the queries in front of this round
+  uint64_t run = 0, used = 0;   // device sizes: the examples and the span slots of the queries in front of this round
+  bool bad = false;             // and a negative size, or a sum past n_ex, in this lane's queries
   for (uint32_t k0 = 0; k0 < l.n_q; k0 += 32) {
     const uint32_t k = k0 + lane;
     uint64_t E = 0, C = 0, eo = 0, co = 0, h = 0;
+    ExQuery e{0, 0};
+    if (kDev && d.sizes) {      // the examples [e0, e1) clamped into [0, n_ex], and the spans over them
+      const int64_t s = k < l.n_q ? d.sizes[k] : 0;
+      const uint64_t z = s < 0 ? 0 : min((uint64_t)s, q.n_ex), zi = warp_incl_scan64(z);
+      bad |= s < 0 || (uint64_t)s > q.n_ex || run + zi > q.n_ex;
+      e.e0 = min(run + zi - z, q.n_ex); e.e1 = min(run + zi, q.n_ex);
+      run = min(run + __shfl_sync(0xFFFFFFFFu, zi, 31), q.n_ex);
+      const uint64_t ns = (e.e1 - e.e0 + d.per - 1) / d.per, ni = warp_incl_scan64(ns);
+      ExSpan* sp = D->spans + d.s0 + used + (ni - ns);
+      for (uint64_t j = 0; j < ns; ++j)
+        sp[j] = ExSpan{r, l.q0 + k, e.e0 + j * d.per, min(e.e0 + (j + 1) * d.per, e.e1)};
+      used += __shfl_sync(0xFFFFFFFFu, ni, 31);
+    } else if (k < l.n_q) {
+      e = Ls.queries[l.q0 + k];
+    }
     if (k < l.n_q) {
-      const ExQuery e = Ls.queries[l.q0 + k];
       if (e.e1 > e.e0) { eo = ex_start<kMode>(T, q, e.e0); E = ex_end<kMode>(T, q, e.e1 - 1) - eo; }
       if (x.n_feat) { co = ex_start<kMode>(T, x, k); C = ex_end<kMode>(T, x, k) - co; }
       else C = 2;
@@ -753,12 +788,31 @@ __global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_lists_kernel(cons
     }
     base += __shfl_sync(0xFFFFFFFFu, inc, 31);
   }
-  ex_frame_request(T, q, r, base, 0, false, T.bad && (T.bad[r] || T.bad[l.ctx]));
+  if (kDev && d.sizes) {        // a bad request emits nothing; the slots behind the spans are empty
+    bad = __any_sync(0xFFFFFFFFu, bad);
+    if (bad) used = 0;
+    for (uint64_t t = used + lane; t < d.n_s; t += 32) D->spans[d.s0 + t] = ExSpan{r, 0, 0, 0};
+  }
+  ex_frame_request(T, q, r, base, 0, false, (kDev && bad) || (T.bad && (T.bad[r] || T.bad[l.ctx])));
+}
+template <int kMode>
+__global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_lists_kernel(const __grid_constant__ ExTables T,
+                                                                            const ExCtxRef* __restrict__ ctx,
+                                                                            const __grid_constant__ ExLists Ls) {
+  ex_frame_lists<kMode, false>(T, ctx, Ls, nullptr);
+}
+// ex_frame_lists_kernel for a call with a PREDICT_ELWCS request whose list sizes are in device memory
+template <int kMode>
+__global__ void __launch_bounds__(32 * kExFrameWarps) ex_frame_lists_dev_kernel(const __grid_constant__ ExTables T,
+                                                                                const ExCtxRef* __restrict__ ctx,
+                                                                                const __grid_constant__ ExLists Ls,
+                                                                                const __grid_constant__ ExDevLists D) {
+  ex_frame_lists<kMode, true>(T, ctx, Ls, &D);
 }
 
 // n_seq_tiles / n_seq_spans: the count tiles and emit spans of the SequenceExample requests, behind T's n_tiles and n_spans
 cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t stream, uint32_t* launched, const ExCtxRef* ctx,
-                                    uint32_t n_seq_tiles, uint32_t n_seq_spans, const ExLists* lists) {
+                                    uint32_t n_seq_tiles, uint32_t n_seq_spans, const ExLists* lists, const ExDevLists* dev) {
   *launched = 0;
   if (T.n_tiles) {
     if (mode == kExColumns) ex_count_kernel<kExColumns><<<T.n_tiles, kExTile, 0, stream>>>(T);
@@ -778,7 +832,12 @@ cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t st
     *launched += 1;
   }
   const uint32_t frame_grid = (T.n_req + kExFrameWarps - 1) / kExFrameWarps;
-  if (lists && T.n_req) {     // the shifts, before every emit (plan.h ExLists)
+  if (dev && T.n_req) {       // the shifts and the device-sized requests' spans (plan.h ExDevLists)
+    if (mode == kExColumns) ex_frame_lists_dev_kernel<kExColumns><<<frame_grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx, *lists, *dev);
+    else if (mode == kExRagged) ex_frame_lists_dev_kernel<kExRagged><<<frame_grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx, *lists, *dev);
+    else ex_frame_lists_dev_kernel<kExDense><<<frame_grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx, *lists, *dev);
+    *launched += 1;
+  } else if (lists && T.n_req) {     // the shifts, before every emit (plan.h ExLists)
     if (mode == kExColumns) ex_frame_lists_kernel<kExColumns><<<frame_grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx, *lists);
     else if (mode == kExRagged) ex_frame_lists_kernel<kExRagged><<<frame_grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx, *lists);
     else ex_frame_lists_kernel<kExDense><<<frame_grid, 32 * kExFrameWarps, 0, stream>>>(T, ctx, *lists);
@@ -812,6 +871,14 @@ cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t st
       if (mode == kExColumns) ex_emit_list_kernel<kExColumns, 0x0A><<<lists->n_spans, kExEmitThreads, 0, stream>>>(Q, lists->shift);
       else if (mode == kExRagged) ex_emit_list_kernel<kExRagged, 0x0A><<<lists->n_spans, kExEmitThreads, 0, stream>>>(Q, lists->shift);
       else ex_emit_list_kernel<kExDense, 0x0A><<<lists->n_spans, kExEmitThreads, 0, stream>>>(Q, lists->shift);
+      *launched += 1;
+    }
+    if (dev && dev->n_spans) {
+      ExTables Qd = T;
+      Qd.spans = dev->spans;
+      if (mode == kExColumns) ex_emit_list_dev_kernel<kExColumns><<<dev->n_spans, kExEmitThreads, 0, stream>>>(Qd, lists->shift);
+      else if (mode == kExRagged) ex_emit_list_dev_kernel<kExRagged><<<dev->n_spans, kExEmitThreads, 0, stream>>>(Qd, lists->shift);
+      else ex_emit_list_dev_kernel<kExDense><<<dev->n_spans, kExEmitThreads, 0, stream>>>(Qd, lists->shift);
       *launched += 1;
     }
     Q.spans += lists->n_spans;

@@ -60,8 +60,10 @@ cudaError_t launch_padded_strings(const PadStrTables& T, uint32_t grid, cudaStre
 // tf.Example requests (example_kernels.cuh): count + scan (when T.n_tiles), emit, frame; *launched receives how many kernels.
 // ctx (device, one ExCtxRef per request; NULL: a call without contexts) selects the frame kernel that writes the contexts.
 // lists (NULL: a call without PREDICT_ELWCS requests): the frame runs before the emits, and the list emits after the others.
+// dev (NULL: no PREDICT_ELWCS request with device list sizes): the frame also plans those requests' spans, emitted by one more kernel.
 cudaError_t launch_example_requests(const ExTables& T, int mode, cudaStream_t stream, uint32_t* launched, const ExCtxRef* ctx,
-                                    uint32_t n_seq_tiles, uint32_t n_seq_spans, const ExLists* lists = nullptr);
+                                    uint32_t n_seq_tiles, uint32_t n_seq_spans, const ExLists* lists = nullptr,
+                                    const ExDevLists* dev = nullptr);
 // Classify / Regress responses (example_resp_kernels.cuh): index, scan, emit, [label compare,] publish; emit_ctas CTAs stride over
 // the rows; *launched receives how many kernels
 cudaError_t launch_example_responses(const XrTables& T, uint32_t emit_ctas, cudaStream_t stream, uint32_t* launched);

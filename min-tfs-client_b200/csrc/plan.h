@@ -451,6 +451,18 @@ struct ExLists {
   uint64_t* cshift;                     // and of its context
   uint32_t n_lists, n_spans, n_ctx_spans, pad_;   // emit spans behind all others: the examples', then one per non-empty context
 };
+// A PREDICT_ELWCS request whose list sizes are in device memory (b200tfs_example_device_lists) has no ExQuery entries and no
+// host-cut spans: ex_frame_lists_dev_kernel scans its sizes into query ranges, clamped into [0, n_ex] (a negative size or an
+// overflow makes the request B200TFS_E_SHAPE), and writes its example spans into n_s scratch slots from s0, cut every `per`
+// examples and at every query's end.  A query adds at most one partial span, so n_s = ceil(n_ex / per) + Q always holds them;
+// the unused slots are empty (e1 == e0), which ex_emit_list_dev_kernel leaves at once.  Its queries' shifts follow those of all
+// host-sized queries (ExList::q0 indexes ExLists::shift / cshift only).  One entry per ExLists::lists entry; sizes NULL: host.
+struct ExListSizes { const int64_t* sizes; uint64_t per; uint32_t s0, n_s; };
+struct ExDevLists {
+  const ExListSizes* lists;
+  ExSpan* spans;                        // scratch: the example spans of the device-sized requests, behind each other
+  uint32_t n_spans, pad_;
+};
 struct ExTables {
   const ExReq* reqs; const ExFeat* feats; const uint8_t* blob;
   const ExSpan* tiles;                  // count / scan CTAs

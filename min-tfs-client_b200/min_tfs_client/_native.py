@@ -188,6 +188,12 @@ class ExampleLists(C.Structure):
                 ("present", C.c_int32)]
 
 
+class ExampleDeviceLists(C.Structure):
+    """b200tfs_example_device_lists: one request's list sizes in device memory (``sizes``: a device int64[n_lists]; None: the
+    host ``list_sizes`` of its ExampleLists entry, or not an EXAMPLES_PREDICT_ELWCS request)."""
+    _fields_ = [("sizes", C.c_void_p)]
+
+
 class PadInput(C.Structure):
     """b200tfs_pad_input: the shapes of one input of b200tfs_encode_padded_requests_async (int64[n, cols]; cols 1: row counts)."""
     _fields_ = [("shapes", C.c_void_p), ("cols", C.c_int32), ("pad_", C.c_int32)]
@@ -405,6 +411,26 @@ SIGNATURES = {
                                                     C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), C.POINTER(RequestSpec),
                                                     C.POINTER(ExampleLists), C.POINTER(Ragged), C.POINTER(Bytes), _vp, C.c_uint64, _u64p,
                                                     _u64p]),
+    "b200tfs_example_device_lists_request_size": (C.c_int, [C.POINTER(ExampleRequest), C.POINTER(ExampleTarget),
+                                                            C.POINTER(ExampleContext), C.POINTER(ExampleTasks), C.POINTER(Ragged),
+                                                            C.POINTER(ExampleSequence), C.POINTER(RequestSpec), C.POINTER(ExampleLists),
+                                                            C.POINTER(Ragged), C.POINTER(ExampleDeviceLists), _u64p]),
+    "b200tfs_example_device_lists_arena_size": (C.c_int, [C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                          C.POINTER(ExampleTarget), C.POINTER(ExampleContext), C.POINTER(Bytes),
+                                                          C.POINTER(ExampleTasks), C.POINTER(ExampleSequence), C.POINTER(RequestSpec),
+                                                          C.POINTER(ExampleLists), C.POINTER(Ragged), C.POINTER(Bytes),
+                                                          C.POINTER(ExampleDeviceLists), _u64p]),
+    "b200tfs_encode_example_device_lists_async": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged),
+                                                            C.POINTER(Bytes), C.POINTER(ExampleTarget), C.POINTER(ExampleContext),
+                                                            C.POINTER(Bytes), C.POINTER(ExampleTasks), C.POINTER(ExampleSequence),
+                                                            C.POINTER(RequestSpec), C.POINTER(ExampleLists), C.POINTER(Ragged),
+                                                            C.POINTER(Bytes), C.POINTER(ExampleDeviceLists), _vp, C.c_uint64]),
+    "b200tfs_encode_example_device_lists_host": (C.c_int, [_vp, C.c_int32, C.POINTER(ExampleRequest), C.POINTER(Ragged),
+                                                           C.POINTER(Bytes), C.POINTER(ExampleTarget), C.POINTER(ExampleContext),
+                                                           C.POINTER(Bytes), C.POINTER(ExampleTasks), C.POINTER(ExampleSequence),
+                                                           C.POINTER(RequestSpec), C.POINTER(ExampleLists), C.POINTER(Ragged),
+                                                           C.POINTER(Bytes), C.POINTER(ExampleDeviceLists), _vp, C.c_uint64, _u64p,
+                                                           _u64p]),
     "b200tfs_multi_inference_response_bound": (C.c_int, [C.c_int32, _i32p, C.c_int32, _u64p, _u64p, _u64p]),
     "b200tfs_decode_multi_inference_responses": (C.c_int, [_vp, C.c_int32, _i32p, _vp, C.c_int32, _u64p, _u64p, _vpp, _u64p, _vpp,
                                                            _u64p]),

@@ -483,6 +483,17 @@ def _example_columns(input_dict: Mapping, context: bool = False):
     return n, preps
 
 
+def _head_rows(v, n: int):
+    """The first n rows of an input value (0-d values as they are), for a request the host assembles."""
+    if isinstance(v, RaggedColumn):
+        return RaggedColumn(_head_rows(v.values, n), v.lengths[:n])
+    if isinstance(v, BytesColumn):
+        per = int(np.prod(v.shape[1:], dtype=np.int64)) if len(v.shape) else 0
+        return BytesColumn(v.data, v.offsets[:n * per + 1], (n, *v.shape[1:])) if len(v.shape) else v
+    a = np.asarray(v)
+    return a[:n] if a.ndim else a
+
+
 def _shape_of(v) -> Tuple[int, ...]:
     if isinstance(v, (BytesColumn, RaggedColumn)):
         return tuple(v.shape)
@@ -1274,7 +1285,15 @@ class Codec:
         ``make_predict_elwcs_request`` (deterministic order); device arrays of such dtypes raise ValueError, and so do device
         lengths or offsets out of range.  ``signature_name``, ``version_label`` and ``output_filter`` as for
         ``encode_predict_requests``.  With one query the bytes equal ``encode_example_requests(..., predict_input=input_key)``'s
-        for that query's context."""
+        for that query's context.
+
+        ``list_sizes`` may also be a device int64 vector (``__cuda_array_interface__`` / DLPack), which the host never reads: the
+        rows of ``input_dict`` are then a capacity N, the sizes may add up to any total <= N, and the rows from the total on are not
+        sent - what a GPU retrieval or filtering stage leaves, a flat candidate buffer and per-query counts.  The rows past the
+        total are still counted, so ragged lengths and string offsets there must keep the rules (length 0, or offsets equal to
+        the last used one, do).  A negative size or a total past N raises ValueError from the encode; so do a device int32 vector
+        and an item whose input values are all 0-d (it has no capacity).  An item the host assembles copies the sizes to the host
+        and cuts the rows to their total."""
         from .requests import _list_sizes, make_predict_elwcs_request
 
         items = list(requests)
@@ -1284,17 +1303,41 @@ class Codec:
         order_code = _ORDER[order] if isinstance(order, str) else int(order)
         pkey = input_key.encode("utf-8") if isinstance(input_key, str) else bytes(input_key)
         out: List[Optional[bytes]] = [None] * len(items)
-        keep, structs, dev_idx, ragged, strs, lists, lragged, lstrs = [], [], [], [], [], [], [], []
+        keep, structs, dev_idx, ragged, strs, lists, lragged, lstrs, dlists = [], [], [], [], [], [], [], [], []
         for i, (model_name, model_version, context_dict, input_dict, list_sizes) in enumerate(items):
-            sizes = _list_sizes(list_sizes)
-            n, q = int(sizes.sum()), sizes.size
+            dsizes = None        # device list sizes: (pointer, keep-alive)
+            if D.is_device_object(list_sizes):
+                ptr, sshape, sdtype, shold = D.device_view(list_sizes)
+                if sdtype != np.int64 or len(sshape) != 1:
+                    raise ValueError(f"device list sizes must be an int64 vector, got {sdtype} of shape {tuple(sshape)}")
+                rows = {_shape_of(v)[0] for v in input_dict.values() if len(_shape_of(v))}
+                if not rows:
+                    raise ValueError("device list sizes need an input value with a row axis: its rows are the candidate capacity")
+                if len(rows) > 1:
+                    raise ValueError(f"inputs disagree on the number of rows: {sorted(rows)}")
+                n, q = rows.pop(), int(sshape[0])
+                dsizes, sizes = (ptr, shold), None
+            else:
+                sizes = _list_sizes(list_sizes)
+                n, q = int(sizes.sum()), sizes.size
             for what, d, m in (("input", input_dict, n), ("context", context_dict, q)):
                 for k, v in d.items():
                     shape = _shape_of(v)
                     if len(shape) and shape[0] != m:
                         raise ValueError(f"{what} {k!r} has {shape[0]} rows, not {m}")
+            on_device = dsizes is not None
+            if on_device and not q:     # no size to read (an empty vector may have no address): no row is sent
+                dsizes, sizes, n = None, np.zeros(0, np.int64), 0
             cols, ccols = _example_columns(input_dict), _example_columns(context_dict)
             if cols is None or ccols is None or (n and not input_dict):
+                if on_device:
+                    if dsizes is not None:
+                        sizes = np.empty(q, dtype=np.int64)
+                        N.check(self._lib.b200tfs_memcpy_d2h(self._ctx, sizes.ctypes.data, dsizes[0], sizes.nbytes))
+                        self.sync()
+                    if (sizes < 0).any() or int(sizes.sum()) > n:
+                        raise ValueError(f"list sizes must be >= 0 and add up to at most the {n} rows")
+                    input_dict = {k: _head_rows(v, int(sizes.sum())) for k, v in input_dict.items()}
                 req = make_predict_elwcs_request(model_name, model_version, context_dict, input_dict, sizes, pkey.decode("utf-8"), **fields)
                 wire = req.SerializeToString(deterministic=True)
                 out[i] = (b"\x00" + len(wire).to_bytes(4, "big") + wire) if grpc_frame else wire
@@ -1307,9 +1350,10 @@ class Codec:
                                             order=order_code, version=int(model_version) if model_version is not None else 0,
                                             n_examples=n, n_features=len(preps), flags=N.RF_GRPC_FRAME if grpc_frame else 0,
                                             features=feats))
-            lists.append(N.ExampleLists(list_sizes=sizes.ctypes.data if q else None, n_lists=q, context=cfeats, n_context=len(cpreps),
-                                        present=1))
-            keep.append((preps, feats, cpreps, cfeats, name, sizes))
+            lists.append(N.ExampleLists(list_sizes=sizes.ctypes.data if q and dsizes is None else None, n_lists=q, context=cfeats,
+                                        n_context=len(cpreps), present=1))
+            dlists.append(N.ExampleDeviceLists(sizes=dsizes[0] or None) if dsizes is not None else N.ExampleDeviceLists())
+            keep.append((preps, feats, cpreps, cfeats, name, sizes, dsizes))
             ragged += [p[3] or N.Ragged() for p in preps]
             strs += [p.bytes_entry or N.Bytes() for p in preps]
             lragged += [p[3] or N.Ragged() for p in cpreps]
@@ -1324,14 +1368,15 @@ class Codec:
             bs = (N.Bytes * len(strs))(*strs) if any(b.offsets for b in strs) else None
             lrg = (N.Ragged * len(lragged))(*lragged) if any(g.lengths for g in lragged) else None
             lbs = (N.Bytes * len(lstrs))(*lstrs) if any(b.offsets for b in lstrs) else None
+            dls = (N.ExampleDeviceLists * m)(*dlists) if any(d.sizes for d in dlists) else None
             cap = C.c_uint64()
             specs = _RequestSpec.array(spec, m)
-            N.check(self._lib.b200tfs_example_lists_arena_size(m, reqs, None, bs, tg, None, None, None, None, specs, ls, lrg, lbs,
-                                                               C.byref(cap)))
+            N.check(self._lib.b200tfs_example_device_lists_arena_size(m, reqs, None, bs, tg, None, None, None, None, specs, ls, lrg, lbs,
+                                                                      dls, C.byref(cap)))
             wire = np.empty(max(int(cap.value), 1), dtype=np.uint8)
             off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
-            N.check(self._lib.b200tfs_encode_example_lists_host(self._ctx, m, reqs, rg, bs, tg, None, None, None, None, specs, ls, lrg, lbs,
-                                                                wire.ctypes.data, cap.value, off, ln))
+            N.check(self._lib.b200tfs_encode_example_device_lists_host(self._ctx, m, reqs, rg, bs, tg, None, None, None, None, specs, ls,
+                                                                       lrg, lbs, dls, wire.ctypes.data, cap.value, off, ln))
             for j, i in enumerate(dev_idx):
                 out[i] = wire[off[j]: off[j] + ln[j]].tobytes()
         return out  # type: ignore[return-value]

@@ -484,7 +484,8 @@ def gpu_predict_sequence_examples_serializer(request) -> bytes:
 def gpu_predict_elwcs_serializer(request) -> bytes:
     """``request_serializer`` for ``channel.unary_unary(PREDICT_METHOD, ...)`` to a TF-Ranking model's ELWC signature:
     (model_name, model_version, context_dict, input_dict, list_sizes, input_key) -> the bytes of
-    ``make_predict_elwcs_request(...).SerializeToString(deterministic=True)``, packed on the GPU.  A trailing ``SpecFields`` sets
+    ``make_predict_elwcs_request(...).SerializeToString(deterministic=True)``, packed on the GPU.  ``list_sizes`` may be a device
+    int64 vector over a capacity of input rows (``Codec.encode_elwc_requests``).  A trailing ``SpecFields`` sets
     ``signature_name`` / ``version_label`` / ``output_filter``."""
     request, spec = _split_fields(request)
     model_name, model_version, context_dict, input_dict, list_sizes, input_key = request
@@ -555,7 +556,9 @@ class TensorServingClient:
                               output_filter=None) -> PredictResponseView:
         """Predict on a TF-Ranking model whose signature takes a DT_STRING vector of serialized ExampleListWithContexts, one per
         query: the Q = ``len(list_sizes)`` ELWCs ``elwcs_from_input_dict(context_dict, input_dict, list_sizes)`` builds, sent as
-        input ``input_key`` in one call and packed on the GPU."""
+        input ``input_key`` in one call and packed on the GPU.  ``list_sizes`` may be a device int64 vector, as a GPU candidate
+        stage leaves it: the rows of ``input_dict`` are then a capacity, and the rows past the sizes' total are not sent
+        (``Codec.encode_elwc_requests``)."""
         call = self._channel.unary_unary(PREDICT_METHOD, request_serializer=gpu_predict_elwcs_serializer,
                                          response_deserializer=gpu_response_deserializer)
         return call((model_name, model_version, context_dict, input_dict, list_sizes, input_key,

@@ -30,6 +30,14 @@ Workloads (one request each unless stated):
   K4  one request of 1 024 queries x 8 candidates: per-query headers and contexts dominate
       (not in the default set; --workloads K3,K3R,K4; beside each, the same queries as single-query PREDICT_ELWC requests through
       Codec.encode_example_requests, what a client sends today; protobuf is timed once, the Python legs over three calls)
+  K5  K3 with list sizes in device memory (b200tfs_encode_example_device_lists_*): 64 requests x 16 queries over a capacity of
+      N = 3 200 candidate rows each, every query's candidates drawn from 0..200 (so the total changes too), 8 such size sets
+      cycled call after call
+  K5L one request of 1 024 queries over N = 16 384 rows, each query's candidates drawn from 0..16 (K4's shape)
+      (not in the default set; --workloads K5,K5L.  Legs: _async eager with host sizes, the host planning every call's new
+      sizes; _async eager with device sizes; the graph captured once and replayed with device sizes.  Before each device-sizes
+      call a device-to-device copy puts the next size set in place, as the GPU stage that produces them would; it is inside
+      the timed region.  Bytes of both device legs are checked against protobuf for every size set after the timed region.)
 Legs: the _async entry point eager (device columns -> device arena), the same captured once as a CUDA graph and replayed,
 _host from pinned columns (copies both ways included), and examples_from_input_dict + SerializeToString(deterministic=True)
 on one host core.  CUDA events over >= 20 calls after warm-up, three runs each; bytes = column bytes read + wire bytes
@@ -475,6 +483,125 @@ def elwcs_workload(name, items, args, codec, out):
     print(name, res, flush=True)
 
 
+def elwcs_device_workloads(rng):
+    """the PREDICT_ELWCS workloads with device list sizes: (context_dict, input_dict over N rows, [size sets]) per request"""
+    def k5(Q, m_max, sets=8):
+        n = Q * m_max
+        inp = {"item": rng.standard_normal((n, 32)).astype(np.float32), "item_id": rng.integers(0, 1 << 40, n)}
+        q = rng.integers(97, 123, Q * 35).astype(np.uint8)
+        ctx = {"user": rng.standard_normal((Q, 256)).astype(np.float32), "hist": rng.integers(0, 50_000, (Q, 50)),
+               "query": BytesColumn(q, np.arange(Q + 1) * 35)}
+        return ctx, inp, [rng.integers(0, m_max + 1, Q).astype(np.int64) for _ in range(sets)]
+
+    return {"K5": lambda: [k5(16, 200) for _ in range(64)], "K5L": lambda: [k5(1024, 16)]}
+
+
+def elwcs_device_workload(name, items, args, out):
+    """_async eager with host sizes (re-planned every call), _async eager with device sizes and the graph replayed with device
+    sizes, over size sets that change call after call; every size set's bytes compared with protobuf afterwards"""
+    import torch
+
+    from min_tfs_client.requests import make_predict_elwcs_request
+
+    lib = N.load()
+    g = Ctx()
+    m, S = len(items), len(items[0][2])
+    keep, structs, strs, lists, lstrs = [], [], [], [], []
+    for ctx, inp, size_sets in items:
+        dctx = {k: BytesColumn(torch.from_numpy(v.data).cuda(), torch.from_numpy(v.offsets).cuda(), v.shape) if isinstance(v, BytesColumn)
+                else torch.from_numpy(np.ascontiguousarray(v)).cuda() for k, v in ctx.items()}
+        dinp = {k: torch.from_numpy(np.ascontiguousarray(v)).cuda() for k, v in inp.items()}
+        _, preps = _example_columns(dinp)
+        _, cpreps = _example_columns(dctx)
+        feats = (N.Feature * len(preps))(*[p[0] for p in preps])
+        cfeats = (N.Feature * len(cpreps))(*[p[0] for p in cpreps])
+        keep += [dctx, dinp, preps, cpreps, feats, cfeats]
+        n = next(iter(inp.values())).shape[0]
+        structs.append(N.ExampleRequest(model_name=b"model", model_name_len=5, has_version=1, order=N.ORDER_UPB, version=1,
+                                        n_examples=n, n_features=len(preps), flags=0, features=feats))
+        lists.append(N.ExampleLists(list_sizes=None, n_lists=len(size_sets[0]), context=cfeats, n_context=len(cpreps), present=1))
+        strs += [p.bytes_entry or N.Bytes() for p in preps]
+        lstrs += [p.bytes_entry or N.Bytes() for p in cpreps]
+    reqs, lsa = (N.ExampleRequest * m)(*structs), (N.ExampleLists * m)(*lists)
+    bsa, lbsa = (N.Bytes * len(strs))(*strs), (N.Bytes * len(lstrs))(*lstrs)
+    tga = (N.ExampleTarget * m)(*[N.ExampleTarget(kind=N.EXAMPLES_PREDICT_ELWCS, key=b"elwcs", key_len=5)] * m)
+    # every size set of every request in device memory, and the live sizes buffer the encode reads
+    Q = [len(it[2][0]) for it in items]
+    q0 = np.concatenate([[0], np.cumsum(Q)]).astype(np.int64)
+    sets = np.stack([np.concatenate([it[2][k] for it in items]) for k in range(S)]).astype(np.int64)     # [S, sum Q]
+    dsets, live = g.malloc(sets.nbytes), g.malloc(sets[0].nbytes)
+    N.check(lib.b200tfs_memcpy_h2d(g.ctx, dsets, sets.ctypes.data, sets.nbytes))
+    dla = (N.ExampleDeviceLists * m)(*[N.ExampleDeviceLists(sizes=live + 8 * int(q0[r])) for r in range(m)])
+    cap = C.c_uint64()
+    N.check(lib.b200tfs_example_device_lists_arena_size(m, reqs, None, bsa, tga, None, None, None, None, None, lsa, None, lbsa, dla,
+                                                        C.byref(cap)))
+    arena = (g.malloc(cap.value + 256) + 255) & ~255
+    step = [0]
+
+    def next_sizes():
+        k = step[0] % S
+        step[0] += 1
+        N.check(lib.b200tfs_memcpy_d2d(g.ctx, live, dsets + k * sets[0].nbytes, sets[0].nbytes))
+        return k
+
+    def device_eager():
+        next_sizes()
+        N.check(lib.b200tfs_encode_example_device_lists_async(g.ctx, m, reqs, None, bsa, tga, None, None, None, None, None, lsa, None,
+                                                              lbsa, dla, arena, cap.value))
+
+    # host sizes: the same columns, n_examples the set's total, planned on the host every call
+    hreqs, hlsa = (N.ExampleRequest * m)(*structs), (N.ExampleLists * m)(*lists)
+
+    def host_eager():
+        k = step[0] % S
+        step[0] += 1
+        for r in range(m):
+            hreqs[r].n_examples = int(sets[k, q0[r]: q0[r + 1]].sum())
+            hlsa[r].list_sizes = sets[k].ctypes.data + 8 * int(q0[r])
+        N.check(lib.b200tfs_encode_example_lists_async(g.ctx, m, hreqs, None, bsa, tga, None, None, None, None, None, hlsa, None, lbsa,
+                                                       arena, cap.value))
+
+    device_eager()
+    N.check(lib.b200tfs_encode_results(g.ctx, m, None, None))
+    N.check(lib.b200tfs_capture_begin(g.ctx))
+    N.check(lib.b200tfs_encode_example_device_lists_async(g.ctx, m, reqs, None, bsa, tga, None, None, None, None, None, lsa, None, lbsa,
+                                                          dla, arena, cap.value))
+    gr = C.c_void_p()
+    N.check(lib.b200tfs_capture_end(g.ctx, C.byref(gr)))
+
+    def replay():
+        next_sizes()
+        N.check(lib.b200tfs_graph_launch(g.ctx, gr))
+
+    res = {"requests": m, "queries": int(q0[-1]), "capacity_rows": sum(int(r.n_examples) for r in structs), "size_sets": S,
+           "examples_per_set": [int(x) for x in sets.sum(axis=1)], "arena_bytes": cap.value}
+    for leg, fn in (("host_sizes_async_us", host_eager), ("device_sizes_async_us", device_eager), ("device_sizes_graph_us", replay)):
+        for _ in range(S):
+            fn()
+        res[leg] = [g.timed(fn, max(args.calls, S)) for _ in range(args.runs)]
+    # after the timed region: every size set through both device legs against protobuf
+    off, ln = (C.c_uint64 * m)(), (C.c_uint64 * m)()
+    host = np.empty(cap.value, np.uint8)
+    for k in range(S):
+        refs = []
+        for r, (ctx, inp, _) in enumerate(items):
+            sz = sets[k, q0[r]: q0[r + 1]]
+            t = int(sz.sum())
+            refs.append(make_predict_elwcs_request("model", 1, ctx, {kk: v[:t] for kk, v in inp.items()}, sz, "elwcs")
+                        .SerializeToString(deterministic=True))
+        for fn in (device_eager, replay):
+            step[0] = k
+            fn()
+            N.check(lib.b200tfs_encode_results(g.ctx, m, off, ln))
+            N.check(lib.b200tfs_memcpy_d2h(g.ctx, host.ctypes.data, arena, cap.value))
+            N.check(lib.b200tfs_sync(g.ctx))
+            assert all(host[off[r]: off[r] + ln[r]].tobytes() == refs[r] for r in range(m)), (name, k)
+    res["bytes_checked_sets"] = S
+    N.check(lib.b200tfs_graph_destroy(gr))
+    out["workloads"][name] = res
+    print(name, res, flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--calls", type=int, default=20)
@@ -493,12 +620,16 @@ def main():
     profile_only = [w for w in args.profile.split(",") if w]
     Q = sequence_workloads(rng)
     K = elwcs_workloads(rng)
+    KD = elwcs_device_workloads(rng)
     for name in (profile_only or args.workloads.split(",")):
         if name in Q:
             sequence_workload(name, Q[name](), args, codec, out)
             continue
         if name in K:
             elwcs_workload(name, K[name](), args, codec, out)
+            continue
+        if name in KD:
+            elwcs_device_workload(name, KD[name](), args, out)
             continue
         pairs = [x if isinstance(x, tuple) else (x, None) for x in W[name]()]
         host_dicts = [d for d, _ in pairs]
